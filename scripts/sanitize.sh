@@ -8,3 +8,7 @@ set -e
 cd "$(dirname "$0")/.."
 SUBSET='test_fused_sra_tiny_and_exact_constant or (test_fused_sra_matches_cpu_oracle and 4-dtype0) or test_fused_sra_mixed_layers_unaligned or (test_quantize_kernel_bytes_match_cpu and dtype0-4-512) or (test_oneshot_kernel_matches_cpu_oracle and 2-dtype0) or test_unaligned_layers_and_mixed_config'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_kernels_gpu.py -m gpu -x -q -k "$SUBSET"
+# hostile inputs: guard bands around unaligned views, non-finite buckets, full slices of 8/16/32/256-element
+# buckets (lg 0/1/2/5), and a five-rank world
+EDGE_SUBSET='w5- or (full_slices and (4-8 or 4-16 or 4-32 or 4-256 or 7-8 or 6-16)) or (standalone and f32-5- and (-8] or -32] or -1]))'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_kernels_edge_gpu.py -m gpu -x -q -k "$EDGE_SUBSET"

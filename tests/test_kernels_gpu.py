@@ -8,6 +8,8 @@ import torch_cgx_b200 as cgx
 from torch_cgx_b200.ops import fake_quantize, quantize, dequantize
 from torch_cgx_b200.ops.oracle import quantize_dequantize_like
 
+from _bitwise import assert_same
+
 pytestmark = pytest.mark.gpu
 C = cgx._C
 DTYPES = [torch.float32, torch.float16, torch.bfloat16]
@@ -25,12 +27,12 @@ def test_quantize_kernel_bytes_match_cpu(dtype, bits, bucket):
     x = (torch.randn(50_003) * 2).to(dtype)
     w_cpu = quantize(x, bits, bucket)
     w_gpu = quantize(x.to(dev()), bits, bucket)
-    assert torch.equal(w_cpu, w_gpu.cpu())
+    assert_same(w_cpu, w_gpu.cpu())
     y_gpu = dequantize(w_gpu, x.to(dev()), bits, bucket)
     y_cpu = dequantize(w_cpu, x, bits, bucket)
-    assert torch.equal(y_cpu, y_gpu.cpu())
+    assert_same(y_cpu, y_gpu.cpu())
     # and against the independent fp32 PyTorch reference of the op
-    assert torch.equal(y_gpu.cpu(), quantize_dequantize_like(x, bits, bucket))
+    assert_same(y_gpu.cpu(), quantize_dequantize_like(x, bits, bucket))
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
@@ -43,29 +45,29 @@ def test_unaligned_layers_and_mixed_config(dtype):
     x = torch.randn(n).to(dtype)
     w_cpu = C.quantize(x, layers, 1, 1, False, 1.0, False, 0, 0, 0, 0, 2048)
     w_gpu = C.quantize(x.to(dev()), layers, 1, 1, False, 1.0, False, 0, 0, 0, 0, 2048)
-    assert torch.equal(w_cpu, w_gpu.cpu())
+    assert_same(w_cpu, w_gpu.cpu())
     y_cpu = C.dequantize(w_cpu, x, layers, 1, 1, False, 2048)
     y_gpu = C.dequantize(w_gpu, x.to(dev()), layers, 1, 1, False, 2048)
-    assert torch.equal(y_cpu, y_gpu.cpu())
+    assert_same(y_cpu, y_gpu.cpu())
 
 
 def test_stochastic_kernel_matches_cpu_philox():
     x = torch.randn(100_000)
     a = fake_quantize(x, 2, 512, stochastic=True, seed=3, seq=5)
     b = fake_quantize(x.to(dev()), 2, 512, stochastic=True, seed=3, seq=5)
-    assert torch.equal(a, b.cpu())
+    assert_same(a, b.cpu())
 
 
 def test_elementwise_helpers():
     x = torch.randn(100_001, device=dev())
     y = torch.randn(100_001, device=dev())
-    assert torch.equal(C.add(x, y), x + y)
+    assert_same(C.add(x, y), x + y)
     z = x.clone()
     C.scale_(z, 0.125)
-    assert torch.equal(z, x * 0.125)
-    assert torch.equal(C.convert(x, torch.float16), x.half())
-    assert torch.equal(C.convert(x.half(), torch.float32), x.half().float())
-    assert torch.equal(C.convert(x, torch.bfloat16), x.bfloat16())
+    assert_same(z, x * 0.125)
+    assert_same(C.convert(x, torch.float16), x.half())
+    assert_same(C.convert(x.half(), torch.float32), x.half().float())
+    assert_same(C.convert(x, torch.bfloat16), x.bfloat16())
 
 
 # --------------------------------------------------------------------------
@@ -82,7 +84,7 @@ def _run_local(world, layers, n, dtype, lanes=8, average=False, skip_incomplete=
         torch.cuda.synchronize()
         g.check()
         for r in range(world):
-            assert torch.equal(gpu[r].cpu(), cpu[r]), f"rank {r} differs from the CPU SRA oracle"
+            assert_same(gpu[r].cpu(), cpu[r], f"rank {r} differs from the CPU SRA oracle")
     return g
 
 
@@ -149,7 +151,7 @@ def test_fused_sra_tiny_and_exact_constant():
             g.allreduce(ins, [(0, n, 4 if n >= 16 else 32, 512)])
             torch.cuda.synchronize()
             for t in ins:
-                assert torch.equal(t.cpu(), torch.full((n,), float(world * (world + 1) // 2)))
+                assert_same(t.cpu(), torch.full((n,), float(world * (world + 1) // 2)))
 
 
 def test_fused_sra_large_buffer_many_lanes():
@@ -164,7 +166,8 @@ def test_fused_sra_large_buffer_many_lanes():
     g.allreduce(gpu, [(0, n, 4, 512)], False, False, False, 0, 1)
     torch.cuda.synchronize()
     g.check()
-    assert torch.equal(gpu[0].cpu(), cpu[0]) and torch.equal(gpu[1].cpu(), cpu[1])
+    assert_same(gpu[0].cpu(), cpu[0])
+    assert_same(gpu[1].cpu(), cpu[1])
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])
@@ -185,7 +188,7 @@ def test_oneshot_kernel_matches_cpu_oracle(world, dtype):
             torch.cuda.synchronize()
             g.check()
             for r in range(world):
-                assert torch.equal(gpu[r].cpu(), cpu[r])
+                assert_same(gpu[r].cpu(), cpu[r])
         # interleave with the three-phase kernel on the same heap
         gpu = [t.to(dev()) for t in ins]
         g.allreduce(gpu, layers, average, False, False, 0, 1)
@@ -193,4 +196,4 @@ def test_oneshot_kernel_matches_cpu_oracle(world, dtype):
         g.allreduce_oneshot(gpu, layers, average, False, False, 0, 1)
         torch.cuda.synchronize()
         for r in range(world):
-            assert torch.equal(gpu[r].cpu(), cpu[r])
+            assert_same(gpu[r].cpu(), cpu[r])

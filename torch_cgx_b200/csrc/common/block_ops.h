@@ -100,10 +100,14 @@ inline float round_to_dtype(float v, int dtype) {
   }
 }
 
-// acc[i] = float(src[elem_off + i]) * prescale
+// acc[i] = float(src[elem_off + i]) * prescale; a NaN product is the GPU's canonical NaN, as it is
+// on the device (raw records carry these values on the wire)
 inline void load_block(const void* src, int dtype, const BlockDesc& d, float prescale, float* acc) {
   const uint32_t n = block_n(d);
-  for (uint32_t i = 0; i < n; ++i) acc[i] = load_elem(src, dtype, (uint64_t)d.elem_off + i) * prescale;
+  for (uint32_t i = 0; i < n; ++i) {
+    const float v = load_elem(src, dtype, (uint64_t)d.elem_off + i) * prescale;
+    acc[i] = v == v ? v : canonical_nan();
+  }
 }
 
 // Quantize n fp32 values into the block's wire record. Buckets are self-contained: bucket k

@@ -11,6 +11,7 @@
 #pragma once
 #include <cmath>
 #include <cstdint>
+#include <cstring>
 
 #if defined(__CUDACC__)
 #define CGX_HD __host__ __device__ __forceinline__
@@ -29,6 +30,21 @@ struct BucketMeta {
   float min;
 };
 
+// The GPU's canonical NaN: what every fp32 arithmetic instruction and min.NaN / max.NaN
+// return when the result is NaN. The host code returns it too wherever a NaN can reach the
+// wire, so that wire bytes of a poisoned bucket are identical on the CPU and the GPU (x86
+// would keep the input's payload, or make 0xFFC00000 out of inf - inf).
+constexpr uint32_t kCanonicalNaNBits = 0x7FFFFFFFu;
+CGX_HD float canonical_nan() {
+#if defined(__CUDA_ARCH__)
+  return __int_as_float((int)kCanonicalNaNBits);
+#else
+  float f;
+  std::memcpy(&f, &kCanonicalNaNBits, 4);
+  return f;
+#endif
+}
+
 // NaN-propagating min/max (a NaN gradient must poison its bucket so that AMP
 // overflow checks on the reduced gradient still fire on every rank).
 CGX_HD float nan_min(float a, float b) {
@@ -37,8 +53,7 @@ CGX_HD float nan_min(float a, float b) {
   asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 #else
-  if (a != a) return a;
-  if (b != b) return b;
+  if (a != a || b != b) return canonical_nan();
   if (a == b) return std::signbit(a) ? a : b;  // -0 < +0, as PTX min does
   return a < b ? a : b;
 #endif
@@ -49,8 +64,7 @@ CGX_HD float nan_max(float a, float b) {
   asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 #else
-  if (a != a) return a;
-  if (b != b) return b;
+  if (a != a || b != b) return canonical_nan();
   if (a == b) return std::signbit(a) ? b : a;  // +0 > -0, as PTX max does
   return a > b ? a : b;
 #endif
@@ -80,6 +94,7 @@ CGX_HD BucketMeta make_meta(float mn, float mx, int bits) {
   m.unit = __fmul_rn(__fsub_rn(mx, mn), rcp_levels(bits));
 #else
   m.unit = (mx - mn) * rcp_levels(bits);
+  if (m.unit != m.unit) m.unit = canonical_nan();  // NaN min/max, or inf - inf
 #endif
   m.min = mn;
   return m;
