@@ -6,6 +6,10 @@ stream around a batch of back-to-back calls (nccl-tests style) over a rotating
 set of buffers larger than L2, MAX over ranks, median of 3 repetitions.
 
   torchrun --nproc-per-node N bench/allreduce_sweep.py --out gpurun_out/sweep_N.json
+  torchrun --nproc-per-node N bench/allreduce_sweep.py --op reduce_scatter   # cgx.reduce_scatter_tensor
+                                                                            # vs ncclReduceScatter
+With --op reduce_scatter the message is the input of W shards; NCCL's bus bandwidth is then
+algbw * (W-1)/W, and wire_bytes_per_rank counts the packed peer chunks (phase A only).
 
 Reported per row:
   time_us        median device time of one allreduce (max over ranks)
@@ -72,6 +76,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--bucket-size", type=int, default=512)
     ap.add_argument("--sizes", default="", help="explicit comma-separated sizes in KB (overrides min/max)")
+    ap.add_argument("--op", default="allreduce", choices=["allreduce", "reduce_scatter"])
     ap.add_argument("--with-nccl-sra", action="store_true",
                     help="also time the reference-structure path: SRA over NCCL send/recv + separate kernels")
     args = ap.parse_args()
@@ -104,17 +109,37 @@ def main():
         s *= 4
     if args.sizes:
         sizes = [int(x) << 10 for x in args.sizes.split(",")]
+    rs = args.op == "reduce_scatter"
+    bus = (world - 1) / world if rs else 2 * (world - 1) / world
+    if rs:
+        sizes = [s for s in sizes if s // es >= world]
+        outs = {}
+
+        def out_for(x):
+            return outs.setdefault(x.numel(), torch.empty(x.numel() // world, dtype=x.dtype, device=dev))
+
+        def nccl_op(x):
+            dist.reduce_scatter_tensor(out_for(x), x, group=nccl)
+
+        def cgx_op(x, bits):
+            cgx.reduce_scatter_tensor(out_for(x), x, bits=bits, bucket_size=args.bucket_size)
+    else:
+        def nccl_op(x):
+            dist.all_reduce(x, group=nccl)
+
+        def cgx_op(x, bits):
+            dist.all_reduce(x)
     rows = []
     for nbytes in sizes:
-        n = nbytes // es
+        n = nbytes // es // world * world if rs else nbytes // es
         # rotating buffers: total > 2x L2 (50 MB) so no call finds its input in cache
         nbuf = max(2, min(64, (288 << 20) // nbytes + 1))
         bufs = [torch.randn(n, device=dev).to(dtype) for _ in range(nbuf)]
         iters = args.iters if nbytes <= (64 << 20) else max(6, args.iters // 3)
-        t_nccl = time_allreduce(lambda x: dist.all_reduce(x, group=nccl), bufs, iters, args.warmup, dev)
-        row_base = {"bytes": nbytes, "dtype": args.dtype, "world": world}
+        t_nccl = time_allreduce(nccl_op, bufs, iters, args.warmup, dev)
+        row_base = {"op": args.op, "bytes": nbytes, "dtype": args.dtype, "world": world}
         r = dict(row_base, impl="nccl", bits=32, time_us=round(t_nccl, 2),
-                 algbw_gbs=round(nbytes / t_nccl / 1e3, 2), busbw_gbs=round(nbytes / t_nccl / 1e3 * 2 * (world - 1) / world, 2))
+                 algbw_gbs=round(nbytes / t_nccl / 1e3, 2), busbw_gbs=round(nbytes / t_nccl / 1e3 * bus, 2))
         rows.append(r)
         if rank == 0:
             print(json.dumps(r), flush=True)
@@ -123,18 +148,18 @@ def main():
             for x in bufs:
                 x.normal_()
             be.reset_stats()
-            t = time_allreduce(lambda x: dist.all_reduce(x), bufs, iters, args.warmup, dev)
+            t = time_allreduce(lambda x: cgx_op(x, bits), bufs, iters, args.warmup, dev)
             st = be.stats()
             wire_per_call = st[3] / max(1, st[0])
             r = dict(row_base, impl="cgx", bits=bits, time_us=round(t, 2), algbw_gbs=round(nbytes / t / 1e3, 2),
-                     busbw_gbs=round(nbytes / t / 1e3 * 2 * (world - 1) / world, 2),
+                     busbw_gbs=round(nbytes / t / 1e3 * bus, 2),
                      wire_bytes_per_rank=int(wire_per_call), wire_gbs=round(wire_per_call / t / 1e3, 2),
                      kernel_launches_per_call=round(st[1] / max(1, st[0]), 2),
                      speedup_vs_nccl=round(t_nccl / t, 3))
             rows.append(r)
             if rank == 0:
                 print(json.dumps(r), flush=True)
-            if nccl_sra is not None and bits < 32 and nbytes >= 4096:
+            if nccl_sra is not None and not rs and bits < 32 and nbytes >= 4096:
                 t2 = time_allreduce(lambda x: dist.all_reduce(x, group=nccl_sra), bufs, iters, args.warmup, dev)
                 r = dict(row_base, impl="cgx_sra_over_nccl_sendrecv", bits=bits, time_us=round(t2, 2),
                          algbw_gbs=round(nbytes / t2 / 1e3, 2),

@@ -12,3 +12,7 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # buckets (lg 0/1/2/5), and a five-rank world
 EDGE_SUBSET='w5- or (full_slices and (4-8 or 4-16 or 4-32 or 4-256 or 7-8 or 6-16)) or (standalone and f32-5- and (-8] or -32] or -1]))'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_kernels_edge_gpu.py -m gpu -x -q -k "$EDGE_SUBSET"
+# compressed reduce-scatter: edge inputs at W 2/3/5 (aligned, unaligned and aliased views), several windows, and
+# interleaved reduce-scatter / allreduce / one-shot calls on one heap
+RS_SUBSET='(edge_inputs and (w2-float32-q1- or w3-float16-q2- or w5-bfloat16-q3-)) or many_windows or interleaved'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_reduce_scatter_gpu.py -m gpu -x -q -k "$RS_SUBSET"

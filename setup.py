@@ -31,6 +31,9 @@ SOURCES = [
     "kernels/sra_f32.cu",
     "kernels/sra_f16.cu",
     "kernels/sra_bf16.cu",
+    "kernels/rs_f32.cu",
+    "kernels/rs_f16.cu",
+    "kernels/rs_bf16.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
     "pg/process_group_cgx.cc",

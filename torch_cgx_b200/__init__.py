@@ -27,7 +27,8 @@ from .backend import (  # noqa: E402
     set_quantization_bits,
     set_quantization_bucket_size,
 )
-from .parallel.functional import all_reduce, compression  # noqa: E402
+from .parallel.functional import all_reduce, compression, reduce_scatter_tensor  # noqa: E402
+from .parallel.fsdp import CGXReduceScatter, set_cgx_reduce_scatter  # noqa: E402
 from .parallel.hooks import CGXState, cgx_hook, register_cgx_hook  # noqa: E402
 from .utils.launch import map_launcher_env  # noqa: E402
 from . import models, ops, utils  # noqa: E402,F401
@@ -36,6 +37,7 @@ register_backend()
 
 __all__ = [
     "BACKEND_NAME",
+    "CGXReduceScatter",
     "CGXState",
     "all_reduce",
     "cgx_hook",
@@ -44,8 +46,10 @@ __all__ = [
     "map_launcher_env",
     "register_backend",
     "register_cgx_hook",
+    "reduce_scatter_tensor",
     "register_layer",
     "reset_layers",
     "set_quantization_bits",
+    "set_cgx_reduce_scatter",
     "set_quantization_bucket_size",
 ]

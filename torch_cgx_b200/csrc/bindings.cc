@@ -3,7 +3,7 @@
 //    set_quantization_bits, set_quantization_bucket_size;
 //    /root/reference/src/ProcessGroupCGX.cc:837-857)
 //  * planning / CPU oracle / standalone kernels for ops and tests
-//  * LocalSraGroup: W virtual ranks of the fused kernel inside ONE process on
+//  * LocalSraGroup: W virtual ranks of the fused kernels inside ONE process on
 //    ONE GPU (W heaps, W streams) so the full protocol is testable on a single
 //    device.
 #include <ATen/cuda/CUDAContext.h>
@@ -144,6 +144,44 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
   }
   Plan plan = build_plan(to_layers(layers), make_opts(1, lanes, dt, skip_incomplete, min_lane_elems));
   oneshot_simulate(plan, bufs, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
+}
+
+// the shard table replicated W times at stride S (chunk c == copy c); S = end of the table
+std::vector<LayerSpec> replicated_shard(const std::vector<LayerTuple>& shard_layers, int world, uint64_t* shard) {
+  std::vector<LayerSpec> one = to_layers(shard_layers), out;
+  uint64_t S = 0;
+  for (const LayerSpec& l : one) S = std::max<uint64_t>(S, l.elem_off + l.numel);
+  for (int c = 0; c < world; ++c)
+    for (LayerSpec l : one) {
+      l.elem_off += (uint64_t)c * S;
+      out.push_back(l);
+    }
+  *shard = S;
+  return out;
+}
+
+void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
+                                const std::vector<LayerTuple>& shard_layers, int lanes, bool average,
+                                bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
+                                int64_t min_lane_elems) {
+  TORCH_CHECK(!inputs.empty() && inputs.size() == outputs.size(), "reduce_scatter_simulate: one input and one output per rank");
+  const int W = (int)inputs.size();
+  const int dt = cgx_dtype(inputs[0]);
+  uint64_t S = 0;
+  auto layers = replicated_shard(shard_layers, W, &S);
+  std::vector<const void*> in;
+  std::vector<void*> out;
+  for (int r = 0; r < W; ++r) {
+    const at::Tensor &i = inputs[r], &o = outputs[r];
+    TORCH_CHECK(i.device().is_cpu() && o.device().is_cpu() && i.is_contiguous() && o.is_contiguous() &&
+                    cgx_dtype(i) == dt && cgx_dtype(o) == dt && (uint64_t)i.numel() == S * W &&
+                    (uint64_t)o.numel() == S,
+                "reduce_scatter_simulate: CPU contiguous tensors of one dtype, inputs of W * S and outputs of S elements");
+    in.push_back(i.data_ptr());
+    out.push_back(o.data_ptr());
+  }
+  Plan plan = build_plan(layers, make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
+  reduce_scatter_simulate(plan, in, out, S, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
 }
 
 // quantize `t` through the plan; returns uint8 wire tensor [world, row_bytes]
@@ -357,6 +395,44 @@ class LocalSraGroup {
     }
   }
 
+  // reduce-scatter: inputs[r] holds W * S elements of virtual rank r, outputs[r] receives shard r
+  void reduce_scatter(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
+                      const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete,
+                      bool stochastic, uint64_t seed, uint32_t seq) {
+    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_, "need one input and one output per virtual rank");
+    const int dt = cgx_dtype(inputs[0]);
+    auto specs = to_layers(shard_layers);
+    auto cur = c10::cuda::getCurrentCUDAStream();
+    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
+    ready.record(cur);
+    bool fresh_plan = false;
+    for (int r = 0; r < world_; ++r) {
+      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
+      TORCH_CHECK(inputs[r].numel() == outputs[r].numel() * world_, "inputs must hold W x the output elements");
+      ready.block(streams_[r]);
+      const size_t before = fused_[r]->num_plans();
+      fused_[r]->prepare_reduce_scatter(specs, dt, skip_incomplete, streams_[r].stream());
+      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
+    }
+    // streams r and r + 8 share a hardware queue (CUDA_DEVICE_MAX_CONNECTIONS = 8): with two kernels
+    // per virtual rank, rank r + 8's first one would wait behind rank r's second, which waits for it
+    TORCH_CHECK(world_ <= 8 || fused_[0]->rs_windows(specs, dt, skip_incomplete, 0).size() <= 1,
+                "LocalSraGroup.reduce_scatter: more than 8 virtual ranks need the shard to fit one window "
+                "(raise slot_bytes)");
+    // every plan upload lands before any virtual rank starts spinning
+    if (fresh_plan)
+      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    for (int r = 0; r < world_; ++r)
+      fused_[r]->reduce_scatter(specs, dt, skip_incomplete, inputs[r].data_ptr(), outputs[r].data_ptr(),
+                                (uint64_t)outputs[r].numel(), average ? 1.0f / (float)world_ : 1.0f, rng, streams_[r].stream());
+    for (int r = 0; r < world_; ++r) {
+      at::cuda::CUDAEvent done(cudaEventDisableTiming);
+      done.record(streams_[r]);
+      done.block(cur);
+    }
+  }
   void check() {
     for (auto& f : fused_) f->check_status();
   }
@@ -400,6 +476,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   py::class_<ProcessGroupCGX, c10d::Backend, c10::intrusive_ptr<ProcessGroupCGX>>(m, "ProcessGroupCGX")
       .def("allreduce_bucket", &ProcessGroupCGX::allreduce_bucket, py::arg("tensor"), py::arg("bucket_idx"),
            py::arg("average") = false, py::call_guard<py::gil_scoped_release>())
+      .def("reduce_scatter_compressed",
+           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, bool average, int bits, int bucket_size,
+              bool skip_incomplete, bool stochastic, int64_t seed, bool overlapped,
+              const std::vector<LayerTuple>& layers) {
+             return pg.reduce_scatter_compressed(out, in, average, bits, bucket_size, skip_incomplete, stochastic,
+                                                 seed, overlapped, to_layers(layers));
+           },
+           py::arg("output"), py::arg("input"), py::arg("average") = false, py::arg("bits") = 4,
+           py::arg("bucket_size") = 512, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
+           py::arg("seed") = -1, py::arg("overlapped") = false, py::arg("layers") = std::vector<LayerTuple>{},
+           py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -497,6 +584,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return plan_to_dict(build_plan(to_layers(layers), make_opts(world, lanes, dtype, skip_incomplete, min_lane_elems)));
   }, py::arg("layers"), py::arg("world"), py::arg("lanes"), py::arg("dtype") = 0, py::arg("skip_incomplete") = false,
         py::arg("min_lane_elems") = 2048);
+  m.def("reduce_scatter_windows", [](const std::vector<LayerTuple>& shard_layers, int world, int lanes, int dtype,
+                                     bool skip_incomplete, int64_t min_lane_elems, int64_t slot_bytes) {
+    std::vector<std::vector<LayerTuple>> out;
+    for (auto& w : reduce_scatter_windows(to_layers(shard_layers),
+                                          make_opts(world, lanes, dtype, skip_incomplete, min_lane_elems),
+                                          (uint32_t)slot_bytes)) {
+      std::vector<LayerTuple> o;
+      for (auto& l : w) o.emplace_back((int64_t)l.elem_off, (int64_t)l.numel, (int64_t)l.bits, (int64_t)l.bucket);
+      out.push_back(std::move(o));
+    }
+    return out;
+  }, py::arg("shard_layers"), py::arg("world"), py::arg("lanes"), py::arg("dtype") = 0,
+        py::arg("skip_incomplete") = false, py::arg("min_lane_elems") = 2048, py::arg("slot_bytes"));
   m.def("split_for_fusion", [](const std::vector<LayerTuple>& layers, int elsize, int64_t fusion_bytes) {
     std::vector<std::vector<LayerTuple>> out;
     for (auto& g : split_for_fusion(to_layers(layers), elsize, fusion_bytes)) {
@@ -510,6 +610,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sra_simulate", &py_sra_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
+  m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
+        py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
+        py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
@@ -582,6 +685,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("allreduce_oneshot", &LocalSraGroup::allreduce_oneshot, py::arg("tensors"), py::arg("layers"),
            py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0)
+      .def("reduce_scatter", &LocalSraGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
+           py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))

@@ -27,6 +27,30 @@ void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float presca
   }
 }
 
+void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& in_bufs,
+                             const std::vector<void*>& out_bufs, uint64_t shard, float prescale,
+                             const RngParams& rng) {
+  const int W = plan.world;
+  if ((int)in_bufs.size() != W || (int)out_bufs.size() != W)
+    throw std::invalid_argument("reduce_scatter_simulate: need one input and one output per rank");
+  std::vector<float> acc(kMaxBlockElems), tmp(kMaxBlockElems);
+  std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
+  for (int c = 0; c < W; ++c) {
+    for (uint32_t b = plan.chunk_begin(c); b < plan.chunk_end(c); ++b) {
+      const BlockDesc& d = plan.blocks[b];
+      cpu::load_block(in_bufs[c], plan.dtype, d, prescale, acc.data());
+      for (int q = 0; q < W; ++q) {
+        if (q == c) continue;
+        cpu::load_block(in_bufs[q], plan.dtype, d, prescale, tmp.data());
+        cpu::quantize_block(tmp.data(), plan.dtype, d, rec.data(), make_rng_key(rng, q, 0), b);
+        cpu::decode_block_add(rec.data(), plan.dtype, d, acc.data());
+      }
+      const uint64_t o = (uint64_t)d.elem_off - (uint64_t)c * shard;
+      for (uint32_t i = 0; i < block_n(d); ++i) cpu::store_elem(out_bufs[c], plan.dtype, o + i, acc[i]);
+    }
+  }
+}
+
 void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng) {
   if (plan.world != 1) throw std::invalid_argument("oneshot_simulate: plan must have a single chunk");
   const int W = (int)bufs.size();

@@ -35,6 +35,14 @@ void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float presca
 // every contribution quantized exactly once; `plan` must be a single-chunk plan (world == 1).
 void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng);
 
+// Reduce-scatter oracle (rs_kernel): `plan` covers a shard table replicated W times at stride
+// `shard` elements, so chunk c is copy c. out_bufs[c][e - c * shard] = T(prescale * in_c[e] + sum over
+// q != c, in rank order, of decode(Q_q(prescale * in_q[e]))) for every element e of chunk c: the
+// allreduce's phase-B sum (same primitives, order and phase-A RNG streams), not requantized.
+void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& in_bufs,
+                             const std::vector<void*>& out_bufs, uint64_t shard, float prescale,
+                             const RngParams& rng);
+
 // Quantize->dequantize round trip of one rank's buffer through the plan's
 // blocks (what a single compression step does to the data); used by the Python
 // ops and the tests.

@@ -23,7 +23,7 @@
 namespace cgx {
 
 struct EngineStats {
-  uint64_t calls = 0;            // allreduce calls
+  uint64_t calls = 0;            // allreduce and compressed reduce-scatter calls, together
   uint64_t kernel_launches = 0;  // fused kernel launches
   uint64_t elements = 0;
   uint64_t wire_bytes = 0;       // bytes this rank pushed over NVLink (both phases)
@@ -102,6 +102,15 @@ class AllreduceEngine {
   // Same, with an explicit layer list (offsets relative to `data`).
   void allreduce_cuda_layers(void* data, int dtype, const std::vector<LayerSpec>& layers, bool average,
                              const CompressionEnv& env, cudaStream_t stream, bool overlapped = false);
+
+  // Compressed reduce-scatter of a CUDA buffer on `stream` (FusedSra::reduce_scatter): `in` holds
+  // world * S elements, `out` receives this rank's shard of S elements. An empty `shard_layers`
+  // means one layer of S elements with `bits` / `bucket`, raw unless S exceeds
+  // CGX_COMPRESSION_MINIMAL_SIZE. Single node, P2P transport only; adds to the same counters as
+  // the allreduce.
+  void reduce_scatter_cuda(const void* in, void* out, int dtype, int64_t shard_numel,
+                           std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
+                           bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped);
 
   void check_health();
   const EngineStats& stats() const { return stats_; }

@@ -595,6 +595,7 @@ __device__ __forceinline__ void raw_wire_load(const uint8_t* p, float (&v)[8]) {
 //   MODE 0: push (phase A / one-shot 1): dst <- T(x * prescale)
 //   MODE 1: reduce (phase B): x * prescale + sum(sources) -> own, dst
 //   MODE 2: receive: out <- source (ss.n == 1) or sum of all sources
+//   MODE 3: reduce-scatter: x * prescale + sum(sources) -> blk (the output shard) only
 // (x may have more than 2 rows -- the prefetch buffer of a 1024 slice -- only rows 0 and 1 are used)
 template <typename T, int MODE, int ROWS, typename DST>
 __device__ __forceinline__ void raw_full_x(float (&x)[ROWS][8], T* __restrict__ blk, const WarpItem& it,
@@ -616,7 +617,7 @@ __device__ __forceinline__ void raw_full_x(float (&x)[ROWS][8], T* __restrict__ 
         for (int j = 0; j < 8; ++j) x[k][j] = __fadd_rn(x[k][j], v[k][j]);
     }
   }
-  if (MODE != 2) {
+  if (MODE == 0 || MODE == 1) {
 #pragma unroll
     for (int k = 0; k < 2; ++k)
       raw_wire_store<T>(ds, it.meta_off + (lane_id() * 2u + (uint32_t)k) * 8u * (uint32_t)sizeof(T), x[k]);
@@ -692,6 +693,66 @@ __device__ __noinline__ void raw_generic(T* __restrict__ blk, const WarpItem it,
         dst_st_u16(du, o, *reinterpret_cast<const uint16_t*>(&t));
     }
     if (mode != 0) blk[i] = t;
+  }
+}
+
+// ======================================================================================
+// reduce-scatter (rs_kernel phase B): my values * prescale + the decoded copies of the W-1
+// sources, in slot order, stored as T to the output shard. Nothing is requantized or published.
+// `src` and `out` are either disjoint or the same address (output aliasing my input chunk):
+// every lane reads an element before it writes it, so they carry no __restrict__.
+// ======================================================================================
+template <typename T, int KB, int GPL, bool VEC>
+__device__ __forceinline__ void full_rs_x(float (&x)[GPL][8], const WarpItem& it, float prescale, const SrcSet& ss,
+                                          T* out) {
+  const int bits = KB ? KB : item_bits(it);
+  slice_scale<GPL>(x, prescale);
+  slice_accumulate<KB, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), bits, x);
+  slice_store<T, GPL, VEC>(out, x);
+}
+template <typename T, int KB, int GPL>
+__device__ __noinline__ void full_rs_unaligned(const T* src, const WarpItem it, float prescale, const SrcSet ss,
+                                               T* out) {
+  float x[GPL][8];
+  slice_load_scalar<T, GPL>(src, x);
+  full_rs_x<T, KB, GPL, false>(x, it, prescale, ss, out);
+}
+
+template <typename T>
+__device__ __noinline__ void bucket_rs(const T* src, const WarpItem it, float prescale, const SrcSet ss, T* out) {
+  const uint32_t n = item_n(it);
+  const int bits = item_bits(it);
+  const uint32_t ng = div_up(n, 8u);
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<T>(src, g, n, prescale, x, nv);
+    bucket_add_sources(ss, it, g, bits, x);
+    store8_scalar<T>(out + g * 8u, nv, x);
+  }
+}
+
+// raw tail, or a full raw item whose input or output is not vector aligned: element-wise
+template <typename T>
+__device__ __noinline__ void raw_rs_generic(const T* src, const WarpItem it, float prescale, const SrcSet ss,
+                                            T* out) {
+  const uint32_t n = item_n(it);
+  for (uint32_t i = lane_id(); i < n; i += 32) {
+    float x = __fmul_rn(DT<T>::to_float(src[i]), prescale);
+    for (int q = 0; q < ss.n; ++q) {
+      if (q == ss.skip) continue;
+      const T* rec = reinterpret_cast<const T*>(ss.base + (size_t)q * ss.stride + it.meta_off);
+      T v;
+      if (sizeof(T) == 4) {
+        const uint32_t b = ld_sys_u32(rec + i);
+        v = *reinterpret_cast<const T*>(&b);
+      } else {
+        const uint16_t b = (uint16_t)ld_sys_u16(rec + i);
+        v = *reinterpret_cast<const T*>(&b);
+      }
+      x = __fadd_rn(x, DT<T>::to_float(v));
+    }
+    out[i] = DT<T>::from_float(x);
   }
 }
 

@@ -10,6 +10,8 @@
 //            stores otherwise -- and write the self-decoded values to my gradient buffer
 //   phase C  acquire each peer's reduced chunk (in order of arrival), dequantize into my buffer
 //
+// rs_kernel (reduce-scatter) is phases A and B without the requantization, the publish and phase C.
+//
 // The grid is G persistent *lanes* (CTAs of 8 warps, two per SM). Lane c of every rank only ever
 // talks to lane c of the other ranks through single-writer epoch flags, so there is no grid-wide
 // or host synchronisation anywhere and lanes pipeline independently. The work of a lane is a
@@ -569,31 +571,114 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(con
   sync_finish(p.sync, epoch, p.lanes);
 }
 
+// ===========================================================================
+// Compressed reduce-scatter: phase A of the SRA (every peer's chunk quantized once and pushed into
+// its owner's recv1 slot), then a phase B that adds the W-1 decoded copies to my own unquantized
+// values in fp32 and stores T(sum) to the output shard. No requantization, no phase C.
+// The plan is the shard's layer table replicated W times at stride S (chunk c == copy c), so an
+// item of my chunk at element e of the input lands on out[e - rank * S] (p.out_shift).
+// Without phase C nothing proves that the peers are done reading my recv1 stores, so the kernel
+// ends with a handshake on flags2 (docs/MEMORY_MODEL.md): a peer's next call can only overwrite
+// the slots after every lane of this call has finished its reads.
+// ===========================================================================
+template <typename T, int KB, int GPL>
+__device__ __forceinline__ void rs_phase_b(const SraParams& p, const LaneItems& li) {
+  const int r = p.rank, W = p.world;
+  const uint32_t warp = threadIdx.x >> 5;
+  const T* data = reinterpret_cast<const T*>(p.data);
+  T* out = reinterpret_cast<T*>(p.out);
+  const SrcSet ss{p.recv1[r], p.slot_bytes, W, r};
+  const OneDst none{nullptr};
+  const uint32_t end = li.pre[1];
+  for (uint32_t i = li.pre[0] + warp; i < end; i += kSraWarps) {
+    const WarpItem it = lane_item(li, p, i, 0);
+    const uint32_t kind = item_kind(it);
+    const T* src = data + it.elem_off;
+    T* dst = out + ((uint64_t)it.elem_off - p.out_shift);
+    const bool al = group_aligned<T>(src) && group_aligned<T>(dst);
+    float x[GPL][8];
+    if (al && kind == kItemFull) slice_load_vec<T, GPL>(src, x);
+    if (al && kind == kItemRaw) raw_load_vec<T, GPL>(src, x);
+    if (i + kSraWarps < end) slice_prefetch_l2<T, GPL>(data + lane_item(li, p, i + kSraWarps, 0).elem_off);
+    if (kind == kItemFull) {
+      if (al)
+        full_rs_x<T, KB, GPL, true>(x, it, p.prescale, ss, dst);
+      else
+        full_rs_unaligned<T, KB, GPL>(src, it, p.prescale, ss, dst);
+    } else if (kind == kItemBucket) {
+      bucket_rs<T>(src, it, p.prescale, ss, dst);
+    } else if (kind == kItemRaw && al) {
+      raw_full_x<T, 3, GPL>(x, dst, it, p.prescale, ss, none);
+    } else {
+      raw_rs_generic<T>(src, it, p.prescale, ss, dst);
+    }
+  }
+}
+
+template <typename T, int KB, int GPL>
+__global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __grid_constant__ SraParams p) {
+  __shared__ LaneItems li;
+  __shared__ int s_abort;
+  const int lane = blockIdx.x;
+  const uint32_t epoch = *reinterpret_cast<volatile uint32_t*>(&p.sync->epoch) + 1u;
+  const uint32_t flag = flag_value(epoch, 0);
+  if (threadIdx.x == 0) s_abort = 0;
+  lane_items_load(li, p, p.world, 1);
+  trace_mark(p, lane, 0, true);
+
+  sra_phase_a<T, KB, GPL>(p, li, epoch, 0);
+  __syncthreads();
+  trace_mark(p, lane, 1);
+  if (threadIdx.x < 32) {
+    signal_peers(p.flags1, p.world, p.rank, p.flag_stride, lane, flag);
+    if (li.pre[1] > li.pre[0] && !wait_peers(p.flags1[p.rank], p, lane, flag, kSraTimeoutPhase1)) s_abort = 1;
+  }
+  __syncthreads();
+  trace_mark(p, lane, 2);
+  if (!s_abort) rs_phase_b<T, KB, GPL>(p, li);
+  __syncthreads();
+  trace_mark(p, lane, 3);
+
+  // slot handshake: every lane, whether or not it had items (a peer's next call may give this
+  // lane's slot range to another lane)
+  if (threadIdx.x < 32 && !s_abort) {
+    signal_peers(p.flags2, p.world, p.rank, p.flag_stride, lane, flag);
+    wait_peers(p.flags2[p.rank], p, lane, flag, kSraTimeoutPhase2);
+  }
+  trace_mark(p, lane, 5);
+  sync_finish(p.sync, epoch, p.lanes);
+}
+
 }  // namespace dev
 
 // ---- host side: pick the instantiation --------------------------------------------------
-template <typename T, int KB, int GPL>
+// RS: the reduce-scatter kernel. It is instantiated in translation units of its own
+// (rs_{f32,f16,bf16}.cu): the out-of-line helpers of phase A are register-allocated per module,
+// and sharing them with rs_kernel would change the allreduce kernels' spill counts.
+template <typename T, int KB, int GPL, bool RS>
 cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
-  if (p.oneshot)
+  if constexpr (RS)
+    dev::rs_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+  else if (p.oneshot)
     dev::oneshot_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else
     dev::sra_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
-template <typename T, int GPL>
+template <typename T, int GPL, bool RS>
 cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
   switch (p.uniform_bits) {
-    case 2: return launch_sra_inst<T, 2, GPL>(p, stream);
-    case 4: return launch_sra_inst<T, 4, GPL>(p, stream);
-    case 8: return launch_sra_inst<T, 8, GPL>(p, stream);
-    default: return launch_sra_inst<T, 0, GPL>(p, stream);
+    case 2: return launch_sra_inst<T, 2, GPL, RS>(p, stream);
+    case 4: return launch_sra_inst<T, 4, GPL, RS>(p, stream);
+    case 8: return launch_sra_inst<T, 8, GPL, RS>(p, stream);
+    default: return launch_sra_inst<T, 0, GPL, RS>(p, stream);
   }
 }
 
-template <typename T>
+template <typename T, bool RS = false>
 cudaError_t launch_sra_t(const SraParams& p, cudaStream_t stream) {
-  return p.slice_elems == 1024 ? launch_sra_gpl<T, 4>(p, stream) : launch_sra_gpl<T, 2>(p, stream);
+  return p.slice_elems == 1024 ? launch_sra_gpl<T, 4, RS>(p, stream) : launch_sra_gpl<T, 2, RS>(p, stream);
 }
 
 template <typename T>
@@ -612,5 +697,9 @@ cudaError_t launch_sra_bf16(const SraParams& p, cudaStream_t stream);
 int sra_resident_per_sm_f32();
 int sra_resident_per_sm_f16();
 int sra_resident_per_sm_bf16();
+// defined once per dtype in rs_{f32,f16,bf16}.cu
+cudaError_t launch_rs_f32(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_rs_f16(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_rs_bf16(const SraParams& p, cudaStream_t stream);
 
 }  // namespace cgx

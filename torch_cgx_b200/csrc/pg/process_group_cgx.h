@@ -177,6 +177,15 @@ class ProcessGroupCGX : public c10d::Backend {
   // allreduce of one DDP bucket whose index is known (no cursor guessing);
   // average == true fuses the 1/world scale into the kernel.
   c10::intrusive_ptr<c10d::Work> allreduce_bucket(at::Tensor& tensor, int64_t bucket_idx, bool average);
+  // Compressed reduce-scatter (reduce_scatter_tensor semantics: `in` holds size() * out.numel()
+  // elements, rank r receives shard r) through the fused P2P kernel; the reduce-scatter entry points
+  // of c10d stay with the delegate. `layers`: quantization table of one shard, (elem_off, numel,
+  // bits, bucket) relative to the shard start, empty = one layer with `bits` / `bucket_size`.
+  // seed < 0: CGX_SEED. overlapped: at most CGX_OVERLAP_LANES CTAs (runs beside compute).
+  c10::intrusive_ptr<c10d::Work> reduce_scatter_compressed(at::Tensor& out, at::Tensor& in, bool average, int bits,
+                                                           int bucket_size, bool skip_incomplete, bool stochastic,
+                                                           int64_t seed, bool overlapped,
+                                                           const std::vector<LayerSpec>& layers);
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

@@ -5,6 +5,7 @@
 #include <string>
 
 #include "../common/config.h"
+#include "../engine/engine.h"  // split_for_fusion
 #include "../kernels/launch.h"
 
 namespace cgx {
@@ -111,6 +112,135 @@ void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngPa
   launch(dp, data, prescale, rng, stream, false);
 }
 
+namespace {
+
+// S: end of the shard table, which must tile [0, S) in order
+uint64_t shard_elems(const std::vector<LayerSpec>& layers) {
+  uint64_t end = 0;
+  for (const LayerSpec& l : layers) {
+    if (l.elem_off != end)
+      throw std::invalid_argument("cgx reduce_scatter: the shard layers must tile [0, S) in order, without gaps");
+    end += l.numel;
+  }
+  return end;
+}
+
+// split_for_fusion cuts a layer at multiples of its bucket size. A bucket above kMaxBlockElems is
+// quantized as kMaxBlockElems-element buckets counted from the layer start, while skip_incomplete
+// counts complete buckets of the requested size: such a layer is cut at multiples of both.
+std::vector<std::vector<LayerSpec>> split_shard(const std::vector<LayerSpec>& layers, int elsize, int64_t budget) {
+  std::vector<LayerSpec> cut = layers;
+  for (LayerSpec& l : cut) {
+    if (l.bits >= kRawBits || l.bucket <= kMaxBlockElems) continue;
+    uint64_t a = l.bucket, b = kMaxBlockElems;
+    while (b) {
+      const uint64_t t = a % b;
+      a = b;
+      b = t;
+    }
+    const uint64_t lcm = (uint64_t)l.bucket / a * kMaxBlockElems;
+    if (lcm > 0xFFFFFFFFull) throw std::invalid_argument("cgx reduce_scatter: quantization bucket size too large");
+    l.bucket = (uint32_t)lcm;
+  }
+  std::vector<std::vector<LayerSpec>> groups = split_for_fusion(cut, elsize, budget);
+  size_t k = 0;
+  for (auto& g : groups)
+    for (LayerSpec& s : g) {
+      while (s.elem_off >= layers[k].elem_off + layers[k].numel) ++k;
+      s.bucket = layers[k].bucket;
+    }
+  return groups;
+}
+
+// the window's table for the plan: W copies at stride S, copy c = chunk c
+std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& window, int world, uint64_t S) {
+  std::vector<LayerSpec> out;
+  out.reserve(window.size() * (size_t)world);
+  for (int c = 0; c < world; ++c)
+    for (LayerSpec l : window) {
+      l.elem_off += (uint64_t)c * S;
+      out.push_back(l);
+    }
+  return out;
+}
+
+}  // namespace
+
+std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<LayerSpec>& shard_layers,
+                                                           const PlanOptions& opt, uint32_t slot_bytes) {
+  const uint64_t S = shard_elems(shard_layers);
+  if (S == 0) return {};
+  if (S * (uint64_t)opt.world >= (1ull << 32))
+    throw std::invalid_argument("cgx reduce_scatter: the input exceeds 2^32 elements");
+  // the largest raw budget whose every window plan fits a slot, halved until it does, starting from
+  // the whole shard or the most a slot can carry at 1 bit per element
+  const int elsize = dtype_size(opt.dtype);
+  for (int64_t budget = (int64_t)std::min<uint64_t>(S * elsize, (uint64_t)slot_bytes * 8 * elsize);; budget /= 2) {
+    if (budget < elsize)
+      throw std::runtime_error("cgx reduce_scatter: one quantization bucket does not fit the heap slots");
+    std::vector<std::vector<LayerSpec>> wins = split_shard(shard_layers, elsize, budget);
+    bool fits = true;
+    for (const auto& w : wins) fits = fits && build_plan(replicate(w, opt.world, S), opt).max_chunk_wire <= slot_bytes;
+    if (fits) return wins;
+  }
+}
+
+const std::vector<std::vector<LayerSpec>>& FusedSra::rs_windows(const std::vector<LayerSpec>& shard_layers, int dtype,
+                                                                bool skip_incomplete, int max_lanes) {
+  PlanOptions opt;
+  opt.world = world();
+  opt.lanes = (max_lanes > 0 && max_lanes < max_lanes_) ? max_lanes : max_lanes_;
+  opt.dtype = dtype;
+  opt.skip_incomplete = skip_incomplete;
+  opt.min_lane_elems = min_lane_elems_;
+  const uint64_t key = plan_key(shard_layers, opt);
+  auto hit = rs_windows_.find(key);
+  if (hit != rs_windows_.end()) return hit->second;
+  std::vector<std::vector<LayerSpec>> wins = reduce_scatter_windows(shard_layers, opt, heap_->layout().slot_bytes);
+  if (rs_windows_.size() >= kMaxCachedPlans) rs_windows_.clear();
+  return rs_windows_.emplace(key, std::move(wins)).first->second;
+}
+
+void FusedSra::prepare_reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                                      cudaStream_t stream, int max_lanes) {
+  const uint64_t S = shard_elems(shard_layers);
+  for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes))
+    prepare(replicate(w, world(), S), dtype, skip_incomplete, stream, max_lanes);
+}
+
+FusedSra::RsCounts FusedSra::reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype,
+                                            bool skip_incomplete, const void* in, void* out, uint64_t out_numel,
+                                            float prescale, const RngParams& rng, cudaStream_t stream,
+                                            int max_lanes) {
+  RsCounts n;
+  const uint64_t S = shard_elems(shard_layers);
+  if (S != out_numel)
+    throw std::invalid_argument("cgx reduce_scatter: the shard layers tile [0, " + std::to_string(S) +
+                                ") but the output has " + std::to_string(out_numel) + " elements");
+  if (S == 0) return n;
+  {
+    const uint64_t es = (uint64_t)dtype_size(dtype);
+    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), o0 = reinterpret_cast<uintptr_t>(out);
+    const bool own_chunk = o0 == i0 + (uint64_t)rank() * S * es;
+    const bool disjoint = o0 + S * es <= i0 || i0 + (uint64_t)world() * S * es <= o0;
+    if (!own_chunk && !disjoint)
+      throw std::invalid_argument("cgx reduce_scatter: the output overlaps the input other than as its chunk " +
+                                  std::to_string(rank()));
+  }
+  // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
+  for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes)) {
+    const DevicePlan* dp = prepare(replicate(w, world(), S), dtype, skip_incomplete, stream, max_lanes);
+    if (dp == nullptr) throw std::runtime_error("cgx reduce_scatter: window plan does not fit the heap slots");
+    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S);
+    const Plan& pl = dp->plan;
+    ++n.launches;
+    n.elements += pl.numel;
+    n.wire_bytes += pl.total_wire - pl.chunk_wire_bytes[rank()];
+    n.raw_bytes += (pl.numel - pl.chunk_elems[rank()]) * (uint64_t)dtype_size(dtype);
+  }
+  return n;
+}
+
 void FusedSra::run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng,
                            cudaStream_t stream) {
   launch(dp, data, prescale, rng, stream, true);
@@ -130,7 +260,7 @@ int FusedSra::pick_stages(const DevicePlan&) const {
 }
 
 void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-                      bool oneshot) {
+                      bool oneshot, void* out, uint64_t out_shift) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   if (dp.plan.items.empty()) return;
   ++epoch_;
@@ -157,7 +287,8 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
     p.flags1[q] = valid ? heap_->flags1(q) : nullptr;
     p.flags2[q] = valid ? heap_->flags2(q) : nullptr;
   }
-  const bool mc = use_mc_ && dp.multicast_ok;
+  // the reduce-scatter kernel uses recv1 and unicast stores only
+  const bool mc = use_mc_ && dp.multicast_ok && out == nullptr;
   p.mc_recv1 = (mc && oneshot) ? heap_->mc_oneshot(0) : nullptr;
   p.mc_recv2 = (mc && !oneshot) ? heap_->mc_recv2() : nullptr;
   p.mc_reduce = (mc && !oneshot && use_mc_reduce_) ? 1 : 0;
@@ -179,7 +310,9 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
   p.uniform_bits = dp.plan.uniform_bits;
   p.slice_elems = (int)dp.plan.slice_elems;
   p.oneshot = oneshot ? 1 : 0;
-  p.stages = oneshot ? 1 : pick_stages(dp);
+  p.stages = (oneshot || out != nullptr) ? 1 : pick_stages(dp);
+  p.out = out;
+  p.out_shift = out_shift;
   cuda_check(launch_sra_fused(p, stream), "launch_sra_fused");
   ++launches_;
 }

@@ -25,6 +25,14 @@ struct DevicePlan {
   bool multicast_ok = false;         // every compressed item has a width multimem.st can carry (2/4/8)
 };
 
+// The windows of a reduce-scatter: the shard's layer table (offsets from the shard start, tiling
+// [0, S) in order; std::invalid_argument otherwise) cut by split_for_fusion into shard-relative
+// tables whose plans -- the window replicated opt.world times at stride S -- fit `slot_bytes` per
+// chunk. Cuts fall on bucket boundaries (for buckets above kMaxBlockElems on multiples of both
+// sizes), so the result of the operation does not depend on the windows.
+std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<LayerSpec>& shard_layers,
+                                                           const PlanOptions& opt, uint32_t slot_bytes);
+
 class FusedSra {
  public:
   FusedSra(SymmetricHeap* heap, int max_lanes, int64_t timeout_ms, uint32_t min_lane_elems);
@@ -51,6 +59,27 @@ class FusedSra {
   const DevicePlan* prepare_oneshot(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                     cudaStream_t stream, int max_lanes = 0);
   void run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream);
+
+  // Compressed reduce-scatter (rs_kernel). `in` holds W * S elements, `out` S elements; this rank
+  // receives shard rank():  out = T(prescale * in[r] + sum over peers p of decode(Q(prescale * in_p[r]))).
+  // `shard_layers` is the quantization table of ONE shard (offsets from the shard start, tiling
+  // [0, S), S == out_numel); every shard uses it, so buckets are counted from each shard's start. `out` is disjoint
+  // from `in` or exactly its chunk rank(); anything else throws std::invalid_argument.
+  // The shard is cut into windows whose worst-case wire fits one slot (split_for_fusion, cuts on
+  // bucket boundaries, so the result does not depend on the slot size) and one kernel is launched
+  // per window. Stream-ordered; every rank must issue the same calls in the same order.
+  struct RsCounts {
+    uint64_t launches = 0, elements = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's share
+  };
+  RsCounts reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete, const void* in,
+                          void* out, uint64_t out_numel, float prescale, const RngParams& rng, cudaStream_t stream,
+                          int max_lanes = 0);
+  // builds and uploads the plans of every window without launching anything
+  void prepare_reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                              cudaStream_t stream, int max_lanes = 0);
+  // reduce_scatter_windows for this heap (cached per shard table)
+  const std::vector<std::vector<LayerSpec>>& rs_windows(const std::vector<LayerSpec>& shard_layers, int dtype,
+                                                        bool skip_incomplete, int max_lanes);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();
@@ -90,8 +119,9 @@ class FusedSra {
   const DevicePlan* prepare_impl(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                  cudaStream_t stream, int plan_world, uint32_t capacity, int max_lanes);
   void launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-              bool oneshot);
+              bool oneshot, void* out = nullptr, uint64_t out_shift = 0);
   std::unordered_map<uint64_t, std::unique_ptr<DevicePlan>> cache_;
+  std::unordered_map<uint64_t, std::vector<std::vector<LayerSpec>>> rs_windows_;
 };
 
 }  // namespace cgx

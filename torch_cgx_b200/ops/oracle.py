@@ -295,6 +295,50 @@ def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *
     return _to_tensors(outs, dtype)
 
 
+def _shards(inputs: Sequence[torch.Tensor], r: int) -> List[torch.Tensor]:
+    W = len(inputs)
+    n = inputs[0].numel()
+    assert n % W == 0, "a reduce-scatter input holds world x shard elements"
+    S = n // W
+    return [t.detach().reshape(-1)[r * S:(r + 1) * S] for t in inputs]
+
+
+def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
+                             world: int | None = None, average: bool = False,
+                             skip_incomplete: bool = False) -> List[torch.Tensor]:
+    """Every rank's output of the compressed reduce-scatter (deterministic rounding).
+
+    ``inputs[r]`` holds W shards of S elements; ``shard_layers`` is one shard's table (offsets from
+    the shard start), the same for every shard, so buckets are counted from each shard's start.
+    Rank r receives, per element of shard r, in fp32:
+        prescale*x_r  (kept unquantized)  +  sum over q != r, in rank order, of Q(prescale*x_q)
+    rounded once to the dtype: the SRA's phase-B accumulator without the requantization. Raw runs
+    round each peer contribution to the dtype. Elements outside every layer are 0.
+    """
+    W = len(inputs)
+    assert world is None or world == W
+    dtype = inputs[0].dtype
+    ps = _prescale(W, average)
+    outs = []
+    for r in range(W):
+        xs = _scaled_inputs(_shards(inputs, r), ps)
+        out = np.zeros(xs[0].size, _F32)
+        for off, m, bits, bucket in layer_segments(shard_layers, skip_incomplete):
+            sl = slice(off, off + m)
+            out[sl] = _sra_acc(xs, sl, np.full(m, r), bits, bucket, dtype)
+        outs.append(out)
+    return _to_tensors(outs, dtype)
+
+
+def reduce_scatter_exact_and_bound(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
+                                   average: bool = False, skip_incomplete: bool = False,
+                                   stochastic: bool = False) -> List[Tuple[np.ndarray, np.ndarray]]:
+    """Per rank r: the fp64 exact sum of shard r and a per-element bound on the reduce-scatter's
+    error (``exact_sum_and_bound`` of one quantization round, rank r's own values exact)."""
+    return [exact_sum_and_bound(_shards(inputs, r), shard_layers, average=average, skip_incomplete=skip_incomplete,
+                                stochastic=stochastic, oneshot=True, exact_rank=r) for r in range(len(inputs))]
+
+
 def _half_ulp(v: np.ndarray, dtype: torch.dtype) -> np.ndarray:
     """Half an ulp of ``dtype`` at magnitude |v| (subnormal spacing below the normal range)."""
     mant, emin = _DTYPE_FMT[dtype]
@@ -312,7 +356,8 @@ def _round_err(unit: np.ndarray, h: float, levels: float) -> np.ndarray:
 
 def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, lanes: int = 1,
                         min_lane_elems: int = 2048, average: bool = False, skip_incomplete: bool = False,
-                        stochastic: bool = False, oneshot: bool = False) -> Tuple[np.ndarray, np.ndarray]:
+                        stochastic: bool = False, oneshot: bool = False,
+                        exact_rank: int | None = None) -> Tuple[np.ndarray, np.ndarray]:
     """fp64 exact sum  sum_q prescale*x_q  and a per-element bound on |result - exact|.
 
     Compressed runs: for every quantized contribution unit/2 of its bucket (a full unit with
@@ -323,6 +368,8 @@ def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer],
     the output dtype; raw runs add half an ulp of the dtype per rounded contribution.
     The bound is meaningful where the exact sum and the inputs are finite. Elements outside
     every layer (each rank keeps its own) have a NaN exact sum.
+    ``oneshot`` with ``exact_rank``: that rank's contribution is added unquantized (the
+    compressed reduce-scatter, one quantization round per peer).
     """
     W = len(inputs)
     dtype = inputs[0].dtype
@@ -339,6 +386,12 @@ def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer],
     h = 1.0 if stochastic else 0.5
     u32 = 2.0 ** -24    # relative error of one fp32 rounding ...
     tiny = 2.0 ** -150  # ... plus this absolute one in the subnormal range
+
+    def _sent(q: int, sl: slice) -> np.ndarray:  # elements where rank q's contribution is quantized
+        if oneshot:
+            return np.full(sl.stop - sl.start, q != exact_rank)
+        return owner[sl] != q
+
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
         sl = slice(off, off + m)
         exact[sl] = total[sl]
@@ -347,7 +400,7 @@ def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer],
             err = np.zeros(m)
             for q in range(W):
                 hu = _half_ulp(xs[q][sl], dtype) if dtype != torch.float32 else 0.0
-                err += hu if oneshot else np.where(owner[sl] != q, hu, 0.0)
+                err += np.where(_sent(q, sl), hu, 0.0)
             b = err + (W + 2) * (u32 * (mag + err) + tiny)
         else:
             levels = float((1 << bits) - 1)
@@ -355,7 +408,7 @@ def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer],
             span = np.zeros(m)
             for q in range(W):
                 unit = _qdq_buckets(xs[q][sl], bits, bucket)[2].astype(np.float64)
-                sent = np.ones(m, bool) if oneshot else owner[sl] != q
+                sent = _sent(q, sl)
                 qerr += np.where(sent, _round_err(unit, h, levels), 0.0)
                 span += unit * levels
             b = qerr

@@ -7,12 +7,17 @@ manager that sets them is all that is needed to quantize *one* collective differ
     with cgx.compression(bits=2, bucket_size=256, stochastic=True):
         dist.all_reduce(grad)              # 2-bit QSGD for this call only
     cgx.all_reduce(t, bits=8, average=True)  # same thing as a function
+
+The compressed reduce-scatter is asked for explicitly (``dist.reduce_scatter_tensor`` on a
+``cgx`` group keeps going to the uncompressed delegate)::
+
+    cgx.reduce_scatter_tensor(shard, flat_grads, bits=4, average=True)
 """
 from __future__ import annotations
 
 import contextlib
 import os
-from typing import Iterator, Optional
+from typing import Iterator, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -59,3 +64,41 @@ def all_reduce(tensor: torch.Tensor, bits: Optional[int] = None, bucket_size: Op
     op = dist.ReduceOp.AVG if average else dist.ReduceOp.SUM
     with compression(bits=bits, bucket_size=bucket_size, **kw):
         return dist.all_reduce(tensor, op=op, group=group, async_op=async_op)
+
+
+def _reduce_scatter(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, average: bool,
+                    group, async_op: bool, stochastic: bool, seed: Optional[int],
+                    layers: Optional[Sequence[Tuple[int, int, int, int]]], skip_incomplete: bool,
+                    overlapped: bool):
+    from .hooks import _native_backend
+
+    native = _native_backend(group if group is not None else dist.group.WORLD, input)
+    if native is None:
+        raise RuntimeError("cgx.reduce_scatter_tensor needs a process group with the cgx backend")
+    work = native.reduce_scatter_compressed(
+        output, input, bool(average), int(bits), int(bucket_size), bool(skip_incomplete), bool(stochastic),
+        -1 if seed is None else int(seed), bool(overlapped),
+        [tuple(int(v) for v in l) for l in (layers or [])])
+    if async_op:
+        return work
+    work.wait()  # the current stream waits for the kernel; the host does not
+    return None
+
+
+def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
+                          average: bool = False, group=None, async_op: bool = False, stochastic: bool = False,
+                          seed: Optional[int] = None, layers: Optional[Sequence[Tuple[int, int, int, int]]] = None,
+                          skip_incomplete: bool = False):
+    """Compressed ``dist.reduce_scatter_tensor`` (SUM, or AVG with ``average=True``) on a ``cgx`` group.
+
+    ``input`` holds ``world * output.numel()`` elements; rank r receives shard r. Every peer's
+    contribution is quantized once (``bits``, buckets of ``bucket_size`` counted from each shard's
+    start) and summed in fp32 with the receiving rank's own, unquantized values. ``layers``
+    optionally gives one shard's quantization table as ``(elem_off, numel, bits, bucket_size)``
+    tuples relative to the shard start (bits 32: uncompressed); the same table applies to every
+    shard. ``seed=None`` uses ``CGX_SEED``. ``output`` may be the rank's own chunk of ``input``.
+    Single node, CUDA float32 / float16 / bfloat16.
+    """
+    return _reduce_scatter(output, input, bits=bits, bucket_size=bucket_size, average=average, group=group,
+                           async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
+                           skip_incomplete=skip_incomplete, overlapped=False)
