@@ -8,8 +8,11 @@ set of buffers larger than L2, MAX over ranks, median of 3 repetitions.
   torchrun --nproc-per-node N bench/allreduce_sweep.py --out gpurun_out/sweep_N.json
   torchrun --nproc-per-node N bench/allreduce_sweep.py --op reduce_scatter   # cgx.reduce_scatter_tensor
                                                                             # vs ncclReduceScatter
-With --op reduce_scatter the message is the input of W shards; NCCL's bus bandwidth is then
-algbw * (W-1)/W, and wire_bytes_per_rank counts the packed peer chunks (phase A only).
+  torchrun --nproc-per-node N bench/allreduce_sweep.py --op all_gather       # cgx.all_gather_into_tensor
+                                                                            # vs ncclAllGather
+With --op reduce_scatter the message is the input of W shards, with --op all_gather the gathered
+output of W shards; NCCL's bus bandwidth is then algbw * (W-1)/W, and wire_bytes_per_rank counts
+the packed chunks this rank sends.
 
 Reported per row:
   time_us        median device time of one allreduce (max over ranks)
@@ -76,7 +79,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--bucket-size", type=int, default=512)
     ap.add_argument("--sizes", default="", help="explicit comma-separated sizes in KB (overrides min/max)")
-    ap.add_argument("--op", default="allreduce", choices=["allreduce", "reduce_scatter"])
+    ap.add_argument("--op", default="allreduce", choices=["allreduce", "reduce_scatter", "all_gather"])
     ap.add_argument("--with-nccl-sra", action="store_true",
                     help="also time the reference-structure path: SRA over NCCL send/recv + separate kernels")
     args = ap.parse_args()
@@ -109,9 +112,9 @@ def main():
         s *= 4
     if args.sizes:
         sizes = [int(x) << 10 for x in args.sizes.split(",")]
-    rs = args.op == "reduce_scatter"
+    rs = args.op in ("reduce_scatter", "all_gather")  # one shard per rank: the message is W shards
     bus = (world - 1) / world if rs else 2 * (world - 1) / world
-    if rs:
+    if args.op == "reduce_scatter":
         sizes = [s for s in sizes if s // es >= world]
         outs = {}
 
@@ -123,6 +126,21 @@ def main():
 
         def cgx_op(x, bits):
             cgx.reduce_scatter_tensor(out_for(x), x, bits=bits, bucket_size=args.bucket_size)
+    elif args.op == "all_gather":
+        sizes = [s for s in sizes if s // es >= world]
+        outs = {}
+
+        def out_for(x):  # x is the gathered message; rank r's input is its chunk r
+            return outs.setdefault(x.numel(), torch.empty(x.numel(), dtype=x.dtype, device=dev))
+
+        def nccl_op(x):
+            s = x.numel() // world
+            dist.all_gather_into_tensor(out_for(x), x[rank * s:(rank + 1) * s], group=nccl)
+
+        def cgx_op(x, bits):
+            s = x.numel() // world
+            cgx.all_gather_into_tensor(out_for(x), x[rank * s:(rank + 1) * s], bits=bits,
+                                       bucket_size=args.bucket_size)
     else:
         def nccl_op(x):
             dist.all_reduce(x, group=nccl)

@@ -4,7 +4,8 @@ kernels) on ONE device. With `mb` MB per virtual rank the GPU executes exactly t
 work of ONE real rank of a (W * mb) MB allreduce on W GPUs -- minus NVLink -- so it isolates the
 compute / HBM efficiency of the fused kernel at W > 1 without multi-GPU time.
 The same for the compressed reduce-scatter (rows with "op": "reduce_scatter"): `mb` MB of input
-per virtual rank, one shard of mb / W MB out.
+per virtual rank, one shard of mb / W MB out; and for the compressed all-gather (rows with
+"op": "all_gather"): one shard of mb / W MB in per virtual rank, `mb` MB out.
 Reports the slope between two sizes (harness overhead cancels)."""
 import argparse
 import json
@@ -86,6 +87,26 @@ def main():
                "times_us": {str(k): round(v, 1) for k, v in res.items()},
                "us_per_equivalent_64MB_reduce_scatter": round(slope * 64 / W, 1),
                "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-input reduce-scatter on W GPUs, "
+                       "NVLink excluded"}
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+        res = {}
+        for mb in [int(x) for x in args.mbs.split(",")]:
+            n = (mb << 20) // 4 // W * W
+            shard = [(0, n // W, bits, args.bucket)]
+            g = C.LocalSraGroup(W, lanes, n * 4 // W * 2 + (1 << 20), 20000, 4096)
+            xs = [torch.randn(n // W, device=dev) for _ in range(W)]
+            outs = [torch.empty(n, device=dev) for _ in range(W)]
+            g.all_gather(xs, outs, shard)
+            torch.cuda.synchronize()
+            g.check()
+            res[mb] = timeit(lambda: g.all_gather(xs, outs, shard))
+            del g, xs, outs
+        slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])
+        row = {"op": "all_gather", "world": W, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
+               "times_us": {str(k): round(v, 1) for k, v in res.items()},
+               "us_per_equivalent_64MB_all_gather": round(slope * 64 / W, 1),
+               "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-output all-gather on W GPUs, "
                        "NVLink excluded"}
         rows.append(row)
         print(json.dumps(row), flush=True)

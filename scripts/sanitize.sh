@@ -16,3 +16,7 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # interleaved reduce-scatter / allreduce / one-shot calls on one heap
 RS_SUBSET='(edge_inputs and (w2-float32-q1- or w3-float16-q2- or w5-bfloat16-q3-)) or many_windows or interleaved'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_reduce_scatter_gpu.py -m gpu -x -q -k "$RS_SUBSET"
+# compressed all-gather: edge inputs at W 2/3/5 (separate and in-place inputs, unaligned views), several windows,
+# and interleaved all-gather / reduce-scatter / allreduce / one-shot calls on one heap
+AG_SUBSET='(edge_inputs and (w2-float32-q1- or w3-float16-q2- or w5-bfloat16-q3-)) or many_windows or interleaved'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_all_gather_gpu.py -m gpu -x -q -k "$AG_SUBSET"

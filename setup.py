@@ -34,6 +34,9 @@ SOURCES = [
     "kernels/rs_f32.cu",
     "kernels/rs_f16.cu",
     "kernels/rs_bf16.cu",
+    "kernels/ag_f32.cu",
+    "kernels/ag_f16.cu",
+    "kernels/ag_bf16.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
     "pg/process_group_cgx.cc",

@@ -27,8 +27,14 @@ from .backend import (  # noqa: E402
     set_quantization_bits,
     set_quantization_bucket_size,
 )
-from .parallel.functional import all_reduce, compression, reduce_scatter_tensor  # noqa: E402
-from .parallel.fsdp import CGXReduceScatter, set_cgx_reduce_scatter  # noqa: E402
+from .parallel.functional import all_gather_into_tensor, all_reduce, compression, reduce_scatter_tensor  # noqa: E402
+from .parallel.fsdp import (  # noqa: E402
+    CGXAllGather,
+    CGXReduceScatter,
+    fsdp_shard_table,
+    set_cgx_all_gather,
+    set_cgx_reduce_scatter,
+)
 from .parallel.hooks import CGXState, cgx_hook, register_cgx_hook  # noqa: E402
 from .utils.launch import map_launcher_env  # noqa: E402
 from . import models, ops, utils  # noqa: E402,F401
@@ -37,11 +43,14 @@ register_backend()
 
 __all__ = [
     "BACKEND_NAME",
+    "CGXAllGather",
     "CGXReduceScatter",
     "CGXState",
+    "all_gather_into_tensor",
     "all_reduce",
     "cgx_hook",
     "compression",
+    "fsdp_shard_table",
     "get_backend",
     "map_launcher_env",
     "register_backend",
@@ -50,6 +59,7 @@ __all__ = [
     "register_layer",
     "reset_layers",
     "set_quantization_bits",
+    "set_cgx_all_gather",
     "set_cgx_reduce_scatter",
     "set_quantization_bucket_size",
 ]

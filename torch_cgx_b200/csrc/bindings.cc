@@ -184,6 +184,37 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
   reduce_scatter_simulate(plan, in, out, S, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
 }
 
+// All-gather oracle (ag_kernel): shard q is one quantization round trip (roundtrip_simulate) of
+// in_q placed at q * S, through copy q of the replicated table and rank q's publish stream (phase
+// 1, the SRA's requantization), so the RNG counters are the kernel's element indices. Every output
+// gets the same bytes.
+void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
+                            const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed,
+                            uint32_t seq) {
+  TORCH_CHECK(!inputs.empty() && inputs.size() == outputs.size(), "all_gather_simulate: one input and one output per rank");
+  const int W = (int)inputs.size();
+  const int dt = cgx_dtype(inputs[0]);
+  uint64_t S = 0;
+  const auto layers = replicated_shard(shard_layers, W, &S);
+  for (int r = 0; r < W; ++r) {
+    const at::Tensor &i = inputs[r], &o = outputs[r];
+    TORCH_CHECK(i.device().is_cpu() && o.device().is_cpu() && i.is_contiguous() && o.is_contiguous() &&
+                    cgx_dtype(i) == dt && cgx_dtype(o) == dt && (uint64_t)i.numel() == S &&
+                    (uint64_t)o.numel() == S * W,
+                "all_gather_simulate: CPU contiguous tensors of one dtype, inputs of S and outputs of W * S elements");
+  }
+  const size_t es = (size_t)dtype_size(dt), per_copy = shard_layers.size();
+  uint8_t* out0 = static_cast<uint8_t*>(outputs[0].data_ptr());
+  for (int q = 0; q < W; ++q) {
+    std::memcpy(out0 + (size_t)q * S * es, inputs[q].data_ptr(), S * es);
+    const std::vector<LayerSpec> copy(layers.begin() + (ptrdiff_t)(q * per_copy),
+                                      layers.begin() + (ptrdiff_t)((q + 1) * per_copy));
+    roundtrip_simulate(build_plan(copy, make_opts(1, 1, dt, false, 1 << 30)), out0, 1.0f,
+                       make_rng(stochastic, seed, seq), q, 1);
+  }
+  for (int r = 1; r < W; ++r) std::memcpy(outputs[r].data_ptr(), out0, S * W * es);
+}
+
 // quantize `t` through the plan; returns uint8 wire tensor [world, row_bytes]
 at::Tensor py_quantize(const at::Tensor& t, const std::vector<LayerTuple>& layers, int world, int lanes,
                        bool skip_incomplete, float prescale, bool stochastic, uint64_t seed, uint32_t seq,
@@ -433,6 +464,42 @@ class LocalSraGroup {
       done.block(cur);
     }
   }
+
+  // all-gather: inputs[r] holds virtual rank r's shard of S elements, outputs[r] receives W * S
+  void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
+                  const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq) {
+    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_, "need one input and one output per virtual rank");
+    const int dt = cgx_dtype(inputs[0]);
+    auto specs = to_layers(shard_layers);
+    auto cur = c10::cuda::getCurrentCUDAStream();
+    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
+    ready.record(cur);
+    bool fresh_plan = false;
+    for (int r = 0; r < world_; ++r) {
+      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
+      TORCH_CHECK(outputs[r].numel() == inputs[r].numel() * world_, "outputs must hold W x the input elements");
+      ready.block(streams_[r]);
+      const size_t before = fused_[r]->num_plans();
+      fused_[r]->prepare_reduce_scatter(specs, dt, false, streams_[r].stream());  // the same window plans
+      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
+    }
+    // one kernel per window and virtual rank: see reduce_scatter
+    TORCH_CHECK(world_ <= 8 || fused_[0]->rs_windows(specs, dt, false, 0).size() <= 1,
+                "LocalSraGroup.all_gather: more than 8 virtual ranks need the shard to fit one window "
+                "(raise slot_bytes)");
+    if (fresh_plan)
+      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    for (int r = 0; r < world_; ++r)
+      fused_[r]->all_gather(specs, dt, inputs[r].data_ptr(), outputs[r].data_ptr(), (uint64_t)inputs[r].numel(), rng,
+                            streams_[r].stream());
+    for (int r = 0; r < world_; ++r) {
+      at::cuda::CUDAEvent done(cudaEventDisableTiming);
+      done.record(streams_[r]);
+      done.block(cur);
+    }
+  }
   void check() {
     for (auto& f : fused_) f->check_status();
   }
@@ -487,6 +554,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("bucket_size") = 512, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = -1, py::arg("overlapped") = false, py::arg("layers") = std::vector<LayerTuple>{},
            py::call_guard<py::gil_scoped_release>())
+      .def("all_gather_compressed",
+           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, int bits, int bucket_size, bool stochastic,
+              int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers) {
+             return pg.all_gather_compressed(out, in, bits, bucket_size, stochastic, seed, overlapped,
+                                             to_layers(layers));
+           },
+           py::arg("output"), py::arg("input"), py::arg("bits") = 4, py::arg("bucket_size") = 512,
+           py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("overlapped") = false,
+           py::arg("layers") = std::vector<LayerTuple>{}, py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -613,6 +689,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
         py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
+  m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
+        py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0);
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
@@ -687,6 +765,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("seed") = 0, py::arg("seq") = 0)
       .def("reduce_scatter", &LocalSraGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
+      .def("all_gather", &LocalSraGroup::all_gather, py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers"),
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),

@@ -78,6 +78,7 @@ class SymmetricHeap {
   uint32_t* flags1(int peer) const { return reinterpret_cast<uint32_t*>(bases_[peer] + layout_.flags1_off); }
   uint32_t* flags2(int peer) const { return reinterpret_cast<uint32_t*>(bases_[peer] + layout_.flags2_off); }
   // multicast aliases (nullptr without NVLS)
+  uint8_t* mc_recv1() const { return mc_base_ ? mc_base_ + layout_.recv1_off : nullptr; }
   uint8_t* mc_recv2() const { return mc_base_ ? mc_base_ + layout_.recv2_off : nullptr; }
   uint8_t* mc_oneshot(int parity) const { return mc_base_ ? mc_base_ + layout_.os_off[parity & 1] : nullptr; }
   DeviceSync* sync_device() const { return reinterpret_cast<DeviceSync*>(bases_[rank_] + layout_.sync_off); }

@@ -23,7 +23,7 @@
 namespace cgx {
 
 struct EngineStats {
-  uint64_t calls = 0;            // allreduce and compressed reduce-scatter calls, together
+  uint64_t calls = 0;            // allreduce and compressed reduce-scatter / all-gather calls, together
   uint64_t kernel_launches = 0;  // fused kernel launches
   uint64_t elements = 0;
   uint64_t wire_bytes = 0;       // bytes this rank pushed over NVLink (both phases)
@@ -111,6 +111,13 @@ class AllreduceEngine {
   void reduce_scatter_cuda(const void* in, void* out, int dtype, int64_t shard_numel,
                            std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
                            bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped);
+
+  // Compressed all-gather of a CUDA buffer on `stream` (FusedSra::all_gather): `in` holds this
+  // rank's shard of S elements, `out` receives world * S, every shard (this rank's included) one
+  // quantization round trip. `shard_layers` as for reduce_scatter_cuda. Single node, P2P
+  // transport only; adds to the same counters.
+  void all_gather_cuda(const void* in, void* out, int dtype, int64_t shard_numel, std::vector<LayerSpec> shard_layers,
+                       int bits, int bucket, const RngParams& rng_in, cudaStream_t stream, bool overlapped);
 
   void check_health();
   const EngineStats& stats() const { return stats_; }

@@ -756,5 +756,58 @@ __device__ __noinline__ void raw_rs_generic(const T* src, const WarpItem it, flo
   }
 }
 
+// ======================================================================================
+// all-gather (ag_kernel publish): a raw item travels as T to every peer and the same T lands in my
+// output. The compressed kinds use *_send / bucket_quantize with their self-decoded output.
+// ======================================================================================
+// rows 0..1 of x (a full raw item after raw_full_x MODE 0) -> the 512 elements at `dst`
+template <typename T, int ROWS>
+__device__ __forceinline__ void raw_store_vec(T* __restrict__ dst, const float (&x)[ROWS][8]) {
+  T* p = dst + lane_id() * 16u;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) store8_vec<T>(p + k * 8, x[k]);
+}
+
+// raw tail, or a full raw item whose input or output is not vector aligned: element-wise.
+// `src` and `out` are disjoint or the same address (every lane reads an element before it writes it).
+template <typename T, typename DST>
+__device__ __noinline__ void raw_ag_generic(const T* src, const WarpItem it, float prescale, const DST ds, T* out) {
+  const uint32_t n = item_n(it);
+  const DST du = unicast_of(ds);
+  for (uint32_t i = lane_id(); i < n; i += 32) {
+    const T t = DT<T>::from_float(__fmul_rn(DT<T>::to_float(src[i]), prescale));
+    const uint32_t o = it.meta_off + i * (uint32_t)sizeof(T);
+    if (sizeof(T) == 4)
+      dst_st_u32(du, o, *reinterpret_cast<const uint32_t*>(&t));
+    else
+      dst_st_u16(du, o, *reinterpret_cast<const uint16_t*>(&t));
+    out[i] = t;
+  }
+}
+
+// all-gather decode of a raw item from ONE source (ss.n == 1): the record's T values unchanged, so a
+// peer's copy has the owner's bits (raw_full_x / raw_generic receive as 0 + v, which turns -0 into +0)
+template <typename T>
+__device__ __noinline__ void raw_ag_recv(const SrcSet ss, const WarpItem it, T* __restrict__ out) {
+  const uint8_t* rec = ss.base + it.meta_off;
+  if (item_kind(it) == kItemRaw && group_aligned<T>(out)) {
+    float v[2][8];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) raw_wire_load<T>(rec + (lane_id() * 2u + (uint32_t)k) * 8u * sizeof(T), v[k]);
+    raw_store_vec<T, 2>(out, v);
+    return;
+  }
+  const uint32_t n = item_n(it);
+  for (uint32_t i = lane_id(); i < n; i += 32) {
+    if (sizeof(T) == 4) {
+      const uint32_t b = ld_sys_u32(rec + i * 4u);
+      out[i] = *reinterpret_cast<const T*>(&b);
+    } else {
+      const uint16_t b = (uint16_t)ld_sys_u16(rec + i * 2u);
+      out[i] = *reinterpret_cast<const T*>(&b);
+    }
+  }
+}
+
 }  // namespace dev
 }  // namespace cgx

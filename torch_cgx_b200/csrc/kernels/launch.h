@@ -50,8 +50,11 @@ struct SraParams {
   int slice_elems;               // 512 or 1024 (plan.slice_elems)
   int oneshot;                   // 0: three-phase SRA, 1: one-shot
   int stages;                    // SRA: pieces every chunk is pipelined in (1..4, stages * world <= 32)
-  void* out;                     // reduce-scatter: output shard (T*); nullptr for the allreduce kernels
-  uint64_t out_shift;            // element of `data` that lands on out[0]: rank * shard stride
+  void* out;                     // reduce-scatter: output shard (T*); all-gather: gathered output (T*);
+                                 // nullptr for the allreduce kernels
+  uint64_t out_shift;            // reduce-scatter: element of `data` that lands on out[0];
+                                 // all-gather: element of `out` that data[0] lands on (rank * shard stride)
+  int gather;                    // with `out`: 1 = all-gather, 0 = reduce-scatter
 };
 
 constexpr int kSraThreads = 256;
@@ -61,7 +64,8 @@ enum SraStatus : uint32_t { kSraOk = 0, kSraTimeoutPhase1 = 1, kSraTimeoutPhase2
 
 // max CTAs of the fused kernel that can be co-resident on the current device
 int sra_max_resident_ctas(int dtype);
-// p.out != nullptr: reduce-scatter kernel, else p.oneshot selects one-shot / three-phase SRA
+// p.out != nullptr: all-gather (p.gather) or reduce-scatter kernel, else p.oneshot selects one-shot /
+// three-phase SRA
 cudaError_t launch_sra_fused(const SraParams& p, cudaStream_t stream);
 
 // ---- standalone item kernels (generic reducers, Python ops, tests, cross-node path) ----

@@ -3,5 +3,5 @@
 #include "sra_kernels.cuh"
 
 namespace cgx {
-cudaError_t launch_rs_bf16(const SraParams& p, cudaStream_t stream) { return launch_sra_t<__nv_bfloat16, true>(p, stream); }
+cudaError_t launch_rs_bf16(const SraParams& p, cudaStream_t stream) { return launch_sra_t<__nv_bfloat16, kOpReduceScatter>(p, stream); }
 }  // namespace cgx

@@ -3,5 +3,5 @@
 #include "sra_kernels.cuh"
 
 namespace cgx {
-cudaError_t launch_rs_f32(const SraParams& p, cudaStream_t stream) { return launch_sra_t<float, true>(p, stream); }
+cudaError_t launch_rs_f32(const SraParams& p, cudaStream_t stream) { return launch_sra_t<float, kOpReduceScatter>(p, stream); }
 }  // namespace cgx

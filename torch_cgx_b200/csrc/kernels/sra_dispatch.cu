@@ -17,6 +17,14 @@ int sra_max_resident_ctas(int dtype) {
 }
 
 cudaError_t launch_sra_fused(const SraParams& p, cudaStream_t stream) {
+  if (p.out != nullptr && p.gather) {
+    switch (p.dtype) {
+      case kF32: return launch_ag_f32(p, stream);
+      case kF16: return launch_ag_f16(p, stream);
+      case kBF16: return launch_ag_bf16(p, stream);
+      default: return cudaErrorInvalidValue;
+    }
+  }
   if (p.out != nullptr) {
     switch (p.dtype) {
       case kF32: return launch_rs_f32(p, stream);

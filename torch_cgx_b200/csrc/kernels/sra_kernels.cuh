@@ -11,6 +11,7 @@
 //   phase C  acquire each peer's reduced chunk (in order of arrival), dequantize into my buffer
 //
 // rs_kernel (reduce-scatter) is phases A and B without the requantization, the publish and phase C.
+// ag_kernel (all-gather) is the publish of phase B (of my unreduced shard) and phase C on recv1.
 //
 // The grid is G persistent *lanes* (CTAs of 8 warps, two per SM). Lane c of every rank only ever
 // talks to lane c of the other ranks through single-writer epoch flags, so there is no grid-wide
@@ -338,16 +339,20 @@ __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems&
 // every warp looks after segment g (polls the flag of its chunk for the value of its stage); the
 // items of a segment are dealt to the warps by flat index. Two items per iteration (ILP) with the
 // packed words of the NEXT two already in flight.
-template <typename T, int KB, int GPL>
-__device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems& li, uint32_t epoch, int stages) {
+// AG (the all-gather's decode): the chunks arrive in recv1 under flags1 and are decoded into p.out;
+// a timed-out wait also sets *abort_out. AG is a compile-time switch so that the allreduce's
+// instantiation is the same code as before it existed.
+template <typename T, int KB, int GPL, bool AG = false>
+__device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems& li, uint32_t epoch, int stages,
+                                            int* abort_out = nullptr) {
   const int lane = blockIdx.x;
   const int r = p.rank, W = p.world;
   const uint32_t warp = threadIdx.x >> 5, wl = threadIdx.x & 31u;
-  T* data = reinterpret_cast<T*>(p.data);
+  T* data = reinterpret_cast<T*>(AG ? p.out : p.data);
   const int my_stage = (int)wl / W, my_slot = (int)wl - my_stage * W;
   const bool mine = my_slot >= 1 && my_stage < stages;
   const uint32_t my_cnt = mine ? li.pre[wl + 1] - li.pre[wl] : 0u;
-  const uint32_t* my_flag = p.flags2[r] + (size_t)((r + my_slot) % W) * p.flag_stride + lane;
+  const uint32_t* my_flag = (AG ? p.flags1[r] : p.flags2[r]) + (size_t)((r + my_slot) % W) * p.flag_stride + lane;
   uint32_t pending = __ballot_sync(kAll, my_cnt > 0);
   uint32_t spins = 0;
   volatile unsigned long long* t0 = &const_cast<LaneItems&>(li).poll_t0[warp];
@@ -373,8 +378,9 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
         const bool aborted = *reinterpret_cast<const volatile uint32_t*>(p.abort_word) != 0;
         if (__any_sync(kAll, aborted || now - *t0 > p.timeout_ns)) {
           if (wl == (uint32_t)__ffs(pending) - 1u)
-            *p.status = (aborted ? (uint32_t)kSraAborted : (uint32_t)kSraTimeoutPhase2) |
+            *p.status = (aborted ? (uint32_t)kSraAborted : (uint32_t)(AG ? kSraTimeoutPhase1 : kSraTimeoutPhase2)) |
                         ((uint32_t)((r + my_slot) % W) << 8) | ((uint32_t)lane << 16);
+          if (AG) *abort_out = 1;
           break;
         }
       }
@@ -387,7 +393,7 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
       ready &= ready - 1;
       const int q = (r + __shfl_sync(kAll, my_slot, s)) % W;
       const uint32_t end = li.pre[s + 1];
-      const uint8_t* slot = p.recv2[r] + (size_t)q * p.slot_bytes;
+      const uint8_t* slot = (AG ? p.recv1[r] : p.recv2[r]) + (size_t)q * p.slot_bytes;
       const SrcSet ss{slot, 0u, 1, -1};
       auto fetch = [&](uint32_t i, WarpItem& it, SliceWords<GPL>& w) -> bool {
         if (i >= end) return false;
@@ -403,6 +409,8 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
           full_recv_w<T, KB, GPL, true>(w, it, blk);
         } else if (kind == kItemFull) {
           full_recv_unaligned<T, KB, GPL>(ss, it, blk);
+        } else if (AG && (kind == kItemRaw || kind == kItemRawTail)) {
+          raw_ag_recv<T>(ss, it, blk);  // the owner's T bits: a -0 must not become 0 + -0 = +0
         } else if (kind == kItemRaw && group_aligned<T>(blk)) {
           float x[2][8];
           raw_full_x<T, 2, 2>(x, blk, it, 1.0f, ss, none);
@@ -649,16 +657,99 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __
   sync_finish(p.sync, epoch, p.lanes);
 }
 
+// ===========================================================================
+// Compressed all-gather: every rank quantizes its own shard once, publishes the record into slot
+// `rank` of every peer's recv1 (one multimem.st with NVLS, W-1 peer stores otherwise) and writes
+// the self-decoded values to its own chunk of the output; then phase C decodes the peers' chunks
+// from recv1, in order of arrival. Every rank's output is the same bytes: decode(Q(in_q)) for
+// every q, the owner's chunk included.
+// The plan is the shard's layer table replicated W times at stride S (chunk c == copy c): an item
+// of my chunk at element e reads in[e - rank * S] (p.out_shift) and writes out[e].
+// Like rs_kernel it ends with a handshake on flags2: a peer's next call can only overwrite my
+// recv1 slots after every lane of this call has decoded them (docs/MEMORY_MODEL.md).
+// ===========================================================================
+template <typename T, int KB, int GPL>
+__device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& li, uint32_t epoch) {
+  const int r = p.rank, W = p.world;
+  const uint32_t warp = threadIdx.x >> 5;
+  const T* in = reinterpret_cast<const T*>(p.data);
+  T* out = reinterpret_cast<T*>(p.out);
+  const RngKey rng = phase_rng(p, epoch, 1u);  // the SRA's publish stream
+  const SrcSet no_src{nullptr, 0u, 0, -1};
+  // my own slot is skipped by the unicast stores; the multicast also lands there, and nobody reads it
+  const MultiDst ds{p.recv1, p.mc_recv1, (uint32_t)r * p.slot_bytes, W, r, nullptr};
+  const uint32_t end = li.pre[1];
+  // `in` is either disjoint from `out` or exactly its chunk r (then src == dst): every lane loads
+  // the elements it later stores itself, before it stores them
+  for (uint32_t i = li.pre[0] + warp; i < end; i += kSraWarps) {
+    const WarpItem it = lane_item(li, p, i, 0);
+    const uint32_t kind = item_kind(it);
+    const T* src = in + ((uint64_t)it.elem_off - p.out_shift);
+    T* dst = out + it.elem_off;
+    const bool al = group_aligned<T>(src) && group_aligned<T>(dst);
+    float x[GPL][8];
+    if (al && kind == kItemFull) slice_load_vec<T, GPL>(src, x);
+    if (al && kind == kItemRaw) raw_load_vec<T, GPL>(src, x);
+    if (i + kSraWarps < end)
+      slice_prefetch_l2<T, GPL>(in + ((uint64_t)lane_item(li, p, i + kSraWarps, 0).elem_off - p.out_shift));
+    if (kind == kItemFull) {
+      if (al)
+        full_send_x<T, KB, GPL, true, true>(x, it, p.prescale, rng, ds, dst);
+      else
+        full_send_unaligned<T, T, KB, GPL, true>(src, it, p.prescale, rng, ds, dst);
+    } else if (kind == kItemBucket) {
+      bucket_quantize<T, T>(src, it, p.prescale, rng, no_src, ds, dst);
+    } else if (kind == kItemRaw && al) {
+      raw_full_x<T, 0, GPL>(x, dst, it, p.prescale, no_src, ds);
+      raw_store_vec<T, GPL>(dst, x);
+    } else {
+      raw_ag_generic<T>(src, it, p.prescale, ds, dst);
+    }
+  }
+}
+
+template <typename T, int KB, int GPL>
+__global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __grid_constant__ SraParams p) {
+  __shared__ LaneItems li;
+  __shared__ int s_abort;
+  const int lane = blockIdx.x;
+  const uint32_t epoch = *reinterpret_cast<volatile uint32_t*>(&p.sync->epoch) + 1u;
+  const uint32_t flag = flag_value(epoch, 0);
+  if (threadIdx.x == 0) s_abort = 0;
+  lane_items_load(li, p, p.world, 1);
+  trace_mark(p, lane, 0, true);
+
+  ag_publish<T, KB, GPL>(p, li, epoch);
+  __syncthreads();
+  trace_mark(p, lane, 3);
+  if (threadIdx.x < 32) signal_peers(p.flags1, p.world, p.rank, p.flag_stride, lane, flag);
+  sra_phase_c<T, KB, GPL, true>(p, li, epoch, 1, &s_abort);
+  __syncthreads();
+
+  // slot handshake, as in rs_kernel: every lane, whether or not it had items
+  if (threadIdx.x < 32 && !s_abort) {
+    signal_peers(p.flags2, p.world, p.rank, p.flag_stride, lane, flag);
+    wait_peers(p.flags2[p.rank], p, lane, flag, kSraTimeoutPhase2);
+  }
+  trace_mark(p, lane, 5);
+  sync_finish(p.sync, epoch, p.lanes);
+}
+
 }  // namespace dev
 
 // ---- host side: pick the instantiation --------------------------------------------------
-// RS: the reduce-scatter kernel. It is instantiated in translation units of its own
-// (rs_{f32,f16,bf16}.cu): the out-of-line helpers of phase A are register-allocated per module,
-// and sharing them with rs_kernel would change the allreduce kernels' spill counts.
-template <typename T, int KB, int GPL, bool RS>
+// OP: kOpAllreduce (SRA / one-shot by p.oneshot), kOpReduceScatter or kOpAllGather. The reduce-
+// scatter and all-gather kernels are instantiated in translation units of their own
+// (rs_* / ag_{f32,f16,bf16}.cu): out-of-line helpers are register-allocated per module, and sharing
+// them with another kernel would change the allreduce kernels' spill counts.
+enum : int { kOpAllreduce = 0, kOpReduceScatter = 1, kOpAllGather = 2 };
+
+template <typename T, int KB, int GPL, int OP>
 cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
-  if constexpr (RS)
+  if constexpr (OP == kOpReduceScatter)
     dev::rs_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+  else if constexpr (OP == kOpAllGather)
+    dev::ag_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if (p.oneshot)
     dev::oneshot_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else
@@ -666,19 +757,19 @@ cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-template <typename T, int GPL, bool RS>
+template <typename T, int GPL, int OP>
 cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
   switch (p.uniform_bits) {
-    case 2: return launch_sra_inst<T, 2, GPL, RS>(p, stream);
-    case 4: return launch_sra_inst<T, 4, GPL, RS>(p, stream);
-    case 8: return launch_sra_inst<T, 8, GPL, RS>(p, stream);
-    default: return launch_sra_inst<T, 0, GPL, RS>(p, stream);
+    case 2: return launch_sra_inst<T, 2, GPL, OP>(p, stream);
+    case 4: return launch_sra_inst<T, 4, GPL, OP>(p, stream);
+    case 8: return launch_sra_inst<T, 8, GPL, OP>(p, stream);
+    default: return launch_sra_inst<T, 0, GPL, OP>(p, stream);
   }
 }
 
-template <typename T, bool RS = false>
+template <typename T, int OP = kOpAllreduce>
 cudaError_t launch_sra_t(const SraParams& p, cudaStream_t stream) {
-  return p.slice_elems == 1024 ? launch_sra_gpl<T, 4, RS>(p, stream) : launch_sra_gpl<T, 2, RS>(p, stream);
+  return p.slice_elems == 1024 ? launch_sra_gpl<T, 4, OP>(p, stream) : launch_sra_gpl<T, 2, OP>(p, stream);
 }
 
 template <typename T>
@@ -701,5 +792,9 @@ int sra_resident_per_sm_bf16();
 cudaError_t launch_rs_f32(const SraParams& p, cudaStream_t stream);
 cudaError_t launch_rs_f16(const SraParams& p, cudaStream_t stream);
 cudaError_t launch_rs_bf16(const SraParams& p, cudaStream_t stream);
+// defined once per dtype in ag_{f32,f16,bf16}.cu
+cudaError_t launch_ag_f32(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_ag_f16(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_ag_bf16(const SraParams& p, cudaStream_t stream);
 
 }  // namespace cgx

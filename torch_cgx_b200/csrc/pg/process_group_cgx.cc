@@ -435,6 +435,59 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::reduce_scatter_compressed(at::Te
   return work;
 }
 
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_gather_compressed(at::Tensor& out, at::Tensor& in, int bits,
+                                                                      int bucket_size, bool stochastic, int64_t seed,
+                                                                      bool overlapped,
+                                                                      const std::vector<LayerSpec>& layers) {
+  TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_gather_compressed needs CUDA tensors");
+  TORCH_CHECK(in.device() == out.device(), "cgx: all_gather_compressed: input and output on different devices");
+  const int dtype = to_cgx_dtype(in.scalar_type());
+  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
+              "cgx: all_gather_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ",
+              in.scalar_type(), " and ", out.scalar_type());
+  TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: all_gather_compressed needs contiguous tensors");
+  TORCH_CHECK(out.numel() == in.numel() * getSize(), "cgx: all_gather_compressed: the output has ", out.numel(),
+              " elements, expected world size (", getSize(), ") x input (", in.numel(), ")");
+  TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: all_gather_compressed: bits must be 1..8 or 32");
+  TORCH_CHECK(engine_->nodes() == 1, "cgx: the compressed all-gather supports a single node only");
+  TORCH_CHECK(cfg_.inner_comm == CommType::kP2P,
+              "cgx: the compressed all-gather needs the P2P transport, not CGX_INNER_COMMUNICATOR_TYPE=",
+              to_string(cfg_.inner_comm));
+  const c10::DeviceIndex dev = in.device().index();
+  ensure_cuda(dev);
+  c10::cuda::CUDAGuard g(dev);
+  auto cur = c10::cuda::getCurrentCUDAStream(dev);
+  auto work = c10::make_intrusive<WorkCGX>(getRank(), c10d::OpType::_ALLGATHER_BASE, "cgx:all_gather",
+                                           std::vector<at::Tensor>{out}, out.device(), *comm_stream_, this);
+  {
+    const std::string failed = poll_failure();
+    if (!failed.empty()) {
+      work->fail_now(std::make_exception_ptr(std::runtime_error(failed)));
+      return work;
+    }
+  }
+  RngParams rng;
+  rng.stochastic = stochastic;
+  rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
+  {
+    std::lock_guard<std::mutex> lk(mu_);
+    ++seq_;
+    work->start_event_.record(cur);
+    work->start_event_.block(*comm_stream_);
+    c10::cuda::CUDACachingAllocator::recordStream(in.storage().data_ptr(), *comm_stream_);
+    c10::cuda::CUDACachingAllocator::recordStream(out.storage().data_ptr(), *comm_stream_);
+    engine_->all_gather_cuda(in.data_ptr(), out.data_ptr(), dtype, in.numel(), layers, bits, bucket_size, rng,
+                             comm_stream_->stream(), overlapped);
+    work->finish_on_stream();
+  }
+  if (engine_->has_p2p() && c10::cuda::currentStreamCaptureStatusMayInitCtx() == c10::cuda::CaptureStatus::None) {
+    std::lock_guard<std::mutex> g2(fail_mu_);
+    inflight_.emplace_back(work);
+    if (inflight_.size() > 4096) inflight_.pop_front();
+  }
+  return work;
+}
+
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx) {
   // host tensors: queued to the worker thread in call order (reference: enqueue/runLoop,
   // ProcessGroupCGX.cc:300-339); the returned Work's future completes when the job is done, errors

@@ -186,6 +186,14 @@ class ProcessGroupCGX : public c10d::Backend {
                                                            int bucket_size, bool skip_incomplete, bool stochastic,
                                                            int64_t seed, bool overlapped,
                                                            const std::vector<LayerSpec>& layers);
+  // Compressed all-gather (all_gather_into_tensor semantics: `out` holds size() * in.numel()
+  // elements, chunk q is rank q's shard) through the fused P2P kernel. Every shard, this rank's
+  // own included, arrives as one quantization round trip, so every rank's `out` is the same.
+  // `in` may be this rank's chunk of `out`. The all-gather entry points of c10d stay with the
+  // delegate. `layers`, seed and overlapped as for reduce_scatter_compressed.
+  c10::intrusive_ptr<c10d::Work> all_gather_compressed(at::Tensor& out, at::Tensor& in, int bits, int bucket_size,
+                                                       bool stochastic, int64_t seed, bool overlapped,
+                                                       const std::vector<LayerSpec>& layers);
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

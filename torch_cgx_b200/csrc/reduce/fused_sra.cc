@@ -241,6 +241,38 @@ FusedSra::RsCounts FusedSra::reduce_scatter(const std::vector<LayerSpec>& shard_
   return n;
 }
 
+FusedSra::RsCounts FusedSra::all_gather(const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
+                                        void* out, uint64_t S, const RngParams& rng, cudaStream_t stream,
+                                        int max_lanes) {
+  RsCounts n;
+  const uint64_t table = shard_elems(shard_layers);
+  if (table != S)
+    throw std::invalid_argument("cgx all_gather: the shard layers tile [0, " + std::to_string(table) +
+                                ") but the input has " + std::to_string(S) + " elements");
+  if (S == 0) return n;
+  {
+    const uint64_t es = (uint64_t)dtype_size(dtype);
+    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), o0 = reinterpret_cast<uintptr_t>(out);
+    const bool own_chunk = i0 == o0 + (uint64_t)rank() * S * es;
+    const bool disjoint = i0 + S * es <= o0 || o0 + (uint64_t)world() * S * es <= i0;
+    if (!own_chunk && !disjoint)
+      throw std::invalid_argument("cgx all_gather: the input overlaps the output other than as its chunk " +
+                                  std::to_string(rank()));
+  }
+  // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
+  for (const auto& w : rs_windows(shard_layers, dtype, false, max_lanes)) {
+    const DevicePlan* dp = prepare(replicate(w, world(), S), dtype, false, stream, max_lanes);
+    if (dp == nullptr) throw std::runtime_error("cgx all_gather: window plan does not fit the heap slots");
+    launch(*dp, const_cast<void*>(in), 1.0f, rng, stream, false, out, (uint64_t)rank() * S, true);
+    const Plan& pl = dp->plan;
+    ++n.launches;
+    n.elements += pl.numel;
+    n.wire_bytes += pl.chunk_wire_bytes[rank()] * (uint64_t)(world() - 1);
+    n.raw_bytes += pl.chunk_elems[rank()] * (uint64_t)(world() - 1) * (uint64_t)dtype_size(dtype);
+  }
+  return n;
+}
+
 void FusedSra::run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng,
                            cudaStream_t stream) {
   launch(dp, data, prescale, rng, stream, true);
@@ -260,7 +292,7 @@ int FusedSra::pick_stages(const DevicePlan&) const {
 }
 
 void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-                      bool oneshot, void* out, uint64_t out_shift) {
+                      bool oneshot, void* out, uint64_t out_shift, bool gather) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   if (dp.plan.items.empty()) return;
   ++epoch_;
@@ -287,11 +319,13 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
     p.flags1[q] = valid ? heap_->flags1(q) : nullptr;
     p.flags2[q] = valid ? heap_->flags2(q) : nullptr;
   }
-  // the reduce-scatter kernel uses recv1 and unicast stores only
-  const bool mc = use_mc_ && dp.multicast_ok && out == nullptr;
-  p.mc_recv1 = (mc && oneshot) ? heap_->mc_oneshot(0) : nullptr;
-  p.mc_recv2 = (mc && !oneshot) ? heap_->mc_recv2() : nullptr;
-  p.mc_reduce = (mc && !oneshot && use_mc_reduce_) ? 1 : 0;
+  // the reduce-scatter kernel uses recv1 and unicast stores only; the all-gather publishes into
+  // recv1, through its multicast alias when it has one
+  const bool mc = use_mc_ && dp.multicast_ok && (out == nullptr || gather);
+  const bool ar = out == nullptr;
+  p.mc_recv1 = (mc && oneshot) ? heap_->mc_oneshot(0) : (mc && gather) ? heap_->mc_recv1() : nullptr;
+  p.mc_recv2 = (mc && ar && !oneshot) ? heap_->mc_recv2() : nullptr;
+  p.mc_reduce = (mc && ar && !oneshot && use_mc_reduce_) ? 1 : 0;
   p.status = heap_->status_device();
   p.abort_word = heap_->abort_device();
   p.timeout_ns = timeout_ns_;
@@ -313,6 +347,7 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
   p.stages = (oneshot || out != nullptr) ? 1 : pick_stages(dp);
   p.out = out;
   p.out_shift = out_shift;
+  p.gather = gather ? 1 : 0;
   cuda_check(launch_sra_fused(p, stream), "launch_sra_fused");
   ++launches_;
 }

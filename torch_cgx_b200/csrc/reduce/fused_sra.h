@@ -77,9 +77,19 @@ class FusedSra {
   // builds and uploads the plans of every window without launching anything
   void prepare_reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                               cudaStream_t stream, int max_lanes = 0);
-  // reduce_scatter_windows for this heap (cached per shard table)
+  // reduce_scatter_windows for this heap (cached per shard table); the all-gather uses the same
+  // windows, since its per-chunk wire is the reduce-scatter's
   const std::vector<std::vector<LayerSpec>>& rs_windows(const std::vector<LayerSpec>& shard_layers, int dtype,
                                                         bool skip_incomplete, int max_lanes);
+
+  // Compressed all-gather (ag_kernel). `in` holds this rank's shard of S elements, `out` W * S:
+  // out[q * S + i] = decode(Q_q(in_q[i])) for every rank q, this rank's own shard included, so
+  // every rank's `out` is the same bytes. Q follows `shard_layers` (as for reduce_scatter: one
+  // shard's table, buckets counted from each shard's start; bits 32 = copied unchanged), rounding
+  // to nearest unless rng.stochastic. `in` is disjoint from `out` or exactly its chunk rank();
+  // anything else throws std::invalid_argument. Windows as for reduce_scatter, one kernel per window.
+  RsCounts all_gather(const std::vector<LayerSpec>& shard_layers, int dtype, const void* in, void* out, uint64_t S,
+                      const RngParams& rng, cudaStream_t stream, int max_lanes = 0);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();
@@ -119,7 +129,7 @@ class FusedSra {
   const DevicePlan* prepare_impl(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                  cudaStream_t stream, int plan_world, uint32_t capacity, int max_lanes);
   void launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-              bool oneshot, void* out = nullptr, uint64_t out_shift = 0);
+              bool oneshot, void* out = nullptr, uint64_t out_shift = 0, bool gather = false);
   std::unordered_map<uint64_t, std::unique_ptr<DevicePlan>> cache_;
   std::unordered_map<uint64_t, std::vector<std::vector<LayerSpec>>> rs_windows_;
 };

@@ -330,6 +330,14 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
     return _to_tensors(outs, dtype)
 
 
+def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer]) -> torch.Tensor:
+    """Every rank's output of the compressed all-gather (deterministic rounding): the concatenation
+    over q of ``quantize_dequantize_layers(inputs[q], shard_layers)``. ``shard_layers`` is one
+    shard's table (offsets from the shard start), so buckets are counted from each shard's start;
+    the owner's shard is quantized like every other. Raw runs are the value in the dtype."""
+    return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers) for t in inputs])
+
+
 def reduce_scatter_exact_and_bound(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
                                    average: bool = False, skip_incomplete: bool = False,
                                    stochastic: bool = False) -> List[Tuple[np.ndarray, np.ndarray]]:

@@ -1,20 +1,24 @@
-"""FSDP2 (``fully_shard``) gradient reduce-scatter through the compressed kernel.
+"""FSDP2 (``fully_shard``) gradient reduce-scatter and parameter all-gather through the compressed
+kernels.
 
-FSDP2 takes a custom reduce-scatter per module (``FSDPModule.set_custom_reduce_scatter``), so no
-FSDP code is patched::
+FSDP2 takes a custom reduce-scatter and all-gather per module (``FSDPModule.set_custom_reduce_scatter``
+/ ``set_custom_all_gather``), so no FSDP code is patched::
 
     model = fully_shard(model)                       # after fully_shard on the sub-modules
     cgx.set_cgx_reduce_scatter(model, bits=8)        # every FSDPModule of the model
+    cgx.set_cgx_all_gather(model, bits=8)            # one comm per FSDPModule, per-parameter table
 """
 from __future__ import annotations
 
-from typing import Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
-from torch.distributed.fsdp._fully_shard._fsdp_api import ReduceScatter
+from torch.distributed.fsdp._fully_shard._fsdp_api import AllGather, ReduceScatter
 
-from .functional import _reduce_scatter
+from .functional import _all_gather, _reduce_scatter
+
+RAW_BITS = 32
 
 
 class CGXReduceScatter(ReduceScatter):
@@ -50,3 +54,76 @@ def set_cgx_reduce_scatter(model: torch.nn.Module, bits: int = 4, bucket_size: i
         if isinstance(m, FSDPModule):
             m.set_custom_reduce_scatter(comm)
     return comm
+
+
+Layer = Tuple[int, int, int, int]
+
+
+def fsdp_shard_table(params: Sequence[Tuple[Sequence[int], int]], bits: int = 4,
+                     bucket_size: int = 512) -> List[Layer]:
+    """The all-gather shard table of one FSDP parameter group.
+
+    ``params`` holds one ``(orig_size, padded_shard_numel)`` pair per parameter, in FSDP's
+    all-gather order. Each parameter is one layer of ``padded_shard_numel`` elements, so no bucket
+    spans two parameters; parameters of at most one dimension (biases, norm weights) travel
+    uncompressed (bits 32): they are small, and their values sit far from those of the weights."""
+    table, off = [], 0
+    for orig_size, n in params:
+        n = int(n)
+        if n == 0:
+            continue
+        table.append((off, n, RAW_BITS if len(orig_size) <= 1 else int(bits), int(bucket_size)))
+        off += n
+    return table
+
+
+class CGXAllGather(AllGather):
+    """FSDP2 all-gather comm: the parameters go through the compressed kernel, quantized to nearest
+    with the shard table ``layers`` (one shard's ``(elem_off, numel, bits, bucket_size)`` tuples;
+    None = one layer of ``bits`` / ``bucket_size``), with at most ``CGX_OVERLAP_LANES`` CTAs since
+    FSDP prefetches during compute. There is no stochastic rounding: the backward re-gather must
+    see the weights the forward saw. A ``uint8`` buffer (FSDP2's all-gather of mixed-dtype inputs)
+    goes to ``dist.all_gather_into_tensor`` unchanged."""
+
+    def __init__(self, bits: int = 4, bucket_size: int = 512, layers: Optional[Sequence[Layer]] = None,
+                 name: str = ""):
+        self.bits = int(bits)
+        self.bucket_size = int(bucket_size)
+        self.layers = None if layers is None else [tuple(int(v) for v in l) for l in layers]
+        self.name = name
+        self.numel = None if self.layers is None else sum(l[1] for l in self.layers)
+
+    def allocate(self, size: Sequence[int], *, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
+        return torch.empty(*size, dtype=dtype, device=device)
+
+    def __call__(self, output_tensor: torch.Tensor, input_tensor: torch.Tensor, group: dist.ProcessGroup,
+                 async_op: bool = False):
+        if input_tensor.dtype == torch.uint8:
+            return dist.all_gather_into_tensor(output_tensor, input_tensor, group=group, async_op=async_op)
+        if self.numel is not None and input_tensor.numel() != self.numel:
+            raise RuntimeError(
+                f"cgx all-gather of module '{self.name}': the all-gather input has {input_tensor.numel()} elements "
+                f"but its shard table covers {self.numel} (parameters changed after set_cgx_all_gather?)")
+        return _all_gather(output_tensor, input_tensor, bits=self.bits, bucket_size=self.bucket_size, group=group,
+                           async_op=async_op, stochastic=False, seed=None, layers=self.layers, overlapped=True)
+
+
+def set_cgx_all_gather(model: torch.nn.Module, bits: int = 4, bucket_size: int = 512) -> List[CGXAllGather]:
+    """Install a :class:`CGXAllGather` on every ``FSDPModule`` of ``model``, each with the
+    per-parameter shard table (:func:`fsdp_shard_table`) of that module's parameter group; returns
+    the comms. Call it after ``fully_shard`` and before the first forward."""
+    from torch.distributed.fsdp import FSDPModule
+
+    comms = []
+    for name, m in model.named_modules():
+        if not isinstance(m, FSDPModule):
+            continue
+        group = m._get_fsdp_state()._fsdp_param_group
+        if group is None:  # a module without parameters of its own
+            continue
+        table = fsdp_shard_table([(p._orig_size, p.padded_sharded_param_size.numel()) for p in group.fsdp_params],
+                                 bits, bucket_size)
+        comm = CGXAllGather(bits, bucket_size, table, name or type(m).__name__)
+        m.set_custom_all_gather(comm)
+        comms.append(comm)
+    return comms

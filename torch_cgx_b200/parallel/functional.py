@@ -12,6 +12,10 @@ The compressed reduce-scatter is asked for explicitly (``dist.reduce_scatter_ten
 ``cgx`` group keeps going to the uncompressed delegate)::
 
     cgx.reduce_scatter_tensor(shard, flat_grads, bits=4, average=True)
+
+and so is the compressed all-gather (``dist.all_gather_into_tensor`` stays uncompressed)::
+
+    cgx.all_gather_into_tensor(flat_params, shard, bits=8)
 """
 from __future__ import annotations
 
@@ -102,3 +106,38 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int =
     return _reduce_scatter(output, input, bits=bits, bucket_size=bucket_size, average=average, group=group,
                            async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
                            skip_incomplete=skip_incomplete, overlapped=False)
+
+
+def _all_gather(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, group, async_op: bool,
+                stochastic: bool, seed: Optional[int], layers: Optional[Sequence[Tuple[int, int, int, int]]],
+                overlapped: bool):
+    from .hooks import _native_backend
+
+    native = _native_backend(group if group is not None else dist.group.WORLD, input)
+    if native is None:
+        raise RuntimeError("cgx.all_gather_into_tensor needs a process group with the cgx backend")
+    work = native.all_gather_compressed(
+        output, input, int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
+        bool(overlapped), [tuple(int(v) for v in l) for l in (layers or [])])
+    if async_op:
+        return work
+    work.wait()  # the current stream waits for the kernel; the host does not
+    return None
+
+
+def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
+                           group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
+                           layers: Optional[Sequence[Tuple[int, int, int, int]]] = None):
+    """Compressed ``dist.all_gather_into_tensor`` on a ``cgx`` group.
+
+    ``output`` holds ``world * input.numel()`` elements; chunk q receives rank q's ``input``
+    quantized once (``bits``, buckets of ``bucket_size`` counted from each shard's start) and
+    decoded. The owner's own chunk is decoded from the same bytes, so every rank's ``output`` is
+    identical (at world 1 it is the quantization round trip of ``input``). ``layers`` optionally
+    gives one shard's quantization table as ``(elem_off, numel, bits, bucket_size)`` tuples
+    (bits 32: copied unchanged). Round to nearest unless ``stochastic``; ``seed=None`` uses
+    ``CGX_SEED``. ``input`` may be the rank's own chunk of ``output``. Single node, CUDA float32 /
+    float16 / bfloat16.
+    """
+    return _all_gather(output, input, bits=bits, bucket_size=bucket_size, group=group, async_op=async_op,
+                       stochastic=stochastic, seed=seed, layers=layers, overlapped=False)
