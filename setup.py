@@ -39,6 +39,7 @@ SOURCES = [
     "kernels/ag_bf16.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
+    "kernels/residual_relu.cu",
     "pg/process_group_cgx.cc",
     "bindings.cc",
 ]

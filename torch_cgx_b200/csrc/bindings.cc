@@ -516,6 +516,44 @@ class LocalSraGroup {
   std::vector<c10::cuda::CUDAStream> streams_;
 };
 
+// ---- ResNet residual join: every operand like `ref` (device, dtype, sizes, strides), all dense ----
+void check_join_operand(const at::Tensor& ref, const at::Tensor& t, const char* op, const char* name) {
+  TORCH_CHECK(t.is_cuda(), op, ": ", name, " must be a CUDA tensor, got ", t.device());
+  TORCH_CHECK(t.device() == ref.device(), op, ": ", name, " is on ", t.device(), ", the others on ", ref.device());
+  TORCH_CHECK(t.scalar_type() == ref.scalar_type(), op, ": ", name, " is ", t.scalar_type(), ", the others ",
+              ref.scalar_type());
+  TORCH_CHECK(t.sizes() == ref.sizes(), op, ": ", name, " has sizes ", t.sizes(), ", the others ", ref.sizes());
+  TORCH_CHECK(t.strides() == ref.strides(), op, ": ", name, " has strides ", t.strides(), ", the others ",
+              ref.strides());
+  TORCH_CHECK(t.is_non_overlapping_and_dense(), op, ": ", name, " must be non-overlapping and dense (strides ",
+              t.strides(), ")");
+}
+
+at::Tensor py_residual_relu_forward(const at::Tensor& a, const at::Tensor& b) {
+  check_join_operand(a, a, "residual_relu_forward", "a");
+  check_join_operand(a, b, "residual_relu_forward", "b");
+  const int dt = cgx_dtype(a);
+  c10::cuda::CUDAGuard g(a.device());
+  at::Tensor y = at::empty_like(a);  // dense input: same strides
+  cuda_check(launch_residual_relu_forward(a.data_ptr(), b.data_ptr(), y.data_ptr(), dt, (uint64_t)a.numel(),
+                                          c10::cuda::getCurrentCUDAStream()),
+             "residual_relu_forward");
+  return y;
+}
+
+at::Tensor py_residual_relu_backward(const at::Tensor& y, const at::Tensor& ga, const std::optional<at::Tensor>& gb) {
+  check_join_operand(y, y, "residual_relu_backward", "y");
+  check_join_operand(y, ga, "residual_relu_backward", "ga");
+  if (gb) check_join_operand(y, *gb, "residual_relu_backward", "gb");
+  const int dt = cgx_dtype(y);
+  c10::cuda::CUDAGuard guard(y.device());
+  at::Tensor g = at::empty_like(y);
+  cuda_check(launch_residual_relu_backward(y.data_ptr(), ga.data_ptr(), gb ? gb->data_ptr() : nullptr, g.data_ptr(),
+                                           dt, (uint64_t)y.numel(), c10::cuda::getCurrentCUDAStream()),
+             "residual_relu_backward");
+  return g;
+}
+
 c10::intrusive_ptr<c10d::Backend> create_backend(const c10::intrusive_ptr<c10d::Store>& store, int rank, int size,
                                                  const std::chrono::milliseconds& timeout,
                                                  c10::intrusive_ptr<c10d::Backend> cpu_delegate,
@@ -729,6 +767,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                "convert");
     return out;
   });
+  m.def("residual_relu_forward", &py_residual_relu_forward, py::arg("a"), py::arg("b"),
+        "y = relu(a + b), bit-identical to the eager add + relu_");
+  m.def("residual_relu_backward", &py_residual_relu_backward, py::arg("y"), py::arg("ga"), py::arg("gb") = py::none(),
+        "g = (y <= 0) ? 0 : ga + gb (ga alone when gb is None), bit-identical to the eager accumulation + "
+        "threshold_backward");
   m.def("max_resident_ctas", [](int dtype) { return sra_max_resident_ctas(dtype); }, py::arg("dtype") = 0);
 
   py::class_<FdChannel>(m, "FdChannel")

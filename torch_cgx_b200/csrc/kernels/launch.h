@@ -100,4 +100,12 @@ cudaError_t launch_add(const void* x, const void* y, void* sum, int dtype, uint6
 cudaError_t launch_convert(const void* src, int src_dtype, void* dst, int dst_dtype, uint64_t n,
                            cudaStream_t stream);
 
+// ---- ResNet residual join (residual_relu.cu): n elements of dense storage, all operands alike ----
+// y = relu(a + b)
+cudaError_t launch_residual_relu_forward(const void* a, const void* b, void* y, int dtype, uint64_t n,
+                                         cudaStream_t stream);
+// g = (y <= 0) ? 0 : ga + gb, or ga alone when gb == nullptr
+cudaError_t launch_residual_relu_backward(const void* y, const void* ga, const void* gb, void* g, int dtype,
+                                          uint64_t n, cudaStream_t stream);
+
 }  // namespace cgx

@@ -4,17 +4,29 @@ The reference trains torchvision ResNet-18 on CIFAR in its example
 (/root/reference/examples/cifar_train.py:120-141) and BASELINE.json names
 ResNet-50 as the headline DDP model; both are defined here so the framework has
 no torchvision dependency. Weights are random-init (no network access).
+
+Each block ends in the native residual join (``residual.py``) and returns the pair ``(y, alias of
+y)``; the next block feeds the first to conv1 and the second to its identity or downsample path.
+A block also accepts a plain tensor. Parameters and their order are torchvision's.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Type, Union
+from typing import List, Optional, Tuple, Type, Union
 
 import torch
 import torch.nn as nn
 
+from .residual import residual_relu
+
 
 def _conv3x3(cin: int, cout: int, stride: int = 1) -> nn.Conv2d:
     return nn.Conv2d(cin, cout, 3, stride, 1, bias=False)
+
+
+def _split(x: Union[torch.Tensor, Tuple[torch.Tensor, torch.Tensor]]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """A block's input: a tensor, or the pair (for conv1, for the identity / downsample path) that
+    the previous block returned (see ``residual.py``)."""
+    return (x, x) if isinstance(x, torch.Tensor) else x
 
 
 class BasicBlock(nn.Module):
@@ -30,10 +42,11 @@ class BasicBlock(nn.Module):
         self.downsample = downsample
 
     def forward(self, x):
-        idt = x if self.downsample is None else self.downsample(x)
-        out = self.relu(self.bn1(self.conv1(x)))
+        xa, xb = _split(x)
+        idt = xb if self.downsample is None else self.downsample(xb)
+        out = self.relu(self.bn1(self.conv1(xa)))
         out = self.bn2(self.conv2(out))
-        return self.relu(out + idt)
+        return residual_relu(out, idt)
 
 
 class Bottleneck(nn.Module):
@@ -51,11 +64,12 @@ class Bottleneck(nn.Module):
         self.downsample = downsample
 
     def forward(self, x):
-        idt = x if self.downsample is None else self.downsample(x)
-        out = self.relu(self.bn1(self.conv1(x)))
+        xa, xb = _split(x)
+        idt = xb if self.downsample is None else self.downsample(xb)
+        out = self.relu(self.bn1(self.conv1(xa)))
         out = self.relu(self.bn2(self.conv2(out)))
         out = self.bn3(self.conv3(out))
-        return self.relu(out + idt)
+        return residual_relu(out, idt)
 
 
 class ResNet(nn.Module):
@@ -102,7 +116,7 @@ class ResNet(nn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         x = self.stem(x)
-        x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        x, _ = self.layer4(self.layer3(self.layer2(self.layer1(x))))  # the alias has no consumer
         return self.fc(torch.flatten(self.pool(x), 1))
 
 
