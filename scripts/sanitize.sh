@@ -23,3 +23,7 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # ResNet residual join: 16-byte and scalar paths, tails, unaligned views, with and without gb (the
 # 103 M-element layer1 shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_residual_relu_gpu.py -m gpu -x -q -k "not layer1 and not training_step"
+# channels_last BatchNorm forward and backward: vector and one-element paths, single-block shapes, the
+# grid merge (staging, self-resetting counters) on the one-element path with a partial last slab
+# (8x100x16x16), unaligned views (the flagship shapes and the training steps are left to the normal GPU run)
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_batchnorm_gpu.py -m gpu -x -q -k "small_shapes or unaligned or rejects or fallbacks"

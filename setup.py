@@ -40,6 +40,7 @@ SOURCES = [
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
     "kernels/residual_relu.cu",
+    "kernels/batchnorm_cl.cu",
     "pg/process_group_cgx.cc",
     "bindings.cc",
 ]

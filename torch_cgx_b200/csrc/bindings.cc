@@ -12,7 +12,10 @@
 #include <pybind11/chrono.h>
 #include <torch/extension.h>
 
+#include <limits>
+#include <map>
 #include <memory>
+#include <mutex>
 #include <tuple>
 #include <vector>
 
@@ -554,6 +557,128 @@ at::Tensor py_residual_relu_backward(const at::Tensor& y, const at::Tensor& ga, 
   return g;
 }
 
+// ---- training BatchNorm on channels_last input ----
+void check_bn_param(const at::Tensor& x, const at::Tensor& t, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.device() == x.device(), "batchnorm_cl: ", name, " must be on ", x.device(),
+              ", got ", t.device());
+  TORCH_CHECK(t.scalar_type() == at::kFloat, "batchnorm_cl: ", name, " must be float32, got ", t.scalar_type());
+  TORCH_CHECK(t.dim() == 1 && t.size(0) == x.size(1) && t.is_contiguous(), "batchnorm_cl: ", name,
+              " must be a contiguous vector of ", x.size(1), " channels, got sizes ", t.sizes());
+}
+
+// The arrival counters of the chain kernels reset themselves, so one zeroed buffer per device and stream
+// serves every launch on that stream. Under CUDA graph capture a zeroing memset would be recorded, not
+// run, so a captured call gets its own zeroed counters, allocated (and zeroed) inside the graph.
+int* bn_semaphores(const at::Tensor& x, int need, at::Tensor& per_call) {
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, at::Tensor> cache;
+  const auto stream = c10::cuda::getCurrentCUDAStream();
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  cuda_check(cudaStreamIsCapturing(stream.stream(), &capture), "cudaStreamIsCapturing");
+  if (capture != cudaStreamCaptureStatusNone) {
+    per_call = at::zeros({need}, x.options().dtype(at::kInt));
+    return per_call.data_ptr<int>();
+  }
+  std::lock_guard<std::mutex> lock(mu);
+  at::Tensor& t = cache[{(int)x.get_device(), stream.stream()}];
+  if (!t.defined() || t.numel() < need) t = at::zeros({need}, x.options().dtype(at::kInt));
+  return t.data_ptr<int>();
+}
+
+void check_bn_input(const at::Tensor& x, const char* op, const char* name) {
+  TORCH_CHECK(x.is_cuda(), op, ": ", name, " must be a CUDA tensor, got ", x.device());
+  TORCH_CHECK(x.dim() == 4, op, ": ", name, " must be 4-D, got sizes ", x.sizes());
+  TORCH_CHECK(x.is_contiguous(at::MemoryFormat::ChannelsLast), op, ": ", name,
+              " must be channels_last, got strides ", x.strides());
+  TORCH_CHECK(x.numel() > 0 && x.numel() <= std::numeric_limits<int32_t>::max(), op, ": ", name,
+              " must have 1 to 2^31 - 1 elements, got ", x.numel());
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor> py_batchnorm_cl_backward(const at::Tensor& g, const at::Tensor& x,
+                                                                        const at::Tensor& weight,
+                                                                        const at::Tensor& bias,
+                                                                        const at::Tensor& mean,
+                                                                        const at::Tensor& invstd, bool relu) {
+  check_bn_input(x, "batchnorm_cl_backward", "x");
+  check_join_operand(x, g, "batchnorm_cl_backward", "g");
+  check_bn_param(x, weight, "weight");
+  check_bn_param(x, bias, "bias");
+  check_bn_param(x, mean, "mean");
+  check_bn_param(x, invstd, "invstd");
+  c10::cuda::CUDAGuard guard(x.device());
+  BnBackwardArgs a{};
+  a.dtype = cgx_dtype(x);
+  a.C = (int)x.size(1);
+  a.M = (int)(x.numel() / a.C);
+  const auto fopt = x.options().dtype(at::kFloat);
+  at::Tensor gx = at::empty_like(x);
+  at::Tensor sums = at::empty({2, a.C}, fopt);
+  at::Tensor gw = at::empty({a.C}, fopt), gb = at::empty({a.C}, fopt);
+  at::Tensor staging, sem_call;
+  const int gy = batchnorm_cl_grid_y(a.M, a.C);
+  if (gy > 1) {
+    staging = at::empty({2 * (int64_t)gy * a.C}, fopt);
+    a.staging = staging.data_ptr<float>();
+  }
+  a.sem_len = a.C / 4 + 1;
+  a.sem = bn_semaphores(x, a.sem_len, sem_call);
+  a.g = g.data_ptr();
+  a.x = x.data_ptr();
+  a.gx = gx.data_ptr();
+  a.weight = weight.data_ptr<float>();
+  a.bias = bias.data_ptr<float>();
+  a.mean = mean.data_ptr<float>();
+  a.invstd = invstd.data_ptr<float>();
+  a.sum_dy = sums.data_ptr<float>();
+  a.sum_dy_xmu = a.sum_dy + a.C;
+  a.grad_weight = gw.data_ptr<float>();
+  a.grad_bias = gb.data_ptr<float>();
+  a.relu = relu;
+  cuda_check(launch_batchnorm_cl_backward(a, c10::cuda::getCurrentCUDAStream()), "batchnorm_cl_backward");
+  return {gx, gw, gb};
+}
+
+std::tuple<at::Tensor, at::Tensor, at::Tensor> py_batchnorm_cl_forward(const at::Tensor& x, const at::Tensor& weight,
+                                                                       const at::Tensor& bias,
+                                                                       const at::Tensor& running_mean,
+                                                                       const at::Tensor& running_var, double momentum,
+                                                                       double eps, bool relu) {
+  check_bn_input(x, "batchnorm_cl_forward", "x");
+  check_bn_param(x, weight, "weight");
+  check_bn_param(x, bias, "bias");
+  check_bn_param(x, running_mean, "running_mean");
+  check_bn_param(x, running_var, "running_var");
+  c10::cuda::CUDAGuard guard(x.device());
+  BnForwardArgs a{};
+  a.dtype = cgx_dtype(x);
+  a.C = (int)x.size(1);
+  a.M = (int)(x.numel() / a.C);
+  at::Tensor y = at::empty_like(x);
+  at::Tensor mean = at::empty({a.C}, x.options().dtype(at::kFloat));
+  at::Tensor invstd = at::empty({a.C}, x.options().dtype(at::kFloat));
+  at::Tensor staging, sem_call;
+  const int gy = batchnorm_cl_grid_y(a.M, a.C);
+  if (gy > 1) {
+    staging = at::empty({3 * (int64_t)gy * a.C}, x.options().dtype(at::kFloat));
+    a.staging = staging.data_ptr<float>();
+  }
+  a.sem_len = a.C / 4 + 1;
+  a.sem = bn_semaphores(x, a.sem_len, sem_call);
+  a.x = x.data_ptr();
+  a.y = y.data_ptr();
+  a.weight = weight.data_ptr<float>();
+  a.bias = bias.data_ptr<float>();
+  a.running_mean = running_mean.data_ptr<float>();
+  a.running_var = running_var.data_ptr<float>();
+  a.save_mean = mean.data_ptr<float>();
+  a.save_invstd = invstd.data_ptr<float>();
+  a.momentum = momentum;
+  a.eps = eps;
+  a.relu = relu;
+  cuda_check(launch_batchnorm_cl_forward(a, c10::cuda::getCurrentCUDAStream()), "batchnorm_cl_forward");
+  return {y, mean, invstd};
+}
+
 c10::intrusive_ptr<c10d::Backend> create_backend(const c10::intrusive_ptr<c10d::Store>& store, int rank, int size,
                                                  const std::chrono::milliseconds& timeout,
                                                  c10::intrusive_ptr<c10d::Backend> cpu_delegate,
@@ -772,6 +897,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("residual_relu_backward", &py_residual_relu_backward, py::arg("y"), py::arg("ga"), py::arg("gb") = py::none(),
         "g = (y <= 0) ? 0 : ga + gb (ga alone when gb is None), bit-identical to the eager accumulation + "
         "threshold_backward");
+  m.def("batchnorm_cl_forward", &py_batchnorm_cl_forward, py::arg("x"), py::arg("weight"), py::arg("bias"),
+        py::arg("running_mean"), py::arg("running_var"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
+        "training BatchNorm of a channels_last x (fp32 / fp16 / bf16) with fp32 parameters: (y, save_mean, "
+        "save_invstd), running stats updated in place; y = relu_(bn(x)) with relu. Bit-identical to "
+        "aten.native_batch_norm (+ relu_)");
+  m.def("batchnorm_cl_backward", &py_batchnorm_cl_backward, py::arg("g"), py::arg("x"), py::arg("weight"),
+        py::arg("bias"), py::arg("mean"), py::arg("invstd"), py::arg("relu"),
+        "backward of batchnorm_cl_forward for g with x's strides: (grad_input, grad_weight, grad_bias), the ReLU "
+        "mask recomputed from x. Bit-identical to threshold_backward + aten.native_batch_norm_backward");
   m.def("max_resident_ctas", [](int dtype) { return sra_max_resident_ctas(dtype); }, py::arg("dtype") = 0);
 
   py::class_<FdChannel>(m, "FdChannel")

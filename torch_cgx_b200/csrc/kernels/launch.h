@@ -108,4 +108,36 @@ cudaError_t launch_residual_relu_forward(const void* a, const void* b, void* y, 
 cudaError_t launch_residual_relu_backward(const void* y, const void* ga, const void* gb, void* g, int dtype,
                                           uint64_t n, cudaStream_t stream);
 
+// ---- training BatchNorm on channels_last input (batchnorm_cl.cu), bit-identical to ATen's kernels ----
+struct BnForwardArgs {
+  const void* x;  // [M][C], dtype
+  void* y;        // like x
+  int dtype, M, C;
+  const float *weight, *bias;
+  float *running_mean, *running_var;  // updated in place
+  float *save_mean, *save_invstd;     // [C]
+  double momentum, eps;
+  bool relu;        // y = relu_(bn(x)) instead of bn(x)
+  float* staging;   // 3 * batchnorm_cl_grid_y(M, C) * C floats when that grid is > 1
+  int* sem;         // sem_len zeroed ints, left zeroed; launches that share them must be stream-ordered
+  int sem_len;      // >= C / 4 + 1
+};
+struct BnBackwardArgs {
+  const void* g;  // gradient of y, like x
+  const void* x;
+  void* gx;       // like x
+  int dtype, M, C;
+  const float *weight, *bias, *mean, *invstd;  // mean, invstd: the forward's save_mean, save_invstd
+  float *sum_dy, *sum_dy_xmu, *grad_weight, *grad_bias;  // [C]
+  bool relu;        // the forward fused the ReLU: g is masked where the forward's output is +0
+  float* staging;   // 2 * batchnorm_cl_grid_y(M, C) * C floats when that grid is > 1
+  int* sem;         // as for the forward
+  int sem_len;
+};
+int batchnorm_cl_grid_y(int M, int C);
+// statistics + running-stat update + invstd, then the transform (with the fused ReLU)
+cudaError_t launch_batchnorm_cl_forward(const BnForwardArgs& args, cudaStream_t stream);
+// reduction (sum_dy, sum_dy_xmu, grad_weight, grad_bias), then grad_input
+cudaError_t launch_batchnorm_cl_backward(const BnBackwardArgs& args, cudaStream_t stream);
+
 }  // namespace cgx

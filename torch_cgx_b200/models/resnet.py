@@ -8,6 +8,10 @@ no torchvision dependency. Weights are random-init (no network access).
 Each block ends in the native residual join (``residual.py``) and returns the pair ``(y, alias of
 y)``; the next block feeds the first to conv1 and the second to its identity or downsample path.
 A block also accepts a plain tensor. Parameters and their order are torchvision's.
+
+``forward`` runs every BatchNorm through ``batch_norm_act`` (``batchnorm.py``), with the ReLU that
+follows it fused; the modules themselves (``stem``, ``bn1``, ``relu``, ``downsample``) are unchanged
+and still compute the unfused model when called directly.
 """
 from __future__ import annotations
 
@@ -16,6 +20,7 @@ from typing import List, Optional, Tuple, Type, Union
 import torch
 import torch.nn as nn
 
+from .batchnorm import batch_norm_act
 from .residual import residual_relu
 
 
@@ -27,6 +32,11 @@ def _split(x: Union[torch.Tensor, Tuple[torch.Tensor, torch.Tensor]]) -> Tuple[t
     """A block's input: a tensor, or the pair (for conv1, for the identity / downsample path) that
     the previous block returned (see ``residual.py``)."""
     return (x, x) if isinstance(x, torch.Tensor) else x
+
+
+def _downsample(down: nn.Sequential, x: torch.Tensor) -> torch.Tensor:
+    """``down(x)`` for the (1x1 conv, BatchNorm) downsample path."""
+    return batch_norm_act(down[1], down[0](x), relu=False)
 
 
 class BasicBlock(nn.Module):
@@ -43,9 +53,9 @@ class BasicBlock(nn.Module):
 
     def forward(self, x):
         xa, xb = _split(x)
-        idt = xb if self.downsample is None else self.downsample(xb)
-        out = self.relu(self.bn1(self.conv1(xa)))
-        out = self.bn2(self.conv2(out))
+        idt = xb if self.downsample is None else _downsample(self.downsample, xb)
+        out = batch_norm_act(self.bn1, self.conv1(xa), relu=True)
+        out = batch_norm_act(self.bn2, self.conv2(out), relu=False)
         return residual_relu(out, idt)
 
 
@@ -65,10 +75,10 @@ class Bottleneck(nn.Module):
 
     def forward(self, x):
         xa, xb = _split(x)
-        idt = xb if self.downsample is None else self.downsample(xb)
-        out = self.relu(self.bn1(self.conv1(xa)))
-        out = self.relu(self.bn2(self.conv2(out)))
-        out = self.bn3(self.conv3(out))
+        idt = xb if self.downsample is None else _downsample(self.downsample, xb)
+        out = batch_norm_act(self.bn1, self.conv1(xa), relu=True)
+        out = batch_norm_act(self.bn2, self.conv2(out), relu=True)
+        out = batch_norm_act(self.bn3, self.conv3(out), relu=False)
         return residual_relu(out, idt)
 
 
@@ -115,7 +125,9 @@ class ResNet(nn.Module):
         return nn.Sequential(*blocks)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        x = self.stem(x)
+        x = batch_norm_act(self.stem[1], self.stem[0](x), relu=True)  # conv, BN + ReLU
+        for m in self.stem[3:]:  # the max-pool of the ImageNet stem
+            x = m(x)
         x, _ = self.layer4(self.layer3(self.layer2(self.layer1(x))))  # the alias has no consumer
         return self.fc(torch.flatten(self.pool(x), 1))
 
