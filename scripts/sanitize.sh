@@ -27,3 +27,6 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # grid merge (staging, self-resetting counters) on the one-element path with a partial last slab
 # (8x100x16x16), unaligned views (the flagship shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_batchnorm_gpu.py -m gpu -x -q -k "small_shapes or unaligned or rejects or fallbacks"
+# quantization-error estimator: 16-byte and scalar loads, bucket sizes 8..8192 and non-multiples of 8,
+# tails, non-finite buckets, binding errors (the DDP run is left to the normal GPU run)
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_adaptive_bits_gpu.py -m gpu -x -q -k "not ddp and not round_trip"

@@ -41,6 +41,7 @@ SOURCES = [
     "kernels/item_kernels.cu",
     "kernels/residual_relu.cu",
     "kernels/batchnorm_cl.cu",
+    "kernels/quant_error.cu",
     "pg/process_group_cgx.cc",
     "bindings.cc",
 ]

@@ -36,12 +36,14 @@ from .parallel.fsdp import (  # noqa: E402
     set_cgx_reduce_scatter,
 )
 from .parallel.hooks import CGXState, cgx_hook, register_cgx_hook  # noqa: E402
+from .parallel.adaptive import AdaptiveCGXState  # noqa: E402
 from .utils.launch import map_launcher_env  # noqa: E402
 from . import models, ops, utils  # noqa: E402,F401
 
 register_backend()
 
 __all__ = [
+    "AdaptiveCGXState",
     "BACKEND_NAME",
     "CGXAllGather",
     "CGXReduceScatter",

@@ -24,6 +24,7 @@
 #include "common/config.h"
 #include "common/layers.h"
 #include "common/plan.h"
+#include "common/quant_error.h"
 #include "common/sra_sim.h"
 #include "kernels/launch.h"
 #include "pg/comm_hook.h"
@@ -557,6 +558,72 @@ at::Tensor py_residual_relu_backward(const at::Tensor& y, const at::Tensor& ga, 
   return g;
 }
 
+// [len(layers), len(candidates)] float64: squared quantization error of every layer at every
+// candidate width (common/quant_error.h); CPU tensors run the C++ path, CUDA tensors the kernel
+at::Tensor py_quantization_error(const at::Tensor& t, const std::vector<LayerTuple>& layers,
+                                 const std::vector<int64_t>& candidates, bool stochastic, double prescale,
+                                 bool skip_incomplete) {
+  TORCH_CHECK(t.device().is_cpu() || t.is_cuda(), "quantization_error: tensor must be on the CPU or a CUDA device");
+  TORCH_CHECK(t.is_contiguous(), "quantization_error: tensor must be contiguous");
+  const int dt = cgx_dtype(t);
+  const int K = (int)candidates.size();
+  TORCH_CHECK(K >= 1 && K <= kQErrMaxCandidates, "quantization_error: need 1 to ", kQErrMaxCandidates,
+              " candidate widths, got ", K);
+  int bits[kQErrMaxCandidates];
+  for (int k = 0; k < K; ++k) {
+    TORCH_CHECK(candidates[k] >= 1 && candidates[k] <= 8, "quantization_error: candidate width ", candidates[k],
+                " is outside 1..8");
+    bits[k] = (int)candidates[k];
+  }
+  std::vector<QErrLayer> ls;
+  ls.reserve(layers.size());
+  for (const auto& l : layers) {
+    const int64_t off = std::get<0>(l), n = std::get<1>(l), bucket = std::get<3>(l);
+    TORCH_CHECK(off >= 0 && n >= 0 && off + n <= t.numel(), "quantization_error: layer (", off, ", ", n,
+                ") is outside the tensor of ", t.numel(), " elements");
+    TORCH_CHECK(bucket >= 1, "quantization_error: bucket size must be >= 1, got ", bucket);
+    // clamped like the plan clamps it (plan.cc: push_segment)
+    const uint32_t B = (uint32_t)std::min<int64_t>(bucket, kMaxBlockElems);
+    // with skip_incomplete the tail bucket travels raw: no error
+    ls.push_back({(uint64_t)off, skip_incomplete ? (uint64_t)n / B * B : (uint64_t)n, B, 0});
+  }
+  const int64_t L = (int64_t)ls.size();
+  if (t.device().is_cpu()) {
+    at::Tensor out = at::zeros({L, (int64_t)K}, at::kDouble);
+    cpu::quantization_error(t.data_ptr(), dt, ls, bits, K, stochastic, (float)prescale, out.data_ptr<double>());
+    return out;
+  }
+  c10::cuda::CUDAGuard g(t.device());
+  auto stream = c10::cuda::getCurrentCUDAStream();
+  const std::vector<uint64_t> first = qerr_first(ls);
+  const uint64_t nb = first.back();
+  TORCH_CHECK(nb < (1ull << 34), "quantization_error: too many buckets for one launch");
+  const size_t lbytes = ls.size() * sizeof(QErrLayer), fbytes = first.size() * sizeof(uint64_t);
+  // layer table and first buckets go up in one copy from pinned memory: no synchronisation with the stream
+  at::Tensor host = at::empty({(int64_t)(lbytes + fbytes)}, at::TensorOptions().dtype(at::kByte).pinned_memory(true));
+  std::memcpy(host.data_ptr<uint8_t>(), ls.data(), lbytes);
+  std::memcpy(host.data_ptr<uint8_t>() + lbytes, first.data(), fbytes);
+  at::Tensor dev = at::empty({(int64_t)(lbytes + fbytes)}, t.options().dtype(at::kByte));
+  dev.copy_(host, /*non_blocking=*/true);
+  at::Tensor partial = at::empty({(int64_t)std::max<uint64_t>(1, nb * (uint64_t)K)}, t.options().dtype(at::kFloat));
+  at::Tensor out = at::empty({L, (int64_t)K}, t.options().dtype(at::kDouble));
+  QErrArgs a;
+  a.data = t.data_ptr();
+  a.dtype = dt;
+  a.layer_table = reinterpret_cast<const QErrLayer*>(dev.data_ptr<uint8_t>());
+  a.first = reinterpret_cast<const uint64_t*>(dev.data_ptr<uint8_t>() + lbytes);
+  a.nbuckets = nb;
+  a.layers = (int)L;
+  a.bits = bits;
+  a.K = K;
+  a.prescale = (float)prescale;
+  a.stochastic = stochastic;
+  a.partial = partial.data_ptr<float>();
+  a.out = out.data_ptr<double>();
+  cuda_check(launch_quantization_error(a, stream), "quantization_error");
+  return out;
+}
+
 // ---- training BatchNorm on channels_last input ----
 void check_bn_param(const at::Tensor& x, const at::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.device() == x.device(), "batchnorm_cl: ", name, " must be on ", x.device(),
@@ -892,6 +959,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                "convert");
     return out;
   });
+  m.def("quantization_error", &py_quantization_error, py::arg("tensor"), py::arg("layers"), py::arg("candidates"),
+        py::arg("stochastic") = false, py::arg("prescale") = 1.0, py::arg("skip_incomplete") = false);
   m.def("residual_relu_forward", &py_residual_relu_forward, py::arg("a"), py::arg("b"),
         "y = relu(a + b), bit-identical to the eager add + relu_");
   m.def("residual_relu_backward", &py_residual_relu_backward, py::arg("y"), py::arg("ga"), py::arg("gb") = py::none(),

@@ -140,4 +140,22 @@ cudaError_t launch_batchnorm_cl_forward(const BnForwardArgs& args, cudaStream_t 
 // reduction (sum_dy, sum_dy_xmu, grad_weight, grad_bias), then grad_input
 cudaError_t launch_batchnorm_cl_backward(const BnBackwardArgs& args, cudaStream_t stream);
 
+// ---- quantization-error estimate of a layer table (quant_error.cu, common/quant_error.h) ----
+struct QErrLayer;
+struct QErrArgs {
+  const void* data;               // flat gradient, dtype
+  int dtype;
+  const QErrLayer* layer_table;   // [layers] device
+  const uint64_t* first;          // [layers + 1] device: first bucket of every layer (qerr_first)
+  uint64_t nbuckets;              // first[layers], also on the host
+  int layers;
+  const int* bits;           // [K] host: candidate widths, 1..8
+  int K;                     // 1..8
+  float prescale;
+  bool stochastic;
+  float* partial;            // [nbuckets * K] device scratch
+  double* out;               // [layers * K] device
+};
+cudaError_t launch_quantization_error(const QErrArgs& args, cudaStream_t stream);
+
 }  // namespace cgx

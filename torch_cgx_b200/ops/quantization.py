@@ -72,3 +72,27 @@ def wire_bytes(numel: int, bits: int, bucket_size: int, elsize: int = 4) -> int:
 
 def compression_ratio(numel: int, bits: int, bucket_size: int, elsize: int = 4) -> float:
     return numel * elsize / wire_bytes(numel, bits, bucket_size, elsize)
+
+
+def quantization_error(
+    t: torch.Tensor,
+    layers: Sequence[Layer],
+    candidates: Sequence[int] = (2, 3, 4, 5, 6, 7, 8),
+    *,
+    stochastic: bool = False,
+    prescale: float = 1.0,
+    skip_incomplete: bool = False,
+) -> torch.Tensor:
+    """Squared quantization error of every layer at every candidate width.
+
+    ``t`` is flat fp32 / fp16 / bf16 on the CPU or a CUDA device; ``layers`` are
+    ``(elem_off, numel, bits, bucket_size)`` tuples whose ``bits`` is ignored. Returns a float64
+    ``[len(layers), len(candidates)]`` tensor on ``t.device``: entry ``[l, k]`` is
+    sum_i (decode(encode(x_i)) - x_i)^2 of layer ``l`` at ``candidates[k]`` bits, with the levels of
+    the real quantizer (or, ``stochastic=True``, the expected squared error of stochastic rounding).
+    ``x_i`` is the fp32 value after ``prescale``. A bucket with NaN / Inf makes its layer's row NaN.
+    CUDA tensors run ``csrc/kernels/quant_error.cu``, CPU tensors its C++ oracle
+    (``csrc/common/quant_error.h``); both give the same bits.
+    """
+    return _C.quantization_error(t.view(-1), [tuple(int(v) for v in l) for l in layers],
+                                 [int(c) for c in candidates], stochastic, float(prescale), skip_incomplete)

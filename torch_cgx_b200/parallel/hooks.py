@@ -107,6 +107,9 @@ def _allreduce_fut(process_group, tensor: torch.Tensor, bucket_idx: int = -1) ->
 
 
 def cgx_hook(state: CGXState, bucket: dist.GradBucket) -> torch.futures.Future[torch.Tensor]:
+    per_bucket = getattr(state, "bucket_hook", None)  # AdaptiveCGXState runs its own per-bucket logic
+    if per_bucket is not None:
+        return per_bucket(bucket)
     if state.step == state.register_step:
         for layer_idx, tensor in enumerate(bucket.gradients()):
             bits = state.quantization_bits if state.should_compress_(tensor) else VALUE_NO_COMPRESS
@@ -122,15 +125,16 @@ def register_cgx_hook(ddp_model, state: CGXState):
     """Install the compressed-allreduce hook on a DistributedDataParallel model.
 
     With the ``cgx`` backend this registers the **native C++ hook** directly on DDP's reducer
-    (no Python in the per-bucket path); with any other backend it falls back to
-    ``ddp_model.register_comm_hook(state, cgx_hook)``. Returns the native state handle or None.
+    (no Python in the per-bucket path); with any other backend, and for an
+    :class:`~torch_cgx_b200.AdaptiveCGXState` (the native hook has no adaptive widths), it falls
+    back to ``ddp_model.register_comm_hook(state, cgx_hook)``. Returns the native state handle or None.
     """
     from .. import _C
 
     params = [p for p in ddp_model.parameters() if p.requires_grad]
     device = params[0].device if params else torch.device("cpu")
     native = _backend.get_backend(state.process_group, device)
-    if native is None:
+    if native is None or hasattr(state, "bucket_hook"):
         ddp_model.register_comm_hook(state, cgx_hook)
         return None
     handle = _C.register_native_hook(ddp_model.reducer, native, int(state.layer_min_size),
