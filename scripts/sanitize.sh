@@ -20,6 +20,10 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # and interleaved all-gather / reduce-scatter / allreduce / one-shot calls on one heap
 AG_SUBSET='(edge_inputs and (w2-float32-q1- or w3-float16-q2- or w5-bfloat16-q3-)) or many_windows or interleaved'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_all_gather_gpu.py -m gpu -x -q -k "$AG_SUBSET"
+# generic reducers on one GPU (quantize / accumulate / quantize_f32 / dequantize item kernels): SRA, Ring,
+# all-to-all and the compressed broadcast at W = 3 on unaligned views, and the 1024-element slice path
+RED_SUBSET='(match_host_and_reference and w3-float32-) or (width_and_slice_variants and 4-1024)'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_reducers_local_gpu.py -m gpu -x -q -k "$RED_SUBSET"
 # ResNet residual join: 16-byte and scalar paths, tails, unaligned views, with and without gb (the
 # 103 M-element layer1 shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_residual_relu_gpu.py -m gpu -x -q -k "not layer1 and not training_step"

@@ -21,6 +21,7 @@ SOURCES = [
     "common/layers.cc",
     "common/sra_sim.cc",
     "comm/fd_channel.cc",
+    "comm/loopback_communicator.cc",
     "comm/symmetric_heap.cc",
     "reduce/fused_sra.cc",
     "reduce/block_backend.cc",

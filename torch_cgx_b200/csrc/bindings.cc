@@ -6,6 +6,8 @@
 //  * LocalSraGroup: W virtual ranks of the fused kernels inside ONE process on
 //    ONE GPU (W heaps, W streams) so the full protocol is testable on a single
 //    device.
+//  * LocalReducerGroup: W virtual ranks of the generic reducers (one host thread
+//    each, loopback transport) on host memory or on ONE GPU.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -16,10 +18,13 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
+#include <thread>
 #include <tuple>
 #include <vector>
 
 #include "comm/fd_channel.h"
+#include "comm/loopback_communicator.h"
 #include "common/block_ops.h"
 #include "common/config.h"
 #include "common/layers.h"
@@ -29,6 +34,8 @@
 #include "kernels/launch.h"
 #include "pg/comm_hook.h"
 #include "pg/process_group_cgx.h"
+#include "reduce/block_backend.h"
+#include "reduce/reducers.h"
 
 namespace py = pybind11;
 using namespace cgx;
@@ -518,6 +525,158 @@ class LocalSraGroup {
   std::vector<std::unique_ptr<SymmetricHeap>> heaps_;
   std::vector<std::unique_ptr<FusedSra>> fused_;
   std::vector<c10::cuda::CUDAStream> streams_;
+};
+
+// W virtual ranks of one generic reducer (make_reducer), each with its own Reducer, BlockBackend,
+// stream and host thread, connected by the loopback transport. CPU tensors run the host backend,
+// tensors of one CUDA device the device backend: the same reducer code on both, in one process.
+class LocalReducerGroup {
+ public:
+  LocalReducerGroup(int world, const std::string& kind, int64_t timeout_ms) : hub_(world, timeout_ms) {
+    TORCH_CHECK(world >= 1 && world <= kMaxPeers, "LocalReducerGroup: world must be 1..", kMaxPeers, ", got ", world);
+    if (kind == "SRA")
+      kind_ = ReductionType::kSRA;
+    else if (kind == "RING")
+      kind_ = ReductionType::kRing;
+    else if (kind == "ALLTOALL")
+      kind_ = ReductionType::kAllToAll;
+    else
+      TORCH_CHECK(false, "LocalReducerGroup: kind must be SRA, RING or ALLTOALL, got ", kind);
+    last_sent_.assign((size_t)world, 0);
+  }
+  ~LocalReducerGroup() {
+    // the device reducers free their scratch on the device they allocated it on
+    std::optional<c10::cuda::CUDAGuard> g;
+    if (device_ >= 0) g.emplace((c10::DeviceIndex)device_);
+    cuda_.clear();
+  }
+
+  // in-place allreduce of one tensor per virtual rank; the prescale is 1/W when averaging
+  void allreduce(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
+                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
+    const auto specs = to_layers(layers);
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    const float prescale = average ? 1.0f / (float)hub_.world() : 1.0f;
+    run(tensors, [&](Reducer& red, void* data, int dt, cudaStream_t s) {
+      red.allreduce(data, dt, specs, skip_incomplete, prescale, rng, s);
+    });
+  }
+  void broadcast_compressed(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int root,
+                            bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
+    TORCH_CHECK(root >= 0 && root < hub_.world(), "LocalReducerGroup: bad root ", root);
+    const auto specs = to_layers(layers);
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    run(tensors, [&](Reducer& red, void* data, int dt, cudaStream_t s) {
+      red.broadcast_compressed(data, dt, specs, skip_incomplete, root, rng, s);
+    });
+  }
+  // bytes each rank's reducer counted as sent during the last call
+  std::vector<int64_t> bytes_sent() const { return last_sent_; }
+  void set_recording(bool on) { record_ = on; }
+  // the messages of the last call (recording on): (exchange index, src, dst, uint8 CPU tensor)
+  std::vector<std::tuple<int64_t, int, int, at::Tensor>> messages() const {
+    std::vector<std::tuple<int64_t, int, int, at::Tensor>> out;
+    for (const auto& m : hub_.messages()) {
+      at::Tensor t = at::empty({(int64_t)m.bytes.size()}, at::kByte);
+      if (!m.bytes.empty()) std::memcpy(t.data_ptr(), m.bytes.data(), m.bytes.size());
+      out.emplace_back(m.exchange, m.src, m.dst, t);
+    }
+    return out;
+  }
+
+ private:
+  struct Rank {
+    std::unique_ptr<LoopbackCommunicator> comm;
+    std::unique_ptr<BlockBackend> ops;
+    std::unique_ptr<Reducer> red;  // declared last: released first, its scratch through `ops`
+  };
+
+  std::vector<Rank>& ranks(bool cuda) {
+    std::vector<Rank>& v = cuda ? cuda_ : cpu_;
+    if (v.empty())
+      for (int r = 0; r < hub_.world(); ++r) {
+        Rank k;
+        k.comm = std::make_unique<LoopbackCommunicator>(&hub_, r, cuda);
+        k.ops = cuda ? make_cuda_block_backend() : make_cpu_block_backend();
+        k.red = make_reducer(kind_, k.comm.get(), k.ops.get());
+        v.push_back(std::move(k));
+      }
+    return v;
+  }
+
+  template <class F>
+  void run(const std::vector<at::Tensor>& tensors, F&& op) {
+    const int W = hub_.world();
+    TORCH_CHECK((int)tensors.size() == W, "LocalReducerGroup: need one tensor per virtual rank (", W, "), got ",
+                tensors.size());
+    const int dt = cgx_dtype(tensors[0]);
+    const bool cuda = tensors[0].is_cuda();
+    for (const at::Tensor& t : tensors)
+      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && t.numel() == tensors[0].numel() &&
+                      t.device() == tensors[0].device(),
+                  "LocalReducerGroup: contiguous tensors of one dtype, size and device");
+    TORCH_CHECK(cuda || tensors[0].device().is_cpu(), "LocalReducerGroup: CPU or CUDA tensors");
+    if (cuda) {
+      const int dev = tensors[0].device().index();
+      TORCH_CHECK(device_ < 0 || device_ == dev, "LocalReducerGroup: all calls use one device (", device_, ")");
+      device_ = dev;
+    }
+    c10::cuda::OptionalCUDAGuard guard;
+    if (cuda) {
+      guard.set_index((c10::DeviceIndex)device_);
+      if (streams_.empty())
+        for (int r = 0; r < W; ++r) streams_.push_back(c10::cuda::getStreamFromPool(false, (c10::DeviceIndex)device_));
+      // every virtual rank starts after the work that produced its input
+      at::cuda::CUDAEvent ready(cudaEventDisableTiming);
+      ready.record(c10::cuda::getCurrentCUDAStream());
+      for (auto& s : streams_) ready.block(s);
+    }
+    std::vector<Rank>& rk = ranks(cuda);
+    std::vector<uint64_t> before(W);
+    for (int r = 0; r < W; ++r) before[r] = rk[r].red->bytes_sent();
+    hub_.reset(record_);
+    {
+      py::gil_scoped_release nogil;
+      std::vector<std::thread> threads;
+      for (int r = 0; r < W; ++r)
+        threads.emplace_back([&, r] {
+          try {
+            c10::cuda::OptionalCUDAGuard g;
+            cudaStream_t s = nullptr;
+            if (cuda) {
+              g.set_index((c10::DeviceIndex)device_);
+              s = streams_[r].stream();
+            }
+            op(*rk[r].red, tensors[r].data_ptr(), dt, s);
+            if (cuda) cuda_check(cudaStreamSynchronize(s), "LocalReducerGroup: synchronise a virtual rank");
+          } catch (const std::exception& e) {
+            hub_.fail("rank " + std::to_string(r) + ": " + e.what());
+          } catch (...) {
+            hub_.fail("rank " + std::to_string(r) + ": unknown exception");
+          }
+          hub_.finish(r);
+        });
+      for (auto& t : threads) t.join();
+      // a rank that threw skipped its own synchronise: nothing it queued may still write the caller's
+      // tensors or the scratch once this returns
+      if (cuda)
+        for (int r = 0; r < W; ++r) {
+          const cudaError_t err = cudaStreamSynchronize(streams_[r].stream());
+          if (err != cudaSuccess)
+            hub_.fail("rank " + std::to_string(r) + ": synchronise after the call: " + cudaGetErrorString(err));
+        }
+    }
+    for (int r = 0; r < W; ++r) last_sent_[r] = (int64_t)(rk[r].red->bytes_sent() - before[r]);
+    TORCH_CHECK(!hub_.failed(), "LocalReducerGroup: ", hub_.failure());
+  }
+
+  LoopbackHub hub_;
+  ReductionType kind_ = ReductionType::kSRA;
+  bool record_ = false;
+  int device_ = -1;
+  std::vector<c10::cuda::CUDAStream> streams_;
+  std::vector<Rank> cpu_, cuda_;
+  std::vector<int64_t> last_sent_;
 };
 
 // ---- ResNet residual join: every operand like `ref` (device, dtype, sizes, strides), all dense ----
@@ -1021,6 +1180,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("status", &LocalSraGroup::status)
       .def("clear", &LocalSraGroup::clear)
       .def("lanes_used", &LocalSraGroup::lanes_used);
+  py::class_<LocalReducerGroup>(m, "LocalReducerGroup")
+      .def(py::init<int, const std::string&, int64_t>(), py::arg("world"), py::arg("kind"),
+           py::arg("timeout_ms") = 10000)
+      .def("allreduce", &LocalReducerGroup::allreduce, py::arg("tensors"), py::arg("layers"),
+           py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
+           py::arg("seed") = 0, py::arg("seq") = 0)
+      .def("broadcast_compressed", &LocalReducerGroup::broadcast_compressed, py::arg("tensors"), py::arg("layers"),
+           py::arg("root"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false, py::arg("seed") = 0,
+           py::arg("seq") = 0)
+      .def("bytes_sent", &LocalReducerGroup::bytes_sent)
+      .def("set_recording", &LocalReducerGroup::set_recording, py::arg("on"))
+      .def("messages", &LocalReducerGroup::messages);
 
   m.attr("MAX_BLOCK_ELEMS") = (int64_t)kMaxBlockElems;
   m.attr("MAX_PEERS") = (int64_t)kMaxPeers;

@@ -70,6 +70,10 @@ class CudaBackend : public BlockBackend {
     void* p = nullptr;
     cuda_check(cudaMalloc(&p, bytes ? bytes : 16), "cudaMalloc(reducer scratch)");
     cuda_check(cudaMemset(p, 0, bytes ? bytes : 16), "cudaMemset(reducer scratch)");
+    // cudaMemset returns before it has run, on the legacy default stream, which does not order the
+    // reducers' non-blocking streams: without this wait it can land after (and zero) the first kernel
+    // writes to the buffer
+    cuda_check(cudaStreamSynchronize(cudaStreamLegacy), "cudaMemset(reducer scratch): wait");
     return p;
   }
   void release(void* p) override { cudaFree(p); }

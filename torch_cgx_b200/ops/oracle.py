@@ -295,6 +295,97 @@ def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *
     return _to_tensors(outs, dtype)
 
 
+# ---- the generic reducers (reduce/reducers.cc): rank chunks of the lanes = 1 plan ------------------
+GENERIC_MIN_LANE_ELEMS = 2048  # Reducer::plan_for: one lane per rank chunk, default min_lane_elems
+
+
+def _quantized(v: np.ndarray, segs, dtype: torch.dtype) -> np.ndarray:
+    """``_contribution`` of every layer run of a whole-buffer fp32 array, buckets counted from
+    each run's start; elements outside every run are returned unchanged."""
+    out = v.copy()
+    for off, m, bits, bucket in segs:
+        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, dtype)
+    return out
+
+
+def _own_values(inputs: Sequence[torch.Tensor]) -> List[np.ndarray]:
+    return [t.detach().reshape(-1).float().cpu().numpy().copy() for t in inputs]
+
+
+def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
+                   skip_incomplete: bool = False) -> List[torch.Tensor]:
+    """Every rank's result of the compressed Ring allreduce (``RingReducer``, deterministic rounding).
+
+    Chunk c is rank c's chunk of the lanes = 1 plan. Rank r starts with acc_r = prescale*x_r in fp32.
+    At hop s = 0 .. W-2 every rank r sends Q(acc_r) restricted to chunk (r - s) mod W to rank r+1,
+    which adds the decoded values to its own accumulator in fp32. Chunk c is then complete on rank
+    (c - 1) mod W; every rank ends with Q(acc_{(c-1) mod W}) on chunk c, stored in the dtype (at
+    W = 1: Q(prescale*x)). Q is one quantization round with buckets counted from the layer start;
+    raw runs replace it by a rounding to the dtype. Elements outside every layer are kept.
+    """
+    W = len(inputs)
+    dtype = inputs[0].dtype
+    n = inputs[0].numel()
+    segs = layer_segments(layers, skip_incomplete)
+    chunk = block_owners(layers, n, W, 1, dtype, skip_incomplete, GENERIC_MIN_LANE_ELEMS)
+    acc = _scaled_inputs(inputs, _prescale(W, average))
+    with np.errstate(all="ignore"):
+        for s in range(W - 1):
+            sent = [_quantized(a, segs, dtype) for a in acc]  # every rank sends before it adds
+            for r in range(W):
+                sel = chunk == (r - s) % W
+                dst = acc[(r + 1) % W]
+                dst[sel] = dst[sel] + sent[r][sel]
+    outs = _own_values(inputs)
+    for c in range(W):
+        sel = chunk == c
+        final = _quantized(acc[(c - 1) % W], segs, dtype)
+        for o in outs:
+            o[sel] = final[sel]
+    return _to_tensors(outs, dtype)
+
+
+def alltoall_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
+                       skip_incomplete: bool = False) -> List[torch.Tensor]:
+    """Every rank's result of the debug all-to-all allreduce (``AllToAllReducer``, deterministic):
+    rank r keeps prescale*x_r unquantized and adds, in fp32 and in ascending rank order, every
+    peer's Q(prescale*x_q); the sum is stored in the dtype once. The ranks' results differ.
+    Elements outside every layer are kept."""
+    W = len(inputs)
+    dtype = inputs[0].dtype
+    segs = layer_segments(layers, skip_incomplete)
+    xs = _scaled_inputs(inputs, _prescale(W, average))
+    qs = [_quantized(x, segs, dtype) for x in xs]
+    outs = _own_values(inputs)
+    with np.errstate(all="ignore"):
+        for r in range(W):
+            acc = xs[r].copy()
+            for q in range(W):
+                if q != r:
+                    acc = acc + qs[q]
+            for off, m, _, _ in segs:
+                outs[r][off:off + m] = acc[off:off + m]
+    return _to_tensors(outs, dtype)
+
+
+def broadcast_compressed_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, root: int,
+                                   skip_incomplete: bool = False) -> List[torch.Tensor]:
+    """Every rank's result of ``Reducer::broadcast_compressed``: one quantization round of the
+    root's values (prescale 1, one chunk, buckets from the layer start; a ``skip_incomplete`` tail
+    stays raw), the root included so that all ranks agree. Elements outside every layer keep each
+    rank's own values. With one rank nothing is sent and the values are unchanged."""
+    W = len(inputs)
+    dtype = inputs[0].dtype
+    outs = _own_values(inputs)
+    if W > 1:
+        segs = layer_segments(layers, skip_incomplete)
+        q = _quantized(_own_values([inputs[root]])[0], segs, dtype)
+        for o in outs:
+            for off, m, _, _ in segs:
+                o[off:off + m] = q[off:off + m]
+    return _to_tensors(outs, dtype)
+
+
 def _shards(inputs: Sequence[torch.Tensor], r: int) -> List[torch.Tensor]:
     W = len(inputs)
     n = inputs[0].numel()
