@@ -4,6 +4,8 @@ NaN-aware; the process-group path at world 1; and, with >= 2 GPUs, the public AP
 
 Inputs and outputs are views at element offsets 1, 3 and 5 into sentinel-filled buffers: the
 elements around each view and the input itself must be unchanged afterwards."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -264,6 +266,33 @@ def _pg_world1(rank, world):
 
 def test_process_group_world1():
     spawn(_pg_world1, 1)
+
+
+def _refused_after_abort(rank, world):
+    torch.cuda.set_device(0)
+    dist.init_process_group("cgx", init_method="env://", rank=rank, world_size=world)
+    be = cgx.get_backend()
+    x = torch.randn(100_003, device="cuda")
+    dist.all_reduce(x)  # the heap is up and every path has run once
+    cgx.reduce_scatter_tensor(torch.empty_like(x), x)
+    cgx.all_gather_into_tensor(torch.empty_like(x), x)
+    torch.cuda.synchronize()
+    be.abort()
+    assert "aborted" in be.failure()
+    before = list(be.stats())
+    calls = {"all_reduce": lambda: dist.all_reduce(x),
+             "reduce_scatter_tensor": lambda: cgx.reduce_scatter_tensor(torch.empty_like(x), x),
+             "all_gather_into_tensor": lambda: cgx.all_gather_into_tensor(torch.empty_like(x), x)}
+    for name, call in calls.items():
+        with pytest.raises(RuntimeError, match="aborted"):
+            call()
+        assert list(be.stats()) == before, f"{name} launched after the abort"
+    os._exit(0)
+
+
+def test_every_collective_is_refused_after_abort():
+    # the allreduce, the reduce-scatter and the all-gather share the refusal of a failed group
+    spawn(_refused_after_abort, 1)
 
 
 # ---- several GPUs ----------------------------------------------------------------------------

@@ -157,41 +157,42 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
   oneshot_simulate(plan, bufs, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
 }
 
-// the shard table replicated W times at stride S (chunk c == copy c); S = end of the table
-std::vector<LayerSpec> replicated_shard(const std::vector<LayerTuple>& shard_layers, int world, uint64_t* shard) {
-  std::vector<LayerSpec> one = to_layers(shard_layers), out;
-  uint64_t S = 0;
-  for (const LayerSpec& l : one) S = std::max<uint64_t>(S, l.elem_off + l.numel);
-  for (int c = 0; c < world; ++c)
-    for (LayerSpec l : one) {
-      l.elem_off += (uint64_t)c * S;
-      out.push_back(l);
-    }
-  *shard = S;
-  return out;
+// Argument checks of the sharded simulators: one CPU contiguous input and output per rank, all of
+// the inputs' dtype, the full buffers of W * S elements and the shards of S. Returns S, the end of
+// the shard table.
+uint64_t check_sharded_simulate(ShardedOp op, const std::vector<at::Tensor>& inputs,
+                                const std::vector<at::Tensor>& outputs, const std::vector<LayerSpec>& shard_layers) {
+  const bool rs = op == ShardedOp::kReduceScatter;
+  TORCH_CHECK(!inputs.empty() && inputs.size() == outputs.size(), op_name(op),
+              "_simulate: one input and one output per rank");
+  const uint64_t W = inputs.size(), S = shard_elems(shard_layers);
+  const int dt = cgx_dtype(inputs[0]);
+  for (size_t r = 0; r < W; ++r) {
+    const at::Tensor &i = inputs[r], &o = outputs[r];
+    TORCH_CHECK(i.device().is_cpu() && o.device().is_cpu() && i.is_contiguous() && o.is_contiguous() &&
+                    cgx_dtype(i) == dt && cgx_dtype(o) == dt && (uint64_t)i.numel() == (rs ? S * W : S) &&
+                    (uint64_t)o.numel() == (rs ? S : S * W),
+                op_name(op), "_simulate: CPU contiguous tensors of one dtype, ",
+                rs ? "inputs of W * S and outputs of S elements" : "inputs of S and outputs of W * S elements");
+  }
+  return S;
 }
 
 void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                                 const std::vector<LayerTuple>& shard_layers, int lanes, bool average,
                                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
                                 int64_t min_lane_elems) {
-  TORCH_CHECK(!inputs.empty() && inputs.size() == outputs.size(), "reduce_scatter_simulate: one input and one output per rank");
+  const auto shard = to_layers(shard_layers);
+  const uint64_t S = check_sharded_simulate(ShardedOp::kReduceScatter, inputs, outputs, shard);
   const int W = (int)inputs.size();
   const int dt = cgx_dtype(inputs[0]);
-  uint64_t S = 0;
-  auto layers = replicated_shard(shard_layers, W, &S);
   std::vector<const void*> in;
   std::vector<void*> out;
   for (int r = 0; r < W; ++r) {
-    const at::Tensor &i = inputs[r], &o = outputs[r];
-    TORCH_CHECK(i.device().is_cpu() && o.device().is_cpu() && i.is_contiguous() && o.is_contiguous() &&
-                    cgx_dtype(i) == dt && cgx_dtype(o) == dt && (uint64_t)i.numel() == S * W &&
-                    (uint64_t)o.numel() == S,
-                "reduce_scatter_simulate: CPU contiguous tensors of one dtype, inputs of W * S and outputs of S elements");
-    in.push_back(i.data_ptr());
-    out.push_back(o.data_ptr());
+    in.push_back(inputs[r].data_ptr());
+    out.push_back(outputs[r].data_ptr());
   }
-  Plan plan = build_plan(layers, make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
+  Plan plan = build_plan(replicate(shard, W, S), make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
   reduce_scatter_simulate(plan, in, out, S, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
 }
 
@@ -202,18 +203,11 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
 void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                             const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed,
                             uint32_t seq) {
-  TORCH_CHECK(!inputs.empty() && inputs.size() == outputs.size(), "all_gather_simulate: one input and one output per rank");
+  const auto shard = to_layers(shard_layers);
+  const uint64_t S = check_sharded_simulate(ShardedOp::kAllGather, inputs, outputs, shard);
   const int W = (int)inputs.size();
   const int dt = cgx_dtype(inputs[0]);
-  uint64_t S = 0;
-  const auto layers = replicated_shard(shard_layers, W, &S);
-  for (int r = 0; r < W; ++r) {
-    const at::Tensor &i = inputs[r], &o = outputs[r];
-    TORCH_CHECK(i.device().is_cpu() && o.device().is_cpu() && i.is_contiguous() && o.is_contiguous() &&
-                    cgx_dtype(i) == dt && cgx_dtype(o) == dt && (uint64_t)i.numel() == S &&
-                    (uint64_t)o.numel() == S * W,
-                "all_gather_simulate: CPU contiguous tensors of one dtype, inputs of S and outputs of W * S elements");
-  }
+  const auto layers = replicate(shard, W, S);
   const size_t es = (size_t)dtype_size(dt), per_copy = shard_layers.size();
   uint8_t* out0 = static_cast<uint8_t*>(outputs[0].data_ptr());
   for (int q = 0; q < W; ++q) {
@@ -403,113 +397,37 @@ class LocalSraGroup {
            bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq, bool oneshot, int absent = -1) {
     TORCH_CHECK((int)tensors.size() == world_, "need one tensor per virtual rank");
     const int dt = cgx_dtype(tensors[0]);
-    auto specs = to_layers(layers);
-    auto cur = c10::cuda::getCurrentCUDAStream();
-    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
-    ready.record(cur);
+    for (const at::Tensor& t : tensors)
+      TORCH_CHECK(t.is_cuda() && t.is_contiguous() && cgx_dtype(t) == dt, "bad tensor");
+    const auto specs = to_layers(layers);
     const RngParams rng = make_rng(stochastic, seed, seq);
+    const float ps = average ? 1.0f / (float)world_ : 1.0f;
     std::vector<const DevicePlan*> plans(world_);
-    bool fresh_plan = false;
-    for (int r = 0; r < world_; ++r) {
-      TORCH_CHECK(tensors[r].is_cuda() && tensors[r].is_contiguous() && cgx_dtype(tensors[r]) == dt, "bad tensor");
-      ready.block(streams_[r]);
-      const size_t before = fused_[r]->num_plans();
-      plans[r] = oneshot ? fused_[r]->prepare_oneshot(specs, dt, skip_incomplete, streams_[r].stream())
-                         : fused_[r]->prepare(specs, dt, skip_incomplete, streams_[r].stream());
-      TORCH_CHECK(plans[r] != nullptr, "plan does not fit the heap slots (raise slot_bytes)");
-      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
-    }
-    // make sure every plan upload has landed before any virtual rank starts spinning
-    if (fresh_plan)
-      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
-    for (int r = 0; r < world_; ++r) {
-      if (r == absent) continue;
-      const float ps = average ? 1.0f / (float)world_ : 1.0f;
-      if (oneshot)
-        fused_[r]->run_oneshot(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
-      else
-        fused_[r]->run(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
-    }
-    for (int r = 0; r < world_; ++r) {
-      at::cuda::CUDAEvent done(cudaEventDisableTiming);
-      done.record(streams_[r]);
-      done.block(cur);
-    }
+    fork_join(
+        [&](int r) {
+          plans[r] = oneshot ? fused_[r]->prepare_oneshot(specs, dt, skip_incomplete, streams_[r].stream())
+                             : fused_[r]->prepare(specs, dt, skip_incomplete, streams_[r].stream());
+          TORCH_CHECK(plans[r] != nullptr, "plan does not fit the heap slots (raise slot_bytes)");
+        },
+        [&](int r) {
+          if (r == absent) return;
+          if (oneshot)
+            fused_[r]->run_oneshot(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
+          else
+            fused_[r]->run(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
+        });
   }
 
   // reduce-scatter: inputs[r] holds W * S elements of virtual rank r, outputs[r] receives shard r
   void reduce_scatter(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                       const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete,
                       bool stochastic, uint64_t seed, uint32_t seq) {
-    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_, "need one input and one output per virtual rank");
-    const int dt = cgx_dtype(inputs[0]);
-    auto specs = to_layers(shard_layers);
-    auto cur = c10::cuda::getCurrentCUDAStream();
-    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
-    ready.record(cur);
-    bool fresh_plan = false;
-    for (int r = 0; r < world_; ++r) {
-      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
-        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
-      TORCH_CHECK(inputs[r].numel() == outputs[r].numel() * world_, "inputs must hold W x the output elements");
-      ready.block(streams_[r]);
-      const size_t before = fused_[r]->num_plans();
-      fused_[r]->prepare_reduce_scatter(specs, dt, skip_incomplete, streams_[r].stream());
-      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
-    }
-    // streams r and r + 8 share a hardware queue (CUDA_DEVICE_MAX_CONNECTIONS = 8): with two kernels
-    // per virtual rank, rank r + 8's first one would wait behind rank r's second, which waits for it
-    TORCH_CHECK(world_ <= 8 || fused_[0]->rs_windows(specs, dt, skip_incomplete, 0).size() <= 1,
-                "LocalSraGroup.reduce_scatter: more than 8 virtual ranks need the shard to fit one window "
-                "(raise slot_bytes)");
-    // every plan upload lands before any virtual rank starts spinning
-    if (fresh_plan)
-      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
-    const RngParams rng = make_rng(stochastic, seed, seq);
-    for (int r = 0; r < world_; ++r)
-      fused_[r]->reduce_scatter(specs, dt, skip_incomplete, inputs[r].data_ptr(), outputs[r].data_ptr(),
-                                (uint64_t)outputs[r].numel(), average ? 1.0f / (float)world_ : 1.0f, rng, streams_[r].stream());
-    for (int r = 0; r < world_; ++r) {
-      at::cuda::CUDAEvent done(cudaEventDisableTiming);
-      done.record(streams_[r]);
-      done.block(cur);
-    }
+    sharded(ShardedOp::kReduceScatter, inputs, outputs, shard_layers, average, skip_incomplete, stochastic, seed, seq);
   }
-
   // all-gather: inputs[r] holds virtual rank r's shard of S elements, outputs[r] receives W * S
   void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                   const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq) {
-    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_, "need one input and one output per virtual rank");
-    const int dt = cgx_dtype(inputs[0]);
-    auto specs = to_layers(shard_layers);
-    auto cur = c10::cuda::getCurrentCUDAStream();
-    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
-    ready.record(cur);
-    bool fresh_plan = false;
-    for (int r = 0; r < world_; ++r) {
-      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
-        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
-      TORCH_CHECK(outputs[r].numel() == inputs[r].numel() * world_, "outputs must hold W x the input elements");
-      ready.block(streams_[r]);
-      const size_t before = fused_[r]->num_plans();
-      fused_[r]->prepare_reduce_scatter(specs, dt, false, streams_[r].stream());  // the same window plans
-      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
-    }
-    // one kernel per window and virtual rank: see reduce_scatter
-    TORCH_CHECK(world_ <= 8 || fused_[0]->rs_windows(specs, dt, false, 0).size() <= 1,
-                "LocalSraGroup.all_gather: more than 8 virtual ranks need the shard to fit one window "
-                "(raise slot_bytes)");
-    if (fresh_plan)
-      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
-    const RngParams rng = make_rng(stochastic, seed, seq);
-    for (int r = 0; r < world_; ++r)
-      fused_[r]->all_gather(specs, dt, inputs[r].data_ptr(), outputs[r].data_ptr(), (uint64_t)inputs[r].numel(), rng,
-                            streams_[r].stream());
-    for (int r = 0; r < world_; ++r) {
-      at::cuda::CUDAEvent done(cudaEventDisableTiming);
-      done.record(streams_[r]);
-      done.block(cur);
-    }
+    sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq);
   }
   void check() {
     for (auto& f : fused_) f->check_status();
@@ -521,6 +439,59 @@ class LocalSraGroup {
   }
 
  private:
+  // Every virtual rank's stream starts after the caller's current stream and runs prepare(r) (plan
+  // builds and uploads), then launch(r); the caller's stream waits for all of them.
+  template <class Prepare, class Launch>
+  void fork_join(Prepare&& prepare, Launch&& launch) {
+    auto cur = c10::cuda::getCurrentCUDAStream();
+    at::cuda::CUDAEvent ready(cudaEventDisableTiming);
+    ready.record(cur);
+    bool fresh_plan = false;
+    for (int r = 0; r < world_; ++r) {
+      ready.block(streams_[r]);
+      const size_t before = fused_[r]->num_plans();
+      prepare(r);
+      fresh_plan = fresh_plan || fused_[r]->num_plans() != before;
+    }
+    // make sure every plan upload has landed before any virtual rank starts spinning
+    if (fresh_plan)
+      for (int r = 0; r < world_; ++r) streams_[r].synchronize();
+    for (int r = 0; r < world_; ++r) launch(r);
+    for (int r = 0; r < world_; ++r) {
+      at::cuda::CUDAEvent done(cudaEventDisableTiming);
+      done.record(streams_[r]);
+      done.block(cur);
+    }
+  }
+
+  void sharded(ShardedOp op, std::vector<at::Tensor>& inputs, std::vector<at::Tensor>& outputs,
+               const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete, bool stochastic,
+               uint64_t seed, uint32_t seq) {
+    const bool rs = op == ShardedOp::kReduceScatter;
+    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_,
+                "need one input and one output per virtual rank");
+    const int dt = cgx_dtype(inputs[0]);
+    for (int r = 0; r < world_; ++r) {
+      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
+      const at::Tensor &full = rs ? inputs[r] : outputs[r], &shard = rs ? outputs[r] : inputs[r];
+      TORCH_CHECK(full.numel() == shard.numel() * world_,
+                  rs ? "inputs must hold W x the output elements" : "outputs must hold W x the input elements");
+    }
+    const auto specs = to_layers(shard_layers);
+    // streams r and r + 8 share a hardware queue (CUDA_DEVICE_MAX_CONNECTIONS = 8): with two kernels
+    // per virtual rank, rank r + 8's first one would wait behind rank r's second, which waits for it
+    TORCH_CHECK(world_ <= 8 || fused_[0]->rs_windows(specs, dt, skip_incomplete, 0).size() <= 1, "LocalSraGroup.",
+                op_name(op), ": more than 8 virtual ranks need the shard to fit one window (raise slot_bytes)");
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    const float ps = average ? 1.0f / (float)world_ : 1.0f;
+    fork_join([&](int r) { fused_[r]->prepare_sharded(specs, dt, skip_incomplete, streams_[r].stream()); },
+              [&](int r) {
+                fused_[r]->sharded(op, specs, dt, skip_incomplete, inputs[r].data_ptr(), outputs[r].data_ptr(),
+                                   (uint64_t)(rs ? outputs[r] : inputs[r]).numel(), ps, rng, streams_[r].stream());
+              });
+  }
+
   int world_;
   std::vector<std::unique_ptr<SymmetricHeap>> heaps_;
   std::vector<std::unique_ptr<FusedSra>> fused_;
@@ -936,8 +907,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, bool average, int bits, int bucket_size,
               bool skip_incomplete, bool stochastic, int64_t seed, bool overlapped,
               const std::vector<LayerTuple>& layers) {
-             return pg.reduce_scatter_compressed(out, in, average, bits, bucket_size, skip_incomplete, stochastic,
-                                                 seed, overlapped, to_layers(layers));
+             return pg.sharded_compressed(ShardedOp::kReduceScatter, out, in, average, bits, bucket_size,
+                                          skip_incomplete, stochastic, seed, overlapped, to_layers(layers));
            },
            py::arg("output"), py::arg("input"), py::arg("average") = false, py::arg("bits") = 4,
            py::arg("bucket_size") = 512, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
@@ -946,8 +917,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("all_gather_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, int bits, int bucket_size, bool stochastic,
               int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers) {
-             return pg.all_gather_compressed(out, in, bits, bucket_size, stochastic, seed, overlapped,
-                                             to_layers(layers));
+             return pg.sharded_compressed(ShardedOp::kAllGather, out, in, false, bits, bucket_size, false,
+                                          stochastic, seed, overlapped, to_layers(layers));
            },
            py::arg("output"), py::arg("input"), py::arg("bits") = 4, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("overlapped") = false,

@@ -187,17 +187,19 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
                         overlapped);
 }
 
-void AllreduceEngine::reduce_scatter_cuda(const void* in, void* out, int dtype, int64_t shard_numel,
-                                          std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
-                                          bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream,
-                                          bool overlapped) {
-  if (nodes() > 1) throw std::runtime_error("cgx: the compressed reduce-scatter supports a single node only");
+void AllreduceEngine::sharded_cuda(ShardedOp op, const void* in, void* out, int dtype, int64_t shard_numel,
+                                   std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
+                                   bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream,
+                                   bool overlapped) {
+  if (nodes() > 1)
+    throw std::runtime_error(std::string("cgx: the compressed ") + op_title(op) + " supports a single node only");
   if (!fused_ || cfg_.inner_comm != CommType::kP2P)
-    throw std::runtime_error("cgx: the compressed reduce-scatter needs the P2P transport "
-                             "(CGX_INNER_COMMUNICATOR_TYPE=P2P)");
+    throw std::runtime_error(std::string("cgx: the compressed ") + op_title(op) +
+                             " needs the P2P transport (CGX_INNER_COMMUNICATOR_TYPE=P2P)");
   fused_->check_status();
   if (shard_numel <= 0) return;
-  NvtxRange range("cgx:reduce_scatter_cuda", (uint64_t)shard_numel);
+  NvtxRange range(op == ShardedOp::kReduceScatter ? "cgx:reduce_scatter_cuda" : "cgx:all_gather_cuda",
+                  (uint64_t)shard_numel);
   if (shard_layers.empty()) {
     LayerSpec l;
     l.elem_off = 0;
@@ -209,40 +211,10 @@ void AllreduceEngine::reduce_scatter_cuda(const void* in, void* out, int dtype, 
   ++call_seq_;
   ++stats_.calls;
   RngParams rng = rng_in;
-  rng.seq = call_seq_ << 4;  // one sequence for every window: the counters are input element indices
+  rng.seq = call_seq_ << 4;  // one sequence for every window: the counters are element indices of the full buffer
   const FusedSra::RsCounts n =
-      fused_->reduce_scatter(shard_layers, dtype, skip_incomplete, in, out, (uint64_t)shard_numel,
-                             average ? 1.0f / (float)world_ : 1.0f, rng, stream, overlapped ? cfg_.overlap_lanes : 0);
-  stats_.kernel_launches += n.launches;
-  stats_.elements += n.elements;
-  stats_.wire_bytes += n.wire_bytes;
-  stats_.raw_bytes += n.raw_bytes;
-}
-
-void AllreduceEngine::all_gather_cuda(const void* in, void* out, int dtype, int64_t shard_numel,
-                                      std::vector<LayerSpec> shard_layers, int bits, int bucket,
-                                      const RngParams& rng_in, cudaStream_t stream, bool overlapped) {
-  if (nodes() > 1) throw std::runtime_error("cgx: the compressed all-gather supports a single node only");
-  if (!fused_ || cfg_.inner_comm != CommType::kP2P)
-    throw std::runtime_error("cgx: the compressed all-gather needs the P2P transport "
-                             "(CGX_INNER_COMMUNICATOR_TYPE=P2P)");
-  fused_->check_status();
-  if (shard_numel <= 0) return;
-  NvtxRange range("cgx:all_gather_cuda", (uint64_t)shard_numel);
-  if (shard_layers.empty()) {
-    LayerSpec l;
-    l.elem_off = 0;
-    l.numel = (uint64_t)shard_numel;
-    l.bits = compression_enabled(shard_numel, bits, cfg_.min_compress_elems) ? bits : kRawBits;
-    l.bucket = (uint32_t)std::max(1, bucket);
-    shard_layers.push_back(l);
-  }
-  ++call_seq_;
-  ++stats_.calls;
-  RngParams rng = rng_in;
-  rng.seq = call_seq_ << 4;  // one sequence for every window: the counters are output element indices
-  const FusedSra::RsCounts n = fused_->all_gather(shard_layers, dtype, in, out, (uint64_t)shard_numel, rng, stream,
-                                                  overlapped ? cfg_.overlap_lanes : 0);
+      fused_->sharded(op, shard_layers, dtype, skip_incomplete, in, out, (uint64_t)shard_numel,
+                      average ? 1.0f / (float)world_ : 1.0f, rng, stream, overlapped ? cfg_.overlap_lanes : 0);
   stats_.kernel_launches += n.launches;
   stats_.elements += n.elements;
   stats_.wire_bytes += n.wire_bytes;

@@ -103,21 +103,16 @@ class AllreduceEngine {
   void allreduce_cuda_layers(void* data, int dtype, const std::vector<LayerSpec>& layers, bool average,
                              const CompressionEnv& env, cudaStream_t stream, bool overlapped = false);
 
-  // Compressed reduce-scatter of a CUDA buffer on `stream` (FusedSra::reduce_scatter): `in` holds
-  // world * S elements, `out` receives this rank's shard of S elements. An empty `shard_layers`
-  // means one layer of S elements with `bits` / `bucket`, raw unless S exceeds
-  // CGX_COMPRESSION_MINIMAL_SIZE. Single node, P2P transport only; adds to the same counters as
-  // the allreduce.
-  void reduce_scatter_cuda(const void* in, void* out, int dtype, int64_t shard_numel,
-                           std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
-                           bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped);
-
-  // Compressed all-gather of a CUDA buffer on `stream` (FusedSra::all_gather): `in` holds this
-  // rank's shard of S elements, `out` receives world * S, every shard (this rank's included) one
-  // quantization round trip. `shard_layers` as for reduce_scatter_cuda. Single node, P2P
-  // transport only; adds to the same counters.
-  void all_gather_cuda(const void* in, void* out, int dtype, int64_t shard_numel, std::vector<LayerSpec> shard_layers,
-                       int bits, int bucket, const RngParams& rng_in, cudaStream_t stream, bool overlapped);
+  // Compressed reduce-scatter or all-gather of CUDA buffers on `stream` (FusedSra::sharded) with
+  // shards of S = shard_numel elements: the reduce-scatter's `in` holds world * S elements and
+  // `out` receives this rank's shard; the all-gather's `in` is this rank's shard and `out`
+  // receives world * S, every shard (this rank's included) one quantization round trip (average
+  // and skip_incomplete false). An empty `shard_layers` means one layer of S elements with
+  // `bits` / `bucket`, raw unless S exceeds CGX_COMPRESSION_MINIMAL_SIZE. Single node, P2P
+  // transport only; adds to the same counters as the allreduce.
+  void sharded_cuda(ShardedOp op, const void* in, void* out, int dtype, int64_t shard_numel,
+                    std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket, bool skip_incomplete,
+                    const RngParams& rng_in, cudaStream_t stream, bool overlapped);
 
   void check_health();
   const EngineStats& stats() const { return stats_; }

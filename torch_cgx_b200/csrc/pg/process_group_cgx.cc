@@ -343,13 +343,15 @@ void ProcessGroupCGX::shutdown() {
   if (cpu_delegate_) cpu_delegate_->shutdown();
 }
 
-c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, bool average, int bucket_idx) {
-  const c10::DeviceIndex dev = t.device().index();
+template <class Run>
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::enqueue_cuda(c10d::OpType op, const char* title, at::Tensor& out,
+                                                             const at::Tensor* in, Run&& run) {
+  const c10::DeviceIndex dev = out.device().index();
   ensure_cuda(dev);
   c10::cuda::CUDAGuard g(dev);
   auto cur = c10::cuda::getCurrentCUDAStream(dev);
-  auto work = c10::make_intrusive<WorkCGX>(getRank(), c10d::OpType::ALLREDUCE, "cgx:all_reduce",
-                                           std::vector<at::Tensor>{t}, t.device(), *comm_stream_, this);
+  auto work = c10::make_intrusive<WorkCGX>(getRank(), op, title, std::vector<at::Tensor>{out}, out.device(),
+                                           *comm_stream_, this);
   {
     // a group that has failed (device timeout, abort) refuses new work: the error travels in the
     // Work and in its Future (DDP raises it from backward) instead of hanging on dead peers
@@ -362,13 +364,13 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, 
   {
     std::lock_guard<std::mutex> lk(mu_);
     ++seq_;
-    // order after the producer of `t` on the caller's stream
+    // order after the producer of the tensors on the caller's stream
     work->start_event_.record(cur);
     work->start_event_.block(*comm_stream_);
     // the caching allocator must not hand this memory out while the comm stream uses it
-    c10::cuda::CUDACachingAllocator::recordStream(t.storage().data_ptr(), *comm_stream_);
-    engine_->allreduce_cuda(t.data_ptr(), to_cgx_dtype(t.scalar_type()), t.numel(), average, bucket_idx,
-                            comm_stream_->stream(), /*overlapped=*/bucket_idx >= 0);
+    if (in != nullptr) c10::cuda::CUDACachingAllocator::recordStream(in->storage().data_ptr(), *comm_stream_);
+    c10::cuda::CUDACachingAllocator::recordStream(out.storage().data_ptr(), *comm_stream_);
+    run(comm_stream_->stream());
     work->finish_on_stream();
   }
   // (works created while a CUDA graph is being captured are not watched: their events belong to
@@ -381,111 +383,44 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, 
   return work;
 }
 
-c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::reduce_scatter_compressed(at::Tensor& out, at::Tensor& in,
-                                                                          bool average, int bits, int bucket_size,
-                                                                          bool skip_incomplete, bool stochastic,
-                                                                          int64_t seed, bool overlapped,
-                                                                          const std::vector<LayerSpec>& layers) {
-  TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: reduce_scatter_compressed needs CUDA tensors");
-  TORCH_CHECK(in.device() == out.device(), "cgx: reduce_scatter_compressed: input and output on different devices");
-  const int dtype = to_cgx_dtype(in.scalar_type());
-  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
-              "cgx: reduce_scatter_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ",
-              in.scalar_type(), " and ", out.scalar_type());
-  TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: reduce_scatter_compressed needs contiguous tensors");
-  TORCH_CHECK(in.numel() == out.numel() * getSize(), "cgx: reduce_scatter_compressed: the input has ", in.numel(),
-              " elements, expected world size (", getSize(), ") x output (", out.numel(), ")");
-  TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: reduce_scatter_compressed: bits must be 1..8 or 32");
-  TORCH_CHECK(engine_->nodes() == 1, "cgx: the compressed reduce-scatter supports a single node only");
-  TORCH_CHECK(cfg_.inner_comm == CommType::kP2P,
-              "cgx: the compressed reduce-scatter needs the P2P transport, not CGX_INNER_COMMUNICATOR_TYPE=",
-              to_string(cfg_.inner_comm));
-  const c10::DeviceIndex dev = in.device().index();
-  ensure_cuda(dev);
-  c10::cuda::CUDAGuard g(dev);
-  auto cur = c10::cuda::getCurrentCUDAStream(dev);
-  auto work = c10::make_intrusive<WorkCGX>(getRank(), c10d::OpType::_REDUCE_SCATTER_BASE, "cgx:reduce_scatter",
-                                           std::vector<at::Tensor>{out}, out.device(), *comm_stream_, this);
-  {
-    const std::string failed = poll_failure();
-    if (!failed.empty()) {
-      work->fail_now(std::make_exception_ptr(std::runtime_error(failed)));
-      return work;
-    }
-  }
-  RngParams rng;
-  rng.stochastic = stochastic;
-  rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
-  {
-    std::lock_guard<std::mutex> lk(mu_);
-    ++seq_;
-    work->start_event_.record(cur);
-    work->start_event_.block(*comm_stream_);
-    c10::cuda::CUDACachingAllocator::recordStream(in.storage().data_ptr(), *comm_stream_);
-    c10::cuda::CUDACachingAllocator::recordStream(out.storage().data_ptr(), *comm_stream_);
-    engine_->reduce_scatter_cuda(in.data_ptr(), out.data_ptr(), dtype, out.numel(), layers, average, bits,
-                                 bucket_size, skip_incomplete, rng, comm_stream_->stream(), overlapped);
-    work->finish_on_stream();
-  }
-  if (engine_->has_p2p() && c10::cuda::currentStreamCaptureStatusMayInitCtx() == c10::cuda::CaptureStatus::None) {
-    std::lock_guard<std::mutex> g2(fail_mu_);
-    inflight_.emplace_back(work);
-    if (inflight_.size() > 4096) inflight_.pop_front();
-  }
-  return work;
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, bool average, int bucket_idx) {
+  return enqueue_cuda(c10d::OpType::ALLREDUCE, "cgx:all_reduce", t, nullptr, [&](cudaStream_t s) {
+    engine_->allreduce_cuda(t.data_ptr(), to_cgx_dtype(t.scalar_type()), t.numel(), average, bucket_idx, s,
+                            /*overlapped=*/bucket_idx >= 0);
+  });
 }
 
-c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_gather_compressed(at::Tensor& out, at::Tensor& in, int bits,
-                                                                      int bucket_size, bool stochastic, int64_t seed,
-                                                                      bool overlapped,
-                                                                      const std::vector<LayerSpec>& layers) {
-  TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_gather_compressed needs CUDA tensors");
-  TORCH_CHECK(in.device() == out.device(), "cgx: all_gather_compressed: input and output on different devices");
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op, at::Tensor& out, at::Tensor& in,
+                                                                   bool average, int bits, int bucket_size,
+                                                                   bool skip_incomplete, bool stochastic,
+                                                                   int64_t seed, bool overlapped,
+                                                                   const std::vector<LayerSpec>& layers) {
+  const bool rs = op == ShardedOp::kReduceScatter;
+  const char* name = op_name(op);
+  TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: ", name, "_compressed needs CUDA tensors");
+  TORCH_CHECK(in.device() == out.device(), "cgx: ", name, "_compressed: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
-  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
-              "cgx: all_gather_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ",
-              in.scalar_type(), " and ", out.scalar_type());
-  TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: all_gather_compressed needs contiguous tensors");
-  TORCH_CHECK(out.numel() == in.numel() * getSize(), "cgx: all_gather_compressed: the output has ", out.numel(),
-              " elements, expected world size (", getSize(), ") x input (", in.numel(), ")");
-  TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: all_gather_compressed: bits must be 1..8 or 32");
-  TORCH_CHECK(engine_->nodes() == 1, "cgx: the compressed all-gather supports a single node only");
-  TORCH_CHECK(cfg_.inner_comm == CommType::kP2P,
-              "cgx: the compressed all-gather needs the P2P transport, not CGX_INNER_COMMUNICATOR_TYPE=",
-              to_string(cfg_.inner_comm));
-  const c10::DeviceIndex dev = in.device().index();
-  ensure_cuda(dev);
-  c10::cuda::CUDAGuard g(dev);
-  auto cur = c10::cuda::getCurrentCUDAStream(dev);
-  auto work = c10::make_intrusive<WorkCGX>(getRank(), c10d::OpType::_ALLGATHER_BASE, "cgx:all_gather",
-                                           std::vector<at::Tensor>{out}, out.device(), *comm_stream_, this);
-  {
-    const std::string failed = poll_failure();
-    if (!failed.empty()) {
-      work->fail_now(std::make_exception_ptr(std::runtime_error(failed)));
-      return work;
-    }
-  }
+  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(), "cgx: ", name,
+              "_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(), " and ",
+              out.scalar_type());
+  TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: ", name, "_compressed needs contiguous tensors");
+  const at::Tensor& full = rs ? in : out;
+  const at::Tensor& shard = rs ? out : in;
+  TORCH_CHECK(full.numel() == shard.numel() * getSize(), "cgx: ", name, "_compressed: the ", rs ? "input" : "output",
+              " has ", full.numel(), " elements, expected world size (", getSize(), ") x ", rs ? "output" : "input",
+              " (", shard.numel(), ")");
+  TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: ", name, "_compressed: bits must be 1..8 or 32");
+  TORCH_CHECK(engine_->nodes() == 1, "cgx: the compressed ", op_title(op), " supports a single node only");
+  TORCH_CHECK(cfg_.inner_comm == CommType::kP2P, "cgx: the compressed ", op_title(op),
+              " needs the P2P transport, not CGX_INNER_COMMUNICATOR_TYPE=", to_string(cfg_.inner_comm));
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
-  {
-    std::lock_guard<std::mutex> lk(mu_);
-    ++seq_;
-    work->start_event_.record(cur);
-    work->start_event_.block(*comm_stream_);
-    c10::cuda::CUDACachingAllocator::recordStream(in.storage().data_ptr(), *comm_stream_);
-    c10::cuda::CUDACachingAllocator::recordStream(out.storage().data_ptr(), *comm_stream_);
-    engine_->all_gather_cuda(in.data_ptr(), out.data_ptr(), dtype, in.numel(), layers, bits, bucket_size, rng,
-                             comm_stream_->stream(), overlapped);
-    work->finish_on_stream();
-  }
-  if (engine_->has_p2p() && c10::cuda::currentStreamCaptureStatusMayInitCtx() == c10::cuda::CaptureStatus::None) {
-    std::lock_guard<std::mutex> g2(fail_mu_);
-    inflight_.emplace_back(work);
-    if (inflight_.size() > 4096) inflight_.pop_front();
-  }
-  return work;
+  return enqueue_cuda(rs ? c10d::OpType::_REDUCE_SCATTER_BASE : c10d::OpType::_ALLGATHER_BASE,
+                      rs ? "cgx:reduce_scatter" : "cgx:all_gather", out, &in, [&](cudaStream_t s) {
+                        engine_->sharded_cuda(op, in.data_ptr(), out.data_ptr(), dtype, shard.numel(), layers,
+                                              average, bits, bucket_size, skip_incomplete, rng, s, overlapped);
+                      });
 }
 
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx) {

@@ -177,23 +177,21 @@ class ProcessGroupCGX : public c10d::Backend {
   // allreduce of one DDP bucket whose index is known (no cursor guessing);
   // average == true fuses the 1/world scale into the kernel.
   c10::intrusive_ptr<c10d::Work> allreduce_bucket(at::Tensor& tensor, int64_t bucket_idx, bool average);
-  // Compressed reduce-scatter (reduce_scatter_tensor semantics: `in` holds size() * out.numel()
-  // elements, rank r receives shard r) through the fused P2P kernel; the reduce-scatter entry points
-  // of c10d stay with the delegate. `layers`: quantization table of one shard, (elem_off, numel,
-  // bits, bucket) relative to the shard start, empty = one layer with `bits` / `bucket_size`.
-  // seed < 0: CGX_SEED. overlapped: at most CGX_OVERLAP_LANES CTAs (runs beside compute).
-  c10::intrusive_ptr<c10d::Work> reduce_scatter_compressed(at::Tensor& out, at::Tensor& in, bool average, int bits,
-                                                           int bucket_size, bool skip_incomplete, bool stochastic,
-                                                           int64_t seed, bool overlapped,
-                                                           const std::vector<LayerSpec>& layers);
-  // Compressed all-gather (all_gather_into_tensor semantics: `out` holds size() * in.numel()
-  // elements, chunk q is rank q's shard) through the fused P2P kernel. Every shard, this rank's
-  // own included, arrives as one quantization round trip, so every rank's `out` is the same.
-  // `in` may be this rank's chunk of `out`. The all-gather entry points of c10d stay with the
-  // delegate. `layers`, seed and overlapped as for reduce_scatter_compressed.
-  c10::intrusive_ptr<c10d::Work> all_gather_compressed(at::Tensor& out, at::Tensor& in, int bits, int bucket_size,
-                                                       bool stochastic, int64_t seed, bool overlapped,
-                                                       const std::vector<LayerSpec>& layers);
+  // Compressed reduce-scatter or all-gather through the fused P2P kernel; the c10d entry points of
+  // both stay with the delegate.
+  //  kReduceScatter (reduce_scatter_tensor semantics): `in` holds size() * out.numel() elements,
+  //  rank r receives shard r.
+  //  kAllGather (all_gather_into_tensor semantics): `out` holds size() * in.numel() elements,
+  //  chunk q is rank q's shard. Every shard, this rank's own included, arrives as one quantization
+  //  round trip, so every rank's `out` is the same. average and skip_incomplete are false.
+  // The shard may be this rank's chunk of the full buffer. `layers`: quantization table of one
+  // shard, (elem_off, numel, bits, bucket) relative to the shard start, empty = one layer with
+  // `bits` / `bucket_size`. seed < 0: CGX_SEED. overlapped: at most CGX_OVERLAP_LANES CTAs (runs
+  // beside compute).
+  c10::intrusive_ptr<c10d::Work> sharded_compressed(ShardedOp op, at::Tensor& out, at::Tensor& in, bool average,
+                                                    int bits, int bucket_size, bool skip_incomplete, bool stochastic,
+                                                    int64_t seed, bool overlapped,
+                                                    const std::vector<LayerSpec>& layers);
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }
@@ -218,6 +216,12 @@ class ProcessGroupCGX : public c10d::Backend {
  private:
   c10::intrusive_ptr<c10d::Backend> delegate_for(const at::Tensor& t, const char* op);
   bool eligible_for_engine(const at::Tensor& t, const c10d::ReduceOp& op) const;
+  // The Work of one collective on the comm stream: refused once the group has failed; otherwise,
+  // under mu_, ordered after the caller's stream, `in` (may be null) and `out` recorded on the comm
+  // stream, run(comm stream) enqueues the engine call; then registered with the watchdog.
+  template <class Run>
+  c10::intrusive_ptr<c10d::Work> enqueue_cuda(c10d::OpType op, const char* title, at::Tensor& out,
+                                              const at::Tensor* in, Run&& run);
   c10::intrusive_ptr<c10d::Work> engine_allreduce(at::Tensor& t, bool average, int bucket_idx);
   c10::intrusive_ptr<c10d::Work> engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx);
   void ensure_cuda(c10::DeviceIndex dev);

@@ -114,17 +114,6 @@ void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngPa
 
 namespace {
 
-// S: end of the shard table, which must tile [0, S) in order
-uint64_t shard_elems(const std::vector<LayerSpec>& layers) {
-  uint64_t end = 0;
-  for (const LayerSpec& l : layers) {
-    if (l.elem_off != end)
-      throw std::invalid_argument("cgx reduce_scatter: the shard layers must tile [0, S) in order, without gaps");
-    end += l.numel;
-  }
-  return end;
-}
-
 // split_for_fusion cuts a layer at multiples of its bucket size. A bucket above kMaxBlockElems is
 // quantized as kMaxBlockElems-element buckets counted from the layer start, while skip_incomplete
 // counts complete buckets of the requested size: such a layer is cut at multiples of both.
@@ -150,18 +139,6 @@ std::vector<std::vector<LayerSpec>> split_shard(const std::vector<LayerSpec>& la
       s.bucket = layers[k].bucket;
     }
   return groups;
-}
-
-// the window's table for the plan: W copies at stride S, copy c = chunk c
-std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& window, int world, uint64_t S) {
-  std::vector<LayerSpec> out;
-  out.reserve(window.size() * (size_t)world);
-  for (int c = 0; c < world; ++c)
-    for (LayerSpec l : window) {
-      l.elem_off += (uint64_t)c * S;
-      out.push_back(l);
-    }
-  return out;
 }
 
 }  // namespace
@@ -201,74 +178,48 @@ const std::vector<std::vector<LayerSpec>>& FusedSra::rs_windows(const std::vecto
   return rs_windows_.emplace(key, std::move(wins)).first->second;
 }
 
-void FusedSra::prepare_reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
-                                      cudaStream_t stream, int max_lanes) {
+void FusedSra::prepare_sharded(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                               cudaStream_t stream, int max_lanes) {
   const uint64_t S = shard_elems(shard_layers);
   for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes))
     prepare(replicate(w, world(), S), dtype, skip_incomplete, stream, max_lanes);
 }
 
-FusedSra::RsCounts FusedSra::reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype,
-                                            bool skip_incomplete, const void* in, void* out, uint64_t out_numel,
-                                            float prescale, const RngParams& rng, cudaStream_t stream,
-                                            int max_lanes) {
+FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype,
+                                     bool skip_incomplete, const void* in, void* out, uint64_t S, float prescale,
+                                     const RngParams& rng, cudaStream_t stream, int max_lanes) {
+  const bool rs = op == ShardedOp::kReduceScatter;
+  const char* name = op_name(op);
   RsCounts n;
-  const uint64_t S = shard_elems(shard_layers);
-  if (S != out_numel)
-    throw std::invalid_argument("cgx reduce_scatter: the shard layers tile [0, " + std::to_string(S) +
-                                ") but the output has " + std::to_string(out_numel) + " elements");
+  const uint64_t table = shard_elems(shard_layers);
+  if (table != S)
+    throw std::invalid_argument(std::string("cgx ") + name + ": the shard layers tile [0, " + std::to_string(table) +
+                                ") but the " + (rs ? "output" : "input") + " has " + std::to_string(S) + " elements");
   if (S == 0) return n;
   {
     const uint64_t es = (uint64_t)dtype_size(dtype);
-    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), o0 = reinterpret_cast<uintptr_t>(out);
-    const bool own_chunk = o0 == i0 + (uint64_t)rank() * S * es;
-    const bool disjoint = o0 + S * es <= i0 || i0 + (uint64_t)world() * S * es <= o0;
+    const uintptr_t full = reinterpret_cast<uintptr_t>(rs ? in : out);
+    const uintptr_t shard = reinterpret_cast<uintptr_t>(rs ? out : in);
+    const bool own_chunk = shard == full + (uint64_t)rank() * S * es;
+    const bool disjoint = shard + S * es <= full || full + (uint64_t)world() * S * es <= shard;
     if (!own_chunk && !disjoint)
-      throw std::invalid_argument("cgx reduce_scatter: the output overlaps the input other than as its chunk " +
-                                  std::to_string(rank()));
+      throw std::invalid_argument(std::string("cgx ") + name +
+                                  (rs ? ": the output overlaps the input" : ": the input overlaps the output") +
+                                  " other than as its chunk " + std::to_string(rank()));
   }
   // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
   for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes)) {
     const DevicePlan* dp = prepare(replicate(w, world(), S), dtype, skip_incomplete, stream, max_lanes);
-    if (dp == nullptr) throw std::runtime_error("cgx reduce_scatter: window plan does not fit the heap slots");
-    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S);
+    if (dp == nullptr)
+      throw std::runtime_error(std::string("cgx ") + name + ": window plan does not fit the heap slots");
+    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs);
     const Plan& pl = dp->plan;
+    const uint64_t mine = pl.chunk_wire_bytes[rank()], my_elems = pl.chunk_elems[rank()];
     ++n.launches;
     n.elements += pl.numel;
-    n.wire_bytes += pl.total_wire - pl.chunk_wire_bytes[rank()];
-    n.raw_bytes += (pl.numel - pl.chunk_elems[rank()]) * (uint64_t)dtype_size(dtype);
-  }
-  return n;
-}
-
-FusedSra::RsCounts FusedSra::all_gather(const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
-                                        void* out, uint64_t S, const RngParams& rng, cudaStream_t stream,
-                                        int max_lanes) {
-  RsCounts n;
-  const uint64_t table = shard_elems(shard_layers);
-  if (table != S)
-    throw std::invalid_argument("cgx all_gather: the shard layers tile [0, " + std::to_string(table) +
-                                ") but the input has " + std::to_string(S) + " elements");
-  if (S == 0) return n;
-  {
-    const uint64_t es = (uint64_t)dtype_size(dtype);
-    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), o0 = reinterpret_cast<uintptr_t>(out);
-    const bool own_chunk = i0 == o0 + (uint64_t)rank() * S * es;
-    const bool disjoint = i0 + S * es <= o0 || o0 + (uint64_t)world() * S * es <= i0;
-    if (!own_chunk && !disjoint)
-      throw std::invalid_argument("cgx all_gather: the input overlaps the output other than as its chunk " +
-                                  std::to_string(rank()));
-  }
-  // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
-  for (const auto& w : rs_windows(shard_layers, dtype, false, max_lanes)) {
-    const DevicePlan* dp = prepare(replicate(w, world(), S), dtype, false, stream, max_lanes);
-    if (dp == nullptr) throw std::runtime_error("cgx all_gather: window plan does not fit the heap slots");
-    launch(*dp, const_cast<void*>(in), 1.0f, rng, stream, false, out, (uint64_t)rank() * S, true);
-    const Plan& pl = dp->plan;
-    ++n.launches;
-    n.elements += pl.numel;
-    n.wire_bytes += pl.chunk_wire_bytes[rank()] * (uint64_t)(world() - 1);
-    n.raw_bytes += pl.chunk_elems[rank()] * (uint64_t)(world() - 1) * (uint64_t)dtype_size(dtype);
+    // the reduce-scatter pushes every chunk but its own, the all-gather its own to W - 1 peers
+    n.wire_bytes += rs ? pl.total_wire - mine : mine * (uint64_t)(world() - 1);
+    n.raw_bytes += (rs ? pl.numel - my_elems : my_elems * (uint64_t)(world() - 1)) * (uint64_t)dtype_size(dtype);
   }
   return n;
 }

@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <memory>
+#include <stdexcept>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -24,6 +25,35 @@ struct DevicePlan {
   uint32_t* d_item_first = nullptr;  // [world * lanes + 1]
   bool multicast_ok = false;         // every compressed item has a width multimem.st can carry (2/4/8)
 };
+
+// The two sharded collectives. Both move S-element shards through one table and the same windows;
+// the reduce-scatter reads W * S elements and writes the shard, the all-gather the other way round.
+enum class ShardedOp { kReduceScatter, kAllGather };
+inline const char* op_name(ShardedOp op) { return op == ShardedOp::kReduceScatter ? "reduce_scatter" : "all_gather"; }
+inline const char* op_title(ShardedOp op) { return op == ShardedOp::kReduceScatter ? "reduce-scatter" : "all-gather"; }
+
+// S: end of a shard table, which must tile [0, S) in order
+inline uint64_t shard_elems(const std::vector<LayerSpec>& layers) {
+  uint64_t end = 0;
+  for (const LayerSpec& l : layers) {
+    if (l.elem_off != end)
+      throw std::invalid_argument("cgx reduce_scatter: the shard layers must tile [0, S) in order, without gaps");
+    end += l.numel;
+  }
+  return end;
+}
+
+// a shard table's plan table: W copies at stride S, copy c = chunk c
+inline std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& shard, int world, uint64_t S) {
+  std::vector<LayerSpec> out;
+  out.reserve(shard.size() * (size_t)world);
+  for (int c = 0; c < world; ++c)
+    for (LayerSpec l : shard) {
+      l.elem_off += (uint64_t)c * S;
+      out.push_back(l);
+    }
+  return out;
+}
 
 // The windows of a reduce-scatter: the shard's layer table (offsets from the shard start, tiling
 // [0, S) in order; std::invalid_argument otherwise) cut by split_for_fusion into shard-relative
@@ -60,36 +90,32 @@ class FusedSra {
                                     cudaStream_t stream, int max_lanes = 0);
   void run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream);
 
-  // Compressed reduce-scatter (rs_kernel). `in` holds W * S elements, `out` S elements; this rank
-  // receives shard rank():  out = T(prescale * in[r] + sum over peers p of decode(Q(prescale * in_p[r]))).
-  // `shard_layers` is the quantization table of ONE shard (offsets from the shard start, tiling
-  // [0, S), S == out_numel); every shard uses it, so buckets are counted from each shard's start. `out` is disjoint
-  // from `in` or exactly its chunk rank(); anything else throws std::invalid_argument.
+  // A sharded collective over S-element shards; `shard_layers` is the quantization table of ONE
+  // shard (offsets from the shard start, tiling [0, S)); every shard uses it, so buckets are counted
+  // from each shard's start. The shard buffer is disjoint from the full buffer or exactly its chunk
+  // rank(); anything else throws std::invalid_argument.
+  //  kReduceScatter (rs_kernel): `in` holds W * S elements, `out` S; this rank receives shard rank():
+  //    out = T(prescale * in[r] + sum over peers p of decode(Q(prescale * in_p[r]))).
+  //  kAllGather (ag_kernel): `in` holds this rank's shard, `out` W * S: out[q * S + i] =
+  //    decode(Q_q(in_q[i])) for every rank q, this rank's own shard included, so every rank's `out`
+  //    is the same bytes (bits 32 = copied unchanged). Rounds to nearest unless rng.stochastic;
+  //    callers pass skip_incomplete = false and prescale = 1.
   // The shard is cut into windows whose worst-case wire fits one slot (split_for_fusion, cuts on
   // bucket boundaries, so the result does not depend on the slot size) and one kernel is launched
   // per window. Stream-ordered; every rank must issue the same calls in the same order.
   struct RsCounts {
     uint64_t launches = 0, elements = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's share
   };
-  RsCounts reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete, const void* in,
-                          void* out, uint64_t out_numel, float prescale, const RngParams& rng, cudaStream_t stream,
-                          int max_lanes = 0);
+  RsCounts sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                   const void* in, void* out, uint64_t S, float prescale, const RngParams& rng, cudaStream_t stream,
+                   int max_lanes = 0);
   // builds and uploads the plans of every window without launching anything
-  void prepare_reduce_scatter(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
-                              cudaStream_t stream, int max_lanes = 0);
+  void prepare_sharded(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                       cudaStream_t stream, int max_lanes = 0);
   // reduce_scatter_windows for this heap (cached per shard table); the all-gather uses the same
   // windows, since its per-chunk wire is the reduce-scatter's
   const std::vector<std::vector<LayerSpec>>& rs_windows(const std::vector<LayerSpec>& shard_layers, int dtype,
                                                         bool skip_incomplete, int max_lanes);
-
-  // Compressed all-gather (ag_kernel). `in` holds this rank's shard of S elements, `out` W * S:
-  // out[q * S + i] = decode(Q_q(in_q[i])) for every rank q, this rank's own shard included, so
-  // every rank's `out` is the same bytes. Q follows `shard_layers` (as for reduce_scatter: one
-  // shard's table, buckets counted from each shard's start; bits 32 = copied unchanged), rounding
-  // to nearest unless rng.stochastic. `in` is disjoint from `out` or exactly its chunk rank();
-  // anything else throws std::invalid_argument. Windows as for reduce_scatter, one kernel per window.
-  RsCounts all_gather(const std::vector<LayerSpec>& shard_layers, int dtype, const void* in, void* out, uint64_t S,
-                      const RngParams& rng, cudaStream_t stream, int max_lanes = 0);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

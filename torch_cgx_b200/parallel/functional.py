@@ -70,23 +70,30 @@ def all_reduce(tensor: torch.Tensor, bits: Optional[int] = None, bucket_size: Op
         return dist.all_reduce(tensor, op=op, group=group, async_op=async_op)
 
 
-def _reduce_scatter(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, average: bool,
-                    group, async_op: bool, stochastic: bool, seed: Optional[int],
-                    layers: Optional[Sequence[Tuple[int, int, int, int]]], skip_incomplete: bool,
-                    overlapped: bool):
+def _sharded(method: str, api: str, output: torch.Tensor, input: torch.Tensor, head: tuple, *, group,
+             async_op: bool, stochastic: bool, seed: Optional[int],
+             layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool):
+    """``native.<method>(output, input, *head, stochastic, seed, overlapped, layers)`` on the group's cgx backend."""
     from .hooks import _native_backend
 
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
     if native is None:
-        raise RuntimeError("cgx.reduce_scatter_tensor needs a process group with the cgx backend")
-    work = native.reduce_scatter_compressed(
-        output, input, bool(average), int(bits), int(bucket_size), bool(skip_incomplete), bool(stochastic),
-        -1 if seed is None else int(seed), bool(overlapped),
-        [tuple(int(v) for v in l) for l in (layers or [])])
+        raise RuntimeError(f"cgx.{api} needs a process group with the cgx backend")
+    work = getattr(native, method)(output, input, *head, bool(stochastic), -1 if seed is None else int(seed),
+                                   bool(overlapped), [tuple(int(v) for v in l) for l in (layers or [])])
     if async_op:
         return work
     work.wait()  # the current stream waits for the kernel; the host does not
     return None
+
+
+def _reduce_scatter(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, average: bool,
+                    group, async_op: bool, stochastic: bool, seed: Optional[int],
+                    layers: Optional[Sequence[Tuple[int, int, int, int]]], skip_incomplete: bool,
+                    overlapped: bool):
+    return _sharded("reduce_scatter_compressed", "reduce_scatter_tensor", output, input,
+                    (bool(average), int(bits), int(bucket_size), bool(skip_incomplete)), group=group,
+                    async_op=async_op, stochastic=stochastic, seed=seed, layers=layers, overlapped=overlapped)
 
 
 def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
@@ -111,18 +118,9 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int =
 def _all_gather(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, group, async_op: bool,
                 stochastic: bool, seed: Optional[int], layers: Optional[Sequence[Tuple[int, int, int, int]]],
                 overlapped: bool):
-    from .hooks import _native_backend
-
-    native = _native_backend(group if group is not None else dist.group.WORLD, input)
-    if native is None:
-        raise RuntimeError("cgx.all_gather_into_tensor needs a process group with the cgx backend")
-    work = native.all_gather_compressed(
-        output, input, int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
-        bool(overlapped), [tuple(int(v) for v in l) for l in (layers or [])])
-    if async_op:
-        return work
-    work.wait()  # the current stream waits for the kernel; the host does not
-    return None
+    return _sharded("all_gather_compressed", "all_gather_into_tensor", output, input, (int(bits), int(bucket_size)),
+                    group=group, async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
+                    overlapped=overlapped)
 
 
 def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
