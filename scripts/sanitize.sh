@@ -31,6 +31,10 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # grid merge (staging, self-resetting counters) on the one-element path with a partial last slab
 # (8x100x16x16), unaligned views (the flagship shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_batchnorm_gpu.py -m gpu -x -q -k "small_shapes or unaligned or rejects or fallbacks"
+# the chain kernels' launch geometries (GY at 8 / 9 / 127, L = 1..13, partial slabs, graph capture), under
+# memcheck and, since their chains, merges and trees meet in shared memory, under racecheck
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_batchnorm_mapping_gpu.py -m gpu -x -q
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_batchnorm_mapping_gpu.py -m gpu -x -q
 # quantization-error estimator: 16-byte and scalar loads, bucket sizes 8..8192 and non-multiples of 8,
 # tails, non-finite buckets, binding errors (the DDP run is left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_adaptive_bits_gpu.py -m gpu -x -q -k "not ddp and not round_trip"

@@ -21,8 +21,10 @@
 // with --fmad=false and writes every FMA explicitly.
 //
 // The physical mapping is free and differs: a thread runs one chain for 8 (16-bit) or 4 (fp32)
-// channels with 16-byte loads and kUnroll rows in flight; a block holds one ATen block row `by` and
-// a slab of up to 128 bytes of channels; the chain results meet in shared memory for the merges.
+// channels with 16-byte loads and U rows in flight; a block holds one ATen block row `by` and a slab
+// of channels; the chain results meet in shared memory for the merges. Short chains run on 256-thread
+// blocks light enough that 3-4 of them share an SM, so one block's merges, fence and arrival run while
+// the others' loads are in flight; long chains on 512-thread blocks (chain_launch).
 #include "device_utils.cuh"
 #include "launch.h"
 
@@ -30,9 +32,10 @@ namespace cgx {
 using namespace dev;
 
 namespace {
-constexpr int kMaxThreads = 512;
-constexpr int kUnroll = 8;        // rows of one chain in flight per thread
+constexpr int kLongChain = 16;    // chains of more rows run on wide blocks (see chain_launch)
+constexpr int block_threads(bool wide) { return wide ? 512 : 256; }
 constexpr int kSmemSlots = 4096;  // chains x slab channels; ATen's configs need at most 4096 (see below)
+constexpr int kMaxStaged = 8;     // staged rows per slot in the grid merge: GY >= 8 means BY >= 16, GY <= 128
 
 template <typename T, int V>
 struct Row {
@@ -69,11 +72,16 @@ __device__ __forceinline__ void welford_merge(int& n, float& mean, float& m2, in
   n += nb;
 }
 
+// The chain results of a block in dynamic shared memory, sized at its launch (forward_t, backward_t): 4*BY*W
+// slots per array. ResNet-50's short-chain blocks need 16.6 KB instead of a fixed 40 KB, so shared memory
+// does not limit how many of them share an SM.
+extern __shared__ float bn_smem[];
+
 struct Smem {
-  float mean[kSmemSlots];
-  float m2[kSmemSlots];
-  int cnt[kSmemSlots / 2];  // one count per chain: counts do not depend on the channel
-  bool last;
+  float* mean;
+  float* m2;
+  int* cnt;  // one count per chain: counts do not depend on the channel
+  __device__ Smem(int slots) : mean(bn_smem), m2(bn_smem + slots), cnt(reinterpret_cast<int*>(bn_smem + 2 * slots)) {}
 };
 
 // halving tree over ty of slot (ty*4) for the W channels of the slab (welford_merge_block_vertical)
@@ -101,18 +109,21 @@ struct StatsArgs {
   float momentum, bessel, eps;
 };
 
-template <typename T, int V>
-__global__ void __launch_bounds__(kMaxThreads) bn_stats_kernel(const T* __restrict__ x, const StatsArgs a) {
-  __shared__ Smem s;
+// U = 4 rows in flight for chains of at most 4 rows (fits four 256-thread blocks per SM), else 8 (three)
+template <typename T, int V, int U, bool WIDE>
+__global__ void __launch_bounds__(block_threads(WIDE), WIDE ? 1 : (U == 4 ? 4 : 3))
+bn_stats_kernel(const T* __restrict__ x, const StatsArgs a) {
   const int G = a.G, W = G * V, by = blockIdx.y;
   const int c0 = blockIdx.x * W;
   const int wvalid = min(W, a.C - c0);
   const int nch = a.BY * 4;
+  Smem s(nch * W);
+  __shared__ bool last;
   const int g = threadIdx.x % G;
   const int c = c0 + g * V;
   const int rstride = a.BY * a.GY;  // rows between a chain's consecutive (4i + j)
 
-  // ---- chains: Welford over rows, kUnroll rows in flight
+  // ---- chains: Welford over rows, U rows in flight
   for (int ch = threadIdx.x / G; ch < nch; ch += blockDim.x / G) {
     const int ty = ch >> 2, j = ch & 3;
     const int m0 = by * a.BY + ty;
@@ -121,10 +132,10 @@ __global__ void __launch_bounds__(kMaxThreads) bn_stats_kernel(const T* __restri
     for (int k = 0; k < V; ++k) mean[k] = m2[k] = 0.0f;
     int cnt = 0;
     if (c < a.C) {
-      for (int i0 = 0; i0 < a.L; i0 += kUnroll) {
-        Row<T, V> r[kUnroll];
+      for (int i0 = 0; i0 < a.L; i0 += U) {
+        Row<T, V> r[U];
 #pragma unroll
-        for (int u = 0; u < kUnroll; ++u) {
+        for (int u = 0; u < U; ++u) {
           const int64_t m = (int64_t)m0 + (int64_t)(4 * (i0 + u) + j) * rstride;
           if (i0 + u < a.L && m < a.M)
             r[u].load(x + m * a.C + c);
@@ -132,7 +143,7 @@ __global__ void __launch_bounds__(kMaxThreads) bn_stats_kernel(const T* __restri
             r[u].zero();
         }
 #pragma unroll
-        for (int u = 0; u < kUnroll; ++u) {
+        for (int u = 0; u < U; ++u) {
           if (i0 + u >= a.L) break;
           const int64_t m = (int64_t)m0 + (int64_t)(4 * (i0 + u) + j) * rstride;
           const bool valid = m < a.M;
@@ -197,30 +208,39 @@ __global__ void __launch_bounds__(kMaxThreads) bn_stats_kernel(const T* __restri
     __syncthreads();
     if (threadIdx.x == 0) {
       const int old = atomicAdd(&a.sem[blockIdx.x], 1);
-      s.last = old == a.GY - 1;
-      if (s.last) a.sem[blockIdx.x] = 0;  // ready for the next launch on this stream
+      last = old == a.GY - 1;
+      if (last) a.sem[blockIdx.x] = 0;  // ready for the next launch on this stream
     }
     __syncthreads();
-    if (!s.last) return;
+    if (!last) return;
     __threadfence();
-    // the last block: slot ty*4 merges staged rows y = ty, ty + BY, ... starting from the zero state
+    // the last block: slot ty*4 merges staged rows y = ty, ty + BY, ... starting from the zero state;
+    // all of a slot's staged loads are issued before its first merge
     for (int idx = threadIdx.x; idx < a.BY * W; idx += blockDim.x) {
       const int ty = idx / W, cc = idx - ty * W;
       if (cc >= wvalid) continue;
+      int nb[kMaxStaged];
+      float mb[kMaxStaged], m2b[kMaxStaged];
+#pragma unroll
+      for (int k = 0; k < kMaxStaged; ++k) {
+        const int y = ty + k * a.BY;
+        nb[k] = 0;
+        mb[k] = m2b[k] = 0.0f;
+        if (y < a.GY) {
+          const size_t o = (size_t)y * a.C + c0 + cc;
+          nb[k] = __ldcg(st_cnt + o);
+          mb[k] = __ldcg(st_mean + o);
+          m2b[k] = __ldcg(st_m2 + o);
+        }
+      }
       int n = 0;
       float mean = 0.0f, m2 = 0.0f;
-      for (int y = ty; y < a.GY; y += a.BY) {
-        const size_t o = (size_t)y * a.C + c0 + cc;
-        welford_merge<false>(n, mean, m2, __ldcg(st_cnt + o), __ldcg(st_mean + o), __ldcg(st_m2 + o));
-      }
+#pragma unroll
+      for (int k = 0; k < kMaxStaged; ++k)
+        if (ty + k * a.BY < a.GY) welford_merge<false>(n, mean, m2, nb[k], mb[k], m2b[k]);
       s.mean[ty * 4 * W + cc] = mean;
       s.m2[ty * 4 * W + cc] = m2;
-    }
-    __syncthreads();
-    if ((int)threadIdx.x < a.BY) {
-      int n = 0;
-      for (int y = threadIdx.x; y < a.GY; y += a.BY) n += __ldcg(st_cnt + (size_t)y * a.C + c0);
-      s.cnt[threadIdx.x * 4] = n;
+      if (cc == 0) s.cnt[ty * 4] = n;
     }
     vertical_tree(s, a.BY, W, wvalid);
   } else if (by != 0) {
@@ -308,10 +328,10 @@ __device__ __forceinline__ float masked_grad(float g, float x, float mu, float w
   return g;
 }
 
-struct SmemSum {
-  float dy[kSmemSlots];
-  float xmu[kSmemSlots];
-  bool last;
+struct SmemSum {  // as Smem
+  float* dy;
+  float* xmu;
+  __device__ SmemSum(int slots) : dy(bn_smem), xmu(bn_smem + slots) {}
 };
 
 struct ReduceArgs {
@@ -336,27 +356,41 @@ __device__ __forceinline__ void sum_tree(SmemSum& s, int BY, int W, int wvalid) 
   __syncthreads();
 }
 
-template <typename T, int V, bool RELU>
-__global__ void __launch_bounds__(kMaxThreads)
+// MASK_SMEM (with RELU, on 256-thread blocks): the mask's invstd, weight and bias come from shared memory,
+// which fits three blocks per SM instead of two
+template <typename T, int V, bool RELU, bool WIDE, bool MASK_SMEM>
+__global__ void __launch_bounds__(block_threads(WIDE), WIDE ? 1 : (RELU && !MASK_SMEM ? 2 : 3))
 bn_bwd_reduce_kernel(const T* __restrict__ gy, const T* __restrict__ x, const ReduceArgs a) {
   constexpr int U = 4;  // rows of one chain in flight per thread, for each of g and x
-  __shared__ SmemSum s;
   const int G = a.G, W = G * V, by = blockIdx.y;
   const int c0 = blockIdx.x * W;
   const int wvalid = min(W, a.C - c0);
   const int nch = a.BY * 4;
+  SmemSum s(nch * W);
+  __shared__ bool last;
   const int g = threadIdx.x % G;
   const int c = c0 + g * V;
   const int rstride = a.BY * a.GY;
 
+  // read at every use (volatile, so they are not hoisted into registers)
+  constexpr bool kMaskSmem = RELU && MASK_SMEM;
+  float* const prm = bn_smem + 2 * nch * W;  // [3][W]
+  if (kMaskSmem) {
+    for (int cc = threadIdx.x; cc < wvalid; cc += blockDim.x) {
+      prm[cc] = a.invstd[c0 + cc];
+      prm[W + cc] = a.weight[c0 + cc];
+      prm[2 * W + cc] = a.bias[c0 + cc];
+    }
+    __syncthreads();
+  }
   if (c < a.C) {
     float mu[V], is[V], w[V], b[V];
 #pragma unroll
     for (int k = 0; k < V; ++k) {
       mu[k] = a.mean[c + k];
-      is[k] = RELU ? a.invstd[c + k] : 0.0f;
-      w[k] = RELU ? a.weight[c + k] : 0.0f;
-      b[k] = RELU ? a.bias[c + k] : 0.0f;
+      is[k] = RELU && !kMaskSmem ? a.invstd[c + k] : 0.0f;
+      w[k] = RELU && !kMaskSmem ? a.weight[c + k] : 0.0f;
+      b[k] = RELU && !kMaskSmem ? a.bias[c + k] : 0.0f;
     }
     for (int ch = threadIdx.x / G; ch < nch; ch += blockDim.x / G) {
       const int ty = ch >> 2, j = ch & 3;
@@ -383,7 +417,14 @@ bn_bwd_reduce_kernel(const T* __restrict__ gy, const T* __restrict__ x, const Re
 #pragma unroll
           for (int k = 0; k < V; ++k) {
             const float xv = rx[u].f(k);
-            const float gv = masked_grad<T, V, RELU>(rg[u].f(k), xv, mu[k], w[k], is[k], b[k]);
+            float isk = is[k], wk = w[k], bk = b[k];
+            if (kMaskSmem) {
+              const volatile float* p = prm + g * V + k;
+              isk = p[0];
+              wk = p[W];
+              bk = p[2 * W];
+            }
+            const float gv = masked_grad<T, V, RELU>(rg[u].f(k), xv, mu[k], wk, isk, bk);
             sdy[k] = __fadd_rn(sdy[k], gv);
             sxmu[k] = __fmaf_rn(__fadd_rn(xv, -mu[k]), gv, sxmu[k]);
           }
@@ -426,20 +467,33 @@ bn_bwd_reduce_kernel(const T* __restrict__ gy, const T* __restrict__ x, const Re
     __syncthreads();
     if (threadIdx.x == 0) {
       const int old = atomicAdd(&a.sem[blockIdx.x], 1);
-      s.last = old == a.GY - 1;
-      if (s.last) a.sem[blockIdx.x] = 0;
+      last = old == a.GY - 1;
+      if (last) a.sem[blockIdx.x] = 0;
     }
     __syncthreads();
-    if (!s.last) return;
+    if (!last) return;
     __threadfence();
     for (int idx = threadIdx.x; idx < a.BY * W; idx += blockDim.x) {
       const int ty = idx / W, cc = idx - ty * W;
       if (cc >= wvalid) continue;
+      float bdy[kMaxStaged], bxmu[kMaxStaged];
+#pragma unroll
+      for (int k = 0; k < kMaxStaged; ++k) {
+        const int y = ty + k * a.BY;
+        bdy[k] = bxmu[k] = 0.0f;
+        if (y < a.GY) {
+          const size_t o = (size_t)y * a.C + c0 + cc;
+          bdy[k] = __ldcg(st_dy + o);
+          bxmu[k] = __ldcg(st_xmu + o);
+        }
+      }
       float dy = 0.0f, xmu = 0.0f;
-      for (int y = ty; y < a.GY; y += a.BY) {
-        const size_t o = (size_t)y * a.C + c0 + cc;
-        dy = __fadd_rn(dy, __ldcg(st_dy + o));
-        xmu = __fadd_rn(xmu, __ldcg(st_xmu + o));
+#pragma unroll
+      for (int k = 0; k < kMaxStaged; ++k) {
+        if (ty + k * a.BY < a.GY) {
+          dy = __fadd_rn(dy, bdy[k]);
+          xmu = __fadd_rn(xmu, bxmu[k]);
+        }
       }
       s.dy[ty * 4 * W + cc] = dy;
       s.xmu[ty * 4 * W + cc] = xmu;
@@ -532,11 +586,17 @@ AtenGrid aten_grid(int M, int C) {
 }
 
 // The launch of the two chain kernels: grid (slabs, GY), G vector groups of V channels per slab, and
-// threads over (chain, group). The chain results of a block fit kSmemSlots: a slab holds at most 64
-// channels (W); with C >= 32, BX = 32 so BY <= 16 and 4*BY*W <= 4096; with C < 32, W = C < 2*BX and
-// 4*BY <= 2048/BX.
+// threads over (chain, group). Two block shapes, chosen from the chain length L:
+//  * short chains (L <= kLongChain; ResNet-50's 28x28 and smaller layers): 256 threads, G <= 4, and three
+//    or four blocks per SM, so the merges and arrivals of one block overlap the loads of the others;
+//  * long chains (its 56x56 and 112x112 layers): 512 threads, G <= 8, one block per SM. There each block
+//    streams long enough that its merges cost little, and smaller blocks measured slower at C >= 128.
+// The chain results of a block fit kSmemSlots: a slab holds at most 64 channels (W); with C >= 32,
+// BX = 32 so BY <= 16 and 4*BY*W <= 4096; with C < 32, W = C < 2*BX and 4*BY <= 2048/BX.
 struct ChainLaunch {
   int by, gy, G, nslab, threads, L;
+  int slots;  // chain results per shared array: 4*BY chains x W channels
+  bool wide;
 };
 template <int V>
 ChainLaunch chain_launch(int M, int C) {
@@ -544,11 +604,19 @@ ChainLaunch chain_launch(int M, int C) {
   ChainLaunch l;
   l.by = ag.by;
   l.gy = ag.gy;
-  l.G = std::min(V == 1 ? 32 : 8, ceil_div(C, V));
-  l.nslab = ceil_div(C, l.G * V);
-  l.threads = l.G * std::min(4 * l.by, kMaxThreads / l.G);
   l.L = 1 + (M - 1) / (l.by * l.gy * 4);
+  l.wide = l.L > kLongChain;
+  l.G = std::min(V == 1 ? 32 : (l.wide ? 8 : 4), ceil_div(C, V));
+  l.nslab = ceil_div(C, l.G * V);
+  l.threads = l.G * std::min(4 * l.by, block_threads(l.wide) / l.G);
+  l.slots = 4 * l.by * l.G * V;
   return l;
+}
+
+// the bounds the chain kernels rely on: shared-memory slots (so at most 40 KB, below the 48 KB a launch
+// may take without opting in) and the staged rows of the grid merge
+bool chain_launch_ok(const ChainLaunch& l) {
+  return l.slots <= kSmemSlots && (l.gy == 1 || ceil_div(l.gy, l.by) <= kMaxStaged);
 }
 
 dim3 elementwise_grid(int M, int C, int V, dim3* block) {
@@ -564,7 +632,7 @@ cudaError_t forward_t(const BnForwardArgs& p, cudaStream_t stream) {
   const int M = p.M, C = p.C;
   const ChainLaunch l = chain_launch<V>(M, C);
   const int by = l.by, gy = l.gy, G = l.G, nslab = l.nslab, threads = l.threads;
-  if (4 * by * G * V > kSmemSlots) return cudaErrorInvalidConfiguration;
+  if (!chain_launch_ok(l)) return cudaErrorInvalidConfiguration;
   if (gy > 1 && (p.staging == nullptr || p.sem_len < nslab)) return cudaErrorInvalidValue;
 
   StatsArgs a;
@@ -584,7 +652,14 @@ cudaError_t forward_t(const BnForwardArgs& p, cudaStream_t stream) {
   a.bessel = (float)((double)M / (double)(M - 1));
   a.eps = (float)p.eps;
   const T* x = (const T*)p.x;
-  bn_stats_kernel<T, V><<<dim3(nslab, gy), threads, 0, stream>>>(x, a);
+  const dim3 grid(nslab, gy);
+  const size_t smem = (2 * (size_t)l.slots + 4 * by) * sizeof(float);  // mean, m2, one count per chain
+  if (l.wide)
+    bn_stats_kernel<T, V, 8, true><<<grid, threads, smem, stream>>>(x, a);
+  else if (l.L <= 4)
+    bn_stats_kernel<T, V, 4, false><<<grid, threads, smem, stream>>>(x, a);
+  else
+    bn_stats_kernel<T, V, 8, false><<<grid, threads, smem, stream>>>(x, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
 
@@ -603,7 +678,7 @@ template <typename T, int V, bool RELU>
 cudaError_t backward_t(const BnBackwardArgs& p, cudaStream_t stream) {
   const int M = p.M, C = p.C;
   const ChainLaunch l = chain_launch<V>(M, C);
-  if (4 * l.by * l.G * V > kSmemSlots) return cudaErrorInvalidConfiguration;
+  if (!chain_launch_ok(l)) return cudaErrorInvalidConfiguration;
   if (l.gy > 1 && (p.staging == nullptr || p.sem_len < l.nslab)) return cudaErrorInvalidValue;
   ReduceArgs a;
   a.M = M;
@@ -624,7 +699,18 @@ cudaError_t backward_t(const BnBackwardArgs& p, cudaStream_t stream) {
   a.grad_bias = p.grad_bias;
   const T* g = (const T*)p.g;
   const T* x = (const T*)p.x;
-  bn_bwd_reduce_kernel<T, V, RELU><<<dim3(l.nslab, l.gy), l.threads, 0, stream>>>(g, x, a);
+  // sum_dy, sum_dy_xmu; on 256-thread blocks with the mask also its invstd, weight and bias per channel
+  // The mask from shared memory pays for its extra loads only where blocks are short-lived (L <= 4: the
+  // 14x14 and 7x7 layers); it measured slower at 28x28.
+  const bool mask_smem = RELU && !l.wide && l.L <= 4;
+  const size_t smem = (2 * (size_t)l.slots + (mask_smem ? 3 * l.G * V : 0)) * sizeof(float);
+  const dim3 rgrid(l.nslab, l.gy);
+  if (l.wide)
+    bn_bwd_reduce_kernel<T, V, RELU, true, false><<<rgrid, l.threads, smem, stream>>>(g, x, a);
+  else if (mask_smem)
+    bn_bwd_reduce_kernel<T, V, RELU, false, RELU><<<rgrid, l.threads, smem, stream>>>(g, x, a);
+  else
+    bn_bwd_reduce_kernel<T, V, RELU, false, false><<<rgrid, l.threads, smem, stream>>>(g, x, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   dim3 block;
