@@ -7,9 +7,14 @@
     bytes read once, and the share of the 3.35 TB/s HBM3 data-sheet bandwidth. If seven candidates
     take clearly longer than one, arithmetic bounds the kernel, otherwise memory does.
 (b) ResNet-50 DDP steps at world 1 (batch 128, bf16 autocast, channels_last, SGD), device-timed with
-    CUDA events: native hook 4 bits, Python hook 4 bits, AdaptiveCGXState period 1 and period 100.
+    CUDA events: native hook 4 bits, Python hook 4 bits, and AdaptiveCGXState on the Python and on
+    the native hook at period 1, 100 and "never" (one decision right after registration, inside
+    the warm-up). The arms run in two rounds, the second in reverse order.
 (c) The fused allreduce (world 1: quantize + decode in one kernel) of every ResNet-50 bucket with
     the adaptive assignment against uniform 4 bits.
+(d) The host time of one decision on the ResNet-50 layer table, replayed call by call: group sum of
+    the float64 table plus the copy to the host, the allocator (C++ against the NumPy reference),
+    the broadcast of the widths and their application to the registry.
 Prints the card and its power limit first; one JSON line per result.
 """
 import argparse
@@ -79,14 +84,17 @@ def bench_estimator():
                       "GBps": round(nbytes / t / 1e9, 1), "hbm_share": round(nbytes / t / HBM_BPS, 3)})
 
 
+NEVER = 1 << 40  # a period no run reaches: only the decision right after registration
+
+
 def make_step(kind, period=None):
     torch.manual_seed(0)
     net = models.resnet50().cuda().to(memory_format=torch.channels_last)
     ddp = torch.nn.parallel.DistributedDataParallel(net, device_ids=[0], gradient_as_bucket_view=True)
     params = {"bits": 4, "bucket_size": BUCKET}
-    if kind == "adaptive":
+    if kind in ("adaptive", "adaptive_native"):
         state = cgx.AdaptiveCGXState(None, MIN_SIZE, params, period=period)
-        ddp.register_comm_hook(state, cgx.cgx_hook)
+        cgx.register_cgx_hook(ddp, state, native=kind == "adaptive_native")
     else:
         state = cgx.CGXState(None, MIN_SIZE, params)
         if kind == "native":
@@ -108,20 +116,74 @@ def make_step(kind, period=None):
 
 
 def bench_steps(steps, warmup):
+    arms = [("native", None), ("python", None)]
+    arms += [(kind, period) for period in (1, 100, NEVER) for kind in ("adaptive", "adaptive_native")]
     adaptive_state = None
-    for kind, period in (("native", None), ("python", None), ("adaptive", 1), ("adaptive", 100)):
-        cgx.reset_layers()
-        step, state, ddp = make_step(kind, period)
-        for _ in range(max(warmup, 4)):
-            step()
-        torch.cuda.synchronize()
-        t = time_events(step, steps)
-        emit({"part": "b", "hook": kind, "period": period, "steps": steps, "step_ms": round(t * 1e3, 2),
-              "images_per_s": round(128 / t, 1)})
-        if kind == "adaptive" and period == 100:
-            adaptive_state = state
-        del step, ddp
+    for rnd, order in enumerate((arms, arms[::-1])):
+        for kind, period in order:
+            cgx.reset_layers()
+            step, state, ddp = make_step(kind, period)
+            for _ in range(max(warmup, 4)):
+                step()
+            torch.cuda.synchronize()
+            t = time_events(step, steps)
+            emit({"part": "b", "round": rnd, "hook": kind, "period": "never" if period == NEVER else period,
+                  "steps": steps, "step_ms": round(t * 1e3, 2), "images_per_s": round(128 / t, 1)})
+            if kind == "adaptive" and period == 100:
+                adaptive_state = state
+            del step, ddp
     return adaptive_state
+
+
+def bench_decision(state, reps=20):
+    """One decision's host work, replayed with the calls both hooks make."""
+    import time
+
+    from torch_cgx_b200 import _C
+    from torch_cgx_b200.ops.bit_allocation import layer_wire_bytes
+    from torch_cgx_b200.ops.oracle import allocate_bits_reference
+
+    rows = list(state.adapted_layers)
+    table = state.last_errors.cuda()
+    K = len(state.candidate_bits)
+    numels = [n for (_, _, _, n) in rows]
+    budget = sum(layer_wire_bytes(n, 4, BUCKET) for n in numels)
+    current = [state.assignment.get((b, l), 4) for (b, l, _, _) in rows]
+    err = state.last_errors.numpy()
+    args = (numels, [BUCKET] * len(rows), list(state.candidate_bits), budget, current)
+
+    def timed(fn):
+        best = []
+        for _ in range(reps):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            best.append(time.perf_counter() - t0)
+        return round(sorted(best)[len(best) // 2] * 1e6, 1)  # median
+
+    def group_sum_copy():
+        t = table.clone()
+        dist.all_reduce(t)
+        t.view(-1, K).cpu()
+
+    picked = _C.allocate_bits(err, *args, 4096, 4)
+    assert picked == allocate_bits_reference(err, *args, 4096, target_bits=4)
+    choice = torch.tensor(picked, dtype=torch.int32)
+
+    def broadcast():
+        c = choice.cuda()
+        dist.broadcast(c, src=0)
+        c.cpu()
+
+    def apply():
+        for (b, l, _, _), bits in zip(rows, picked):
+            _C.set_quantization_bits(b, l, bits)
+
+    emit({"part": "d", "layers": len(rows), "candidates": K,
+          "group_sum_copy_us": timed(group_sum_copy),
+          "allocator_cpp_us": timed(lambda: _C.allocate_bits(err, *args, 4096, 4)),
+          "allocator_numpy_us": timed(lambda: allocate_bits_reference(err, *args, 4096, target_bits=4)),
+          "broadcast_us": timed(broadcast), "apply_from_python_us": timed(apply)})
 
 
 def bench_mixed_allreduce(state):
@@ -167,6 +229,7 @@ def main():
     dist.init_process_group("cgx", init_method=f"tcp://127.0.0.1:{port}", rank=0, world_size=1)
     try:
         state = bench_steps(args.steps, args.warmup)
+        bench_decision(state)
         bench_mixed_allreduce(state)
     finally:
         dist.destroy_process_group()

@@ -20,6 +20,7 @@ SOURCES = [
     "common/config.cc",
     "common/layers.cc",
     "common/sra_sim.cc",
+    "common/bit_allocation.cc",
     "comm/fd_channel.cc",
     "comm/loopback_communicator.cc",
     "comm/symmetric_heap.cc",
@@ -29,6 +30,7 @@ SOURCES = [
     "pg/c10d_communicator.cc",
     "pg/comm_hook.cc",
     "engine/engine.cc",
+    "engine/quant_error_table.cc",
     "kernels/sra_f32.cu",
     "kernels/sra_f16.cu",
     "kernels/sra_bf16.cu",

@@ -12,6 +12,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
 #include <pybind11/chrono.h>
+#include <pybind11/numpy.h>
 #include <torch/extension.h>
 
 #include <limits>
@@ -25,12 +26,14 @@
 
 #include "comm/fd_channel.h"
 #include "comm/loopback_communicator.h"
+#include "common/bit_allocation.h"
 #include "common/block_ops.h"
 #include "common/config.h"
 #include "common/layers.h"
 #include "common/plan.h"
 #include "common/quant_error.h"
 #include "common/sra_sim.h"
+#include "engine/quant_error_table.h"
 #include "kernels/launch.h"
 #include "pg/comm_hook.h"
 #include "pg/process_group_cgx.h"
@@ -689,69 +692,14 @@ at::Tensor py_residual_relu_backward(const at::Tensor& y, const at::Tensor& ga, 
 }
 
 // [len(layers), len(candidates)] float64: squared quantization error of every layer at every
-// candidate width (common/quant_error.h); CPU tensors run the C++ path, CUDA tensors the kernel
+// candidate width (engine/quant_error_table.h)
 at::Tensor py_quantization_error(const at::Tensor& t, const std::vector<LayerTuple>& layers,
                                  const std::vector<int64_t>& candidates, bool stochastic, double prescale,
                                  bool skip_incomplete) {
-  TORCH_CHECK(t.device().is_cpu() || t.is_cuda(), "quantization_error: tensor must be on the CPU or a CUDA device");
-  TORCH_CHECK(t.is_contiguous(), "quantization_error: tensor must be contiguous");
-  const int dt = cgx_dtype(t);
-  const int K = (int)candidates.size();
-  TORCH_CHECK(K >= 1 && K <= kQErrMaxCandidates, "quantization_error: need 1 to ", kQErrMaxCandidates,
-              " candidate widths, got ", K);
-  int bits[kQErrMaxCandidates];
-  for (int k = 0; k < K; ++k) {
-    TORCH_CHECK(candidates[k] >= 1 && candidates[k] <= 8, "quantization_error: candidate width ", candidates[k],
-                " is outside 1..8");
-    bits[k] = (int)candidates[k];
-  }
-  std::vector<QErrLayer> ls;
-  ls.reserve(layers.size());
-  for (const auto& l : layers) {
-    const int64_t off = std::get<0>(l), n = std::get<1>(l), bucket = std::get<3>(l);
-    TORCH_CHECK(off >= 0 && n >= 0 && off + n <= t.numel(), "quantization_error: layer (", off, ", ", n,
-                ") is outside the tensor of ", t.numel(), " elements");
-    TORCH_CHECK(bucket >= 1, "quantization_error: bucket size must be >= 1, got ", bucket);
-    // clamped like the plan clamps it (plan.cc: push_segment)
-    const uint32_t B = (uint32_t)std::min<int64_t>(bucket, kMaxBlockElems);
-    // with skip_incomplete the tail bucket travels raw: no error
-    ls.push_back({(uint64_t)off, skip_incomplete ? (uint64_t)n / B * B : (uint64_t)n, B, 0});
-  }
-  const int64_t L = (int64_t)ls.size();
-  if (t.device().is_cpu()) {
-    at::Tensor out = at::zeros({L, (int64_t)K}, at::kDouble);
-    cpu::quantization_error(t.data_ptr(), dt, ls, bits, K, stochastic, (float)prescale, out.data_ptr<double>());
-    return out;
-  }
-  c10::cuda::CUDAGuard g(t.device());
-  auto stream = c10::cuda::getCurrentCUDAStream();
-  const std::vector<uint64_t> first = qerr_first(ls);
-  const uint64_t nb = first.back();
-  TORCH_CHECK(nb < (1ull << 34), "quantization_error: too many buckets for one launch");
-  const size_t lbytes = ls.size() * sizeof(QErrLayer), fbytes = first.size() * sizeof(uint64_t);
-  // layer table and first buckets go up in one copy from pinned memory: no synchronisation with the stream
-  at::Tensor host = at::empty({(int64_t)(lbytes + fbytes)}, at::TensorOptions().dtype(at::kByte).pinned_memory(true));
-  std::memcpy(host.data_ptr<uint8_t>(), ls.data(), lbytes);
-  std::memcpy(host.data_ptr<uint8_t>() + lbytes, first.data(), fbytes);
-  at::Tensor dev = at::empty({(int64_t)(lbytes + fbytes)}, t.options().dtype(at::kByte));
-  dev.copy_(host, /*non_blocking=*/true);
-  at::Tensor partial = at::empty({(int64_t)std::max<uint64_t>(1, nb * (uint64_t)K)}, t.options().dtype(at::kFloat));
-  at::Tensor out = at::empty({L, (int64_t)K}, t.options().dtype(at::kDouble));
-  QErrArgs a;
-  a.data = t.data_ptr();
-  a.dtype = dt;
-  a.layer_table = reinterpret_cast<const QErrLayer*>(dev.data_ptr<uint8_t>());
-  a.first = reinterpret_cast<const uint64_t*>(dev.data_ptr<uint8_t>() + lbytes);
-  a.nbuckets = nb;
-  a.layers = (int)L;
-  a.bits = bits;
-  a.K = K;
-  a.prescale = (float)prescale;
-  a.stochastic = stochastic;
-  a.partial = partial.data_ptr<float>();
-  a.out = out.data_ptr<double>();
-  cuda_check(launch_quantization_error(a, stream), "quantization_error");
-  return out;
+  std::vector<QErrSpan> spans;
+  spans.reserve(layers.size());
+  for (const auto& l : layers) spans.push_back({std::get<0>(l), std::get<1>(l), std::get<3>(l)});
+  return quantization_error_table(t, spans, candidates, stochastic, prescale, skip_incomplete);
 }
 
 // ---- training BatchNorm on channels_last input ----
@@ -938,19 +886,63 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("enable_trace", &ProcessGroupCGX::enable_trace)
       .def("read_trace", &ProcessGroupCGX::read_trace);
 
+  using Assignment = std::map<std::pair<int64_t, int64_t>, int>;
   py::class_<HookState, std::shared_ptr<HookState>>(m, "NativeHookState")
       .def_property_readonly("step", [](const HookState& h) { return h.step.load(); })
       .def_readonly("layer_min_size", &HookState::layer_min_size)
       .def_readonly("bits", &HookState::bits)
       .def_readonly("bucket_size", &HookState::bucket_size)
-      .def_readonly("register_step", &HookState::register_step);
+      .def_readonly("register_step", &HookState::register_step)
+      .def_readonly("candidates", &HookState::candidates)
+      .def_readonly("period", &HookState::period)
+      // (bucket, layer) -> width applied by a decision or a loaded assignment
+      .def_property_readonly("assignment", [](HookState& h) {
+        std::lock_guard<std::mutex> lk(h.mu);
+        return h.assignment;
+      })
+      // group-summed [rows, candidates] float64 table of the last decision, or None
+      .def_property_readonly("last_errors", [](HookState& h) -> std::optional<at::Tensor> {
+        std::lock_guard<std::mutex> lk(h.mu);
+        if (!h.last_errors.defined()) return std::nullopt;
+        return h.last_errors;
+      })
+      // (bucket, layer, elem_off, numel) of every adapted layer, in bucket order
+      .def_property_readonly("adapted_layers", [](HookState& h) {
+        std::vector<std::tuple<int64_t, int64_t, int64_t, int64_t>> out;
+        for (const AdaptedLayer& l : h.adapted_layers()) out.emplace_back(l.bucket, l.layer, l.elem_off, l.numel);
+        return out;
+      })
+      // widths to apply when the layers are registered (a checkpoint's assignment)
+      .def("load_assignment", [](HookState& h, const Assignment& a) {
+        std::lock_guard<std::mutex> lk(h.mu);
+        h.loaded = a;
+      }, py::arg("assignment"));
   m.def("register_native_hook",
         [](const std::shared_ptr<c10d::Reducer>& reducer, const c10::intrusive_ptr<ProcessGroupCGX>& pg,
-           int64_t layer_min_size, int bits, int bucket_size, int register_step) {
-          return register_native_hook(reducer, pg, layer_min_size, bits, bucket_size, register_step);
+           int64_t layer_min_size, int bits, int bucket_size, int register_step, std::vector<int64_t> candidates,
+           int64_t period, Assignment assignment) {
+          return register_native_hook(reducer, pg, layer_min_size, bits, bucket_size, register_step,
+                                      std::move(candidates), period, std::move(assignment));
         },
         py::arg("reducer"), py::arg("backend"), py::arg("layer_min_size"), py::arg("bits"), py::arg("bucket_size"),
-        py::arg("register_step") = 2);
+        py::arg("register_step") = 2, py::arg("candidates") = std::vector<int64_t>{}, py::arg("period") = 1,
+        py::arg("assignment") = Assignment{});
+  m.def("layer_wire_bytes", &layer_wire_bytes, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"));
+  m.def("allocate_bits",
+        [](py::array_t<double, py::array::c_style | py::array::forcecast> errors, const std::vector<int64_t>& numels,
+           const std::vector<int64_t>& bucket_sizes, const std::vector<int>& candidates, int64_t budget_bytes,
+           const std::optional<std::vector<int>>& current, int64_t resolution, std::optional<int> target_bits) {
+          const int64_t L = (int64_t)numels.size(), K = (int64_t)candidates.size();
+          TORCH_CHECK(errors.ndim() == 2 && errors.shape(0) == L && errors.shape(1) == K,
+                      "allocate_bits: errors must be [", L, ", ", K, "]");
+          TORCH_CHECK(K >= 1 && resolution >= 1 && (int64_t)bucket_sizes.size() >= L,
+                      "allocate_bits: need a candidate, resolution >= 1 and a bucket size per layer");
+          py::gil_scoped_release nogil;
+          return allocate_bits(errors.data(), L, numels, bucket_sizes, candidates, budget_bytes,
+                               current ? &*current : nullptr, resolution, target_bits);
+        },
+        py::arg("errors"), py::arg("numels"), py::arg("bucket_sizes"), py::arg("candidates"), py::arg("budget_bytes"),
+        py::arg("current") = py::none(), py::arg("resolution") = 4096, py::arg("target_bits") = py::none());
 
   m.def("create_backend", &create_backend, py::arg("store"), py::arg("rank"), py::arg("size"), py::arg("timeout"),
         py::arg("cpu_delegate"), py::arg("cuda_delegate"), py::arg("local_size") = 0,

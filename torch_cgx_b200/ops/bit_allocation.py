@@ -3,22 +3,23 @@
 ``allocate_bits`` picks one candidate width per layer so that the summed quantization error
 (``quantization_error``) is smallest while the summed wire bytes stay within a budget: a
 multiple-choice knapsack, solved by dynamic programming over the budget split into ``resolution``
-bins. Host logic that runs once per adaptation period.
+bins. Host logic that runs once per adaptation period, in C++ (``csrc/common/bit_allocation.cc``);
+the native DDP hook calls the same function. ``ops.oracle.allocate_bits_reference`` is its NumPy
+twin.
 """
 from __future__ import annotations
 
+import math
 from typing import List, Optional, Sequence
 
 import numpy as np
 
-from .quantization import wire_bytes
-
-MAX_BUCKET = 8192  # the plan clamps quantization buckets to this (csrc/common/wire.h: kMaxBlockElems)
+from .. import _C
 
 
 def layer_wire_bytes(numel: int, bits: int, bucket_size: int) -> int:
     """Wire bytes of one layer at ``bits``, with the bucket clamped as the plan clamps it."""
-    return wire_bytes(int(numel), int(bits), max(1, min(int(bucket_size), MAX_BUCKET)))
+    return _C.layer_wire_bytes(int(numel), int(bits), int(bucket_size))
 
 
 def allocate_bits(
@@ -51,53 +52,10 @@ def allocate_bits(
         raise ValueError(f"allocate_bits: errors has shape {err.shape}, expected ({L}, {K})")
     if K == 0 or resolution < 1:
         raise ValueError("allocate_bits: need at least one candidate and resolution >= 1")
-    cost = np.array([[layer_wire_bytes(n, b, bs) for b in cands] for n, bs in zip(numels, bucket_sizes)],
-                    dtype=np.int64).reshape(L, K)
-    if target_bits is None:
-        fits = [k for k in range(K) if cost[:, k].sum() <= budget_bytes]
-        target_bits = max(cands[k] for k in fits) if fits else min(cands)
-    keep = [int(c) for c in current] if current is not None else [int(target_bits)] * L
-    out = list(keep)
-    finite = np.isfinite(err).all(axis=1)
-    free = [l for l in range(L) if finite[l]]
-    fixed_bytes = sum(layer_wire_bytes(numels[l], keep[l], bucket_sizes[l]) for l in range(L) if not finite[l])
-    room = int(budget_bytes) - fixed_bytes
-    k_t = cands.index(target_bits) if target_bits in cands else None
-    uniform = list(out)
-    for l in free:
-        uniform[l] = int(target_bits)
-    if not free or room <= 0:
-        return uniform
-
-    # bins[l, k] = ceil(cost * resolution / room): any choice with sum(bins) <= resolution fits
-    R = int(resolution)
-    bins = (cost[free] * R + room - 1) // room
-    e = err[free]
-    # candidates visited in (bytes, index) order with strict improvement: ties keep fewer bytes
-    order = np.lexsort((np.arange(K)[None, :].repeat(len(free), 0), cost[free]), axis=1)
-    dp = np.zeros(R + 1)  # least error of the layers so far within c bins
-    choice = np.zeros((len(free), R + 1), dtype=np.int16)
-    for i in range(len(free)):
-        best = np.full(R + 1, np.inf)
-        pick = np.zeros(R + 1, dtype=np.int16)
-        for k in order[i]:
-            c = int(bins[i, k])
-            if c > R:
-                continue
-            cand = np.full(R + 1, np.inf)
-            cand[c:] = dp[: R + 1 - c] + e[i, k]
-            better = cand < best
-            best[better] = cand[better]
-            pick[better] = k
-        dp, choice[i] = best, pick
-    if not np.isfinite(dp[R]):
-        return uniform
-    c = int(np.argmax(dp == dp[R]))  # fewest bins that reach the least error (dp is non-increasing)
-    total = dp[R]
-    for i in range(len(free) - 1, -1, -1):
-        k = int(choice[i, c])
-        out[free[i]] = cands[k]
-        c -= int(bins[i, k])
-    if k_t is not None and cost[free, k_t].sum() <= room and total > e[:, k_t].sum():
-        return uniform
-    return out
+    if len(bucket_sizes) < L:
+        raise ValueError(f"allocate_bits: {len(bucket_sizes)} bucket sizes for {L} layers")
+    # costs are whole bytes, so sum <= budget and sum <= floor(budget) agree
+    return _C.allocate_bits(np.ascontiguousarray(err), [int(n) for n in numels],
+                            [int(b) for b in list(bucket_sizes)[:L]], cands, math.floor(budget_bytes),
+                            None if current is None else [int(c) for c in current], int(resolution),
+                            None if target_bits is None else int(target_bits))

@@ -527,3 +527,73 @@ def exact_sum_and_bound(inputs: Sequence[torch.Tensor], layers: Sequence[Layer],
         b = b + _half_ulp(np.abs(exact[sl]) + b, dtype)
         bound[sl] = b
     return exact, bound
+
+
+# ---- bit allocation ------------------------------------------------------------------------------
+def _layer_wire_bytes(numel: int, bits: int, bucket_size: int) -> int:
+    """Wire bytes of one layer (ops.wire_bytes) with the bucket clamped as the plan clamps it."""
+    from .quantization import wire_bytes
+
+    return wire_bytes(int(numel), int(bits), effective_bucket(bucket_size))
+
+
+def allocate_bits_reference(errors, numels: Sequence[int], bucket_sizes: Sequence[int], candidates: Sequence[int],
+                            budget_bytes: int, current=None, resolution: int = 4096, *, target_bits=None) -> List[int]:
+    """NumPy dynamic program of ``ops.allocate_bits`` (same arguments, same result for every input)."""
+    err = np.asarray(errors, dtype=np.float64)
+    cands = [int(c) for c in candidates]
+    L, K = len(numels), len(cands)
+    if err.shape != (L, K):
+        raise ValueError(f"allocate_bits: errors has shape {err.shape}, expected ({L}, {K})")
+    if K == 0 or resolution < 1:
+        raise ValueError("allocate_bits: need at least one candidate and resolution >= 1")
+    cost = np.array([[_layer_wire_bytes(n, b, bs) for b in cands] for n, bs in zip(numels, bucket_sizes)],
+                    dtype=np.int64).reshape(L, K)
+    if target_bits is None:
+        fits = [k for k in range(K) if cost[:, k].sum() <= budget_bytes]
+        target_bits = max(cands[k] for k in fits) if fits else min(cands)
+    keep = [int(c) for c in current] if current is not None else [int(target_bits)] * L
+    out = list(keep)
+    finite = np.isfinite(err).all(axis=1)
+    free = [l for l in range(L) if finite[l]]
+    fixed_bytes = sum(_layer_wire_bytes(numels[l], keep[l], bucket_sizes[l]) for l in range(L) if not finite[l])
+    room = int(budget_bytes) - fixed_bytes
+    k_t = cands.index(target_bits) if target_bits in cands else None
+    uniform = list(out)
+    for l in free:
+        uniform[l] = int(target_bits)
+    if not free or room <= 0:
+        return uniform
+
+    # bins[l, k] = ceil(cost * resolution / room): any choice with sum(bins) <= resolution fits
+    R = int(resolution)
+    bins = (cost[free] * R + room - 1) // room
+    e = err[free]
+    # candidates visited in (bytes, index) order with strict improvement: ties keep fewer bytes
+    order = np.lexsort((np.arange(K)[None, :].repeat(len(free), 0), cost[free]), axis=1)
+    dp = np.zeros(R + 1)  # least error of the layers so far within c bins
+    choice = np.zeros((len(free), R + 1), dtype=np.int16)
+    for i in range(len(free)):
+        best = np.full(R + 1, np.inf)
+        pick = np.zeros(R + 1, dtype=np.int16)
+        for k in order[i]:
+            c = int(bins[i, k])
+            if c > R:
+                continue
+            cand = np.full(R + 1, np.inf)
+            cand[c:] = dp[: R + 1 - c] + e[i, k]
+            better = cand < best
+            best[better] = cand[better]
+            pick[better] = k
+        dp, choice[i] = best, pick
+    if not np.isfinite(dp[R]):
+        return uniform
+    c = int(np.argmax(dp == dp[R]))  # fewest bins that reach the least error (dp is non-increasing)
+    total = dp[R]
+    for i in range(len(free) - 1, -1, -1):
+        k = int(choice[i, c])
+        out[free[i]] = cands[k]
+        c -= int(bins[i, k])
+    if k_t is not None and cost[free, k_t].sum() <= room and total > e[:, k_t].sum():
+        return uniform
+    return out

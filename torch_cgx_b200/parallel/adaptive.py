@@ -14,6 +14,10 @@ Usage (the Python hook; ``register_cgx_hook`` installs it too and returns None):
 
     state = cgx.AdaptiveCGXState(None, compression_params={"bits": 4, "bucket_size": 1024}, period=1000)
     ddp.register_comm_hook(state, cgx.cgx_hook)
+
+On a ``cgx`` group, ``cgx.register_cgx_hook(ddp, state, native=True)`` runs the same steps in the
+native C++ hook (``csrc/pg/comm_hook.cc``) with the same results; ``assignment``, ``last_errors``,
+``adapted_layers``, ``state_dict`` and ``load_state_dict`` then read and write the native state.
 """
 from __future__ import annotations
 
@@ -58,6 +62,7 @@ class AdaptiveCGXState(CGXState):
         if period < 1:
             raise ValueError(f"period must be >= 1, got {period}")
         self.period = int(period)
+        self.native = None  # the native hook's state, once register_cgx_hook(..., native=True) installed it
         self.assignment: Dict[Tuple[int, int], int] = {}
         self.last_errors: Optional[torch.Tensor] = None
         self.adapted_layers: list = []  # (bucket, layer, elem_off, numel), registration order
@@ -66,6 +71,31 @@ class AdaptiveCGXState(CGXState):
         self._loaded: Dict[Tuple[int, int], int] = {}
         self._step_open = False
         self._device = torch.device("cpu")
+
+    # ---- state of whichever hook runs: the native one once installed --------------------------
+    @property
+    def assignment(self) -> Dict[Tuple[int, int], int]:
+        return dict(self.native.assignment) if self.native is not None else self._assignment
+
+    @assignment.setter
+    def assignment(self, value: Dict[Tuple[int, int], int]) -> None:
+        self._assignment = value
+
+    @property
+    def last_errors(self) -> Optional[torch.Tensor]:
+        return self.native.last_errors if self.native is not None else self._last_errors
+
+    @last_errors.setter
+    def last_errors(self, value: Optional[torch.Tensor]) -> None:
+        self._last_errors = value
+
+    @property
+    def adapted_layers(self) -> list:
+        return list(self.native.adapted_layers) if self.native is not None else self._adapted_layers
+
+    @adapted_layers.setter
+    def adapted_layers(self, value: list) -> None:
+        self._adapted_layers = value
 
     # ---- checkpoint -------------------------------------------------------------------------
     def state_dict(self) -> Dict:
@@ -76,6 +106,8 @@ class AdaptiveCGXState(CGXState):
     def load_state_dict(self, sd: Dict) -> None:
         super().load_state_dict(sd)
         self._loaded = {tuple(k): int(v) for k, v in dict(sd.get("assignment", {})).items()}
+        if self.native is not None:
+            self.native.load_assignment(self._loaded)
 
     # ---- per-bucket hook body (called by cgx_hook) -------------------------------------------
     def bucket_hook(self, bucket: dist.GradBucket) -> torch.futures.Future[torch.Tensor]:

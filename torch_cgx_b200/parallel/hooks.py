@@ -121,25 +121,37 @@ def cgx_hook(state: CGXState, bucket: dist.GradBucket) -> torch.futures.Future[t
     return _allreduce_fut(state.process_group, bucket.buffer(), bucket.index() if registered else -1)
 
 
-def register_cgx_hook(ddp_model, state: CGXState):
+def register_cgx_hook(ddp_model, state: CGXState, native: Optional[bool] = None):
     """Install the compressed-allreduce hook on a DistributedDataParallel model.
 
-    With the ``cgx`` backend this registers the **native C++ hook** directly on DDP's reducer
-    (no Python in the per-bucket path); with any other backend, and for an
-    :class:`~torch_cgx_b200.AdaptiveCGXState` (the native hook has no adaptive widths), it falls
-    back to ``ddp_model.register_comm_hook(state, cgx_hook)``. Returns the native state handle or None.
+    ``native=None`` (default): with the ``cgx`` backend a :class:`CGXState` gets the **native C++
+    hook**, registered directly on DDP's reducer (no Python in the per-bucket path); with any other
+    backend, and for an :class:`~torch_cgx_b200.AdaptiveCGXState`, this falls back to
+    ``ddp_model.register_comm_hook(state, cgx_hook)``.
+
+    ``native=True`` installs the native hook for either state, adaptive widths included; it raises
+    ``ValueError`` when the group has no ``cgx`` backend. ``native=False`` always installs the Python
+    hook. Returns the native state handle (also stored as ``state.native``) or None.
     """
     from .. import _C
 
     params = [p for p in ddp_model.parameters() if p.requires_grad]
     device = params[0].device if params else torch.device("cpu")
-    native = _backend.get_backend(state.process_group, device)
-    if native is None or hasattr(state, "bucket_hook"):
+    backend = _backend.get_backend(state.process_group, device)
+    adaptive = hasattr(state, "bucket_hook")
+    if native is None:
+        native = backend is not None and not adaptive
+    elif native and backend is None:
+        raise ValueError("register_cgx_hook(native=True) needs a process group with the cgx backend")
+    if not native:
         ddp_model.register_comm_hook(state, cgx_hook)
         return None
-    handle = _C.register_native_hook(ddp_model.reducer, native, int(state.layer_min_size),
+    extra = {}
+    if adaptive:
+        extra = dict(candidates=list(state.candidate_bits), period=int(state.period), assignment=dict(state._loaded))
+    handle = _C.register_native_hook(ddp_model.reducer, backend, int(state.layer_min_size),
                                      int(state.quantization_bits), int(state.quantization_bucket_size),
-                                     int(state.register_step))
+                                     int(state.register_step), **extra)
     try:
         ddp_model.logger._set_comm_hook_name("cgx_native_hook")
     except Exception:  # noqa: BLE001
