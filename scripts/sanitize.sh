@@ -24,6 +24,10 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # all-to-all and the compressed broadcast at W = 3 on unaligned views, and the 1024-element slice path
 RED_SUBSET='(match_host_and_reference and w3-float32-) or (width_and_slice_variants and 4-1024)'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_reducers_local_gpu.py -m gpu -x -q -k "$RED_SUBSET"
+# the allreduce engine with W engines on one GPU: fused groups halved and replayed from the bucket fast
+# path, a two-level hierarchy with the compressed broadcast, the sharded collectives
+ENG_SUBSET='(single_node and w2-float32) or (replays_the_slow_path and sr-2) or w4l2-SRA-RING or reduce_scatter_and_all_gather'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_engine_local_gpu.py -m gpu -x -q -k "$ENG_SUBSET"
 # ResNet residual join: 16-byte and scalar paths, tails, unaligned views, with and without gb (the
 # 103 M-element layer1 shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_residual_relu_gpu.py -m gpu -x -q -k "not layer1 and not training_step"

@@ -8,6 +8,8 @@
 //    device.
 //  * LocalReducerGroup: W virtual ranks of the generic reducers (one host thread
 //    each, loopback transport) on host memory or on ONE GPU.
+//  * LocalEngineGroup: W AllreduceEngines wired as the process group wires them, in one process,
+//    with a log of the stages each one issues.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
@@ -130,9 +132,14 @@ RngParams make_rng(bool stochastic, uint64_t seed, uint32_t seq) {
 size_t wire_row_bytes(const Plan& p) { return ((size_t)p.max_chunk_wire + 255) / 256 * 256; }
 
 // ---- CPU oracle ops -------------------------------------------------------
+// `prescale`: the factor every contribution is multiplied by first; none means 1/W when averaging, else 1
+float sim_prescale(std::optional<double> prescale, bool average, int W) {
+  return prescale ? (float)*prescale : average ? 1.0f / (float)W : 1.0f;
+}
+
 void py_sra_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int lanes,
                      bool average, bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                     int64_t min_lane_elems) {
+                     int64_t min_lane_elems, std::optional<double> prescale) {
   TORCH_CHECK(!tensors.empty(), "need tensors");
   const int W = (int)tensors.size();
   const int dt = cgx_dtype(tensors[0]);
@@ -142,12 +149,12 @@ void py_sra_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTup
     bufs.push_back(t.data_ptr());
   }
   Plan plan = build_plan(to_layers(layers), make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
-  sra_simulate(plan, bufs, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
+  sra_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
 }
 
 void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int lanes,
                          bool average, bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                         int64_t min_lane_elems) {
+                         int64_t min_lane_elems, std::optional<double> prescale) {
   TORCH_CHECK(!tensors.empty(), "need tensors");
   const int W = (int)tensors.size();
   const int dt = cgx_dtype(tensors[0]);
@@ -157,7 +164,7 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
     bufs.push_back(t.data_ptr());
   }
   Plan plan = build_plan(to_layers(layers), make_opts(1, lanes, dt, skip_incomplete, min_lane_elems));
-  oneshot_simulate(plan, bufs, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
+  oneshot_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
 }
 
 // Argument checks of the sharded simulators: one CPU contiguous input and output per rank, all of
@@ -525,12 +532,13 @@ class LocalReducerGroup {
     cuda_.clear();
   }
 
-  // in-place allreduce of one tensor per virtual rank; the prescale is 1/W when averaging
+  // in-place allreduce of one tensor per virtual rank; the prescale is 1/W when averaging unless given
   void allreduce(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
-                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
+                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
+                 std::optional<double> prescale_in) {
     const auto specs = to_layers(layers);
     const RngParams rng = make_rng(stochastic, seed, seq);
-    const float prescale = average ? 1.0f / (float)hub_.world() : 1.0f;
+    const float prescale = sim_prescale(prescale_in, average, hub_.world());
     run(tensors, [&](Reducer& red, void* data, int dt, cudaStream_t s) {
       red.allreduce(data, dt, specs, skip_incomplete, prescale, rng, s);
     });
@@ -651,6 +659,319 @@ class LocalReducerGroup {
   std::vector<c10::cuda::CUDAStream> streams_;
   std::vector<Rank> cpu_, cuda_;
   std::vector<int64_t> last_sent_;
+};
+
+// W AllreduceEngines in one process, `local_size` consecutive virtual ranks per node, wired as
+// ProcessGroupCGX wires them: per node a set of connect_local heaps (the fused kernels) and one
+// loopback hub (the generic intra-node reducers and broadcasts), per local rank one loopback hub
+// across the nodes (the cross-node reducers), for host and for device memory. Each rank's call runs
+// on its own host thread and stream. An observer logs every stage the engine issues, and before a
+// fused launch waits until every rank of the node has reached the same launch: the ranks share one
+// CUDA context, where one rank's plan upload or cudaFree can wait for a peer's kernel that spins
+// until this rank launches.
+class LocalEngineGroup {
+ public:
+  LocalEngineGroup(int world, int local_size, const py::dict& config, int lanes, int64_t slot_bytes,
+                   int64_t timeout_ms)
+      : world_(world), local_size_(local_size) {
+    TORCH_CHECK(world >= 1 && world <= kMaxPeers, "LocalEngineGroup: world must be 1..", kMaxPeers, ", got ", world);
+    TORCH_CHECK(local_size >= 1 && world % local_size == 0, "LocalEngineGroup: local_size ", local_size,
+                " does not divide the world ", world);
+    // streams r and r + 8 share a hardware queue: a rank's kernel could wait behind a peer's that spins for it
+    TORCH_CHECK(local_size <= 8, "LocalEngineGroup: at most 8 ranks per node, got ", local_size);
+    TORCH_CHECK(lanes >= 1, "LocalEngineGroup: lanes must be positive");
+    EngineConfig cfg = EngineConfig::read();
+    cfg.timeout_ms = timeout_ms;
+    cfg.lanes = lanes;
+    cfg.local_size = local_size;
+    bool p2p = true;
+    for (const auto& kv : config) {
+      const std::string k = py::cast<std::string>(kv.first);
+      const py::handle v = kv.second;
+      if (k == "fusion_bytes") cfg.fusion_bytes = py::cast<int64_t>(v);
+      else if (k == "oneshot_max_bytes") cfg.oneshot_max_bytes = py::cast<int64_t>(v);
+      else if (k == "min_lane_elems") cfg.min_lane_elems = py::cast<uint32_t>(v);
+      else if (k == "min_compress_elems") cfg.min_compress_elems = py::cast<int>(v);
+      else if (k == "inner_reduction") cfg.inner_reduction = reduction(py::cast<std::string>(v));
+      else if (k == "cross_reduction") cfg.cross_reduction = reduction(py::cast<std::string>(v));
+      else if (k == "intra_broadcast") cfg.intra_broadcast = py::cast<bool>(v);
+      else if (k == "intra_compress") cfg.intra_compress = py::cast<bool>(v);
+      else if (k == "dummy_compression") cfg.dummy_compression = py::cast<bool>(v);
+      else if (k == "overlap_lanes") cfg.overlap_lanes = py::cast<int>(v);
+      else if (k == "p2p") p2p = py::cast<bool>(v);
+      else TORCH_CHECK(false, "LocalEngineGroup: unknown config key '", k, "'");
+    }
+    // without heaps the intra-node stage runs the generic reducers
+    cfg.inner_comm = p2p ? CommType::kP2P : CommType::kNCCL;
+    cfg.fake_ratio = 1.0;
+    const int nodes = world / local_size;
+    if (p2p) {
+      // every heap's CTAs spin on their peers': all of them must be resident at once, with room to
+      // spare for the generic reducers' kernels. The nodes' kernels run side by side on this one GPU.
+      int resident = std::numeric_limits<int>::max();
+      for (int dt : {kF32, kF16, kBF16}) resident = std::min(resident, sra_max_resident_ctas(dt));
+      TORCH_CHECK((int64_t)world * lanes <= resident / 2, "LocalEngineGroup: ", world, " ranks x ", lanes,
+                  " lanes cannot all be resident (", resident, " CTAs, half of them usable)");
+      TORCH_CHECK(cudaGetDevice(&device_) == cudaSuccess, "LocalEngineGroup: no CUDA device");
+    }
+    for (int n = 0; n < nodes; ++n) intra_hubs_.push_back(std::make_unique<LoopbackHub>(local_size, timeout_ms));
+    for (int l = 0; l < local_size; ++l) cross_hubs_.push_back(std::make_unique<LoopbackHub>(nodes, timeout_ms));
+    for (int r = 0; r < world; ++r) {
+      auto e = std::make_unique<AllreduceEngine>(r, world, cfg);
+      e->set_topology(local_size);
+      for (bool cuda : {false, true}) {
+        std::unique_ptr<Communicator> intra, cross;
+        if (local_size > 1) intra = std::make_unique<LoopbackCommunicator>(intra_hub(r), e->local_rank(), cuda);
+        if (nodes > 1) cross = std::make_unique<LoopbackCommunicator>(cross_hub(r), e->node(), cuda);
+        e->attach_generic(cuda, std::move(intra), std::move(cross));
+      }
+      engines_.push_back(std::move(e));
+      observers_.push_back(std::make_unique<Observer>(this, r));
+      engines_[r]->set_observer(observers_[r].get());
+    }
+    if (p2p) {
+      layout_ = HeapLayout::make(local_size, lanes, (size_t)slot_bytes,
+                                 AllreduceEngine::required_oneshot_slot_bytes(cfg));
+      for (int n = 0; n < nodes; ++n) {
+        std::vector<std::unique_ptr<SymmetricHeap>> heaps;
+        std::vector<SymmetricHeap*> all;
+        for (int l = 0; l < local_size; ++l) {
+          heaps.push_back(std::make_unique<SymmetricHeap>(l, local_size, layout_));
+          all.push_back(heaps.back().get());
+        }
+        for (auto& h : heaps) h->connect_local(all);
+        for (int l = 0; l < local_size; ++l) engines_[n * local_size + l]->attach_heap(std::move(heaps[l]), lanes);
+      }
+    }
+  }
+  ~LocalEngineGroup() {
+    std::optional<c10::cuda::CUDAGuard> g;
+    if (device_ >= 0) g.emplace((c10::DeviceIndex)device_);
+    engines_.clear();
+  }
+
+  void allreduce(std::vector<at::Tensor> tensors, bool average, int explicit_bucket, bool overlapped) {
+    run(tensors, [&](AllreduceEngine& e, int, void* data, int dt, int64_t n, bool cuda, cudaStream_t s) {
+      if (cuda)
+        e.allreduce_cuda(data, dt, n, average, explicit_bucket, s, overlapped);
+      else
+        e.allreduce_cpu(data, dt, n, average, explicit_bucket);
+    });
+  }
+  void allreduce_layers(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average) {
+    const auto specs = to_layers(layers);
+    run(tensors, [&](AllreduceEngine& e, int, void* data, int dt, int64_t, bool cuda, cudaStream_t s) {
+      AllreduceEngine::CpuCall call;
+      call.env = CompressionEnv::read();
+      call.layers = specs;
+      if (cuda)
+        e.allreduce_cuda_layers(data, dt, specs, average, call.env, s);
+      else
+        e.allreduce_cpu_prepared(data, dt, call, average);
+    });
+  }
+  // inputs[r] / outputs[r]: rank r's buffers of the reduce-scatter (W * S -> S) or the all-gather
+  // (S -> W * S); one layer of S elements with the environment's width and bucket size
+  void sharded(bool reduce_scatter, std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, bool average) {
+    const ShardedOp op = reduce_scatter ? ShardedOp::kReduceScatter : ShardedOp::kAllGather;
+    TORCH_CHECK((int)outputs.size() == world_, "LocalEngineGroup: one output per virtual rank");
+    const CompressionEnv env = CompressionEnv::read();
+    RngParams rng = make_rng(env.stochastic, env.seed, 0);
+    run(inputs, [&](AllreduceEngine& e, int r, void* in, int dt, int64_t n, bool cuda, cudaStream_t s) {
+      TORCH_CHECK(cuda && outputs[r].is_cuda() && outputs[r].is_contiguous() && cgx_dtype(outputs[r]) == dt,
+                  "LocalEngineGroup: the sharded collectives take contiguous CUDA tensors of one dtype");
+      const int64_t S = reduce_scatter ? outputs[r].numel() : n;
+      TORCH_CHECK((reduce_scatter ? n : outputs[r].numel()) == S * world_, "LocalEngineGroup: the full buffer holds W x S");
+      // upload every window's plan and wait for it before any rank launches (see the class comment)
+      LayerSpec l;
+      l.numel = (uint64_t)S;
+      l.bits = compression_enabled(S, env.bits, e.config().min_compress_elems) ? env.bits : kRawBits;
+      l.bucket = (uint32_t)std::max(1, env.bucket_size);
+      if (e.fused()) {
+        e.fused()->prepare_sharded({l}, dt, env.skip_incomplete, s);
+        cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: plan upload");
+        intra_hub(r)->barrier(e.local_rank());
+      }
+      e.sharded_cuda(op, in, outputs[r].data_ptr(), dt, S, {}, average, env.bits, env.bucket_size,
+                     env.skip_incomplete, rng, s, false);
+    });
+  }
+
+  py::dict stats(int r) const {
+    TORCH_CHECK(r >= 0 && r < world_, "LocalEngineGroup: bad rank ", r);
+    const EngineStats& s = engines_[r]->stats();
+    py::dict d;
+    d["calls"] = s.calls;
+    d["kernel_launches"] = s.kernel_launches;
+    d["elements"] = s.elements;
+    d["wire_bytes"] = s.wire_bytes;
+    d["raw_bytes"] = s.raw_bytes;
+    return d;
+  }
+  void check() {
+    for (auto& e : engines_) e->check_health();
+  }
+  // the stages rank r issued in the last call, in order
+  py::list log(int r) const {
+    TORCH_CHECK(r >= 0 && r < world_, "LocalEngineGroup: bad rank ", r);
+    py::list out;
+    for (const Entry& e : observers_[r]->log) {
+      py::dict d;
+      d["kind"] = e.kind;
+      d["layers"] = e.layers;
+      d["lanes"] = e.lanes;
+      d["numel"] = e.numel;
+      d["seed"] = e.seed;
+      d["seq"] = e.seq;
+      d["stochastic"] = e.stochastic;
+      d["scale"] = e.scale;
+      out.append(d);
+    }
+    return out;
+  }
+  // (slot bytes, one-shot slot bytes) of the heaps; (0, 0) without them
+  std::pair<int64_t, int64_t> slot_bytes() const {
+    return {(int64_t)layout_.slot_bytes, (int64_t)layout_.os_slot_bytes};
+  }
+  int64_t num_plans(int r) const {
+    TORCH_CHECK(r >= 0 && r < world_, "LocalEngineGroup: bad rank ", r);
+    return engines_[r]->fused() ? (int64_t)engines_[r]->fused()->num_plans() : 0;
+  }
+
+ private:
+  struct Entry {
+    std::string kind;
+    std::vector<LayerTuple> layers;
+    int64_t lanes = 0, numel = 0;
+    uint64_t seed = 0;
+    uint32_t seq = 0;
+    bool stochastic = false;
+    float scale = 1.0f;
+  };
+  struct Observer : EngineObserver {
+    Observer(LocalEngineGroup* g, int r) : group(g), rank(r) {}
+    void before_fused_launch(const DevicePlan&, cudaStream_t stream) override {
+      FusedSra* f = group->engines_[rank]->fused();
+      if (f->num_plans() != plans_seen || f->generation() != generation_seen) {
+        cuda_check(cudaStreamSynchronize(stream), "LocalEngineGroup: plan upload");
+        plans_seen = f->num_plans();
+        generation_seen = f->generation();
+      }
+      group->intra_hub(rank)->barrier(group->engines_[rank]->local_rank());
+    }
+    void stage(const EngineStage& s) override {
+      static const char* kNames[] = {"oneshot", "sra", "generic_intra", "cross", "bcast_compressed", "bcast_raw"};
+      Entry e;
+      e.kind = kNames[s.kind];
+      if (s.layers)
+        for (const LayerSpec& l : *s.layers)
+          e.layers.emplace_back((int64_t)l.elem_off, (int64_t)l.numel, (int64_t)l.bits, (int64_t)l.bucket);
+      if (s.dp) {
+        e.lanes = s.dp->plan.lanes;
+        e.numel = (int64_t)s.dp->plan.numel;
+      } else {
+        for (const LayerSpec& l : *s.layers) e.numel += (int64_t)l.numel;
+      }
+      e.seed = s.rng.seed;
+      e.seq = s.rng.seq;
+      e.stochastic = s.rng.stochastic;
+      e.scale = s.scale;
+      log.push_back(std::move(e));
+    }
+    LocalEngineGroup* group;
+    int rank;
+    size_t plans_seen = 0;
+    uint64_t generation_seen = 0;
+    std::vector<Entry> log;
+  };
+
+  static ReductionType reduction(const std::string& k) {
+    if (k == "SRA") return ReductionType::kSRA;
+    if (k == "RING") return ReductionType::kRing;
+    if (k == "ALLTOALL") return ReductionType::kAllToAll;
+    TORCH_CHECK(false, "LocalEngineGroup: a reduction is SRA, RING or ALLTOALL, got ", k);
+    return ReductionType::kSRA;
+  }
+  LoopbackHub* intra_hub(int r) const { return intra_hubs_[r / local_size_].get(); }
+  LoopbackHub* cross_hub(int r) const { return cross_hubs_[r % local_size_].get(); }
+  void fail_all(const std::string& msg) {
+    for (auto& h : intra_hubs_) h->fail(msg);
+    for (auto& h : cross_hubs_) h->fail(msg);
+  }
+
+  // op(engine, rank, data, dtype, numel, cuda, stream) on every rank's thread; every rank's stream is
+  // synchronised before this returns, and the first failure of any rank is raised
+  template <class F>
+  void run(const std::vector<at::Tensor>& tensors, F&& op) {
+    const int W = world_;
+    TORCH_CHECK((int)tensors.size() == W, "LocalEngineGroup: need one tensor per virtual rank (", W, "), got ",
+                tensors.size());
+    const int dt = cgx_dtype(tensors[0]);
+    const bool cuda = tensors[0].is_cuda();
+    for (const at::Tensor& t : tensors)
+      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && t.numel() == tensors[0].numel() &&
+                      t.device() == tensors[0].device(),
+                  "LocalEngineGroup: contiguous tensors of one dtype, size and device");
+    TORCH_CHECK(cuda || tensors[0].device().is_cpu(), "LocalEngineGroup: CPU or CUDA tensors");
+    c10::cuda::OptionalCUDAGuard guard;
+    if (cuda) {
+      const int dev = tensors[0].device().index();
+      TORCH_CHECK(device_ < 0 || device_ == dev, "LocalEngineGroup: all calls use one device (", device_, ")");
+      device_ = dev;
+      guard.set_index((c10::DeviceIndex)device_);
+      if (streams_.empty())
+        for (int r = 0; r < W; ++r) streams_.push_back(c10::cuda::getStreamFromPool(false, (c10::DeviceIndex)device_));
+      at::cuda::CUDAEvent ready(cudaEventDisableTiming);
+      ready.record(c10::cuda::getCurrentCUDAStream());
+      for (auto& s : streams_) ready.block(s);
+    }
+    for (auto& h : intra_hubs_) h->reset(false);
+    for (auto& h : cross_hubs_) h->reset(false);
+    for (auto& o : observers_) o->log.clear();
+    const int64_t n = tensors[0].numel();
+    {
+      py::gil_scoped_release nogil;
+      std::vector<std::thread> threads;
+      for (int r = 0; r < W; ++r)
+        threads.emplace_back([&, r] {
+          try {
+            c10::cuda::OptionalCUDAGuard g;
+            cudaStream_t s = nullptr;
+            if (cuda) {
+              g.set_index((c10::DeviceIndex)device_);
+              s = streams_[r].stream();
+            }
+            op(*engines_[r], r, tensors[r].data_ptr(), dt, n, cuda, s);
+            if (cuda) cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: synchronise a virtual rank");
+          } catch (const std::exception& e) {
+            fail_all("rank " + std::to_string(r) + ": " + e.what());
+          } catch (...) {
+            fail_all("rank " + std::to_string(r) + ": unknown exception");
+          }
+          intra_hub(r)->finish(engines_[r]->local_rank());
+          cross_hub(r)->finish(engines_[r]->node());
+        });
+      for (auto& t : threads) t.join();
+      // a rank that threw skipped its own synchronise: nothing it queued may run on after this returns
+      if (cuda)
+        for (int r = 0; r < W; ++r) {
+          const cudaError_t err = cudaStreamSynchronize(streams_[r].stream());
+          if (err != cudaSuccess)
+            fail_all("rank " + std::to_string(r) + ": synchronise after the call: " + cudaGetErrorString(err));
+        }
+    }
+    for (auto& h : intra_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
+    for (auto& h : cross_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
+    if (cuda) check();
+  }
+
+  int world_, local_size_;
+  int device_ = -1;
+  HeapLayout layout_{};
+  std::vector<std::unique_ptr<LoopbackHub>> intra_hubs_, cross_hubs_;
+  std::vector<std::unique_ptr<AllreduceEngine>> engines_;  // after the hubs: released first
+  std::vector<std::unique_ptr<Observer>> observers_;
+  std::vector<c10::cuda::CUDAStream> streams_;
 };
 
 // ---- ResNet residual join: every operand like `ref` (device, dtype, sizes, strides), all dense ----
@@ -1037,7 +1358,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   m.def("sra_simulate", &py_sra_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
+        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
   m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
         py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
@@ -1045,7 +1366,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0);
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
+        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
   m.def("quantize", &py_quantize, py::arg("tensor"), py::arg("layers"), py::arg("world") = 1, py::arg("lanes") = 1,
         py::arg("skip_incomplete") = false, py::arg("prescale") = 1.0f, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("rank") = 0, py::arg("phase") = 0,
@@ -1148,13 +1469,35 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("timeout_ms") = 10000)
       .def("allreduce", &LocalReducerGroup::allreduce, py::arg("tensors"), py::arg("layers"),
            py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-           py::arg("seed") = 0, py::arg("seq") = 0)
+           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none())
       .def("broadcast_compressed", &LocalReducerGroup::broadcast_compressed, py::arg("tensors"), py::arg("layers"),
            py::arg("root"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0)
       .def("bytes_sent", &LocalReducerGroup::bytes_sent)
       .def("set_recording", &LocalReducerGroup::set_recording, py::arg("on"))
       .def("messages", &LocalReducerGroup::messages);
+  py::class_<LocalEngineGroup>(m, "LocalEngineGroup")
+      .def(py::init<int, int, const py::dict&, int, int64_t, int64_t>(), py::arg("world"), py::arg("local_size"),
+           py::arg("config"), py::arg("lanes") = 2, py::arg("slot_bytes") = 1 << 20, py::arg("timeout_ms") = 20000)
+      .def("allreduce", &LocalEngineGroup::allreduce, py::arg("tensors"), py::arg("average") = false,
+           py::arg("explicit_bucket") = -1, py::arg("overlapped") = false)
+      .def("allreduce_layers", &LocalEngineGroup::allreduce_layers, py::arg("tensors"), py::arg("layers"),
+           py::arg("average") = false)
+      .def("reduce_scatter",
+           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out, bool average) {
+             g.sharded(true, std::move(in), std::move(out), average);
+           },
+           py::arg("inputs"), py::arg("outputs"), py::arg("average") = false)
+      .def("all_gather",
+           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out) {
+             g.sharded(false, std::move(in), std::move(out), false);
+           },
+           py::arg("inputs"), py::arg("outputs"))
+      .def("stats", &LocalEngineGroup::stats, py::arg("rank"))
+      .def("check", &LocalEngineGroup::check)
+      .def("log", &LocalEngineGroup::log, py::arg("rank"))
+      .def("slot_bytes", &LocalEngineGroup::slot_bytes)
+      .def("num_plans", &LocalEngineGroup::num_plans, py::arg("rank"));
 
   m.attr("MAX_BLOCK_ELEMS") = (int64_t)kMaxBlockElems;
   m.attr("MAX_PEERS") = (int64_t)kMaxPeers;

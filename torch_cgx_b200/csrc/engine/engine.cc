@@ -104,10 +104,15 @@ static std::vector<LayerSpec> resolve_layers(int64_t numel, const EngineConfig& 
   return LayerRegistry::instance().extract(n_eff, env, cfg.min_compress_elems, explicit_bucket, &resolved);
 }
 
-void AllreduceEngine::launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream) {
+void AllreduceEngine::launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream,
+                                   const std::vector<LayerSpec>* layers) {
   const int elsize = dtype_size(l.dp->plan.dtype);
   rng.seq = (rng.seq << 3) | (l.rng_sub & 7u);
   const int lw = fused_->world(), lr = fused_->rank();
+  if (observer_) {
+    observer_->stage(EngineStage{l.oneshot ? EngineStage::kOneshot : EngineStage::kSra, layers, l.dp, rng, prescale});
+    observer_->before_fused_launch(*l.dp, stream);
+  }
   if (l.oneshot) {
     fused_->run_oneshot(*l.dp, data, prescale, rng, stream);
     stats_.wire_bytes += l.dp->plan.total_wire * (uint64_t)(lw - 1);
@@ -146,11 +151,9 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
       rng.seed = env.seed;
       rng.stochastic = env.stochastic;
       const float prescale = average ? 1.0f / (float)world_ : 1.0f;
-      uint32_t sub = 0;
-      const DevicePlan* prev_group = nullptr;
-      (void)prev_group;
+      // the sequence numbers of the slow path: fusion group in the call's, piece in the launch's
       for (const Launch& l : f.launches) {
-        rng.seq = (call_seq_ << 4) | ((sub++) & 15u);
+        rng.seq = (call_seq_ << 4) | (l.rng_group & 15u);
         launch_fused(l, data, prescale, rng, stream);
       }
       return;
@@ -276,7 +279,7 @@ void AllreduceEngine::intra_stage(bool cuda, void* data, int dtype, const std::v
         const DevicePlan* dp = fused_->prepare_oneshot(group, dtype, skip_incomplete, stream, lane_cap_);
         // every rank pushes its whole packed image to W-1 peers: keep that egress small
         if (dp != nullptr && dp->plan.total_wire * (uint64_t)(fused_->world() - 1) <= (4ull << 20)) {
-          launch_fused(Launch{dp, true, 0u}, data, prescale, rng, stream);
+          launch_fused(Launch{dp, true, rng.seq & 15u, 0u}, data, prescale, rng, stream, &group);
           return;
         }
       }
@@ -309,12 +312,13 @@ void AllreduceEngine::intra_stage(bool cuda, void* data, int dtype, const std::v
         }
         continue;
       }
-      launch_fused(Launch{dp, false, sub++}, data, prescale, rng, stream);
+      launch_fused(Launch{dp, false, rng.seq & 15u, sub++}, data, prescale, rng, stream, &gl);
     }
     return;
   }
   if (g.intra) {
     const uint64_t before = g.intra->bytes_sent();
+    observe(EngineStage::kGenericIntra, &group, rng, prescale);
     g.intra->allreduce(data, dtype, group, skip_incomplete, prescale, rng, stream);
     stats_.wire_bytes += g.intra->bytes_sent() - before;
     uint64_t n = 0;
@@ -360,7 +364,10 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
     crng.seq = rng.seq ^ 0x40000000u;
     const float cross_scale = (local_size_ > 1) ? 1.0f : prescale;
     if (cfg_.intra_broadcast && local_size_ > 1) {
-      if (local_rank() == 0) g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream);
+      if (local_rank() == 0) {
+        observe(EngineStage::kCross, &group, crng, cross_scale);
+        g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream);
+      }
       // leaders hand the result to the rest of their node: packed when the intra-node stage
       // compresses (reference: Reducer::Broadcast with do_compression && intra_compress_,
       // mpi_allreduce_operations.cc:171-176, reducer.cc:96-160), raw bytes of the span otherwise
@@ -370,6 +377,7 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
         RngParams brng = rng;
         brng.seq = rng.seq ^ 0x20000000u;
         const uint64_t before = g.intra->bytes_sent();
+        observe(EngineStage::kBcastCompressed, &group, brng, 1.0f);
         g.intra->broadcast_compressed(data, dtype, group, env.skip_incomplete, 0, brng, stream);
         stats_.wire_bytes += g.intra->bytes_sent() - before;
       } else {
@@ -378,10 +386,13 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
           lo = std::min<uint64_t>(lo, l.elem_off);
           hi = std::max<uint64_t>(hi, l.elem_off + l.numel);
         }
-        if (hi > lo && g.intra)
+        if (hi > lo && g.intra) {
+          observe(EngineStage::kBcastRaw, &group, rng, 1.0f);
           g.intra->broadcast(static_cast<uint8_t*>(data) + lo * elsize, (size_t)(hi - lo) * elsize, 0, stream);
+        }
       }
     } else {
+      observe(EngineStage::kCross, &group, crng, cross_scale);
       g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream);
     }
   }

@@ -38,6 +38,25 @@ struct EngineStats {
 std::vector<std::vector<LayerSpec>> split_for_fusion(const std::vector<LayerSpec>& layers, int elsize,
                                                      int64_t fusion_bytes);
 
+// One stage of an allreduce as the engine issues it (EngineObserver::stage).
+struct EngineStage {
+  enum Kind { kOneshot, kSra, kGenericIntra, kCross, kBcastCompressed, kBcastRaw };
+  Kind kind;
+  const std::vector<LayerSpec>* layers;  // the stage's layer table; null for a fused launch of the bucket fast path
+  const DevicePlan* dp;                  // the plan of a fused launch (kOneshot / kSra), else null
+  RngParams rng;                         // the sequence number the stage runs with
+  float scale;                           // prescale of an allreduce stage, 1 for a broadcast
+};
+
+// Test seam: sees every stage an engine issues. Production engines have none (one branch per stage).
+class EngineObserver {
+ public:
+  virtual ~EngineObserver() = default;
+  // right before a fused kernel launch, slow and fast path alike
+  virtual void before_fused_launch(const DevicePlan& dp, cudaStream_t stream) = 0;
+  virtual void stage(const EngineStage& s) = 0;
+};
+
 // Reducers of one memory kind (host or device): the generic intra-node and
 // cross-node stages of the hierarchical allreduce.
 struct GenericPath {
@@ -115,6 +134,7 @@ class AllreduceEngine {
                     const RngParams& rng_in, cudaStream_t stream, bool overlapped);
 
   void check_health();
+  void set_observer(EngineObserver* o) { observer_ = o; }
   const EngineStats& stats() const { return stats_; }
   void reset_stats() { stats_ = EngineStats(); }
 
@@ -130,7 +150,8 @@ class AllreduceEngine {
   struct Launch {
     const DevicePlan* dp;
     bool oneshot;
-    uint32_t rng_sub;  // low bits of the RNG sequence used for this launch
+    uint32_t rng_group;  // fusion group of this launch (low bits of the call's RNG sequence)
+    uint32_t rng_sub;    // piece of the group (low bits of the launch's RNG sequence)
   };
   struct BucketFast {
     uint64_t registry_version = 0;
@@ -144,7 +165,11 @@ class AllreduceEngine {
   };
   std::vector<BucketFast> fast_;
   std::vector<Launch>* recording_ = nullptr;
-  void launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream);
+  void launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream,
+                    const std::vector<LayerSpec>* layers = nullptr);
+  void observe(EngineStage::Kind kind, const std::vector<LayerSpec>* layers, const RngParams& rng, float scale) {
+    if (observer_) observer_->stage(EngineStage{kind, layers, nullptr, rng, scale});
+  }
 
   int rank_, world_;
   int local_size_;
@@ -156,6 +181,7 @@ class AllreduceEngine {
   uint32_t call_seq_ = 0;
   int lane_cap_ = 0;  // lane cap of the call being issued (0 = none)
   EngineStats stats_;
+  EngineObserver* observer_ = nullptr;
 };
 
 }  // namespace cgx

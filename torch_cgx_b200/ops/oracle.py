@@ -203,7 +203,11 @@ def block_owners(layers: Sequence[Layer], numel: int, world: int, lanes: int, dt
     return owner
 
 
-def _prescale(world: int, average: bool) -> _F32:
+def _prescale(world: int, average: bool, prescale: float | None = None) -> _F32:
+    """The factor every contribution is multiplied by first: ``prescale`` when given, else 1/world
+    when averaging, else 1."""
+    if prescale is not None:
+        return _F32(prescale)
     return _F32(1.0) / _F32(world) if average else _F32(1.0)
 
 
@@ -249,7 +253,7 @@ def _sra_acc(xs: Sequence[np.ndarray], sl: slice, own: np.ndarray, bits: int, bu
 
 def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, world: int | None = None,
                   lanes: int = 1, min_lane_elems: int = 2048, average: bool = False,
-                  skip_incomplete: bool = False) -> List[torch.Tensor]:
+                  skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
     """Every rank's result of the deterministic compressed SRA allreduce (DESIGN §2.3).
 
     For each bucket, the owner c (the rank whose chunk holds it) forms in fp32
@@ -263,7 +267,7 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
     assert world is None or world == W
     dtype = inputs[0].dtype
     n = inputs[0].numel()
-    xs = _scaled_inputs(inputs, _prescale(W, average))
+    xs = _scaled_inputs(inputs, _prescale(W, average, prescale))
     owner = block_owners(layers, n, W, lanes, dtype, skip_incomplete, min_lane_elems)
     outs = [t.detach().reshape(-1).float().cpu().numpy().copy() for t in inputs]
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
@@ -275,13 +279,13 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
 
 
 def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
-                      skip_incomplete: bool = False) -> List[torch.Tensor]:
+                      skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
     """Every rank's result of the one-shot allreduce: each contribution, the own one included,
     is quantized once (raw runs: rounded to the dtype) and the decoded values are summed in
     fp32 in rank order starting from +0; no second quantization, one rounding to the dtype."""
     W = len(inputs)
     dtype = inputs[0].dtype
-    xs = _scaled_inputs(inputs, _prescale(W, average))
+    xs = _scaled_inputs(inputs, _prescale(W, average, prescale))
     outs = [t.detach().reshape(-1).float().cpu().numpy().copy() for t in inputs]
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
         sl = slice(off, off + m)
@@ -313,7 +317,7 @@ def _own_values(inputs: Sequence[torch.Tensor]) -> List[np.ndarray]:
 
 
 def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
-                   skip_incomplete: bool = False) -> List[torch.Tensor]:
+                   skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
     """Every rank's result of the compressed Ring allreduce (``RingReducer``, deterministic rounding).
 
     Chunk c is rank c's chunk of the lanes = 1 plan. Rank r starts with acc_r = prescale*x_r in fp32.
@@ -328,7 +332,7 @@ def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, a
     n = inputs[0].numel()
     segs = layer_segments(layers, skip_incomplete)
     chunk = block_owners(layers, n, W, 1, dtype, skip_incomplete, GENERIC_MIN_LANE_ELEMS)
-    acc = _scaled_inputs(inputs, _prescale(W, average))
+    acc = _scaled_inputs(inputs, _prescale(W, average, prescale))
     with np.errstate(all="ignore"):
         for s in range(W - 1):
             sent = [_quantized(a, segs, dtype) for a in acc]  # every rank sends before it adds
@@ -346,7 +350,7 @@ def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, a
 
 
 def alltoall_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
-                       skip_incomplete: bool = False) -> List[torch.Tensor]:
+                       skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
     """Every rank's result of the debug all-to-all allreduce (``AllToAllReducer``, deterministic):
     rank r keeps prescale*x_r unquantized and adds, in fp32 and in ascending rank order, every
     peer's Q(prescale*x_q); the sum is stored in the dtype once. The ranks' results differ.
@@ -354,7 +358,7 @@ def alltoall_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], 
     W = len(inputs)
     dtype = inputs[0].dtype
     segs = layer_segments(layers, skip_incomplete)
-    xs = _scaled_inputs(inputs, _prescale(W, average))
+    xs = _scaled_inputs(inputs, _prescale(W, average, prescale))
     qs = [_quantized(x, segs, dtype) for x in xs]
     outs = _own_values(inputs)
     with np.errstate(all="ignore"):
@@ -384,6 +388,194 @@ def broadcast_compressed_reference(inputs: Sequence[torch.Tensor], layers: Seque
             for off, m, _, _ in segs:
                 o[off:off + m] = q[off:off + m]
     return _to_tensors(outs, dtype)
+
+
+# ---- the allreduce engine (engine/engine.cc): stages composed from the references above ------------
+ENGINE_DEFAULTS = dict(fusion_bytes=64 << 20, oneshot_max_bytes=2 << 20, min_lane_elems=4096, min_compress_elems=16,
+                       inner_reduction="SRA", cross_reduction="RING", intra_broadcast=True, intra_compress=True,
+                       dummy_compression=False, overlap_lanes=64, p2p=True)
+ONESHOT_MAX_EGRESS = 4 << 20  # a one-shot rank pushes its packed image to every peer: at most this many bytes
+_U32 = 0xFFFFFFFF
+_ELSIZE = {torch.float32: 4, torch.float16: 2, torch.bfloat16: 2}
+ENGINE_PERTURBATIONS = ("prescale_local", "raw_broadcast", "cross_seq_unmarked", "oneshot_shifted")
+
+
+def _generic_allreduce(kind, ins, layers, *, prescale, skip_incomplete, stochastic, seed, seq):
+    """One generic reducer's allreduce over ``ins`` (one tensor per rank of its group)."""
+    if stochastic:
+        from .. import _C
+
+        out = [t.clone() for t in ins]
+        _C.LocalReducerGroup(len(ins), kind, 20_000).allreduce(out, layers, False, skip_incomplete, True, seed, seq,
+                                                               prescale=float(prescale))
+        return out
+    kw = dict(skip_incomplete=skip_incomplete, prescale=prescale)
+    if kind == "SRA":
+        return sra_reference(ins, layers, lanes=1, min_lane_elems=GENERIC_MIN_LANE_ELEMS, **kw)
+    if kind == "RING":
+        return ring_reference(ins, layers, **kw)
+    return alltoall_reference(ins, layers, **kw)
+
+
+def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, local_size: int, config: dict,
+                     lanes: int, slot_bytes: Tuple[int, int] = (0, 0), average: bool = False, call_seq: int = 1,
+                     cuda: bool = True, overlapped: bool = False, skip_incomplete: bool = False,
+                     stochastic: bool = False, seed: int = 0, perturb: str | None = None):
+    """Every rank's result of one ``AllreduceEngine`` allreduce over ``layers`` and the stages each
+    rank issues, ``(outputs, stages)``; ``stages[r]`` is a list of dicts (kind, layers, lanes, numel,
+    seed, seq, stochastic, scale) in the order rank r issues them.
+
+    The stages follow engine.cc, written out here from the configuration (keys of
+    ``ENGINE_DEFAULTS``) rather than read from a run. ``local_size`` consecutive ranks form a node.
+    Layers are cut into fusion groups (``split_for_fusion``); group g of call ``call_seq`` runs with
+    RNG sequence ``call_seq << 4 | (g & 15)`` and, per group:
+      1. inside the node (skipped when nodes have one rank and there are several nodes): with every
+         rank's contribution prescaled by 1/W when averaging. With ``cuda`` and heaps (``p2p``), and
+         the SRA or no intra-node reducer, the fused kernel: the one-shot kernel when the group
+         fits ``oneshot_max_bytes``, its single-chunk plan the one-shot slot and its egress 4 MiB;
+         otherwise the three-phase SRA of each piece of the group, halving (by layers, then at
+         bucket boundaries) every piece whose plan does not fit the slot, pieces numbered in launch
+         order into the low 3 bits of ``seq << 3``. Else the generic ``inner_reduction``. With
+         several nodes and no ``intra_compress`` this stage sends every layer raw.
+      2. across nodes, between the ranks of one local rank, with ``seq ^ 0x40000000`` and scale 1
+         (1/W when nodes have one rank): the node leaders only with ``intra_broadcast``, which then
+         hand the result to their node, compressed from root 0 with ``seq ^ 0x20000000`` when the
+         intra-node stage compresses and the group has a compressed layer, else as raw bytes of
+         the group's span.
+    ``stochastic`` composes the CPU simulators (``C.sra_simulate``, ``C.oneshot_simulate`` and
+    ``C.LocalReducerGroup``) with these sequence numbers instead of the deterministic references.
+    ``perturb`` (one of ``ENGINE_PERTURBATIONS``) switches on a wrong semantics, for the tests that
+    show the reference tells it apart.
+    """
+    from .. import _C
+
+    cfg = dict(ENGINE_DEFAULTS, **config)
+    W, L = len(inputs), local_size
+    nodes = W // L
+    multi = nodes > 1
+    dtype = inputs[0].dtype
+    es = _ELSIZE[dtype]
+    dt = _DTYPE_CODE[dtype]
+    layers = [tuple(int(v) for v in l) for l in layers]
+    if cfg["dummy_compression"]:
+        layers = [(o, n, RAW_BITS, b) for o, n, _, b in layers]
+    ps = _prescale(W, average)
+    ps1 = _prescale(L, average) if perturb == "prescale_local" else ps
+    cap = cfg["overlap_lanes"] if overlapped else 0
+    plan_lanes = cap if 0 < cap < lanes else lanes
+    slot, os_slot = slot_bytes
+    fused = cuda and cfg["p2p"] and (cfg["inner_reduction"] == "SRA" or L == 1)
+    groups = _C.split_for_fusion(layers, es, cfg["fusion_bytes"])
+    oneshot_limit = cfg["oneshot_max_bytes"]
+    if perturb == "oneshot_shifted":  # the largest group that takes the one-shot kernel takes the SRA instead
+        fits = [sum(l[1] for l in g) * es for g in groups if sum(l[1] for l in g) * es <= oneshot_limit]
+        oneshot_limit = max(fits) - 1 if fits else oneshot_limit
+    state = [t.detach().reshape(-1).cpu().clone() for t in inputs]
+    stages = [[] for _ in range(W)]
+
+    def log(ranks, kind, ls, seq, scale, lanes_=0, numel=None):
+        for r in ranks:
+            stages[r].append(dict(kind=kind, layers=[tuple(l) for l in ls], lanes=lanes_,
+                                  numel=sum(l[1] for l in ls) if numel is None else numel, seed=seed,
+                                  seq=seq & _U32, stochastic=stochastic, scale=float(scale)))
+
+    def node_ranks(nd):
+        return list(range(nd * L, (nd + 1) * L))
+
+    def setvals(ranks, outs):
+        for r, o in zip(ranks, outs):
+            state[r] = o.reshape(-1).clone()
+
+    def fused_pieces(gl):
+        """[(kind, layers, plan)] of one group's fused launches, in launch order."""
+        n = sum(l[1] for l in gl)
+        if L > 1 and oneshot_limit > 0 and n * es <= oneshot_limit:
+            p = _C.build_plan(gl, world=1, lanes=plan_lanes, dtype=dt, skip_incomplete=skip_incomplete,
+                              min_lane_elems=cfg["min_lane_elems"])
+            if p["max_chunk_wire"] <= os_slot and p["total_wire"] * (L - 1) <= ONESHOT_MAX_EGRESS:
+                return [("oneshot", gl, p)]
+        out, todo = [], [list(gl)]
+        while todo:
+            cur = todo.pop()
+            p = _C.build_plan(cur, world=L, lanes=plan_lanes, dtype=dt, skip_incomplete=skip_incomplete,
+                              min_lane_elems=cfg["min_lane_elems"])
+            if p["max_chunk_wire"] <= slot:
+                out.append(("sra", cur, p))
+                continue
+            if len(cur) > 1:
+                h = len(cur) // 2
+                todo += [cur[h:], cur[:h]]
+                continue
+            off, m, bits, bucket = cur[0]
+            gran = 512 if bits >= RAW_BITS else max(1, bucket)
+            assert m > gran, "fusion buffer too small for a single quantization bucket"
+            h = max(gran, (m // 2) // gran * gran)
+            todo += [[(off + h, m - h, bits, bucket)], [(off, h, bits, bucket)]]
+        return out
+
+    for g, group in enumerate(groups):
+        seq = ((call_seq << 4) | (g & 15)) & _U32
+        intra = [(o, n, RAW_BITS, b) for o, n, _, b in group] if (multi and not cfg["intra_compress"]) else group
+        if L > 1 or not multi:
+            for nd in range(nodes):
+                rk = node_ranks(nd)
+                ins = [state[r] for r in rk]
+                if fused:
+                    for sub, (kind, gl, p) in enumerate(fused_pieces(intra)):
+                        s3 = ((seq << 3) | (sub & 7)) & _U32
+                        log(rk, kind, gl, s3, ps1, p["lanes"], p["numel"])
+                        if stochastic:
+                            outs = [t.clone() for t in ins]
+                            sim = _C.oneshot_simulate if kind == "oneshot" else _C.sra_simulate
+                            sim(outs, gl, plan_lanes, False, skip_incomplete, True, seed, s3, cfg["min_lane_elems"],
+                                prescale=float(ps1))
+                        elif kind == "oneshot":
+                            outs = oneshot_reference(ins, gl, skip_incomplete=skip_incomplete, prescale=ps1)
+                        else:
+                            outs = sra_reference(ins, gl, lanes=plan_lanes, min_lane_elems=cfg["min_lane_elems"],
+                                                 skip_incomplete=skip_incomplete, prescale=ps1)
+                        ins = [o.reshape(-1) for o in outs]
+                else:
+                    log(rk, "generic_intra", intra, seq, ps1)
+                    ins = _generic_allreduce(cfg["inner_reduction"], ins, intra, prescale=ps1,
+                                             skip_incomplete=skip_incomplete, stochastic=stochastic, seed=seed,
+                                             seq=seq)
+                setvals(rk, ins)
+        if not multi:
+            continue
+        cseq = seq if perturb == "cross_seq_unmarked" else seq ^ 0x40000000
+        cscale = _F32(1.0) if L > 1 else ps
+        leaders_only = cfg["intra_broadcast"] and L > 1
+        for lr in range(1 if leaders_only else L):
+            rk = [nd * L + lr for nd in range(nodes)]
+            log(rk, "cross", group, cseq, cscale)
+            setvals(rk, _generic_allreduce(cfg["cross_reduction"], [state[r] for r in rk], group, prescale=cscale,
+                                           skip_incomplete=skip_incomplete, stochastic=stochastic, seed=seed,
+                                           seq=cseq))
+        if not leaders_only:
+            continue
+        compressed = (cfg["intra_compress"] and any(l[2] < RAW_BITS for l in group)
+                      and perturb != "raw_broadcast")
+        for nd in range(nodes):
+            rk = node_ranks(nd)
+            if compressed:
+                bseq = seq ^ 0x20000000
+                log(rk, "bcast_compressed", group, bseq, 1.0)
+                ins = [state[r] for r in rk]
+                if stochastic:
+                    outs = [t.clone() for t in ins]
+                    _C.LocalReducerGroup(L, "SRA", 20_000).broadcast_compressed(outs, group, 0, skip_incomplete,
+                                                                                True, seed, bseq)
+                else:
+                    outs = broadcast_compressed_reference(ins, group, root=0, skip_incomplete=skip_incomplete)
+                setvals(rk, outs)
+            else:
+                log(rk, "bcast_raw", group, seq, 1.0)
+                lo = min(l[0] for l in group)
+                hi = max(l[0] + l[1] for l in group)
+                for r in rk[1:]:
+                    state[r][lo:hi] = state[rk[0]][lo:hi]
+    return [s.view_as(t).to(t.dtype) for s, t in zip(state, inputs)], stages
 
 
 def _shards(inputs: Sequence[torch.Tensor], r: int) -> List[torch.Tensor]:
