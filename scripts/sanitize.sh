@@ -28,6 +28,9 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # path, a two-level hierarchy with the compressed broadcast, the sharded collectives
 ENG_SUBSET='(single_node and w2-float32) or (replays_the_slow_path and sr-2) or w4l2-SRA-RING or reduce_scatter_and_all_gather'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_engine_local_gpu.py -m gpu -x -q -k "$ENG_SUBSET"
+# the sharded collectives over several nodes: Reducer::reduce_scatter / all_gather through CudaBackend, the
+# engine's two stages with and without heaps, the one-node NCCL-transport path
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_sharded_hierarchy_gpu.py -m gpu -x -q -k "not across_nodes"
 # ResNet residual join: 16-byte and scalar paths, tails, unaligned views, with and without gb (the
 # 103 M-element layer1 shapes and the training steps are left to the normal GPU run)
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_residual_relu_gpu.py -m gpu -x -q -k "not layer1 and not training_step"

@@ -191,7 +191,7 @@ uint64_t check_sharded_simulate(ShardedOp op, const std::vector<at::Tensor>& inp
 void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                                 const std::vector<LayerTuple>& shard_layers, int lanes, bool average,
                                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                                int64_t min_lane_elems) {
+                                int64_t min_lane_elems, std::optional<double> prescale) {
   const auto shard = to_layers(shard_layers);
   const uint64_t S = check_sharded_simulate(ShardedOp::kReduceScatter, inputs, outputs, shard);
   const int W = (int)inputs.size();
@@ -203,7 +203,7 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
     out.push_back(outputs[r].data_ptr());
   }
   Plan plan = build_plan(replicate(shard, W, S), make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
-  reduce_scatter_simulate(plan, in, out, S, average ? 1.0f / (float)W : 1.0f, make_rng(stochastic, seed, seq));
+  reduce_scatter_simulate(plan, in, out, S, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
 }
 
 // All-gather oracle (ag_kernel): shard q is one quantization round trip (roundtrip_simulate) of
@@ -539,7 +539,7 @@ class LocalReducerGroup {
     const auto specs = to_layers(layers);
     const RngParams rng = make_rng(stochastic, seed, seq);
     const float prescale = sim_prescale(prescale_in, average, hub_.world());
-    run(tensors, [&](Reducer& red, void* data, int dt, cudaStream_t s) {
+    run(tensors, [&](Reducer& red, int, void* data, int dt, cudaStream_t s) {
       red.allreduce(data, dt, specs, skip_incomplete, prescale, rng, s);
     });
   }
@@ -548,8 +548,31 @@ class LocalReducerGroup {
     TORCH_CHECK(root >= 0 && root < hub_.world(), "LocalReducerGroup: bad root ", root);
     const auto specs = to_layers(layers);
     const RngParams rng = make_rng(stochastic, seed, seq);
-    run(tensors, [&](Reducer& red, void* data, int dt, cudaStream_t s) {
+    run(tensors, [&](Reducer& red, int, void* data, int dt, cudaStream_t s) {
       red.broadcast_compressed(data, dt, specs, skip_incomplete, root, rng, s);
+    });
+  }
+  // Reducer::reduce_scatter: inputs[r] holds W * S elements, outputs[r] receives shard r
+  void reduce_scatter(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
+                      const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete,
+                      bool stochastic, uint64_t seed, uint32_t seq, std::optional<double> prescale_in) {
+    const auto specs = to_layers(shard_layers);
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    const float prescale = sim_prescale(prescale_in, average, hub_.world());
+    check_outputs(inputs, outputs, true);
+    run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
+      red.reduce_scatter(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, prescale, rng, s);
+    });
+  }
+  // Reducer::all_gather: inputs[r] holds rank r's shard of S elements, outputs[r] receives W * S
+  void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
+                  const std::vector<LayerTuple>& shard_layers, bool skip_incomplete, bool stochastic, uint64_t seed,
+                  uint32_t seq) {
+    const auto specs = to_layers(shard_layers);
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    check_outputs(inputs, outputs, false);
+    run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
+      red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s);
     });
   }
   // bytes each rank's reducer counted as sent during the last call
@@ -584,6 +607,20 @@ class LocalReducerGroup {
         v.push_back(std::move(k));
       }
     return v;
+  }
+
+  // one output per rank, contiguous, of the inputs' dtype and device, holding S (reduce-scatter) or
+  // W * S elements (all-gather) for inputs of W * S or S
+  void check_outputs(const std::vector<at::Tensor>& inputs, const std::vector<at::Tensor>& outputs, bool rs) const {
+    const int64_t W = hub_.world();
+    TORCH_CHECK(inputs.size() == outputs.size(), "LocalReducerGroup: one output per input");
+    for (size_t r = 0; r < inputs.size(); ++r) {
+      const at::Tensor &i = inputs[r], &o = outputs[r];
+      TORCH_CHECK(o.is_contiguous() && o.scalar_type() == i.scalar_type() && o.device() == i.device() &&
+                      (rs ? i.numel() == o.numel() * W : o.numel() == i.numel() * W),
+                  "LocalReducerGroup: contiguous outputs of the inputs' dtype and device, ",
+                  rs ? "inputs of W * S and outputs of S elements" : "inputs of S and outputs of W * S elements");
+    }
   }
 
   template <class F>
@@ -629,7 +666,7 @@ class LocalReducerGroup {
               g.set_index((c10::DeviceIndex)device_);
               s = streams_[r].stream();
             }
-            op(*rk[r].red, tensors[r].data_ptr(), dt, s);
+            op(*rk[r].red, r, tensors[r].data_ptr(), dt, s);
             if (cuda) cuda_check(cudaStreamSynchronize(s), "LocalReducerGroup: synchronise a virtual rank");
           } catch (const std::exception& e) {
             hub_.fail("rank " + std::to_string(r) + ": " + e.what());
@@ -673,7 +710,7 @@ class LocalEngineGroup {
  public:
   LocalEngineGroup(int world, int local_size, const py::dict& config, int lanes, int64_t slot_bytes,
                    int64_t timeout_ms)
-      : world_(world), local_size_(local_size) {
+      : world_(world), local_size_(local_size), nodes_(local_size >= 1 ? world / local_size : 1) {
     TORCH_CHECK(world >= 1 && world <= kMaxPeers, "LocalEngineGroup: world must be 1..", kMaxPeers, ", got ", world);
     TORCH_CHECK(local_size >= 1 && world % local_size == 0, "LocalEngineGroup: local_size ", local_size,
                 " does not divide the world ", world);
@@ -716,6 +753,7 @@ class LocalEngineGroup {
     }
     for (int n = 0; n < nodes; ++n) intra_hubs_.push_back(std::make_unique<LoopbackHub>(local_size, timeout_ms));
     for (int l = 0; l < local_size; ++l) cross_hubs_.push_back(std::make_unique<LoopbackHub>(nodes, timeout_ms));
+    world_hub_ = std::make_unique<LoopbackHub>(world, timeout_ms);
     for (int r = 0; r < world; ++r) {
       auto e = std::make_unique<AllreduceEngine>(r, world, cfg);
       e->set_topology(local_size);
@@ -771,29 +809,37 @@ class LocalEngineGroup {
     });
   }
   // inputs[r] / outputs[r]: rank r's buffers of the reduce-scatter (W * S -> S) or the all-gather
-  // (S -> W * S); one layer of S elements with the environment's width and bucket size
-  void sharded(bool reduce_scatter, std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, bool average) {
+  // (S -> W * S); `shard_layers` is one shard's table, by default one layer of S elements with the
+  // environment's width and bucket size. Host tensors run the generic reducers (no heaps). The
+  // all-gather runs without skip_incomplete, as the process group's does.
+  void sharded(bool reduce_scatter, std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, bool average,
+               const std::optional<std::vector<LayerTuple>>& shard_layers) {
     const ShardedOp op = reduce_scatter ? ShardedOp::kReduceScatter : ShardedOp::kAllGather;
     TORCH_CHECK((int)outputs.size() == world_, "LocalEngineGroup: one output per virtual rank");
     const CompressionEnv env = CompressionEnv::read();
+    const bool skip = reduce_scatter && env.skip_incomplete;
     RngParams rng = make_rng(env.stochastic, env.seed, 0);
+    const std::vector<LayerSpec> given = shard_layers ? to_layers(*shard_layers) : std::vector<LayerSpec>{};
     run(inputs, [&](AllreduceEngine& e, int r, void* in, int dt, int64_t n, bool cuda, cudaStream_t s) {
-      TORCH_CHECK(cuda && outputs[r].is_cuda() && outputs[r].is_contiguous() && cgx_dtype(outputs[r]) == dt,
-                  "LocalEngineGroup: the sharded collectives take contiguous CUDA tensors of one dtype");
+      TORCH_CHECK(outputs[r].is_contiguous() && cgx_dtype(outputs[r]) == dt &&
+                      outputs[r].device() == inputs[r].device(),
+                  "LocalEngineGroup: contiguous outputs of the inputs' dtype and device");
+      TORCH_CHECK(cuda || !e.fused(), "LocalEngineGroup: host tensors need a group without heaps (p2p=False)");
       const int64_t S = reduce_scatter ? outputs[r].numel() : n;
       TORCH_CHECK((reduce_scatter ? n : outputs[r].numel()) == S * world_, "LocalEngineGroup: the full buffer holds W x S");
+      const std::vector<LayerSpec> table = e.sharded_table(S, given, env.bits, env.bucket_size);
+      at::Tensor staging;
+      if (const int64_t sn = e.sharded_staging_numel(S)) staging = at::empty({sn}, inputs[r].options());
       // upload every window's plan and wait for it before any rank launches (see the class comment)
-      LayerSpec l;
-      l.numel = (uint64_t)S;
-      l.bits = compression_enabled(S, env.bits, e.config().min_compress_elems) ? env.bits : kRawBits;
-      l.bucket = (uint32_t)std::max(1, env.bucket_size);
       if (e.fused()) {
-        e.fused()->prepare_sharded({l}, dt, env.skip_incomplete, s);
+        e.prepare_sharded(op, table, dt, skip, s);
         cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: plan upload");
         intra_hub(r)->barrier(e.local_rank());
       }
-      e.sharded_cuda(op, in, outputs[r].data_ptr(), dt, S, {}, average, env.bits, env.bucket_size,
-                     env.skip_incomplete, rng, s, false);
+      e.sharded(cuda, op, in, outputs[r].data_ptr(), staging.defined() ? staging.data_ptr() : nullptr, dt, S, table,
+                average, skip, rng, s, false);
+      // the staging buffer is freed on the caller's stream when this returns: let its work finish first
+      if (staging.defined() && cuda) cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: sharded call");
     });
   }
 
@@ -860,7 +906,17 @@ class LocalEngineGroup {
       group->intra_hub(rank)->barrier(group->engines_[rank]->local_rank());
     }
     void stage(const EngineStage& s) override {
-      static const char* kNames[] = {"oneshot", "sra", "generic_intra", "cross", "bcast_compressed", "bcast_raw"};
+      static const char* kNames[] = {"oneshot", "sra",     "generic_intra", "cross",      "bcast_compressed", "bcast_raw",
+                                     "rs",      "ag",      "generic_rs",    "generic_ag", "cross_rs",         "cross_ag"};
+      // A sharded call over several nodes runs fused launches next to generic stages, whose
+      // cudaMalloc / cudaFree can wait for a fused kernel of another node that spins for a peer the
+      // same driver call holds up. Every rank issues the same sharded stages, so before each of them
+      // all ranks drain their streams and meet: no fused kernel runs while a generic stage does.
+      if (s.sharded() && group->nodes_ > 1) {
+        if (group->call_cuda_)
+          cuda_check(cudaStreamSynchronize(group->streams_[rank].stream()), "LocalEngineGroup: quiesce");
+        group->world_hub_->barrier(rank);
+      }
       Entry e;
       e.kind = kNames[s.kind];
       if (s.layers)
@@ -897,6 +953,7 @@ class LocalEngineGroup {
   void fail_all(const std::string& msg) {
     for (auto& h : intra_hubs_) h->fail(msg);
     for (auto& h : cross_hubs_) h->fail(msg);
+    world_hub_->fail(msg);
   }
 
   // op(engine, rank, data, dtype, numel, cuda, stream) on every rank's thread; every rank's stream is
@@ -927,6 +984,8 @@ class LocalEngineGroup {
     }
     for (auto& h : intra_hubs_) h->reset(false);
     for (auto& h : cross_hubs_) h->reset(false);
+    world_hub_->reset(false);
+    call_cuda_ = cuda;
     for (auto& o : observers_) o->log.clear();
     const int64_t n = tensors[0].numel();
     {
@@ -950,6 +1009,7 @@ class LocalEngineGroup {
           }
           intra_hub(r)->finish(engines_[r]->local_rank());
           cross_hub(r)->finish(engines_[r]->node());
+          world_hub_->finish(r);
         });
       for (auto& t : threads) t.join();
       // a rank that threw skipped its own synchronise: nothing it queued may run on after this returns
@@ -962,13 +1022,16 @@ class LocalEngineGroup {
     }
     for (auto& h : intra_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
     for (auto& h : cross_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
+    TORCH_CHECK(!world_hub_->failed(), "LocalEngineGroup: ", world_hub_->failure());
     if (cuda) check();
   }
 
-  int world_, local_size_;
+  int world_, local_size_, nodes_;
   int device_ = -1;
+  bool call_cuda_ = false;  // the running call's tensors are device memory
   HeapLayout layout_{};
   std::vector<std::unique_ptr<LoopbackHub>> intra_hubs_, cross_hubs_;
+  std::unique_ptr<LoopbackHub> world_hub_;  // barriers of every rank (Observer::stage)
   std::vector<std::unique_ptr<AllreduceEngine>> engines_;  // after the hubs: released first
   std::vector<std::unique_ptr<Observer>> observers_;
   std::vector<c10::cuda::CUDAStream> streams_;
@@ -1361,7 +1424,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
   m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
-        py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048);
+        py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048,
+        py::arg("prescale") = py::none());
   m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0);
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
@@ -1473,6 +1537,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("broadcast_compressed", &LocalReducerGroup::broadcast_compressed, py::arg("tensors"), py::arg("layers"),
            py::arg("root"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0)
+      .def("reduce_scatter", &LocalReducerGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
+           py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none())
+      .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
+           py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
+           py::arg("seed") = 0, py::arg("seq") = 0)
       .def("bytes_sent", &LocalReducerGroup::bytes_sent)
       .def("set_recording", &LocalReducerGroup::set_recording, py::arg("on"))
       .def("messages", &LocalReducerGroup::messages);
@@ -1484,15 +1554,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("allreduce_layers", &LocalEngineGroup::allreduce_layers, py::arg("tensors"), py::arg("layers"),
            py::arg("average") = false)
       .def("reduce_scatter",
-           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out, bool average) {
-             g.sharded(true, std::move(in), std::move(out), average);
+           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out, bool average,
+              std::optional<std::vector<LayerTuple>> shard_layers) {
+             g.sharded(true, std::move(in), std::move(out), average, shard_layers);
            },
-           py::arg("inputs"), py::arg("outputs"), py::arg("average") = false)
+           py::arg("inputs"), py::arg("outputs"), py::arg("average") = false, py::arg("shard_layers") = py::none())
       .def("all_gather",
-           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out) {
-             g.sharded(false, std::move(in), std::move(out), false);
+           [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out,
+              std::optional<std::vector<LayerTuple>> shard_layers) {
+             g.sharded(false, std::move(in), std::move(out), false, shard_layers);
            },
-           py::arg("inputs"), py::arg("outputs"))
+           py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none())
       .def("stats", &LocalEngineGroup::stats, py::arg("rank"))
       .def("check", &LocalEngineGroup::check)
       .def("log", &LocalEngineGroup::log, py::arg("rank"))

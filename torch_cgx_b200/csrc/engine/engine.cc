@@ -190,38 +190,131 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
                         overlapped);
 }
 
-void AllreduceEngine::sharded_cuda(ShardedOp op, const void* in, void* out, int dtype, int64_t shard_numel,
-                                   std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket,
-                                   bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream,
-                                   bool overlapped) {
-  if (nodes() > 1)
-    throw std::runtime_error(std::string("cgx: the compressed ") + op_title(op) + " supports a single node only");
-  if (!fused_ || cfg_.inner_comm != CommType::kP2P)
-    throw std::runtime_error(std::string("cgx: the compressed ") + op_title(op) +
-                             " needs the P2P transport (CGX_INNER_COMMUNICATOR_TYPE=P2P)");
-  fused_->check_status();
-  if (shard_numel <= 0) return;
-  NvtxRange range(op == ShardedOp::kReduceScatter ? "cgx:reduce_scatter_cuda" : "cgx:all_gather_cuda",
-                  (uint64_t)shard_numel);
-  if (shard_layers.empty()) {
+std::vector<LayerSpec> AllreduceEngine::sharded_table(int64_t shard_numel, std::vector<LayerSpec> layers, int bits,
+                                                      int bucket) const {
+  if (layers.empty() && shard_numel > 0) {
     LayerSpec l;
     l.elem_off = 0;
     l.numel = (uint64_t)shard_numel;
     l.bits = compression_enabled(shard_numel, bits, cfg_.min_compress_elems) ? bits : kRawBits;
     l.bucket = (uint32_t)std::max(1, bucket);
-    shard_layers.push_back(l);
+    layers.push_back(l);
   }
+  return layers;
+}
+
+std::vector<LayerSpec> AllreduceEngine::sharded_intra_table(ShardedOp op, std::vector<LayerSpec> table) const {
+  if (nodes() > 1 && (op == ShardedOp::kAllGather || !cfg_.intra_compress))
+    for (LayerSpec& l : table) l.bits = kRawBits;
+  return table;
+}
+
+void AllreduceEngine::prepare_sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype,
+                                      bool skip_incomplete, cudaStream_t stream) {
+  if (fused_) fused_->prepare_sharded(sharded_intra_table(op, shard_layers), dtype, skip_incomplete, stream);
+}
+
+void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
+                                    const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale,
+                                    const RngParams& rng, cudaStream_t stream, bool overlapped) {
+  const bool rs = op == ShardedOp::kReduceScatter;
+  if (fused_sharded(cuda)) {
+    FusedSra::WindowHook hook;
+    if (observer_)
+      hook = [&](const std::vector<LayerSpec>& w, const DevicePlan& dp) {
+        observer_->stage(EngineStage{rs ? EngineStage::kRs : EngineStage::kAg, &w, &dp, rng, prescale});
+        observer_->before_fused_launch(dp, stream);
+      };
+    const FusedSra::RsCounts n = fused_->sharded(op, table, dtype, skip_incomplete, in, out, S, prescale, rng,
+                                                 stream, overlapped ? cfg_.overlap_lanes : 0, hook);
+    stats_.kernel_launches += n.launches;
+    stats_.elements += n.elements;
+    stats_.wire_bytes += n.wire_bytes;
+    stats_.raw_bytes += n.raw_bytes;
+    return;
+  }
+  GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  const uint64_t before = g.intra->bytes_sent();
+  observe(rs ? EngineStage::kGenericRs : EngineStage::kGenericAg, &table, rng, prescale);
+  if (rs)
+    g.intra->reduce_scatter(in, out, dtype, table, skip_incomplete, prescale, rng, stream);
+  else
+    g.intra->all_gather(in, out, dtype, table, skip_incomplete, rng, stream);
+  // the fused kernel's conventions: the elements of the window, the raw bytes a raw exchange would move
+  const uint64_t L = (uint64_t)local_size_, es = (uint64_t)dtype_size(dtype);
+  stats_.wire_bytes += g.intra->bytes_sent() - before;
+  stats_.elements += L * S;
+  stats_.raw_bytes += S * (L - 1) * es;
+}
+
+// Two stages when there are several nodes (DESIGN §2.9b), N = nodes(), L = local_size_, r = n * L + l:
+//  reduce-scatter: 1. per node block b, the node-local reduce-scatter of in[b*L*S, (b+1)*L*S) into
+//                     staging[b*S, (b+1)*S) (the node's partial of chunk b*L + l), prescaled by 1/W;
+//                  2. the cross-node reduce-scatter of the N partials among the ranks of local rank l,
+//                     prescale 1 (1/W and straight from `in` when L = 1).
+//  all-gather:     1. the cross-node all-gather of the shard into staging (into `out` when L = 1);
+//                  2. per node n', the node-local all-gather of staging[n'*S, (n'+1)*S) into
+//                     out[n'*L*S, (n'+1)*L*S) with a raw table: every shard is quantized once.
+// RNG sequences: node block b runs with call_seq << 4 ^ b (one node: today's call_seq << 4), the
+// cross-node stage with call_seq << 4 ^ 0x40000000, the allreduce's cross-node marker.
+void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out, void* staging, int dtype,
+                              int64_t shard_numel, const std::vector<LayerSpec>& shard_layers, bool average,
+                              bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped) {
+  GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  const int N = nodes(), L = local_size_;
+  const std::string title = std::string("cgx: the compressed ") + op_title(op);
+  const bool fused = fused_sharded(cuda);
+  if (fused) fused_->check_status();
+  if (shard_numel <= 0) return;
+  check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_);
+  if (!fused && (L > 1 || N == 1) && !g.intra)
+    throw std::runtime_error(title + (L > 1 ? " has no intra-node reducer" : " of one rank needs the P2P transport"));
+  if (N > 1 && !g.cross) throw std::runtime_error(title + ": multi-node topology but no cross-node reducer");
+  if (sharded_staging_numel(shard_numel) > 0 && staging == nullptr)
+    throw std::runtime_error(title + ": several nodes need a staging buffer");
+  NvtxRange range(op == ShardedOp::kReduceScatter ? "cgx:reduce_scatter_cuda" : "cgx:all_gather_cuda",
+                  (uint64_t)shard_numel);
   ++call_seq_;
   ++stats_.calls;
-  RngParams rng = rng_in;
-  rng.seq = call_seq_ << 4;  // one sequence for every window: the counters are element indices of the full buffer
-  const FusedSra::RsCounts n =
-      fused_->sharded(op, shard_layers, dtype, skip_incomplete, in, out, (uint64_t)shard_numel,
-                      average ? 1.0f / (float)world_ : 1.0f, rng, stream, overlapped ? cfg_.overlap_lanes : 0);
-  stats_.kernel_launches += n.launches;
-  stats_.elements += n.elements;
-  stats_.wire_bytes += n.wire_bytes;
-  stats_.raw_bytes += n.raw_bytes;
+  const uint64_t S = (uint64_t)shard_numel;
+  const size_t shard_bytes = (size_t)S * (size_t)dtype_size(dtype);
+  const float prescale = average ? 1.0f / (float)world_ : 1.0f;
+  const uint32_t seq = call_seq_ << 4;  // one sequence for every window: the counters are element indices
+  RngParams rng = rng_in, crng = rng_in;
+  crng.seq = seq ^ 0x40000000u;
+  const std::vector<LayerSpec> intra_table = sharded_intra_table(op, shard_layers);
+  const bool intra = L > 1 || N == 1;
+  auto at = [](const void* p, size_t off) { return static_cast<uint8_t*>(const_cast<void*>(p)) + off; };
+  if (op == ShardedOp::kReduceScatter) {
+    void* partial = N > 1 ? staging : out;
+    if (intra)
+      for (int b = 0; b < N; ++b) {
+        rng.seq = seq ^ (uint32_t)b;
+        NvtxRange r1("cgx:intra_node", (uint64_t)b);
+        sharded_intra(cuda, op, at(in, (size_t)b * L * shard_bytes), at(partial, (size_t)b * shard_bytes), dtype, S,
+                      intra_table, skip_incomplete, prescale, rng, stream, overlapped);
+      }
+    if (N == 1) return;
+    NvtxRange r2("cgx:cross_node", (uint64_t)N);
+    const float cross_scale = L > 1 ? 1.0f : prescale;
+    observe(EngineStage::kCrossRs, &shard_layers, crng, cross_scale);
+    g.cross->reduce_scatter(L > 1 ? partial : in, out, dtype, shard_layers, skip_incomplete, cross_scale, crng, stream);
+    return;
+  }
+  void* gathered = L > 1 ? staging : out;
+  if (N > 1) {
+    NvtxRange r2("cgx:cross_node", (uint64_t)N);
+    observe(EngineStage::kCrossAg, &shard_layers, crng, 1.0f);
+    g.cross->all_gather(in, gathered, dtype, shard_layers, skip_incomplete, crng, stream);
+  }
+  if (!intra) return;
+  for (int n = 0; n < N; ++n) {
+    rng.seq = seq ^ (uint32_t)n;
+    NvtxRange r1("cgx:intra_node", (uint64_t)n);
+    sharded_intra(cuda, op, N > 1 ? at(gathered, (size_t)n * shard_bytes) : in,
+                  at(out, (size_t)n * L * shard_bytes), dtype, S, intra_table, skip_incomplete, 1.0f, rng, stream,
+                  overlapped);
+  }
 }
 
 void AllreduceEngine::allreduce_cpu(void* data, int dtype, int64_t numel, bool average, int explicit_bucket) {

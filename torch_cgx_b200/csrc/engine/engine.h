@@ -38,14 +38,22 @@ struct EngineStats {
 std::vector<std::vector<LayerSpec>> split_for_fusion(const std::vector<LayerSpec>& layers, int elsize,
                                                      int64_t fusion_bytes);
 
-// One stage of an allreduce as the engine issues it (EngineObserver::stage).
+// One stage of an allreduce or of a sharded collective as the engine issues it (EngineObserver::stage).
+// kRs / kAg are fused launches (one per window), kGenericRs / kGenericAg the generic intra-node
+// reducer, kCrossRs / kCrossAg the cross-node stage of a sharded call.
 struct EngineStage {
-  enum Kind { kOneshot, kSra, kGenericIntra, kCross, kBcastCompressed, kBcastRaw };
+  enum Kind {
+    kOneshot, kSra, kGenericIntra, kCross, kBcastCompressed, kBcastRaw,
+    kRs, kAg, kGenericRs, kGenericAg, kCrossRs, kCrossAg
+  };
   Kind kind;
-  const std::vector<LayerSpec>* layers;  // the stage's layer table; null for a fused launch of the bucket fast path
-  const DevicePlan* dp;                  // the plan of a fused launch (kOneshot / kSra), else null
+  // the stage's layer table (a sharded stage: one shard's, or a fused launch's window of it); null
+  // for a fused launch of the bucket fast path
+  const std::vector<LayerSpec>* layers;
+  const DevicePlan* dp;                  // the plan of a fused launch (kOneshot / kSra / kRs / kAg), else null
   RngParams rng;                         // the sequence number the stage runs with
-  float scale;                           // prescale of an allreduce stage, 1 for a broadcast
+  float scale;                           // prescale of a reduction stage, 1 for a broadcast or an all-gather
+  bool sharded() const { return kind >= kRs; }
 };
 
 // Test seam: sees every stage an engine issues. Production engines have none (one branch per stage).
@@ -122,16 +130,30 @@ class AllreduceEngine {
   void allreduce_cuda_layers(void* data, int dtype, const std::vector<LayerSpec>& layers, bool average,
                              const CompressionEnv& env, cudaStream_t stream, bool overlapped = false);
 
-  // Compressed reduce-scatter or all-gather of CUDA buffers on `stream` (FusedSra::sharded) with
-  // shards of S = shard_numel elements: the reduce-scatter's `in` holds world * S elements and
-  // `out` receives this rank's shard; the all-gather's `in` is this rank's shard and `out`
-  // receives world * S, every shard (this rank's included) one quantization round trip (average
-  // and skip_incomplete false). An empty `shard_layers` means one layer of S elements with
-  // `bits` / `bucket`, raw unless S exceeds CGX_COMPRESSION_MINIMAL_SIZE. Single node, P2P
-  // transport only; adds to the same counters as the allreduce.
-  void sharded_cuda(ShardedOp op, const void* in, void* out, int dtype, int64_t shard_numel,
-                    std::vector<LayerSpec> shard_layers, bool average, int bits, int bucket, bool skip_incomplete,
-                    const RngParams& rng_in, cudaStream_t stream, bool overlapped);
+  // Compressed reduce-scatter or all-gather of device (cuda) or host buffers on `stream` with shards
+  // of S = shard_numel elements: the reduce-scatter's `in` holds world * S elements and `out`
+  // receives this rank's shard; the all-gather's `in` is this rank's shard and `out` receives
+  // world * S, every shard (this rank's included) one quantization round trip (average and
+  // skip_incomplete false). `shard_layers` is one shard's table (sharded_table).
+  // One node: the fused kernel (FusedSra::sharded) on the P2P transport, else the generic intra-node
+  // reducer. Several nodes: two stages (DESIGN §2.9b), the node-local one as on one node, the other
+  // through the cross-node reducer; `staging` then holds sharded_staging_numel(S) elements of the
+  // dtype for the node partials / the gathered shards. Host memory runs the generic reducers only.
+  // Adds to the same counters as the allreduce.
+  void sharded(bool cuda, ShardedOp op, const void* in, void* out, void* staging, int dtype, int64_t shard_numel,
+               const std::vector<LayerSpec>& shard_layers, bool average, bool skip_incomplete,
+               const RngParams& rng_in, cudaStream_t stream, bool overlapped);
+  // The table of one S-element shard: `layers` when given, else one layer of S elements with `bits`
+  // / `bucket`, raw unless S exceeds CGX_COMPRESSION_MINIMAL_SIZE.
+  std::vector<LayerSpec> sharded_table(int64_t shard_numel, std::vector<LayerSpec> layers, int bits,
+                                       int bucket) const;
+  // elements of the staging buffer sharded() needs: N * S with several nodes of several ranks, else 0
+  int64_t sharded_staging_numel(int64_t shard_numel) const {
+    return (nodes() > 1 && local_size_ > 1) ? (int64_t)nodes() * shard_numel : 0;
+  }
+  // builds and uploads every fused plan a sharded() call with this table launches, without launching
+  void prepare_sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
+                       cudaStream_t stream);
 
   void check_health();
   void set_observer(EngineObserver* o) { observer_ = o; }
@@ -143,6 +165,14 @@ class AllreduceEngine {
                   const CompressionEnv& env, cudaStream_t stream);
   void intra_stage(bool cuda, void* data, int dtype, const std::vector<LayerSpec>& group, bool skip_incomplete,
                    float prescale, RngParams rng, cudaStream_t stream);
+  // the node-local stage of a sharded call over the local ranks: fused kernel or generic reducer
+  void sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
+                     const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale, const RngParams& rng,
+                     cudaStream_t stream, bool overlapped);
+  bool fused_sharded(bool cuda) const { return cuda && fused_ && cfg_.inner_comm == CommType::kP2P; }
+  // the node-local stage's table: raw in a multi-node all-gather, and in a multi-node
+  // reduce-scatter without CGX_INTRA_COMPRESS
+  std::vector<LayerSpec> sharded_intra_table(ShardedOp op, std::vector<LayerSpec> table) const;
 
   // Fast path for registered DDP buckets: once a bucket's plans are known (and nothing that
   // influences them changed) a call is just "launch these kernels" -- no layer extraction,

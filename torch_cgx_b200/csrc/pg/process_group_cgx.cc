@@ -410,16 +410,22 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
               " has ", full.numel(), " elements, expected world size (", getSize(), ") x ", rs ? "output" : "input",
               " (", shard.numel(), ")");
   TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: ", name, "_compressed: bits must be 1..8 or 32");
-  TORCH_CHECK(engine_->nodes() == 1, "cgx: the compressed ", op_title(op), " supports a single node only");
-  TORCH_CHECK(cfg_.inner_comm == CommType::kP2P, "cgx: the compressed ", op_title(op),
-              " needs the P2P transport, not CGX_INNER_COMMUNICATOR_TYPE=", to_string(cfg_.inner_comm));
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
+  const std::vector<LayerSpec> table = engine_->sharded_table(shard.numel(), layers, bits, bucket_size);
   return enqueue_cuda(rs ? c10d::OpType::_REDUCE_SCATTER_BASE : c10d::OpType::_ALLGATHER_BASE,
                       rs ? "cgx:reduce_scatter" : "cgx:all_gather", out, &in, [&](cudaStream_t s) {
-                        engine_->sharded_cuda(op, in.data_ptr(), out.data_ptr(), dtype, shard.numel(), layers,
-                                              average, bits, bucket_size, skip_incomplete, rng, s, overlapped);
+                        // several nodes: the node partials / gathered shards, N x S elements
+                        at::Tensor staging;
+                        if (const int64_t n = engine_->sharded_staging_numel(shard.numel())) {
+                          c10::cuda::CUDAStreamGuard sg(*comm_stream_);
+                          staging = at::empty({n}, in.options());
+                          c10::cuda::CUDACachingAllocator::recordStream(staging.storage().data_ptr(), *comm_stream_);
+                        }
+                        engine_->sharded(true, op, in.data_ptr(), out.data_ptr(),
+                                         staging.defined() ? staging.data_ptr() : nullptr, dtype, shard.numel(), table,
+                                         average, skip_incomplete, rng, s, overlapped);
                       });
 }
 

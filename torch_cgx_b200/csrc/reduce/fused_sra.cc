@@ -143,6 +143,26 @@ std::vector<std::vector<LayerSpec>> split_shard(const std::vector<LayerSpec>& la
 
 }  // namespace
 
+void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
+                           const void* out, uint64_t S, int rank, int world) {
+  const bool rs = op == ShardedOp::kReduceScatter;
+  const char* name = op_name(op);
+  const uint64_t table = shard_elems(shard_layers);
+  if (table != S)
+    throw std::invalid_argument(std::string("cgx ") + name + ": the shard layers tile [0, " + std::to_string(table) +
+                                ") but the " + (rs ? "output" : "input") + " has " + std::to_string(S) + " elements");
+  if (S == 0) return;
+  const uint64_t es = (uint64_t)dtype_size(dtype);
+  const uintptr_t full = reinterpret_cast<uintptr_t>(rs ? in : out);
+  const uintptr_t shard = reinterpret_cast<uintptr_t>(rs ? out : in);
+  const bool own_chunk = shard == full + (uint64_t)rank * S * es;
+  const bool disjoint = shard + S * es <= full || full + (uint64_t)world * S * es <= shard;
+  if (!own_chunk && !disjoint)
+    throw std::invalid_argument(std::string("cgx ") + name +
+                                (rs ? ": the output overlaps the input" : ": the input overlaps the output") +
+                                " other than as its chunk " + std::to_string(rank));
+}
+
 std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<LayerSpec>& shard_layers,
                                                            const PlanOptions& opt, uint32_t slot_bytes) {
   const uint64_t S = shard_elems(shard_layers);
@@ -187,31 +207,19 @@ void FusedSra::prepare_sharded(const std::vector<LayerSpec>& shard_layers, int d
 
 FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype,
                                      bool skip_incomplete, const void* in, void* out, uint64_t S, float prescale,
-                                     const RngParams& rng, cudaStream_t stream, int max_lanes) {
+                                     const RngParams& rng, cudaStream_t stream, int max_lanes,
+                                     const WindowHook& before_launch) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
   RsCounts n;
-  const uint64_t table = shard_elems(shard_layers);
-  if (table != S)
-    throw std::invalid_argument(std::string("cgx ") + name + ": the shard layers tile [0, " + std::to_string(table) +
-                                ") but the " + (rs ? "output" : "input") + " has " + std::to_string(S) + " elements");
+  check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world());
   if (S == 0) return n;
-  {
-    const uint64_t es = (uint64_t)dtype_size(dtype);
-    const uintptr_t full = reinterpret_cast<uintptr_t>(rs ? in : out);
-    const uintptr_t shard = reinterpret_cast<uintptr_t>(rs ? out : in);
-    const bool own_chunk = shard == full + (uint64_t)rank() * S * es;
-    const bool disjoint = shard + S * es <= full || full + (uint64_t)world() * S * es <= shard;
-    if (!own_chunk && !disjoint)
-      throw std::invalid_argument(std::string("cgx ") + name +
-                                  (rs ? ": the output overlaps the input" : ": the input overlaps the output") +
-                                  " other than as its chunk " + std::to_string(rank()));
-  }
   // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
   for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes)) {
     const DevicePlan* dp = prepare(replicate(w, world(), S), dtype, skip_incomplete, stream, max_lanes);
     if (dp == nullptr)
       throw std::runtime_error(std::string("cgx ") + name + ": window plan does not fit the heap slots");
+    if (before_launch) before_launch(w, *dp);
     launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs);
     const Plan& pl = dp->plan;
     const uint64_t mine = pl.chunk_wire_bytes[rank()], my_elems = pl.chunk_elems[rank()];

@@ -7,6 +7,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <functional>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -54,6 +55,12 @@ inline std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& shard, int
     }
   return out;
 }
+
+// The buffers of one rank's sharded call: `shard_layers` tiles [0, S) in order, and the shard buffer
+// (the reduce-scatter's `out`, the all-gather's `in`) is disjoint from the full one or exactly its
+// chunk `rank` of `world`; std::invalid_argument otherwise.
+void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
+                           const void* out, uint64_t S, int rank, int world);
 
 // The windows of a reduce-scatter: the shard's layer table (offsets from the shard start, tiling
 // [0, S) in order; std::invalid_argument otherwise) cut by split_for_fusion into shard-relative
@@ -103,12 +110,14 @@ class FusedSra {
   // The shard is cut into windows whose worst-case wire fits one slot (split_for_fusion, cuts on
   // bucket boundaries, so the result does not depend on the slot size) and one kernel is launched
   // per window. Stream-ordered; every rank must issue the same calls in the same order.
+  // `before_launch`, when set, sees each window's table and plan right before its kernel is launched.
   struct RsCounts {
     uint64_t launches = 0, elements = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's share
   };
+  using WindowHook = std::function<void(const std::vector<LayerSpec>& window, const DevicePlan& dp)>;
   RsCounts sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                    const void* in, void* out, uint64_t S, float prescale, const RngParams& rng, cudaStream_t stream,
-                   int max_lanes = 0);
+                   int max_lanes = 0, const WindowHook& before_launch = nullptr);
   // builds and uploads the plans of every window without launching anything
   void prepare_sharded(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                        cudaStream_t stream, int max_lanes = 0);

@@ -3,6 +3,8 @@
 #include <algorithm>
 #include <stdexcept>
 
+#include "fused_sra.h"  // shard_elems, replicate
+
 namespace cgx {
 
 Reducer::Reducer(Communicator* comm, BlockBackend* ops) : comm_(comm), ops_(ops) {}
@@ -84,6 +86,84 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
     x.push_back({false, wire, bytes, root});
     comm_->exchange(x, stream);
     ops_->dequantize(wire, 0, nb, data, stream);
+  }
+}
+
+// ------------------------------------------------------- sharded collectives --
+void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
+                             bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream) {
+  const int W = comm_->size(), r = comm_->rank();
+  const uint64_t S = shard_elems(shard_layers);
+  if (S == 0) return;
+  if (S * (uint64_t)W >= (1ull << 32))
+    throw std::invalid_argument("cgx reduce_scatter: the input exceeds 2^32 elements");
+  const Plan& plan = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete);
+  ops_->bind(plan, stream);
+  const size_t row = row_bytes(plan);
+  uint8_t* sendb = scratch(0, row * W);
+  uint8_t* recvb = scratch(1, row * W);
+  uint32_t lo, hi;
+  chunk_span(plan, r, &lo, &hi);
+  float* acc = reinterpret_cast<float*>(scratch(3, (size_t)(hi - lo) * sizeof(float) + 16));
+  const uint32_t cb = plan.chunk_begin(r), cn = plan.chunk_end(r) - cb;
+  // my quantized copy of every peer's chunk -> that peer (the SRA's phase 1)
+  std::vector<P2POp> x;
+  for (int p = 0; p < W; ++p) {
+    if (p == r) continue;
+    const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
+    if (pn) ops_->quantize(in, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
+    if (plan.chunk_wire_bytes[p]) x.push_back({true, sendb + row * p, plan.chunk_wire_bytes[p], p});
+    if (plan.chunk_wire_bytes[r]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[r], p});
+    bytes_sent_ += plan.chunk_wire_bytes[p];
+  }
+  comm_->exchange(x, stream);
+  if (!cn) return;
+  ops_->accumulate(nullptr, cb, cn, acc, lo, in, prescale, stream);
+  for (int q = 0; q < W; ++q)
+    if (q != r) ops_->accumulate(recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
+  // store the fp32 sums as T: a raw plan of one shard does exactly that (acc[i] is element i of the
+  // shard, chunk r starting at r * S)
+  std::vector<LayerSpec> raw = shard_layers;
+  for (LayerSpec& l : raw) l.bits = kRawBits;
+  const Plan& rp = plan_for(raw, dtype, false, 1);
+  ops_->bind(rp, stream);
+  ops_->quantize_f32(acc, lo - (uint32_t)(r * S), 0, (uint32_t)rp.blocks.size(), scratch(2, row_bytes(rp)),
+                     make_rng_key(rng, r, 1), out, stream);
+}
+
+void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
+                         bool skip_incomplete, const RngParams& rng, cudaStream_t stream) {
+  const int W = comm_->size(), r = comm_->rank();
+  const uint64_t S = shard_elems(shard_layers);
+  if (S == 0) return;
+  if (S * (uint64_t)W >= (1ull << 32))
+    throw std::invalid_argument("cgx all_gather: the output exceeds 2^32 elements");
+  const Plan& plan = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete);
+  ops_->bind(plan, stream);
+  const size_t row = row_bytes(plan);
+  uint8_t* recvb = scratch(1, row * W);
+  uint8_t* mine = scratch(2, row);
+  const size_t shard_bytes = (size_t)S * dtype_size(dtype);
+  uint8_t* own = static_cast<uint8_t*>(out) + (size_t)r * shard_bytes;
+  if (in != own) ops_->copy(own, in, shard_bytes, stream);
+  // the root's part of the compressed broadcast: quantize once, keep what the peers will decode
+  const uint32_t cb = plan.chunk_begin(r), cn = plan.chunk_end(r) - cb;
+  if (cn) {
+    ops_->quantize(out, cb, cn, mine, 1.0f, make_rng_key(rng, r, 1), stream);
+    ops_->dequantize(mine, cb, cn, out, stream);
+  }
+  std::vector<P2POp> x;
+  for (int p = 0; p < W; ++p) {
+    if (p == r) continue;
+    if (plan.chunk_wire_bytes[r]) x.push_back({true, mine, plan.chunk_wire_bytes[r], p});
+    if (plan.chunk_wire_bytes[p]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[p], p});
+    bytes_sent_ += plan.chunk_wire_bytes[r];
+  }
+  comm_->exchange(x, stream);
+  for (int p = 0; p < W; ++p) {
+    if (p == r) continue;
+    const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
+    if (pn) ops_->dequantize(recvb + row * p, pb, pn, out, stream);
   }
 }
 

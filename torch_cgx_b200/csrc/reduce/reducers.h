@@ -41,6 +41,22 @@ class Reducer {
   // bytes to every peer; receivers decode. Raw layers travel as T inside the same record.
   void broadcast_compressed(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
                             int root, const RngParams& rng, cudaStream_t stream);
+  // Compressed reduce-scatter over the communicator's W ranks, the scatter phase of the SRA alone.
+  // `shard_layers` is ONE shard's table (offsets from the shard start, tiling [0, S)); the plan is
+  // that table replicated W times at stride S, so chunk c is copy c and buckets are counted from each
+  // shard's start. `in` holds W * S elements, `out` receives shard rank():
+  //   out = T(prescale * in[r] + sum over peers q, in rank order, of decode(Q_q(prescale * in_q[r])))
+  // accumulated in fp32 and stored once in the dtype, not requantized. Bitwise the fused rs_kernel
+  // (same plan, primitives, order and RNG streams: rank q's phase-0 stream, full-buffer indices).
+  void reduce_scatter(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
+                      bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream);
+  // Compressed all-gather: the compressed broadcast with every rank as a root. `in` holds this rank's
+  // shard of S elements, `out` W * S; rank q quantizes its shard once (copy q of the replicated table,
+  // its phase-1 stream), decodes it into its own chunk and sends the same bytes to every peer, which
+  // decode them. Every rank's `out` is the same bytes, bitwise the fused ag_kernel's; raw layers
+  // (bits 32) are copied unchanged. `in` may be `out`'s chunk rank(), or disjoint from it.
+  void all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
+                  bool skip_incomplete, const RngParams& rng, cudaStream_t stream);
   uint64_t bytes_sent() const { return bytes_sent_; }
 
  protected:

@@ -588,7 +588,7 @@ def _shards(inputs: Sequence[torch.Tensor], r: int) -> List[torch.Tensor]:
 
 def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
                              world: int | None = None, average: bool = False,
-                             skip_incomplete: bool = False) -> List[torch.Tensor]:
+                             skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
     """Every rank's output of the compressed reduce-scatter (deterministic rounding).
 
     ``inputs[r]`` holds W shards of S elements; ``shard_layers`` is one shard's table (offsets from
@@ -596,12 +596,13 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
     Rank r receives, per element of shard r, in fp32:
         prescale*x_r  (kept unquantized)  +  sum over q != r, in rank order, of Q(prescale*x_q)
     rounded once to the dtype: the SRA's phase-B accumulator without the requantization. Raw runs
-    round each peer contribution to the dtype. Elements outside every layer are 0.
+    round each peer contribution to the dtype. Elements outside every layer are 0. The prescale is
+    ``prescale`` when given, else 1/W when averaging, else 1.
     """
     W = len(inputs)
     assert world is None or world == W
     dtype = inputs[0].dtype
-    ps = _prescale(W, average)
+    ps = _prescale(W, average, prescale)
     outs = []
     for r in range(W):
         xs = _scaled_inputs(_shards(inputs, r), ps)
@@ -619,6 +620,241 @@ def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[
     shard's table (offsets from the shard start), so buckets are counted from each shard's start;
     the owner's shard is quantized like every other. Raw runs are the value in the dtype."""
     return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers) for t in inputs])
+
+
+# ---- the sharded collectives over several nodes (AllreduceEngine::sharded, DESIGN §2.9b) -----------
+SHARDED_PERTURBATIONS = ("prescale_local", "requantized_gather", "quantized_own_partial", "transposed_ranks")
+_CROSS_SEQ = 0x40000000  # the allreduce's cross-node marker
+
+
+def _hier_rank(n: int, l: int, nodes: int, local_size: int, perturb: str | None) -> int:
+    """The rank of local rank l on node n: n*L + l (l*N + n under ``transposed_ranks``)."""
+    return l * nodes + n if perturb == "transposed_ranks" else n * local_size + l
+
+
+def _raw_table(layers: Sequence[Layer]) -> List[Layer]:
+    return [(int(o), int(n), RAW_BITS, int(b)) for o, n, _, b in layers]
+
+
+def _rs_quantized_own(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *, prescale: float,
+                      skip_incomplete: bool) -> List[torch.Tensor]:
+    """``reduce_scatter_reference`` with each rank's own contribution quantized like its peers' (the
+    wrong semantics ``quantized_own_partial``)."""
+    dtype = inputs[0].dtype
+    segs = layer_segments(shard_layers, skip_incomplete)
+    outs = []
+    for r in range(len(inputs)):
+        xs = _scaled_inputs(_shards(inputs, r), _F32(prescale))
+        xs[r] = _quantized(xs[r], segs, dtype)
+        out = np.zeros(xs[0].size, _F32)
+        for off, m, bits, bucket in segs:
+            sl = slice(off, off + m)
+            out[sl] = _sra_acc(xs, sl, np.full(m, r), bits, bucket, dtype)
+        outs.append(out)
+    return _to_tensors(outs, dtype)
+
+
+def _rs_hier(inputs, shard_layers, local_size, *, average, intra_compress, perturb, stage, seq=0):
+    """The two-stage reduce-scatter, each flat reduce-scatter computed by
+    ``stage(ins, table, prescale, seq, cross)``."""
+    W, L = len(inputs), local_size
+    N = W // L
+    assert N * L == W, "the local size divides the world"
+    dtype = inputs[0].dtype
+    ps = _prescale(W, average)
+    full = [t.detach().reshape(-1).cpu() for t in inputs]
+    S = full[0].numel() // W
+    shard_layers = [tuple(int(v) for v in l) for l in shard_layers]
+    if L > 1 or N == 1:
+        # 1. inside node n, for every node block b: the local reduce-scatter of in[b*L*S, (b+1)*L*S)
+        ps1 = _prescale(L, average) if perturb == "prescale_local" else ps
+        t1 = _raw_table(shard_layers) if (N > 1 and not intra_compress) else shard_layers
+        partial = [torch.empty(N * S, dtype=dtype) for _ in range(W)]
+        for n in range(N):
+            rk = [_hier_rank(n, l, N, L, perturb) for l in range(L)]
+            for b in range(N):
+                outs = stage([full[r][b * L * S:(b + 1) * L * S] for r in rk], t1, ps1, seq ^ b, False)
+                for r, o in zip(rk, outs):
+                    partial[r][b * S:(b + 1) * S] = o.reshape(-1)
+        if N == 1:
+            return partial
+        ps2 = _F32(1.0)
+    else:
+        partial, ps2 = full, ps
+    # 2. across nodes, among the ranks of local rank l: node n's partial P[n] unquantized, Q of the others
+    result = [None] * W
+    for l in range(L):
+        rk = [_hier_rank(n, l, N, L, perturb) for n in range(N)]
+        for r, o in zip(rk, stage([partial[r] for r in rk], shard_layers, ps2, seq ^ _CROSS_SEQ, True)):
+            result[r] = o.reshape(-1)
+    return result
+
+
+def reduce_scatter_hier_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
+                                  local_size: int, average: bool = False, skip_incomplete: bool = False,
+                                  intra_compress: bool = True, perturb: str | None = None) -> List[torch.Tensor]:
+    """Every rank's output of the compressed reduce-scatter over N = W / L nodes of L = ``local_size``
+    consecutive ranks (deterministic rounding); rank r = n*L + l, ``inputs[r]`` holds W shards of S.
+
+    1. Inside node n (skipped when L = 1), for each node block b: ``reduce_scatter_reference`` of the
+       L local ranks' in[b*L*S, (b+1)*L*S) with the shard table (raw when N > 1 and not
+       ``intra_compress``) and prescale 1/W when averaging; local rank l keeps P[b] = the node's
+       partial of chunk b*L + l, stored in the dtype.
+    2. Across nodes, among the N ranks of local rank l: ``reduce_scatter_reference`` of the N
+       partial buffers with prescale 1 (with L = 1: of the inputs, prescale 1/W when averaging):
+       rank (n, l) gets P[n] unquantized plus Q of every other node's P[n], in node order.
+    With N = 1 this is ``reduce_scatter_reference``, and with L = 1 bitwise the same over W ranks.
+    ``perturb`` (one of ``SHARDED_PERTURBATIONS``) switches on a wrong semantics for the tests.
+    """
+    def stage(ins, table, prescale, _seq, cross):
+        fn = _rs_quantized_own if (cross and perturb == "quantized_own_partial") else reduce_scatter_reference
+        return fn(ins, table, prescale=prescale, skip_incomplete=skip_incomplete)
+
+    return _rs_hier(inputs, shard_layers, local_size, average=average, intra_compress=intra_compress,
+                    perturb=perturb, stage=stage)
+
+
+def _ag_hier(inputs, shard_layers, local_size, *, perturb, stage, seq=0):
+    """The two-stage all-gather, each flat compressed all-gather computed by ``stage(ins, table, seq)``
+    (one tensor, every rank's output)."""
+    W, L = len(inputs), local_size
+    N = W // L
+    assert N * L == W, "the local size divides the world"
+    shards = [t.detach().reshape(-1).cpu() for t in inputs]
+    shard_layers = [tuple(int(v) for v in l) for l in shard_layers]
+    if N == 1:
+        return [stage(shards, shard_layers, seq)] * W
+    S = shards[0].numel()
+    # 1. across nodes: the ranks of local rank l gather Q of each other's shard, G = N shards
+    gathered = [None] * W
+    for l in range(L):
+        rk = [_hier_rank(n, l, N, L, perturb) for n in range(N)]
+        g = stage([shards[r] for r in rk], shard_layers, seq ^ _CROSS_SEQ)
+        for r in rk:
+            gathered[r] = g
+    # 2. inside node n, for every n2: local rank l2's G[n2] travels raw (re-quantized under
+    #    ``requantized_gather``) to out[(n2*L + l2)*S]
+    result = [None] * W
+    for n in range(N):
+        out = torch.empty(W * S, dtype=shards[0].dtype)
+        for n2 in range(N):
+            for l2 in range(L):
+                piece = gathered[_hier_rank(n, l2, N, L, perturb)][n2 * S:(n2 + 1) * S]
+                if perturb == "requantized_gather" and L > 1:
+                    piece = quantize_dequantize_layers(piece, shard_layers)
+                out[(n2 * L + l2) * S:(n2 * L + l2 + 1) * S] = piece
+        for l in range(L):
+            result[_hier_rank(n, l, N, L, perturb)] = out
+    return result
+
+
+def all_gather_hier_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *, local_size: int,
+                              perturb: str | None = None) -> List[torch.Tensor]:
+    """Every rank's output of the compressed all-gather over N = W / L nodes of L = ``local_size``
+    consecutive ranks (deterministic rounding); ``inputs[r]`` is rank r's shard of S elements.
+
+    1. Across nodes (skipped when N = 1), among the N ranks of local rank l: ``all_gather_reference``
+       of their shards, G = Q of each, node by node.
+    2. Inside node n (with N = 1 the compressed all-gather itself): local rank l2's G[n2] is copied
+       unchanged (a raw table) to out[(n2*L + l2)*S, ...) of every rank of the node.
+    Every shard gets exactly one quantization round trip, so every rank's output is
+    ``all_gather_reference`` of all W inputs, for every (N, L).
+    """
+    return _ag_hier(inputs, shard_layers, local_size, perturb=perturb,
+                    stage=lambda ins, table, _seq: all_gather_reference(ins, table))
+
+
+def _replicated(window: Sequence[Layer], world: int, S: int) -> List[Layer]:
+    return [(o + c * S, n, b, k) for c in range(world) for o, n, b, k in window]
+
+
+def sharded_engine_reference(op: str, inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
+                             local_size: int, config: dict, lanes: int, slot_bytes: Tuple[int, int] = (0, 0),
+                             average: bool = False, call_seq: int = 1, cuda: bool = True,
+                             skip_incomplete: bool = False, stochastic: bool = False, seed: int = 0):
+    """Every rank's output of one ``AllreduceEngine::sharded`` call and the stages each rank issues,
+    ``(outputs, stages)``, stages as in ``engine_reference``; ``op`` is "reduce_scatter" or
+    "all_gather" (which runs without ``skip_incomplete``).
+
+    The call runs with RNG sequence ``call_seq << 4``. Node-local stages (every node block b, or
+    every gathered node n2) run with ``seq ^ b``, the cross-node stage with ``seq ^ 0x40000000``.
+    A node-local stage is the fused kernel with ``cuda`` and heaps (``p2p``): one "rs" / "ag" launch
+    per window of ``C.reduce_scatter_windows`` at the heap's slot size, logged with the window's
+    table; otherwise one "generic_rs" / "generic_ag" stage with the whole table. The cross-node
+    stage is "cross_rs" / "cross_ag". Scales: 1/W when averaging for the reduce-scatter's first
+    stage (the cross one when L = 1), else 1. ``stochastic`` composes ``C.reduce_scatter_simulate``
+    and ``C.all_gather_simulate`` with these sequence numbers; otherwise the values are
+    ``reduce_scatter_hier_reference`` / ``all_gather_hier_reference``.
+    """
+    from .. import _C
+
+    cfg = dict(ENGINE_DEFAULTS, **config)
+    W, L = len(inputs), local_size
+    N = W // L
+    rs = op == "reduce_scatter"
+    assert rs or op == "all_gather"
+    skip = skip_incomplete and rs
+    dtype = inputs[0].dtype
+    dt = _DTYPE_CODE[dtype]
+    table = [tuple(int(v) for v in l) for l in shard_layers]
+    S = sum(l[1] for l in table)
+    ps = _prescale(W, average)
+    seq = (call_seq << 4) & _U32
+    intra_table = _raw_table(table) if N > 1 and (not rs or not cfg["intra_compress"]) else table
+
+    stages = [[] for _ in range(W)]
+
+    def log(r, kind, ls, s, scale, lanes_=0, numel=None):
+        stages[r].append(dict(kind=kind, layers=[tuple(l) for l in ls], lanes=lanes_,
+                              numel=sum(l[1] for l in ls) if numel is None else numel, seed=seed,
+                              seq=s & _U32, stochastic=stochastic, scale=float(scale)))
+
+    def intra(r, s, scale):
+        if not (cuda and cfg["p2p"]):
+            log(r, "generic_rs" if rs else "generic_ag", intra_table, s, scale)
+            return
+        for w in _C.reduce_scatter_windows(intra_table, world=L, lanes=lanes, dtype=dt, skip_incomplete=skip,
+                                           min_lane_elems=cfg["min_lane_elems"], slot_bytes=slot_bytes[0]):
+            p = _C.build_plan(_replicated(w, L, S), world=L, lanes=lanes, dtype=dt, skip_incomplete=skip,
+                              min_lane_elems=cfg["min_lane_elems"])
+            log(r, "rs" if rs else "ag", w, s, scale, p["lanes"], p["numel"])
+
+    local = L > 1 or N == 1
+    for r in range(W):
+        if rs:
+            for b in range(N if local else 0):
+                intra(r, seq ^ b, ps)
+            if N > 1:
+                log(r, "cross_rs", table, seq ^ _CROSS_SEQ, _F32(1.0) if L > 1 else ps)
+        else:
+            if N > 1:
+                log(r, "cross_ag", table, seq ^ _CROSS_SEQ, 1.0)
+            for n in range(N if local else 0):
+                intra(r, seq ^ n, 1.0)
+
+    if not stochastic:
+        if rs:
+            outs = reduce_scatter_hier_reference(inputs, table, local_size=L, average=average, skip_incomplete=skip,
+                                                 intra_compress=cfg["intra_compress"])
+        else:
+            outs = all_gather_hier_reference(inputs, table, local_size=L)
+        return outs, stages
+
+    def rs_stage(ins, t, prescale, s, _cross):
+        outs = [torch.empty(ins[0].numel() // len(ins), dtype=dtype) for _ in ins]
+        _C.reduce_scatter_simulate([x.contiguous() for x in ins], outs, t, 1, False, skip, True, seed, s,
+                                   cfg["min_lane_elems"], prescale=float(prescale))
+        return outs
+
+    def ag_stage(ins, t, s):
+        outs = [torch.empty(ins[0].numel() * len(ins), dtype=dtype) for _ in ins]
+        _C.all_gather_simulate([x.contiguous() for x in ins], outs, t, True, seed, s)
+        return outs[0]
+
+    if rs:
+        return _rs_hier(inputs, table, L, average=average, intra_compress=cfg["intra_compress"], perturb=None,
+                        stage=rs_stage, seq=seq), stages
+    return _ag_hier(inputs, table, L, perturb=None, stage=ag_stage, seq=seq), stages
 
 
 def reduce_scatter_exact_and_bound(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,

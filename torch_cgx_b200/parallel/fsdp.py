@@ -7,6 +7,9 @@ FSDP2 takes a custom reduce-scatter and all-gather per module (``FSDPModule.set_
     model = fully_shard(model)                       # after fully_shard on the sub-modules
     cgx.set_cgx_reduce_scatter(model, bits=8)        # every FSDPModule of the model
     cgx.set_cgx_all_gather(model, bits=8)            # one comm per FSDPModule, per-parameter table
+
+Both work over any number of nodes: across nodes they run in two stages, the semantics of
+``reduce_scatter_tensor`` and ``all_gather_into_tensor`` (functional.py).
 """
 from __future__ import annotations
 

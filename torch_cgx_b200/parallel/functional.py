@@ -108,7 +108,15 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int =
     optionally gives one shard's quantization table as ``(elem_off, numel, bits, bucket_size)``
     tuples relative to the shard start (bits 32: uncompressed); the same table applies to every
     shard. ``seed=None`` uses ``CGX_SEED``. ``output`` may be the rank's own chunk of ``input``.
-    Single node, CUDA float32 / float16 / bfloat16.
+    CUDA float32 / float16 / bfloat16.
+
+    Over several nodes (``local_size`` consecutive ranks each) the reduction has two stages: inside
+    each node, for every node's block of shards, the reduce-scatter above over the local ranks
+    (prescaled by 1/world when averaging; uncompressed with ``CGX_INTRA_COMPRESS=0``) gives the
+    node's partial sum of each shard; then across nodes, among the ranks of one local rank, the
+    same reduce-scatter of those partials: a rank's own node partial stays unquantized and every
+    other node's is quantized once. A local peer's values are thus quantized once and a remote
+    one's at most twice. With one rank per node it is the single-stage reduce-scatter over all ranks.
     """
     return _reduce_scatter(output, input, bits=bits, bucket_size=bucket_size, average=average, group=group,
                            async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
@@ -134,8 +142,13 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int 
     identical (at world 1 it is the quantization round trip of ``input``). ``layers`` optionally
     gives one shard's quantization table as ``(elem_off, numel, bits, bucket_size)`` tuples
     (bits 32: copied unchanged). Round to nearest unless ``stochastic``; ``seed=None`` uses
-    ``CGX_SEED``. ``input`` may be the rank's own chunk of ``output``. Single node, CUDA float32 /
-    float16 / bfloat16.
+    ``CGX_SEED``. ``input`` may be the rank's own chunk of ``output``. CUDA float32 / float16 /
+    bfloat16.
+
+    Over several nodes the owner's quantized bytes first go to the ranks of the same local rank on
+    the other nodes, which decode them; each node then shares the decoded shards among its ranks
+    uncompressed. Every shard is still quantized exactly once, so with round-to-nearest every
+    rank's ``output`` is the same as on one node.
     """
     return _all_gather(output, input, bits=bits, bucket_size=bucket_size, group=group, async_op=async_op,
                        stochastic=stochastic, seed=seed, layers=layers, overlapped=False)
