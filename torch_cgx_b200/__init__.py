@@ -37,6 +37,7 @@ from .parallel.fsdp import (  # noqa: E402
 )
 from .parallel.hooks import CGXState, cgx_hook, register_cgx_hook  # noqa: E402
 from .parallel.adaptive import AdaptiveCGXState  # noqa: E402
+from .parallel.adaptive_fsdp import AdaptiveFSDPState, set_cgx_adaptive  # noqa: E402
 from .utils.launch import map_launcher_env  # noqa: E402
 from . import models, ops, utils  # noqa: E402,F401
 
@@ -44,6 +45,7 @@ register_backend()
 
 __all__ = [
     "AdaptiveCGXState",
+    "AdaptiveFSDPState",
     "BACKEND_NAME",
     "CGXAllGather",
     "CGXReduceScatter",
@@ -61,6 +63,7 @@ __all__ = [
     "register_layer",
     "reset_layers",
     "set_quantization_bits",
+    "set_cgx_adaptive",
     "set_cgx_all_gather",
     "set_cgx_reduce_scatter",
     "set_quantization_bucket_size",

@@ -1079,11 +1079,11 @@ at::Tensor py_residual_relu_backward(const at::Tensor& y, const at::Tensor& ga, 
 // candidate width (engine/quant_error_table.h)
 at::Tensor py_quantization_error(const at::Tensor& t, const std::vector<LayerTuple>& layers,
                                  const std::vector<int64_t>& candidates, bool stochastic, double prescale,
-                                 bool skip_incomplete) {
+                                 bool skip_incomplete, int64_t chunks, int64_t skip_chunk) {
   std::vector<QErrSpan> spans;
   spans.reserve(layers.size());
   for (const auto& l : layers) spans.push_back({std::get<0>(l), std::get<1>(l), std::get<3>(l)});
-  return quantization_error_table(t, spans, candidates, stochastic, prescale, skip_incomplete);
+  return quantization_error_table(t, spans, candidates, stochastic, prescale, skip_incomplete, chunks, skip_chunk);
 }
 
 // ---- training BatchNorm on channels_last input ----
@@ -1467,7 +1467,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return out;
   });
   m.def("quantization_error", &py_quantization_error, py::arg("tensor"), py::arg("layers"), py::arg("candidates"),
-        py::arg("stochastic") = false, py::arg("prescale") = 1.0, py::arg("skip_incomplete") = false);
+        py::arg("stochastic") = false, py::arg("prescale") = 1.0, py::arg("skip_incomplete") = false,
+        py::arg("chunks") = 1, py::arg("skip_chunk") = -1);
   m.def("residual_relu_forward", &py_residual_relu_forward, py::arg("a"), py::arg("b"),
         "y = relu(a + b), bit-identical to the eager add + relu_");
   m.def("residual_relu_backward", &py_residual_relu_backward, py::arg("y"), py::arg("ga"), py::arg("gb") = py::none(),

@@ -17,6 +17,12 @@
 // then the 32 lane sums are combined by an xor butterfly (strides 16, 8, 4, 2, 1). The fp32 bucket
 // partials go into the fp64 layer total the same way: bucket j of the layer to lane j % 32, in order,
 // then the butterfly.
+//
+// Sharded mode (a reduce-scatter input): the tensor holds `chunks` copies of one shard's layer table
+// at stride S = numel / chunks, and chunk `skip_chunk` (the receiving rank's own, -1 for none) is
+// left out. Row l is the error of layer l summed over the included chunks: its fp32 bucket partials
+// form one list, chunk-major (included chunks in increasing order), then bucket, and list entry i
+// goes to lane i % 32 in order, then the butterfly. With chunks = 1 the list is the layer's buckets.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -106,20 +112,26 @@ inline void bucket_quantization_error(const float* x, uint32_t n, const int* bit
   }
 }
 
-// out[l * K + k]: the error of layer l at bits[k] (see the top of this file).
+// out[l * K + k]: the error of layer l at bits[k] (see the top of this file), summed over chunks
+// 0..chunks-1 at stride chunk_stride except skip_chunk (-1: none).
 inline void quantization_error(const void* t, int dtype, const std::vector<QErrLayer>& layers, const int* bits,
-                               int K, bool stochastic, float prescale, double* out) {
+                               int K, bool stochastic, float prescale, double* out, int chunks = 1,
+                               uint64_t chunk_stride = 0, int skip_chunk = -1) {
   std::vector<float> x(kMaxBlockElems);
   float part[kQErrMaxCandidates];
   for (size_t l = 0; l < layers.size(); ++l) {
     const QErrLayer& L = layers[l];
     double tot[kQErrMaxCandidates][kQErrLanes] = {};
-    uint64_t j = 0;
-    for (uint64_t o = 0; o < L.numel; o += L.bucket, ++j) {
-      const uint32_t n = (uint32_t)(L.numel - o < L.bucket ? L.numel - o : L.bucket);
-      for (uint32_t i = 0; i < n; ++i) x[i] = load_elem(t, dtype, L.elem_off + o + i) * prescale;
-      bucket_quantization_error(x.data(), n, bits, K, stochastic, part);
-      for (int k = 0; k < K; ++k) tot[k][j % kQErrLanes] += (double)part[k];
+    uint64_t j = 0;  // position in the layer's chunk-major list of bucket partials
+    for (int c = 0; c < chunks; ++c) {
+      if (c == skip_chunk) continue;
+      const uint64_t base = (uint64_t)c * chunk_stride + L.elem_off;
+      for (uint64_t o = 0; o < L.numel; o += L.bucket, ++j) {
+        const uint32_t n = (uint32_t)(L.numel - o < L.bucket ? L.numel - o : L.bucket);
+        for (uint32_t i = 0; i < n; ++i) x[i] = load_elem(t, dtype, base + o + i) * prescale;
+        bucket_quantization_error(x.data(), n, bits, K, stochastic, part);
+        for (int k = 0; k < K; ++k) tot[k][j % kQErrLanes] += (double)part[k];
+      }
     }
     for (int k = 0; k < K; ++k) out[l * K + k] = lane_butterfly(tot[k]);
   }

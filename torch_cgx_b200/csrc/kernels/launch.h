@@ -147,14 +147,19 @@ struct QErrArgs {
   int dtype;
   const QErrLayer* layer_table;   // [layers] device
   const uint64_t* first;          // [layers + 1] device: first bucket of every layer (qerr_first)
-  uint64_t nbuckets;              // first[layers], also on the host
+  uint64_t nbuckets;              // first[layers], also on the host: the buckets of one chunk
   int layers;
   const int* bits;           // [K] host: candidate widths, 1..8
   int K;                     // 1..8
   float prescale;
   bool stochastic;
-  float* partial;            // [nbuckets * K] device scratch
+  float* partial;            // [included chunks * nbuckets * K] device scratch
   double* out;               // [layers * K] device
+  // sharded mode (common/quant_error.h): `chunks` copies of the layer table at stride chunk_stride
+  // elements, chunk skip_chunk left out (-1: none); row l sums the included chunks
+  int chunks = 1;
+  uint64_t chunk_stride = 0;
+  int skip_chunk = -1;
 };
 cudaError_t launch_quantization_error(const QErrArgs& args, cudaStream_t stream);
 

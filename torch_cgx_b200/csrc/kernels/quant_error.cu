@@ -11,6 +11,12 @@
 // qerr_layers: one warp per (layer, candidate) adds the bucket partials into the fp64 layer total:
 // lane j % 32 takes bucket j in order, then an xor butterfly. No atomics: the result is the same bits
 // on every run, and the CPU's.
+//
+// Sharded mode (a reduce-scatter input: `chunks` copies of one shard's table at stride S, chunk
+// skip_chunk left out): qerr_buckets' index space is (included chunk j, shard bucket), b = j * nb +
+// bucket; the chunk is j, or j + 1 from skip_chunk on. qerr_layers reads layer l's partials as one
+// list, chunk-major then bucket, and lane i % 32 takes list entry i in order. With chunks = 1 both
+// are the single-chunk kernels above, bit for bit.
 #include "../common/quant_error.h"
 #include "item_path.cuh"
 #include "launch.h"
@@ -112,23 +118,26 @@ struct Cands {
 
 template <typename T, bool STOCH>
 __global__ void __launch_bounds__(kThreads) qerr_buckets(const T* __restrict__ t, const QErrLayer* __restrict__ layers,
-                                                         const uint64_t* __restrict__ first, int L, Cands cands, int K,
+                                                         const uint64_t* __restrict__ first, int L, uint64_t nb,
+                                                         uint64_t total, uint64_t stride, int skip, Cands cands, int K,
                                                          float prescale, float* __restrict__ partial) {
   const uint64_t b = (uint64_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-  if (b >= first[L]) return;
-  int lo = 0, hi = L - 1;  // the layer l with first[l] <= b < first[l + 1]
+  if (b >= total) return;
+  const uint64_t j = b / nb, sb = b - j * nb;  // included chunk, bucket of the shard table
+  const uint64_t c = (skip >= 0 && j >= (uint64_t)skip) ? j + 1 : j;
+  int lo = 0, hi = L - 1;  // the layer l with first[l] <= sb < first[l + 1]
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
-    if (first[mid] <= b)
+    if (first[mid] <= sb)
       lo = mid;
     else
       hi = mid - 1;
   }
   const QErrLayer ly = layers[lo];
-  const uint64_t o = (b - first[lo]) * ly.bucket;
+  const uint64_t o = (sb - first[lo]) * ly.bucket;
   const uint64_t left = ly.numel - o;
   const uint32_t n = left < ly.bucket ? (uint32_t)left : ly.bucket;
-  const T* p = t + ly.elem_off + o;
+  const T* p = t + c * stride + ly.elem_off + o;
   float* out = partial + b * (uint64_t)K;
   if (group_aligned<T>(p))
     bucket_error<T, true, STOCH>(p, n, prescale, cands.bits, K, out);
@@ -138,31 +147,43 @@ __global__ void __launch_bounds__(kThreads) qerr_buckets(const T* __restrict__ t
 
 __global__ void __launch_bounds__(kThreads) qerr_layers(const float* __restrict__ partial,
                                                         const uint64_t* __restrict__ first, int L, int K,
-                                                        double* __restrict__ out) {
+                                                        uint64_t nb, uint64_t included, double* __restrict__ out) {
   const int i = blockIdx.x * kWarps + (threadIdx.x >> 5);
   if (i >= L * K) return;
   const int l = i / K, k = i % K;
+  const uint64_t f = first[l], nbl = first[l + 1] - f, len = included * nbl;
   double acc = 0.0;
-  for (uint64_t b = first[l] + lane_id(); b < first[l + 1]; b += 32u) acc += (double)partial[b * (uint64_t)K + (uint64_t)k];
+  for (uint64_t e = lane_id(); e < len; e += 32u) {  // entry e of the chunk-major list: chunk e / nbl
+    const uint64_t j = e / nbl;
+    acc += (double)partial[(j * nb + f + (e - j * nbl)) * (uint64_t)K + (uint64_t)k];
+  }
 #pragma unroll
   for (int s = 16; s >= 1; s >>= 1) acc += __shfl_xor_sync(kAll, acc, s);
   if (lane_id() == 0) out[i] = acc;
 }
 
+uint64_t included_chunks(const QErrArgs& a) {
+  return (uint64_t)a.chunks - (a.skip_chunk >= 0 ? 1u : 0u);
+}
+
 template <typename T>
 void launch_buckets(const QErrArgs& a, const Cands& c, cudaStream_t s) {
-  const unsigned blocks = (unsigned)((a.nbuckets + kWarps - 1) / kWarps);
+  const uint64_t total = included_chunks(a) * a.nbuckets;
+  const unsigned blocks = (unsigned)((total + kWarps - 1) / kWarps);
   const T* t = static_cast<const T*>(a.data);
   if (a.stochastic)
-    qerr_buckets<T, true><<<blocks, kThreads, 0, s>>>(t, a.layer_table, a.first, a.layers, c, a.K, a.prescale, a.partial);
+    qerr_buckets<T, true><<<blocks, kThreads, 0, s>>>(t, a.layer_table, a.first, a.layers, a.nbuckets, total,
+                                                      a.chunk_stride, a.skip_chunk, c, a.K, a.prescale, a.partial);
   else
-    qerr_buckets<T, false><<<blocks, kThreads, 0, s>>>(t, a.layer_table, a.first, a.layers, c, a.K, a.prescale, a.partial);
+    qerr_buckets<T, false><<<blocks, kThreads, 0, s>>>(t, a.layer_table, a.first, a.layers, a.nbuckets, total,
+                                                       a.chunk_stride, a.skip_chunk, c, a.K, a.prescale, a.partial);
 }
 }  // namespace
 
 cudaError_t launch_quantization_error(const QErrArgs& a, cudaStream_t stream) {
   if (a.K < 1 || a.K > K8) return cudaErrorInvalidValue;
-  if (a.nbuckets > 0) {
+  if (a.chunks < 1 || a.skip_chunk < -1 || a.skip_chunk >= a.chunks) return cudaErrorInvalidValue;
+  if (a.nbuckets > 0 && included_chunks(a) > 0) {
     Cands c;
     for (int k = 0; k < K8; ++k) c.bits[k] = k < a.K ? a.bits[k] : 8;
     switch (a.dtype) {
@@ -175,7 +196,8 @@ cudaError_t launch_quantization_error(const QErrArgs& a, cudaStream_t stream) {
   }
   if (a.layers > 0) {
     const int n = a.layers * a.K;
-    qerr_layers<<<(n + kWarps - 1) / kWarps, kThreads, 0, stream>>>(a.partial, a.first, a.layers, a.K, a.out);
+    qerr_layers<<<(n + kWarps - 1) / kWarps, kThreads, 0, stream>>>(a.partial, a.first, a.layers, a.K, a.nbuckets,
+                                                                     included_chunks(a), a.out);
   }
   return cudaGetLastError();
 }

@@ -82,6 +82,8 @@ def quantization_error(
     stochastic: bool = False,
     prescale: float = 1.0,
     skip_incomplete: bool = False,
+    chunks: int = 1,
+    skip_chunk: int = -1,
 ) -> torch.Tensor:
     """Squared quantization error of every layer at every candidate width.
 
@@ -93,6 +95,14 @@ def quantization_error(
     ``x_i`` is the fp32 value after ``prescale``. A bucket with NaN / Inf makes its layer's row NaN.
     CUDA tensors run ``csrc/kernels/quant_error.cu``, CPU tensors its C++ oracle
     (``csrc/common/quant_error.h``); both give the same bits.
+
+    ``chunks > 1`` estimates what a reduce-scatter quantizes, in one launch: ``t`` holds ``chunks``
+    shards of ``t.numel() // chunks`` elements, ``layers`` is one shard's table (offsets from the
+    shard start, as in ``reduce_scatter_tensor``), and row ``l`` is layer ``l``'s error summed over
+    every shard except ``skip_chunk`` (the receiving rank's own, which is not quantized; -1 keeps
+    all). The sum runs chunk by chunk, then bucket by bucket, in the same order on the CPU and the
+    GPU. ``chunks=1`` is the plain table above, bit for bit.
     """
     return _C.quantization_error(t.view(-1), [tuple(int(v) for v in l) for l in layers],
-                                 [int(c) for c in candidates], stochastic, float(prescale), skip_incomplete)
+                                 [int(c) for c in candidates], stochastic, float(prescale), skip_incomplete,
+                                 int(chunks), int(skip_chunk))

@@ -21,7 +21,7 @@ native C++ hook (``csrc/pg/comm_hook.cc``) with the same results; ``assignment``
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -35,6 +35,39 @@ from .hooks import VALUE_NO_COMPRESS, CGXState, _allreduce_fut
 
 def _capturing() -> bool:
     return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+# (numels, bucket_sizes, budget_bytes, current widths, target_bits) of consecutive table rows
+AllocationPart = Tuple[Sequence[int], Sequence[int], int, Sequence[int], int]
+
+
+def _sum_allocate_broadcast(tables: Sequence[torch.Tensor], parts: Sequence[AllocationPart],
+                            candidate_bits: Sequence[int], group: dist.ProcessGroup,
+                            device: torch.device) -> Tuple[torch.Tensor, List[int]]:
+    """The decision step of the adaptive states: sum the concatenated float64 estimate tables over
+    ``group``, run one ``allocate_bits`` per part on group rank 0, broadcast its int32 widths.
+
+    ``tables`` are ``[rows, len(candidate_bits)]`` estimates in row order; ``parts`` split those
+    rows into consecutive ranges that are allocated separately. Returns the summed table (CPU,
+    ``[rows, K]``) and the broadcast width of every row, the same on every rank."""
+    K = len(candidate_bits)
+    table = torch.cat([t.reshape(-1) for t in tables])
+    # float64 never takes the compressed path: the sum does not depend on any CGX_* width setting
+    dist.all_reduce(table, group=group)
+    table = table.view(-1, K).cpu()
+    assert table.shape[0] == sum(len(p[0]) for p in parts)
+    choice = torch.zeros(table.shape[0], dtype=torch.int32)
+    if group.rank() == 0:
+        picked, r = [], 0
+        for numels, buckets, budget, current, target in parts:
+            n = len(numels)
+            picked += allocate_bits(table[r:r + n].numpy(), numels, buckets, candidate_bits, budget, current,
+                                    target_bits=target)
+            r += n
+        choice = torch.tensor(picked, dtype=torch.int32)
+    choice = choice.to(device)
+    dist.broadcast(choice, src=dist.get_global_rank(group, 0), group=group)
+    return table, choice.cpu().tolist()
 
 
 class AdaptiveCGXState(CGXState):
@@ -160,25 +193,17 @@ class AdaptiveCGXState(CGXState):
         if _capturing():
             raise RuntimeError("AdaptiveCGXState: a decision step cannot run during CUDA graph capture")
         keys = sorted(self._tables)
-        K = len(self.candidate_bits)
-        table = torch.cat([self._tables[k].reshape(-1) for k in keys])
+        tables = [self._tables[k] for k in keys]
         self._tables = {}
-        # float64 never takes the compressed path: the sum does not depend on any CGX_* width setting
-        dist.all_reduce(table, group=self.process_group)
-        table = table.view(-1, K).cpu()
         rows = [l for k in keys for l in self._by_bucket[k]]
-        assert table.shape[0] == len(rows)
         bs = self.quantization_bucket_size
-        choice = torch.zeros(len(rows), dtype=torch.int32)
-        if self.process_group.rank() == 0:
-            budget = sum(layer_wire_bytes(n, self.quantization_bits, bs) for (_, _, _, n) in rows)
-            current = [self.assignment.get((b, l), self.quantization_bits) for (b, l, _, _) in rows]
-            picked = allocate_bits(table.numpy(), [n for (_, _, _, n) in rows], [bs] * len(rows),
-                                   self.candidate_bits, budget, current, target_bits=self.quantization_bits)
-            choice = torch.tensor(picked, dtype=torch.int32)
-        choice = choice.to(self._device)
-        dist.broadcast(choice, src=dist.get_global_rank(self.process_group, 0), group=self.process_group)
-        for (b, l, _, _), bits in zip(rows, choice.cpu().tolist()):
+        numels = [n for (_, _, _, n) in rows]
+        budget = sum(layer_wire_bytes(n, self.quantization_bits, bs) for n in numels)
+        current = [self.assignment.get((b, l), self.quantization_bits) for (b, l, _, _) in rows]
+        table, choice = _sum_allocate_broadcast(
+            tables, [(numels, [bs] * len(rows), budget, current, self.quantization_bits)], self.candidate_bits,
+            self.process_group, self._device)
+        for (b, l, _, _), bits in zip(rows, choice):
             _backend.set_quantization_bits(b, l, bits)
             self.assignment[(b, l)] = bits
         self.last_errors = table

@@ -24,15 +24,30 @@ from .functional import _all_gather, _reduce_scatter
 RAW_BITS = 32
 
 
+Layer = Tuple[int, int, int, int]
+
+
+def _table(layers: Optional[Sequence[Layer]]) -> Optional[List[Layer]]:
+    return None if layers is None else [tuple(int(v) for v in l) for l in layers]
+
+
 class CGXReduceScatter(ReduceScatter):
     """FSDP2 reduce-scatter comm: SUM and AVG go through the compressed kernel (with at most
     ``CGX_OVERLAP_LANES`` CTAs, since FSDP overlaps it with backward); any other op, such as
-    premul-sum, goes to ``dist.reduce_scatter_tensor`` unchanged."""
+    premul-sum, goes to ``dist.reduce_scatter_tensor`` unchanged. ``layers`` optionally gives one
+    shard's table as ``(elem_off, numel, bits, bucket_size)`` tuples (None = one layer of ``bits`` /
+    ``bucket_size`` per shard). ``adaptive`` is an :class:`~torch_cgx_b200.AdaptiveFSDPState` that
+    rewrites ``layers``; ``set_cgx_adaptive`` sets it."""
 
-    def __init__(self, bits: int = 4, bucket_size: int = 512, stochastic: bool = False):
+    def __init__(self, bits: int = 4, bucket_size: int = 512, stochastic: bool = False,
+                 layers: Optional[Sequence[Layer]] = None, name: str = "", adaptive=None):
         self.bits = int(bits)
         self.bucket_size = int(bucket_size)
         self.stochastic = bool(stochastic)
+        self.layers = _table(layers)
+        self.name = name
+        self.numel = None if self.layers is None else sum(l[1] for l in self.layers)
+        self.adaptive = adaptive
 
     def allocate(self, size: Sequence[int], *, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
         return torch.empty(*size, dtype=dtype, device=device)
@@ -40,9 +55,15 @@ class CGXReduceScatter(ReduceScatter):
     def __call__(self, output_tensor: torch.Tensor, input_tensor: torch.Tensor, group: dist.ProcessGroup,
                  op, async_op: bool = False):
         if op == dist.ReduceOp.SUM or op == dist.ReduceOp.AVG:
+            if self.numel is not None and output_tensor.numel() != self.numel:
+                raise RuntimeError(
+                    f"cgx reduce-scatter of module '{self.name}': the shard has {output_tensor.numel()} elements "
+                    f"but its table covers {self.numel} (parameters changed after the comm was installed?)")
+            if self.adaptive is not None:
+                self.adaptive.maybe_estimate(self, input_tensor, group, average=op == dist.ReduceOp.AVG)
             return _reduce_scatter(output_tensor, input_tensor, bits=self.bits, bucket_size=self.bucket_size,
                                    average=op == dist.ReduceOp.AVG, group=group, async_op=async_op,
-                                   stochastic=self.stochastic, seed=None, layers=None, skip_incomplete=False,
+                                   stochastic=self.stochastic, seed=None, layers=self.layers, skip_incomplete=False,
                                    overlapped=True)
         return dist.reduce_scatter_tensor(output_tensor, input_tensor, op=op, group=group, async_op=async_op)
 
@@ -57,9 +78,6 @@ def set_cgx_reduce_scatter(model: torch.nn.Module, bits: int = 4, bucket_size: i
         if isinstance(m, FSDPModule):
             m.set_custom_reduce_scatter(comm)
     return comm
-
-
-Layer = Tuple[int, int, int, int]
 
 
 def fsdp_shard_table(params: Sequence[Tuple[Sequence[int], int]], bits: int = 4,
@@ -86,15 +104,17 @@ class CGXAllGather(AllGather):
     None = one layer of ``bits`` / ``bucket_size``), with at most ``CGX_OVERLAP_LANES`` CTAs since
     FSDP prefetches during compute. There is no stochastic rounding: the backward re-gather must
     see the weights the forward saw. A ``uint8`` buffer (FSDP2's all-gather of mixed-dtype inputs)
-    goes to ``dist.all_gather_into_tensor`` unchanged."""
+    goes to ``dist.all_gather_into_tensor`` unchanged. ``adaptive`` is an
+    :class:`~torch_cgx_b200.AdaptiveFSDPState` that rewrites ``layers``; ``set_cgx_adaptive`` sets it."""
 
     def __init__(self, bits: int = 4, bucket_size: int = 512, layers: Optional[Sequence[Layer]] = None,
-                 name: str = ""):
+                 name: str = "", adaptive=None):
         self.bits = int(bits)
         self.bucket_size = int(bucket_size)
-        self.layers = None if layers is None else [tuple(int(v) for v in l) for l in layers]
+        self.layers = _table(layers)
         self.name = name
         self.numel = None if self.layers is None else sum(l[1] for l in self.layers)
+        self.adaptive = adaptive
 
     def allocate(self, size: Sequence[int], *, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
         return torch.empty(*size, dtype=dtype, device=device)
@@ -107,6 +127,8 @@ class CGXAllGather(AllGather):
             raise RuntimeError(
                 f"cgx all-gather of module '{self.name}': the all-gather input has {input_tensor.numel()} elements "
                 f"but its shard table covers {self.numel} (parameters changed after set_cgx_all_gather?)")
+        if self.adaptive is not None:
+            self.adaptive.maybe_estimate(self, input_tensor, group, average=False)
         return _all_gather(output_tensor, input_tensor, bits=self.bits, bucket_size=self.bucket_size, group=group,
                            async_op=async_op, stochastic=False, seed=None, layers=self.layers, overlapped=True)
 
