@@ -10,6 +10,9 @@ set of buffers larger than L2, MAX over ranks, median of 3 repetitions.
                                                                             # vs ncclReduceScatter
   torchrun --nproc-per-node N bench/allreduce_sweep.py --op all_gather       # cgx.all_gather_into_tensor
                                                                             # vs ncclAllGather
+  torchrun --nproc-per-node N bench/allreduce_sweep.py --op all_to_all       # cgx.all_to_all_single
+                                                                            # vs dist.all_to_all_single (NCCL)
+With --op all_to_all the message is a rank's input of W equal chunks.
 With --op reduce_scatter the message is the input of W shards, with --op all_gather the gathered
 output of W shards; NCCL's bus bandwidth is then algbw * (W-1)/W, and wire_bytes_per_rank counts
 the packed chunks this rank sends.
@@ -79,7 +82,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--bucket-size", type=int, default=512)
     ap.add_argument("--sizes", default="", help="explicit comma-separated sizes in KB (overrides min/max)")
-    ap.add_argument("--op", default="allreduce", choices=["allreduce", "reduce_scatter", "all_gather"])
+    ap.add_argument("--op", default="allreduce", choices=["allreduce", "reduce_scatter", "all_gather", "all_to_all"])
     ap.add_argument("--with-nccl-sra", action="store_true",
                     help="also time the reference-structure path: SRA over NCCL send/recv + separate kernels")
     args = ap.parse_args()
@@ -112,7 +115,7 @@ def main():
         s *= 4
     if args.sizes:
         sizes = [int(x) << 10 for x in args.sizes.split(",")]
-    rs = args.op in ("reduce_scatter", "all_gather")  # one shard per rank: the message is W shards
+    rs = args.op in ("reduce_scatter", "all_gather", "all_to_all")  # one shard per rank: the message is W shards
     bus = (world - 1) / world if rs else 2 * (world - 1) / world
     if args.op == "reduce_scatter":
         sizes = [s for s in sizes if s // es >= world]
@@ -141,6 +144,18 @@ def main():
             s = x.numel() // world
             cgx.all_gather_into_tensor(out_for(x), x[rank * s:(rank + 1) * s], bits=bits,
                                        bucket_size=args.bucket_size)
+    elif args.op == "all_to_all":
+        sizes = [s for s in sizes if s // es >= world]
+        outs = {}
+
+        def out_for(x):
+            return outs.setdefault(x.numel(), torch.empty(x.numel(), dtype=x.dtype, device=dev))
+
+        def nccl_op(x):
+            dist.all_to_all_single(out_for(x), x, group=nccl)
+
+        def cgx_op(x, bits):
+            cgx.all_to_all_single(out_for(x), x, bits=bits, bucket_size=args.bucket_size)
     else:
         def nccl_op(x):
             dist.all_reduce(x, group=nccl)

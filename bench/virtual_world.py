@@ -6,7 +6,13 @@ compute / HBM efficiency of the fused kernel at W > 1 without multi-GPU time.
 The same for the compressed reduce-scatter (rows with "op": "reduce_scatter"): `mb` MB of input
 per virtual rank, one shard of mb / W MB out; and for the compressed all-gather (rows with
 "op": "all_gather"): one shard of mb / W MB in per virtual rank, `mb` MB out.
-Reports the slope between two sizes (harness overhead cancels)."""
+Reports the slope between two sizes (harness overhead cancels).
+
+--op all_to_all times the compressed all-to-all (a2a_kernel) instead: `mb` MB of input per virtual
+rank in W chunks, with equal splits and with skewed ones (chunk q -> r gets a share proportional to
+1 + (r - q) mod W, so every rank still sends and receives `mb` MB but pairs differ up to W : 1),
+next to the reduce-scatter (rs_kernel) of the same `mb` MB input per rank, same dtype, bits and
+bucket. Both move the same packed bytes; the reduce-scatter also accumulates."""
 import argparse
 import json
 import sys
@@ -44,12 +50,21 @@ def main():
     ap.add_argument("--bucket", type=int, default=512)
     ap.add_argument("--mbs", default="8,32")
     ap.add_argument("--out", default="gpurun_out/virtual_world.json")
+    ap.add_argument("--op", default="sra", choices=["sra", "all_to_all"],
+                    help="sra: allreduce, reduce-scatter and all-gather rows; all_to_all: a2a next to rs_kernel")
+    ap.add_argument("--dtypes", default="float32", help="--op all_to_all: comma-separated dtypes")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     W = args.world
     lanes = 264 // W
     rows = []
     sampler = ClockSampler(0).start()
+    if args.op == "all_to_all":
+        rows = all_to_all_rows(args, dev, W, lanes)
+        clocks = sampler.stop()
+        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
+        return
     for bits in [int(b) for b in args.bits.split(",")]:
         res = {}
         for mb in [int(x) for x in args.mbs.split(",")]:
@@ -113,6 +128,50 @@ def main():
     clocks = sampler.stop()
     Path(args.out).parent.mkdir(parents=True, exist_ok=True)
     Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
+
+
+def skewed_counts(W, n):
+    """counts[q][r] ~ 1 + (r - q) mod W, every row and column summing to n (a Latin square)."""
+    tot = W * (W + 1) // 2
+    base = [n * (1 + k) // tot for k in range(W)]
+    base[-1] += n - sum(base)
+    return [[base[(r - q) % W] for r in range(W)] for q in range(W)]
+
+
+def all_to_all_rows(args, dev, W, lanes):
+    rows = []
+    for dtype in [getattr(torch, d) for d in args.dtypes.split(",")]:
+        es = torch.empty((), dtype=dtype).element_size()
+        for bits in [int(b) for b in args.bits.split(",")]:
+            for mb in [int(x) for x in args.mbs.split(",")]:
+                n = (mb << 20) // es // W * W
+                slot = n * es // W * 2 + (1 << 20)
+                row = {"op": "all_to_all", "world": W, "dtype": str(dtype).replace("torch.", ""), "bits": bits,
+                       "bucket": args.bucket, "mb_per_rank": mb, "lanes_per_rank": lanes}
+                g = C.LocalSraGroup(W, lanes, slot, 20000, 4096)
+                xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
+                for kind, c in (("equal", [[n // W] * W for _ in range(W)]), ("skewed", skewed_counts(W, n))):
+                    outs = [torch.empty(sum(c[q][r] for q in range(W)), device=dev, dtype=dtype) for r in range(W)]
+                    g.all_to_all(xs, outs, c, bits=bits, bucket_size=args.bucket)
+                    torch.cuda.synchronize()
+                    g.check()
+                    row[f"a2a_{kind}_us"] = round(timeit(lambda: g.all_to_all(xs, outs, c, bits=bits,
+                                                                              bucket_size=args.bucket)), 1)
+                    del outs
+                shard = [(0, n // W, bits, args.bucket)]
+                routs = [torch.empty(n // W, device=dev, dtype=dtype) for _ in range(W)]
+                g.reduce_scatter(xs, routs, shard)
+                torch.cuda.synchronize()
+                g.check()
+                row["rs_us"] = round(timeit(lambda: g.reduce_scatter(xs, routs, shard)), 1)
+                row["a2a_equal_over_rs"] = round(row["a2a_equal_us"] / row["rs_us"], 3)
+                row["note"] = ("W virtual ranks on one GPU, all W kernels of a call: the device work of W real ranks, "
+                               "NVLink excluded; rs = rs_kernel on the same mb MB input per rank")
+                del g, xs, routs
+                torch.cuda.empty_cache()
+                rows.append(row)
+                print(json.dumps(row), flush=True)
+    return rows
 
 
 if __name__ == "__main__":

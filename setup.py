@@ -40,6 +40,9 @@ SOURCES = [
     "kernels/ag_f32.cu",
     "kernels/ag_f16.cu",
     "kernels/ag_bf16.cu",
+    "kernels/a2a_f32.cu",
+    "kernels/a2a_f16.cu",
+    "kernels/a2a_bf16.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
     "kernels/residual_relu.cu",

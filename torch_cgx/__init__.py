@@ -3,6 +3,8 @@ registers the ``cgx`` backend and exposes ``register_layer`` /
 ``set_quantization_bits`` / ``set_quantization_bucket_size``
 (/root/reference/src/ProcessGroupCGX.cc:852-857, README.md:40-48)."""
 from torch_cgx_b200 import (  # noqa: F401
+    all_to_all_single,
+    differentiable_all_to_all_single,
     register_backend,
     register_layer,
     reset_layers,

@@ -27,7 +27,14 @@ from .backend import (  # noqa: E402
     set_quantization_bits,
     set_quantization_bucket_size,
 )
-from .parallel.functional import all_gather_into_tensor, all_reduce, compression, reduce_scatter_tensor  # noqa: E402
+from .parallel.functional import (  # noqa: E402
+    all_gather_into_tensor,
+    all_reduce,
+    all_to_all_single,
+    compression,
+    differentiable_all_to_all_single,
+    reduce_scatter_tensor,
+)
 from .parallel.fsdp import (  # noqa: E402
     CGXAllGather,
     CGXReduceScatter,
@@ -60,6 +67,8 @@ __all__ = [
     "register_backend",
     "register_cgx_hook",
     "reduce_scatter_tensor",
+    "all_to_all_single",
+    "differentiable_all_to_all_single",
     "register_layer",
     "reset_layers",
     "set_quantization_bits",

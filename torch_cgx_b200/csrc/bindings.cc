@@ -28,6 +28,7 @@
 
 #include "comm/fd_channel.h"
 #include "comm/loopback_communicator.h"
+#include "common/a2a.h"
 #include "common/bit_allocation.h"
 #include "common/block_ops.h"
 #include "common/config.h"
@@ -228,6 +229,112 @@ void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
                        make_rng(stochastic, seed, seq), q, 1);
   }
   for (int r = 1; r < W; ++r) std::memcpy(outputs[r].data_ptr(), out0, S * W * es);
+}
+
+// ---- all-to-all: counts[q][r] elements go from rank q to rank r ------------------------------
+using CountMatrix = std::vector<std::vector<int64_t>>;
+
+std::vector<std::vector<uint64_t>> check_counts(const CountMatrix& counts, size_t W) {
+  TORCH_CHECK(counts.size() == W, "all_to_all: counts must be a W x W matrix");
+  std::vector<std::vector<uint64_t>> out(W, std::vector<uint64_t>(W));
+  for (size_t q = 0; q < W; ++q) {
+    TORCH_CHECK(counts[q].size() == W, "all_to_all: counts must be a W x W matrix");
+    for (size_t r = 0; r < W; ++r) {
+      TORCH_CHECK(counts[q][r] >= 0, "all_to_all: negative count");
+      out[q][r] = (uint64_t)counts[q][r];
+    }
+  }
+  return out;
+}
+
+// rank r's input holds row r of the matrix, its output column r
+void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<at::Tensor>& outputs,
+                       const std::vector<std::vector<uint64_t>>& counts, bool cuda) {
+  const size_t W = counts.size();
+  TORCH_CHECK(inputs.size() == W && outputs.size() == W, "all_to_all: one input and one output per rank");
+  const int dt = cgx_dtype(inputs[0]);
+  for (size_t r = 0; r < W; ++r) {
+    uint64_t nin = 0, nout = 0;
+    for (size_t q = 0; q < W; ++q) {
+      nin += counts[r][q];
+      nout += counts[q][r];
+    }
+    for (const at::Tensor* t : {&inputs[r], &outputs[r]})
+      TORCH_CHECK(t->is_cuda() == cuda && t->is_contiguous() && cgx_dtype(*t) == dt,
+                  "all_to_all: contiguous tensors of one dtype, all on ", cuda ? "the GPU" : "the CPU");
+    TORCH_CHECK((uint64_t)inputs[r].numel() == nin && (uint64_t)outputs[r].numel() == nout,
+                "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
+  }
+}
+
+void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
+                            const CountMatrix& counts_in, int bits, int64_t bucket, bool stochastic, uint64_t seed,
+                            uint32_t seq) {
+  const auto counts = check_counts(counts_in, inputs.size());
+  check_a2a_tensors(inputs, outputs, counts, false);
+  std::vector<const void*> in;
+  std::vector<void*> out;
+  for (size_t r = 0; r < inputs.size(); ++r) {
+    in.push_back(inputs[r].data_ptr());
+    out.push_back(outputs[r].data_ptr());
+  }
+  all_to_all_simulate(cgx_dtype(inputs[0]), in, out, counts, bits, (uint32_t)bucket, make_rng(stochastic, seed, seq));
+}
+
+// the items of one chunk from common/a2a.h, rows as in plan_to_dict, offsets in the contiguous image
+at::Tensor py_a2a_items(int64_t n, int bits, int64_t bucket, int dtype) {
+  const A2aGeom g = a2a_geom((uint32_t)n, bits, (uint32_t)bucket, dtype_size(dtype));
+  std::vector<WarpItem> its;
+  for (uint32_t b = 0; b < a2a_num_blocks(g); ++b)
+    for (uint32_t j = 0; j < a2a_block_num_items(g, a2a_block_n(g, b)); ++j) {
+      WarpItem it = a2a_block_item(g, b, j);
+      it.meta_off += b * g.block_wire;
+      it.pay_off += b * g.block_wire;
+      its.push_back(it);
+    }
+  auto items = at::empty({(int64_t)its.size(), 7}, at::kLong);
+  auto* ip = items.data_ptr<int64_t>();
+  for (size_t i = 0; i < its.size(); ++i) {
+    ip[i * 7 + 0] = its[i].elem_off;
+    ip[i * 7 + 1] = its[i].meta_off;
+    ip[i * 7 + 2] = its[i].pay_off;
+    ip[i * 7 + 3] = item_kind(its[i]);
+    ip[i * 7 + 4] = item_lpb_log2(its[i]);
+    ip[i * 7 + 5] = item_bits(its[i]);
+    ip[i * 7 + 6] = item_n(its[i]);
+  }
+  return items;
+}
+
+// The windows of one chunk: for every lane, a list of windows, each a list of its blocks as
+// (first element, elements, wire bytes); plus the lane's share of a slot.
+py::dict py_a2a_windows(int64_t n, int bits, int64_t bucket, int dtype, int64_t slot_bytes, int lanes) {
+  TORCH_CHECK(lanes >= 1, "a2a_windows: lanes must be >= 1");
+  const A2aGeom g = a2a_geom((uint32_t)n, bits, (uint32_t)bucket, dtype_size(dtype));
+  const uint32_t share = a2a_lane_slot_bytes((uint32_t)slot_bytes, lanes);
+  const uint32_t bpw = a2a_window_blocks(g, share);
+  py::dict d;
+  d["lane_slot"] = share;
+  d["window_blocks"] = bpw;
+  d["block_elems"] = g.block_elems;
+  d["block_wire"] = g.block_wire;
+  std::vector<std::vector<std::vector<std::tuple<int64_t, int64_t, int64_t>>>> lanes_out(lanes);
+  if (bpw > 0) {
+    for (int c = 0; c < lanes; ++c) {
+      const uint32_t nw = a2a_lane_windows(g, c, lanes, bpw);
+      const uint32_t lb = a2a_lane_blocks(a2a_num_blocks(g), c, lanes);
+      for (uint32_t k = 0; k < nw; ++k) {
+        std::vector<std::tuple<int64_t, int64_t, int64_t>> w;
+        for (uint32_t j = k * bpw; j < lb && j < (k + 1) * bpw; ++j) {
+          const uint32_t b = (uint32_t)c + j * (uint32_t)lanes, bn = a2a_block_n(g, b);
+          w.emplace_back((int64_t)b * g.block_elems, (int64_t)bn, (int64_t)block_wire_bytes(bn, g.bits, g.bucket, g.elsize));
+        }
+        lanes_out[c].push_back(std::move(w));
+      }
+    }
+  }
+  d["lanes"] = lanes_out;
+  return d;
 }
 
 // quantize `t` through the plan; returns uint8 wire tensor [world, row_bytes]
@@ -439,6 +546,22 @@ class LocalSraGroup {
                   const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq) {
     sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq);
   }
+  // all-to-all: counts[q][r] elements go from virtual rank q to r; inputs[r] holds row r of the
+  // matrix in destination order, outputs[r] receives column r in source order
+  void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
+                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+    const auto counts = check_counts(counts_in, (size_t)world_);
+    check_a2a_tensors(inputs, outputs, counts, true);
+    const int dt = cgx_dtype(inputs[0]);
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    fork_join([](int) {},
+              [&](int r) {
+                std::vector<uint64_t> out_counts(world_);
+                for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
+                fused_[r]->all_to_all(inputs[r].data_ptr(), outputs[r].data_ptr(), counts[r], out_counts, dt, bits,
+                                      (uint32_t)bucket, rng, streams_[r].stream());
+              });
+  }
   void check() {
     for (auto& f : fused_) f->check_status();
   }
@@ -575,6 +698,18 @@ class LocalReducerGroup {
       red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s);
     });
   }
+  // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
+  void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
+                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+    const auto counts = check_counts(counts_in, (size_t)hub_.world());
+    check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda());
+    const RngParams rng = make_rng(stochastic, seed, seq);
+    run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
+      std::vector<uint64_t> out_counts(counts.size());
+      for (size_t q = 0; q < counts.size(); ++q) out_counts[q] = counts[q][r];
+      red.all_to_all(in, outputs[r].data_ptr(), counts[r], out_counts, dt, bits, (uint32_t)bucket, rng, s);
+    }, false);
+  }
   // bytes each rank's reducer counted as sent during the last call
   std::vector<int64_t> bytes_sent() const { return last_sent_; }
   void set_recording(bool on) { record_ = on; }
@@ -623,15 +758,16 @@ class LocalReducerGroup {
     }
   }
 
+  // same_size false: the ranks' tensors may differ in size (all_to_all)
   template <class F>
-  void run(const std::vector<at::Tensor>& tensors, F&& op) {
+  void run(const std::vector<at::Tensor>& tensors, F&& op, bool same_size = true) {
     const int W = hub_.world();
     TORCH_CHECK((int)tensors.size() == W, "LocalReducerGroup: need one tensor per virtual rank (", W, "), got ",
                 tensors.size());
     const int dt = cgx_dtype(tensors[0]);
     const bool cuda = tensors[0].is_cuda();
     for (const at::Tensor& t : tensors)
-      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && t.numel() == tensors[0].numel() &&
+      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && (!same_size || t.numel() == tensors[0].numel()) &&
                       t.device() == tensors[0].device(),
                   "LocalReducerGroup: contiguous tensors of one dtype, size and device");
     TORCH_CHECK(cuda || tensors[0].device().is_cpu(), "LocalReducerGroup: CPU or CUDA tensors");
@@ -1255,6 +1391,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("output"), py::arg("input"), py::arg("bits") = 4, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("overlapped") = false,
            py::arg("layers") = std::vector<LayerTuple>{}, py::call_guard<py::gil_scoped_release>())
+      .def("all_to_all_compressed",
+           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
+              const std::vector<int64_t>& in_splits, int bits, int bucket_size, bool stochastic, int64_t seed) {
+             return pg.all_to_all_compressed(out, in, out_splits, in_splits, bits, bucket_size, stochastic, seed);
+           },
+           py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
+           py::arg("input_split_sizes") = std::vector<int64_t>{}, py::arg("bits") = 8, py::arg("bucket_size") = 512,
+           py::arg("stochastic") = false, py::arg("seed") = -1, py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -1426,6 +1570,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
         py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048,
         py::arg("prescale") = py::none());
+  m.def("all_to_all_simulate", &py_all_to_all_simulate, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
+        py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
+        py::arg("seq") = 0);
+  m.def("a2a_items", &py_a2a_items, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
+  m.def("a2a_windows", &py_a2a_windows, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype"),
+        py::arg("slot_bytes"), py::arg("lanes"));
   m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0);
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
@@ -1522,6 +1672,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
       .def("all_gather", &LocalSraGroup::all_gather, py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers"),
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
+      .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
+           py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
+           py::arg("seq") = 0)
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))
@@ -1541,6 +1694,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("reduce_scatter", &LocalReducerGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none())
+      .def("all_to_all", &LocalReducerGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
+           py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
+           py::arg("seq") = 0)
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0)

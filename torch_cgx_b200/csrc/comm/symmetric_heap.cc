@@ -63,7 +63,11 @@ HeapLayout HeapLayout::make(int world, int max_lanes, size_t slot_bytes, size_t 
   l.recv2_off = l.recv1_off + (size_t)world * slot;
   l.os_off[0] = l.recv2_off + (size_t)world * slot;
   l.os_off[1] = l.os_off[0] + (size_t)world * os_slot;
-  l.total = l.os_off[1] + (size_t)world * os_slot;
+  // the all-to-all's flags go last, so every region the other kernels use keeps its offset
+  const size_t flags64_bytes = round_up((size_t)world * l.flag_stride * sizeof(uint64_t), 256);
+  l.a2a_landed_off = l.os_off[1] + (size_t)world * os_slot;
+  l.a2a_released_off = l.a2a_landed_off + flags64_bytes;
+  l.total = l.a2a_released_off + flags64_bytes;
   return l;
 }
 

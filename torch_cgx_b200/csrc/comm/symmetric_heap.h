@@ -1,6 +1,6 @@
 // Symmetric peer-mapped device heap: the H100 replacement for the reference's
 // three point-to-point transports. Every rank owns ONE region
-//   [sync][flags1][flags2][recv1: W slots][recv2: W slots][one-shot A: W slots][one-shot B: W slots]
+//   [sync][flags1][flags2][recv1: W slots][recv2: W slots][one-shot A: W slots][one-shot B: W slots][a2a landed][a2a released]
 // and maps every peer's region into its own address space, so kernels move data with ordinary
 // ld/st over NVLink 4 / NVSwitch and signal with release/acquire flags -- no host staging, no
 // semaphores, no MPI.
@@ -35,7 +35,8 @@ struct HeapLayout {
   uint32_t flag_stride = 0;  // lanes capacity (multiple of 32)
   uint32_t slot_bytes = 0;   // bytes per (source rank) slot, multiple of 256
   uint32_t os_slot_bytes = 0;  // per-source slot of the two one-shot regions
-  size_t sync_off = 0, flags1_off = 0, flags2_off = 0, recv1_off = 0, recv2_off = 0, os_off[2] = {0, 0}, total = 0;
+  // a2a_landed / a2a_released: the all-to-all's 64-bit window flags, [source * flag_stride + lane]
+  size_t sync_off = 0, flags1_off = 0, flags2_off = 0, a2a_landed_off = 0, a2a_released_off = 0, recv1_off = 0, recv2_off = 0, os_off[2] = {0, 0}, total = 0;
   // throws std::invalid_argument when a slot size does not fit the 32-bit offsets kernels use
   static HeapLayout make(int world, int max_lanes, size_t slot_bytes, size_t os_slot_bytes = 0);
 };
@@ -77,6 +78,10 @@ class SymmetricHeap {
   uint8_t* oneshot(int peer, int parity) const { return bases_[peer] + layout_.os_off[parity & 1]; }
   uint32_t* flags1(int peer) const { return reinterpret_cast<uint32_t*>(bases_[peer] + layout_.flags1_off); }
   uint32_t* flags2(int peer) const { return reinterpret_cast<uint32_t*>(bases_[peer] + layout_.flags2_off); }
+  uint64_t* a2a_landed(int peer) const { return reinterpret_cast<uint64_t*>(bases_[peer] + layout_.a2a_landed_off); }
+  uint64_t* a2a_released(int peer) const {
+    return reinterpret_cast<uint64_t*>(bases_[peer] + layout_.a2a_released_off);
+  }
   // multicast aliases (nullptr without NVLS)
   uint8_t* mc_recv1() const { return mc_base_ ? mc_base_ + layout_.recv1_off : nullptr; }
   uint8_t* mc_recv2() const { return mc_base_ ? mc_base_ + layout_.recv2_off : nullptr; }

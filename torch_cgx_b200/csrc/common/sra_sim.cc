@@ -1,6 +1,9 @@
 #include "sra_sim.h"
 
+#include <cstring>
 #include <stdexcept>
+
+#include "a2a.h"
 
 #include "block_ops.h"
 
@@ -67,6 +70,49 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
     }
     for (int p = 0; p < W; ++p)
       for (uint32_t i = 0; i < n; ++i) cpu::store_elem(bufs[p], plan.dtype, (uint64_t)d.elem_off + i, acc[i]);
+  }
+}
+
+void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, const std::vector<void*>& out_bufs,
+                         const std::vector<std::vector<uint64_t>>& counts, int bits, uint32_t bucket,
+                         const RngParams& rng) {
+  const int W = (int)in_bufs.size();
+  if ((int)out_bufs.size() != W || (int)counts.size() != W)
+    throw std::invalid_argument("all_to_all_simulate: need one input, output and count row per rank");
+  for (const auto& row : counts)
+    if ((int)row.size() != W) throw std::invalid_argument("all_to_all_simulate: counts must be W x W");
+  const int es = dtype_size(dtype);
+  std::vector<float> acc(kMaxBlockElems);
+  std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
+  for (int q = 0; q < W; ++q) {
+    uint64_t in_off = 0;
+    for (int r = 0; r < W; ++r) {
+      uint64_t out_off = 0;
+      for (int s = 0; s < q; ++s) out_off += counts[s][r];
+      const uint64_t n = counts[q][r];
+      const uint8_t* src = static_cast<const uint8_t*>(in_bufs[q]) + in_off * es;
+      uint8_t* dst = static_cast<uint8_t*>(out_bufs[r]) + out_off * es;
+      in_off += n;
+      if (n == 0) continue;
+      if (q == r || bits >= kRawBits) {
+        std::memcpy(dst, src, n * es);
+        continue;
+      }
+      if (n >= (1ull << 32)) throw std::invalid_argument("all_to_all_simulate: chunk exceeds 2^32 elements");
+      const A2aGeom g = a2a_geom((uint32_t)n, bits, bucket, es);
+      RngKey key = make_rng_key(rng, q, 0);
+      key.stream = a2a_rng_stream(q, r);
+      for (uint32_t b = 0; b < a2a_num_blocks(g); ++b) {
+        BlockDesc d;
+        d.elem_off = b * g.block_elems;
+        d.wire_off = 0;
+        d.n_bits = (a2a_block_n(g, b) & 0xFFFFFFu) | ((uint32_t)g.bits << 24);
+        d.bucket = g.bucket;
+        cpu::load_block(src, dtype, d, 1.0f, acc.data());
+        cpu::quantize_block(acc.data(), dtype, d, rec.data(), key, b);
+        cpu::decode_block_store(rec.data(), dtype, d, dst);
+      }
+    }
   }
 }
 

@@ -3,7 +3,9 @@
 #include "../common/nvtx.h"
 
 #include <algorithm>
+#include <cstring>
 #include <stdexcept>
+#include <string>
 
 namespace cgx {
 
@@ -315,6 +317,49 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
                   at(out, (size_t)n * L * shard_bytes), dtype, S, intra_table, skip_incomplete, 1.0f, rng, stream,
                   overlapped);
   }
+}
+
+void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                                 const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
+                                 const RngParams& rng_in, cudaStream_t stream) {
+  if (nodes() > 1)
+    throw std::runtime_error("cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE " +
+                             std::to_string(local_size_) + " < world size " + std::to_string(world_) + ")");
+  GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  const bool fused = fused_sharded(cuda);
+  if (fused) fused_->check_status();
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rank_, world_);
+  if (!fused && world_ > 1 && !g.intra) throw std::runtime_error("cgx: the compressed all_to_all has no intra-node reducer");
+  uint64_t total = 0;
+  for (uint64_t n : in_counts) total += n;
+  NvtxRange range("cgx:all_to_all_cuda", total);
+  ++call_seq_;
+  ++stats_.calls;
+  RngParams rng = rng_in;
+  rng.seq = call_seq_ << 4;
+  stats_.elements += total;
+  if (fused) {
+    const FusedSra::A2aCounts n =
+        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream);
+    stats_.kernel_launches += n.launches;
+    stats_.wire_bytes += n.wire_bytes;
+    stats_.raw_bytes += n.raw_bytes;
+    return;
+  }
+  if (world_ == 1) {
+    const size_t bytes = (size_t)in_counts[0] * (size_t)dtype_size(dtype);
+    if (bytes == 0) return;
+    if (cuda)
+      cuda_check(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, stream), "all_to_all copy");
+    else
+      std::memcpy(out, in, bytes);
+    return;
+  }
+  const uint64_t before = g.intra->bytes_sent();
+  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream);
+  stats_.wire_bytes += g.intra->bytes_sent() - before;
+  for (int q = 0; q < world_; ++q)
+    if (q != rank_) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);
 }
 
 void AllreduceEngine::allreduce_cpu(void* data, int dtype, int64_t numel, bool average, int explicit_bucket) {

@@ -155,6 +155,13 @@ class AllreduceEngine {
   void prepare_sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                        cudaStream_t stream);
 
+  // Compressed all-to-all of device (cuda) or host buffers on `stream` (FusedSra::all_to_all for
+  // the arguments): the fused kernel on the P2P transport, else the generic intra-node reducer. One
+  // node only: with several nodes every rank throws the same std::runtime_error before anything runs.
+  void all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                  const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
+                  const RngParams& rng_in, cudaStream_t stream);
+
   void check_health();
   void set_observer(EngineObserver* o) { observer_ = o; }
   const EngineStats& stats() const { return stats_; }

@@ -68,6 +68,41 @@ int sra_max_resident_ctas(int dtype);
 // three-phase SRA
 cudaError_t launch_sra_fused(const SraParams& p, cudaStream_t stream);
 
+// ---- compressed all-to-all (a2a_kernel.cuh) ------------------------------------
+// One launch per call, whatever the splits: every chunk's items and windows are derived on the
+// device from (elements, bits, bucket, dtype) (common/a2a.h), so nothing is uploaded per call.
+struct A2aParams {
+  const void* in;                  // T*: my chunks, in destination order
+  void* out;                       // T*: the chunks I receive, in source order
+  uint32_t in_off[kMaxPeers];      // my chunk for rank q: elements [in_off[q], in_off[q] + in_cnt[q]) of `in`
+  uint32_t in_cnt[kMaxPeers];
+  uint32_t out_off[kMaxPeers];     // rank q's chunk for me: elements [out_off[q], + out_cnt[q]) of `out`
+  uint32_t out_cnt[kMaxPeers];
+  int rank;
+  int world;
+  int lanes;                       // == gridDim.x, the same on every rank
+  int dtype;
+  int bits;                        // 1..8, or >= 32 for raw
+  uint32_t bucket;                 // as requested (a2a_geom clamps it)
+  uint32_t epoch_hint;             // host mirror of the epoch (advances the RNG sequence on graph replay)
+  RngKey rng;                      // .stream is filled in per pair (a2a_rng_stream)
+  uint32_t slot_bytes;             // stride between per-source slots inside recv
+  uint32_t lane_slot;              // a lane's share of a slot (a2a_lane_slot_bytes)
+  uint32_t flag_stride;
+  uint8_t* recv[kMaxPeers];        // recv[p]: base of rank p's recv1 region (peer-mapped)
+  uint32_t* flags2[kMaxPeers];     // closing handshake, as rs_kernel / ag_kernel
+  uint64_t* landed[kMaxPeers];     // landed[p][src * flag_stride + lane]: window of src landed in p's slot
+  uint64_t* released[kMaxPeers];   // released[p][dst * flag_stride + lane]: dst is done with p's window
+  uint32_t* status;
+  const uint32_t* abort_word;
+  uint64_t timeout_ns;
+  DeviceSync* sync;
+};
+// defined once per dtype in a2a_{f32,f16,bf16}.cu
+cudaError_t launch_a2a_f32(const A2aParams& p, cudaStream_t stream);
+cudaError_t launch_a2a_f16(const A2aParams& p, cudaStream_t stream);
+cudaError_t launch_a2a_bf16(const A2aParams& p, cudaStream_t stream);
+
 // ---- standalone item kernels (generic reducers, Python ops, tests, cross-node path) ----
 // All operate on items [first, first+count) of a device item table; `wire` is the base of the
 // chunk's wire slot (records live at wire + item offsets). `slice_elems` / `uniform_bits` are

@@ -429,6 +429,70 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
                       });
 }
 
+namespace {
+
+// per-rank element counts of one side of an all_to_all_single, from its dim-0 splits
+std::vector<uint64_t> a2a_counts(const at::Tensor& t, const std::vector<int64_t>& splits, int world, int64_t row,
+                                 const char* side) {
+  const int64_t rows = t.dim() > 0 ? t.size(0) : 0;
+  std::vector<uint64_t> counts((size_t)world);
+  if (splits.empty()) {
+    TORCH_CHECK(rows % world == 0, "cgx: all_to_all: the ", side, " has ", rows,
+                " rows, not divisible by the world size ", world, " (give ", side, "_split_sizes)");
+    for (auto& c : counts) c = (uint64_t)(rows / world * row);
+    return counts;
+  }
+  TORCH_CHECK((int)splits.size() == world, "cgx: all_to_all: ", side, "_split_sizes has ", splits.size(),
+              " entries, expected the world size ", world);
+  int64_t sum = 0;
+  for (int q = 0; q < world; ++q) {
+    TORCH_CHECK(splits[q] >= 0, "cgx: all_to_all: ", side, "_split_sizes[", q, "] is negative (", splits[q], ")");
+    sum += splits[q];
+    counts[q] = (uint64_t)(splits[q] * row);
+  }
+  TORCH_CHECK(sum == rows, "cgx: all_to_all: ", side, "_split_sizes sums to ", sum, " but the ", side, " has ", rows,
+              " rows");
+  return counts;
+}
+
+}  // namespace
+
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor& out, at::Tensor& in,
+                                                                      const std::vector<int64_t>& out_splits,
+                                                                      const std::vector<int64_t>& in_splits, int bits,
+                                                                      int bucket_size, bool stochastic, int64_t seed) {
+  TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
+  TORCH_CHECK(in.device() == out.device(), "cgx: all_to_all: input and output on different devices");
+  const int dtype = to_cgx_dtype(in.scalar_type());
+  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
+              "cgx: all_to_all needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(),
+              " and ", out.scalar_type());
+  TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: all_to_all needs contiguous tensors");
+  TORCH_CHECK(in.dim() >= 1 && out.dim() >= 1, "cgx: all_to_all needs tensors with at least one dimension");
+  TORCH_CHECK(in.sizes().slice(1) == out.sizes().slice(1), "cgx: all_to_all: the input rows ", in.sizes().slice(1),
+              " and the output rows ", out.sizes().slice(1), " differ");
+  TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: all_to_all: bits must be 1..8 or 32");
+  TORCH_CHECK(bucket_size >= 1, "cgx: all_to_all: bucket_size must be >= 1");
+  const int W = getSize();
+  TORCH_CHECK(W <= kMaxPeers, "cgx: all_to_all supports at most ", kMaxPeers, " ranks");
+  // every rank evaluates the same condition, so every rank refuses and none is left waiting
+  TORCH_CHECK(local_size() >= W, "cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE ",
+              local_size(), " < world size ", W, ")");
+  int64_t row = 1;
+  for (int64_t d : in.sizes().slice(1)) row *= d;
+  const std::vector<uint64_t> in_counts = a2a_counts(in, in_splits, W, row, "input");
+  const std::vector<uint64_t> out_counts = a2a_counts(out, out_splits, W, row, "output");
+  RngParams rng;
+  rng.stochastic = stochastic;
+  rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
+  check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, (uint32_t)bucket_size,
+                   getRank(), W);
+  return enqueue_cuda(c10d::OpType::ALLTOALL_BASE, "cgx:all_to_all", out, &in, [&](cudaStream_t s) {
+    engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits,
+                        (uint32_t)bucket_size, rng, s);
+  });
+}
+
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx) {
   // host tensors: queued to the worker thread in call order (reference: enqueue/runLoop,
   // ProcessGroupCGX.cc:300-339); the returned Work's future completes when the job is done, errors

@@ -192,6 +192,15 @@ class ProcessGroupCGX : public c10d::Backend {
                                                     int bits, int bucket_size, bool skip_incomplete, bool stochastic,
                                                     int64_t seed, bool overlapped,
                                                     const std::vector<LayerSpec>& layers);
+  // Compressed all_to_all_single: dim-0 rows of `in` go to the ranks by `in_splits`, rows of `out`
+  // come from the ranks by `out_splits` (empty: equal splits). The own chunk is copied, every other
+  // chunk quantized once with `bits` (1..8; 32: raw) and buckets of `bucket_size` counted from the
+  // chunk's start. seed < 0: CGX_SEED. Malformed splits throw before anything is enqueued; the
+  // splits of a pair must agree on both ranks (the caller's contract). One node only.
+  c10::intrusive_ptr<c10d::Work> all_to_all_compressed(at::Tensor& out, at::Tensor& in,
+                                                       const std::vector<int64_t>& out_splits,
+                                                       const std::vector<int64_t>& in_splits, int bits,
+                                                       int bucket_size, bool stochastic, int64_t seed);
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

@@ -77,6 +77,7 @@ class CudaBackend : public BlockBackend {
     return p;
   }
   void release(void* p) override { cudaFree(p); }
+  void unbind() override { plan_ = nullptr; }
   void bind(const Plan& plan, cudaStream_t stream) override {
     if (plan_ == &plan) return;  // plans are cached by the reducers and immutable: upload once
     plan_ = &plan;

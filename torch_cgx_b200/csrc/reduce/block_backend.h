@@ -21,6 +21,8 @@ class BlockBackend {
   virtual void release(void* p) = 0;
   // make `plan` usable by the calls below (uploads the table for CUDA)
   virtual void bind(const Plan& plan, cudaStream_t stream) = 0;
+  // forget the bound plan, so that a plan later built at the same address is uploaded again
+  virtual void unbind() {}
   // wire = quantize(src[T] * prescale) for blocks [first, first+count)
   virtual void quantize(const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
                         const RngKey& rng, cudaStream_t stream) = 0;

@@ -4,6 +4,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "../common/a2a.h"
 #include "../common/config.h"
 #include "../engine/engine.h"  // split_for_fusion
 #include "../kernels/launch.h"
@@ -309,6 +310,95 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
   p.gather = gather ? 1 : 0;
   cuda_check(launch_sra_fused(p, stream), "launch_sra_fused");
   ++launches_;
+}
+
+void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
+                      const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
+                      int world) {
+  if ((int)in_counts.size() != world || (int)out_counts.size() != world)
+    throw std::invalid_argument("cgx all_to_all: need one input and one output count per rank");
+  if (bits < 1 || (bits > 8 && bits < kRawBits))
+    throw std::invalid_argument("cgx all_to_all: bits must be in 1..8, or 32 for none");
+  if (bucket < 1) throw std::invalid_argument("cgx all_to_all: bucket_size must be >= 1");
+  if (in_counts[rank] != out_counts[rank])
+    throw std::invalid_argument("cgx all_to_all: a rank's chunk for itself must be as large as the one it receives from itself");
+  uint64_t nin = 0, nout = 0;
+  for (int q = 0; q < world; ++q) {
+    nin += in_counts[q];
+    nout += out_counts[q];
+  }
+  if (nin >= (1ull << 32) || nout >= (1ull << 32))
+    throw std::invalid_argument("cgx all_to_all: tensors must have fewer than 2^32 elements");
+  const uint64_t es = (uint64_t)dtype_size(dtype);
+  const uintptr_t a = reinterpret_cast<uintptr_t>(in), b = reinterpret_cast<uintptr_t>(out);
+  if (nin > 0 && nout > 0 && a < b + nout * es && b < a + nin * es)
+    throw std::invalid_argument("cgx all_to_all: the output overlaps the input");
+}
+
+FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                                         const std::vector<uint64_t>& out_counts, int dtype, int bits,
+                                         uint32_t bucket, const RngParams& rng, cudaStream_t stream) {
+  if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
+  const int W = world(), r = rank();
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W);
+  const uint64_t es = (uint64_t)dtype_size(dtype);
+  const int G = max_lanes_;
+  const uint32_t lane_slot = a2a_lane_slot_bytes(heap_->layout().slot_bytes, G);
+  if (a2a_window_blocks(a2a_geom(0, bits, bucket, (int)es), lane_slot) == 0)
+    throw std::invalid_argument("cgx all_to_all: one quantization block does not fit a lane's share of the heap slots "
+                                "(raise CGX_FUSION_BUFFER_SIZE_MB)");
+
+  A2aParams p;
+  std::memset(&p, 0, sizeof(p));
+  p.in = in;
+  p.out = out;
+  A2aCounts n;
+  uint64_t io = 0, oo = 0;
+  for (int q = 0; q < W; ++q) {
+    p.in_off[q] = (uint32_t)io;
+    p.in_cnt[q] = (uint32_t)in_counts[q];
+    p.out_off[q] = (uint32_t)oo;
+    p.out_cnt[q] = (uint32_t)out_counts[q];
+    io += in_counts[q];
+    oo += out_counts[q];
+    if (q == r || in_counts[q] == 0) continue;
+    n.wire_bytes += a2a_chunk_wire(a2a_geom((uint32_t)in_counts[q], bits, bucket, (int)es));
+    n.raw_bytes += in_counts[q] * es;
+  }
+  ++epoch_;
+  p.rank = r;
+  p.world = W;
+  p.lanes = G;
+  p.dtype = dtype;
+  p.bits = bits >= kRawBits ? kRawBits : bits;
+  p.bucket = bucket;
+  p.epoch_hint = epoch_;
+  p.rng = make_rng_key(rng, r, 0);
+  p.slot_bytes = heap_->layout().slot_bytes;
+  p.lane_slot = lane_slot;
+  p.flag_stride = heap_->layout().flag_stride;
+  for (int q = 0; q < W; ++q) {
+    p.recv[q] = heap_->recv1(q);
+    p.flags2[q] = heap_->flags2(q);
+    p.landed[q] = heap_->a2a_landed(q);
+    p.released[q] = heap_->a2a_released(q);
+  }
+  p.status = heap_->status_device();
+  p.abort_word = heap_->abort_device();
+  p.timeout_ns = timeout_ns_;
+  p.sync = heap_->sync_device();
+  last_lanes_ = G;
+  cudaError_t e = cudaErrorInvalidValue;
+  switch (dtype) {
+    case kF32: e = launch_a2a_f32(p, stream); break;
+    case kF16: e = launch_a2a_f16(p, stream); break;
+    case kBF16: e = launch_a2a_bf16(p, stream); break;
+    default: break;
+  }
+  cuda_check(e, "launch_a2a");
+  ++launches_;
+  n.launches = 1;
+  return n;
 }
 
 std::string FusedSra::status_message() const {

@@ -70,6 +70,14 @@ void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_lay
 std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<LayerSpec>& shard_layers,
                                                            const PlanOptions& opt, uint32_t slot_bytes);
 
+// The arguments of one rank's all-to-all (FusedSra::all_to_all, Reducer::all_to_all): a count per
+// rank on both sides, bits 1..8 or >= 32, a bucket >= 1, the own chunk the same size on both sides,
+// tensors below 2^32 elements and an output that does not overlap the input; std::invalid_argument
+// otherwise.
+void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
+                      const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
+                      int world);
+
 class FusedSra {
  public:
   FusedSra(SymmetricHeap* heap, int max_lanes, int64_t timeout_ms, uint32_t min_lane_elems);
@@ -125,6 +133,19 @@ class FusedSra {
   // windows, since its per-chunk wire is the reduce-scatter's
   const std::vector<std::vector<LayerSpec>>& rs_windows(const std::vector<LayerSpec>& shard_layers, int dtype,
                                                         bool skip_incomplete, int max_lanes);
+
+  // Compressed all-to-all (a2a_kernel), one launch whatever the splits. in_counts[q] elements of
+  // `in` (consecutive, in rank order) go to rank q; out_counts[q] elements from rank q land in `out`
+  // (consecutive, in rank order). My own chunk is copied; every other chunk is decode(Q(chunk)) with
+  // `bits` (1..8; >= 32 moves it raw) and buckets of `bucket` counted from the chunk's first
+  // element. The counts of a pair must agree on both ends (the caller's contract, as with NCCL).
+  // Throws std::invalid_argument on a malformed call before anything is launched.
+  struct A2aCounts {
+    uint64_t launches = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's sends
+  };
+  A2aCounts all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                       const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
+                       const RngParams& rng, cudaStream_t stream);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

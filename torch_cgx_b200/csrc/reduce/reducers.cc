@@ -3,7 +3,8 @@
 #include <algorithm>
 #include <stdexcept>
 
-#include "fused_sra.h"  // shard_elems, replicate
+#include "../common/a2a.h"
+#include "fused_sra.h"  // shard_elems, replicate, check_all_to_all
 
 namespace cgx {
 
@@ -164,6 +165,77 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
     if (pn) ops_->dequantize(recvb + row * p, pb, pn, out, stream);
+  }
+}
+
+void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                         const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
+                         const RngParams& rng, cudaStream_t stream) {
+  const int W = comm_->size(), r = comm_->rank();
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W);
+  const size_t es = (size_t)dtype_size(dtype);
+  const bool raw = bits >= kRawBits;
+  const uint8_t* src = static_cast<const uint8_t*>(in);
+  uint8_t* dst = static_cast<uint8_t*>(out);
+  std::vector<size_t> io(W), oo(W), so(W + 1, 0), ro(W + 1, 0);
+  std::vector<const Plan*> sp(W, nullptr), rp(W, nullptr);
+  if (a2a_plans_.size() + 2 * (size_t)W > kMaxA2aPlans) {
+    // host-side tables only: the device backend keeps its own copy of the bound one, and a plan
+    // rebuilt at a freed address must not be mistaken for the bound one
+    ops_->unbind();
+    a2a_plans_.clear();
+  }
+  auto chunk_plan = [&](uint64_t n) -> const Plan* {
+    PlanOptions opt;
+    opt.world = 1;
+    opt.lanes = 1;
+    opt.dtype = dtype;
+    const std::vector<LayerSpec> layer{LayerSpec{0, n, bits, bucket}};
+    const uint64_t key = plan_key(layer, opt);
+    auto it = a2a_plans_.find(key);
+    if (it == a2a_plans_.end()) it = a2a_plans_.emplace(key, std::make_unique<Plan>(build_plan(layer, opt))).first;
+    return it->second.get();
+  };
+  uint64_t i = 0, o = 0;
+  for (int q = 0; q < W; ++q) {
+    io[q] = (size_t)i * es;
+    oo[q] = (size_t)o * es;
+    i += in_counts[q];
+    o += out_counts[q];
+    const bool peer = q != r && !raw;
+    if (peer && in_counts[q]) sp[q] = chunk_plan(in_counts[q]);
+    if (peer && out_counts[q]) rp[q] = chunk_plan(out_counts[q]);
+    so[q + 1] = so[q] + (sp[q] ? (sp[q]->chunk_wire_bytes[0] + 255) / 256 * 256 : 0);
+    ro[q + 1] = ro[q] + (rp[q] ? (rp[q]->chunk_wire_bytes[0] + 255) / 256 * 256 : 0);
+  }
+  if (in_counts[r]) ops_->copy(dst + oo[r], src + io[r], in_counts[r] * es, stream);
+  uint8_t* sendb = raw ? nullptr : scratch(0, so[W] + 16);
+  uint8_t* recvb = raw ? nullptr : scratch(1, ro[W] + 16);
+  for (int q = 0; q < W; ++q) {
+    if (!sp[q]) continue;
+    RngKey key = make_rng_key(rng, r, 0);
+    key.stream = a2a_rng_stream(r, q);
+    ops_->bind(*sp[q], stream);
+    ops_->quantize(src + io[q], 0, (uint32_t)sp[q]->blocks.size(), sendb + so[q], 1.0f, key, stream);
+  }
+  std::vector<P2POp> x;
+  for (int q = 0; q < W; ++q) {
+    if (q == r) continue;
+    if (raw) {
+      if (in_counts[q]) x.push_back({true, const_cast<uint8_t*>(src + io[q]), in_counts[q] * es, q});
+      if (out_counts[q]) x.push_back({false, dst + oo[q], out_counts[q] * es, q});
+      bytes_sent_ += in_counts[q] * es;
+      continue;
+    }
+    if (sp[q]) x.push_back({true, sendb + so[q], sp[q]->chunk_wire_bytes[0], q});
+    if (rp[q]) x.push_back({false, recvb + ro[q], rp[q]->chunk_wire_bytes[0], q});
+    if (sp[q]) bytes_sent_ += sp[q]->chunk_wire_bytes[0];
+  }
+  comm_->exchange(x, stream);
+  for (int q = 0; q < W; ++q) {
+    if (!rp[q]) continue;
+    ops_->bind(*rp[q], stream);
+    ops_->dequantize(recvb + ro[q], 0, (uint32_t)rp[q]->blocks.size(), dst + oo[q], stream);
   }
 }
 

@@ -57,6 +57,13 @@ class Reducer {
   // (bits 32) are copied unchanged. `in` may be `out`'s chunk rank(), or disjoint from it.
   void all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
                   bool skip_incomplete, const RngParams& rng, cudaStream_t stream);
+  // Compressed all-to-all over the communicator's W ranks, bitwise FusedSra::all_to_all (same
+  // arguments and checks): each chunk for a peer is quantized by the standalone item kernels through
+  // a one-layer plan of the chunk, the records are exchanged and every peer's chunk is decoded into
+  // its rows; the own chunk is copied, and with bits >= 32 every chunk travels as its bytes.
+  void all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                  const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, const RngParams& rng,
+                  cudaStream_t stream);
   uint64_t bytes_sent() const { return bytes_sent_; }
 
  protected:
@@ -73,6 +80,10 @@ class Reducer {
 
  private:
   std::unordered_map<uint64_t, std::unique_ptr<Plan>> plans_;
+  // all_to_all: one-layer plans per chunk size; MoE splits change every call, so this cache is
+  // bounded (kMaxA2aPlans) and dropped as a whole when a call could overflow it
+  std::unordered_map<uint64_t, std::unique_ptr<Plan>> a2a_plans_;
+  static constexpr size_t kMaxA2aPlans = 256;
   struct Buf {
     uint8_t* p = nullptr;
     size_t cap = 0;

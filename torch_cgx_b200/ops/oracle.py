@@ -622,6 +622,29 @@ def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[
     return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers) for t in inputs])
 
 
+def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, bits: int,
+                         bucket_size: int) -> List[torch.Tensor]:
+    """Every rank's output of the compressed all-to-all (round to nearest). ``counts[q][r]`` elements
+    go from rank q to rank r; rank q's input holds its chunks in destination order and rank r's
+    output the chunks it receives in source order. The own chunk, and every chunk when ``bits`` is
+    32, is the input unchanged; every other chunk is ``quantize_dequantize_layers`` of one layer, so
+    buckets are counted from the chunk's first element."""
+    W = len(inputs)
+    flat = [t.detach().reshape(-1).cpu() for t in inputs]
+    outs = []
+    for r in range(W):
+        parts = []
+        for q in range(W):
+            a = sum(int(c) for c in counts[q][:r])
+            n = int(counts[q][r])
+            chunk = flat[q][a:a + n].clone()
+            if q != r and bits < RAW_BITS and n > 0:
+                chunk = quantize_dequantize_layers(chunk, [(0, n, int(bits), int(bucket_size))])
+            parts.append(chunk)
+        outs.append(torch.cat(parts) if parts else flat[r].new_empty(0))
+    return outs
+
+
 # ---- the sharded collectives over several nodes (AllreduceEngine::sharded, DESIGN §2.9b) -----------
 SHARDED_PERTURBATIONS = ("prescale_local", "requantized_gather", "quantized_own_partial", "transposed_ranks")
 _CROSS_SEQ = 0x40000000  # the allreduce's cross-node marker

@@ -16,12 +16,18 @@ The compressed reduce-scatter is asked for explicitly (``dist.reduce_scatter_ten
 and so is the compressed all-gather (``dist.all_gather_into_tensor`` stays uncompressed)::
 
     cgx.all_gather_into_tensor(flat_params, shard, bits=8)
+
+and the compressed all-to-all of expert-parallel MoE layers (``dist.all_to_all_single`` stays
+uncompressed)::
+
+    cgx.all_to_all_single(recv, tokens, recv_splits, send_splits, bits=8)
+    y = cgx.differentiable_all_to_all_single(tokens, recv_splits, send_splits, bits=8)
 """
 from __future__ import annotations
 
 import contextlib
 import os
-from typing import Iterator, Optional, Sequence, Tuple
+from typing import Iterator, List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -152,3 +158,80 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int 
     """
     return _all_gather(output, input, bits=bits, bucket_size=bucket_size, group=group, async_op=async_op,
                        stochastic=stochastic, seed=seed, layers=layers, overlapped=False)
+
+
+def _splits(s: Optional[Sequence[int]]) -> List[int]:
+    return [] if s is None else [int(v) for v in s]
+
+
+def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
+                      input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8, bucket_size: int = 512,
+                      group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None):
+    """Compressed ``dist.all_to_all_single`` on a ``cgx`` group.
+
+    Splits count dim-0 rows (``None``: equal splits). Rows ``input_split_sizes[q]`` of ``input`` go
+    to rank q, and the chunk from rank q lands in the ``output_split_sizes[q]`` rows of ``output``.
+    The rank's own chunk is copied bit for bit. Every other chunk is quantized once by the sender
+    (``bits`` 1..8, max-min, buckets of ``bucket_size`` counted from the chunk's first element) and
+    decoded by the receiver; ``bits=32`` moves every chunk unchanged. Round to nearest unless
+    ``stochastic``; ``seed=None`` uses ``CGX_SEED``.
+
+    As with NCCL, the splits are the caller's contract: rank q's ``input_split_sizes[r]`` must equal
+    rank r's ``output_split_sizes[q]``. Malformed splits on one rank (wrong length, sum or sign, or
+    rows of another size than the output's) raise ``RuntimeError`` before anything is launched.
+    CUDA float32 / float16 / bfloat16, contiguous, ``output`` not overlapping ``input``, at most 16
+    ranks, all on one node (several nodes raise on every rank).
+    """
+    from .hooks import _native_backend
+
+    native = _native_backend(group if group is not None else dist.group.WORLD, input)
+    if native is None:
+        raise RuntimeError("cgx.all_to_all_single needs a process group with the cgx backend")
+    work = native.all_to_all_compressed(output, input, _splits(output_split_sizes), _splits(input_split_sizes),
+                                        int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed))
+    if async_op:
+        return work
+    work.wait()  # the current stream waits for the kernel; the host does not
+    return None
+
+
+def _a2a_output(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]], world: int) -> torch.Tensor:
+    rows = sum(int(v) for v in output_split_sizes) if output_split_sizes is not None else input.shape[0]
+    return input.new_empty((rows,) + tuple(input.shape[1:]))
+
+
+class _AllToAll(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, input, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size, group, stochastic):
+        ctx.splits = (output_split_sizes, input_split_sizes)
+        ctx.grad_bits, ctx.bucket_size, ctx.group, ctx.stochastic = grad_bits, bucket_size, group, stochastic
+        ctx.in_shape = input.shape
+        world = dist.get_world_size(group)
+        input = input.contiguous()
+        out = _a2a_output(input, output_split_sizes, world)
+        all_to_all_single(out, input, output_split_sizes, input_split_sizes, bits=bits, bucket_size=bucket_size,
+                          group=group, stochastic=stochastic)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        out_splits, in_splits = ctx.splits
+        grad = grad.contiguous()
+        gin = grad.new_empty(ctx.in_shape)
+        # the gradient travels back: the forward's output splits are its input splits
+        all_to_all_single(gin, grad, in_splits, out_splits, bits=ctx.grad_bits, bucket_size=ctx.bucket_size,
+                          group=ctx.group, stochastic=ctx.stochastic)
+        return gin, None, None, None, None, None, None, None
+
+
+def differentiable_all_to_all_single(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
+                                     input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8,
+                                     grad_bits: Optional[int] = None, bucket_size: int = 512, group=None,
+                                     stochastic: bool = False) -> torch.Tensor:
+    """``all_to_all_single`` that returns its output and has a backward pass: the compressed
+    all-to-all of the gradient with the splits swapped, at ``grad_bits`` (``None``: ``bits``; 32:
+    exact). This is the form an MoE layer calls for its token dispatch and combine."""
+    gb = int(bits if grad_bits is None else grad_bits)
+    return _AllToAll.apply(input, None if output_split_sizes is None else _splits(output_split_sizes),
+                           None if input_split_sizes is None else _splits(input_split_sizes), int(bits), gb,
+                           int(bucket_size), group, bool(stochastic))
