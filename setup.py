@@ -24,6 +24,7 @@ SOURCES = [
     "comm/fd_channel.cc",
     "comm/loopback_communicator.cc",
     "comm/symmetric_heap.cc",
+    "reduce/plan_cache.cc",
     "reduce/fused_sra.cc",
     "reduce/block_backend.cc",
     "reduce/reducers.cc",

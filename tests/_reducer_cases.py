@@ -119,3 +119,31 @@ def expected_bytes_sent(op, layers, world, dtype, skip_incomplete):
         return [sum(cw[(r - s) % W] + cw[(r + 1 - s) % W] for s in range(W - 1)) for r in range(W)]
     row = (p["max_chunk_wire"] + 255) // 256 * 256  # all-to-all: the whole wire image to every peer
     return [(W - 1) * W * row for _ in range(W)]
+
+
+PLAN_CACHE_BOUND = 256  # plans a generic reducer keeps before it drops its cache (Reducer::kMaxPlans)
+
+
+def check_many_layouts(world, device, calls=300):
+    """More distinct allreduce layouts than a reducer's plan cache holds, through one SRA group on
+    `device`: every call equals sra_simulate bit for bit (stochastic rounding, so the RNG streams
+    count too), across the drop, and no rank's cache ever holds more than PLAN_CACHE_BOUND plans."""
+    from _bitwise import assert_same
+
+    g = C.LocalReducerGroup(world, "SRA", 20_000)
+    gen = torch.Generator().manual_seed(world)
+    most = 0
+    for i in range(calls):
+        n = 700 + 3 * i
+        layers = [(0, 37, 32, 512), (37, n - 37, 4, 64)]
+        ins = [torch.randn(n, generator=gen) * (r + 1) for r in range(world)]
+        got = [t.clone().to(device) for t in ins]
+        g.allreduce(got, layers, True, False, True, 7, i)
+        sim = [t.clone() for t in ins]
+        C.sra_simulate(sim, layers, 1, True, False, True, 7, i, O.GENERIC_MIN_LANE_ELEMS)
+        for r in range(world):
+            assert_same(got[r].cpu(), sim[r], f"call {i} rank {r}")
+        held = [g.num_plans(r) for r in range(world)]
+        assert max(held) <= PLAN_CACHE_BOUND, f"call {i}: {held} plans cached"
+        most = max(most, *held)
+    assert most == PLAN_CACHE_BOUND and max(held) < PLAN_CACHE_BOUND, "the plan cache never filled and dropped"

@@ -83,6 +83,9 @@ def test_item_helper_equals_build_plan(bits, bucket, dtype):
         plan = _C.build_plan([(0, n, bits, bucket)], 1, 1, dtype, False, 1 << 30)
         got = _C.a2a_items(n, bits, bucket, dtype)
         assert torch.equal(got, plan["items"]), (n, bits, bucket)
+        # the record bytes of the chunk, which the generic reducer sends from a2a.h alone
+        w = _C.a2a_windows(n, bits, bucket, dtype, 1 << 30, 1)
+        assert sum(b[2] for lane in w["lanes"] for win in lane for b in win) == plan["chunk_wire_bytes"][0]
         # slice size: 1024-element slices exactly for 1024-element buckets
         assert plan["slice_elems"] == (1024 if bits < 32 and bucket == 1024 else 512)
 
@@ -177,3 +180,4 @@ def test_generic_reducer_plan_cache_is_bounded():
         sim = _simulate(xs, c, 3, 16)
         for r in range(W):
             assert_same(outs[r], sim[r], f"call {it} rank {r}")
+            assert red.num_plans(r) <= 256

@@ -177,10 +177,10 @@ def test_generic_path_equals_fused(bits, bucket, dtype):
 
 def test_generic_path_across_many_chunk_sizes():
     # more distinct chunk sizes than the generic reducer's plan cache holds: it is dropped and rebuilt
-    # mid-run, and a plan rebuilt at a freed address must still be uploaded
+    # mid-run, and the plans rebuilt after the drop are uploaded again
     W, dtype = 2, torch.bfloat16
     red = C.LocalReducerGroup(W, "SRA", 5000)
-    for it in range(80):
+    for it in range(140):
         c = [[100 + it, 3000 + 7 * it], [2000 + 5 * it, 50 + it]]
         xs = inputs(c, dtype, it)
         outs = outputs(c, dtype, device=dev())
@@ -190,6 +190,7 @@ def test_generic_path_across_many_chunk_sizes():
         C.all_to_all_simulate(xs, sim, c, bits=4, bucket_size=64)
         for r in range(W):
             assert_same(outs[r].cpu(), sim[r], f"call {it} rank {r}")
+            assert red.num_plans(r) <= 256
 
 
 def test_cuda_graph_virtual_ranks():

@@ -13,8 +13,8 @@ import torch_cgx_b200 as cgx
 from torch_cgx_b200.ops import oracle as O
 
 from _bitwise import assert_same, mismatch
-from _reducer_cases import (OPS, config_id, configs, expected_bytes_sent, group_for, make_case, reference,
-                            run_op)
+from _reducer_cases import (OPS, check_many_layouts, config_id, configs, expected_bytes_sent, group_for, make_case,
+                            reference, run_op)
 
 C = cgx._C
 CONFIGS = configs()
@@ -176,3 +176,7 @@ def test_group_rejects_bad_arguments():
     out = [t.clone() for t in ins]
     g.allreduce(out, [(0, 100, 4, 8)])
     assert_same(out[1], O.ring_reference(ins, [(0, 100, 4, 8)])[1])
+
+
+def test_host_plan_cache_is_bounded_across_many_layouts():
+    check_many_layouts(3, "cpu")

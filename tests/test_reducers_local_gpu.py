@@ -17,7 +17,9 @@ import torch_cgx_b200 as cgx
 from torch_cgx_b200.ops import oracle as O
 
 from _bitwise import assert_same
-from _reducer_cases import (DT_CODE, OPS, config_id, configs, group_for, make_case, reference, run_op)
+from _a2a_cases import counts as a2a_counts, inputs as a2a_inputs, outputs as a2a_outputs
+from _reducer_cases import (DT_CODE, OPS, check_many_layouts, config_id, configs, group_for, make_case, reference,
+                            run_op)
 
 pytestmark = pytest.mark.gpu
 C = cgx._C
@@ -195,9 +197,9 @@ def test_device_grid_wraps_past_one_wave(op):
 @pytest.mark.parametrize("op", OPS)
 @pytest.mark.parametrize("record", [True, False], ids=["recorded", "unrecorded"])
 def test_device_repeated_calls_with_alternating_tables(record, op):
-    # one group per backend for the whole sequence: plan cache hits and misses, the plan upload that
-    # bind() skips when a call uses the table of the call before (a, a and big, big; all-to-all binds
-    # a raw plan inside each call, so it re-uploads) and scratch buffers that grow between calls
+    # one group per backend for the whole sequence: plan cache hits and misses, tables uploaded on a
+    # plan's first use only (a, a and big, big; all-to-all also uses a raw plan inside each call) and
+    # scratch buffers that grow between calls
     W, dtype = 3, torch.bfloat16
     a = [(0, 37, 32, 512), (37, 9000, 4, 512)]
     b = [(0, 4000, 8, 64), (4000, 5037, 2, 1024)]
@@ -209,3 +211,49 @@ def test_device_repeated_calls_with_alternating_tables(record, op):
         ins = [(torch.randn(total, generator=g) * (r + 1)).to(dtype) for r in range(W)]
         compare_backends(op, ins, layers, offset=(1, 3, 5)[i % 3], groups=groups, record=record,
                          **op_kwargs(op, i % 2 == 0, False))
+
+
+def test_device_plan_cache_is_bounded_across_many_layouts():
+    check_many_layouts(3, "cuda")
+
+
+def test_device_interleaved_collectives_upload_each_table_once():
+    # reduce-scatter, all-to-all with fixed splits and all-to-all with new splits on one device group,
+    # bitwise the host group's; after the first round the fixed calls find their tables uploaded
+    W, dtype = 4, torch.bfloat16
+    shard = [(0, 37, 32, 512), (37, 3000, 4, 64)]
+    S = 3037
+    fixed = [[1500 + 100 * q + 10 * r for r in range(W)] for q in range(W)]
+    hg, dg = C.LocalReducerGroup(W, "SRA", 20_000), C.LocalReducerGroup(W, "SRA", 20_000)
+    g = torch.Generator().manual_seed(3)
+
+    def reduce_scatter(i):
+        ins = [(torch.randn(W * S, generator=g) * (r + 1)).to(dtype) for r in range(W)]
+        host = [torch.empty(S, dtype=dtype) for _ in range(W)]
+        hg.reduce_scatter(ins, host, shard, True, False, True, 5, i)
+        got = [torch.empty(S, dtype=dtype, device="cuda") for _ in range(W)]
+        dg.reduce_scatter([t.cuda() for t in ins], got, shard, True, False, True, 5, i)
+        return host, got
+
+    def all_to_all(c, i):
+        xs = a2a_inputs(c, dtype, i)
+        host = a2a_outputs(c, dtype)
+        hg.all_to_all(xs, host, c, bits=3, bucket_size=100, stochastic=True, seed=5, seq=i)
+        got = a2a_outputs(c, dtype, device="cuda")
+        dg.all_to_all([x.cuda() for x in xs], got, c, bits=3, bucket_size=100, stochastic=True, seed=5, seq=i)
+        return host, got
+
+    for i in range(4):
+        for what, run in [("reduce_scatter", lambda: reduce_scatter(i)),
+                          ("fixed splits", lambda: all_to_all(fixed, i)),
+                          ("new splits", lambda: all_to_all(a2a_counts(W, "uneven", 2000, seed=i), i))]:
+            before = [dg.plan_uploads(r) for r in range(W)]
+            host, got = run()
+            torch.cuda.synchronize()
+            for r in range(W):
+                assert_same(got[r].cpu(), host[r], f"round {i} {what} rank {r}: device vs host")
+            uploads = [dg.plan_uploads(r) - before[r] for r in range(W)]
+            if i == 0 or what == "new splits":
+                assert sum(uploads) > 0, f"round {i} {what}: no table uploaded"
+            else:
+                assert uploads == [0] * W, f"round {i} {what}: tables uploaded again {uploads}"

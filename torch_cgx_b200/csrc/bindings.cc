@@ -421,55 +421,40 @@ class PreparedCodec {
  public:
   PreparedCodec(const std::vector<LayerTuple>& layers, at::ScalarType dtype, int64_t device, bool skip_incomplete) {
     at::Tensor probe = at::empty({0}, at::TensorOptions().dtype(dtype));
-    dt_ = cgx_dtype(probe);
-    plan_ = build_plan(to_layers(layers), make_opts(1, 1, dt_, skip_incomplete, 1 << 30));
     c10::cuda::CUDAGuard g((c10::DeviceIndex)device);
-    items_ = at::empty({(int64_t)(plan_.items.size() * sizeof(WarpItem) + 16)},
-                       at::TensorOptions().dtype(at::kByte).device(at::kCUDA, device));
-    cuda_check(cudaMemcpy(items_.data_ptr(), plan_.items.data(), plan_.items.size() * sizeof(WarpItem),
-                          cudaMemcpyHostToDevice),
-               "upload items");
+    cudaStream_t s = c10::cuda::getCurrentCUDAStream().stream();
+    dp_ = &plans_.get(to_layers(layers), make_opts(1, 1, cgx_dtype(probe), skip_incomplete, 1 << 30), s);
+    plans_.upload(*dp_, s);
+    cuda_check(cudaStreamSynchronize(s), "upload items");  // the calls may run on any stream
   }
-  int64_t wire_bytes() const { return (int64_t)wire_row_bytes(plan_); }
-  int64_t numel() const { return (int64_t)plan_.numel; }
-  int64_t num_items() const { return (int64_t)plan_.items.size(); }
+  int64_t wire_bytes() const { return (int64_t)wire_row_bytes(dp_->plan); }
+  int64_t numel() const { return (int64_t)dp_->plan.numel; }
+  int64_t num_items() const { return (int64_t)dp_->plan.items.size(); }
   void quantize(const at::Tensor& x, at::Tensor& wire, double prescale, bool stochastic, uint64_t seed, uint32_t seq) {
     check(x, wire);
     c10::cuda::CUDAGuard g(x.device());
-    cuda_check(launch_quantize_items(args(), x.data_ptr(), wire.data_ptr<uint8_t>(), (float)prescale,
-                                     make_rng_key(make_rng(stochastic, seed, seq), 0, 0),
-                                     c10::cuda::getCurrentCUDAStream()),
-               "quantize_items");
+    ops_->quantize(*dp_, x.data_ptr(), 0, (uint32_t)dp_->plan.blocks.size(), wire.data_ptr<uint8_t>(), (float)prescale,
+                   make_rng_key(make_rng(stochastic, seed, seq), 0, 0), c10::cuda::getCurrentCUDAStream());
   }
   void dequantize(const at::Tensor& wire, at::Tensor& out) {
     check(out, wire);
     c10::cuda::CUDAGuard g(out.device());
-    cuda_check(launch_dequantize_items(args(), wire.data_ptr<uint8_t>(), out.data_ptr(),
-                                       c10::cuda::getCurrentCUDAStream()),
-               "dequantize_items");
+    ops_->dequantize(*dp_, wire.data_ptr<uint8_t>(), 0, (uint32_t)dp_->plan.blocks.size(), out.data_ptr(),
+                     c10::cuda::getCurrentCUDAStream());
   }
 
  private:
   void check(const at::Tensor& x, const at::Tensor& wire) const {
-    TORCH_CHECK(x.is_cuda() && x.is_contiguous() && cgx_dtype(x) == dt_ && (uint64_t)x.numel() == plan_.numel,
+    TORCH_CHECK(x.is_cuda() && x.is_contiguous() && cgx_dtype(x) == dp_->plan.dtype &&
+                    (uint64_t)x.numel() == dp_->plan.numel,
                 "PreparedCodec: tensor does not match the prepared layout");
     TORCH_CHECK(wire.is_cuda() && wire.is_contiguous() && wire.scalar_type() == at::kByte &&
-                    (size_t)wire.numel() >= wire_row_bytes(plan_),
+                    (size_t)wire.numel() >= wire_row_bytes(dp_->plan),
                 "PreparedCodec: wire buffer too small");
   }
-  ItemKernelArgs args() const {
-    ItemKernelArgs a;
-    a.items = (const WarpItem*)items_.data_ptr();
-    a.first = 0;
-    a.count = (uint32_t)plan_.items.size();
-    a.dtype = dt_;
-    a.slice_elems = (int)plan_.slice_elems;
-    a.uniform_bits = plan_.uniform_bits;
-    return a;
-  }
-  Plan plan_;
-  int dt_ = kF32;
-  at::Tensor items_;
+  PlanCache plans_{1};
+  const DevicePlan* dp_ = nullptr;
+  std::unique_ptr<BlockBackend> ops_ = make_cuda_block_backend();
 };
 
 // ---- single-process multi-rank harness --------------------------------------
@@ -712,6 +697,10 @@ class LocalReducerGroup {
   }
   // bytes each rank's reducer counted as sent during the last call
   std::vector<int64_t> bytes_sent() const { return last_sent_; }
+  // plans cached by rank r's reducer, and tables it has uploaded so far, on the backend (host or
+  // device memory) of the last call
+  int64_t num_plans(int r) { return (int64_t)rank_of_last_call(r).red->num_plans(); }
+  int64_t plan_uploads(int r) { return (int64_t)rank_of_last_call(r).red->plan_uploads(); }
   void set_recording(bool on) { record_ = on; }
   // the messages of the last call (recording on): (exchange index, src, dst, uint8 CPU tensor)
   std::vector<std::tuple<int64_t, int, int, at::Tensor>> messages() const {
@@ -730,6 +719,11 @@ class LocalReducerGroup {
     std::unique_ptr<BlockBackend> ops;
     std::unique_ptr<Reducer> red;  // declared last: released first, its scratch through `ops`
   };
+
+  Rank& rank_of_last_call(int r) {
+    TORCH_CHECK(r >= 0 && r < hub_.world(), "LocalReducerGroup: bad rank ", r);
+    return ranks(last_cuda_)[(size_t)r];
+  }
 
   std::vector<Rank>& ranks(bool cuda) {
     std::vector<Rank>& v = cuda ? cuda_ : cpu_;
@@ -787,6 +781,7 @@ class LocalReducerGroup {
       for (auto& s : streams_) ready.block(s);
     }
     std::vector<Rank>& rk = ranks(cuda);
+    last_cuda_ = cuda;
     std::vector<uint64_t> before(W);
     for (int r = 0; r < W; ++r) before[r] = rk[r].red->bytes_sent();
     hub_.reset(record_);
@@ -828,6 +823,7 @@ class LocalReducerGroup {
   LoopbackHub hub_;
   ReductionType kind_ = ReductionType::kSRA;
   bool record_ = false;
+  bool last_cuda_ = false;
   int device_ = -1;
   std::vector<c10::cuda::CUDAStream> streams_;
   std::vector<Rank> cpu_, cuda_;
@@ -1701,6 +1697,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0)
       .def("bytes_sent", &LocalReducerGroup::bytes_sent)
+      .def("num_plans", &LocalReducerGroup::num_plans, py::arg("rank"))
+      .def("plan_uploads", &LocalReducerGroup::plan_uploads, py::arg("rank"))
       .def("set_recording", &LocalReducerGroup::set_recording, py::arg("on"))
       .def("messages", &LocalReducerGroup::messages);
   py::class_<LocalEngineGroup>(m, "LocalEngineGroup")

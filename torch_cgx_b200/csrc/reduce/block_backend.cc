@@ -21,50 +21,47 @@ class CpuBackend : public BlockBackend {
     return p;
   }
   void release(void* p) override { std::free(p); }
-  void bind(const Plan& plan, cudaStream_t) override { plan_ = &plan; }
-  void quantize(const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale, const RngKey& rng,
-                cudaStream_t) override {
+  void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
+                const RngKey& rng, cudaStream_t) override {
+    const Plan& p = dp.plan;
     std::vector<float> acc(kMaxBlockElems);
     for (uint32_t b = first; b < first + count; ++b) {
-      const BlockDesc& d = plan_->blocks[b];
-      cpu::load_block(src, plan_->dtype, d, prescale, acc.data());
-      cpu::quantize_block(acc.data(), plan_->dtype, d, wire + d.wire_off, rng, b);
+      const BlockDesc& d = p.blocks[b];
+      cpu::load_block(src, p.dtype, d, prescale, acc.data());
+      cpu::quantize_block(acc.data(), p.dtype, d, wire + d.wire_off, rng, b);
     }
   }
-  void accumulate(const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32, uint32_t base_elem,
-                  const void* init_src, float prescale, cudaStream_t) override {
+  void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
+                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t) override {
+    const Plan& p = dp.plan;
     for (uint32_t b = first; b < first + count; ++b) {
-      const BlockDesc& d = plan_->blocks[b];
+      const BlockDesc& d = p.blocks[b];
       float* a = acc_f32 + (d.elem_off - base_elem);
-      if (init_src) cpu::load_block(init_src, plan_->dtype, d, prescale, a);
-      if (wire) cpu::decode_block_add(wire + d.wire_off, plan_->dtype, d, a);
+      if (init_src) cpu::load_block(init_src, p.dtype, d, prescale, a);
+      if (wire) cpu::decode_block_add(wire + d.wire_off, p.dtype, d, a);
     }
   }
-  void quantize_f32(const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count, uint8_t* wire,
-                    const RngKey& rng, void* out, cudaStream_t) override {
+  void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
+                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t) override {
+    const Plan& p = dp.plan;
     for (uint32_t b = first; b < first + count; ++b) {
-      const BlockDesc& d = plan_->blocks[b];
-      cpu::quantize_block(acc_f32 + (d.elem_off - base_elem), plan_->dtype, d, wire + d.wire_off, rng, b);
-      if (out) cpu::decode_block_store(wire + d.wire_off, plan_->dtype, d, out);
+      const BlockDesc& d = p.blocks[b];
+      cpu::quantize_block(acc_f32 + (d.elem_off - base_elem), p.dtype, d, wire + d.wire_off, rng, b);
+      if (out) cpu::decode_block_store(wire + d.wire_off, p.dtype, d, out);
     }
   }
-  void dequantize(const uint8_t* wire, uint32_t first, uint32_t count, void* dst, cudaStream_t) override {
+  void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
+                  cudaStream_t) override {
     for (uint32_t b = first; b < first + count; ++b) {
-      const BlockDesc& d = plan_->blocks[b];
-      cpu::decode_block_store(wire + d.wire_off, plan_->dtype, d, dst);
+      const BlockDesc& d = dp.plan.blocks[b];
+      cpu::decode_block_store(wire + d.wire_off, dp.plan.dtype, d, dst);
     }
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t) override { std::memcpy(dst, src, bytes); }
-
- private:
-  const Plan* plan_ = nullptr;
 };
 
 class CudaBackend : public BlockBackend {
  public:
-  ~CudaBackend() override {
-    if (d_items_) cudaFree(d_items_);
-  }
   bool is_cuda() const override { return true; }
   void* alloc(size_t bytes) override {
     void* p = nullptr;
@@ -77,38 +74,24 @@ class CudaBackend : public BlockBackend {
     return p;
   }
   void release(void* p) override { cudaFree(p); }
-  void unbind() override { plan_ = nullptr; }
-  void bind(const Plan& plan, cudaStream_t stream) override {
-    if (plan_ == &plan) return;  // plans are cached by the reducers and immutable: upload once
-    plan_ = &plan;
-    const size_t bytes = plan.items.size() * sizeof(WarpItem);
-    if (bytes > cap_) {
-      if (d_items_) {
-        cuda_check(cudaStreamSynchronize(stream), "sync before plan realloc");
-        cudaFree(d_items_);
-      }
-      cuda_check(cudaMalloc((void**)&d_items_, bytes), "cudaMalloc(plan)");
-      cap_ = bytes;
-    }
-    if (bytes)
-      cuda_check(cudaMemcpyAsync(d_items_, plan.items.data(), bytes, cudaMemcpyHostToDevice, stream), "upload plan");
+  void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
+                const RngKey& rng, cudaStream_t stream) override {
+    cuda_check(launch_quantize_items(args(dp, first, count), src, wire, prescale, rng, stream), "quantize_items");
   }
-  void quantize(const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale, const RngKey& rng,
-                cudaStream_t stream) override {
-    cuda_check(launch_quantize_items(args(first, count), src, wire, prescale, rng, stream), "quantize_items");
+  void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
+                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream) override {
+    cuda_check(
+        launch_accumulate_items_f32(args(dp, first, count), wire, acc_f32, base_elem, init_src, prescale, stream),
+        "accumulate_items");
   }
-  void accumulate(const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32, uint32_t base_elem,
-                  const void* init_src, float prescale, cudaStream_t stream) override {
-    cuda_check(launch_accumulate_items_f32(args(first, count), wire, acc_f32, base_elem, init_src, prescale, stream),
-               "accumulate_items");
-  }
-  void quantize_f32(const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count, uint8_t* wire,
-                    const RngKey& rng, void* out, cudaStream_t stream) override {
-    cuda_check(launch_quantize_items_f32(args(first, count), acc_f32, base_elem, wire, rng, out, stream),
+  void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
+                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) override {
+    cuda_check(launch_quantize_items_f32(args(dp, first, count), acc_f32, base_elem, wire, rng, out, stream),
                "quantize_items_f32");
   }
-  void dequantize(const uint8_t* wire, uint32_t first, uint32_t count, void* dst, cudaStream_t stream) override {
-    cuda_check(launch_dequantize_items(args(first, count), wire, dst, stream), "dequantize_items");
+  void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
+                  cudaStream_t stream) override {
+    cuda_check(launch_dequantize_items(args(dp, first, count), wire, dst, stream), "dequantize_items");
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) override {
     cuda_check(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, stream), "cudaMemcpyAsync");
@@ -116,19 +99,17 @@ class CudaBackend : public BlockBackend {
 
  private:
   // blocks [first, first+count) -> their warp items (items are emitted block by block)
-  ItemKernelArgs args(uint32_t first, uint32_t count) const {
+  static ItemKernelArgs args(const DevicePlan& dp, uint32_t first, uint32_t count) {
     ItemKernelArgs a;
-    a.items = d_items_;
-    a.first = plan_->block_item_first[first];
-    a.count = plan_->block_item_first[first + count] - a.first;
-    a.dtype = plan_->dtype;
-    a.slice_elems = (int)plan_->slice_elems;
-    a.uniform_bits = plan_->uniform_bits;
+    a.items = dp.d_items;
+    a.first = dp.plan.block_item_first[first];
+    a.count = dp.plan.block_item_first[first + count] - a.first;
+    a.dtype = dp.plan.dtype;
+    a.slice_elems = (int)dp.plan.slice_elems;
+    a.uniform_bits = dp.plan.uniform_bits;
+    if (a.count && !dp.d_items) throw std::logic_error("cgx: the device backend got a plan that was not uploaded");
     return a;
   }
-  const Plan* plan_ = nullptr;
-  WarpItem* d_items_ = nullptr;
-  size_t cap_ = 0;
 };
 
 }  // namespace

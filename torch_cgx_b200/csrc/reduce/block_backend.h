@@ -9,6 +9,7 @@
 
 #include "../common/philox.h"
 #include "../common/plan.h"
+#include "plan_cache.h"
 
 namespace cgx {
 
@@ -19,22 +20,21 @@ class BlockBackend {
   // scratch memory of the backend's kind (zero-initialised)
   virtual void* alloc(size_t bytes) = 0;
   virtual void release(void* p) = 0;
-  // make `plan` usable by the calls below (uploads the table for CUDA)
-  virtual void bind(const Plan& plan, cudaStream_t stream) = 0;
-  // forget the bound plan, so that a plan later built at the same address is uploaded again
-  virtual void unbind() {}
-  // wire = quantize(src[T] * prescale) for blocks [first, first+count)
-  virtual void quantize(const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
-                        const RngKey& rng, cudaStream_t stream) = 0;
+  // The block primitives work on blocks [first, first+count) of `dp`'s plan; the device backend
+  // reads its uploaded tables (PlanCache::upload), the host backend the plan alone.
+  // wire = quantize(src[T] * prescale)
+  virtual void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire,
+                        float prescale, const RngKey& rng, cudaStream_t stream) = 0;
   // acc_f32[elem_off - base_elem + i] = float(init_src[elem_off + i]) * prescale   (init_src != nullptr)
   // acc_f32[...] += decode(wire)                                                   (wire != nullptr)
-  virtual void accumulate(const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32, uint32_t base_elem,
-                          const void* init_src, float prescale, cudaStream_t stream) = 0;
+  virtual void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
+                          uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream) = 0;
   // wire = quantize(acc_f32); out[T] = decode(wire) when out != nullptr
-  virtual void quantize_f32(const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count, uint8_t* wire,
-                            const RngKey& rng, void* out, cudaStream_t stream) = 0;
+  virtual void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first,
+                            uint32_t count, uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) = 0;
   // dst[T] = decode(wire)
-  virtual void dequantize(const uint8_t* wire, uint32_t first, uint32_t count, void* dst, cudaStream_t stream) = 0;
+  virtual void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
+                          cudaStream_t stream) = 0;
   virtual void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) = 0;
 };
 

@@ -41,10 +41,6 @@ std::vector<uint64_t> FusedSra::read_trace() {
 
 FusedSra::~FusedSra() {
   if (d_trace_) cudaFree(d_trace_);
-  for (auto& kv : cache_) {
-    if (kv.second->d_items) cudaFree(kv.second->d_items);
-    if (kv.second->d_item_first) cudaFree(kv.second->d_item_first);
-  }
 }
 
 const DevicePlan* FusedSra::prepare(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
@@ -66,47 +62,10 @@ const DevicePlan* FusedSra::prepare_impl(const std::vector<LayerSpec>& layers, i
   opt.dtype = dtype;
   opt.skip_incomplete = skip_incomplete;
   opt.min_lane_elems = min_lane_elems_;
-  const uint64_t key = plan_key(layers, opt);
-  auto it = cache_.find(key);
-  if (it == cache_.end()) {
-    if (cache_.size() >= kMaxCachedPlans) {
-      // workloads with ever-changing message sizes: drop everything (kernels that still read the
-      // old tables are ordered before the frees by the synchronize) and invalidate derived caches
-      cuda_check(cudaStreamSynchronize(stream), "sync before trimming the plan cache");
-      for (auto& kv : cache_) {
-        if (kv.second->d_items) cudaFree(kv.second->d_items);
-        if (kv.second->d_item_first) cudaFree(kv.second->d_item_first);
-      }
-      cache_.clear();
-      ++generation_;
-    }
-    auto dp = std::make_unique<DevicePlan>();
-    dp->plan = build_plan(layers, opt);
-    {
-      bool ok = true;
-      for (const BlockDesc& bd : dp->plan.blocks) {
-        const int bb = block_bits(bd);
-        ok = ok && (block_is_raw(bd) || bb == 2 || bb == 4 || bb == 8);
-      }
-      dp->multicast_ok = ok;
-    }
-    if (dp->plan.max_chunk_wire <= capacity && !dp->plan.items.empty()) {
-      const size_t ib = dp->plan.items.size() * sizeof(WarpItem);
-      const size_t fb = dp->plan.item_first.size() * sizeof(uint32_t);
-      cuda_check(cudaMalloc((void**)&dp->d_items, ib), "cudaMalloc(plan items)");
-      cuda_check(cudaMalloc((void**)&dp->d_item_first, fb), "cudaMalloc(plan lanes)");
-      // pageable source: the runtime stages it before returning, so the vectors may be reused
-      cuda_check(cudaMemcpyAsync(dp->d_items, dp->plan.items.data(), ib, cudaMemcpyHostToDevice, stream),
-                 "upload plan items");
-      cuda_check(cudaMemcpyAsync(dp->d_item_first, dp->plan.item_first.data(), fb, cudaMemcpyHostToDevice, stream),
-                 "upload plan lanes");
-    }
-    if (log_level() >= 2) log_msg(2, "cgx[%d]: new plan %s", rank(), describe_plan(dp->plan).c_str());
-    it = cache_.emplace(key, std::move(dp)).first;
-  }
-  const DevicePlan* dp = it->second.get();
-  if (dp->plan.max_chunk_wire > capacity) return nullptr;
-  return dp;
+  const DevicePlan& dp = plans_.get(layers, opt, stream);
+  if (dp.plan.max_chunk_wire > capacity) return nullptr;
+  plans_.upload(dp, stream);
+  return &dp;
 }
 
 void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream) {

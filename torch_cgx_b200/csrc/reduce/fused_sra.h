@@ -17,15 +17,9 @@
 #include "../comm/symmetric_heap.h"
 #include "../common/plan.h"
 #include "../common/sra_sim.h"
+#include "plan_cache.h"
 
 namespace cgx {
-
-struct DevicePlan {
-  Plan plan;
-  WarpItem* d_items = nullptr;       // flattened warp work list (device)
-  uint32_t* d_item_first = nullptr;  // [world * lanes + 1]
-  bool multicast_ok = false;         // every compressed item has a width multimem.st can carry (2/4/8)
-};
 
 // The two sharded collectives. Both move S-element shards through one table and the same windows;
 // the reduce-scatter reads W * S elements and writes the shard, the all-gather the other way round.
@@ -162,9 +156,9 @@ class FusedSra {
   int last_lanes() const { return last_lanes_; }
   uint64_t launches() const { return launches_; }
   // bumped whenever cached DevicePlan pointers become invalid (cache trimmed)
-  uint64_t generation() const { return generation_; }
+  uint64_t generation() const { return plans_.generation(); }
   uint32_t epoch() const { return epoch_; }
-  size_t num_plans() const { return cache_.size(); }
+  size_t num_plans() const { return plans_.size(); }
 
  private:
   SymmetricHeap* heap_;
@@ -180,13 +174,12 @@ class FusedSra {
   unsigned long long* d_trace_ = nullptr;
   bool trace_on_ = false;
   int last_lanes_ = 0;
-  uint64_t generation_ = 1;
   static constexpr size_t kMaxCachedPlans = 1024;
+  PlanCache plans_{kMaxCachedPlans};  // no byte bound
   const DevicePlan* prepare_impl(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                  cudaStream_t stream, int plan_world, uint32_t capacity, int max_lanes);
   void launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
               bool oneshot, void* out = nullptr, uint64_t out_shift = 0, bool gather = false);
-  std::unordered_map<uint64_t, std::unique_ptr<DevicePlan>> cache_;
   std::unordered_map<uint64_t, std::vector<std::vector<LayerSpec>>> rs_windows_;
 };
 

@@ -15,16 +15,16 @@ Reducer::~Reducer() {
     if (b.p) ops_->release(b.p);
 }
 
-const Plan& Reducer::plan_for(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete, int world) {
+const DevicePlan& Reducer::plan_for(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
+                                    cudaStream_t stream, int world) {
   PlanOptions opt;
   opt.world = world > 0 ? world : comm_->size();
   opt.lanes = 1;  // rank chunks only: one kernel launch per chunk handles all of its blocks
   opt.dtype = dtype;
   opt.skip_incomplete = skip_incomplete;
-  const uint64_t key = plan_key(layers, opt);
-  auto it = plans_.find(key);
-  if (it == plans_.end()) it = plans_.emplace(key, std::make_unique<Plan>(build_plan(layers, opt))).first;
-  return *it->second;
+  const DevicePlan& dp = plans_.get(layers, opt, stream);
+  if (ops_->is_cuda()) plans_.upload(dp, stream);
+  return dp;
 }
 
 uint8_t* Reducer::scratch(int slot, size_t bytes) {
@@ -69,16 +69,16 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
                                    int root, const RngParams& rng, cudaStream_t stream) {
   const int W = comm_->size(), r = comm_->rank();
   if (W == 1) return;
-  const Plan& plan = plan_for(layers, dtype, skip_incomplete, 1);  // the whole buffer is one chunk
+  const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream, 1);  // the whole buffer is one chunk
+  const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
-  ops_->bind(plan, stream);
   const uint32_t nb = (uint32_t)plan.blocks.size();
   const size_t bytes = plan.chunk_wire_bytes[0];
   uint8_t* wire = scratch(4, row_bytes(plan));
   std::vector<P2POp> x;
   if (r == root) {
-    ops_->quantize(data, 0, nb, wire, 1.0f, make_rng_key(rng, root, 2), stream);
-    ops_->dequantize(wire, 0, nb, data, stream);  // the root keeps what the receivers will decode
+    ops_->quantize(dp, data, 0, nb, wire, 1.0f, make_rng_key(rng, root, 2), stream);
+    ops_->dequantize(dp, wire, 0, nb, data, stream);  // the root keeps what the receivers will decode
     for (int p = 0; p < W; ++p)
       if (p != root) x.push_back({true, wire, bytes, p});
     bytes_sent_ += bytes * (uint64_t)(W - 1);
@@ -86,7 +86,7 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
   } else {
     x.push_back({false, wire, bytes, root});
     comm_->exchange(x, stream);
-    ops_->dequantize(wire, 0, nb, data, stream);
+    ops_->dequantize(dp, wire, 0, nb, data, stream);
   }
 }
 
@@ -98,8 +98,8 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
   if (S == 0) return;
   if (S * (uint64_t)W >= (1ull << 32))
     throw std::invalid_argument("cgx reduce_scatter: the input exceeds 2^32 elements");
-  const Plan& plan = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete);
-  ops_->bind(plan, stream);
+  const DevicePlan& dp = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete, stream);
+  const Plan& plan = dp.plan;
   const size_t row = row_bytes(plan);
   uint8_t* sendb = scratch(0, row * W);
   uint8_t* recvb = scratch(1, row * W);
@@ -112,24 +112,23 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->quantize(in, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
+    if (pn) ops_->quantize(dp, in, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
     if (plan.chunk_wire_bytes[p]) x.push_back({true, sendb + row * p, plan.chunk_wire_bytes[p], p});
     if (plan.chunk_wire_bytes[r]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[r], p});
     bytes_sent_ += plan.chunk_wire_bytes[p];
   }
   comm_->exchange(x, stream);
   if (!cn) return;
-  ops_->accumulate(nullptr, cb, cn, acc, lo, in, prescale, stream);
+  ops_->accumulate(dp, nullptr, cb, cn, acc, lo, in, prescale, stream);
   for (int q = 0; q < W; ++q)
-    if (q != r) ops_->accumulate(recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
+    if (q != r) ops_->accumulate(dp, recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
   // store the fp32 sums as T: a raw plan of one shard does exactly that (acc[i] is element i of the
   // shard, chunk r starting at r * S)
   std::vector<LayerSpec> raw = shard_layers;
   for (LayerSpec& l : raw) l.bits = kRawBits;
-  const Plan& rp = plan_for(raw, dtype, false, 1);
-  ops_->bind(rp, stream);
-  ops_->quantize_f32(acc, lo - (uint32_t)(r * S), 0, (uint32_t)rp.blocks.size(), scratch(2, row_bytes(rp)),
-                     make_rng_key(rng, r, 1), out, stream);
+  const DevicePlan& rp = plan_for(raw, dtype, false, stream, 1);
+  ops_->quantize_f32(rp, acc, lo - (uint32_t)(r * S), 0, (uint32_t)rp.plan.blocks.size(),
+                     scratch(2, row_bytes(rp.plan)), make_rng_key(rng, r, 1), out, stream);
 }
 
 void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
@@ -139,8 +138,8 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   if (S == 0) return;
   if (S * (uint64_t)W >= (1ull << 32))
     throw std::invalid_argument("cgx all_gather: the output exceeds 2^32 elements");
-  const Plan& plan = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete);
-  ops_->bind(plan, stream);
+  const DevicePlan& dp = plan_for(replicate(shard_layers, W, S), dtype, skip_incomplete, stream);
+  const Plan& plan = dp.plan;
   const size_t row = row_bytes(plan);
   uint8_t* recvb = scratch(1, row * W);
   uint8_t* mine = scratch(2, row);
@@ -150,8 +149,8 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   // the root's part of the compressed broadcast: quantize once, keep what the peers will decode
   const uint32_t cb = plan.chunk_begin(r), cn = plan.chunk_end(r) - cb;
   if (cn) {
-    ops_->quantize(out, cb, cn, mine, 1.0f, make_rng_key(rng, r, 1), stream);
-    ops_->dequantize(mine, cb, cn, out, stream);
+    ops_->quantize(dp, out, cb, cn, mine, 1.0f, make_rng_key(rng, r, 1), stream);
+    ops_->dequantize(dp, mine, cb, cn, out, stream);
   }
   std::vector<P2POp> x;
   for (int p = 0; p < W; ++p) {
@@ -164,7 +163,7 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->dequantize(recvb + row * p, pb, pn, out, stream);
+    if (pn) ops_->dequantize(dp, recvb + row * p, pb, pn, out, stream);
   }
 }
 
@@ -177,46 +176,31 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
   const bool raw = bits >= kRawBits;
   const uint8_t* src = static_cast<const uint8_t*>(in);
   uint8_t* dst = static_cast<uint8_t*>(out);
-  std::vector<size_t> io(W), oo(W), so(W + 1, 0), ro(W + 1, 0);
-  std::vector<const Plan*> sp(W, nullptr), rp(W, nullptr);
-  if (a2a_plans_.size() + 2 * (size_t)W > kMaxA2aPlans) {
-    // host-side tables only: the device backend keeps its own copy of the bound one, and a plan
-    // rebuilt at a freed address must not be mistaken for the bound one
-    ops_->unbind();
-    a2a_plans_.clear();
-  }
-  auto chunk_plan = [&](uint64_t n) -> const Plan* {
-    PlanOptions opt;
-    opt.world = 1;
-    opt.lanes = 1;
-    opt.dtype = dtype;
-    const std::vector<LayerSpec> layer{LayerSpec{0, n, bits, bucket}};
-    const uint64_t key = plan_key(layer, opt);
-    auto it = a2a_plans_.find(key);
-    if (it == a2a_plans_.end()) it = a2a_plans_.emplace(key, std::make_unique<Plan>(build_plan(layer, opt))).first;
-    return it->second.get();
-  };
+  // A peer chunk's record bytes follow from its size (common/a2a.h, which is build_plan's one-layer
+  // plan of the chunk); its plan is asked for right where it is quantized or decoded.
+  std::vector<size_t> io(W), oo(W), sw(W, 0), rw(W, 0), so(W + 1, 0), ro(W + 1, 0);
   uint64_t i = 0, o = 0;
   for (int q = 0; q < W; ++q) {
     io[q] = (size_t)i * es;
     oo[q] = (size_t)o * es;
     i += in_counts[q];
     o += out_counts[q];
-    const bool peer = q != r && !raw;
-    if (peer && in_counts[q]) sp[q] = chunk_plan(in_counts[q]);
-    if (peer && out_counts[q]) rp[q] = chunk_plan(out_counts[q]);
-    so[q + 1] = so[q] + (sp[q] ? (sp[q]->chunk_wire_bytes[0] + 255) / 256 * 256 : 0);
-    ro[q + 1] = ro[q] + (rp[q] ? (rp[q]->chunk_wire_bytes[0] + 255) / 256 * 256 : 0);
+    if (q != r && !raw) {
+      sw[q] = a2a_chunk_wire(a2a_geom((uint32_t)in_counts[q], bits, bucket, (int)es));
+      rw[q] = a2a_chunk_wire(a2a_geom((uint32_t)out_counts[q], bits, bucket, (int)es));
+    }
+    so[q + 1] = so[q] + (sw[q] + 255) / 256 * 256;
+    ro[q + 1] = ro[q] + (rw[q] + 255) / 256 * 256;
   }
   if (in_counts[r]) ops_->copy(dst + oo[r], src + io[r], in_counts[r] * es, stream);
   uint8_t* sendb = raw ? nullptr : scratch(0, so[W] + 16);
   uint8_t* recvb = raw ? nullptr : scratch(1, ro[W] + 16);
   for (int q = 0; q < W; ++q) {
-    if (!sp[q]) continue;
+    if (!sw[q]) continue;
     RngKey key = make_rng_key(rng, r, 0);
     key.stream = a2a_rng_stream(r, q);
-    ops_->bind(*sp[q], stream);
-    ops_->quantize(src + io[q], 0, (uint32_t)sp[q]->blocks.size(), sendb + so[q], 1.0f, key, stream);
+    const DevicePlan& dp = plan_for({LayerSpec{0, in_counts[q], bits, bucket}}, dtype, false, stream, 1);
+    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, key, stream);
   }
   std::vector<P2POp> x;
   for (int q = 0; q < W; ++q) {
@@ -227,25 +211,25 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
       bytes_sent_ += in_counts[q] * es;
       continue;
     }
-    if (sp[q]) x.push_back({true, sendb + so[q], sp[q]->chunk_wire_bytes[0], q});
-    if (rp[q]) x.push_back({false, recvb + ro[q], rp[q]->chunk_wire_bytes[0], q});
-    if (sp[q]) bytes_sent_ += sp[q]->chunk_wire_bytes[0];
+    if (sw[q]) x.push_back({true, sendb + so[q], sw[q], q});
+    if (rw[q]) x.push_back({false, recvb + ro[q], rw[q], q});
+    bytes_sent_ += sw[q];
   }
   comm_->exchange(x, stream);
   for (int q = 0; q < W; ++q) {
-    if (!rp[q]) continue;
-    ops_->bind(*rp[q], stream);
-    ops_->dequantize(recvb + ro[q], 0, (uint32_t)rp[q]->blocks.size(), dst + oo[q], stream);
+    if (!rw[q]) continue;
+    const DevicePlan& dp = plan_for({LayerSpec{0, out_counts[q], bits, bucket}}, dtype, false, stream, 1);
+    ops_->dequantize(dp, recvb + ro[q], 0, (uint32_t)dp.plan.blocks.size(), dst + oo[q], stream);
   }
 }
 
 // ---------------------------------------------------------------------- SRA --
 void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
                            float prescale, const RngParams& rng, cudaStream_t stream) {
-  const Plan& plan = plan_for(layers, dtype, skip_incomplete);
+  const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
+  const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
   const int W = comm_->size(), r = comm_->rank();
-  ops_->bind(plan, stream);
   const size_t row = row_bytes(plan);
   uint8_t* sendb = scratch(0, row * W);
   uint8_t* recvb = scratch(1, row * W);
@@ -260,7 +244,7 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->quantize(data, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
+    if (pn) ops_->quantize(dp, data, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
     if (plan.chunk_wire_bytes[p]) x.push_back({true, sendb + row * p, plan.chunk_wire_bytes[p], p});
     if (plan.chunk_wire_bytes[r]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[r], p});
     bytes_sent_ += plan.chunk_wire_bytes[p];
@@ -268,11 +252,11 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   comm_->exchange(x, stream);
   // reduce my chunk in fp32: own raw values first, then the peers in rank order
   if (cn) {
-    ops_->accumulate(nullptr, cb, cn, acc, lo, data, prescale, stream);
+    ops_->accumulate(dp, nullptr, cb, cn, acc, lo, data, prescale, stream);
     for (int q = 0; q < W; ++q)
-      if (q != r) ops_->accumulate(recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
+      if (q != r) ops_->accumulate(dp, recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
     // requantize + self-decode so that every rank ends with identical values
-    ops_->quantize_f32(acc, lo, cb, cn, mine, make_rng_key(rng, r, 1), data, stream);
+    ops_->quantize_f32(dp, acc, lo, cb, cn, mine, make_rng_key(rng, r, 1), data, stream);
   }
   // phase 2: all-gather of the reduced chunks
   x.clear();
@@ -286,17 +270,17 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->dequantize(recvb + row * p, pb, pn, data, stream);
+    if (pn) ops_->dequantize(dp, recvb + row * p, pb, pn, data, stream);
   }
 }
 
 // --------------------------------------------------------------------- Ring --
 void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
                             float prescale, const RngParams& rng, cudaStream_t stream) {
-  const Plan& plan = plan_for(layers, dtype, skip_incomplete);
+  const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
+  const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
   const int W = comm_->size(), r = comm_->rank();
-  ops_->bind(plan, stream);
   const size_t row = row_bytes(plan);
   uint8_t* bufa = scratch(0, row);
   uint8_t* bufb = scratch(1, row);
@@ -306,20 +290,21 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
   const uint32_t nblocks = (uint32_t)plan.blocks.size();
   auto cb = [&](int c) { return plan.chunk_begin(c); };
   auto cn = [&](int c) { return plan.chunk_end(c) - plan.chunk_begin(c); };
-  ops_->accumulate(nullptr, 0, nblocks, acc, lo, data, prescale, stream);
+  ops_->accumulate(dp, nullptr, 0, nblocks, acc, lo, data, prescale, stream);
   const int right = (r + 1) % W, left = (r + W - 1) % W;
   // reduce-scatter: W-1 hops, the travelling partial sum is requantized at every hop
   for (int s = 0; s + 1 < W; ++s) {
     const int sseg = (r - s + W) % W, rseg = (r - s - 1 + 2 * W) % W;
     RngParams hop = rng;
     hop.seq = rng.seq * 16u + (uint32_t)s;
-    if (cn(sseg)) ops_->quantize_f32(acc, lo, cb(sseg), cn(sseg), bufa, make_rng_key(hop, r, 0), nullptr, stream);
+    if (cn(sseg))
+      ops_->quantize_f32(dp, acc, lo, cb(sseg), cn(sseg), bufa, make_rng_key(hop, r, 0), nullptr, stream);
     std::vector<P2POp> x;
     if (plan.chunk_wire_bytes[sseg]) x.push_back({true, bufa, plan.chunk_wire_bytes[sseg], right});
     if (plan.chunk_wire_bytes[rseg]) x.push_back({false, bufb, plan.chunk_wire_bytes[rseg], left});
     bytes_sent_ += plan.chunk_wire_bytes[sseg];
     comm_->exchange(x, stream);
-    if (cn(rseg)) ops_->accumulate(bufb, cb(rseg), cn(rseg), acc, lo, nullptr, 1.0f, stream);
+    if (cn(rseg)) ops_->accumulate(dp, bufb, cb(rseg), cn(rseg), acc, lo, nullptr, 1.0f, stream);
   }
   // the fully reduced segment of this rank: requantize once more and self-decode
   int cur = (r + 1) % W;
@@ -328,7 +313,7 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
   fin.seq = rng.seq * 16u + 15u;
   uint8_t* have = bufa;
   uint8_t* next = bufb;
-  if (cn(cur)) ops_->quantize_f32(acc, lo, cb(cur), cn(cur), have, make_rng_key(fin, r, 1), data, stream);
+  if (cn(cur)) ops_->quantize_f32(dp, acc, lo, cb(cur), cn(cur), have, make_rng_key(fin, r, 1), data, stream);
   // all-gather: forward the already-compressed bytes around the ring, decode locally
   for (int s = 0; s + 1 < W; ++s) {
     const int rseg = (cur + W - 1) % W;
@@ -337,7 +322,7 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
     if (plan.chunk_wire_bytes[rseg]) x.push_back({false, next, plan.chunk_wire_bytes[rseg], left});
     bytes_sent_ += plan.chunk_wire_bytes[cur];
     comm_->exchange(x, stream);
-    if (cn(rseg)) ops_->dequantize(next, cb(rseg), cn(rseg), data, stream);
+    if (cn(rseg)) ops_->dequantize(dp, next, cb(rseg), cn(rseg), data, stream);
     std::swap(have, next);
     cur = rseg;
   }
@@ -346,10 +331,10 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
 // ----------------------------------------------------------------- AllToAll --
 void AllToAllReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
                                 float prescale, const RngParams& rng, cudaStream_t stream) {
-  const Plan& plan = plan_for(layers, dtype, skip_incomplete);
+  const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
+  const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
   const int W = comm_->size(), r = comm_->rank();
-  ops_->bind(plan, stream);
   const size_t row = row_bytes(plan);
   const size_t whole = row * W;  // chunk c of the wire image lives at row * c
   uint8_t* sendb = scratch(0, whole);
@@ -359,7 +344,7 @@ void AllToAllReducer::allreduce(void* data, int dtype, const std::vector<LayerSp
   float* acc = reinterpret_cast<float*>(scratch(3, (size_t)(hi - lo) * sizeof(float) + 16));
   for (int c = 0; c < W; ++c) {
     const uint32_t b0 = plan.chunk_begin(c), bn = plan.chunk_end(c) - b0;
-    if (bn) ops_->quantize(data, b0, bn, sendb + row * c, prescale, make_rng_key(rng, r, 0), stream);
+    if (bn) ops_->quantize(dp, data, b0, bn, sendb + row * c, prescale, make_rng_key(rng, r, 0), stream);
   }
   std::vector<P2POp> x;
   for (int p = 0; p < W; ++p) {
@@ -369,23 +354,23 @@ void AllToAllReducer::allreduce(void* data, int dtype, const std::vector<LayerSp
     bytes_sent_ += whole;
   }
   comm_->exchange(x, stream);
-  ops_->accumulate(nullptr, 0, (uint32_t)plan.blocks.size(), acc, lo, data, prescale, stream);
+  ops_->accumulate(dp, nullptr, 0, (uint32_t)plan.blocks.size(), acc, lo, data, prescale, stream);
   for (int q = 0; q < W; ++q) {
     if (q == r) continue;
     for (int c = 0; c < W; ++c) {
       const uint32_t b0 = plan.chunk_begin(c), bn = plan.chunk_end(c) - b0;
-      if (bn) ops_->accumulate(recvb + whole * q + row * c, b0, bn, acc, lo, nullptr, 1.0f, stream);
+      if (bn) ops_->accumulate(dp, recvb + whole * q + row * c, b0, bn, acc, lo, nullptr, 1.0f, stream);
     }
   }
   // store the fp32 sums back as T: a "raw" plan of the same layers does exactly that
   std::vector<LayerSpec> raw = layers;
   for (LayerSpec& l : raw) l.bits = kRawBits;
-  const Plan& rp = plan_for(raw, dtype, false);
-  ops_->bind(rp, stream);
+  const DevicePlan& rdp = plan_for(raw, dtype, false, stream);
+  const Plan& rp = rdp.plan;
   uint8_t* tmp = scratch(2, row_bytes(rp) * W);
   for (int c = 0; c < W; ++c) {
     const uint32_t b0 = rp.chunk_begin(c), bn = rp.chunk_end(c) - b0;
-    if (bn) ops_->quantize_f32(acc, lo, b0, bn, tmp + row_bytes(rp) * c, make_rng_key(rng, r, 1), data, stream);
+    if (bn) ops_->quantize_f32(rdp, acc, lo, b0, bn, tmp + row_bytes(rp) * c, make_rng_key(rng, r, 1), data, stream);
   }
 }
 

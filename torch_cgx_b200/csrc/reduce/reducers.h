@@ -14,7 +14,6 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <memory>
-#include <unordered_map>
 #include <vector>
 
 #include "../comm/communicator.h"
@@ -22,6 +21,7 @@
 #include "../common/plan.h"
 #include "../common/sra_sim.h"
 #include "block_backend.h"
+#include "plan_cache.h"
 
 namespace cgx {
 
@@ -65,10 +65,16 @@ class Reducer {
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, const RngParams& rng,
                   cudaStream_t stream);
   uint64_t bytes_sent() const { return bytes_sent_; }
+  size_t num_plans() const { return plans_.size(); }
+  uint64_t plan_uploads() const { return plans_.uploads(); }
 
  protected:
-  // world <= 0: one chunk per rank of the communicator; otherwise that many chunks
-  const Plan& plan_for(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete, int world = 0);
+  // The plan of `layers`, uploaded when the backend is the device's. world <= 0: one chunk per rank
+  // of the communicator; otherwise that many chunks. A call never uses a plan after it has asked for
+  // another: the request may drop the cache, which frees every earlier plan (after synchronising
+  // `stream`, so no kernel still reads them).
+  const DevicePlan& plan_for(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
+                             cudaStream_t stream, int world = 0);
   uint8_t* scratch(int slot, size_t bytes);  // grow-only scratch buffers of the backend's memory kind
   static size_t row_bytes(const Plan& p) { return ((size_t)p.max_chunk_wire + 255) / 256 * 256; }
   // [first element, one past last element) spanned by the blocks of a chunk / of the whole plan
@@ -79,11 +85,12 @@ class Reducer {
   uint64_t bytes_sent_ = 0;
 
  private:
-  std::unordered_map<uint64_t, std::unique_ptr<Plan>> plans_;
-  // all_to_all: one-layer plans per chunk size; MoE splits change every call, so this cache is
-  // bounded (kMaxA2aPlans) and dropped as a whole when a call could overflow it
-  std::unordered_map<uint64_t, std::unique_ptr<Plan>> a2a_plans_;
-  static constexpr size_t kMaxA2aPlans = 256;
+  // Bounded, since tensor sizes and MoE splits may change every call. Both figures are design
+  // choices, not measurements: 256 plans covers the layouts of a training step with room to spare,
+  // and 64 MiB of tables is about four million warp items, the tables of some 2G elements.
+  static constexpr size_t kMaxPlans = 256;
+  static constexpr size_t kMaxTableBytes = 64ull << 20;
+  PlanCache plans_{kMaxPlans, kMaxTableBytes};
   struct Buf {
     uint8_t* p = nullptr;
     size_t cap = 0;
