@@ -1,0 +1,168 @@
+#!/usr/bin/env python
+"""MoE token dispatch and combine on W virtual ranks of one GPU (C.LocalSraGroup): the routed
+all-to-all (rows gathered and scattered by index inside a2a_kernel) against the composition a
+caller writes without it, index_select + plain all-to-all + index_copy_.
+
+Every rank holds T tokens of H elements and routes each to top-k of E = 8 W experts (8 per rank),
+seeded. The sent rows are sorted by destination rank: row i is token input_index[i]; the combine
+returns them into T k slots (token * k + choice), slot output_index[j] for received row j.
+
+  dispatch (a): send = x.index_select(0, input_index); all_to_all(recv, send)
+  dispatch (b): all_to_all(recv, x, input_index)
+  combine  (a): all_to_all(back, recv); out.index_copy_(0, output_index, back)
+  combine  (b): all_to_all(out, recv, output_index)
+
+Arms alternate in one run, CUDA events around each, medians over --iters after --warmup. The HBM
+bytes of an arm are computed from shapes, all ranks together: the kernel reads the sent rows and
+writes the received rows (2 N H es), writes and reads its wire image once (2 N H bits / 8, plus
+8 bytes per 512-element bucket; raw at 32 bits, and own chunks are copied, not counted as wire);
+arm (a) adds the permutation's read and write of N rows (2 N H es). Virtual ranks share one GPU's
+HBM and exchange through it, so NVLink is not part of these numbers.
+"""
+import argparse
+import json
+import subprocess
+import sys
+from pathlib import Path
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+import torch  # noqa: E402
+
+import torch_cgx_b200 as cgx  # noqa: E402
+
+C = cgx._C
+
+
+def gpu_info():
+    name = torch.cuda.get_device_name(0)
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        out = "unknown"
+    return name, out
+
+
+def routing(W, T, k, seed, device):
+    g = torch.Generator(device=device).manual_seed(seed)
+    E = 8 * W
+    per_rank = []
+    for _ in range(W):
+        experts = torch.rand(T, E, generator=g, device=device).topk(k, dim=1).indices  # [T, k], distinct
+        dest = (experts // 8).reshape(-1)
+        order = torch.argsort(dest, stable=True)
+        per_rank.append((order // k, order, torch.bincount(dest, minlength=W).tolist()))
+    return per_rank
+
+
+def median(xs):
+    xs = sorted(xs)
+    return xs[len(xs) // 2]
+
+
+def run_config(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
+    dev = torch.device("cuda", 0)
+    es = torch.tensor([], dtype=dtype).element_size()
+    route = routing(W, T, k, seed=T * 31 + H * 7 + k, device=dev)
+    send_rows = [route[q][2] for q in range(W)]
+    recv_n = [sum(send_rows[q][r] for q in range(W)) for r in range(W)]
+    disp_counts = [[send_rows[q][r] * H for r in range(W)] for q in range(W)]
+    comb_counts = [[disp_counts[r][q] for r in range(W)] for q in range(W)]
+    g = C.LocalSraGroup(W, lanes, slot_mb << 20, 20000, 256)
+    xs = [torch.randn(T, H, device=dev, dtype=dtype) for _ in range(W)]
+    send = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    recv = [torch.empty(recv_n[r], H, device=dev, dtype=dtype) for r in range(W)]
+    back = send  # free once the dispatch has run: the combine's arm (a) reuses it
+    out = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    ii = [route[q][0] for q in range(W)]
+    oi = [route[q][1] for q in range(W)]
+    flat = lambda ts: [t.reshape(-1) for t in ts]  # noqa: E731
+
+    def disp_a():
+        for q in range(W):
+            torch.index_select(xs[q], 0, ii[q], out=send[q])
+        g.all_to_all(flat(send), flat(recv), disp_counts, bits=bits, bucket_size=512)
+
+    def disp_b():
+        g.all_to_all(flat(xs), flat(recv), disp_counts, bits=bits, bucket_size=512, input_index=ii, row=H)
+
+    def comb_a():
+        g.all_to_all(flat(recv), flat(back), comb_counts, bits=bits, bucket_size=512)
+        for q in range(W):
+            out[q].index_copy_(0, oi[q], back[q])
+
+    def comb_b():
+        g.all_to_all(flat(recv), flat(out), comb_counts, bits=bits, bucket_size=512, output_index=oi, row=H)
+
+    arms = {"dispatch_a": disp_a, "dispatch_b": disp_b, "combine_a": comb_a, "combine_b": comb_b}
+    ts = {name: [] for name in arms}
+    for it in range(warmup + iters):
+        for name, fn in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            if it >= warmup:
+                ts[name].append(e0.elapsed_time(e1) * 1000.0)
+    g.check()
+    # the arms compute the same bytes
+    ref_out = [o.clone() for o in out]
+    comb_a()
+    torch.cuda.synchronize()
+    for q in range(W):
+        assert torch.equal(ref_out[q], out[q]), "combine arms differ"
+
+    N = T * k * W  # rows sent by all ranks
+    own = sum(send_rows[q][q] for q in range(W))
+    elems_wire = (N - own) * H
+    wire = elems_wire * es if bits >= 32 else elems_wire * bits // 8 + (elems_wire // 512) * 8
+    kernel_bytes = 2 * N * H * es + 2 * wire
+    perm_bytes = 2 * N * H * es
+    res = {"W": W, "T": T, "H": H, "topk": k, "bits": bits, "dtype": str(dtype).replace("torch.", "")}
+    for name in arms:
+        res[name + "_us"] = round(median(ts[name]), 1)
+    res["bytes_b_GB"] = round(kernel_bytes / 1e9, 3)
+    res["bytes_a_GB"] = round((kernel_bytes + perm_bytes) / 1e9, 3)
+    del g, xs, send, recv, back, out
+    torch.cuda.empty_cache()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--world", type=int, default=8)
+    ap.add_argument("--hidden", type=int, nargs="+", default=[4096, 7168])
+    ap.add_argument("--tokens", type=int, nargs="+", default=[4096, 16384])
+    ap.add_argument("--topk", type=int, nargs="+", default=[2, 8])
+    ap.add_argument("--bits", type=int, nargs="+", default=[4, 8, 32])
+    ap.add_argument("--iters", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    # 16 lanes x 8 ranks = 128 CTAs: the virtual ranks together occupy the GPU, as one real rank would its own
+    ap.add_argument("--lanes", type=int, default=16)
+    ap.add_argument("--slot-mb", type=int, default=4)
+    ap.add_argument("--max-gb", type=float, default=60.0, help="skip configurations whose buffers exceed this")
+    ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
+    args = ap.parse_args()
+    name, power = gpu_info()
+    print(json.dumps({"gpu": name, "power_limit": power}), flush=True)
+    rows = []
+    for H in args.hidden:
+        for T in args.tokens:
+            for k in args.topk:
+                need = args.world * (3 * T * k + T) * H * 2 / 1e9
+                if need > args.max_gb:
+                    print(json.dumps({"H": H, "T": T, "topk": k, "skipped": f"needs {need:.1f} GB"}), flush=True)
+                    continue
+                for bits in args.bits:
+                    r = run_config(args.world, T, H, k, bits, args.iters, args.warmup, args.lanes, args.slot_mb)
+                    r.update(gpu=name, power_limit=power)
+                    rows.append(r)
+                    print(json.dumps(r), flush=True)
+    if args.out:
+        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in rows))
+
+
+if __name__ == "__main__":
+    main()

@@ -233,6 +233,8 @@ void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
 
 // ---- all-to-all: counts[q][r] elements go from rank q to rank r ------------------------------
 using CountMatrix = std::vector<std::vector<int64_t>>;
+// one optional row index per virtual rank (the routed all-to-all)
+using IndexList = std::vector<std::optional<at::Tensor>>;
 
 std::vector<std::vector<uint64_t>> check_counts(const CountMatrix& counts, size_t W) {
   TORCH_CHECK(counts.size() == W, "all_to_all: counts must be a W x W matrix");
@@ -532,11 +534,55 @@ class LocalSraGroup {
     sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq);
   }
   // all-to-all: counts[q][r] elements go from virtual rank q to r; inputs[r] holds row r of the
-  // matrix in destination order, outputs[r] receives column r in source order
+  // matrix in destination order, outputs[r] receives column r in source order.
+  // Routed form (the fused kernel's, so a2a_rows_fit(row, ...) must hold): input_index[r] /
+  // output_index[r], when given and not None, are rank r's int64 row indices into inputs[r] /
+  // outputs[r], rows of `row` elements; the counts then describe the logical buffers of whole rows.
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
-                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq, const IndexList& input_index,
+                  const IndexList& output_index, int64_t row) {
     const auto counts = check_counts(counts_in, (size_t)world_);
-    check_a2a_tensors(inputs, outputs, counts, true);
+    const bool routed = !input_index.empty() || !output_index.empty();
+    TORCH_CHECK(input_index.empty() || (int)input_index.size() == world_, "all_to_all: one input_index per rank");
+    TORCH_CHECK(output_index.empty() || (int)output_index.size() == world_, "all_to_all: one output_index per rank");
+    std::vector<A2aRoute> routes((size_t)world_);
+    if (routed) {
+      TORCH_CHECK(row >= 1, "all_to_all: row must be >= 1");
+      for (int r = 0; r < world_; ++r) {
+        A2aRoute& rt = routes[r];
+        rt.row = (uint64_t)row;
+        rt.in_rows = (uint64_t)inputs[r].numel() / (uint64_t)row;
+        rt.out_rows = (uint64_t)outputs[r].numel() / (uint64_t)row;
+        uint64_t nin = 0, nout = 0;
+        for (int q = 0; q < world_; ++q) {
+          nin += counts[r][q];
+          nout += counts[q][r];
+        }
+        for (int side = 0; side < 2; ++side) {
+          const IndexList& list = side ? output_index : input_index;
+          if (list.empty() || !list[r].has_value()) continue;
+          const at::Tensor& ix = *list[r];
+          TORCH_CHECK(ix.is_cuda() && ix.scalar_type() == at::kLong && ix.dim() == 1 && ix.is_contiguous() &&
+                          (uint64_t)ix.numel() * (uint64_t)row == (side ? nout : nin),
+                      "all_to_all: rank ", r, "'s ", side ? "output" : "input",
+                      "_index must be a contiguous CUDA int64 vector of one entry per row of its counts");
+          (side ? rt.out_index : rt.in_index) = ix.data_ptr<int64_t>();
+        }
+      }
+    }
+    for (int r = 0; r < world_; ++r) {
+      const bool in_ix = routes[r].in_index != nullptr, out_ix = routes[r].out_index != nullptr;
+      uint64_t nin = 0, nout = 0;
+      for (int q = 0; q < world_; ++q) {
+        nin += counts[r][q];
+        nout += counts[q][r];
+      }
+      for (const at::Tensor* t : {&inputs[r], &outputs[r]})
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == cgx_dtype(inputs[0]),
+                    "all_to_all: contiguous tensors of one dtype, all on the GPU");
+      TORCH_CHECK((in_ix || (uint64_t)inputs[r].numel() == nin) && (out_ix || (uint64_t)outputs[r].numel() == nout),
+                  "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
+    }
     const int dt = cgx_dtype(inputs[0]);
     const RngParams rng = make_rng(stochastic, seed, seq);
     fork_join([](int) {},
@@ -544,7 +590,7 @@ class LocalSraGroup {
                 std::vector<uint64_t> out_counts(world_);
                 for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
                 fused_[r]->all_to_all(inputs[r].data_ptr(), outputs[r].data_ptr(), counts[r], out_counts, dt, bits,
-                                      (uint32_t)bucket, rng, streams_[r].stream());
+                                      (uint32_t)bucket, rng, streams_[r].stream(), routed ? &routes[r] : nullptr);
               });
   }
   void check() {
@@ -1389,12 +1435,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("layers") = std::vector<LayerTuple>{}, py::call_guard<py::gil_scoped_release>())
       .def("all_to_all_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
-              const std::vector<int64_t>& in_splits, int bits, int bucket_size, bool stochastic, int64_t seed) {
-             return pg.all_to_all_compressed(out, in, out_splits, in_splits, bits, bucket_size, stochastic, seed);
+              const std::vector<int64_t>& in_splits, int bits, int bucket_size, bool stochastic, int64_t seed,
+              const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index) {
+             return pg.all_to_all_compressed(out, in, out_splits, in_splits, bits, bucket_size, stochastic, seed,
+                                             in_index.value_or(at::Tensor()), out_index.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
            py::arg("input_split_sizes") = std::vector<int64_t>{}, py::arg("bits") = 8, py::arg("bucket_size") = 512,
-           py::arg("stochastic") = false, py::arg("seed") = -1, py::call_guard<py::gil_scoped_release>())
+           py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("input_index") = py::none(),
+           py::arg("output_index") = py::none(), py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -1570,6 +1619,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
         py::arg("seq") = 0);
   m.def("a2a_items", &py_a2a_items, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
+  m.def(
+      "a2a_rows_fit",
+      [](int64_t row, int bits, int64_t bucket, int dtype) {
+        return row >= 1 && row < (1ll << 32) && a2a_rows_fit((uint32_t)row, bits, (uint32_t)bucket, dtype_size(dtype));
+      },
+      py::arg("row"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
   m.def("a2a_windows", &py_a2a_windows, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype"),
         py::arg("slot_bytes"), py::arg("lanes"));
   m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
@@ -1670,7 +1725,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
       .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
-           py::arg("seq") = 0)
+           py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
+           py::arg("row") = 1)
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))

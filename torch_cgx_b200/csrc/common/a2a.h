@@ -112,6 +112,25 @@ CGX_HD WarpItem a2a_block_item(const A2aGeom& g, uint32_t b, uint32_t j) {
   return it;
 }
 
+// ---- routed rows --------------------------------------------------------------------------------
+// True iff every item a2a_block_item can produce for a chunk of whole rows of H elements lies
+// inside one row, so that the routed kernel can address an item as one span of one indexed row.
+// Items start at multiples of their span within a block, blocks at multiples of every span, and a
+// chunk of rows ends on a row boundary; so this holds iff H is a multiple of the span: 512 raw
+// elements, the slice for power-of-two buckets up to the slice (a chunk of whole slices has no
+// bucket tail), otherwise the clamped bucket. The element size does not enter.
+CGX_HD bool a2a_rows_fit(uint32_t H, int bits, uint32_t bucket, int elsize) {
+  const A2aGeom g = a2a_geom(0, bits, bucket, elsize);
+  uint32_t span;
+  if (g.bits >= kRawBits)
+    span = kRawItemElems;
+  else if (g.bucket >= 8u && (g.bucket & (g.bucket - 1u)) == 0u && g.bucket <= g.slice)
+    span = g.slice;
+  else
+    span = g.bucket;
+  return H >= 1u && H % span == 0u;
+}
+
 // ---- windows ----------------------------------------------------------------------------------
 // a lane's share of a per-source slot (16-byte granular)
 CGX_HD uint32_t a2a_lane_slot_bytes(uint32_t slot_bytes, int lanes) {

@@ -1,5 +1,6 @@
 #include "engine.h"
 
+#include "../common/a2a.h"
 #include "../common/nvtx.h"
 
 #include <algorithm>
@@ -321,14 +322,17 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
 
 void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                  const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                                 const RngParams& rng_in, cudaStream_t stream) {
+                                 const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route) {
   if (nodes() > 1)
     throw std::runtime_error("cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE " +
                              std::to_string(local_size_) + " < world size " + std::to_string(world_) + ")");
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rank_, world_);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rank_, world_, route);
+  const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
+  if (routed && !routes_in_kernel(cuda, dtype, bits, bucket, route->row))
+    throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
   if (!fused && world_ > 1 && !g.intra) throw std::runtime_error("cgx: the compressed all_to_all has no intra-node reducer");
   uint64_t total = 0;
   for (uint64_t n : in_counts) total += n;
@@ -340,7 +344,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
   stats_.elements += total;
   if (fused) {
     const FusedSra::A2aCounts n =
-        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream);
+        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream, route);
     stats_.kernel_launches += n.launches;
     stats_.wire_bytes += n.wire_bytes;
     stats_.raw_bytes += n.raw_bytes;
@@ -360,6 +364,10 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
   stats_.wire_bytes += g.intra->bytes_sent() - before;
   for (int q = 0; q < world_; ++q)
     if (q != rank_) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);
+}
+
+bool AllreduceEngine::routes_in_kernel(bool cuda, int dtype, int bits, uint32_t bucket, uint64_t row) const {
+  return fused_sharded(cuda) && row < (1ull << 32) && a2a_rows_fit((uint32_t)row, bits, bucket, dtype_size(dtype));
 }
 
 void AllreduceEngine::allreduce_cpu(void* data, int dtype, int64_t numel, bool average, int explicit_bucket) {

@@ -158,9 +158,14 @@ class AllreduceEngine {
   // Compressed all-to-all of device (cuda) or host buffers on `stream` (FusedSra::all_to_all for
   // the arguments): the fused kernel on the P2P transport, else the generic intra-node reducer. One
   // node only: with several nodes every rank throws the same std::runtime_error before anything runs.
+  // A `route` with an index needs routes_in_kernel(); callers compose index_select / index_copy_
+  // around a plain call otherwise.
   void all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                  const RngParams& rng_in, cudaStream_t stream);
+                  const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route = nullptr);
+  // whether a routed all-to-all of rows of `row` elements runs inside the fused kernel: the P2P
+  // transport with a heap, and rows that hold whole quantization items (a2a_rows_fit)
+  bool routes_in_kernel(bool cuda, int dtype, int bits, uint32_t bucket, uint64_t row) const;
 
   void check_health();
   void set_observer(EngineObserver* o) { observer_ = o; }

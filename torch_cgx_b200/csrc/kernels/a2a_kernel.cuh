@@ -87,6 +87,43 @@ __device__ __forceinline__ void a2a_raw_send(const T* src, const WarpItem& it, u
   }
 }
 
+// Routed form: element e of a logical buffer of whole rows of p.row elements lives in row
+// index[e / row] of `base`, column e % row (index == nullptr: the logical buffer is `base`). Called
+// with the same e by every lane of a warp, so the index load is one broadcast. A row outside
+// [0, rows) is never dereferenced: the status records which index held it and nullptr is returned.
+template <typename T>
+__device__ __forceinline__ T* a2a_row_addr(const A2aParams& p, T* base, const int64_t* index, uint64_t rows,
+                                          uint32_t e, uint32_t which) {
+  if (index == nullptr) return base + e;
+  const uint32_t row = e / p.row;
+  const int64_t i = index[row];
+  if (i < 0 || (uint64_t)i >= rows) {
+    if (lane_id() == 0) *p.status = (uint32_t)kSraBadIndex | ((uint32_t)p.rank << 8) | (which << 16);
+    return nullptr;
+  }
+  return base + (uint64_t)i * p.row + (e - row * p.row);
+}
+
+// my own chunk, routed: one warp per row, through both indices
+template <typename T>
+__device__ __forceinline__ void a2a_copy_own_rows(const A2aParams& p) {
+  const uint32_t H = p.row, rows = p.in_cnt[p.rank] / H;
+  const uint32_t nwarps = gridDim.x * kSraWarps;
+  for (uint32_t j = blockIdx.x * kSraWarps + (threadIdx.x >> 5); j < rows; j += nwarps) {
+    const T* src = a2a_row_addr(p, reinterpret_cast<const T*>(p.in), p.in_index, p.in_rows, p.in_off[p.rank] + j * H, 0u);
+    T* dst = a2a_row_addr(p, reinterpret_cast<T*>(p.out), p.out_index, p.out_rows, p.out_off[p.rank] + j * H, 1u);
+    if (src == nullptr || dst == nullptr) continue;
+    uint32_t done = 0;
+    if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
+      const uint32_t vecs = H * (uint32_t)sizeof(T) / 16u;
+      for (uint32_t v = lane_id(); v < vecs; v += 32)
+        reinterpret_cast<uint4*>(dst)[v] = reinterpret_cast<const uint4*>(src)[v];
+      done = vecs * 16u / (uint32_t)sizeof(T);
+    }
+    for (uint32_t i = done + lane_id(); i < H; i += 32) dst[i] = src[i];
+  }
+}
+
 // my own chunk: a bit copy, spread over every thread of the grid
 template <typename T>
 __device__ __forceinline__ void a2a_copy_own(const A2aParams& p) {
@@ -131,7 +168,7 @@ __device__ __forceinline__ bool a2a_window_item(const A2aGeom& g, const A2aWindo
   return true;
 }
 
-template <typename T, int KB, int GPL>
+template <typename T, int KB, int GPL, bool IDX>
 __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k,
                                                 const RngKey& rng) {
   const int r = p.rank;
@@ -145,7 +182,14 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
     uint32_t wire;
     if (!a2a_window_item(g, w, t, it, wire)) continue;
     const OneDst push{share + wire};
-    const T* src = chunk + it.elem_off;
+    const T* src;
+    if constexpr (IDX) {
+      // the item lies inside one row (a2a_rows_fit): one index load moves all of it
+      src = a2a_row_addr(p, reinterpret_cast<const T*>(p.in), p.in_index, p.in_rows, p.in_off[q] + it.elem_off, 0u);
+      if (src == nullptr) continue;
+    } else {
+      src = chunk + it.elem_off;
+    }
     const uint32_t kind = item_kind(it);
     if (kind == kItemFull) {
       if (group_aligned<T>(src)) {
@@ -163,7 +207,7 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
   }
 }
 
-template <typename T, int KB, int GPL>
+template <typename T, int KB, int GPL, bool IDX>
 __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k) {
   const int r = p.rank;
   const A2aGeom g = a2a_geom(p.out_cnt[q], p.bits, p.bucket, (int)sizeof(T));
@@ -175,7 +219,13 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
     uint32_t wire;
     if (!a2a_window_item(g, w, t, it, wire)) continue;
     const SrcSet ss{share + wire, 0u, 1, -1};
-    T* dst = chunk + it.elem_off;
+    T* dst;
+    if constexpr (IDX) {
+      dst = a2a_row_addr(p, reinterpret_cast<T*>(p.out), p.out_index, p.out_rows, p.out_off[q] + it.elem_off, 1u);
+      if (dst == nullptr) continue;
+    } else {
+      dst = chunk + it.elem_off;
+    }
     const uint32_t kind = item_kind(it);
     if (kind == kItemFull) {
       if (group_aligned<T>(dst)) {
@@ -193,7 +243,9 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
   }
 }
 
-template <typename T, int KB, int GPL>
+// IDX: the routed form (A2aParams::in_index / out_index); only the item addresses and the own-chunk
+// copy differ, and the plain instantiations compile as before
+template <typename T, int KB, int GPL, bool IDX = false>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const __grid_constant__ A2aParams p) {
   __shared__ int s_abort;
   __shared__ uint32_t s_send[kMaxPeers], s_recv[kMaxPeers];  // this lane's windows per destination / source
@@ -228,7 +280,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
       const int q = (r + s) % W;
       if (s_send[q] <= k) continue;
       rng.stream = a2a_rng_stream(r, q);
-      a2a_send_window<T, KB, GPL>(p, q, bpw, k, rng);
+      a2a_send_window<T, KB, GPL, IDX>(p, q, bpw, k, rng);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_send)
@@ -239,7 +291,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if (s_abort) break;
     for (int s = 1; s < W; ++s) {
       const int q = (r + W - s) % W;
-      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL>(p, q, bpw, k);
+      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX>(p, q, bpw, k);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_recv)
@@ -247,7 +299,12 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
   }
 
   // my own chunk last: the pushes to the peers are on the critical path, the copy is not
-  if (!s_abort) a2a_copy_own<T>(p);
+  if (!s_abort) {
+    if constexpr (IDX)
+      a2a_copy_own_rows<T>(p);
+    else
+      a2a_copy_own<T>(p);
+  }
 
   // slot handshake, as in rs_kernel: every lane, whether or not it had windows
   if (threadIdx.x < 32 && !s_abort) {
@@ -265,21 +322,28 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 
 }  // namespace dev
 
-template <typename T, int GPL>
+template <typename T, int GPL, bool IDX>
 cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
   const int kb = (p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0;
   switch (kb) {
-    case 2: dev::a2a_kernel<T, 2, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
-    case 4: dev::a2a_kernel<T, 4, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
-    case 8: dev::a2a_kernel<T, 8, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
-    default: dev::a2a_kernel<T, 0, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 2: dev::a2a_kernel<T, 2, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 4: dev::a2a_kernel<T, 4, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 8: dev::a2a_kernel<T, 8, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    default: dev::a2a_kernel<T, 0, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
   }
   return cudaGetLastError();
 }
 
+template <typename T, bool IDX>
+cudaError_t launch_a2a_idx(const A2aParams& p, cudaStream_t stream) {
+  return a2a_slice_elems(p.bits, p.bucket) == 1024u ? launch_a2a_gpl<T, 4, IDX>(p, stream)
+                                                    : launch_a2a_gpl<T, 2, IDX>(p, stream);
+}
+
 template <typename T>
 cudaError_t launch_a2a_t(const A2aParams& p, cudaStream_t stream) {
-  return a2a_slice_elems(p.bits, p.bucket) == 1024u ? launch_a2a_gpl<T, 4>(p, stream) : launch_a2a_gpl<T, 2>(p, stream);
+  return (p.in_index != nullptr || p.out_index != nullptr) ? launch_a2a_idx<T, true>(p, stream)
+                                                           : launch_a2a_idx<T, false>(p, stream);
 }
 
 }  // namespace cgx

@@ -60,7 +60,9 @@ struct SraParams {
 constexpr int kSraThreads = 256;
 constexpr int kSraWarps = kSraThreads / 32;
 constexpr int kSraCtasPerSm = 2;
-enum SraStatus : uint32_t { kSraOk = 0, kSraTimeoutPhase1 = 1, kSraTimeoutPhase2 = 2, kSraAborted = 3 };
+// kSraBadIndex: the routed all-to-all met an index naming a row outside its tensor; the status word
+// then holds (rank << 8) | (0 input_index, 1 output_index) << 16 instead of the peer and the lane
+enum SraStatus : uint32_t { kSraOk = 0, kSraTimeoutPhase1 = 1, kSraTimeoutPhase2 = 2, kSraAborted = 3, kSraBadIndex = 4 };
 
 // max CTAs of the fused kernel that can be co-resident on the current device
 int sra_max_resident_ctas(int dtype);
@@ -97,8 +99,18 @@ struct A2aParams {
   const uint32_t* abort_word;
   uint64_t timeout_ns;
   DeviceSync* sync;
+  // Routed form (launched only when a2a_rows_fit(row, bits, bucket, dtype)): the offsets and counts
+  // above are those of the logical buffers of whole rows of `row` elements; row i of the logical
+  // send buffer is row in_index[i] of `in` (in_rows rows), row j of the logical receive buffer is
+  // row out_index[j] of `out` (out_rows rows). A nullptr index: that side is the logical buffer.
+  const int64_t* in_index;
+  const int64_t* out_index;
+  uint32_t row;
+  uint64_t in_rows;
+  uint64_t out_rows;
 };
-// defined once per dtype in a2a_{f32,f16,bf16}.cu
+// defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
+// p.out_index is set
 cudaError_t launch_a2a_f32(const A2aParams& p, cudaStream_t stream);
 cudaError_t launch_a2a_f16(const A2aParams& p, cudaStream_t stream);
 cudaError_t launch_a2a_bf16(const A2aParams& p, cudaStream_t stream);

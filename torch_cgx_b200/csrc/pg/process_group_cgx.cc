@@ -431,14 +431,16 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
 
 namespace {
 
-// per-rank element counts of one side of an all_to_all_single, from its dim-0 splits
-std::vector<uint64_t> a2a_counts(const at::Tensor& t, const std::vector<int64_t>& splits, int world, int64_t row,
-                                 const char* side) {
-  const int64_t rows = t.dim() > 0 ? t.size(0) : 0;
+// per-rank element counts of one side of an all_to_all_single, from its dim-0 splits; `rows` are
+// the rows of the side's tensor, or the entries of its index when `indexed`
+std::vector<uint64_t> a2a_counts(int64_t rows, const std::vector<int64_t>& splits, int world, int64_t row,
+                                 const char* side, bool indexed) {
+  const std::string what = indexed ? std::string(side) + "_index" : std::string(side);
+  const char* unit = indexed ? " entries" : " rows";
   std::vector<uint64_t> counts((size_t)world);
   if (splits.empty()) {
-    TORCH_CHECK(rows % world == 0, "cgx: all_to_all: the ", side, " has ", rows,
-                " rows, not divisible by the world size ", world, " (give ", side, "_split_sizes)");
+    TORCH_CHECK(rows % world == 0, "cgx: all_to_all: the ", what, " has ", rows, unit,
+                ", not divisible by the world size ", world, " (give ", side, "_split_sizes)");
     for (auto& c : counts) c = (uint64_t)(rows / world * row);
     return counts;
   }
@@ -450,9 +452,18 @@ std::vector<uint64_t> a2a_counts(const at::Tensor& t, const std::vector<int64_t>
     sum += splits[q];
     counts[q] = (uint64_t)(splits[q] * row);
   }
-  TORCH_CHECK(sum == rows, "cgx: all_to_all: ", side, "_split_sizes sums to ", sum, " but the ", side, " has ", rows,
-              " rows");
+  TORCH_CHECK(sum == rows, "cgx: all_to_all: ", side, "_split_sizes sums to ", sum, " but the ", what, " has ", rows,
+              unit);
   return counts;
+}
+
+void check_a2a_index(const at::Tensor& index, const at::Tensor& like, const char* name) {
+  if (!index.defined()) return;
+  TORCH_CHECK(index.is_cuda() && index.device() == like.device(), "cgx: all_to_all: ", name,
+              " must be on the device of the tensors (", like.device(), "), got ", index.device());
+  TORCH_CHECK(index.scalar_type() == at::kLong, "cgx: all_to_all: ", name, " must be int64, got ", index.scalar_type());
+  TORCH_CHECK(index.dim() == 1 && index.is_contiguous(), "cgx: all_to_all: ", name,
+              " must be a contiguous 1-d tensor, got sizes ", index.sizes());
 }
 
 }  // namespace
@@ -460,7 +471,9 @@ std::vector<uint64_t> a2a_counts(const at::Tensor& t, const std::vector<int64_t>
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                                       const std::vector<int64_t>& out_splits,
                                                                       const std::vector<int64_t>& in_splits, int bits,
-                                                                      int bucket_size, bool stochastic, int64_t seed) {
+                                                                      int bucket_size, bool stochastic, int64_t seed,
+                                                                      const at::Tensor& in_index,
+                                                                      const at::Tensor& out_index) {
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
   TORCH_CHECK(in.device() == out.device(), "cgx: all_to_all: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
@@ -478,18 +491,46 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   // every rank evaluates the same condition, so every rank refuses and none is left waiting
   TORCH_CHECK(local_size() >= W, "cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE ",
               local_size(), " < world size ", W, ")");
+  check_a2a_index(in_index, in, "input_index");
+  check_a2a_index(out_index, out, "output_index");
+  const bool ii = in_index.defined(), oi = out_index.defined();
   int64_t row = 1;
   for (int64_t d : in.sizes().slice(1)) row *= d;
-  const std::vector<uint64_t> in_counts = a2a_counts(in, in_splits, W, row, "input");
-  const std::vector<uint64_t> out_counts = a2a_counts(out, out_splits, W, row, "output");
+  const std::vector<uint64_t> in_counts = a2a_counts(ii ? in_index.size(0) : in.size(0), in_splits, W, row, "input", ii);
+  const std::vector<uint64_t> out_counts =
+      a2a_counts(oi ? out_index.size(0) : out.size(0), out_splits, W, row, "output", oi);
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
+  A2aRoute route;
+  route.in_index = ii ? in_index.data_ptr<int64_t>() : nullptr;
+  route.out_index = oi ? out_index.data_ptr<int64_t>() : nullptr;
+  route.row = (uint64_t)row;
+  route.in_rows = (uint64_t)in.size(0);
+  route.out_rows = (uint64_t)out.size(0);
+  const bool routed = ii || oi;
   check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, (uint32_t)bucket_size,
-                   getRank(), W);
+                   getRank(), W, routed ? &route : nullptr);
+  // the one place that decides where the rows are routed: inside the fused kernel when it can
+  // address them, else around a plain call, which computes the same by definition
+  const bool in_kernel = routed && engine_->routes_in_kernel(true, dtype, bits, (uint32_t)bucket_size, (uint64_t)row);
   return enqueue_cuda(c10d::OpType::ALLTOALL_BASE, "cgx:all_to_all", out, &in, [&](cudaStream_t s) {
-    engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits,
+    for (const at::Tensor* t : {&in_index, &out_index})
+      if (t->defined()) c10::cuda::CUDACachingAllocator::recordStream(t->storage().data_ptr(), *comm_stream_);
+    if (!routed || in_kernel) {
+      engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits,
+                          (uint32_t)bucket_size, rng, s, routed ? &route : nullptr);
+      return;
+    }
+    // the temporaries live on the comm stream only
+    c10::cuda::CUDAStreamGuard sg(*comm_stream_);
+    const at::Tensor send = ii ? in.index_select(0, in_index) : in;
+    std::vector<int64_t> recv_shape = out.sizes().vec();
+    recv_shape[0] = oi ? out_index.size(0) : out.size(0);
+    at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;
+    engine_->all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits,
                         (uint32_t)bucket_size, rng, s);
+    if (oi) out.index_copy_(0, out_index, recv);
   });
 }
 

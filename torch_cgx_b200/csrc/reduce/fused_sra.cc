@@ -273,7 +273,7 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
 
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
-                      int world) {
+                      int world, const A2aRoute* route) {
   if ((int)in_counts.size() != world || (int)out_counts.size() != world)
     throw std::invalid_argument("cgx all_to_all: need one input and one output count per rank");
   if (bits < 1 || (bits > 8 && bits < kRawBits))
@@ -288,6 +288,16 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
   }
   if (nin >= (1ull << 32) || nout >= (1ull << 32))
     throw std::invalid_argument("cgx all_to_all: tensors must have fewer than 2^32 elements");
+  if (route != nullptr) {
+    const uint64_t row = route->row;
+    if (row < 1 || row >= (1ull << 32)) throw std::invalid_argument("cgx all_to_all: rows must have 1 to 2^32 - 1 elements");
+    for (int q = 0; q < world; ++q)
+      if (in_counts[q] % row || out_counts[q] % row)
+        throw std::invalid_argument("cgx all_to_all: with an index, every chunk must be whole rows");
+    // the tensors the kernel touches: the indexed ones in full
+    if (route->in_index) nin = route->in_rows * row;
+    if (route->out_index) nout = route->out_rows * row;
+  }
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const uintptr_t a = reinterpret_cast<uintptr_t>(in), b = reinterpret_cast<uintptr_t>(out);
   if (nin > 0 && nout > 0 && a < b + nout * es && b < a + nin * es)
@@ -296,11 +306,16 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
 
 FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                          const std::vector<uint64_t>& out_counts, int dtype, int bits,
-                                         uint32_t bucket, const RngParams& rng, cudaStream_t stream) {
+                                         uint32_t bucket, const RngParams& rng, cudaStream_t stream,
+                                         const A2aRoute* route) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   const int W = world(), r = rank();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W, route);
   const uint64_t es = (uint64_t)dtype_size(dtype);
+  const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
+  if (routed && !a2a_rows_fit((uint32_t)route->row, bits, bucket, (int)es))
+    throw std::invalid_argument("cgx all_to_all: rows of " + std::to_string(route->row) +
+                                " elements do not hold whole quantization items at this bucket size");
   const int G = max_lanes_;
   const uint32_t lane_slot = a2a_lane_slot_bytes(heap_->layout().slot_bytes, G);
   if (a2a_window_blocks(a2a_geom(0, bits, bucket, (int)es), lane_slot) == 0)
@@ -346,6 +361,13 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
   p.abort_word = heap_->abort_device();
   p.timeout_ns = timeout_ns_;
   p.sync = heap_->sync_device();
+  if (routed) {
+    p.in_index = route->in_index;
+    p.out_index = route->out_index;
+    p.row = (uint32_t)route->row;
+    p.in_rows = route->in_rows;
+    p.out_rows = route->out_rows;
+  }
   last_lanes_ = G;
   cudaError_t e = cudaErrorInvalidValue;
   switch (dtype) {
@@ -364,6 +386,10 @@ std::string FusedSra::status_message() const {
   const uint32_t s = heap_->status_host();
   if (s == 0) return std::string();
   const uint32_t code = s & 0xFF, peer = (s >> 8) & 0xFF, lane = s >> 16;
+  if (code == kSraBadIndex)
+    return "cgx: all_to_all on rank " + std::to_string(peer) + ": " + (lane ? "output_index" : "input_index") +
+           " holds a row outside the " + (lane ? "output" : "input") +
+           " (that row was skipped; the group refuses further collectives)";
   if (code == kSraAborted)
     return "cgx: fused allreduce kernel on rank " + std::to_string(rank()) + " was aborted while waiting for rank " +
            std::to_string(peer) + " (lane " + std::to_string(lane) + ")";

@@ -64,13 +64,25 @@ void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_lay
 std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<LayerSpec>& shard_layers,
                                                            const PlanOptions& opt, uint32_t slot_bytes);
 
+// The routed form of one rank's all-to-all: the counts describe logical buffers of whole rows of
+// `row` elements; row i of the logical send buffer is row in_index[i] of `in` (in_rows rows), row j
+// of the logical receive buffer is written to row out_index[j] of `out` (out_rows rows). A nullptr
+// index means that side is the logical buffer itself. The index values live on the device and are
+// checked by the kernel (kSraBadIndex), not here.
+struct A2aRoute {
+  const int64_t* in_index = nullptr;
+  const int64_t* out_index = nullptr;
+  uint64_t row = 1;
+  uint64_t in_rows = 0, out_rows = 0;
+};
+
 // The arguments of one rank's all-to-all (FusedSra::all_to_all, Reducer::all_to_all): a count per
 // rank on both sides, bits 1..8 or >= 32, a bucket >= 1, the own chunk the same size on both sides,
-// tensors below 2^32 elements and an output that does not overlap the input; std::invalid_argument
-// otherwise.
+// tensors below 2^32 elements and an output that does not overlap the input; with a route, counts
+// of whole rows and no overlap of the tensors the indices address; std::invalid_argument otherwise.
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
-                      int world);
+                      int world, const A2aRoute* route = nullptr);
 
 class FusedSra {
  public:
@@ -134,12 +146,15 @@ class FusedSra {
   // `bits` (1..8; >= 32 moves it raw) and buckets of `bucket` counted from the chunk's first
   // element. The counts of a pair must agree on both ends (the caller's contract, as with NCCL).
   // Throws std::invalid_argument on a malformed call before anything is launched.
+  // With a `route` that has an index, the routed kernel gathers the sent rows and scatters the
+  // received ones by index; that needs a2a_rows_fit(route->row, bits, bucket, dtype) (else
+  // std::invalid_argument: the caller composes index_select / index_copy_ around a plain call).
   struct A2aCounts {
     uint64_t launches = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's sends
   };
   A2aCounts all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                        const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                       const RngParams& rng, cudaStream_t stream);
+                       const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

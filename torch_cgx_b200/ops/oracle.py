@@ -645,6 +645,33 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
     return outs
 
 
+def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
+                                input_index: Sequence[torch.Tensor | None],
+                                output_index: Sequence[torch.Tensor | None], row: int, *, bits: int,
+                                bucket_size: int, outputs: Sequence[torch.Tensor] | None = None) -> List[torch.Tensor]:
+    """Every rank's output of the routed all-to-all, as the composition that defines it: rank q sends
+    ``inputs[q].index_select(0, input_index[q])`` (rows of ``row`` elements; ``None``: the input
+    itself), ``all_to_all_reference`` exchanges the rows (``counts[q][r]`` elements, whole rows), and
+    rank r writes what it receives with ``index_copy_(0, output_index[r], ...)`` into a copy of
+    ``outputs[r]`` (``None``: the received rows are the output). Outputs are flat."""
+    W = len(inputs)
+    send = []
+    for q in range(W):
+        x = inputs[q].detach().cpu().reshape(-1, row)
+        ix = input_index[q]
+        send.append((x if ix is None else x.index_select(0, ix.cpu())).reshape(-1))
+    recv = all_to_all_reference(send, counts, bits=bits, bucket_size=bucket_size)
+    outs = []
+    for r in range(W):
+        ix = output_index[r]
+        if ix is None:
+            outs.append(recv[r])
+            continue
+        base = outputs[r].detach().cpu().reshape(-1, row).clone()
+        outs.append(base.index_copy_(0, ix.cpu(), recv[r].reshape(-1, row)).reshape(-1))
+    return outs
+
+
 # ---- the sharded collectives over several nodes (AllreduceEngine::sharded, DESIGN §2.9b) -----------
 SHARDED_PERTURBATIONS = ("prescale_local", "requantized_gather", "quantized_own_partial", "transposed_ranks")
 _CROSS_SEQ = 0x40000000  # the allreduce's cross-node marker

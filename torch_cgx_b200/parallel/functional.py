@@ -166,7 +166,8 @@ def _splits(s: Optional[Sequence[int]]) -> List[int]:
 
 def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
                       input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8, bucket_size: int = 512,
-                      group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None):
+                      group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
+                      input_index: Optional[torch.Tensor] = None, output_index: Optional[torch.Tensor] = None):
     """Compressed ``dist.all_to_all_single`` on a ``cgx`` group.
 
     Splits count dim-0 rows (``None``: equal splits). Rows ``input_split_sizes[q]`` of ``input`` go
@@ -175,6 +176,18 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     (``bits`` 1..8, max-min, buckets of ``bucket_size`` counted from the chunk's first element) and
     decoded by the receiver; ``bits=32`` moves every chunk unchanged. Round to nearest unless
     ``stochastic``; ``seed=None`` uses ``CGX_SEED``.
+
+    Routed form, for MoE token dispatch and combine without a permutation copy: ``input_index``
+    (CUDA int64, ``sum(input_split_sizes)`` entries in ``[0, input.shape[0])``, repeats allowed)
+    makes row i of the sent buffer ``input[input_index[i]]``; ``output_index`` (``sum(output_split_sizes)``
+    entries in ``[0, output.shape[0])``) writes row j of the received buffer to
+    ``output[output_index[j]]`` and leaves the other rows of ``output`` unchanged (duplicates: unspecified,
+    as with ``index_copy_``). The result is bitwise that of ``input.index_select(0, input_index)``,
+    the plain call, then ``output.index_copy_(0, output_index, received)``; on the P2P transport,
+    when every quantization item lies inside one row, the gather and the scatter happen inside the
+    kernel. With an index, ``None`` splits divide the index's entries equally. An index value out of
+    range is not checked on the host: the kernel skips that row and the call fails (``work.wait()``
+    raises, naming the index), after which the group refuses further collectives.
 
     As with NCCL, the splits are the caller's contract: rank q's ``input_split_sizes[r]`` must equal
     rank r's ``output_split_sizes[q]``. Malformed splits on one rank (wrong length, sum or sign, or
@@ -188,50 +201,84 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     if native is None:
         raise RuntimeError("cgx.all_to_all_single needs a process group with the cgx backend")
     work = native.all_to_all_compressed(output, input, _splits(output_split_sizes), _splits(input_split_sizes),
-                                        int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed))
+                                        int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
+                                        input_index, output_index)
     if async_op:
         return work
     work.wait()  # the current stream waits for the kernel; the host does not
     return None
 
 
-def _a2a_output(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]], world: int) -> torch.Tensor:
-    rows = sum(int(v) for v in output_split_sizes) if output_split_sizes is not None else input.shape[0]
+def _a2a_output(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]],
+                input_index: Optional[torch.Tensor]) -> torch.Tensor:
+    if output_split_sizes is not None:
+        rows = sum(int(v) for v in output_split_sizes)
+    else:
+        rows = input_index.shape[0] if input_index is not None else input.shape[0]
     return input.new_empty((rows,) + tuple(input.shape[1:]))
+
+
+def _routes(input_index: Optional[torch.Tensor], output_index: Optional[torch.Tensor]) -> dict:
+    """the index keywords of all_to_all_single that are set"""
+    kw = {"input_index": input_index, "output_index": output_index}
+    return {k: v for k, v in kw.items() if v is not None}
 
 
 class _AllToAll(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, input, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size, group, stochastic):
+    def forward(ctx, input, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size, group, stochastic,
+                input_index, output_index, output_rows):
         ctx.splits = (output_split_sizes, input_split_sizes)
         ctx.grad_bits, ctx.bucket_size, ctx.group, ctx.stochastic = grad_bits, bucket_size, group, stochastic
         ctx.in_shape = input.shape
-        world = dist.get_world_size(group)
+        ctx.index = (input_index, output_index)
         input = input.contiguous()
-        out = _a2a_output(input, output_split_sizes, world)
+        if output_index is None:
+            out = _a2a_output(input, output_split_sizes, input_index)
+        else:
+            out = input.new_zeros((int(output_rows),) + tuple(input.shape[1:]))  # rows nobody names stay zero
         all_to_all_single(out, input, output_split_sizes, input_split_sizes, bits=bits, bucket_size=bucket_size,
-                          group=group, stochastic=stochastic)
+                          group=group, stochastic=stochastic, **_routes(input_index, output_index))
         return out
 
     @staticmethod
     def backward(ctx, grad):
         out_splits, in_splits = ctx.splits
+        input_index, output_index = ctx.index
         grad = grad.contiguous()
-        gin = grad.new_empty(ctx.in_shape)
-        # the gradient travels back: the forward's output splits are its input splits
+        # the gradient travels back: the forward's output splits are its input splits, and the rows
+        # the forward scattered by output_index are gathered by it on the way back
+        if input_index is None:
+            gin = grad.new_empty(ctx.in_shape)
+        else:
+            rows = sum(int(v) for v in in_splits) if in_splits is not None else input_index.shape[0]
+            gin = grad.new_empty((rows,) + tuple(ctx.in_shape[1:]))
         all_to_all_single(gin, grad, in_splits, out_splits, bits=ctx.grad_bits, bucket_size=ctx.bucket_size,
-                          group=ctx.group, stochastic=ctx.stochastic)
-        return gin, None, None, None, None, None, None, None
+                          group=ctx.group, stochastic=ctx.stochastic, **_routes(output_index, None))
+        if input_index is not None:
+            # a row sent to several ranks collects every copy's gradient (index_select's backward)
+            gin = grad.new_zeros(ctx.in_shape).index_add_(0, input_index, gin)
+        return gin, None, None, None, None, None, None, None, None, None, None
 
 
 def differentiable_all_to_all_single(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
                                      input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8,
                                      grad_bits: Optional[int] = None, bucket_size: int = 512, group=None,
-                                     stochastic: bool = False) -> torch.Tensor:
+                                     stochastic: bool = False, input_index: Optional[torch.Tensor] = None,
+                                     output_index: Optional[torch.Tensor] = None,
+                                     output_rows: Optional[int] = None) -> torch.Tensor:
     """``all_to_all_single`` that returns its output and has a backward pass: the compressed
     all-to-all of the gradient with the splits swapped, at ``grad_bits`` (``None``: ``bits``; 32:
-    exact). This is the form an MoE layer calls for its token dispatch and combine."""
+    exact). This is the form an MoE layer calls for its token dispatch and combine.
+
+    ``input_index`` / ``output_index`` route rows as in ``all_to_all_single``. With ``output_index``
+    the result has ``output_rows`` rows, and rows it does not name are zero. The backward gathers
+    the gradient by ``output_index`` inside the exchange and, with ``input_index``, sums what
+    comes back into a zero gradient with ``index_add_``, so a row sent to several ranks receives
+    the sum of its copies' gradients."""
+    if output_index is not None and output_rows is None:
+        raise ValueError("cgx.differentiable_all_to_all_single: output_index needs output_rows")
     gb = int(bits if grad_bits is None else grad_bits)
     return _AllToAll.apply(input, None if output_split_sizes is None else _splits(output_split_sizes),
                            None if input_split_sizes is None else _splits(input_split_sizes), int(bits), gb,
-                           int(bucket_size), group, bool(stochastic))
+                           int(bucket_size), group, bool(stochastic), input_index, output_index, output_rows)
