@@ -1,0 +1,91 @@
+#!/usr/bin/env python
+"""Error of the all-to-all wire codecs, computed on the CPU with the simulator (C.all_to_all_simulate,
+bit for bit what a2a_kernel delivers) from seeded inputs: max-min 8-bit against the FP8 formats
+e4m3 and e5m2, at buckets of 128 and 512 elements.
+
+Inputs, rows of H = 7168 fp32 elements (one MoE hidden state per row):
+  gaussian   N(0, 1)
+  outliers   N(0, 1) with 8 fixed channels scaled by 50 (the outlier channels of an FFN's input);
+             the error is reported on the other channels
+  student_t  Student-t with 3 degrees of freedom (heavy tails everywhere)
+
+Reported per (input, bucket, codec): the relative L2 error ||dec - x|| / ||x|| and the largest
+per-element relative error |dec - x| / |x| over elements with |x| >= 1e-3 * rms(x). This says
+nothing about training accuracy.
+"""
+import argparse
+import json
+import sys
+from pathlib import Path
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+import torch  # noqa: E402
+
+import torch_cgx_b200 as cgx  # noqa: E402
+
+C = cgx._C
+H = 7168
+OUTLIER_CHANNELS = 8
+
+
+def make_rows(kind, rows, seed):
+    g = torch.Generator().manual_seed(seed)
+    mask = torch.zeros(H, dtype=torch.bool)
+    if kind == "student_t":
+        x = _student_t(rows, g)
+    else:
+        x = torch.randn(rows, H, generator=g, dtype=torch.float64)
+    if kind == "outliers":
+        ch = torch.randperm(H, generator=g)[:OUTLIER_CHANNELS]
+        x[:, ch] *= 50.0
+        mask[ch] = True
+    return x.float(), mask
+
+
+def _student_t(rows, g, dof=3.0):
+    """t = z / sqrt(chi2 / dof), chi2 the sum of dof squared normals (seeded, no global state)"""
+    z = torch.randn(rows, H, generator=g, dtype=torch.float64)
+    chi2 = (torch.randn(int(dof), rows, H, generator=g, dtype=torch.float64) ** 2).sum(0)
+    return z / torch.sqrt(chi2 / dof)
+
+
+def decode(x, bits, bucket):
+    """x's rows sent from rank 0 to rank 1 through the codec: what rank 1 receives"""
+    n = x.numel()
+    out = [torch.empty(0), torch.empty(n)]
+    C.all_to_all_simulate([x.reshape(-1), torch.empty(0)], out, [[0, n], [0, 0]], bits=bits, bucket_size=bucket)
+    return out[1].reshape(x.shape)
+
+
+def errors(x, dec, keep):
+    x, dec = x[:, keep].double(), dec[:, keep].double()
+    rel_l2 = float((dec - x).norm() / x.norm())
+    big = x.abs() >= 1e-3 * x.pow(2).mean().sqrt()
+    max_rel = float(((dec - x).abs() / x.abs())[big].max())
+    return rel_l2, max_rel
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--rows", type=int, default=64)
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--buckets", type=int, nargs="+", default=[128, 512])
+    ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
+    args = ap.parse_args()
+    res = []
+    for i, kind in enumerate(("gaussian", "outliers", "student_t")):
+        x, mask = make_rows(kind, args.rows, args.seed + i)
+        for bucket in args.buckets:
+            for bits in (8, "e4m3", "e5m2"):
+                rel_l2, max_rel = errors(x, decode(x, bits, bucket), ~mask)
+                r = {"input": kind, "bucket": bucket, "codec": "maxmin8" if bits == 8 else bits,
+                     "rel_l2_pct": round(100 * rel_l2, 3), "max_rel_pct": round(100 * max_rel, 2)}
+                res.append(r)
+                print(json.dumps(r), flush=True)
+    if args.out:
+        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in res))
+
+
+if __name__ == "__main__":
+    main()

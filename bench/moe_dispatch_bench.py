@@ -116,7 +116,8 @@ def run_config(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bflo
     N = T * k * W  # rows sent by all ranks
     own = sum(send_rows[q][q] for q in range(W))
     elems_wire = (N - own) * H
-    wire = elems_wire * es if bits >= 32 else elems_wire * bits // 8 + (elems_wire // 512) * 8
+    wbits = 8 if isinstance(bits, str) else bits  # the FP8 formats move the bytes of bits 8
+    wire = elems_wire * es if wbits >= 32 else elems_wire * wbits // 8 + (elems_wire // 512) * 8
     kernel_bytes = 2 * N * H * es + 2 * wire
     perm_bytes = 2 * N * H * es
     res = {"W": W, "T": T, "H": H, "topk": k, "bits": bits, "dtype": str(dtype).replace("torch.", "")}
@@ -135,7 +136,8 @@ def main():
     ap.add_argument("--hidden", type=int, nargs="+", default=[4096, 7168])
     ap.add_argument("--tokens", type=int, nargs="+", default=[4096, 16384])
     ap.add_argument("--topk", type=int, nargs="+", default=[2, 8])
-    ap.add_argument("--bits", type=int, nargs="+", default=[4, 8, 32])
+    ap.add_argument("--bits", type=lambda b: b if b in ("e4m3", "e5m2") else int(b), nargs="+", default=[4, 8, 32],
+                    help="widths 1..8 or 32, or the FP8 wire formats e4m3 / e5m2")
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     # 16 lanes x 8 ranks = 128 CTAs: the virtual ranks together occupy the GPU, as one real rank would its own

@@ -12,7 +12,9 @@ Reports the slope between two sizes (harness overhead cancels).
 rank in W chunks, with equal splits and with skewed ones (chunk q -> r gets a share proportional to
 1 + (r - q) mod W, so every rank still sends and receives `mb` MB but pairs differ up to W : 1),
 next to the reduce-scatter (rs_kernel) of the same `mb` MB input per rank, same dtype, bits and
-bucket. Both move the same packed bytes; the reduce-scatter also accumulates."""
+bucket. Both move the same packed bytes; the reduce-scatter also accumulates. Its --bits may name
+the FP8 wire formats, e4m3 and e5m2, which move the bytes of bits 8 (the reduce-scatter row next to
+them runs at bits 8)."""
 import argparse
 import json
 import sys
@@ -138,11 +140,16 @@ def skewed_counts(W, n):
     return [[base[(r - q) % W] for r in range(W)] for q in range(W)]
 
 
+def a2a_bits(b):
+    """an all-to-all --bits entry: an integer width, or an FP8 format name"""
+    return b if b in ("e4m3", "e5m2") else int(b)
+
+
 def all_to_all_rows(args, dev, W, lanes):
     rows = []
     for dtype in [getattr(torch, d) for d in args.dtypes.split(",")]:
         es = torch.empty((), dtype=dtype).element_size()
-        for bits in [int(b) for b in args.bits.split(",")]:
+        for bits in [a2a_bits(b) for b in args.bits.split(",")]:
             for mb in [int(x) for x in args.mbs.split(",")]:
                 n = (mb << 20) // es // W * W
                 slot = n * es // W * 2 + (1 << 20)
@@ -158,7 +165,7 @@ def all_to_all_rows(args, dev, W, lanes):
                     row[f"a2a_{kind}_us"] = round(timeit(lambda: g.all_to_all(xs, outs, c, bits=bits,
                                                                               bucket_size=args.bucket)), 1)
                     del outs
-                shard = [(0, n // W, bits, args.bucket)]
+                shard = [(0, n // W, 8 if isinstance(bits, str) else bits, args.bucket)]
                 routs = [torch.empty(n // W, device=dev, dtype=dtype) for _ in range(W)]
                 g.reduce_scatter(xs, routs, shard)
                 torch.cuda.synchronize()

@@ -20,6 +20,10 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 # and interleaved all-gather / reduce-scatter / allreduce / one-shot calls on one heap
 AG_SUBSET='(edge_inputs and (w2-float32-q1- or w3-float16-q2- or w5-bfloat16-q3-)) or many_windows or interleaved'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_all_gather_gpu.py -m gpu -x -q -k "$AG_SUBSET"
+# all-to-all FP8 wire formats: edge inputs on unaligned views (full slices and bucket items), small slots with many
+# windows, the routed form, FP8 / max-min / raw calls on one heap, and the generic reducer's FP8 item kernels
+FP8_SUBSET='edge_inputs or small_slots or (routed and float32) or interleaved or (generic_path and float16)'
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_a2a_fp8_gpu.py -m gpu -x -q -k "$FP8_SUBSET"
 # generic reducers on one GPU (quantize / accumulate / quantize_f32 / dequantize item kernels): SRA, Ring,
 # all-to-all and the compressed broadcast at W = 3 on unaligned views, and the 1024-element slice path
 RED_SUBSET='(match_host_and_reference and w3-float32-) or (width_and_slice_variants and 4-1024)'

@@ -24,6 +24,7 @@
 #include <optional>
 #include <thread>
 #include <tuple>
+#include <variant>
 #include <vector>
 
 #include "comm/fd_channel.h"
@@ -269,9 +270,35 @@ void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<
   }
 }
 
+// The `bits` of every all-to-all binding: 1..8 or 32 (max-min levels, or raw), or the name of an FP8
+// wire codec, which travels in 8-bit records and rounds to nearest only. Integers are checked where
+// they are used, as before; an unknown name, or an FP8 codec with stochastic rounding, raises
+// ValueError before anything runs.
+using A2aBitsArg = std::variant<int64_t, std::string>;
+struct A2aBits {
+  int bits;
+  WireCodec codec;
+};
+A2aBits a2a_bits(const A2aBitsArg& arg, bool stochastic) {
+  const std::string* name = std::get_if<std::string>(&arg);
+  if (name == nullptr) return {(int)std::get<int64_t>(arg), kMaxMin};
+  WireCodec codec;
+  if (*name == "e4m3")
+    codec = kE4M3;
+  else if (*name == "e5m2")
+    codec = kE5M2;
+  else
+    throw py::value_error("cgx all_to_all: bits must be 1..8, 32, \"e4m3\" or \"e5m2\", got \"" + *name + "\"");
+  if (stochastic)
+    throw py::value_error("cgx all_to_all: bits=\"" + *name +
+                          "\" rounds to nearest only; stochastic rounding needs integer bits");
+  return {8, codec};
+}
+
 void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
-                            const CountMatrix& counts_in, int bits, int64_t bucket, bool stochastic, uint64_t seed,
-                            uint32_t seq) {
+                            const CountMatrix& counts_in, const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic,
+                            uint64_t seed, uint32_t seq) {
+  const A2aBits wb = a2a_bits(bits_arg, stochastic);
   const auto counts = check_counts(counts_in, inputs.size());
   check_a2a_tensors(inputs, outputs, counts, false);
   std::vector<const void*> in;
@@ -280,7 +307,8 @@ void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
     in.push_back(inputs[r].data_ptr());
     out.push_back(outputs[r].data_ptr());
   }
-  all_to_all_simulate(cgx_dtype(inputs[0]), in, out, counts, bits, (uint32_t)bucket, make_rng(stochastic, seed, seq));
+  all_to_all_simulate(cgx_dtype(inputs[0]), in, out, counts, wb.bits, wb.codec, (uint32_t)bucket,
+                      make_rng(stochastic, seed, seq));
 }
 
 // the items of one chunk from common/a2a.h, rows as in plan_to_dict, offsets in the contiguous image
@@ -539,8 +567,9 @@ class LocalSraGroup {
   // output_index[r], when given and not None, are rank r's int64 row indices into inputs[r] /
   // outputs[r], rows of `row` elements; the counts then describe the logical buffers of whole rows.
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
-                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq, const IndexList& input_index,
-                  const IndexList& output_index, int64_t row) {
+                  const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
+                  const IndexList& input_index, const IndexList& output_index, int64_t row) {
+    const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)world_);
     const bool routed = !input_index.empty() || !output_index.empty();
     TORCH_CHECK(input_index.empty() || (int)input_index.size() == world_, "all_to_all: one input_index per rank");
@@ -589,8 +618,8 @@ class LocalSraGroup {
               [&](int r) {
                 std::vector<uint64_t> out_counts(world_);
                 for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
-                fused_[r]->all_to_all(inputs[r].data_ptr(), outputs[r].data_ptr(), counts[r], out_counts, dt, bits,
-                                      (uint32_t)bucket, rng, streams_[r].stream(), routed ? &routes[r] : nullptr);
+                fused_[r]->all_to_all(inputs[r].data_ptr(), outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits,
+                                      wb.codec, (uint32_t)bucket, rng, streams_[r].stream(), routed ? &routes[r] : nullptr);
               });
   }
   void check() {
@@ -731,14 +760,16 @@ class LocalReducerGroup {
   }
   // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
-                  int bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+                  const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+    const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)hub_.world());
     check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda());
     const RngParams rng = make_rng(stochastic, seed, seq);
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
       std::vector<uint64_t> out_counts(counts.size());
       for (size_t q = 0; q < counts.size(); ++q) out_counts[q] = counts[q][r];
-      red.all_to_all(in, outputs[r].data_ptr(), counts[r], out_counts, dt, bits, (uint32_t)bucket, rng, s);
+      red.all_to_all(in, outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits, wb.codec, (uint32_t)bucket, rng,
+                     s);
     }, false);
   }
   // bytes each rank's reducer counted as sent during the last call
@@ -1435,9 +1466,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("layers") = std::vector<LayerTuple>{}, py::call_guard<py::gil_scoped_release>())
       .def("all_to_all_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
-              const std::vector<int64_t>& in_splits, int bits, int bucket_size, bool stochastic, int64_t seed,
-              const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index) {
-             return pg.all_to_all_compressed(out, in, out_splits, in_splits, bits, bucket_size, stochastic, seed,
+              const std::vector<int64_t>& in_splits, const A2aBitsArg& bits, int bucket_size, bool stochastic,
+              int64_t seed, const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index) {
+             const A2aBits wb = a2a_bits(bits, stochastic);
+             return pg.all_to_all_compressed(out, in, out_splits, in_splits, wb.bits, wb.codec, bucket_size,
+                                             stochastic, seed,
                                              in_index.value_or(at::Tensor()), out_index.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
@@ -1618,6 +1651,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("all_to_all_simulate", &py_all_to_all_simulate, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
         py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
         py::arg("seq") = 0);
+  m.def(
+      "a2a_bits",
+      [](const A2aBitsArg& bits, bool stochastic) {
+        const A2aBits wb = a2a_bits(bits, stochastic);
+        return std::make_tuple(wb.bits, (int)wb.codec);
+      },
+      py::arg("bits"), py::arg("stochastic") = false);
   m.def("a2a_items", &py_a2a_items, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
   m.def(
       "a2a_rows_fit",

@@ -191,6 +191,53 @@ inline void decode_block_foreach(const uint8_t* rec, int dtype, const BlockDesc&
   }
 }
 
+// FP8 codecs (quant_math.h) of an 8-bit block: the record layout of quantize_block at bits 8,
+// meta {unit, +0} per bucket and element i's code at byte i of its bucket's payload
+inline void quantize_block_fp8(const float* acc, const BlockDesc& d, uint8_t* rec, int codec) {
+  const uint32_t n = block_n(d);
+  const uint32_t B = d.bucket;
+  const uint32_t nb = block_num_buckets(n, B);
+  const uint32_t gpb = bucket_groups(B);
+  BucketMeta* meta = reinterpret_cast<BucketMeta*>(rec);
+  uint8_t* pay = rec + block_meta_bytes(n, B);
+  for (uint32_t b = 0; b < nb; ++b) {
+    const uint32_t lo = b * B, hi = lo + B < n ? lo + B : n;
+    float mn = acc[lo], mx = acc[lo];
+    for (uint32_t i = lo + 1; i < hi; ++i) {
+      mn = nan_min(mn, acc[i]);
+      mx = nan_max(mx, acc[i]);
+    }
+    meta[b] = fp8_meta(mn, mx, codec);
+    const float inv = fp8_inv_unit(meta[b].unit);
+    uint8_t* dst = pay + (size_t)b * gpb * 8u;
+    for (uint32_t i = lo; i < lo + div_up(hi - lo, 8u) * 8u; ++i)
+      dst[i - lo] = i < hi ? (uint8_t)fp8_encode(acc[i], inv, codec) : 0u;
+  }
+  {
+    uint32_t used = nb * 8u, tot = block_meta_bytes(n, B);
+    std::memset(rec + used, 0, tot - used);
+  }
+  {
+    uint32_t used = block_num_groups(n, B) * 8u, tot = block_payload_bytes(n, 8, B);
+    std::memset(pay + used, 0, tot - used);
+  }
+}
+
+inline void decode_block_fp8_store(const uint8_t* rec, int dtype, const BlockDesc& d, void* dst, int codec) {
+  const uint32_t n = block_n(d);
+  const uint32_t B = d.bucket;
+  const uint32_t nb = block_num_buckets(n, B);
+  const uint32_t gpb = bucket_groups(B);
+  const BucketMeta* meta = reinterpret_cast<const BucketMeta*>(rec);
+  const uint8_t* pay = rec + block_meta_bytes(n, B);
+  for (uint32_t b = 0; b < nb; ++b) {
+    const uint32_t lo = b * B, hi = lo + B < n ? lo + B : n;
+    const uint8_t* src = pay + (size_t)b * gpb * 8u;
+    for (uint32_t i = lo; i < hi; ++i)
+      store_elem(dst, dtype, (uint64_t)d.elem_off + i, fp8_decode(src[i - lo], meta[b].unit, codec));
+  }
+}
+
 inline void decode_block_add(const uint8_t* rec, int dtype, const BlockDesc& d, float* acc) {
   decode_block_foreach(rec, dtype, d, [&](uint32_t i, float v) { acc[i] += v; });
 }

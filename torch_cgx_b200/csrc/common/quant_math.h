@@ -145,4 +145,128 @@ CGX_HD uint32_t unpack1(uint64_t w, int j, int bits) {
   return (uint32_t)(w >> (j * bits)) & ((1u << bits) - 1u);
 }
 
+// ---- FP8 wire codec (compressed all-to-all only) ---------------------------------------------
+// What the bytes of an 8-bit record mean. kMaxMin: levels of [min, max] (above). kE4M3 / kE5M2:
+// one fp32 scale per bucket, unit = max|x| * fp32(1 / FMAX), and one FP8 code per element,
+// code = cvt.rn.satfinite(x * (1 / unit)), decoded as float(code) * unit. The record keeps the
+// 8-bit layout: meta {unit, +0.0f} where max-min stores {unit, min}, then one byte per element.
+// A NaN or an Inf in a bucket makes unit NaN or Inf and every element decodes to NaN (0 * Inf is
+// NaN); a bucket whose unit is below 2^-126 has 1 / unit = 0 and decodes to signed zeros.
+enum WireCodec : int { kMaxMin = 0, kE4M3 = 1, kE5M2 = 2 };
+
+constexpr float kFp8MinUnit = 1.17549435e-38f;  // 2^-126: a smaller unit decodes its bucket to zeros
+constexpr uint32_t kFp8NaNCode = 0x7Fu;         // the code cvt.rn.satfinite writes for any NaN
+
+// largest finite value of the format, and its reciprocal correctly rounded to fp32 (a literal per
+// format, as rcp_levels)
+CGX_HD float fp8_max(int codec) { return codec == kE5M2 ? 57344.0f : 448.0f; }
+CGX_HD float fp8_rcp_max(int codec) { return codec == kE5M2 ? 1.0f / 57344.0f : 1.0f / 448.0f; }
+
+// steps 1-2: unit = nan_max(-min, max) * fp32(1 / FMAX), one rounding; the meta's second word is +0
+CGX_HD BucketMeta fp8_meta(float mn, float mx, int codec) {
+  BucketMeta m;
+  const float a = nan_max(-mn, mx);
+#if defined(__CUDA_ARCH__)
+  m.unit = __fmul_rn(a, fp8_rcp_max(codec));
+#else
+  m.unit = a * fp8_rcp_max(codec);
+  if (m.unit != m.unit) m.unit = canonical_nan();
+#endif
+  m.min = 0.f;
+  return m;
+}
+
+// step 3: 1 / unit, or 0 below 2^-126 (NaN stays NaN: NaN < x is false)
+CGX_HD float fp8_inv_unit(float unit) {
+#if defined(__CUDA_ARCH__)
+  return unit < kFp8MinUnit ? 0.f : __frcp_rn(unit);
+#else
+  return unit < kFp8MinUnit ? 0.f : 1.0f / unit;
+#endif
+}
+
+// Software cvt.rn.satfinite.{e4m3,e5m2}.f32 of one value: round to nearest even on the format's grid
+// (subnormals included), anything beyond the largest finite value -- infinities too -- saturates to
+// it, and a NaN of any sign or payload becomes kFp8NaNCode.
+inline uint32_t fp8_from_float_host(float v, int codec) {
+  const int mb = codec == kE5M2 ? 2 : 3, bias = codec == kE5M2 ? 15 : 7;
+  const uint32_t maxcode = codec == kE5M2 ? 0x7Bu : 0x7Eu;
+  uint32_t u;
+  std::memcpy(&u, &v, 4);
+  const uint32_t sign = (u >> 24) & 0x80u, ax = u & 0x7FFFFFFFu;
+  if (ax > 0x7F800000u) return kFp8NaNCode;
+  const int e = (int)(ax >> 23) - 127;
+  if (e == -127) return sign;  // zero or an fp32 subnormal: far below half the smallest FP8 subnormal
+  const uint32_t man = (ax & 0x7FFFFFu) | 0x800000u;
+  const int emin = 1 - bias;
+  const int shift = 23 - mb + (e < emin ? emin - e : 0);
+  if (shift > 24) return sign;  // below half the smallest subnormal
+  uint32_t q = man >> shift;
+  const uint32_t rem = man & ((1u << shift) - 1u), half = 1u << (shift - 1);
+  if (rem > half || (rem == half && (q & 1u))) ++q;
+  // a subnormal that rounds up to 2^mb, or a mantissa that rounds over, carries into the exponent
+  uint32_t code = e < emin ? q : ((uint32_t)(e + bias) << mb) + q - (1u << mb);
+  if (code > maxcode) code = maxcode;
+  return sign | code;
+}
+
+// exact value of an FP8 code
+inline float fp8_to_float_host(uint32_t code, int codec) {
+  const int mb = codec == kE5M2 ? 2 : 3, bias = codec == kE5M2 ? 15 : 7;
+  const uint32_t mag = code & 0x7Fu, ef = mag >> mb, mf = mag & ((1u << mb) - 1u);
+  float v;
+  if (codec == kE5M2 ? ef == 0x1Fu : mag == 0x7Fu)
+    v = (codec == kE5M2 && mf == 0) ? INFINITY : canonical_nan();
+  else if (ef == 0)
+    v = std::ldexp((float)mf, 1 - bias - mb);
+  else
+    v = std::ldexp((float)(mf | (1u << mb)), (int)ef - bias - mb);
+  return (code & 0x80u) ? -v : v;
+}
+
+// steps 4-5 for two elements, the unit the device converts: the code of x0 in bits 0..7, of x1 in
+// bits 8..15 (the order of the 8-bit record). cvt's first source goes to the upper byte.
+CGX_HD uint32_t fp8x2_encode(float x0, float x1, float inv, int codec) {
+#if defined(__CUDA_ARCH__)
+  const float a = __fmul_rn(x0, inv), b = __fmul_rn(x1, inv);
+  unsigned short h;
+  if (codec == kE5M2)
+    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
+  else
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
+  return h;
+#else
+  return fp8_from_float_host(x0 * inv, codec) | (fp8_from_float_host(x1 * inv, codec) << 8);
+#endif
+}
+CGX_HD void fp8x2_decode(uint32_t pair, float unit, int codec, float& d0, float& d1) {
+#if defined(__CUDA_ARCH__)
+  const unsigned short in = (unsigned short)pair;
+  uint32_t h2;
+  if (codec == kE5M2)
+    asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(h2) : "h"(in));
+  else
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(in));
+  float f0, f1;
+  asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\tcvt.f32.f16 %0, lo;\n\tcvt.f32.f16 %1, hi;\n\t}"
+      : "=f"(f0), "=f"(f1)
+      : "r"(h2));
+  d0 = __fmul_rn(f0, unit);
+  d1 = __fmul_rn(f1, unit);
+#else
+  d0 = fp8_to_float_host(pair & 0xFFu, codec) * unit;
+  d1 = fp8_to_float_host((pair >> 8) & 0xFFu, codec) * unit;
+  if (d0 != d0) d0 = canonical_nan();
+  if (d1 != d1) d1 = canonical_nan();
+#endif
+}
+
+// one element (the host codec and the generic paths)
+CGX_HD uint32_t fp8_encode(float x, float inv, int codec) { return fp8x2_encode(x, 0.f, inv, codec) & 0xFFu; }
+CGX_HD float fp8_decode(uint32_t code, float unit, int codec) {
+  float d0, d1;
+  fp8x2_decode(code & 0xFFu, unit, codec, d0, d1);
+  return d0;
+}
+
 }  // namespace cgx

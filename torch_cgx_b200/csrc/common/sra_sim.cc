@@ -74,8 +74,8 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
 }
 
 void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, const std::vector<void*>& out_bufs,
-                         const std::vector<std::vector<uint64_t>>& counts, int bits, uint32_t bucket,
-                         const RngParams& rng) {
+                         const std::vector<std::vector<uint64_t>>& counts, int bits, WireCodec codec,
+                         uint32_t bucket, const RngParams& rng) {
   const int W = (int)in_bufs.size();
   if ((int)out_bufs.size() != W || (int)counts.size() != W)
     throw std::invalid_argument("all_to_all_simulate: need one input, output and count row per rank");
@@ -109,6 +109,11 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
         d.n_bits = (a2a_block_n(g, b) & 0xFFFFFFu) | ((uint32_t)g.bits << 24);
         d.bucket = g.bucket;
         cpu::load_block(src, dtype, d, 1.0f, acc.data());
+        if (codec != kMaxMin) {
+          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+          cpu::decode_block_fp8_store(rec.data(), dtype, d, dst, codec);
+          continue;
+        }
         cpu::quantize_block(acc.data(), dtype, d, rec.data(), key, b);
         cpu::decode_block_store(rec.data(), dtype, d, dst);
       }

@@ -9,6 +9,7 @@
 #include <vector>
 #include "philox.h"
 #include "plan.h"
+#include "quant_math.h"
 
 namespace cgx {
 
@@ -47,10 +48,11 @@ void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& i
 // lie in in_bufs[q] in destination order, rank r's output holds the chunks in source order. The own
 // chunk is copied, and so is every chunk when bits >= kRawBits (raw). Every other chunk is decode(Q(x))
 // with buckets counted from the chunk's first element (common/a2a.h) and the pair's random stream
-// a2a_rng_stream(q, r).
+// a2a_rng_stream(q, r). With an FP8 codec (bits 8) the chunks use its records instead of max-min's
+// and round to nearest.
 void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, const std::vector<void*>& out_bufs,
-                         const std::vector<std::vector<uint64_t>>& counts, int bits, uint32_t bucket,
-                         const RngParams& rng);
+                         const std::vector<std::vector<uint64_t>>& counts, int bits, WireCodec codec,
+                         uint32_t bucket, const RngParams& rng);
 
 // Quantize->dequantize round trip of one rank's buffer through the plan's
 // blocks (what a single compression step does to the data); used by the Python

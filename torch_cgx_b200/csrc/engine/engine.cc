@@ -321,15 +321,16 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
 }
 
 void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
-                                 const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                                 const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route) {
+                                 const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
+                                 uint32_t bucket, const RngParams& rng_in, cudaStream_t stream,
+                                 const A2aRoute* route) {
   if (nodes() > 1)
     throw std::runtime_error("cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE " +
                              std::to_string(local_size_) + " < world size " + std::to_string(world_) + ")");
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rank_, world_, route);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
   if (routed && !routes_in_kernel(cuda, dtype, bits, bucket, route->row))
     throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
@@ -344,7 +345,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
   stats_.elements += total;
   if (fused) {
     const FusedSra::A2aCounts n =
-        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream, route);
+        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, route);
     stats_.kernel_launches += n.launches;
     stats_.wire_bytes += n.wire_bytes;
     stats_.raw_bytes += n.raw_bytes;
@@ -360,7 +361,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
     return;
   }
   const uint64_t before = g.intra->bytes_sent();
-  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, rng, stream);
+  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream);
   stats_.wire_bytes += g.intra->bytes_sent() - before;
   for (int q = 0; q < world_; ++q)
     if (q != rank_) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);

@@ -161,7 +161,7 @@ class AllreduceEngine {
   // A `route` with an index needs routes_in_kernel(); callers compose index_select / index_copy_
   // around a plain call otherwise.
   void all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
-                  const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
+                  const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
                   const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route = nullptr);
   // whether a routed all-to-all of rows of `row` elements runs inside the fused kernel: the P2P
   // transport with a heap, and rows that hold whole quantization items (a2a_rows_fit)

@@ -168,7 +168,37 @@ __device__ __forceinline__ bool a2a_window_item(const A2aGeom& g, const A2aWindo
   return true;
 }
 
-template <typename T, int KB, int GPL, bool IDX>
+// one item of a chunk for a peer in an FP8 codec (KB 8 records, round to nearest)
+template <typename T, int CODEC, int GPL>
+__device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& it, const OneDst& push) {
+  if (item_kind(it) == kItemFull) {
+    if (group_aligned<T>(src)) {
+      float x[GPL][8];
+      slice_load_vec<T, GPL>(src, x);
+      full_send_fp8_x<CODEC, GPL>(x, it, push);
+    } else {
+      full_send_fp8_unaligned<T, CODEC, GPL>(src, it, push);
+    }
+  } else {
+    bucket_quantize_fp8<T, CODEC>(src, it, push);
+  }
+}
+template <typename T, int CODEC, int GPL>
+__device__ __forceinline__ void a2a_recv_item_fp8(const uint8_t* rec, const WarpItem& it, T* dst) {
+  if (item_kind(it) == kItemFull) {
+    if (group_aligned<T>(dst)) {
+      SliceWords<GPL> sw;
+      slice_fetch<8, GPL>(rec, it.meta_off, it.pay_off, item_lpb_log2(it), 8, sw);
+      full_recv_fp8_w<T, CODEC, GPL, true>(sw, dst);
+    } else {
+      full_recv_fp8_unaligned<T, CODEC, GPL>(rec, it, dst);
+    }
+  } else {
+    bucket_recv_fp8<T, CODEC>(rec, it, dst);
+  }
+}
+
+template <typename T, int KB, int GPL, bool IDX, int CODEC>
 __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k,
                                                 const RngKey& rng) {
   const int r = p.rank;
@@ -190,6 +220,10 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
     } else {
       src = chunk + it.elem_off;
     }
+    if constexpr (CODEC != kMaxMin) {
+      a2a_send_item_fp8<T, CODEC, GPL>(src, it, push);
+      continue;
+    }
     const uint32_t kind = item_kind(it);
     if (kind == kItemFull) {
       if (group_aligned<T>(src)) {
@@ -207,7 +241,7 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
   }
 }
 
-template <typename T, int KB, int GPL, bool IDX>
+template <typename T, int KB, int GPL, bool IDX, int CODEC>
 __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k) {
   const int r = p.rank;
   const A2aGeom g = a2a_geom(p.out_cnt[q], p.bits, p.bucket, (int)sizeof(T));
@@ -225,6 +259,10 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
       if (dst == nullptr) continue;
     } else {
       dst = chunk + it.elem_off;
+    }
+    if constexpr (CODEC != kMaxMin) {
+      a2a_recv_item_fp8<T, CODEC, GPL>(ss.base, it, dst);
+      continue;
     }
     const uint32_t kind = item_kind(it);
     if (kind == kItemFull) {
@@ -244,9 +282,11 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
 }
 
 // IDX: the routed form (A2aParams::in_index / out_index); only the item addresses and the own-chunk
-// copy differ, and the plain instantiations compile as before
-template <typename T, int KB, int GPL, bool IDX = false>
+// copy differ, and the plain instantiations compile as before.
+// CODEC: the wire codec of the peers' chunks (quant_math.h); the FP8 ones exist with KB 8 only.
+template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const __grid_constant__ A2aParams p) {
+  static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   __shared__ int s_abort;
   __shared__ uint32_t s_send[kMaxPeers], s_recv[kMaxPeers];  // this lane's windows per destination / source
   const int lane = blockIdx.x, r = p.rank, W = p.world;
@@ -280,7 +320,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
       const int q = (r + s) % W;
       if (s_send[q] <= k) continue;
       rng.stream = a2a_rng_stream(r, q);
-      a2a_send_window<T, KB, GPL, IDX>(p, q, bpw, k, rng);
+      a2a_send_window<T, KB, GPL, IDX, CODEC>(p, q, bpw, k, rng);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_send)
@@ -291,7 +331,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if (s_abort) break;
     for (int s = 1; s < W; ++s) {
       const int q = (r + W - s) % W;
-      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX>(p, q, bpw, k);
+      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX, CODEC>(p, q, bpw, k);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_recv)
@@ -324,6 +364,16 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 
 template <typename T, int GPL, bool IDX>
 cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
+  if (p.codec != kMaxMin) {
+    if (p.bits != 8) return cudaErrorInvalidValue;
+    if (p.codec == kE4M3)
+      dev::a2a_kernel<T, 8, GPL, IDX, kE4M3><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    else if (p.codec == kE5M2)
+      dev::a2a_kernel<T, 8, GPL, IDX, kE5M2><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    else
+      return cudaErrorInvalidValue;
+    return cudaGetLastError();
+  }
   const int kb = (p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0;
   switch (kb) {
     case 2: dev::a2a_kernel<T, 2, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;

@@ -162,6 +162,49 @@ accumulate_items_kernel(const uint8_t* __restrict__ wire, const WarpItem* __rest
   }
 }
 
+// The FP8 codecs of an 8-bit plan (the generic all-to-all): wire = quantize(src), dst = decode(wire).
+// Plain T tensors, no prescale, round to nearest; the plan has no raw items.
+template <typename T, int CODEC, int GPL>
+__global__ void __launch_bounds__(kThreads, 3)
+quantize_items_fp8_kernel(const T* __restrict__ src, const WarpItem* __restrict__ items, uint32_t first,
+                          uint32_t count, uint8_t* wire) {
+  const OneDst ds{wire};
+  CGX_ITEM_LOOP(it) {
+    const T* s = src + it.elem_off;
+    if (item_kind(it) == kItemFull) {
+      if (group_aligned<T>(s)) {
+        float x[GPL][8];
+        slice_load_vec<T, GPL>(s, x);
+        full_send_fp8_x<CODEC, GPL>(x, it, ds);
+      } else {
+        full_send_fp8_unaligned<T, CODEC, GPL>(s, it, ds);
+      }
+    } else {
+      bucket_quantize_fp8<T, CODEC>(s, it, ds);
+    }
+  }
+}
+
+template <typename T, int CODEC, int GPL>
+__global__ void __launch_bounds__(kThreads, 3)
+dequantize_items_fp8_kernel(const uint8_t* __restrict__ wire, const WarpItem* __restrict__ items, uint32_t first,
+                            uint32_t count, T* __restrict__ dst) {
+  CGX_ITEM_LOOP(it) {
+    T* o = dst + it.elem_off;
+    if (item_kind(it) == kItemFull) {
+      if (group_aligned<T>(o)) {
+        SliceWords<GPL> w;
+        slice_fetch<8, GPL>(wire, it.meta_off, it.pay_off, item_lpb_log2(it), 8, w);
+        full_recv_fp8_w<T, CODEC, GPL, true>(w, o);
+      } else {
+        full_recv_fp8_unaligned<T, CODEC, GPL>(wire, it, o);
+      }
+    } else {
+      bucket_recv_fp8<T, CODEC>(wire, it, o);
+    }
+  }
+}
+
 template <typename T>
 __global__ void scale_kernel(T* __restrict__ data, uint64_t n, float scale) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -237,6 +280,42 @@ cudaError_t dequantize_t(const ItemKernelArgs& a, const uint8_t* wire, T* dst, c
   return cudaGetLastError();
 }
 
+// CODEC x GPL dispatch of the FP8 kernels (8-bit plans only)
+#define CGX_DISPATCH_FP8(a, CALL)                                  \
+  do {                                                             \
+    if ((a).uniform_bits != 8) return cudaErrorInvalidValue;       \
+    const bool g4_ = (a).slice_elems == 1024;                      \
+    if ((a).codec == kE4M3) {                                      \
+      if (g4_) { CALL(kE4M3, 4); } else { CALL(kE4M3, 2); }       \
+    } else if ((a).codec == kE5M2) {                               \
+      if (g4_) { CALL(kE5M2, 4); } else { CALL(kE5M2, 2); }       \
+    } else {                                                       \
+      return cudaErrorInvalidValue;                                \
+    }                                                              \
+  } while (0)
+
+template <typename T>
+cudaError_t quantize_fp8_t(const ItemKernelArgs& a, const T* src, uint8_t* wire, cudaStream_t stream) {
+  if (a.count == 0) return cudaSuccess;
+  const int grid = grid_for(a.count);
+#define CGX_CALL(C_, GPL_) \
+  quantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(src, a.items, a.first, a.count, wire)
+  CGX_DISPATCH_FP8(a, CGX_CALL);
+#undef CGX_CALL
+  return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t dequantize_fp8_t(const ItemKernelArgs& a, const uint8_t* wire, T* dst, cudaStream_t stream) {
+  if (a.count == 0) return cudaSuccess;
+  const int grid = grid_for(a.count);
+#define CGX_CALL(C_, GPL_) \
+  dequantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(wire, a.items, a.first, a.count, dst)
+  CGX_DISPATCH_FP8(a, CGX_CALL);
+#undef CGX_CALL
+  return cudaGetLastError();
+}
+
 template <typename T>
 cudaError_t accumulate_t(const ItemKernelArgs& a, const uint8_t* wire, float* acc, uint32_t base_elem,
                          const T* init_src, float prescale, cudaStream_t stream) {
@@ -262,6 +341,12 @@ cudaError_t accumulate_t(const ItemKernelArgs& a, const uint8_t* wire, float* ac
 
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,
                                   const RngKey& rng, cudaStream_t stream) {
+  if (a.codec != kMaxMin) {
+    if (prescale != 1.0f || rng.enabled) return cudaErrorInvalidValue;
+    CGX_BY_DTYPE(a.dtype, (quantize_fp8_t<float>(a, (const float*)src, wire, stream)),
+                 (quantize_fp8_t<__half>(a, (const __half*)src, wire, stream)),
+                 (quantize_fp8_t<__nv_bfloat16>(a, (const __nv_bfloat16*)src, wire, stream)))
+  }
   CGX_BY_DTYPE(a.dtype,
                (quantize_t<float, float>(a, (const float*)src, 0, wire, prescale, rng, nullptr, stream)),
                (quantize_t<__half, __half>(a, (const __half*)src, 0, wire, prescale, rng, nullptr, stream)),
@@ -271,12 +356,17 @@ cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint
 
 cudaError_t launch_quantize_items_f32(const ItemKernelArgs& a, const float* src_f32, uint32_t base_elem,
                                       uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) {
+  if (a.codec != kMaxMin) return cudaErrorInvalidValue;
   CGX_BY_DTYPE(a.dtype, (quantize_t<float, float>(a, src_f32, base_elem, wire, 1.0f, rng, (float*)out, stream)),
                (quantize_t<float, __half>(a, src_f32, base_elem, wire, 1.0f, rng, (__half*)out, stream)),
                (quantize_t<float, __nv_bfloat16>(a, src_f32, base_elem, wire, 1.0f, rng, (__nv_bfloat16*)out, stream)))
 }
 
 cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire, void* dst, cudaStream_t stream) {
+  if (a.codec != kMaxMin)
+    CGX_BY_DTYPE(a.dtype, (dequantize_fp8_t<float>(a, wire, (float*)dst, stream)),
+                 (dequantize_fp8_t<__half>(a, wire, (__half*)dst, stream)),
+                 (dequantize_fp8_t<__nv_bfloat16>(a, wire, (__nv_bfloat16*)dst, stream)))
   CGX_BY_DTYPE(a.dtype, (dequantize_t<float>(a, wire, (float*)dst, stream)),
                (dequantize_t<__half>(a, wire, (__half*)dst, stream)),
                (dequantize_t<__nv_bfloat16>(a, wire, (__nv_bfloat16*)dst, stream)))
@@ -285,6 +375,7 @@ cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire
 cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* wire, float* acc_f32,
                                         uint32_t base_elem, const void* init_src, float prescale,
                                         cudaStream_t stream) {
+  if (a.codec != kMaxMin) return cudaErrorInvalidValue;
   CGX_BY_DTYPE(a.dtype, (accumulate_t<float>(a, wire, acc_f32, base_elem, (const float*)init_src, prescale, stream)),
                (accumulate_t<__half>(a, wire, acc_f32, base_elem, (const __half*)init_src, prescale, stream)),
                (accumulate_t<__nv_bfloat16>(a, wire, acc_f32, base_elem, (const __nv_bfloat16*)init_src, prescale,

@@ -809,5 +809,139 @@ __device__ __noinline__ void raw_ag_recv(const SrcSet ss, const WarpItem it, T* 
   }
 }
 
+// ======================================================================================
+// FP8 codecs of the compressed all-to-all (quant_math.h, CODEC = kE4M3 / kE5M2): 8-bit records
+// whose meta is {unit, +0} and whose byte j of a group is element j's FP8 code. Same slices, same
+// min/max reductions and the same 8-bit word loads and stores as max-min; only the element
+// arithmetic differs: one FMUL + half a cvt.satfinite per element to encode, half a cvt.f16x2 +
+// one F2F + one FMUL to decode. Round to nearest only.
+// ======================================================================================
+// per-row NaN-propagating min / max of the bucket each row of the slice belongs to (slice_meta's
+// reductions)
+template <int GPL>
+__device__ __forceinline__ void slice_minmax(const float (&x)[GPL][8], uint32_t lg, float (&mn)[GPL],
+                                             float (&mx)[GPL]) {
+#pragma unroll
+  for (int k = 0; k < GPL; ++k) {
+    mn[k] = CGX_INF_POS;
+    mx[k] = CGX_INF_NEG;
+    minmax8(x[k], mn[k], mx[k]);
+  }
+  if (lg == 0) return;  // 8-element buckets: every row is its own bucket
+  float a = mn[0], b = mx[0];
+#pragma unroll
+  for (int k = 1; k < GPL; ++k) {
+    a = nan_min(a, mn[k]);
+    b = nan_max(b, mx[k]);
+  }
+  if (slice_single_bucket<GPL>(lg))
+    warp_minmax(a, b);
+  else
+    subwarp_minmax(a, b, lg - 1u);  // (512-slices only) a bucket = all rows of 2^(lg-1) adjacent lanes
+#pragma unroll
+  for (int k = 0; k < GPL; ++k) {
+    mn[k] = a;
+    mx[k] = b;
+  }
+}
+
+// 8 values of one group -> their codes, element j in byte j of (lo, hi)
+template <int CODEC>
+__device__ __forceinline__ void fp8_encode8(const float (&x)[8], float inv, uint32_t& lo, uint32_t& hi) {
+  const uint32_t p0 = fp8x2_encode(x[0], x[1], inv, CODEC), p1 = fp8x2_encode(x[2], x[3], inv, CODEC);
+  const uint32_t p2 = fp8x2_encode(x[4], x[5], inv, CODEC), p3 = fp8x2_encode(x[6], x[7], inv, CODEC);
+  lo = __byte_perm(p0, p1, 0x5410);
+  hi = __byte_perm(p2, p3, 0x5410);
+}
+template <int CODEC>
+__device__ __forceinline__ void fp8_decode8(uint32_t lo, uint32_t hi, float unit, float (&x)[8]) {
+  fp8x2_decode(lo, unit, CODEC, x[0], x[1]);
+  fp8x2_decode(lo >> 16, unit, CODEC, x[2], x[3]);
+  fp8x2_decode(hi, unit, CODEC, x[4], x[5]);
+  fp8x2_decode(hi >> 16, unit, CODEC, x[6], x[7]);
+}
+
+// full item, values already in registers: meta + codes to the destination
+template <int CODEC, int GPL, typename DST>
+__device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds) {
+  const uint32_t lg = item_lpb_log2(it);
+  float mn[GPL], mx[GPL];
+  slice_minmax<GPL>(x, lg, mn, mx);
+  BucketMeta m[GPL];
+  uint32_t lo[GPL], hi[GPL];
+#pragma unroll
+  for (int k = 0; k < GPL; ++k) {
+    m[k] = fp8_meta(mn[k], mx[k], CODEC);
+    fp8_encode8<CODEC>(x[k], fp8_inv_unit(m[k].unit), lo[k], hi[k]);
+  }
+  slice_store_meta<GPL>(m, lg, ds, it.meta_off);
+  store_words<8, GPL>(ds, it.pay_off, 8, lo, hi);
+}
+template <typename TS, int CODEC, int GPL, typename DST>
+__device__ __noinline__ void full_send_fp8_unaligned(const TS* __restrict__ src, const WarpItem it, const DST ds) {
+  float x[GPL][8];
+  slice_load_scalar<TS, GPL>(src, x);
+  full_send_fp8_x<CODEC, GPL>(x, it, ds);
+}
+
+// out = decode(already fetched words of ONE source)
+template <typename TO, int CODEC, int GPL, bool VEC>
+__device__ __forceinline__ void full_recv_fp8_w(const SliceWords<GPL>& w, TO* __restrict__ out) {
+  float x[GPL][8];
+#pragma unroll
+  for (int k = 0; k < GPL; ++k) fp8_decode8<CODEC>(w.lo[k], w.hi[k], w.pm[k].unit, x[k]);
+  slice_store<TO, GPL, VEC>(out, x);
+}
+template <typename TO, int CODEC, int GPL>
+__device__ __noinline__ void full_recv_fp8_unaligned(const uint8_t* rec, const WarpItem it, TO* __restrict__ out) {
+  SliceWords<GPL> w;
+  slice_fetch<8, GPL>(rec, it.meta_off, it.pay_off, item_lpb_log2(it), 8, w);
+  full_recv_fp8_w<TO, CODEC, GPL, false>(w, out);
+}
+
+// generic bucket item (cold): ONE bucket of n <= kMaxBlockElems elements, any alignment; the codes
+// of the last group's missing elements are 0, as on the host
+template <typename TS, int CODEC, typename DST>
+__device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const DST ds) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  float mn = CGX_INF_POS, mx = CGX_INF_NEG;
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<TS>(src, g, n, 1.0f, x, nv);
+    minmax8_pred(x, nv, mn, mx);
+  }
+  warp_minmax(mn, mx);
+  const BucketMeta m = fp8_meta(mn, mx, CODEC);
+  const float inv = fp8_inv_unit(m.unit);
+  const DST du = unicast_of(ds);
+  if (lane_id() == 0) dst_st_v2(du, it.meta_off, __float_as_uint(m.unit), __float_as_uint(m.min));
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<TS>(src, g, n, 1.0f, x, nv);
+    uint32_t lo, hi;
+    fp8_encode8<CODEC>(x, inv, lo, hi);
+    const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
+    const uint32_t o = it.pay_off + g * 8u;
+    for (int t = 0; t < 8; ++t) dst_st_u8(du, o + t, (uint32_t)(w >> (8 * t)) & 0xFFu);
+  }
+}
+
+template <typename TO, int CODEC>
+__device__ __noinline__ void bucket_recv_fp8(const uint8_t* rec, const WarpItem it, TO* __restrict__ out) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  const float unit = __uint_as_float(ld_sys_v2(rec + it.meta_off).x);
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    uint32_t lo, hi;
+    load_word<0>(rec + it.pay_off, g, 8, lo, hi);
+    float x[8];
+    fp8_decode8<CODEC>(lo, hi, unit, x);
+    store8_scalar<TO>(out + g * 8u, (int)min(8u, n - g * 8u), x);
+  }
+}
+
 }  // namespace dev
 }  // namespace cgx

@@ -108,6 +108,7 @@ struct A2aParams {
   uint32_t row;
   uint64_t in_rows;
   uint64_t out_rows;
+  int codec;                       // WireCodec (common/quant_math.h); FP8 codecs need bits 8, round to nearest
 };
 // defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
 // p.out_index is set
@@ -125,6 +126,8 @@ struct ItemKernelArgs {
   int dtype;
   int slice_elems;
   int uniform_bits;
+  int codec = 0;  // WireCodec: an FP8 codec needs an 8-bit plan and is supported by launch_quantize_items
+                  // (prescale 1, deterministic rounding) and launch_dequantize_items only
 };
 // wire = quantize(src[T] * prescale)
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,

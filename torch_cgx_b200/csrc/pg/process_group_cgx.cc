@@ -471,7 +471,8 @@ void check_a2a_index(const at::Tensor& index, const at::Tensor& like, const char
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                                       const std::vector<int64_t>& out_splits,
                                                                       const std::vector<int64_t>& in_splits, int bits,
-                                                                      int bucket_size, bool stochastic, int64_t seed,
+                                                                      WireCodec codec, int bucket_size, bool stochastic,
+                                                                      int64_t seed,
                                                                       const at::Tensor& in_index,
                                                                       const at::Tensor& out_index) {
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
@@ -486,6 +487,8 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
               " and the output rows ", out.sizes().slice(1), " differ");
   TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: all_to_all: bits must be 1..8 or 32");
   TORCH_CHECK(bucket_size >= 1, "cgx: all_to_all: bucket_size must be >= 1");
+  TORCH_CHECK(codec == kMaxMin || (bits == 8 && !stochastic),
+              "cgx: all_to_all: the FP8 codecs use bits 8 and round to nearest");
   const int W = getSize();
   TORCH_CHECK(W <= kMaxPeers, "cgx: all_to_all supports at most ", kMaxPeers, " ranks");
   // every rank evaluates the same condition, so every rank refuses and none is left waiting
@@ -509,7 +512,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   route.in_rows = (uint64_t)in.size(0);
   route.out_rows = (uint64_t)out.size(0);
   const bool routed = ii || oi;
-  check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, (uint32_t)bucket_size,
+  check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec, (uint32_t)bucket_size,
                    getRank(), W, routed ? &route : nullptr);
   // the one place that decides where the rows are routed: inside the fused kernel when it can
   // address them, else around a plain call, which computes the same by definition
@@ -518,7 +521,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     for (const at::Tensor* t : {&in_index, &out_index})
       if (t->defined()) c10::cuda::CUDACachingAllocator::recordStream(t->storage().data_ptr(), *comm_stream_);
     if (!routed || in_kernel) {
-      engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits,
+      engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec,
                           (uint32_t)bucket_size, rng, s, routed ? &route : nullptr);
       return;
     }
@@ -528,7 +531,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     std::vector<int64_t> recv_shape = out.sizes().vec();
     recv_shape[0] = oi ? out_index.size(0) : out.size(0);
     at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;
-    engine_->all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits,
+    engine_->all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits, codec,
                         (uint32_t)bucket_size, rng, s);
     if (oi) out.index_copy_(0, out_index, recv);
   });

@@ -195,7 +195,7 @@ class ProcessGroupCGX : public c10d::Backend {
   // Compressed all_to_all_single: dim-0 rows of `in` go to the ranks by `in_splits`, rows of `out`
   // come from the ranks by `out_splits` (empty: equal splits). The own chunk is copied, every other
   // chunk quantized once with `bits` (1..8; 32: raw) and buckets of `bucket_size` counted from the
-  // chunk's start. seed < 0: CGX_SEED. Malformed splits throw before anything is enqueued; the
+  // chunk's start; an FP8 `codec` (bits 8, round to nearest) gives the 8-bit records FP8 codes. seed < 0: CGX_SEED. Malformed splits throw before anything is enqueued; the
   // splits of a pair must agree on both ranks (the caller's contract). One node only.
   // Routed form: with `in_index` row i of the sent rows is in[in_index[i]], with `out_index` row j
   // of the received rows goes to out[out_index[j]] (undefined tensors: no index). The splits then
@@ -204,8 +204,8 @@ class ProcessGroupCGX : public c10d::Backend {
   c10::intrusive_ptr<c10d::Work> all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                        const std::vector<int64_t>& out_splits,
                                                        const std::vector<int64_t>& in_splits, int bits,
-                                                       int bucket_size, bool stochastic, int64_t seed,
-                                                       const at::Tensor& in_index = at::Tensor(),
+                                                       WireCodec codec, int bucket_size, bool stochastic,
+                                                       int64_t seed, const at::Tensor& in_index = at::Tensor(),
                                                        const at::Tensor& out_index = at::Tensor());
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);

@@ -12,6 +12,12 @@
 namespace cgx {
 namespace {
 
+// what the FP8 codecs of the block primitives support: 8-bit plans, no prescale, round to nearest
+void check_fp8(const Plan& p, float prescale, const RngKey& rng) {
+  if (p.uniform_bits != 8 || prescale != 1.0f || rng.enabled)
+    throw std::invalid_argument("cgx: an FP8 codec needs an 8-bit plan, prescale 1 and round to nearest");
+}
+
 class CpuBackend : public BlockBackend {
  public:
   bool is_cuda() const override { return false; }
@@ -22,13 +28,17 @@ class CpuBackend : public BlockBackend {
   }
   void release(void* p) override { std::free(p); }
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
-                const RngKey& rng, cudaStream_t) override {
+                const RngKey& rng, cudaStream_t, WireCodec codec) override {
     const Plan& p = dp.plan;
+    if (codec != kMaxMin) check_fp8(p, prescale, rng);
     std::vector<float> acc(kMaxBlockElems);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
       cpu::load_block(src, p.dtype, d, prescale, acc.data());
-      cpu::quantize_block(acc.data(), p.dtype, d, wire + d.wire_off, rng, b);
+      if (codec != kMaxMin)
+        cpu::quantize_block_fp8(acc.data(), d, wire + d.wire_off, codec);
+      else
+        cpu::quantize_block(acc.data(), p.dtype, d, wire + d.wire_off, rng, b);
     }
   }
   void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
@@ -51,10 +61,14 @@ class CpuBackend : public BlockBackend {
     }
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
-                  cudaStream_t) override {
+                  cudaStream_t, WireCodec codec) override {
+    if (codec != kMaxMin) check_fp8(dp.plan, 1.0f, RngKey{});
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = dp.plan.blocks[b];
-      cpu::decode_block_store(wire + d.wire_off, dp.plan.dtype, d, dst);
+      if (codec != kMaxMin)
+        cpu::decode_block_fp8_store(wire + d.wire_off, dp.plan.dtype, d, dst, codec);
+      else
+        cpu::decode_block_store(wire + d.wire_off, dp.plan.dtype, d, dst);
     }
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t) override { std::memcpy(dst, src, bytes); }
@@ -75,8 +89,10 @@ class CudaBackend : public BlockBackend {
   }
   void release(void* p) override { cudaFree(p); }
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
-                const RngKey& rng, cudaStream_t stream) override {
-    cuda_check(launch_quantize_items(args(dp, first, count), src, wire, prescale, rng, stream), "quantize_items");
+                const RngKey& rng, cudaStream_t stream, WireCodec codec) override {
+    if (codec != kMaxMin) check_fp8(dp.plan, prescale, rng);
+    cuda_check(launch_quantize_items(args(dp, first, count, codec), src, wire, prescale, rng, stream),
+               "quantize_items");
   }
   void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
                   uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream) override {
@@ -90,8 +106,9 @@ class CudaBackend : public BlockBackend {
                "quantize_items_f32");
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
-                  cudaStream_t stream) override {
-    cuda_check(launch_dequantize_items(args(dp, first, count), wire, dst, stream), "dequantize_items");
+                  cudaStream_t stream, WireCodec codec) override {
+    if (codec != kMaxMin) check_fp8(dp.plan, 1.0f, RngKey{});
+    cuda_check(launch_dequantize_items(args(dp, first, count, codec), wire, dst, stream), "dequantize_items");
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) override {
     cuda_check(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, stream), "cudaMemcpyAsync");
@@ -99,8 +116,9 @@ class CudaBackend : public BlockBackend {
 
  private:
   // blocks [first, first+count) -> their warp items (items are emitted block by block)
-  static ItemKernelArgs args(const DevicePlan& dp, uint32_t first, uint32_t count) {
+  static ItemKernelArgs args(const DevicePlan& dp, uint32_t first, uint32_t count, WireCodec codec = kMaxMin) {
     ItemKernelArgs a;
+    a.codec = codec;
     a.items = dp.d_items;
     a.first = dp.plan.block_item_first[first];
     a.count = dp.plan.block_item_first[first + count] - a.first;

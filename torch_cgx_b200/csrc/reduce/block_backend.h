@@ -9,6 +9,7 @@
 
 #include "../common/philox.h"
 #include "../common/plan.h"
+#include "../common/quant_math.h"
 #include "plan_cache.h"
 
 namespace cgx {
@@ -22,9 +23,10 @@ class BlockBackend {
   virtual void release(void* p) = 0;
   // The block primitives work on blocks [first, first+count) of `dp`'s plan; the device backend
   // reads its uploaded tables (PlanCache::upload), the host backend the plan alone.
-  // wire = quantize(src[T] * prescale)
+  // wire = quantize(src[T] * prescale). An FP8 `codec` (common/quant_math.h) needs an 8-bit plan,
+  // prescale 1 and deterministic rounding; its records are read back by dequantize with the same codec.
   virtual void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire,
-                        float prescale, const RngKey& rng, cudaStream_t stream) = 0;
+                        float prescale, const RngKey& rng, cudaStream_t stream, WireCodec codec = kMaxMin) = 0;
   // acc_f32[elem_off - base_elem + i] = float(init_src[elem_off + i]) * prescale   (init_src != nullptr)
   // acc_f32[...] += decode(wire)                                                   (wire != nullptr)
   virtual void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
@@ -34,7 +36,7 @@ class BlockBackend {
                             uint32_t count, uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) = 0;
   // dst[T] = decode(wire)
   virtual void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
-                          cudaStream_t stream) = 0;
+                          cudaStream_t stream, WireCodec codec = kMaxMin) = 0;
   virtual void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) = 0;
 };
 

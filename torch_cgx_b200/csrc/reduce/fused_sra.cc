@@ -272,12 +272,15 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
 }
 
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
-                      const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
-                      int world, const A2aRoute* route) {
+                      const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
+                      int rank, int world, const A2aRoute* route) {
   if ((int)in_counts.size() != world || (int)out_counts.size() != world)
     throw std::invalid_argument("cgx all_to_all: need one input and one output count per rank");
   if (bits < 1 || (bits > 8 && bits < kRawBits))
     throw std::invalid_argument("cgx all_to_all: bits must be in 1..8, or 32 for none");
+  if (codec != kMaxMin && codec != kE4M3 && codec != kE5M2)
+    throw std::invalid_argument("cgx all_to_all: unknown wire codec");
+  if (codec != kMaxMin && bits != 8) throw std::invalid_argument("cgx all_to_all: the FP8 codecs use bits 8");
   if (bucket < 1) throw std::invalid_argument("cgx all_to_all: bucket_size must be >= 1");
   if (in_counts[rank] != out_counts[rank])
     throw std::invalid_argument("cgx all_to_all: a rank's chunk for itself must be as large as the one it receives from itself");
@@ -306,11 +309,13 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
 
 FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                          const std::vector<uint64_t>& out_counts, int dtype, int bits,
-                                         uint32_t bucket, const RngParams& rng, cudaStream_t stream,
-                                         const A2aRoute* route) {
+                                         WireCodec codec, uint32_t bucket, const RngParams& rng,
+                                         cudaStream_t stream, const A2aRoute* route) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   const int W = world(), r = rank();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W, route);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, route);
+  if (codec != kMaxMin && rng.stochastic)
+    throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
   if (routed && !a2a_rows_fit((uint32_t)route->row, bits, bucket, (int)es))
@@ -346,6 +351,7 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
   p.dtype = dtype;
   p.bits = bits >= kRawBits ? kRawBits : bits;
   p.bucket = bucket;
+  p.codec = codec;
   p.epoch_hint = epoch_;
   p.rng = make_rng_key(rng, r, 0);
   p.slot_bytes = heap_->layout().slot_bytes;

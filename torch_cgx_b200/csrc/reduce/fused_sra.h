@@ -77,12 +77,12 @@ struct A2aRoute {
 };
 
 // The arguments of one rank's all-to-all (FusedSra::all_to_all, Reducer::all_to_all): a count per
-// rank on both sides, bits 1..8 or >= 32, a bucket >= 1, the own chunk the same size on both sides,
+// rank on both sides, bits 1..8 or >= 32 (8 with an FP8 codec), a bucket >= 1, the own chunk the same size on both sides,
 // tensors below 2^32 elements and an output that does not overlap the input; with a route, counts
 // of whole rows and no overlap of the tensors the indices address; std::invalid_argument otherwise.
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
-                      const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, int rank,
-                      int world, const A2aRoute* route = nullptr);
+                      const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
+                      int rank, int world, const A2aRoute* route = nullptr);
 
 class FusedSra {
  public:
@@ -144,7 +144,9 @@ class FusedSra {
   // `in` (consecutive, in rank order) go to rank q; out_counts[q] elements from rank q land in `out`
   // (consecutive, in rank order). My own chunk is copied; every other chunk is decode(Q(chunk)) with
   // `bits` (1..8; >= 32 moves it raw) and buckets of `bucket` counted from the chunk's first
-  // element. The counts of a pair must agree on both ends (the caller's contract, as with NCCL).
+  // element. `codec` says what the bytes of the 8-bit records mean (common/quant_math.h): max-min
+  // levels, or an FP8 code per element with a per-bucket scale (bits 8, round to nearest; the caller
+  // rejects stochastic rounding). The counts of a pair must agree on both ends (the caller's contract, as with NCCL).
   // Throws std::invalid_argument on a malformed call before anything is launched.
   // With a `route` that has an index, the routed kernel gathers the sent rows and scatters the
   // received ones by index; that needs a2a_rows_fit(route->row, bits, bucket, dtype) (else
@@ -153,8 +155,8 @@ class FusedSra {
     uint64_t launches = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's sends
   };
   A2aCounts all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
-                       const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                       const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr);
+                       const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
+                       uint32_t bucket, const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

@@ -168,10 +168,10 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
 }
 
 void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
-                         const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket,
-                         const RngParams& rng, cudaStream_t stream) {
+                         const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
+                         uint32_t bucket, const RngParams& rng, cudaStream_t stream) {
   const int W = comm_->size(), r = comm_->rank();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, bucket, r, W);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W);
   const size_t es = (size_t)dtype_size(dtype);
   const bool raw = bits >= kRawBits;
   const uint8_t* src = static_cast<const uint8_t*>(in);
@@ -200,7 +200,7 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
     RngKey key = make_rng_key(rng, r, 0);
     key.stream = a2a_rng_stream(r, q);
     const DevicePlan& dp = plan_for({LayerSpec{0, in_counts[q], bits, bucket}}, dtype, false, stream, 1);
-    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, key, stream);
+    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, key, stream, codec);
   }
   std::vector<P2POp> x;
   for (int q = 0; q < W; ++q) {
@@ -219,7 +219,7 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
   for (int q = 0; q < W; ++q) {
     if (!rw[q]) continue;
     const DevicePlan& dp = plan_for({LayerSpec{0, out_counts[q], bits, bucket}}, dtype, false, stream, 1);
-    ops_->dequantize(dp, recvb + ro[q], 0, (uint32_t)dp.plan.blocks.size(), dst + oo[q], stream);
+    ops_->dequantize(dp, recvb + ro[q], 0, (uint32_t)dp.plan.blocks.size(), dst + oo[q], stream, codec);
   }
 }
 

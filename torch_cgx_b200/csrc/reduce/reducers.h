@@ -60,10 +60,11 @@ class Reducer {
   // Compressed all-to-all over the communicator's W ranks, bitwise FusedSra::all_to_all (same
   // arguments and checks): each chunk for a peer is quantized by the standalone item kernels through
   // a one-layer plan of the chunk, the records are exchanged and every peer's chunk is decoded into
-  // its rows; the own chunk is copied, and with bits >= 32 every chunk travels as its bytes.
+  // its rows; the own chunk is copied, and with bits >= 32 every chunk travels as its bytes. An FP8
+  // `codec` quantizes and decodes the 8-bit records with the block backend's FP8 primitives.
   void all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
-                  const std::vector<uint64_t>& out_counts, int dtype, int bits, uint32_t bucket, const RngParams& rng,
-                  cudaStream_t stream);
+                  const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
+                  const RngParams& rng, cudaStream_t stream);
   uint64_t bytes_sent() const { return bytes_sent_; }
   size_t num_plans() const { return plans_.size(); }
   uint64_t plan_uploads() const { return plans_.uploads(); }

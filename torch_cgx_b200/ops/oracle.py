@@ -622,13 +622,58 @@ def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[
     return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers) for t in inputs])
 
 
-def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, bits: int,
+# ---- FP8 wire formats of the all-to-all (common/quant_math.h, DESIGN §2.13b) ------------------------
+# name -> (torch dtype, largest finite value)
+FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0)}
+_FP8_MIN_UNIT = _F32(2.0 ** -126)
+
+
+def _fp8_qdq_buckets(v: np.ndarray, fmt: str, bucket: int) -> np.ndarray:
+    """FP8 round trip of a flat fp32 array whose buckets start at index 0, in numpy fp32 arithmetic
+    and torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126),
+    code = float8(clamp(x * inv, ±FMAX)), decoded as float(code) * unit. The clamp stands for the
+    hardware's saturation: torch's casts give NaN / Inf past the largest finite value."""
+    tdt, fmax = FP8_FORMATS[fmt]
+    n = v.size
+    if n == 0:
+        return np.zeros(0, _F32)
+    nb = -(-n // bucket)
+    pad = nb * bucket - n
+    vp = np.concatenate([v, np.repeat(v[-1:], pad)]) if pad else v
+    b = vp.reshape(nb, bucket)
+    with np.errstate(all="ignore"):
+        mn, mx = _nan_minmax(b)
+        a = np.maximum(-mn, mx)  # NaN propagates
+        a = np.where(a == 0, _F32(0.0), a)  # +0, as max.NaN gives for a zero bucket
+        unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
+        inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
+        t = np.clip((b * inv).astype(_F32), _F32(-fmax), _F32(fmax))
+        code = torch.from_numpy(np.ascontiguousarray(t)).to(tdt).float().numpy()
+        dec = (code * unit).astype(_F32)
+    return dec.reshape(-1)[:n]
+
+
+def fp8_quantize_dequantize(x: torch.Tensor, fmt: str, bucket_size: int) -> torch.Tensor:
+    """FP8 (``fmt`` "e4m3" / "e5m2") round trip of a flat tensor, buckets of ``bucket_size``
+    (clamped as every bucket) from its first element, rounded to ``x.dtype``."""
+    if fmt not in FP8_FORMATS:
+        raise ValueError(f"unknown FP8 format {fmt!r}")
+    v = x.detach().reshape(-1).float().cpu().numpy()
+    dec = _fp8_qdq_buckets(v, fmt, effective_bucket(bucket_size))
+    return _to_tensors([dec], x.dtype)[0].view_as(x)
+
+
+def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, bits: int | str,
                          bucket_size: int) -> List[torch.Tensor]:
     """Every rank's output of the compressed all-to-all (round to nearest). ``counts[q][r]`` elements
     go from rank q to rank r; rank q's input holds its chunks in destination order and rank r's
     output the chunks it receives in source order. The own chunk, and every chunk when ``bits`` is
     32, is the input unchanged; every other chunk is ``quantize_dequantize_layers`` of one layer, so
-    buckets are counted from the chunk's first element."""
+    buckets are counted from the chunk's first element. ``bits`` "e4m3" / "e5m2": every other chunk
+    is ``fp8_quantize_dequantize`` instead."""
+    if isinstance(bits, str) and bits not in FP8_FORMATS:
+        raise ValueError(f"unknown FP8 format {bits!r}")
+    fp8 = isinstance(bits, str)
     W = len(inputs)
     flat = [t.detach().reshape(-1).cpu() for t in inputs]
     outs = []
@@ -638,7 +683,9 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
             a = sum(int(c) for c in counts[q][:r])
             n = int(counts[q][r])
             chunk = flat[q][a:a + n].clone()
-            if q != r and bits < RAW_BITS and n > 0:
+            if q != r and n > 0 and fp8:
+                chunk = fp8_quantize_dequantize(chunk, bits, bucket_size)
+            elif q != r and n > 0 and bits < RAW_BITS:
                 chunk = quantize_dequantize_layers(chunk, [(0, n, int(bits), int(bucket_size))])
             parts.append(chunk)
         outs.append(torch.cat(parts) if parts else flat[r].new_empty(0))
@@ -647,7 +694,7 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
 
 def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
                                 input_index: Sequence[torch.Tensor | None],
-                                output_index: Sequence[torch.Tensor | None], row: int, *, bits: int,
+                                output_index: Sequence[torch.Tensor | None], row: int, *, bits: int | str,
                                 bucket_size: int, outputs: Sequence[torch.Tensor] | None = None) -> List[torch.Tensor]:
     """Every rank's output of the routed all-to-all, as the composition that defines it: rank q sends
     ``inputs[q].index_select(0, input_index[q])`` (rows of ``row`` elements; ``None``: the input

@@ -21,13 +21,13 @@ and the compressed all-to-all of expert-parallel MoE layers (``dist.all_to_all_s
 uncompressed)::
 
     cgx.all_to_all_single(recv, tokens, recv_splits, send_splits, bits=8)
-    y = cgx.differentiable_all_to_all_single(tokens, recv_splits, send_splits, bits=8)
+    y = cgx.differentiable_all_to_all_single(tokens, recv_splits, send_splits, bits="e4m3", grad_bits="e5m2")
 """
 from __future__ import annotations
 
 import contextlib
 import os
-from typing import Iterator, List, Optional, Sequence, Tuple
+from typing import Iterator, List, Optional, Sequence, Tuple, Union
 
 import torch
 import torch.distributed as dist
@@ -164,8 +164,23 @@ def _splits(s: Optional[Sequence[int]]) -> List[int]:
     return [] if s is None else [int(v) for v in s]
 
 
+A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2"
+
+
+def _a2a_bits(bits: A2aBits, stochastic: bool) -> A2aBits:
+    """``bits`` as the native all-to-all takes it: an int, or an FP8 format name. An unknown name, or
+    an FP8 format with ``stochastic``, raises ValueError (the native parser's check, run here so that
+    it fires before anything is sent)."""
+    if not isinstance(bits, str):
+        return int(bits)
+    from .. import _C
+
+    _C.a2a_bits(bits, bool(stochastic))
+    return bits
+
+
 def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
-                      input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8, bucket_size: int = 512,
+                      input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8, bucket_size: int = 512,
                       group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
                       input_index: Optional[torch.Tensor] = None, output_index: Optional[torch.Tensor] = None):
     """Compressed ``dist.all_to_all_single`` on a ``cgx`` group.
@@ -176,6 +191,14 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     (``bits`` 1..8, max-min, buckets of ``bucket_size`` counted from the chunk's first element) and
     decoded by the receiver; ``bits=32`` moves every chunk unchanged. Round to nearest unless
     ``stochastic``; ``seed=None`` uses ``CGX_SEED``.
+
+    ``bits="e4m3"`` or ``"e5m2"`` sends the same bytes as ``bits=8`` but as FP8: per bucket one fp32
+    scale ``unit = max|x| / FMAX`` (448 or 57344) and one FP8 code of ``x / unit`` per element,
+    converted by Hopper's FP8 instructions. Its relative error per element is at most 2^-4 (e4m3)
+    or 2^-3 (e5m2) whatever else the bucket holds, so it suits rows with a few outlier channels;
+    max-min 8-bit is more accurate on well-behaved data. A bucket holding a NaN or an Inf decodes to
+    NaN in every element. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as
+    does any other string.
 
     Routed form, for MoE token dispatch and combine without a permutation copy: ``input_index``
     (CUDA int64, ``sum(input_split_sizes)`` entries in ``[0, input.shape[0])``, repeats allowed)
@@ -197,11 +220,12 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     """
     from .hooks import _native_backend
 
+    bits = _a2a_bits(bits, stochastic)
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
     if native is None:
         raise RuntimeError("cgx.all_to_all_single needs a process group with the cgx backend")
     work = native.all_to_all_compressed(output, input, _splits(output_split_sizes), _splits(input_split_sizes),
-                                        int(bits), int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
+                                        bits, int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
                                         input_index, output_index)
     if async_op:
         return work
@@ -262,14 +286,16 @@ class _AllToAll(torch.autograd.Function):
 
 
 def differentiable_all_to_all_single(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
-                                     input_split_sizes: Optional[Sequence[int]] = None, bits: int = 8,
-                                     grad_bits: Optional[int] = None, bucket_size: int = 512, group=None,
+                                     input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8,
+                                     grad_bits: Optional[A2aBits] = None, bucket_size: int = 512, group=None,
                                      stochastic: bool = False, input_index: Optional[torch.Tensor] = None,
                                      output_index: Optional[torch.Tensor] = None,
                                      output_rows: Optional[int] = None) -> torch.Tensor:
     """``all_to_all_single`` that returns its output and has a backward pass: the compressed
     all-to-all of the gradient with the splits swapped, at ``grad_bits`` (``None``: ``bits``; 32:
-    exact). This is the form an MoE layer calls for its token dispatch and combine.
+    exact). This is the form an MoE layer calls for its token dispatch and combine. Either may be an
+    FP8 format; ``bits="e4m3", grad_bits="e5m2"`` is the usual FP8 recipe. Both are checked before
+    the forward sends anything.
 
     ``input_index`` / ``output_index`` route rows as in ``all_to_all_single``. With ``output_index``
     the result has ``output_rows`` rows, and rows it does not name are zero. The backward gathers
@@ -278,7 +304,8 @@ def differentiable_all_to_all_single(input: torch.Tensor, output_split_sizes: Op
     the sum of its copies' gradients."""
     if output_index is not None and output_rows is None:
         raise ValueError("cgx.differentiable_all_to_all_single: output_index needs output_rows")
-    gb = int(bits if grad_bits is None else grad_bits)
+    bits = _a2a_bits(bits, stochastic)
+    gb = _a2a_bits(bits if grad_bits is None else grad_bits, stochastic)
     return _AllToAll.apply(input, None if output_split_sizes is None else _splits(output_split_sizes),
-                           None if input_split_sizes is None else _splits(input_split_sizes), int(bits), gb,
+                           None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
                            int(bucket_size), group, bool(stochastic), input_index, output_index, output_rows)
