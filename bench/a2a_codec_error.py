@@ -12,6 +12,12 @@ Inputs, rows of H = 7168 fp32 elements (one MoE hidden state per row):
 Reported per (input, bucket, codec): the relative L2 error ||dec - x|| / ||x|| and the largest
 per-element relative error |dec - x| / |x| over elements with |x| >= 1e-3 * rms(x). This says
 nothing about training accuracy.
+
+--op reduce_scatter / all_gather report the same for the compressed reduce-scatter and all-gather
+of --world ranks (C.reduce_scatter_simulate / C.all_gather_simulate, bit for bit what rs_kernel and
+ag_kernel deliver): every rank holds --rows rows of its own seeded input (rows divisible by the
+world); the reduce-scatter's result is compared with the exact fp64 sum of each shard, the
+all-gather's with the gathered inputs.
 """
 import argparse
 import json
@@ -57,6 +63,26 @@ def decode(x, bits, bucket):
     return out[1].reshape(x.shape)
 
 
+def sharded(op, kind, rows, seed, world, bits, bucket):
+    """(exact, received) of one sharded call of `world` ranks, rows of H as in make_rows; the
+    received result of every rank, stacked, and the exact one of the same shape"""
+    xs = [make_rows(kind, rows, seed + 1000 * q)[0] for q in range(world)]
+    mask = make_rows(kind, rows, seed)[1]
+    n = rows * H
+    S = n // world
+    fmt = bits if isinstance(bits, str) else None
+    table = [(0, S, 8 if fmt else bits, bucket)]
+    if op == "reduce_scatter":
+        outs = [torch.empty(S) for _ in range(world)]
+        C.reduce_scatter_simulate([x.reshape(-1) for x in xs], outs, table, bits=fmt)
+        exact = torch.stack([x.double() for x in xs]).sum(0).reshape(-1)
+        return exact.float().reshape(rows, H), torch.cat(outs).reshape(rows, H), mask
+    shards = [xs[q].reshape(-1)[q * S:(q + 1) * S].clone() for q in range(world)]
+    outs = [torch.empty(n) for _ in range(world)]
+    C.all_gather_simulate(shards, outs, table, bits=fmt)
+    return torch.cat(shards).reshape(rows, H), outs[0].reshape(rows, H), mask
+
+
 def errors(x, dec, keep):
     x, dec = x[:, keep].double(), dec[:, keep].double()
     rel_l2 = float((dec - x).norm() / x.norm())
@@ -71,14 +97,22 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--buckets", type=int, nargs="+", default=[128, 512])
     ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
+    ap.add_argument("--op", default="all_to_all", choices=["all_to_all", "reduce_scatter", "all_gather"])
+    ap.add_argument("--world", type=int, default=8, help="--op reduce_scatter / all_gather: ranks")
     args = ap.parse_args()
+    if args.op != "all_to_all" and args.rows % args.world:
+        ap.error("--rows must be divisible by --world")
     res = []
     for i, kind in enumerate(("gaussian", "outliers", "student_t")):
         x, mask = make_rows(kind, args.rows, args.seed + i)
         for bucket in args.buckets:
             for bits in (8, "e4m3", "e5m2"):
-                rel_l2, max_rel = errors(x, decode(x, bits, bucket), ~mask)
-                r = {"input": kind, "bucket": bucket, "codec": "maxmin8" if bits == 8 else bits,
+                if args.op == "all_to_all":
+                    rel_l2, max_rel = errors(x, decode(x, bits, bucket), ~mask)
+                else:
+                    exact, got, m = sharded(args.op, kind, args.rows, args.seed + i, args.world, bits, bucket)
+                    rel_l2, max_rel = errors(exact, got, ~m)
+                r = {"op": args.op, "input": kind, "bucket": bucket, "codec": "maxmin8" if bits == 8 else bits,
                      "rel_l2_pct": round(100 * rel_l2, 3), "max_rel_pct": round(100 * max_rel, 2)}
                 res.append(r)
                 print(json.dumps(r), flush=True)

@@ -14,7 +14,10 @@ rank in W chunks, with equal splits and with skewed ones (chunk q -> r gets a sh
 next to the reduce-scatter (rs_kernel) of the same `mb` MB input per rank, same dtype, bits and
 bucket. Both move the same packed bytes; the reduce-scatter also accumulates. Its --bits may name
 the FP8 wire formats, e4m3 and e5m2, which move the bytes of bits 8 (the reduce-scatter row next to
-them runs at bits 8)."""
+them runs at bits 8).
+
+--op sra --bits may name them too: they time the reduce-scatter and all-gather rows only (there is
+no FP8 allreduce). Every row is timed for each of --dtypes."""
 import argparse
 import json
 import sys
@@ -54,7 +57,7 @@ def main():
     ap.add_argument("--out", default="gpurun_out/virtual_world.json")
     ap.add_argument("--op", default="sra", choices=["sra", "all_to_all"],
                     help="sra: allreduce, reduce-scatter and all-gather rows; all_to_all: a2a next to rs_kernel")
-    ap.add_argument("--dtypes", default="float32", help="--op all_to_all: comma-separated dtypes")
+    ap.add_argument("--dtypes", default="float32", help="comma-separated dtypes")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     W = args.world
@@ -67,69 +70,83 @@ def main():
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
         Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
         return
-    for bits in [int(b) for b in args.bits.split(",")]:
+    for dtype in [getattr(torch, d) for d in args.dtypes.split(",")]:
+        for bits in [a2a_bits(b) for b in args.bits.split(",")]:
+            rows += sra_rows(args, dev, W, lanes, dtype, bits)
+    clocks = sampler.stop()
+    Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+    Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
+
+
+def sra_rows(args, dev, W, lanes, dtype, bits):
+    """the allreduce, reduce-scatter and all-gather rows of one dtype and --bits entry; an FP8 format
+    times the reduce-scatter and all-gather only (its records are those of bits 8)"""
+    rows = []
+    fmt = bits if isinstance(bits, str) else None
+    width = 8 if fmt else bits
+    es = torch.empty(0, dtype=dtype).element_size()
+    dt = str(dtype).replace("torch.", "")
+    mbs = sorted(int(x) for x in args.mbs.split(","))
+    if fmt is None:
         res = {}
-        for mb in [int(x) for x in args.mbs.split(",")]:
-            n = (mb << 20) // 4
+        for mb in mbs:
+            n = (mb << 20) // es
             layers = [(0, n, bits, args.bucket)]
-            g = C.LocalSraGroup(W, lanes, n * 4 // W * 2 + (1 << 20), 20000, 4096)
-            xs = [torch.randn(n, device=dev) for _ in range(W)]
+            g = C.LocalSraGroup(W, lanes, n * es // W * 2 + (1 << 20), 20000, 4096)
+            xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
             g.allreduce(xs, layers)
             torch.cuda.synchronize()
             g.check()
             res[mb] = timeit(lambda: g.allreduce(xs, layers))
             del g, xs
-        mbs = sorted(res)
         slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])  # us per MB per virtual rank
-        row = {"world": W, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
+        row = {"world": W, "dtype": dt, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
                "times_us": {str(k): round(v, 1) for k, v in res.items()},
                "us_per_equivalent_64MB_allreduce": round(slope * 64 / W, 1),
                "note": "slope * (64 MB / W): device work of one real rank of a 64 MB allreduce on W GPUs, NVLink excluded"}
         rows.append(row)
         print(json.dumps(row), flush=True)
-        res = {}
-        for mb in [int(x) for x in args.mbs.split(",")]:
-            n = (mb << 20) // 4 // W * W
-            shard = [(0, n // W, bits, args.bucket)]
-            g = C.LocalSraGroup(W, lanes, n * 4 // W * 2 + (1 << 20), 20000, 4096)
-            xs = [torch.randn(n, device=dev) for _ in range(W)]
-            outs = [torch.empty(n // W, device=dev) for _ in range(W)]
-            g.reduce_scatter(xs, outs, shard)
-            torch.cuda.synchronize()
-            g.check()
-            res[mb] = timeit(lambda: g.reduce_scatter(xs, outs, shard))
-            del g, xs, outs
-        slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])
-        row = {"op": "reduce_scatter", "world": W, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
-               "times_us": {str(k): round(v, 1) for k, v in res.items()},
-               "us_per_equivalent_64MB_reduce_scatter": round(slope * 64 / W, 1),
-               "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-input reduce-scatter on W GPUs, "
-                       "NVLink excluded"}
-        rows.append(row)
-        print(json.dumps(row), flush=True)
-        res = {}
-        for mb in [int(x) for x in args.mbs.split(",")]:
-            n = (mb << 20) // 4 // W * W
-            shard = [(0, n // W, bits, args.bucket)]
-            g = C.LocalSraGroup(W, lanes, n * 4 // W * 2 + (1 << 20), 20000, 4096)
-            xs = [torch.randn(n // W, device=dev) for _ in range(W)]
-            outs = [torch.empty(n, device=dev) for _ in range(W)]
-            g.all_gather(xs, outs, shard)
-            torch.cuda.synchronize()
-            g.check()
-            res[mb] = timeit(lambda: g.all_gather(xs, outs, shard))
-            del g, xs, outs
-        slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])
-        row = {"op": "all_gather", "world": W, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
-               "times_us": {str(k): round(v, 1) for k, v in res.items()},
-               "us_per_equivalent_64MB_all_gather": round(slope * 64 / W, 1),
-               "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-output all-gather on W GPUs, "
-                       "NVLink excluded"}
-        rows.append(row)
-        print(json.dumps(row), flush=True)
-    clocks = sampler.stop()
-    Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-    Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
+    res = {}
+    for mb in mbs:
+        n = (mb << 20) // es // W * W
+        shard = [(0, n // W, width, args.bucket)]
+        g = C.LocalSraGroup(W, lanes, n * es // W * 2 + (1 << 20), 20000, 4096)
+        xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
+        outs = [torch.empty(n // W, device=dev, dtype=dtype) for _ in range(W)]
+        g.reduce_scatter(xs, outs, shard, bits=fmt)
+        torch.cuda.synchronize()
+        g.check()
+        res[mb] = timeit(lambda: g.reduce_scatter(xs, outs, shard, bits=fmt))
+        del g, xs, outs
+    slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])
+    row = {"op": "reduce_scatter", "world": W, "dtype": dt, "bits": bits, "bucket": args.bucket,
+           "lanes_per_rank": lanes, "times_us": {str(k): round(v, 1) for k, v in res.items()},
+           "us_per_equivalent_64MB_reduce_scatter": round(slope * 64 / W, 1),
+           "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-input reduce-scatter on W GPUs, "
+                   "NVLink excluded"}
+    rows.append(row)
+    print(json.dumps(row), flush=True)
+    res = {}
+    for mb in mbs:
+        n = (mb << 20) // es // W * W
+        shard = [(0, n // W, width, args.bucket)]
+        g = C.LocalSraGroup(W, lanes, n * es // W * 2 + (1 << 20), 20000, 4096)
+        xs = [torch.randn(n // W, device=dev).to(dtype) for _ in range(W)]
+        outs = [torch.empty(n, device=dev, dtype=dtype) for _ in range(W)]
+        g.all_gather(xs, outs, shard, bits=fmt)
+        torch.cuda.synchronize()
+        g.check()
+        res[mb] = timeit(lambda: g.all_gather(xs, outs, shard, bits=fmt))
+        del g, xs, outs
+    slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])
+    row = {"op": "all_gather", "world": W, "dtype": dt, "bits": bits, "bucket": args.bucket,
+           "lanes_per_rank": lanes, "times_us": {str(k): round(v, 1) for k, v in res.items()},
+           "us_per_equivalent_64MB_all_gather": round(slope * 64 / W, 1),
+           "note": "slope * (64 MB / W): device work of one real rank of a 64 MB-output all-gather on W GPUs, "
+                   "NVLink excluded"}
+    rows.append(row)
+    print(json.dumps(row), flush=True)
+    return rows
 
 
 def skewed_counts(W, n):

@@ -169,6 +169,47 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
   oneshot_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
 }
 
+// The `bits` of every all-to-all, reduce-scatter and all-gather binding: 1..8 or 32 (max-min levels,
+// or raw), or the name of an FP8 wire codec, which travels in 8-bit records and rounds to nearest
+// only. Integers are checked where they are used, as before; an unknown name, or an FP8 codec with
+// stochastic rounding, raises ValueError naming `op` before anything runs.
+using A2aBitsArg = std::variant<int64_t, std::string>;
+struct A2aBits {
+  int bits;
+  WireCodec codec;
+};
+A2aBits a2a_bits(const A2aBitsArg& arg, bool stochastic, const char* op = "all_to_all") {
+  const std::string* name = std::get_if<std::string>(&arg);
+  if (name == nullptr) return {(int)std::get<int64_t>(arg), kMaxMin};
+  WireCodec codec;
+  if (*name == "e4m3")
+    codec = kE4M3;
+  else if (*name == "e5m2")
+    codec = kE5M2;
+  else
+    throw py::value_error(std::string("cgx ") + op + ": bits must be 1..8, 32, \"e4m3\" or \"e5m2\", got \"" +
+                          *name + "\"");
+  if (stochastic)
+    throw py::value_error(std::string("cgx ") + op + ": bits=\"" + *name +
+                          "\" rounds to nearest only; stochastic rounding needs integer bits");
+  return {8, codec};
+}
+
+// The codec of a sharded binding that takes a layer table: None or an integer `bits` keeps max-min
+// (the table gives the widths); an FP8 name selects that codec for the table's 8-bit layers, and
+// every layer must then have bits 8 or 32. ValueError otherwise, before anything runs.
+WireCodec sharded_codec(const std::optional<A2aBitsArg>& bits, const std::vector<LayerSpec>& layers, bool stochastic,
+                        const char* op) {
+  if (!bits) return kMaxMin;
+  const A2aBits wb = a2a_bits(*bits, stochastic, op);
+  if (wb.codec != kMaxMin)
+    for (const LayerSpec& l : layers)
+      if (l.bits != 8 && l.bits < kRawBits)
+        throw py::value_error(std::string("cgx ") + op + ": an FP8 format needs layers of bits 8 or 32, got " +
+                              std::to_string(l.bits));
+  return wb.codec;
+}
+
 // Argument checks of the sharded simulators: one CPU contiguous input and output per rank, all of
 // the inputs' dtype, the full buffers of W * S elements and the shards of S. Returns S, the end of
 // the shard table.
@@ -193,8 +234,10 @@ uint64_t check_sharded_simulate(ShardedOp op, const std::vector<at::Tensor>& inp
 void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                                 const std::vector<LayerTuple>& shard_layers, int lanes, bool average,
                                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                                int64_t min_lane_elems, std::optional<double> prescale) {
+                                int64_t min_lane_elems, std::optional<double> prescale,
+                                const std::optional<A2aBitsArg>& bits) {
   const auto shard = to_layers(shard_layers);
+  const WireCodec codec = sharded_codec(bits, shard, stochastic, "reduce_scatter");
   const uint64_t S = check_sharded_simulate(ShardedOp::kReduceScatter, inputs, outputs, shard);
   const int W = (int)inputs.size();
   const int dt = cgx_dtype(inputs[0]);
@@ -205,7 +248,8 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
     out.push_back(outputs[r].data_ptr());
   }
   Plan plan = build_plan(replicate(shard, W, S), make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
-  reduce_scatter_simulate(plan, in, out, S, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
+  reduce_scatter_simulate(plan, in, out, S, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq),
+                          codec);
 }
 
 // All-gather oracle (ag_kernel): shard q is one quantization round trip (roundtrip_simulate) of
@@ -214,8 +258,9 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
 // gets the same bytes.
 void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                             const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed,
-                            uint32_t seq) {
+                            uint32_t seq, const std::optional<A2aBitsArg>& bits) {
   const auto shard = to_layers(shard_layers);
+  const WireCodec codec = sharded_codec(bits, shard, stochastic, "all_gather");
   const uint64_t S = check_sharded_simulate(ShardedOp::kAllGather, inputs, outputs, shard);
   const int W = (int)inputs.size();
   const int dt = cgx_dtype(inputs[0]);
@@ -227,7 +272,7 @@ void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
     const std::vector<LayerSpec> copy(layers.begin() + (ptrdiff_t)(q * per_copy),
                                       layers.begin() + (ptrdiff_t)((q + 1) * per_copy));
     roundtrip_simulate(build_plan(copy, make_opts(1, 1, dt, false, 1 << 30)), out0, 1.0f,
-                       make_rng(stochastic, seed, seq), q, 1);
+                       make_rng(stochastic, seed, seq), q, 1, codec);
   }
   for (int r = 1; r < W; ++r) std::memcpy(outputs[r].data_ptr(), out0, S * W * es);
 }
@@ -268,31 +313,6 @@ void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<
     TORCH_CHECK((uint64_t)inputs[r].numel() == nin && (uint64_t)outputs[r].numel() == nout,
                 "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
   }
-}
-
-// The `bits` of every all-to-all binding: 1..8 or 32 (max-min levels, or raw), or the name of an FP8
-// wire codec, which travels in 8-bit records and rounds to nearest only. Integers are checked where
-// they are used, as before; an unknown name, or an FP8 codec with stochastic rounding, raises
-// ValueError before anything runs.
-using A2aBitsArg = std::variant<int64_t, std::string>;
-struct A2aBits {
-  int bits;
-  WireCodec codec;
-};
-A2aBits a2a_bits(const A2aBitsArg& arg, bool stochastic) {
-  const std::string* name = std::get_if<std::string>(&arg);
-  if (name == nullptr) return {(int)std::get<int64_t>(arg), kMaxMin};
-  WireCodec codec;
-  if (*name == "e4m3")
-    codec = kE4M3;
-  else if (*name == "e5m2")
-    codec = kE5M2;
-  else
-    throw py::value_error("cgx all_to_all: bits must be 1..8, 32, \"e4m3\" or \"e5m2\", got \"" + *name + "\"");
-  if (stochastic)
-    throw py::value_error("cgx all_to_all: bits=\"" + *name +
-                          "\" rounds to nearest only; stochastic rounding needs integer bits");
-  return {8, codec};
 }
 
 void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
@@ -551,15 +571,18 @@ class LocalSraGroup {
   }
 
   // reduce-scatter: inputs[r] holds W * S elements of virtual rank r, outputs[r] receives shard r
+  // (`bits`: sharded_codec)
   void reduce_scatter(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                       const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete,
-                      bool stochastic, uint64_t seed, uint32_t seq) {
-    sharded(ShardedOp::kReduceScatter, inputs, outputs, shard_layers, average, skip_incomplete, stochastic, seed, seq);
+                      bool stochastic, uint64_t seed, uint32_t seq, const std::optional<A2aBitsArg>& bits) {
+    sharded(ShardedOp::kReduceScatter, inputs, outputs, shard_layers, average, skip_incomplete, stochastic, seed, seq,
+            bits);
   }
   // all-gather: inputs[r] holds virtual rank r's shard of S elements, outputs[r] receives W * S
   void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
-                  const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq) {
-    sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq);
+                  const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq,
+                  const std::optional<A2aBitsArg>& bits) {
+    sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq, bits);
   }
   // all-to-all: counts[q][r] elements go from virtual rank q to r; inputs[r] holds row r of the
   // matrix in destination order, outputs[r] receives column r in source order.
@@ -659,8 +682,9 @@ class LocalSraGroup {
 
   void sharded(ShardedOp op, std::vector<at::Tensor>& inputs, std::vector<at::Tensor>& outputs,
                const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete, bool stochastic,
-               uint64_t seed, uint32_t seq) {
+               uint64_t seed, uint32_t seq, const std::optional<A2aBitsArg>& bits) {
     const bool rs = op == ShardedOp::kReduceScatter;
+    const WireCodec codec = sharded_codec(bits, to_layers(shard_layers), stochastic, op_name(op));
     TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_,
                 "need one input and one output per virtual rank");
     const int dt = cgx_dtype(inputs[0]);
@@ -681,7 +705,8 @@ class LocalSraGroup {
     fork_join([&](int r) { fused_[r]->prepare_sharded(specs, dt, skip_incomplete, streams_[r].stream()); },
               [&](int r) {
                 fused_[r]->sharded(op, specs, dt, skip_incomplete, inputs[r].data_ptr(), outputs[r].data_ptr(),
-                                   (uint64_t)(rs ? outputs[r] : inputs[r]).numel(), ps, rng, streams_[r].stream());
+                                   (uint64_t)(rs ? outputs[r] : inputs[r]).numel(), ps, rng, streams_[r].stream(), 0,
+                                   nullptr, codec);
               });
   }
 
@@ -738,24 +763,27 @@ class LocalReducerGroup {
   // Reducer::reduce_scatter: inputs[r] holds W * S elements, outputs[r] receives shard r
   void reduce_scatter(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                       const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete,
-                      bool stochastic, uint64_t seed, uint32_t seq, std::optional<double> prescale_in) {
+                      bool stochastic, uint64_t seed, uint32_t seq, std::optional<double> prescale_in,
+                      const std::optional<A2aBitsArg>& bits) {
     const auto specs = to_layers(shard_layers);
+    const WireCodec codec = sharded_codec(bits, specs, stochastic, "reduce_scatter");
     const RngParams rng = make_rng(stochastic, seed, seq);
     const float prescale = sim_prescale(prescale_in, average, hub_.world());
     check_outputs(inputs, outputs, true);
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
-      red.reduce_scatter(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, prescale, rng, s);
+      red.reduce_scatter(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, prescale, rng, s, codec);
     });
   }
   // Reducer::all_gather: inputs[r] holds rank r's shard of S elements, outputs[r] receives W * S
   void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                   const std::vector<LayerTuple>& shard_layers, bool skip_incomplete, bool stochastic, uint64_t seed,
-                  uint32_t seq) {
+                  uint32_t seq, const std::optional<A2aBitsArg>& bits) {
     const auto specs = to_layers(shard_layers);
+    const WireCodec codec = sharded_codec(bits, specs, stochastic, "all_gather");
     const RngParams rng = make_rng(stochastic, seed, seq);
     check_outputs(inputs, outputs, false);
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
-      red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s);
+      red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s, codec);
     });
   }
   // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
@@ -1020,12 +1048,21 @@ class LocalEngineGroup {
   // inputs[r] / outputs[r]: rank r's buffers of the reduce-scatter (W * S -> S) or the all-gather
   // (S -> W * S); `shard_layers` is one shard's table, by default one layer of S elements with the
   // environment's width and bucket size. Host tensors run the generic reducers (no heaps). The
-  // all-gather runs without skip_incomplete, as the process group's does.
+  // all-gather runs without skip_incomplete, as the process group's does. `bits`, when given,
+  // replaces the environment's width: an integer, or an FP8 format name (a2a_bits; the table's
+  // layers then need bits 8 or 32).
   void sharded(bool reduce_scatter, std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, bool average,
-               const std::optional<std::vector<LayerTuple>>& shard_layers) {
+               const std::optional<std::vector<LayerTuple>>& shard_layers, const std::optional<A2aBitsArg>& bits) {
     const ShardedOp op = reduce_scatter ? ShardedOp::kReduceScatter : ShardedOp::kAllGather;
     TORCH_CHECK((int)outputs.size() == world_, "LocalEngineGroup: one output per virtual rank");
-    const CompressionEnv env = CompressionEnv::read();
+    CompressionEnv env = CompressionEnv::read();
+    WireCodec codec = kMaxMin;
+    if (bits) {
+      const A2aBits wb = a2a_bits(*bits, env.stochastic, op_name(op));
+      env.bits = wb.bits;
+      codec = sharded_codec(bits, shard_layers ? to_layers(*shard_layers) : std::vector<LayerSpec>{},
+                            env.stochastic, op_name(op));
+    }
     const bool skip = reduce_scatter && env.skip_incomplete;
     RngParams rng = make_rng(env.stochastic, env.seed, 0);
     const std::vector<LayerSpec> given = shard_layers ? to_layers(*shard_layers) : std::vector<LayerSpec>{};
@@ -1046,7 +1083,7 @@ class LocalEngineGroup {
         intra_hub(r)->barrier(e.local_rank());
       }
       e.sharded(cuda, op, in, outputs[r].data_ptr(), staging.defined() ? staging.data_ptr() : nullptr, dt, S, table,
-                average, skip, rng, s, false);
+                average, skip, rng, s, false, codec);
       // the staging buffer is freed on the caller's stream when this returns: let its work finish first
       if (staging.defined() && cuda) cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: sharded call");
     });
@@ -1445,21 +1482,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("allreduce_bucket", &ProcessGroupCGX::allreduce_bucket, py::arg("tensor"), py::arg("bucket_idx"),
            py::arg("average") = false, py::call_guard<py::gil_scoped_release>())
       .def("reduce_scatter_compressed",
-           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, bool average, int bits, int bucket_size,
-              bool skip_incomplete, bool stochastic, int64_t seed, bool overlapped,
+           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, bool average, const A2aBitsArg& bits,
+              int bucket_size, bool skip_incomplete, bool stochastic, int64_t seed, bool overlapped,
               const std::vector<LayerTuple>& layers) {
-             return pg.sharded_compressed(ShardedOp::kReduceScatter, out, in, average, bits, bucket_size,
-                                          skip_incomplete, stochastic, seed, overlapped, to_layers(layers));
+             const auto table = to_layers(layers);
+             const A2aBits wb = a2a_bits(bits, stochastic, "reduce_scatter");
+             sharded_codec(bits, table, stochastic, "reduce_scatter");
+             return pg.sharded_compressed(ShardedOp::kReduceScatter, out, in, average, wb.bits, wb.codec, bucket_size,
+                                          skip_incomplete, stochastic, seed, overlapped, table);
            },
            py::arg("output"), py::arg("input"), py::arg("average") = false, py::arg("bits") = 4,
            py::arg("bucket_size") = 512, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = -1, py::arg("overlapped") = false, py::arg("layers") = std::vector<LayerTuple>{},
            py::call_guard<py::gil_scoped_release>())
       .def("all_gather_compressed",
-           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, int bits, int bucket_size, bool stochastic,
-              int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers) {
-             return pg.sharded_compressed(ShardedOp::kAllGather, out, in, false, bits, bucket_size, false,
-                                          stochastic, seed, overlapped, to_layers(layers));
+           [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const A2aBitsArg& bits, int bucket_size,
+              bool stochastic, int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers) {
+             const auto table = to_layers(layers);
+             const A2aBits wb = a2a_bits(bits, stochastic, "all_gather");
+             sharded_codec(bits, table, stochastic, "all_gather");
+             return pg.sharded_compressed(ShardedOp::kAllGather, out, in, false, wb.bits, wb.codec, bucket_size, false,
+                                          stochastic, seed, overlapped, table);
            },
            py::arg("output"), py::arg("input"), py::arg("bits") = 4, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("overlapped") = false,
@@ -1647,17 +1690,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
         py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048,
-        py::arg("prescale") = py::none());
+        py::arg("prescale") = py::none(), py::arg("bits") = py::none());
   m.def("all_to_all_simulate", &py_all_to_all_simulate, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
         py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
         py::arg("seq") = 0);
   m.def(
       "a2a_bits",
-      [](const A2aBitsArg& bits, bool stochastic) {
-        const A2aBits wb = a2a_bits(bits, stochastic);
+      [](const A2aBitsArg& bits, bool stochastic, const std::string& op) {
+        const A2aBits wb = a2a_bits(bits, stochastic, op.c_str());
         return std::make_tuple(wb.bits, (int)wb.codec);
       },
-      py::arg("bits"), py::arg("stochastic") = false);
+      py::arg("bits"), py::arg("stochastic") = false, py::arg("op") = "all_to_all");
   m.def("a2a_items", &py_a2a_items, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
   m.def(
       "a2a_rows_fit",
@@ -1668,7 +1711,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("a2a_windows", &py_a2a_windows, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype"),
         py::arg("slot_bytes"), py::arg("lanes"));
   m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
-        py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0);
+        py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0,
+        py::arg("bits") = py::none());
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
@@ -1760,9 +1804,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("seed") = 0, py::arg("seq") = 0)
       .def("reduce_scatter", &LocalSraGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
-           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("all_gather", &LocalSraGroup::all_gather, py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers"),
-           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0)
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
@@ -1785,13 +1829,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("seq") = 0)
       .def("reduce_scatter", &LocalReducerGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
-           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none())
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none(),
+           py::arg("bits") = py::none())
       .def("all_to_all", &LocalReducerGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0)
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-           py::arg("seed") = 0, py::arg("seq") = 0)
+           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("bytes_sent", &LocalReducerGroup::bytes_sent)
       .def("num_plans", &LocalReducerGroup::num_plans, py::arg("rank"))
       .def("plan_uploads", &LocalReducerGroup::plan_uploads, py::arg("rank"))
@@ -1806,16 +1851,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("average") = false)
       .def("reduce_scatter",
            [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out, bool average,
-              std::optional<std::vector<LayerTuple>> shard_layers) {
-             g.sharded(true, std::move(in), std::move(out), average, shard_layers);
+              std::optional<std::vector<LayerTuple>> shard_layers, std::optional<A2aBitsArg> bits) {
+             g.sharded(true, std::move(in), std::move(out), average, shard_layers, bits);
            },
-           py::arg("inputs"), py::arg("outputs"), py::arg("average") = false, py::arg("shard_layers") = py::none())
+           py::arg("inputs"), py::arg("outputs"), py::arg("average") = false, py::arg("shard_layers") = py::none(),
+           py::arg("bits") = py::none())
       .def("all_gather",
            [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out,
-              std::optional<std::vector<LayerTuple>> shard_layers) {
-             g.sharded(false, std::move(in), std::move(out), false, shard_layers);
+              std::optional<std::vector<LayerTuple>> shard_layers, std::optional<A2aBitsArg> bits) {
+             g.sharded(false, std::move(in), std::move(out), false, shard_layers, bits);
            },
-           py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none())
+           py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none(), py::arg("bits") = py::none())
       .def("stats", &LocalEngineGroup::stats, py::arg("rank"))
       .def("check", &LocalEngineGroup::check)
       .def("log", &LocalEngineGroup::log, py::arg("rank"))

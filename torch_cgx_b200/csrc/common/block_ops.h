@@ -238,6 +238,24 @@ inline void decode_block_fp8_store(const uint8_t* rec, int dtype, const BlockDes
   }
 }
 
+// acc[i] = fl(acc[i] + fl(float(code) * unit)): the reduce-scatter's accumulation of an FP8 record
+inline void decode_block_fp8_add(const uint8_t* rec, const BlockDesc& d, float* acc, int codec) {
+  const uint32_t n = block_n(d);
+  const uint32_t B = d.bucket;
+  const uint32_t nb = block_num_buckets(n, B);
+  const uint32_t gpb = bucket_groups(B);
+  const BucketMeta* meta = reinterpret_cast<const BucketMeta*>(rec);
+  const uint8_t* pay = rec + block_meta_bytes(n, B);
+  for (uint32_t b = 0; b < nb; ++b) {
+    const uint32_t lo = b * B, hi = lo + B < n ? lo + B : n;
+    const uint8_t* src = pay + (size_t)b * gpb * 8u;
+    for (uint32_t i = lo; i < hi; ++i) {
+      const float v = acc[i] + fp8_decode(src[i - lo], meta[b].unit, codec);
+      acc[i] = v == v ? v : canonical_nan();
+    }
+  }
+}
+
 inline void decode_block_add(const uint8_t* rec, int dtype, const BlockDesc& d, float* acc) {
   decode_block_foreach(rec, dtype, d, [&](uint32_t i, float v) { acc[i] += v; });
 }

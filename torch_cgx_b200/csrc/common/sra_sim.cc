@@ -32,7 +32,7 @@ void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float presca
 
 void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& in_bufs,
                              const std::vector<void*>& out_bufs, uint64_t shard, float prescale,
-                             const RngParams& rng) {
+                             const RngParams& rng, WireCodec codec) {
   const int W = plan.world;
   if ((int)in_bufs.size() != W || (int)out_bufs.size() != W)
     throw std::invalid_argument("reduce_scatter_simulate: need one input and one output per rank");
@@ -45,6 +45,11 @@ void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& i
       for (int q = 0; q < W; ++q) {
         if (q == c) continue;
         cpu::load_block(in_bufs[q], plan.dtype, d, prescale, tmp.data());
+        if (codec != kMaxMin && block_bits(d) < kRawBits) {
+          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+          cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
+          continue;
+        }
         cpu::quantize_block(tmp.data(), plan.dtype, d, rec.data(), make_rng_key(rng, q, 0), b);
         cpu::decode_block_add(rec.data(), plan.dtype, d, acc.data());
       }
@@ -121,12 +126,18 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
   }
 }
 
-void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngParams& rng, int rank, int phase) {
+void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngParams& rng, int rank, int phase,
+                        WireCodec codec) {
   std::vector<float> acc(kMaxBlockElems);
   std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
   for (uint32_t b = 0; b < plan.blocks.size(); ++b) {
     const BlockDesc& d = plan.blocks[b];
     cpu::load_block(buf, plan.dtype, d, prescale, acc.data());
+    if (codec != kMaxMin && block_bits(d) < kRawBits) {
+      cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+      cpu::decode_block_fp8_store(rec.data(), plan.dtype, d, buf, codec);
+      continue;
+    }
     cpu::quantize_block(acc.data(), plan.dtype, d, rec.data(), make_rng_key(rng, rank, phase), b);
     cpu::decode_block_store(rec.data(), plan.dtype, d, buf);
   }

@@ -42,7 +42,7 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
 // allreduce's phase-B sum (same primitives, order and phase-A RNG streams), not requantized.
 void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& in_bufs,
                              const std::vector<void*>& out_bufs, uint64_t shard, float prescale,
-                             const RngParams& rng);
+                             const RngParams& rng, WireCodec codec = kMaxMin);
 
 // All-to-all oracle (a2a_kernel): counts[q][r] elements go from rank q to rank r. Rank q's chunks
 // lie in in_bufs[q] in destination order, rank r's output holds the chunks in source order. The own
@@ -57,6 +57,9 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
 // Quantize->dequantize round trip of one rank's buffer through the plan's
 // blocks (what a single compression step does to the data); used by the Python
 // ops and the tests.
-void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngParams& rng, int rank, int phase);
+// An FP8 `codec` (8-bit plans) quantizes the compressed blocks with its records (round to nearest);
+// raw blocks are the same either way.
+void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngParams& rng, int rank, int phase,
+                        WireCodec codec = kMaxMin);
 
 }  // namespace cgx

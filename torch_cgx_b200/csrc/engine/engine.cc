@@ -219,7 +219,7 @@ void AllreduceEngine::prepare_sharded(ShardedOp op, const std::vector<LayerSpec>
 
 void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
                                     const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale,
-                                    const RngParams& rng, cudaStream_t stream, bool overlapped) {
+                                    const RngParams& rng, cudaStream_t stream, bool overlapped, WireCodec codec) {
   const bool rs = op == ShardedOp::kReduceScatter;
   if (fused_sharded(cuda)) {
     FusedSra::WindowHook hook;
@@ -229,7 +229,7 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
         observer_->before_fused_launch(dp, stream);
       };
     const FusedSra::RsCounts n = fused_->sharded(op, table, dtype, skip_incomplete, in, out, S, prescale, rng,
-                                                 stream, overlapped ? cfg_.overlap_lanes : 0, hook);
+                                                 stream, overlapped ? cfg_.overlap_lanes : 0, hook, codec);
     stats_.kernel_launches += n.launches;
     stats_.elements += n.elements;
     stats_.wire_bytes += n.wire_bytes;
@@ -240,9 +240,9 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
   const uint64_t before = g.intra->bytes_sent();
   observe(rs ? EngineStage::kGenericRs : EngineStage::kGenericAg, &table, rng, prescale);
   if (rs)
-    g.intra->reduce_scatter(in, out, dtype, table, skip_incomplete, prescale, rng, stream);
+    g.intra->reduce_scatter(in, out, dtype, table, skip_incomplete, prescale, rng, stream, codec);
   else
-    g.intra->all_gather(in, out, dtype, table, skip_incomplete, rng, stream);
+    g.intra->all_gather(in, out, dtype, table, skip_incomplete, rng, stream, codec);
   // the fused kernel's conventions: the elements of the window, the raw bytes a raw exchange would move
   const uint64_t L = (uint64_t)local_size_, es = (uint64_t)dtype_size(dtype);
   stats_.wire_bytes += g.intra->bytes_sent() - before;
@@ -262,14 +262,17 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
 // cross-node stage with call_seq << 4 ^ 0x40000000, the allreduce's cross-node marker.
 void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out, void* staging, int dtype,
                               int64_t shard_numel, const std::vector<LayerSpec>& shard_layers, bool average,
-                              bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped) {
+                              bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped,
+                              WireCodec codec) {
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const int N = nodes(), L = local_size_;
   const std::string title = std::string("cgx: the compressed ") + op_title(op);
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
   if (shard_numel <= 0) return;
-  check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_);
+  check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_, codec);
+  if (codec != kMaxMin && rng_in.stochastic)
+    throw std::invalid_argument(title + ": the FP8 formats round to nearest only");
   if (!fused && (L > 1 || N == 1) && !g.intra)
     throw std::runtime_error(title + (L > 1 ? " has no intra-node reducer" : " of one rank needs the P2P transport"));
   if (N > 1 && !g.cross) throw std::runtime_error(title + ": multi-node topology but no cross-node reducer");
@@ -295,20 +298,21 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
         rng.seq = seq ^ (uint32_t)b;
         NvtxRange r1("cgx:intra_node", (uint64_t)b);
         sharded_intra(cuda, op, at(in, (size_t)b * L * shard_bytes), at(partial, (size_t)b * shard_bytes), dtype, S,
-                      intra_table, skip_incomplete, prescale, rng, stream, overlapped);
+                      intra_table, skip_incomplete, prescale, rng, stream, overlapped, codec);
       }
     if (N == 1) return;
     NvtxRange r2("cgx:cross_node", (uint64_t)N);
     const float cross_scale = L > 1 ? 1.0f : prescale;
     observe(EngineStage::kCrossRs, &shard_layers, crng, cross_scale);
-    g.cross->reduce_scatter(L > 1 ? partial : in, out, dtype, shard_layers, skip_incomplete, cross_scale, crng, stream);
+    g.cross->reduce_scatter(L > 1 ? partial : in, out, dtype, shard_layers, skip_incomplete, cross_scale, crng, stream,
+                            codec);
     return;
   }
   void* gathered = L > 1 ? staging : out;
   if (N > 1) {
     NvtxRange r2("cgx:cross_node", (uint64_t)N);
     observe(EngineStage::kCrossAg, &shard_layers, crng, 1.0f);
-    g.cross->all_gather(in, gathered, dtype, shard_layers, skip_incomplete, crng, stream);
+    g.cross->all_gather(in, gathered, dtype, shard_layers, skip_incomplete, crng, stream, codec);
   }
   if (!intra) return;
   for (int n = 0; n < N; ++n) {
@@ -316,7 +320,7 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
     NvtxRange r1("cgx:intra_node", (uint64_t)n);
     sharded_intra(cuda, op, N > 1 ? at(gathered, (size_t)n * shard_bytes) : in,
                   at(out, (size_t)n * L * shard_bytes), dtype, S, intra_table, skip_incomplete, 1.0f, rng, stream,
-                  overlapped);
+                  overlapped, codec);
   }
 }
 

@@ -162,12 +162,13 @@ accumulate_items_kernel(const uint8_t* __restrict__ wire, const WarpItem* __rest
   }
 }
 
-// The FP8 codecs of an 8-bit plan (the generic all-to-all): wire = quantize(src), dst = decode(wire).
-// Plain T tensors, no prescale, round to nearest; the plan has no raw items.
+// The FP8 codecs of an 8-bit plan (the generic all-to-all, reduce-scatter and all-gather):
+// wire = quantize(src * prescale), dst = decode(wire), acc (+)= decode(wire). Plain T tensors, round
+// to nearest; the items are all compressed (the reducers pass raw layers to the max-min kernels).
 template <typename T, int CODEC, int GPL>
 __global__ void __launch_bounds__(kThreads, 3)
 quantize_items_fp8_kernel(const T* __restrict__ src, const WarpItem* __restrict__ items, uint32_t first,
-                          uint32_t count, uint8_t* wire) {
+                          uint32_t count, uint8_t* wire, float prescale) {
   const OneDst ds{wire};
   CGX_ITEM_LOOP(it) {
     const T* s = src + it.elem_off;
@@ -175,12 +176,13 @@ quantize_items_fp8_kernel(const T* __restrict__ src, const WarpItem* __restrict_
       if (group_aligned<T>(s)) {
         float x[GPL][8];
         slice_load_vec<T, GPL>(s, x);
+        slice_scale<GPL>(x, prescale);
         full_send_fp8_x<CODEC, GPL>(x, it, ds);
       } else {
-        full_send_fp8_unaligned<T, CODEC, GPL>(s, it, ds);
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(s, it, prescale, ds, (T*)nullptr);
       }
     } else {
-      bucket_quantize_fp8<T, CODEC>(s, it, ds);
+      bucket_send_fp8<T, T, CODEC>(s, it, prescale, ds, (T*)nullptr);
     }
   }
 }
@@ -201,6 +203,46 @@ dequantize_items_fp8_kernel(const uint8_t* __restrict__ wire, const WarpItem* __
       }
     } else {
       bucket_recv_fp8<T, CODEC>(wire, it, o);
+    }
+  }
+}
+
+// acc (fp32 scratch) = float(init_src) * prescale   (init_src != nullptr)
+// acc = fl(acc + fl(float(code) * unit))            (wire != nullptr)
+template <typename T, int CODEC, int GPL>
+__global__ void __launch_bounds__(kThreads, 3)
+accumulate_items_fp8_kernel(const uint8_t* __restrict__ wire, const WarpItem* __restrict__ items, uint32_t first,
+                            uint32_t count, float* __restrict__ acc, uint32_t base_elem,
+                            const T* __restrict__ init_src, float prescale) {
+  const SrcSet ss{wire, 0u, 1, -1};
+  CGX_ITEM_LOOP(it) {
+    float* a = acc + (it.elem_off - base_elem);
+    if (item_kind(it) == kItemFull) {
+      float x[GPL][8];
+      if (init_src) {
+        slice_load_scalar<T, GPL>(init_src + it.elem_off, x);
+        slice_scale<GPL>(x, prescale);
+      } else {
+        slice_load_scalar<float, GPL>(a, x);
+      }
+      if (wire) slice_accumulate_fp8<CODEC, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), x);
+      slice_store<float, GPL, false>(a, x);
+    } else {
+      const uint32_t n = item_n(it);
+      const uint32_t ng = div_up(n, 8u);
+      for (uint32_t g = lane_id(); g < ng; g += 32) {
+        const int nv = (int)min(8u, n - g * 8u);
+        float x[8];
+        if (init_src) {
+          load8_scalar<T>(init_src + it.elem_off + g * 8u, nv, x);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) x[j] = __fmul_rn(x[j], prescale);
+        } else {
+          load8_scalar<float>(a + g * 8u, nv, x);
+        }
+        if (wire) bucket_add_sources_fp8<CODEC>(ss, it, g, x);
+        store8_scalar<float>(a + g * 8u, nv, x);
+      }
     }
   }
 }
@@ -295,11 +337,12 @@ cudaError_t dequantize_t(const ItemKernelArgs& a, const uint8_t* wire, T* dst, c
   } while (0)
 
 template <typename T>
-cudaError_t quantize_fp8_t(const ItemKernelArgs& a, const T* src, uint8_t* wire, cudaStream_t stream) {
+cudaError_t quantize_fp8_t(const ItemKernelArgs& a, const T* src, uint8_t* wire, float prescale,
+                           cudaStream_t stream) {
   if (a.count == 0) return cudaSuccess;
   const int grid = grid_for(a.count);
 #define CGX_CALL(C_, GPL_) \
-  quantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(src, a.items, a.first, a.count, wire)
+  quantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(src, a.items, a.first, a.count, wire, prescale)
   CGX_DISPATCH_FP8(a, CGX_CALL);
 #undef CGX_CALL
   return cudaGetLastError();
@@ -311,6 +354,19 @@ cudaError_t dequantize_fp8_t(const ItemKernelArgs& a, const uint8_t* wire, T* ds
   const int grid = grid_for(a.count);
 #define CGX_CALL(C_, GPL_) \
   dequantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(wire, a.items, a.first, a.count, dst)
+  CGX_DISPATCH_FP8(a, CGX_CALL);
+#undef CGX_CALL
+  return cudaGetLastError();
+}
+
+template <typename T>
+cudaError_t accumulate_fp8_t(const ItemKernelArgs& a, const uint8_t* wire, float* acc, uint32_t base_elem,
+                             const T* init_src, float prescale, cudaStream_t stream) {
+  if (a.count == 0) return cudaSuccess;
+  const int grid = grid_for(a.count);
+#define CGX_CALL(C_, GPL_)                                                                                \
+  accumulate_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(wire, a.items, a.first, a.count, acc, \
+                                                                          base_elem, init_src, prescale)
   CGX_DISPATCH_FP8(a, CGX_CALL);
 #undef CGX_CALL
   return cudaGetLastError();
@@ -342,10 +398,10 @@ cudaError_t accumulate_t(const ItemKernelArgs& a, const uint8_t* wire, float* ac
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,
                                   const RngKey& rng, cudaStream_t stream) {
   if (a.codec != kMaxMin) {
-    if (prescale != 1.0f || rng.enabled) return cudaErrorInvalidValue;
-    CGX_BY_DTYPE(a.dtype, (quantize_fp8_t<float>(a, (const float*)src, wire, stream)),
-                 (quantize_fp8_t<__half>(a, (const __half*)src, wire, stream)),
-                 (quantize_fp8_t<__nv_bfloat16>(a, (const __nv_bfloat16*)src, wire, stream)))
+    if (rng.enabled) return cudaErrorInvalidValue;
+    CGX_BY_DTYPE(a.dtype, (quantize_fp8_t<float>(a, (const float*)src, wire, prescale, stream)),
+                 (quantize_fp8_t<__half>(a, (const __half*)src, wire, prescale, stream)),
+                 (quantize_fp8_t<__nv_bfloat16>(a, (const __nv_bfloat16*)src, wire, prescale, stream)))
   }
   CGX_BY_DTYPE(a.dtype,
                (quantize_t<float, float>(a, (const float*)src, 0, wire, prescale, rng, nullptr, stream)),
@@ -375,7 +431,12 @@ cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire
 cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* wire, float* acc_f32,
                                         uint32_t base_elem, const void* init_src, float prescale,
                                         cudaStream_t stream) {
-  if (a.codec != kMaxMin) return cudaErrorInvalidValue;
+  if (a.codec != kMaxMin)
+    CGX_BY_DTYPE(a.dtype,
+                 (accumulate_fp8_t<float>(a, wire, acc_f32, base_elem, (const float*)init_src, prescale, stream)),
+                 (accumulate_fp8_t<__half>(a, wire, acc_f32, base_elem, (const __half*)init_src, prescale, stream)),
+                 (accumulate_fp8_t<__nv_bfloat16>(a, wire, acc_f32, base_elem, (const __nv_bfloat16*)init_src,
+                                                  prescale, stream)))
   CGX_BY_DTYPE(a.dtype, (accumulate_t<float>(a, wire, acc_f32, base_elem, (const float*)init_src, prescale, stream)),
                (accumulate_t<__half>(a, wire, acc_f32, base_elem, (const __half*)init_src, prescale, stream)),
                (accumulate_t<__nv_bfloat16>(a, wire, acc_f32, base_elem, (const __nv_bfloat16*)init_src, prescale,

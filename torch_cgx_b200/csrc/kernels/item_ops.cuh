@@ -861,14 +861,14 @@ __device__ __forceinline__ void fp8_decode8(uint32_t lo, uint32_t hi, float unit
   fp8x2_decode(hi >> 16, unit, CODEC, x[6], x[7]);
 }
 
-// full item, values already in registers: meta + codes to the destination
+// full item, values already in registers: meta + codes to the destination; the codes stay in
+// (lo, hi) and the units in m for a caller that decodes them itself
 template <int CODEC, int GPL, typename DST>
-__device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds) {
+__device__ __forceinline__ void full_send_fp8_codes(const float (&x)[GPL][8], const WarpItem& it, const DST& ds,
+                                                    BucketMeta (&m)[GPL], uint32_t (&lo)[GPL], uint32_t (&hi)[GPL]) {
   const uint32_t lg = item_lpb_log2(it);
   float mn[GPL], mx[GPL];
   slice_minmax<GPL>(x, lg, mn, mx);
-  BucketMeta m[GPL];
-  uint32_t lo[GPL], hi[GPL];
 #pragma unroll
   for (int k = 0; k < GPL; ++k) {
     m[k] = fp8_meta(mn[k], mx[k], CODEC);
@@ -876,6 +876,12 @@ __device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const 
   }
   slice_store_meta<GPL>(m, lg, ds, it.meta_off);
   store_words<8, GPL>(ds, it.pay_off, 8, lo, hi);
+}
+template <int CODEC, int GPL, typename DST>
+__device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds) {
+  BucketMeta m[GPL];
+  uint32_t lo[GPL], hi[GPL];
+  full_send_fp8_codes<CODEC, GPL>(x, it, ds, m, lo, hi);
 }
 template <typename TS, int CODEC, int GPL, typename DST>
 __device__ __noinline__ void full_send_fp8_unaligned(const TS* __restrict__ src, const WarpItem it, const DST ds) {
@@ -901,15 +907,17 @@ __device__ __noinline__ void full_recv_fp8_unaligned(const uint8_t* rec, const W
 
 // generic bucket item (cold): ONE bucket of n <= kMaxBlockElems elements, any alignment; the codes
 // of the last group's missing elements are 0, as on the host
-template <typename TS, int CODEC, typename DST>
-__device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const DST ds) {
+// of the values src * prescale; self_out != nullptr: also the values decoded from the codes there
+template <typename TS, typename TO, int CODEC, typename DST>
+__device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, const WarpItem& it, float prescale,
+                                                const DST& ds, TO* __restrict__ self_out) {
   const uint32_t n = item_n(it);
   const uint32_t ng = div_up(n, 8u);
   float mn = CGX_INF_POS, mx = CGX_INF_NEG;
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, 1.0f, x, nv);
+    bucket_load_group<TS>(src, g, n, prescale, x, nv);
     minmax8_pred(x, nv, mn, mx);
   }
   warp_minmax(mn, mx);
@@ -920,13 +928,22 @@ __device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, con
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, 1.0f, x, nv);
+    bucket_load_group<TS>(src, g, n, prescale, x, nv);
     uint32_t lo, hi;
     fp8_encode8<CODEC>(x, inv, lo, hi);
     const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
     const uint32_t o = it.pay_off + g * 8u;
     for (int t = 0; t < 8; ++t) dst_st_u8(du, o + t, (uint32_t)(w >> (8 * t)) & 0xFFu);
+    if (self_out != nullptr) {
+      float dec[8];
+      fp8_decode8<CODEC>(lo, hi, m.unit, dec);
+      store8_scalar<TO>(self_out + g * 8u, nv, dec);
+    }
   }
+}
+template <typename TS, int CODEC, typename DST>
+__device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const DST ds) {
+  bucket_fp8_body<TS, float, CODEC>(src, it, 1.0f, ds, (float*)nullptr);
 }
 
 template <typename TO, int CODEC>
@@ -940,6 +957,119 @@ __device__ __noinline__ void bucket_recv_fp8(const uint8_t* rec, const WarpItem 
     float x[8];
     fp8_decode8<CODEC>(lo, hi, unit, x);
     store8_scalar<TO>(out + g * 8u, (int)min(8u, n - g * 8u), x);
+  }
+}
+
+// ======================================================================================
+// FP8 in the sharded collectives (rs_kernel, ag_kernel and the generic reducers' item kernels).
+// The sender prescales, then encodes as above; the all-gather's owner writes what every receiver
+// decodes from the same codes; the reduce-scatter's owner adds each source's decoded value,
+// fl(float(code) * unit), to its fp32 accumulator with a separate rounding (no FMA), in slot order.
+// ======================================================================================
+// full item, values in registers and already prescaled: publish meta + codes, and the decoded
+// values to `out` (VEC: group aligned)
+template <typename TO, int CODEC, int GPL, bool VEC, typename DST>
+__device__ __forceinline__ void full_publish_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds,
+                                                   TO* __restrict__ out) {
+  BucketMeta m[GPL];
+  uint32_t lo[GPL], hi[GPL];
+  full_send_fp8_codes<CODEC, GPL>(x, it, ds, m, lo, hi);
+  float d[GPL][8];
+#pragma unroll
+  for (int k = 0; k < GPL; ++k) fp8_decode8<CODEC>(lo[k], hi[k], m[k].unit, d[k]);
+  slice_store<TO, GPL, VEC>(out, d);
+}
+// unaligned full item of src * prescale; SELF: also the decoded values to `self_out`
+template <typename TS, typename TO, int CODEC, int GPL, bool SELF, typename DST>
+__device__ __noinline__ void full_send_fp8_scaled_unaligned(const TS* __restrict__ src, const WarpItem it,
+                                                            float prescale, const DST ds, TO* __restrict__ self_out) {
+  float x[GPL][8];
+  slice_load_scalar<TS, GPL>(src, x);
+  slice_scale<GPL>(x, prescale);
+  if (SELF)
+    full_publish_fp8_x<TO, CODEC, GPL, false>(x, it, ds, self_out);
+  else
+    full_send_fp8_x<CODEC, GPL>(x, it, ds);
+}
+// generic bucket item of src * prescale; self_out != nullptr: also the decoded values there
+template <typename TS, typename TO, int CODEC, typename DST>
+__device__ __noinline__ void bucket_send_fp8(const TS* __restrict__ src, const WarpItem it, float prescale,
+                                             const DST ds, TO* __restrict__ self_out) {
+  bucket_fp8_body<TS, TO, CODEC>(src, it, prescale, ds, self_out);
+}
+
+// x = fl(x + fl(float(code) * unit)) for every source of the set, in slot order; the words of
+// several sources are in flight at once, as in slice_accumulate
+template <int CODEC, int GPL>
+__device__ __forceinline__ void slice_accumulate_fp8(const SrcSet& ss, uint32_t meta_off, uint32_t pay_off,
+                                                     uint32_t lg, float (&x)[GPL][8]) {
+  const int cnt = ss.n - (ss.skip >= 0 ? 1 : 0);
+  constexpr int kB = GPL == 4 ? 2 : 4;
+  for (int i0 = 0; i0 < cnt; i0 += kB) {
+    SliceWords<GPL> w[kB];
+#pragma unroll
+    for (int u = 0; u < kB; ++u) {
+      // past the end: re-read the last source (its value is not added)
+      const int i = min(i0 + u, cnt - 1);
+      const int q = (ss.skip >= 0 && i >= ss.skip) ? i + 1 : i;
+      slice_fetch<8, GPL>(ss.base + (size_t)q * ss.stride, meta_off, pay_off, lg, 8, w[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < kB; ++u) {
+      if (i0 + u < cnt) {
+#pragma unroll
+        for (int k = 0; k < GPL; ++k) {
+          float d[8];
+          fp8_decode8<CODEC>(w[u].lo[k], w[u].hi[k], w[u].pm[k].unit, d);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) x[k][j] = __fadd_rn(x[k][j], d[j]);
+        }
+      }
+    }
+  }
+}
+
+// reduce-scatter of a full item: my values * prescale + the decoded sources -> out (as full_rs_x)
+template <typename T, int CODEC, int GPL, bool VEC>
+__device__ __forceinline__ void full_rs_fp8_x(float (&x)[GPL][8], const WarpItem& it, float prescale,
+                                              const SrcSet& ss, T* out) {
+  slice_scale<GPL>(x, prescale);
+  slice_accumulate_fp8<CODEC, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), x);
+  slice_store<T, GPL, VEC>(out, x);
+}
+template <typename T, int CODEC, int GPL>
+__device__ __noinline__ void full_rs_fp8_unaligned(const T* src, const WarpItem it, float prescale, const SrcSet ss,
+                                                   T* out) {
+  float x[GPL][8];
+  slice_load_scalar<T, GPL>(src, x);
+  full_rs_fp8_x<T, CODEC, GPL, false>(x, it, prescale, ss, out);
+}
+
+// x[8] of group g += the decoded values of every source of the set (slot order)
+template <int CODEC>
+__device__ __forceinline__ void bucket_add_sources_fp8(const SrcSet& ss, const WarpItem& it, uint32_t g,
+                                                       float (&x)[8]) {
+  for (int q = 0; q < ss.n; ++q) {
+    if (q == ss.skip) continue;
+    const uint8_t* rec = ss.base + (size_t)q * ss.stride;
+    uint32_t lo, hi;
+    load_word<0>(rec + it.pay_off, g, 8, lo, hi);
+    float d[8];
+    fp8_decode8<CODEC>(lo, hi, __uint_as_float(ld_sys_v2(rec + it.meta_off).x), d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) x[j] = __fadd_rn(x[j], d[j]);
+  }
+}
+template <typename T, int CODEC>
+__device__ __noinline__ void bucket_rs_fp8(const T* src, const WarpItem it, float prescale, const SrcSet ss, T* out) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<T>(src, g, n, prescale, x, nv);
+    bucket_add_sources_fp8<CODEC>(ss, it, g, x);
+    store8_scalar<T>(out + g * 8u, nv, x);
   }
 }
 

@@ -55,6 +55,8 @@ struct SraParams {
   uint64_t out_shift;            // reduce-scatter: element of `data` that lands on out[0];
                                  // all-gather: element of `out` that data[0] lands on (rank * shard stride)
   int gather;                    // with `out`: 1 = all-gather, 0 = reduce-scatter
+  int codec;                     // WireCodec of the reduce-scatter / all-gather (common/quant_math.h); an FP8
+                                 // codec needs uniform_bits 8
 };
 
 constexpr int kSraThreads = 256;
@@ -126,8 +128,8 @@ struct ItemKernelArgs {
   int dtype;
   int slice_elems;
   int uniform_bits;
-  int codec = 0;  // WireCodec: an FP8 codec needs an 8-bit plan and is supported by launch_quantize_items
-                  // (prescale 1, deterministic rounding) and launch_dequantize_items only
+  int codec = 0;  // WireCodec: an FP8 codec needs an 8-bit plan whose items [first, first+count) are all
+                  // compressed, and deterministic rounding; launch_quantize_items_f32 does not take one
 };
 // wire = quantize(src[T] * prescale)
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,
@@ -140,6 +142,7 @@ cudaError_t launch_quantize_items_f32(const ItemKernelArgs& a, const float* src_
 cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire, void* dst, cudaStream_t stream);
 // acc_f32[elem_off - base_elem + i] = float(init_src[elem_off + i]) * prescale   (init_src != nullptr)
 // acc_f32[...] += decode(wire)                                                   (wire != nullptr)
+// (an FP8 codec adds fl(float(code) * unit), a separate rounding)
 cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* wire, float* acc_f32,
                                         uint32_t base_elem, const void* init_src, float prescale,
                                         cudaStream_t stream);

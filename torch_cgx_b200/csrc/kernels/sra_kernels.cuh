@@ -221,8 +221,8 @@ __device__ __forceinline__ RngKey phase_rng(const SraParams& p, uint32_t epoch, 
 // ---- phase A: my copy of every other chunk -> its owner. The items of all destinations are dealt
 // round-robin to the warps; each warp takes them two at a time (ILP) and pulls the pair after that
 // towards L2. With the in-switch reduction the full raw items of ALL chunks (mine included) are
-// staged locally.
-template <typename T, int KB, int GPL>
+// staged locally. CODEC: the wire codec of the compressed items (the reduce-scatter's FP8 forms).
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __device__ __forceinline__ void sra_phase_a(const SraParams& p, const LaneItems& li, uint32_t epoch, int stage) {
   const int r = p.rank, W = p.world;
   const int seg0 = stage * W;
@@ -249,6 +249,21 @@ __device__ __forceinline__ void sra_phase_a(const SraParams& p, const LaneItems&
       if (cs == 0) return;  // my own chunk: nothing else to send
     }
     const OneDst push{p.recv1[dstp] + (size_t)r * p.slot_bytes};
+    if constexpr (CODEC != kMaxMin) {
+      if (hot == 1) {
+        slice_scale<GPL>(x, p.prescale);
+        full_send_fp8_x<CODEC, GPL>(x, it, push);
+        return;
+      }
+      if (kind == kItemFull) {
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, push, (T*)nullptr);
+        return;
+      }
+      if (kind == kItemBucket) {
+        bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, push, (T*)nullptr);
+        return;
+      }
+    }
     if (hot == 1)
       full_send_x<T, KB, GPL, false, true>(x, it, p.prescale, rng, push, (T*)nullptr);
     else if (hot == 2)
@@ -281,7 +296,7 @@ __device__ __forceinline__ void sra_phase_a(const SraParams& p, const LaneItems&
       }
     }
     bool done = false;
-    if (hota == 1 && hotb == 1 && !(p.mc_reduce && sa == seg0)) {
+    if (CODEC == kMaxMin && hota == 1 && hotb == 1 && !(p.mc_reduce && sa == seg0)) {
       const OneDst pa{p.recv1[(r + sa - seg0) % W] + (size_t)r * p.slot_bytes};
       const OneDst pb{p.recv1[(r + sb - seg0) % W] + (size_t)r * p.slot_bytes};
       done = full_send_pair<KB, GPL>(xa, xb, ita, itb, p.prescale, rng, pa, pb);
@@ -341,8 +356,8 @@ __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems&
 // packed words of the NEXT two already in flight.
 // AG (the all-gather's decode): the chunks arrive in recv1 under flags1 and are decoded into p.out;
 // a timed-out wait also sets *abort_out. AG is a compile-time switch so that the allreduce's
-// instantiation is the same code as before it existed.
-template <typename T, int KB, int GPL, bool AG = false>
+// instantiation is the same code as before it existed. CODEC: the all-gather's wire codec.
+template <typename T, int KB, int GPL, bool AG = false, int CODEC = kMaxMin>
 __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems& li, uint32_t epoch, int stages,
                                             int* abort_out = nullptr) {
   const int lane = blockIdx.x;
@@ -405,6 +420,20 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
       auto one = [&](const WarpItem& it, const SliceWords<GPL>& w, bool hot) {
         const uint32_t kind = item_kind(it);
         T* blk = data + it.elem_off;
+        if constexpr (CODEC != kMaxMin) {
+          if (hot) {
+            full_recv_fp8_w<T, CODEC, GPL, true>(w, blk);
+            return;
+          }
+          if (kind == kItemFull) {
+            full_recv_fp8_unaligned<T, CODEC, GPL>(slot, it, blk);
+            return;
+          }
+          if (kind == kItemBucket) {
+            bucket_recv_fp8<T, CODEC>(slot, it, blk);
+            return;
+          }
+        }
         if (hot) {
           full_recv_w<T, KB, GPL, true>(w, it, blk);
         } else if (kind == kItemFull) {
@@ -427,7 +456,10 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
       while (i < end) {
         const uint32_t in = i + 2 * kSraWarps;
         const bool hna = fetch(in, na, wna), hnb = fetch(in + kSraWarps, nb, wnb);
-        if (hota && hotb) {
+        if (CODEC != kMaxMin && hota && hotb) {
+          full_recv_fp8_w<T, CODEC, GPL, true>(wa, data + ita.elem_off);
+          full_recv_fp8_w<T, CODEC, GPL, true>(wb, data + itb.elem_off);
+        } else if (hota && hotb) {
           full_recv_pair<T, KB, GPL>(wa, wb, ita, itb, data + ita.elem_off, data + itb.elem_off);
         } else {
           one(ita, wa, hota);
@@ -589,7 +621,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(con
 // ends with a handshake on flags2 (docs/MEMORY_MODEL.md): a peer's next call can only overwrite
 // the slots after every lane of this call has finished its reads.
 // ===========================================================================
-template <typename T, int KB, int GPL>
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __device__ __forceinline__ void rs_phase_b(const SraParams& p, const LaneItems& li) {
   const int r = p.rank, W = p.world;
   const uint32_t warp = threadIdx.x >> 5;
@@ -608,7 +640,14 @@ __device__ __forceinline__ void rs_phase_b(const SraParams& p, const LaneItems& 
     if (al && kind == kItemFull) slice_load_vec<T, GPL>(src, x);
     if (al && kind == kItemRaw) raw_load_vec<T, GPL>(src, x);
     if (i + kSraWarps < end) slice_prefetch_l2<T, GPL>(data + lane_item(li, p, i + kSraWarps, 0).elem_off);
-    if (kind == kItemFull) {
+    if (CODEC != kMaxMin && kind == kItemFull) {
+      if (al)
+        full_rs_fp8_x<T, CODEC, GPL, true>(x, it, p.prescale, ss, dst);
+      else
+        full_rs_fp8_unaligned<T, CODEC, GPL>(src, it, p.prescale, ss, dst);
+    } else if (CODEC != kMaxMin && kind == kItemBucket) {
+      bucket_rs_fp8<T, CODEC>(src, it, p.prescale, ss, dst);
+    } else if (kind == kItemFull) {
       if (al)
         full_rs_x<T, KB, GPL, true>(x, it, p.prescale, ss, dst);
       else
@@ -623,8 +662,10 @@ __device__ __forceinline__ void rs_phase_b(const SraParams& p, const LaneItems& 
   }
 }
 
-template <typename T, int KB, int GPL>
+// CODEC: the wire codec of the compressed items; the FP8 ones exist with KB 8 only.
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __grid_constant__ SraParams p) {
+  static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   __shared__ LaneItems li;
   __shared__ int s_abort;
   const int lane = blockIdx.x;
@@ -634,7 +675,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __
   lane_items_load(li, p, p.world, 1);
   trace_mark(p, lane, 0, true);
 
-  sra_phase_a<T, KB, GPL>(p, li, epoch, 0);
+  sra_phase_a<T, KB, GPL, CODEC>(p, li, epoch, 0);
   __syncthreads();
   trace_mark(p, lane, 1);
   if (threadIdx.x < 32) {
@@ -643,7 +684,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __
   }
   __syncthreads();
   trace_mark(p, lane, 2);
-  if (!s_abort) rs_phase_b<T, KB, GPL>(p, li);
+  if (!s_abort) rs_phase_b<T, KB, GPL, CODEC>(p, li);
   __syncthreads();
   trace_mark(p, lane, 3);
 
@@ -668,7 +709,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __
 // Like rs_kernel it ends with a handshake on flags2: a peer's next call can only overwrite my
 // recv1 slots after every lane of this call has decoded them (docs/MEMORY_MODEL.md).
 // ===========================================================================
-template <typename T, int KB, int GPL>
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& li, uint32_t epoch) {
   const int r = p.rank, W = p.world;
   const uint32_t warp = threadIdx.x >> 5;
@@ -692,7 +733,16 @@ __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& 
     if (al && kind == kItemRaw) raw_load_vec<T, GPL>(src, x);
     if (i + kSraWarps < end)
       slice_prefetch_l2<T, GPL>(in + ((uint64_t)lane_item(li, p, i + kSraWarps, 0).elem_off - p.out_shift));
-    if (kind == kItemFull) {
+    if (CODEC != kMaxMin && kind == kItemFull) {
+      if (al) {
+        slice_scale<GPL>(x, p.prescale);
+        full_publish_fp8_x<T, CODEC, GPL, true>(x, it, ds, dst);
+      } else {
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, true>(src, it, p.prescale, ds, dst);
+      }
+    } else if (CODEC != kMaxMin && kind == kItemBucket) {
+      bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, ds, dst);
+    } else if (kind == kItemFull) {
       if (al)
         full_send_x<T, KB, GPL, true, true>(x, it, p.prescale, rng, ds, dst);
       else
@@ -708,8 +758,9 @@ __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& 
   }
 }
 
-template <typename T, int KB, int GPL>
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __grid_constant__ SraParams p) {
+  static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   __shared__ LaneItems li;
   __shared__ int s_abort;
   const int lane = blockIdx.x;
@@ -719,11 +770,11 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __
   lane_items_load(li, p, p.world, 1);
   trace_mark(p, lane, 0, true);
 
-  ag_publish<T, KB, GPL>(p, li, epoch);
+  ag_publish<T, KB, GPL, CODEC>(p, li, epoch);
   __syncthreads();
   trace_mark(p, lane, 3);
   if (threadIdx.x < 32) signal_peers(p.flags1, p.world, p.rank, p.flag_stride, lane, flag);
-  sra_phase_c<T, KB, GPL, true>(p, li, epoch, 1, &s_abort);
+  sra_phase_c<T, KB, GPL, true, CODEC>(p, li, epoch, 1, &s_abort);
   __syncthreads();
 
   // slot handshake, as in rs_kernel: every lane, whether or not it had items
@@ -744,12 +795,12 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __
 // them with another kernel would change the allreduce kernels' spill counts.
 enum : int { kOpAllreduce = 0, kOpReduceScatter = 1, kOpAllGather = 2 };
 
-template <typename T, int KB, int GPL, int OP>
+template <typename T, int KB, int GPL, int OP, int CODEC = kMaxMin>
 cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
   if constexpr (OP == kOpReduceScatter)
-    dev::rs_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    dev::rs_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if constexpr (OP == kOpAllGather)
-    dev::ag_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    dev::ag_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if (p.oneshot)
     dev::oneshot_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else
@@ -759,6 +810,16 @@ cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
 
 template <typename T, int GPL, int OP>
 cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
+  if (p.codec != kMaxMin) {  // FP8: the reduce-scatter and all-gather of 8-bit plans only
+    if constexpr (OP == kOpAllreduce) {
+      return cudaErrorInvalidValue;
+    } else {
+      if (p.uniform_bits != 8) return cudaErrorInvalidValue;
+      if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, OP, kE4M3>(p, stream);
+      if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, OP, kE5M2>(p, stream);
+      return cudaErrorInvalidValue;
+    }
+  }
   switch (p.uniform_bits) {
     case 2: return launch_sra_inst<T, 2, GPL, OP>(p, stream);
     case 4: return launch_sra_inst<T, 4, GPL, OP>(p, stream);

@@ -391,8 +391,9 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, 
 }
 
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op, at::Tensor& out, at::Tensor& in,
-                                                                   bool average, int bits, int bucket_size,
-                                                                   bool skip_incomplete, bool stochastic,
+                                                                   bool average, int bits, WireCodec codec,
+                                                                   int bucket_size, bool skip_incomplete,
+                                                                   bool stochastic,
                                                                    int64_t seed, bool overlapped,
                                                                    const std::vector<LayerSpec>& layers) {
   const bool rs = op == ShardedOp::kReduceScatter;
@@ -410,10 +411,16 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
               " has ", full.numel(), " elements, expected world size (", getSize(), ") x ", rs ? "output" : "input",
               " (", shard.numel(), ")");
   TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: ", name, "_compressed: bits must be 1..8 or 32");
+  TORCH_CHECK(codec == kMaxMin || (bits == 8 && !stochastic), "cgx: ", name,
+              "_compressed: the FP8 formats use bits 8 and round to nearest");
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
   const std::vector<LayerSpec> table = engine_->sharded_table(shard.numel(), layers, bits, bucket_size);
+  if (codec != kMaxMin)
+    for (const LayerSpec& l : table)
+      TORCH_CHECK(l.bits == 8 || l.bits >= kRawBits, "cgx: ", name,
+                  "_compressed: an FP8 format needs layers of bits 8 or 32, got ", l.bits);
   return enqueue_cuda(rs ? c10d::OpType::_REDUCE_SCATTER_BASE : c10d::OpType::_ALLGATHER_BASE,
                       rs ? "cgx:reduce_scatter" : "cgx:all_gather", out, &in, [&](cudaStream_t s) {
                         // several nodes: the node partials / gathered shards, N x S elements
@@ -425,7 +432,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
                         }
                         engine_->sharded(true, op, in.data_ptr(), out.data_ptr(),
                                          staging.defined() ? staging.data_ptr() : nullptr, dtype, shard.numel(), table,
-                                         average, skip_incomplete, rng, s, overlapped);
+                                         average, skip_incomplete, rng, s, overlapped, codec);
                       });
 }
 

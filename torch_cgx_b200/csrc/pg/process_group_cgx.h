@@ -188,8 +188,10 @@ class ProcessGroupCGX : public c10d::Backend {
   // shard, (elem_off, numel, bits, bucket) relative to the shard start, empty = one layer with
   // `bits` / `bucket_size`. seed < 0: CGX_SEED. overlapped: at most CGX_OVERLAP_LANES CTAs (runs
   // beside compute).
+  // An FP8 `codec` (bits 8, round to nearest; `layers` of bits 8 or 32) gives the 8-bit records FP8 codes.
   c10::intrusive_ptr<c10d::Work> sharded_compressed(ShardedOp op, at::Tensor& out, at::Tensor& in, bool average,
-                                                    int bits, int bucket_size, bool skip_incomplete, bool stochastic,
+                                                    int bits, WireCodec codec, int bucket_size, bool skip_incomplete,
+                                                    bool stochastic,
                                                     int64_t seed, bool overlapped,
                                                     const std::vector<LayerSpec>& layers);
   // Compressed all_to_all_single: dim-0 rows of `in` go to the ranks by `in_splits`, rows of `out`

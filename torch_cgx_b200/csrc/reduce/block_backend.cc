@@ -12,10 +12,13 @@
 namespace cgx {
 namespace {
 
-// what the FP8 codecs of the block primitives support: 8-bit plans, no prescale, round to nearest
-void check_fp8(const Plan& p, float prescale, const RngKey& rng) {
-  if (p.uniform_bits != 8 || prescale != 1.0f || rng.enabled)
-    throw std::invalid_argument("cgx: an FP8 codec needs an 8-bit plan, prescale 1 and round to nearest");
+// what the FP8 codecs of the block primitives support: compressed blocks of 8-bit plans, rounded to
+// nearest (the reducers pass raw blocks with kMaxMin)
+void check_fp8(const Plan& p, uint32_t first, uint32_t count, const RngKey& rng) {
+  bool ok = p.uniform_bits == 8 && !rng.enabled;
+  for (uint32_t b = first; ok && b < first + count; ++b) ok = block_bits(p.blocks[b]) < kRawBits;
+  if (!ok)
+    throw std::invalid_argument("cgx: an FP8 codec needs compressed blocks of an 8-bit plan and round to nearest");
 }
 
 class CpuBackend : public BlockBackend {
@@ -30,7 +33,7 @@ class CpuBackend : public BlockBackend {
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
                 const RngKey& rng, cudaStream_t, WireCodec codec) override {
     const Plan& p = dp.plan;
-    if (codec != kMaxMin) check_fp8(p, prescale, rng);
+    if (codec != kMaxMin) check_fp8(p, first, count, rng);
     std::vector<float> acc(kMaxBlockElems);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
@@ -42,13 +45,18 @@ class CpuBackend : public BlockBackend {
     }
   }
   void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
-                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t) override {
+                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t,
+                  WireCodec codec) override {
     const Plan& p = dp.plan;
+    if (codec != kMaxMin) check_fp8(p, first, count, RngKey{});
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
       float* a = acc_f32 + (d.elem_off - base_elem);
       if (init_src) cpu::load_block(init_src, p.dtype, d, prescale, a);
-      if (wire) cpu::decode_block_add(wire + d.wire_off, p.dtype, d, a);
+      if (wire && codec != kMaxMin)
+        cpu::decode_block_fp8_add(wire + d.wire_off, d, a, codec);
+      else if (wire)
+        cpu::decode_block_add(wire + d.wire_off, p.dtype, d, a);
     }
   }
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
@@ -62,7 +70,7 @@ class CpuBackend : public BlockBackend {
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                   cudaStream_t, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, 1.0f, RngKey{});
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = dp.plan.blocks[b];
       if (codec != kMaxMin)
@@ -90,15 +98,17 @@ class CudaBackend : public BlockBackend {
   void release(void* p) override { cudaFree(p); }
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
                 const RngKey& rng, cudaStream_t stream, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, prescale, rng);
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng);
     cuda_check(launch_quantize_items(args(dp, first, count, codec), src, wire, prescale, rng, stream),
                "quantize_items");
   }
   void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
-                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream) override {
-    cuda_check(
-        launch_accumulate_items_f32(args(dp, first, count), wire, acc_f32, base_elem, init_src, prescale, stream),
-        "accumulate_items");
+                  uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream,
+                  WireCodec codec) override {
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
+    cuda_check(launch_accumulate_items_f32(args(dp, first, count, codec), wire, acc_f32, base_elem, init_src, prescale,
+                                           stream),
+               "accumulate_items");
   }
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
                     uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) override {
@@ -107,7 +117,7 @@ class CudaBackend : public BlockBackend {
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                   cudaStream_t stream, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, 1.0f, RngKey{});
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
     cuda_check(launch_dequantize_items(args(dp, first, count, codec), wire, dst, stream), "dequantize_items");
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) override {

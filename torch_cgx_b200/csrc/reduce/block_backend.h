@@ -23,14 +23,17 @@ class BlockBackend {
   virtual void release(void* p) = 0;
   // The block primitives work on blocks [first, first+count) of `dp`'s plan; the device backend
   // reads its uploaded tables (PlanCache::upload), the host backend the plan alone.
-  // wire = quantize(src[T] * prescale). An FP8 `codec` (common/quant_math.h) needs an 8-bit plan,
-  // prescale 1 and deterministic rounding; its records are read back by dequantize with the same codec.
+  // wire = quantize(src[T] * prescale). An FP8 `codec` (common/quant_math.h) needs compressed blocks
+  // of an 8-bit plan and deterministic rounding; its records are read back by dequantize and
+  // accumulate with the same codec.
   virtual void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire,
                         float prescale, const RngKey& rng, cudaStream_t stream, WireCodec codec = kMaxMin) = 0;
   // acc_f32[elem_off - base_elem + i] = float(init_src[elem_off + i]) * prescale   (init_src != nullptr)
   // acc_f32[...] += decode(wire)                                                   (wire != nullptr)
+  // (an FP8 codec adds fl(float(code) * unit), a separate rounding)
   virtual void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
-                          uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream) = 0;
+                          uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream,
+                          WireCodec codec = kMaxMin) = 0;
   // wire = quantize(acc_f32); out[T] = decode(wire) when out != nullptr
   virtual void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first,
                             uint32_t count, uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) = 0;

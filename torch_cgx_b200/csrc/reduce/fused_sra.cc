@@ -104,9 +104,16 @@ std::vector<std::vector<LayerSpec>> split_shard(const std::vector<LayerSpec>& la
 }  // namespace
 
 void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
-                           const void* out, uint64_t S, int rank, int world) {
+                           const void* out, uint64_t S, int rank, int world, WireCodec codec) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
+  if (codec != kMaxMin && codec != kE4M3 && codec != kE5M2)
+    throw std::invalid_argument(std::string("cgx ") + name + ": unknown wire codec");
+  if (codec != kMaxMin)
+    for (const LayerSpec& l : shard_layers)
+      if (l.bits != 8 && l.bits < kRawBits)
+        throw std::invalid_argument(std::string("cgx ") + name + ": an FP8 format needs layers of bits 8 or 32, got " +
+                                    std::to_string(l.bits));
   const uint64_t table = shard_elems(shard_layers);
   if (table != S)
     throw std::invalid_argument(std::string("cgx ") + name + ": the shard layers tile [0, " + std::to_string(table) +
@@ -168,11 +175,13 @@ void FusedSra::prepare_sharded(const std::vector<LayerSpec>& shard_layers, int d
 FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype,
                                      bool skip_incomplete, const void* in, void* out, uint64_t S, float prescale,
                                      const RngParams& rng, cudaStream_t stream, int max_lanes,
-                                     const WindowHook& before_launch) {
+                                     const WindowHook& before_launch, WireCodec codec) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
   RsCounts n;
-  check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world());
+  check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world(), codec);
+  if (codec != kMaxMin && rng.stochastic)
+    throw std::invalid_argument(std::string("cgx ") + name + ": the FP8 formats round to nearest only");
   if (S == 0) return n;
   // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
   for (const auto& w : rs_windows(shard_layers, dtype, skip_incomplete, max_lanes)) {
@@ -180,7 +189,7 @@ FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>&
     if (dp == nullptr)
       throw std::runtime_error(std::string("cgx ") + name + ": window plan does not fit the heap slots");
     if (before_launch) before_launch(w, *dp);
-    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs);
+    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs, codec);
     const Plan& pl = dp->plan;
     const uint64_t mine = pl.chunk_wire_bytes[rank()], my_elems = pl.chunk_elems[rank()];
     ++n.launches;
@@ -211,7 +220,7 @@ int FusedSra::pick_stages(const DevicePlan&) const {
 }
 
 void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-                      bool oneshot, void* out, uint64_t out_shift, bool gather) {
+                      bool oneshot, void* out, uint64_t out_shift, bool gather, WireCodec codec) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   if (dp.plan.items.empty()) return;
   ++epoch_;
@@ -267,6 +276,8 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
   p.out = out;
   p.out_shift = out_shift;
   p.gather = gather ? 1 : 0;
+  // a window of raw layers only has no compressed item: the max-min kernel moves it the same way
+  p.codec = dp.plan.uniform_bits == 0 ? kMaxMin : codec;
   cuda_check(launch_sra_fused(p, stream), "launch_sra_fused");
   ++launches_;
 }

@@ -52,9 +52,10 @@ inline std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& shard, int
 
 // The buffers of one rank's sharded call: `shard_layers` tiles [0, S) in order, and the shard buffer
 // (the reduce-scatter's `out`, the all-gather's `in`) is disjoint from the full one or exactly its
-// chunk `rank` of `world`; std::invalid_argument otherwise.
+// chunk `rank` of `world`; with an FP8 `codec` every layer has bits 8 or 32 (raw);
+// std::invalid_argument otherwise.
 void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
-                           const void* out, uint64_t S, int rank, int world);
+                           const void* out, uint64_t S, int rank, int world, WireCodec codec = kMaxMin);
 
 // The windows of a reduce-scatter: the shard's layer table (offsets from the shard start, tiling
 // [0, S) in order; std::invalid_argument otherwise) cut by split_for_fusion into shard-relative
@@ -125,13 +126,16 @@ class FusedSra {
   // bucket boundaries, so the result does not depend on the slot size) and one kernel is launched
   // per window. Stream-ordered; every rank must issue the same calls in the same order.
   // `before_launch`, when set, sees each window's table and plan right before its kernel is launched.
+  // An FP8 `codec` (common/quant_math.h; layers of bits 8 or 32, round to nearest) gives the 8-bit
+  // records FP8 codes: the sender encodes prescale * x, the reduce-scatter adds each decoded value
+  // fl(float(code) * unit) with its own rounding, and the all-gather's owner keeps the decoded codes.
   struct RsCounts {
     uint64_t launches = 0, elements = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's share
   };
   using WindowHook = std::function<void(const std::vector<LayerSpec>& window, const DevicePlan& dp)>;
   RsCounts sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                    const void* in, void* out, uint64_t S, float prescale, const RngParams& rng, cudaStream_t stream,
-                   int max_lanes = 0, const WindowHook& before_launch = nullptr);
+                   int max_lanes = 0, const WindowHook& before_launch = nullptr, WireCodec codec = kMaxMin);
   // builds and uploads the plans of every window without launching anything
   void prepare_sharded(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                        cudaStream_t stream, int max_lanes = 0);
@@ -196,7 +200,8 @@ class FusedSra {
   const DevicePlan* prepare_impl(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                  cudaStream_t stream, int plan_world, uint32_t capacity, int max_lanes);
   void launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-              bool oneshot, void* out = nullptr, uint64_t out_shift = 0, bool gather = false);
+              bool oneshot, void* out = nullptr, uint64_t out_shift = 0, bool gather = false,
+              WireCodec codec = kMaxMin);
   std::unordered_map<uint64_t, std::vector<std::vector<LayerSpec>>> rs_windows_;
 };
 

@@ -7,6 +7,26 @@
 #include "fused_sra.h"  // shard_elems, replicate, check_all_to_all
 
 namespace cgx {
+namespace {
+
+// Blocks [first, first + count) of `p` in maximal runs of compressed or of raw blocks, each with
+// the codec it travels in: an FP8 codec covers the compressed blocks, raw blocks are raw either way.
+template <class F>
+void codec_runs(const Plan& p, uint32_t first, uint32_t count, WireCodec codec, F&& f) {
+  if (codec == kMaxMin) {
+    f(first, count, kMaxMin);
+    return;
+  }
+  for (uint32_t b = first, end = first + count; b < end;) {
+    const bool raw = block_bits(p.blocks[b]) >= kRawBits;
+    uint32_t e = b + 1;
+    while (e < end && (block_bits(p.blocks[e]) >= kRawBits) == raw) ++e;
+    f(b, e - b, raw ? kMaxMin : codec);
+    b = e;
+  }
+}
+
+}  // namespace
 
 Reducer::Reducer(Communicator* comm, BlockBackend* ops) : comm_(comm), ops_(ops) {}
 
@@ -92,7 +112,8 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
 
 // ------------------------------------------------------- sharded collectives --
 void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                             bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream) {
+                             bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream,
+                             WireCodec codec) {
   const int W = comm_->size(), r = comm_->rank();
   const uint64_t S = shard_elems(shard_layers);
   if (S == 0) return;
@@ -112,7 +133,9 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->quantize(dp, in, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
+    codec_runs(plan, pb, pn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->quantize(dp, in, b, n, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream, c);
+    });
     if (plan.chunk_wire_bytes[p]) x.push_back({true, sendb + row * p, plan.chunk_wire_bytes[p], p});
     if (plan.chunk_wire_bytes[r]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[r], p});
     bytes_sent_ += plan.chunk_wire_bytes[p];
@@ -121,7 +144,10 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
   if (!cn) return;
   ops_->accumulate(dp, nullptr, cb, cn, acc, lo, in, prescale, stream);
   for (int q = 0; q < W; ++q)
-    if (q != r) ops_->accumulate(dp, recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
+    if (q != r)
+      codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->accumulate(dp, recvb + row * q, b, n, acc, lo, nullptr, 1.0f, stream, c);
+      });
   // store the fp32 sums as T: a raw plan of one shard does exactly that (acc[i] is element i of the
   // shard, chunk r starting at r * S)
   std::vector<LayerSpec> raw = shard_layers;
@@ -132,7 +158,7 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
 }
 
 void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                         bool skip_incomplete, const RngParams& rng, cudaStream_t stream) {
+                         bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
   const int W = comm_->size(), r = comm_->rank();
   const uint64_t S = shard_elems(shard_layers);
   if (S == 0) return;
@@ -148,10 +174,10 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   if (in != own) ops_->copy(own, in, shard_bytes, stream);
   // the root's part of the compressed broadcast: quantize once, keep what the peers will decode
   const uint32_t cb = plan.chunk_begin(r), cn = plan.chunk_end(r) - cb;
-  if (cn) {
-    ops_->quantize(dp, out, cb, cn, mine, 1.0f, make_rng_key(rng, r, 1), stream);
-    ops_->dequantize(dp, mine, cb, cn, out, stream);
-  }
+  codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+    ops_->quantize(dp, out, b, n, mine, 1.0f, make_rng_key(rng, r, 1), stream, c);
+    ops_->dequantize(dp, mine, b, n, out, stream, c);
+  });
   std::vector<P2POp> x;
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
@@ -163,7 +189,9 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->dequantize(dp, recvb + row * p, pb, pn, out, stream);
+    codec_runs(plan, pb, pn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->dequantize(dp, recvb + row * p, b, n, out, stream, c);
+    });
   }
 }
 

@@ -48,15 +48,18 @@ class Reducer {
   //   out = T(prescale * in[r] + sum over peers q, in rank order, of decode(Q_q(prescale * in_q[r])))
   // accumulated in fp32 and stored once in the dtype, not requantized. Bitwise the fused rs_kernel
   // (same plan, primitives, order and RNG streams: rank q's phase-0 stream, full-buffer indices).
+  // An FP8 `codec` (8-bit layers) quantizes the compressed layers with its records, round to nearest,
+  // and adds each decoded value with its own rounding; raw layers are unchanged. The same for all_gather.
   void reduce_scatter(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                      bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream);
+                      bool skip_incomplete, float prescale, const RngParams& rng, cudaStream_t stream,
+                      WireCodec codec = kMaxMin);
   // Compressed all-gather: the compressed broadcast with every rank as a root. `in` holds this rank's
   // shard of S elements, `out` W * S; rank q quantizes its shard once (copy q of the replicated table,
   // its phase-1 stream), decodes it into its own chunk and sends the same bytes to every peer, which
   // decode them. Every rank's `out` is the same bytes, bitwise the fused ag_kernel's; raw layers
   // (bits 32) are copied unchanged. `in` may be `out`'s chunk rank(), or disjoint from it.
   void all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                  bool skip_incomplete, const RngParams& rng, cudaStream_t stream);
+                  bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec = kMaxMin);
   // Compressed all-to-all over the communicator's W ranks, bitwise FusedSra::all_to_all (same
   // arguments and checks): each chunk for a peer is quantized by the standalone item kernels through
   // a one-layer plan of the chunk, the records are exchanged and every peer's chunk is decoded into

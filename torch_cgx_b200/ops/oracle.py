@@ -216,23 +216,27 @@ def _scaled_inputs(inputs: Sequence[torch.Tensor], ps: _F32) -> List[np.ndarray]
         return [t.detach().reshape(-1).float().cpu().numpy() * ps for t in inputs]
 
 
-def _contribution(v: np.ndarray, bits: int, bucket: int, dtype: torch.dtype) -> np.ndarray:
-    """What a receiver decodes of one sent contribution: one quantization round, or the value
-    rounded to the dtype for raw runs."""
+def _contribution(v: np.ndarray, bits: int, bucket: int, dtype: torch.dtype, fmt: str | None = None) -> np.ndarray:
+    """What a receiver decodes of one sent contribution: one quantization round (in the FP8 format
+    ``fmt`` when given), or the value rounded to the dtype for raw runs."""
     if bits >= RAW_BITS:
         return round_to_dtype(v, dtype)
+    if fmt is not None:
+        return _fp8_qdq_buckets(v, fmt, bucket)
     return _qdq_buckets(v, bits, bucket)[0]
 
 
 def quantize_dequantize_layers(x: torch.Tensor, layers: Sequence[Layer], *, skip_incomplete: bool = False,
-                               prescale: float = 1.0) -> torch.Tensor:
+                               prescale: float = 1.0, fmt: str | None = None) -> torch.Tensor:
     """One quantize -> dequantize round trip of ``prescale * x`` through a layer table, in
     ``x.dtype`` (raw runs: the value rounded to the dtype). Elements outside every layer are 0,
-    as in a freshly dequantized tensor."""
+    as in a freshly dequantized tensor. ``fmt`` ("e4m3" / "e5m2"): the compressed layers (bits 8)
+    take the FP8 round trip of ``fp8_quantize_dequantize`` instead of max-min's."""
+    _check_fp8_table(layers, fmt)
     v = _scaled_inputs([x], _F32(prescale))[0]
     out = np.zeros(v.size, _F32)
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
-        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, x.dtype)
+        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, x.dtype, fmt)
     return _to_tensors([out], x.dtype)[0].view_as(x)
 
 
@@ -241,14 +245,24 @@ def _to_tensors(outs: Sequence[np.ndarray], dtype: torch.dtype) -> List[torch.Te
 
 
 def _sra_acc(xs: Sequence[np.ndarray], sl: slice, own: np.ndarray, bits: int, bucket: int,
-             dtype: torch.dtype) -> np.ndarray:
+             dtype: torch.dtype, fmt: str | None = None) -> np.ndarray:
     """The owner's fp32 accumulator of one run of the SRA: its own value, then every peer's
-    decoded contribution in rank order."""
+    decoded contribution in rank order (each an fp32 add of its own)."""
     acc = np.choose(own, [x[sl] for x in xs]).astype(_F32)
     with np.errstate(all="ignore"):
         for q in range(len(xs)):
-            acc = np.where(own != q, acc + _contribution(xs[q][sl], bits, bucket, dtype), acc)
+            acc = np.where(own != q, acc + _contribution(xs[q][sl], bits, bucket, dtype, fmt), acc)
     return acc
+
+
+def _check_fp8_table(layers: Sequence[Layer], fmt: str | None) -> None:
+    if fmt is None:
+        return
+    if fmt not in FP8_FORMATS:
+        raise ValueError(f"unknown FP8 format {fmt!r}")
+    for l in layers:
+        if int(l[2]) != 8 and int(l[2]) < RAW_BITS:
+            raise ValueError(f"an FP8 format needs layers of bits 8 or {RAW_BITS}, got {l[2]}")
 
 
 def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, world: int | None = None,
@@ -588,7 +602,8 @@ def _shards(inputs: Sequence[torch.Tensor], r: int) -> List[torch.Tensor]:
 
 def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
                              world: int | None = None, average: bool = False,
-                             skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
+                             skip_incomplete: bool = False, prescale: float | None = None,
+                             fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's output of the compressed reduce-scatter (deterministic rounding).
 
     ``inputs[r]`` holds W shards of S elements; ``shard_layers`` is one shard's table (offsets from
@@ -597,8 +612,11 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
         prescale*x_r  (kept unquantized)  +  sum over q != r, in rank order, of Q(prescale*x_q)
     rounded once to the dtype: the SRA's phase-B accumulator without the requantization. Raw runs
     round each peer contribution to the dtype. Elements outside every layer are 0. The prescale is
-    ``prescale`` when given, else 1/W when averaging, else 1.
+    ``prescale`` when given, else 1/W when averaging, else 1. ``fmt`` ("e4m3" / "e5m2"): Q is
+    the FP8 round trip (``fp8_quantize_dequantize`` of the prescaled values), and the table's
+    compressed layers have bits 8.
     """
+    _check_fp8_table(shard_layers, fmt)
     W = len(inputs)
     assert world is None or world == W
     dtype = inputs[0].dtype
@@ -609,17 +627,19 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
         out = np.zeros(xs[0].size, _F32)
         for off, m, bits, bucket in layer_segments(shard_layers, skip_incomplete):
             sl = slice(off, off + m)
-            out[sl] = _sra_acc(xs, sl, np.full(m, r), bits, bucket, dtype)
+            out[sl] = _sra_acc(xs, sl, np.full(m, r), bits, bucket, dtype, fmt)
         outs.append(out)
     return _to_tensors(outs, dtype)
 
 
-def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer]) -> torch.Tensor:
+def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer],
+                         fmt: str | None = None) -> torch.Tensor:
     """Every rank's output of the compressed all-gather (deterministic rounding): the concatenation
-    over q of ``quantize_dequantize_layers(inputs[q], shard_layers)``. ``shard_layers`` is one
-    shard's table (offsets from the shard start), so buckets are counted from each shard's start;
-    the owner's shard is quantized like every other. Raw runs are the value in the dtype."""
-    return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers) for t in inputs])
+    over q of ``quantize_dequantize_layers(inputs[q], shard_layers, fmt=fmt)``. ``shard_layers`` is
+    one shard's table (offsets from the shard start), so buckets are counted from each shard's
+    start; the owner's shard is quantized like every other. Raw runs are the value in the dtype."""
+    return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers, fmt=fmt)
+                      for t in inputs])
 
 
 # ---- FP8 wire formats of the all-to-all (common/quant_math.h, DESIGN §2.13b) ------------------------

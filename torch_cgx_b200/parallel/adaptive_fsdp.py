@@ -70,6 +70,9 @@ class AdaptiveFSDPState:
                  stochastic: bool = False):
         self.targets = {"reduce_scatter": reduce_scatter_bits, "all_gather": all_gather_bits}
         for kind, bits in self.targets.items():
+            if isinstance(bits, str):
+                raise ValueError(f"{kind}_bits must be a max-min width in 1..8 or None: adaptive widths do not "
+                                 f"take FP8 formats, got {bits!r}")
             if bits is not None and not 1 <= int(bits) <= 8:
                 raise ValueError(f"{kind}_bits must be a width in 1..8 or None, got {bits}")
         self.targets = {k: None if b is None else int(b) for k, b in self.targets.items()}

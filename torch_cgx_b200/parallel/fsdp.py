@@ -8,6 +8,9 @@ FSDP2 takes a custom reduce-scatter and all-gather per module (``FSDPModule.set_
     cgx.set_cgx_reduce_scatter(model, bits=8)        # every FSDPModule of the model
     cgx.set_cgx_all_gather(model, bits=8)            # one comm per FSDPModule, per-parameter table
 
+``bits`` may also be an FP8 wire format: ``"e4m3"`` for the parameter all-gather and ``"e5m2"`` for
+the gradient reduce-scatter are the usual choice.
+
 Both work over any number of nodes: across nodes they run in two stages, the semantics of
 ``reduce_scatter_tensor`` and ``all_gather_into_tensor`` (functional.py).
 """
@@ -19,7 +22,7 @@ import torch
 import torch.distributed as dist
 from torch.distributed.fsdp._fully_shard._fsdp_api import AllGather, ReduceScatter
 
-from .functional import _all_gather, _reduce_scatter
+from .functional import A2aBits, _all_gather, _reduce_scatter
 
 RAW_BITS = 32
 
@@ -31,17 +34,32 @@ def _table(layers: Optional[Sequence[Layer]]) -> Optional[List[Layer]]:
     return None if layers is None else [tuple(int(v) for v in l) for l in layers]
 
 
+def _bits(bits: A2aBits, adaptive) -> A2aBits:
+    """a comm's ``bits``: an int, or an FP8 format name, which adaptive widths do not take"""
+    if isinstance(bits, str):
+        if adaptive is not None:
+            raise ValueError(f"cgx: adaptive widths are max-min widths; bits={bits!r} cannot be adapted")
+        return bits
+    return int(bits)
+
+
+def _table_bits(bits: A2aBits) -> int:
+    """the width of a table entry for ``bits``: an FP8 format travels in 8-bit records"""
+    return 8 if isinstance(bits, str) else int(bits)
+
+
 class CGXReduceScatter(ReduceScatter):
     """FSDP2 reduce-scatter comm: SUM and AVG go through the compressed kernel (with at most
     ``CGX_OVERLAP_LANES`` CTAs, since FSDP overlaps it with backward); any other op, such as
     premul-sum, goes to ``dist.reduce_scatter_tensor`` unchanged. ``layers`` optionally gives one
     shard's table as ``(elem_off, numel, bits, bucket_size)`` tuples (None = one layer of ``bits`` /
     ``bucket_size`` per shard). ``adaptive`` is an :class:`~torch_cgx_b200.AdaptiveFSDPState` that
-    rewrites ``layers``; ``set_cgx_adaptive`` sets it."""
+    rewrites ``layers``; ``set_cgx_adaptive`` sets it. ``bits`` may be an FP8 format, ``"e5m2"`` or
+    ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``stochastic``, no ``adaptive``)."""
 
-    def __init__(self, bits: int = 4, bucket_size: int = 512, stochastic: bool = False,
+    def __init__(self, bits: A2aBits = 4, bucket_size: int = 512, stochastic: bool = False,
                  layers: Optional[Sequence[Layer]] = None, name: str = "", adaptive=None):
-        self.bits = int(bits)
+        self.bits = _bits(bits, adaptive)
         self.bucket_size = int(bucket_size)
         self.stochastic = bool(stochastic)
         self.layers = _table(layers)
@@ -68,7 +86,7 @@ class CGXReduceScatter(ReduceScatter):
         return dist.reduce_scatter_tensor(output_tensor, input_tensor, op=op, group=group, async_op=async_op)
 
 
-def set_cgx_reduce_scatter(model: torch.nn.Module, bits: int = 4, bucket_size: int = 512,
+def set_cgx_reduce_scatter(model: torch.nn.Module, bits: A2aBits = 4, bucket_size: int = 512,
                            stochastic: bool = False) -> CGXReduceScatter:
     """Install one :class:`CGXReduceScatter` on every ``FSDPModule`` of ``model``; returns it."""
     from torch.distributed.fsdp import FSDPModule
@@ -80,20 +98,21 @@ def set_cgx_reduce_scatter(model: torch.nn.Module, bits: int = 4, bucket_size: i
     return comm
 
 
-def fsdp_shard_table(params: Sequence[Tuple[Sequence[int], int]], bits: int = 4,
+def fsdp_shard_table(params: Sequence[Tuple[Sequence[int], int]], bits: A2aBits = 4,
                      bucket_size: int = 512) -> List[Layer]:
     """The all-gather shard table of one FSDP parameter group.
 
     ``params`` holds one ``(orig_size, padded_shard_numel)`` pair per parameter, in FSDP's
     all-gather order. Each parameter is one layer of ``padded_shard_numel`` elements, so no bucket
     spans two parameters; parameters of at most one dimension (biases, norm weights) travel
-    uncompressed (bits 32): they are small, and their values sit far from those of the weights."""
+    uncompressed (bits 32): they are small, and their values sit far from those of the weights.
+    With an FP8 ``bits`` the other parameters get 8, the width of its records."""
     table, off = [], 0
     for orig_size, n in params:
         n = int(n)
         if n == 0:
             continue
-        table.append((off, n, RAW_BITS if len(orig_size) <= 1 else int(bits), int(bucket_size)))
+        table.append((off, n, RAW_BITS if len(orig_size) <= 1 else _table_bits(bits), int(bucket_size)))
         off += n
     return table
 
@@ -105,11 +124,12 @@ class CGXAllGather(AllGather):
     FSDP prefetches during compute. There is no stochastic rounding: the backward re-gather must
     see the weights the forward saw. A ``uint8`` buffer (FSDP2's all-gather of mixed-dtype inputs)
     goes to ``dist.all_gather_into_tensor`` unchanged. ``adaptive`` is an
-    :class:`~torch_cgx_b200.AdaptiveFSDPState` that rewrites ``layers``; ``set_cgx_adaptive`` sets it."""
+    :class:`~torch_cgx_b200.AdaptiveFSDPState` that rewrites ``layers``; ``set_cgx_adaptive`` sets it.
+    ``bits`` may be an FP8 format, usually ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``adaptive``)."""
 
-    def __init__(self, bits: int = 4, bucket_size: int = 512, layers: Optional[Sequence[Layer]] = None,
+    def __init__(self, bits: A2aBits = 4, bucket_size: int = 512, layers: Optional[Sequence[Layer]] = None,
                  name: str = "", adaptive=None):
-        self.bits = int(bits)
+        self.bits = _bits(bits, adaptive)
         self.bucket_size = int(bucket_size)
         self.layers = _table(layers)
         self.name = name
@@ -133,7 +153,8 @@ class CGXAllGather(AllGather):
                            async_op=async_op, stochastic=False, seed=None, layers=self.layers, overlapped=True)
 
 
-def set_cgx_all_gather(model: torch.nn.Module, bits: int = 4, bucket_size: int = 512) -> List[CGXAllGather]:
+def set_cgx_all_gather(model: torch.nn.Module, bits: A2aBits = 4,
+                       bucket_size: int = 512) -> List[CGXAllGather]:
     """Install a :class:`CGXAllGather` on every ``FSDPModule`` of ``model``, each with the
     per-parameter shard table (:func:`fsdp_shard_table`) of that module's parameter group; returns
     the comms. Call it after ``fully_shard`` and before the first forward."""

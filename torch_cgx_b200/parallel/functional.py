@@ -17,6 +17,8 @@ and so is the compressed all-gather (``dist.all_gather_into_tensor`` stays uncom
 
     cgx.all_gather_into_tensor(flat_params, shard, bits=8)
 
+Both also take an FP8 wire format, ``bits="e4m3"`` or ``"e5m2"``, in place of max-min 8-bit.
+
 and the compressed all-to-all of expert-parallel MoE layers (``dist.all_to_all_single`` stays
 uncompressed)::
 
@@ -93,16 +95,36 @@ def _sharded(method: str, api: str, output: torch.Tensor, input: torch.Tensor, h
     return None
 
 
-def _reduce_scatter(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, average: bool,
+A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2"
+
+
+def _sharded_bits(bits: A2aBits, stochastic: bool, layers: Optional[Sequence[Tuple[int, int, int, int]]],
+                  op: str) -> A2aBits:
+    """``bits`` of the compressed reduce-scatter / all-gather as the native call takes it: an int, or
+    an FP8 format name, whose ``layers`` table may hold bits 8 (FP8) and 32 (raw) only. ValueError
+    otherwise, before anything is sent."""
+    if not isinstance(bits, str):
+        return int(bits)
+    from .. import _C
+
+    _C.a2a_bits(bits, bool(stochastic), op)
+    for l in layers or []:
+        if int(l[2]) != 8 and int(l[2]) < 32:
+            raise ValueError(f"cgx {op}: bits={bits!r} needs a layer table of bits 8 or 32, got a layer of {l[2]}")
+    return bits
+
+
+def _reduce_scatter(output: torch.Tensor, input: torch.Tensor, *, bits: A2aBits, bucket_size: int, average: bool,
                     group, async_op: bool, stochastic: bool, seed: Optional[int],
                     layers: Optional[Sequence[Tuple[int, int, int, int]]], skip_incomplete: bool,
                     overlapped: bool):
+    bits = _sharded_bits(bits, stochastic, layers, "reduce_scatter")
     return _sharded("reduce_scatter_compressed", "reduce_scatter_tensor", output, input,
-                    (bool(average), int(bits), int(bucket_size), bool(skip_incomplete)), group=group,
+                    (bool(average), bits, int(bucket_size), bool(skip_incomplete)), group=group,
                     async_op=async_op, stochastic=stochastic, seed=seed, layers=layers, overlapped=overlapped)
 
 
-def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
+def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBits = 4, bucket_size: int = 512,
                           average: bool = False, group=None, async_op: bool = False, stochastic: bool = False,
                           seed: Optional[int] = None, layers: Optional[Sequence[Tuple[int, int, int, int]]] = None,
                           skip_incomplete: bool = False):
@@ -115,6 +137,14 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int =
     tuples relative to the shard start (bits 32: uncompressed); the same table applies to every
     shard. ``seed=None`` uses ``CGX_SEED``. ``output`` may be the rank's own chunk of ``input``.
     CUDA float32 / float16 / bfloat16.
+
+    ``bits="e4m3"`` or ``"e5m2"`` sends the bytes of ``bits=8`` as FP8 (see ``all_to_all_single``):
+    per bucket one fp32 scale ``unit = max|y| / FMAX`` of the prescaled values ``y``, and one FP8 code
+    of ``y / unit`` per element. The receiver adds each decoded value ``code * unit`` to its fp32 sum
+    in rank order. ``e5m2``'s wider exponent range suits gradients. A ``layers`` table may then hold
+    bits 8 (FP8) and 32 (raw) only. A NaN or an Inf in a peer's bucket makes that bucket of the sum
+    NaN. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as does any other
+    string.
 
     Over several nodes (``local_size`` consecutive ranks each) the reduction has two stages: inside
     each node, for every node's block of shards, the reduce-scatter above over the local ranks
@@ -129,15 +159,16 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: int =
                            skip_incomplete=skip_incomplete, overlapped=False)
 
 
-def _all_gather(output: torch.Tensor, input: torch.Tensor, *, bits: int, bucket_size: int, group, async_op: bool,
-                stochastic: bool, seed: Optional[int], layers: Optional[Sequence[Tuple[int, int, int, int]]],
-                overlapped: bool):
-    return _sharded("all_gather_compressed", "all_gather_into_tensor", output, input, (int(bits), int(bucket_size)),
+def _all_gather(output: torch.Tensor, input: torch.Tensor, *, bits: A2aBits, bucket_size: int, group,
+                async_op: bool, stochastic: bool, seed: Optional[int],
+                layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool):
+    bits = _sharded_bits(bits, stochastic, layers, "all_gather")
+    return _sharded("all_gather_compressed", "all_gather_into_tensor", output, input, (bits, int(bucket_size)),
                     group=group, async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
                     overlapped=overlapped)
 
 
-def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int = 4, bucket_size: int = 512,
+def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBits = 4, bucket_size: int = 512,
                            group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
                            layers: Optional[Sequence[Tuple[int, int, int, int]]] = None):
     """Compressed ``dist.all_gather_into_tensor`` on a ``cgx`` group.
@@ -151,6 +182,12 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int 
     ``CGX_SEED``. ``input`` may be the rank's own chunk of ``output``. CUDA float32 / float16 /
     bfloat16.
 
+    ``bits="e4m3"`` or ``"e5m2"`` sends the bytes of ``bits=8`` as FP8 (see ``all_to_all_single``),
+    the usual choice for weights being ``e4m3``. Every rank, the owner included, writes the values
+    decoded from the same codes, so at world 1 the output is ``ops.oracle.fp8_quantize_dequantize``
+    of the input. A ``layers`` table may then hold bits 8 (FP8) and 32 (raw) only; FP8 rounds to
+    nearest only.
+
     Over several nodes the owner's quantized bytes first go to the ranks of the same local rank on
     the other nodes, which decode them; each node then shares the decoded shards among its ranks
     uncompressed. Every shard is still quantized exactly once, so with round-to-nearest every
@@ -162,9 +199,6 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: int 
 
 def _splits(s: Optional[Sequence[int]]) -> List[int]:
     return [] if s is None else [int(v) for v in s]
-
-
-A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2"
 
 
 def _a2a_bits(bits: A2aBits, stochastic: bool) -> A2aBits:
