@@ -16,8 +16,10 @@ bucket. Both move the same packed bytes; the reduce-scatter also accumulates. It
 the FP8 wire formats, e4m3 and e5m2, which move the bytes of bits 8 (the reduce-scatter row next to
 them runs at bits 8).
 
---op sra --bits may name them too: they time the reduce-scatter and all-gather rows only (there is
-no FP8 allreduce). Every row is timed for each of --dtypes."""
+--op sra --bits may name them too: every row then runs at bits 8 with that format, the allreduce's
+included. The allreduce also gets a one-shot row ("kernel": "oneshot") at --oneshot-kbs KB per
+virtual rank, the sizes the engine sends through the one-shot kernel. Every row is timed for each of
+--dtypes."""
 import argparse
 import json
 import sys
@@ -58,6 +60,7 @@ def main():
     ap.add_argument("--op", default="sra", choices=["sra", "all_to_all"],
                     help="sra: allreduce, reduce-scatter and all-gather rows; all_to_all: a2a next to rs_kernel")
     ap.add_argument("--dtypes", default="float32", help="comma-separated dtypes")
+    ap.add_argument("--oneshot-kbs", default="256,1024", help="one-shot allreduce sizes, KB per virtual rank")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     W = args.world
@@ -79,33 +82,48 @@ def main():
 
 
 def sra_rows(args, dev, W, lanes, dtype, bits):
-    """the allreduce, reduce-scatter and all-gather rows of one dtype and --bits entry; an FP8 format
-    times the reduce-scatter and all-gather only (its records are those of bits 8)"""
+    """the allreduce (SRA and one-shot), reduce-scatter and all-gather rows of one dtype and --bits
+    entry; an FP8 format moves the records of bits 8"""
     rows = []
     fmt = bits if isinstance(bits, str) else None
     width = 8 if fmt else bits
     es = torch.empty(0, dtype=dtype).element_size()
     dt = str(dtype).replace("torch.", "")
     mbs = sorted(int(x) for x in args.mbs.split(","))
-    if fmt is None:
-        res = {}
-        for mb in mbs:
-            n = (mb << 20) // es
-            layers = [(0, n, bits, args.bucket)]
-            g = C.LocalSraGroup(W, lanes, n * es // W * 2 + (1 << 20), 20000, 4096)
-            xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
-            g.allreduce(xs, layers)
-            torch.cuda.synchronize()
-            g.check()
-            res[mb] = timeit(lambda: g.allreduce(xs, layers))
-            del g, xs
-        slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])  # us per MB per virtual rank
-        row = {"world": W, "dtype": dt, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
-               "times_us": {str(k): round(v, 1) for k, v in res.items()},
-               "us_per_equivalent_64MB_allreduce": round(slope * 64 / W, 1),
-               "note": "slope * (64 MB / W): device work of one real rank of a 64 MB allreduce on W GPUs, NVLink excluded"}
-        rows.append(row)
-        print(json.dumps(row), flush=True)
+    res = {}
+    for mb in mbs:
+        n = (mb << 20) // es
+        layers = [(0, n, width, args.bucket)]
+        g = C.LocalSraGroup(W, lanes, n * es // W * 2 + (1 << 20), 20000, 4096)
+        xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
+        g.allreduce(xs, layers, bits=fmt)
+        torch.cuda.synchronize()
+        g.check()
+        res[mb] = timeit(lambda: g.allreduce(xs, layers, bits=fmt))
+        del g, xs
+    slope = (res[mbs[-1]] - res[mbs[0]]) / (mbs[-1] - mbs[0])  # us per MB per virtual rank
+    row = {"world": W, "dtype": dt, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
+           "times_us": {str(k): round(v, 1) for k, v in res.items()},
+           "us_per_equivalent_64MB_allreduce": round(slope * 64 / W, 1),
+           "note": "slope * (64 MB / W): device work of one real rank of a 64 MB allreduce on W GPUs, NVLink excluded"}
+    rows.append(row)
+    print(json.dumps(row), flush=True)
+    res = {}
+    for kb in sorted(int(x) for x in args.oneshot_kbs.split(",")):
+        n = (kb << 10) // es
+        layers = [(0, n, width, args.bucket)]
+        g = C.LocalSraGroup(W, lanes, n * es * 2 + (1 << 20), 20000, 4096)
+        xs = [torch.randn(n, device=dev).to(dtype) for _ in range(W)]
+        g.allreduce_oneshot(xs, layers, bits=fmt)
+        torch.cuda.synchronize()
+        g.check()
+        res[kb] = timeit(lambda: g.allreduce_oneshot(xs, layers, bits=fmt), iters=50, warmup=10)
+        del g, xs
+    row = {"kernel": "oneshot", "world": W, "dtype": dt, "bits": bits, "bucket": args.bucket, "lanes_per_rank": lanes,
+           "times_us_by_kb": {str(k): round(v, 1) for k, v in res.items()},
+           "note": "one call of W virtual ranks, each `kb` KB: the one-shot kernel's latency-bound sizes"}
+    rows.append(row)
+    print(json.dumps(row), flush=True)
     res = {}
     for mb in mbs:
         n = (mb << 20) // es // W * W

@@ -41,6 +41,9 @@ SOURCES = [
     "kernels/ag_f32.cu",
     "kernels/ag_f16.cu",
     "kernels/ag_bf16.cu",
+    "kernels/sra_fp8_f32.cu",
+    "kernels/sra_fp8_f16.cu",
+    "kernels/sra_fp8_bf16.cu",
     "kernels/a2a_f32.cu",
     "kernels/a2a_f16.cu",
     "kernels/a2a_bf16.cu",

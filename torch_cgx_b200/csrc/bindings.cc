@@ -139,9 +139,13 @@ float sim_prescale(std::optional<double> prescale, bool average, int W) {
   return prescale ? (float)*prescale : average ? 1.0f / (float)W : 1.0f;
 }
 
+WireCodec allreduce_codec(const std::optional<std::variant<int64_t, std::string>>& bits,
+                          const std::vector<LayerSpec>& layers, bool stochastic);
+
 void py_sra_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int lanes,
                      bool average, bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                     int64_t min_lane_elems, std::optional<double> prescale) {
+                     int64_t min_lane_elems, std::optional<double> prescale,
+                     const std::optional<std::variant<int64_t, std::string>>& bits) {
   TORCH_CHECK(!tensors.empty(), "need tensors");
   const int W = (int)tensors.size();
   const int dt = cgx_dtype(tensors[0]);
@@ -150,13 +154,16 @@ void py_sra_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTup
     TORCH_CHECK(t.device().is_cpu() && t.is_contiguous() && cgx_dtype(t) == dt, "sra_simulate: CPU contiguous tensors of one dtype");
     bufs.push_back(t.data_ptr());
   }
-  Plan plan = build_plan(to_layers(layers), make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
-  sra_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
+  const auto specs = to_layers(layers);
+  const WireCodec codec = allreduce_codec(bits, specs, stochastic);
+  Plan plan = build_plan(specs, make_opts(W, lanes, dt, skip_incomplete, min_lane_elems));
+  sra_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq), codec);
 }
 
 void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int lanes,
                          bool average, bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                         int64_t min_lane_elems, std::optional<double> prescale) {
+                         int64_t min_lane_elems, std::optional<double> prescale,
+                         const std::optional<std::variant<int64_t, std::string>>& bits) {
   TORCH_CHECK(!tensors.empty(), "need tensors");
   const int W = (int)tensors.size();
   const int dt = cgx_dtype(tensors[0]);
@@ -165,8 +172,10 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
     TORCH_CHECK(t.device().is_cpu() && t.is_contiguous() && cgx_dtype(t) == dt, "oneshot_simulate: CPU contiguous tensors");
     bufs.push_back(t.data_ptr());
   }
-  Plan plan = build_plan(to_layers(layers), make_opts(1, lanes, dt, skip_incomplete, min_lane_elems));
-  oneshot_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq));
+  const auto specs = to_layers(layers);
+  const WireCodec codec = allreduce_codec(bits, specs, stochastic);
+  Plan plan = build_plan(specs, make_opts(1, lanes, dt, skip_incomplete, min_lane_elems));
+  oneshot_simulate(plan, bufs, sim_prescale(prescale, average, W), make_rng(stochastic, seed, seq), codec);
 }
 
 // The `bits` of every all-to-all, reduce-scatter and all-gather binding: 1..8 or 32 (max-min levels,
@@ -208,6 +217,11 @@ WireCodec sharded_codec(const std::optional<A2aBitsArg>& bits, const std::vector
         throw py::value_error(std::string("cgx ") + op + ": an FP8 format needs layers of bits 8 or 32, got " +
                               std::to_string(l.bits));
   return wb.codec;
+}
+// the same for the allreduce bindings that take a layer table
+WireCodec allreduce_codec(const std::optional<A2aBitsArg>& bits, const std::vector<LayerSpec>& layers,
+                          bool stochastic) {
+  return sharded_codec(bits, layers, stochastic, "allreduce");
 }
 
 // Argument checks of the sharded simulators: one CPU contiguous input and output per rank, all of
@@ -525,13 +539,18 @@ class LocalSraGroup {
   }
 
   // in-place allreduce of W same-device tensors, one per virtual rank
+  // `bits`: None or an integer keeps max-min, an FP8 format name sends the 8-bit layers as FP8
   void allreduce_oneshot(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
-                         bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
-    run(std::move(tensors), layers, average, skip_incomplete, stochastic, seed, seq, true);
+                         bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
+                         const std::optional<A2aBitsArg>& bits) {
+    run(std::move(tensors), layers, average, skip_incomplete, stochastic, seed, seq, true, -1,
+        allreduce_codec(bits, to_layers(layers), stochastic));
   }
   void allreduce(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
-                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
-    run(std::move(tensors), layers, average, skip_incomplete, stochastic, seed, seq, false);
+                 bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
+                 const std::optional<A2aBitsArg>& bits) {
+    run(std::move(tensors), layers, average, skip_incomplete, stochastic, seed, seq, false, -1,
+        allreduce_codec(bits, to_layers(layers), stochastic));
   }
   // fault injection: virtual rank `absent` never launches its kernel (a dead / stuck peer)
   void allreduce_with_absent_rank(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers,
@@ -546,7 +565,8 @@ class LocalSraGroup {
     for (auto& f : fused_) f->clear_status();
   }
   void run(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
-           bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq, bool oneshot, int absent = -1) {
+           bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq, bool oneshot, int absent = -1,
+           WireCodec codec = kMaxMin) {
     TORCH_CHECK((int)tensors.size() == world_, "need one tensor per virtual rank");
     const int dt = cgx_dtype(tensors[0]);
     for (const at::Tensor& t : tensors)
@@ -564,9 +584,9 @@ class LocalSraGroup {
         [&](int r) {
           if (r == absent) return;
           if (oneshot)
-            fused_[r]->run_oneshot(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
+            fused_[r]->run_oneshot(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream(), codec);
           else
-            fused_[r]->run(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream());
+            fused_[r]->run(*plans[r], tensors[r].data_ptr(), ps, rng, streams_[r].stream(), codec);
         });
   }
 
@@ -743,21 +763,25 @@ class LocalReducerGroup {
   // in-place allreduce of one tensor per virtual rank; the prescale is 1/W when averaging unless given
   void allreduce(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
                  bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
-                 std::optional<double> prescale_in) {
+                 std::optional<double> prescale_in, const std::optional<A2aBitsArg>& bits) {
     const auto specs = to_layers(layers);
+    const WireCodec codec = allreduce_codec(bits, specs, stochastic);
+    if (codec != kMaxMin && kind_ == ReductionType::kAllToAll) throw py::value_error(kAllToAllNoFp8);
     const RngParams rng = make_rng(stochastic, seed, seq);
     const float prescale = sim_prescale(prescale_in, average, hub_.world());
     run(tensors, [&](Reducer& red, int, void* data, int dt, cudaStream_t s) {
-      red.allreduce(data, dt, specs, skip_incomplete, prescale, rng, s);
+      red.allreduce(data, dt, specs, skip_incomplete, prescale, rng, s, codec);
     });
   }
   void broadcast_compressed(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, int root,
-                            bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq) {
+                            bool skip_incomplete, bool stochastic, uint64_t seed, uint32_t seq,
+                            const std::optional<A2aBitsArg>& bits) {
     TORCH_CHECK(root >= 0 && root < hub_.world(), "LocalReducerGroup: bad root ", root);
     const auto specs = to_layers(layers);
+    const WireCodec codec = allreduce_codec(bits, specs, stochastic);
     const RngParams rng = make_rng(stochastic, seed, seq);
     run(tensors, [&](Reducer& red, int, void* data, int dt, cudaStream_t s) {
-      red.broadcast_compressed(data, dt, specs, skip_incomplete, root, rng, s);
+      red.broadcast_compressed(data, dt, specs, skip_incomplete, root, rng, s, codec);
     });
   }
   // Reducer::reduce_scatter: inputs[r] holds W * S elements, outputs[r] receives shard r
@@ -1025,19 +1049,29 @@ class LocalEngineGroup {
     engines_.clear();
   }
 
-  void allreduce(std::vector<at::Tensor> tensors, bool average, int explicit_bucket, bool overlapped) {
+  // `bits`, when given, is the wire format of the 8-bit layers (a2a_bits: an FP8 name, or an integer
+  // for max-min) in place of CGX_COMPRESSION_FORMAT's; the widths stay the environment's / the table's
+  void allreduce(std::vector<at::Tensor> tensors, bool average, int explicit_bucket, bool overlapped,
+                 const std::optional<A2aBitsArg>& bits) {
+    const std::optional<WireCodec> codec = format_of(bits);
     run(tensors, [&](AllreduceEngine& e, int, void* data, int dt, int64_t n, bool cuda, cudaStream_t s) {
-      if (cuda)
-        e.allreduce_cuda(data, dt, n, average, explicit_bucket, s, overlapped);
-      else
-        e.allreduce_cpu(data, dt, n, average, explicit_bucket);
+      if (cuda) {
+        e.allreduce_cuda(data, dt, n, average, explicit_bucket, s, overlapped, codec);
+      } else {
+        AllreduceEngine::CpuCall call = e.prepare_cpu(n, explicit_bucket);
+        if (codec) call.env.codec = *codec;
+        e.allreduce_cpu_prepared(data, dt, call, average);
+      }
     });
   }
-  void allreduce_layers(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average) {
+  void allreduce_layers(std::vector<at::Tensor> tensors, const std::vector<LayerTuple>& layers, bool average,
+                        const std::optional<A2aBitsArg>& bits) {
     const auto specs = to_layers(layers);
+    const std::optional<WireCodec> codec = format_of(bits);
     run(tensors, [&](AllreduceEngine& e, int, void* data, int dt, int64_t, bool cuda, cudaStream_t s) {
       AllreduceEngine::CpuCall call;
       call.env = CompressionEnv::read();
+      if (codec) call.env.codec = *codec;
       call.layers = specs;
       if (cuda)
         e.allreduce_cuda_layers(data, dt, specs, average, call.env, s);
@@ -1187,6 +1221,10 @@ class LocalEngineGroup {
     std::vector<Entry> log;
   };
 
+  static std::optional<WireCodec> format_of(const std::optional<A2aBitsArg>& bits) {
+    if (!bits) return std::nullopt;
+    return a2a_bits(*bits, CompressionEnv::read().stochastic, "allreduce").codec;
+  }
   static ReductionType reduction(const std::string& k) {
     if (k == "SRA") return ReductionType::kSRA;
     if (k == "RING") return ReductionType::kRing;
@@ -1479,8 +1517,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   py::module::import("torch._C._distributed_c10d");
 
   py::class_<ProcessGroupCGX, c10d::Backend, c10::intrusive_ptr<ProcessGroupCGX>>(m, "ProcessGroupCGX")
-      .def("allreduce_bucket", &ProcessGroupCGX::allreduce_bucket, py::arg("tensor"), py::arg("bucket_idx"),
-           py::arg("average") = false, py::call_guard<py::gil_scoped_release>())
+      .def(
+          "allreduce_bucket",
+          [](ProcessGroupCGX& pg, at::Tensor& tensor, int64_t bucket_idx, bool average,
+             const std::optional<A2aBitsArg>& bits) {
+            // an FP8 name replaces CGX_COMPRESSION_FORMAT's wire format; the widths stay the registry's
+            std::optional<WireCodec> codec;
+            if (bits) codec = a2a_bits(*bits, CompressionEnv::read().stochastic, "allreduce").codec;
+            py::gil_scoped_release nogil;
+            return pg.allreduce_bucket(tensor, bucket_idx, average, codec);
+          },
+          py::arg("tensor"), py::arg("bucket_idx"), py::arg("average") = false, py::arg("bits") = py::none())
       .def("reduce_scatter_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, bool average, const A2aBitsArg& bits,
               int bucket_size, bool skip_incomplete, bool stochastic, int64_t seed, bool overlapped,
@@ -1568,10 +1615,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       }, py::arg("assignment"));
   m.def("register_native_hook",
         [](const std::shared_ptr<c10d::Reducer>& reducer, const c10::intrusive_ptr<ProcessGroupCGX>& pg,
-           int64_t layer_min_size, int bits, int bucket_size, int register_step, std::vector<int64_t> candidates,
-           int64_t period, Assignment assignment) {
-          return register_native_hook(reducer, pg, layer_min_size, bits, bucket_size, register_step,
-                                      std::move(candidates), period, std::move(assignment));
+           int64_t layer_min_size, const A2aBitsArg& bits, int bucket_size, int register_step,
+           std::vector<int64_t> candidates, int64_t period, Assignment assignment) {
+          // an FP8 name: layers registered at 8 bits, sent in that format
+          const A2aBits wb = a2a_bits(bits, false, "allreduce");
+          std::optional<WireCodec> codec;
+          if (wb.codec != kMaxMin) codec = wb.codec;
+          return register_native_hook(reducer, pg, layer_min_size, wb.bits, bucket_size, register_step,
+                                      std::move(candidates), period, std::move(assignment), codec);
         },
         py::arg("reducer"), py::arg("backend"), py::arg("layer_min_size"), py::arg("bits"), py::arg("bucket_size"),
         py::arg("register_step") = 2, py::arg("candidates") = std::vector<int64_t>{}, py::arg("period") = 1,
@@ -1686,7 +1737,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   m.def("sra_simulate", &py_sra_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
+        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none(),
+        py::arg("bits") = py::none());
   m.def("reduce_scatter_simulate", &py_reduce_scatter_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("lanes") = 1, py::arg("average") = false, py::arg("skip_incomplete") = false,
         py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048,
@@ -1715,7 +1767,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("bits") = py::none());
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none());
+        py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none(),
+        py::arg("bits") = py::none());
   m.def("quantize", &py_quantize, py::arg("tensor"), py::arg("layers"), py::arg("world") = 1, py::arg("lanes") = 1,
         py::arg("skip_incomplete") = false, py::arg("prescale") = 1.0f, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("rank") = 0, py::arg("phase") = 0,
@@ -1798,10 +1851,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("slot_bytes"), py::arg("timeout_ms") = 5000, py::arg("min_lane_elems") = 2048)
       .def("allreduce", &LocalSraGroup::allreduce, py::arg("tensors"), py::arg("layers"), py::arg("average") = false,
            py::arg("skip_incomplete") = false, py::arg("stochastic") = false, py::arg("seed") = 0,
-           py::arg("seq") = 0)
+           py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("allreduce_oneshot", &LocalSraGroup::allreduce_oneshot, py::arg("tensors"), py::arg("layers"),
            py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-           py::arg("seed") = 0, py::arg("seq") = 0)
+           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("reduce_scatter", &LocalSraGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
@@ -1823,10 +1876,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("timeout_ms") = 10000)
       .def("allreduce", &LocalReducerGroup::allreduce, py::arg("tensors"), py::arg("layers"),
            py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none())
+           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none(), py::arg("bits") = py::none())
       .def("broadcast_compressed", &LocalReducerGroup::broadcast_compressed, py::arg("tensors"), py::arg("layers"),
            py::arg("root"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false, py::arg("seed") = 0,
-           py::arg("seq") = 0)
+           py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("reduce_scatter", &LocalReducerGroup::reduce_scatter, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("prescale") = py::none(),
@@ -1846,9 +1899,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def(py::init<int, int, const py::dict&, int, int64_t, int64_t>(), py::arg("world"), py::arg("local_size"),
            py::arg("config"), py::arg("lanes") = 2, py::arg("slot_bytes") = 1 << 20, py::arg("timeout_ms") = 20000)
       .def("allreduce", &LocalEngineGroup::allreduce, py::arg("tensors"), py::arg("average") = false,
-           py::arg("explicit_bucket") = -1, py::arg("overlapped") = false)
+           py::arg("explicit_bucket") = -1, py::arg("overlapped") = false, py::arg("bits") = py::none())
       .def("allreduce_layers", &LocalEngineGroup::allreduce_layers, py::arg("tensors"), py::arg("layers"),
-           py::arg("average") = false)
+           py::arg("average") = false, py::arg("bits") = py::none())
       .def("reduce_scatter",
            [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out, bool average,
               std::optional<std::vector<LayerTuple>> shard_layers, std::optional<A2aBitsArg> bits) {

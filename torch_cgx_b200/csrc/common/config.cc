@@ -5,6 +5,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <stdexcept>
+
+#include "quant_math.h"
 
 namespace cgx {
 
@@ -87,7 +90,16 @@ CompressionEnv CompressionEnv::read() {
   c.skip_incomplete = env_bool(kEnvSkipIncomplete, false);
   c.stochastic = env_bool(kEnvStochastic, false);
   c.seed = (uint64_t)env_int(kEnvSeed, 0);
+  c.codec = parse_wire_format(env_str(kEnvFormat, ""), kEnvFormat);
   return c;
+}
+
+int parse_wire_format(const std::string& name, const char* what) {
+  if (name.empty() || name == "maxmin") return kMaxMin;
+  if (name == "e4m3") return kE4M3;
+  if (name == "e5m2") return kE5M2;
+  throw std::invalid_argument(std::string("cgx: ") + what + " must be \"maxmin\", \"e4m3\" or \"e5m2\", got \"" +
+                              name + "\"");
 }
 
 EngineConfig EngineConfig::read() {

@@ -43,6 +43,8 @@ constexpr const char* kEnvOverlapLanes = "CGX_OVERLAP_LANES";  // CTAs of a DDP-
 constexpr const char* kEnvVmm = "CGX_VMM";                      // 0: cudaMalloc + cudaIpc heap instead of VMM + fd handles
 constexpr const char* kEnvNvls = "CGX_NVLS";                    // 0: never create the NVLS multicast mapping
 constexpr const char* kEnvNvlsReduce = "CGX_NVLS_REDUCE";       // 0: raw layers use the two-shot path even with NVLS
+constexpr const char* kEnvFormat = "CGX_COMPRESSION_FORMAT";    // wire format of the allreduce's 8-bit layers:
+                                                                // unset / "maxmin", "e4m3" or "e5m2"
 
 constexpr int kDefaultBits = 32;          // 32 == compression off
 constexpr int kDefaultBucketSize = 512;   // reference compressor.h:32
@@ -71,8 +73,11 @@ struct CompressionEnv {
   bool skip_incomplete = false;
   bool stochastic = false;
   uint64_t seed = 0;
+  int codec = 0;  // WireCodec (quant_math.h) of CGX_COMPRESSION_FORMAT; std::invalid_argument on an unknown name
   static CompressionEnv read();
 };
+// "maxmin" (or empty) / "e4m3" / "e5m2" -> WireCodec; std::invalid_argument naming `what` otherwise
+int parse_wire_format(const std::string& name, const char* what);
 
 // Read once per engine.
 struct EngineConfig {

@@ -9,7 +9,8 @@
 
 namespace cgx {
 
-void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng) {
+void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng,
+                  WireCodec codec) {
   const int W = plan.world;
   if ((int)bufs.size() != W) throw std::invalid_argument("sra_simulate: need one buffer per rank");
   std::vector<float> acc(kMaxBlockElems), tmp(kMaxBlockElems);
@@ -18,6 +19,17 @@ void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float presca
     for (uint32_t b = plan.chunk_begin(c); b < plan.chunk_end(c); ++b) {
       const BlockDesc& d = plan.blocks[b];
       cpu::load_block(bufs[c], plan.dtype, d, prescale, acc.data());
+      if (codec != kMaxMin && block_bits(d) < kRawBits) {
+        for (int q = 0; q < W; ++q) {
+          if (q == c) continue;
+          cpu::load_block(bufs[q], plan.dtype, d, prescale, tmp.data());
+          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+          cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
+        }
+        cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+        for (int p = 0; p < W; ++p) cpu::decode_block_fp8_store(rec.data(), plan.dtype, d, bufs[p], codec);
+        continue;
+      }
       for (int q = 0; q < W; ++q) {
         if (q == c) continue;
         cpu::load_block(bufs[q], plan.dtype, d, prescale, tmp.data());
@@ -59,7 +71,8 @@ void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& i
   }
 }
 
-void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng) {
+void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng,
+                      WireCodec codec) {
   if (plan.world != 1) throw std::invalid_argument("oneshot_simulate: plan must have a single chunk");
   const int W = (int)bufs.size();
   std::vector<float> acc(kMaxBlockElems), tmp(kMaxBlockElems);
@@ -70,6 +83,11 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
     for (uint32_t i = 0; i < n; ++i) acc[i] = 0.f;
     for (int q = 0; q < W; ++q) {
       cpu::load_block(bufs[q], plan.dtype, d, prescale, tmp.data());
+      if (codec != kMaxMin && block_bits(d) < kRawBits) {
+        cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+        cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
+        continue;
+      }
       cpu::quantize_block(tmp.data(), plan.dtype, d, rec.data(), make_rng_key(rng, q, 0), b);
       cpu::decode_block_add(rec.data(), plan.dtype, d, acc.data());
     }

@@ -30,11 +30,18 @@ inline RngKey make_rng_key(const RngParams& r, int rank, int phase) {
 }
 
 // bufs[r] = base pointer of rank r's tensor (dtype plan.dtype), reduced in place.
-void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng);
+// An FP8 `codec` (8-bit plans; raw blocks are the same either way): chunk c's owner sums
+// fl(x_c * prescale) and, for every q != c in rank order, fl(float(code_q) * unit_q) of the FP8
+// record of fl(x_q * prescale), each add rounded on its own; the fp32 sum is encoded once and every
+// rank stores the values decoded from those codes. Round to nearest.
+void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng,
+                  WireCodec codec = kMaxMin);
 
 // One-shot allreduce oracle: result = T( sum over ranks r (in order) of decode(Q_r(x_r * prescale)) ),
 // every contribution quantized exactly once; `plan` must be a single-chunk plan (world == 1).
-void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng);
+// An FP8 `codec`: Q_r is the FP8 record and the sum starts from +0.
+void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float prescale, const RngParams& rng,
+                      WireCodec codec = kMaxMin);
 
 // Reduce-scatter oracle (rs_kernel): `plan` covers a shard table replicated W times at stride
 // `shard` elements, so chunk c is copy c. out_bufs[c][e - c * shard] = T(prescale * in_c[e] + sum over

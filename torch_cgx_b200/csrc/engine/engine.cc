@@ -108,7 +108,7 @@ static std::vector<LayerSpec> resolve_layers(int64_t numel, const EngineConfig& 
 }
 
 void AllreduceEngine::launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream,
-                                   const std::vector<LayerSpec>* layers) {
+                                   WireCodec codec, const std::vector<LayerSpec>* layers) {
   const int elsize = dtype_size(l.dp->plan.dtype);
   rng.seq = (rng.seq << 3) | (l.rng_sub & 7u);
   const int lw = fused_->world(), lr = fused_->rank();
@@ -117,11 +117,11 @@ void AllreduceEngine::launch_fused(const Launch& l, void* data, float prescale, 
     observer_->before_fused_launch(*l.dp, stream);
   }
   if (l.oneshot) {
-    fused_->run_oneshot(*l.dp, data, prescale, rng, stream);
+    fused_->run_oneshot(*l.dp, data, prescale, rng, stream, codec);
     stats_.wire_bytes += l.dp->plan.total_wire * (uint64_t)(lw - 1);
     stats_.raw_bytes += l.dp->plan.numel * (uint64_t)elsize * (uint64_t)(lw - 1);
   } else {
-    fused_->run(*l.dp, data, prescale, rng, stream);
+    fused_->run(*l.dp, data, prescale, rng, stream, codec);
     // bytes pushed by this rank: phase A = every chunk but mine, phase B = mine to W-1 peers
     const uint64_t mine = l.dp->plan.chunk_wire_bytes[lr];
     stats_.wire_bytes += (l.dp->plan.total_wire - mine) + mine * (uint64_t)(lw - 1);
@@ -134,10 +134,11 @@ void AllreduceEngine::launch_fused(const Launch& l, void* data, float prescale, 
 }
 
 void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool average, int explicit_bucket,
-                                     cudaStream_t stream, bool overlapped) {
+                                     cudaStream_t stream, bool overlapped, std::optional<WireCodec> codec) {
   if (numel <= 0) return;
   NvtxRange range("cgx:allreduce_cuda", (uint64_t)numel);
   CompressionEnv env = CompressionEnv::read();
+  if (codec) env.codec = *codec;
   const bool cacheable = explicit_bucket >= 0 && explicit_bucket < 4096 && nodes() == 1 && fused_ &&
                          cfg_.inner_comm == CommType::kP2P && !cfg_.dummy_compression && cfg_.fake_ratio >= 1.0;
   if (cacheable) {
@@ -145,7 +146,7 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
     BucketFast& f = fast_[(size_t)explicit_bucket];
     const uint64_t ver = LayerRegistry::instance().version();
     if (f.registry_version == ver && f.plan_generation == fused_->generation() && f.numel == numel &&
-        f.dtype == dtype && f.env_bits == env.bits && f.env_bucket == env.bucket_size &&
+        f.dtype == dtype && f.env_bits == env.bits && f.env_bucket == env.bucket_size && f.env_codec == env.codec &&
         f.skip_incomplete == env.skip_incomplete && f.overlapped == overlapped && !f.launches.empty()) {
       fused_->check_status();
       ++call_seq_;
@@ -157,7 +158,7 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
       // the sequence numbers of the slow path: fusion group in the call's, piece in the launch's
       for (const Launch& l : f.launches) {
         rng.seq = (call_seq_ << 4) | (l.rng_group & 15u);
-        launch_fused(l, data, prescale, rng, stream);
+        launch_fused(l, data, prescale, rng, stream, (WireCodec)env.codec);
       }
       return;
     }
@@ -184,6 +185,7 @@ void AllreduceEngine::allreduce_cuda(void* data, int dtype, int64_t numel, bool 
     f.dtype = dtype;
     f.env_bits = env.bits;
     f.env_bucket = env.bucket_size;
+    f.env_codec = env.codec;
     f.skip_incomplete = env.skip_incomplete;
     f.overlapped = overlapped;
     f.launches = std::move(rec);
@@ -415,7 +417,8 @@ void AllreduceEngine::allreduce_cuda_layers(void* data, int dtype, const std::ve
 // One node-local allreduce of a fusion group: fused P2P kernel when available,
 // otherwise the generic reducer over the intra-node communicator.
 void AllreduceEngine::intra_stage(bool cuda, void* data, int dtype, const std::vector<LayerSpec>& group,
-                                  bool skip_incomplete, float prescale, RngParams rng, cudaStream_t stream) {
+                                  bool skip_incomplete, float prescale, RngParams rng, cudaStream_t stream,
+                                  WireCodec codec) {
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const int elsize = dtype_size(dtype);
   // the fused kernel implements SRA (+ the one-shot variant); an explicitly requested Ring or
@@ -430,7 +433,7 @@ void AllreduceEngine::intra_stage(bool cuda, void* data, int dtype, const std::v
         const DevicePlan* dp = fused_->prepare_oneshot(group, dtype, skip_incomplete, stream, lane_cap_);
         // every rank pushes its whole packed image to W-1 peers: keep that egress small
         if (dp != nullptr && dp->plan.total_wire * (uint64_t)(fused_->world() - 1) <= (4ull << 20)) {
-          launch_fused(Launch{dp, true, rng.seq & 15u, 0u}, data, prescale, rng, stream, &group);
+          launch_fused(Launch{dp, true, rng.seq & 15u, 0u}, data, prescale, rng, stream, codec, &group);
           return;
         }
       }
@@ -463,14 +466,14 @@ void AllreduceEngine::intra_stage(bool cuda, void* data, int dtype, const std::v
         }
         continue;
       }
-      launch_fused(Launch{dp, false, rng.seq & 15u, sub++}, data, prescale, rng, stream, &gl);
+      launch_fused(Launch{dp, false, rng.seq & 15u, sub++}, data, prescale, rng, stream, codec, &gl);
     }
     return;
   }
   if (g.intra) {
     const uint64_t before = g.intra->bytes_sent();
     observe(EngineStage::kGenericIntra, &group, rng, prescale);
-    g.intra->allreduce(data, dtype, group, skip_incomplete, prescale, rng, stream);
+    g.intra->allreduce(data, dtype, group, skip_incomplete, prescale, rng, stream, codec);
     stats_.wire_bytes += g.intra->bytes_sent() - before;
     uint64_t n = 0;
     for (const LayerSpec& l : group) n += l.numel;
@@ -489,12 +492,23 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
     for (LayerSpec& l : layers) l.bits = kRawBits;
   const int elsize = dtype_size(dtype);
   const float prescale = average ? 1.0f / (float)world_ : 1.0f;
+  const bool multi_node = nodes() > 1;
+  const WireCodec codec = (WireCodec)env.codec;
+  if (codec != kMaxMin) {  // checked before anything is counted or sent
+    if (env.stochastic) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
+    for (const LayerSpec& l : layers)
+      if (l.bits != 8 && l.bits < kRawBits)
+        throw std::invalid_argument("cgx allreduce: an FP8 format needs layers of bits 8 or 32, got " +
+                                    std::to_string(l.bits));
+    if (cfg_.inner_reduction == ReductionType::kAllToAll ||
+        (multi_node && cfg_.cross_reduction == ReductionType::kAllToAll))
+      throw std::invalid_argument(kAllToAllNoFp8);
+  }
   ++call_seq_;
   ++stats_.calls;
   RngParams rng;
   rng.seed = env.seed;
   rng.stochastic = env.stochastic;
-  const bool multi_node = nodes() > 1;
   if (multi_node && !g.cross) throw std::runtime_error("cgx: multi-node topology but no cross-node reducer");
 
   uint32_t sub = 0;
@@ -506,7 +520,7 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
       for (LayerSpec& l : intra_layers) l.bits = kRawBits;
     if (local_size_ > 1 || !multi_node) {
       NvtxRange r1("cgx:intra_node", (uint64_t)intra_layers.size());
-      intra_stage(cuda, data, dtype, intra_layers, env.skip_incomplete, prescale, rng, stream);
+      intra_stage(cuda, data, dtype, intra_layers, env.skip_incomplete, prescale, rng, stream, codec);
     }
     if (!multi_node) continue;
     NvtxRange r2("cgx:cross_node", (uint64_t)group.size());
@@ -517,7 +531,7 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
     if (cfg_.intra_broadcast && local_size_ > 1) {
       if (local_rank() == 0) {
         observe(EngineStage::kCross, &group, crng, cross_scale);
-        g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream);
+        g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream, codec);
       }
       // leaders hand the result to the rest of their node: packed when the intra-node stage
       // compresses (reference: Reducer::Broadcast with do_compression && intra_compress_,
@@ -529,7 +543,7 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
         brng.seq = rng.seq ^ 0x20000000u;
         const uint64_t before = g.intra->bytes_sent();
         observe(EngineStage::kBcastCompressed, &group, brng, 1.0f);
-        g.intra->broadcast_compressed(data, dtype, group, env.skip_incomplete, 0, brng, stream);
+        g.intra->broadcast_compressed(data, dtype, group, env.skip_incomplete, 0, brng, stream, codec);
         stats_.wire_bytes += g.intra->bytes_sent() - before;
       } else {
         uint64_t lo = ~0ull, hi = 0;
@@ -544,7 +558,7 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
       }
     } else {
       observe(EngineStage::kCross, &group, crng, cross_scale);
-      g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream);
+      g.cross->allreduce(data, dtype, group, env.skip_incomplete, cross_scale, crng, stream, codec);
     }
   }
 }

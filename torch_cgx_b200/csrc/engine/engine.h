@@ -10,6 +10,7 @@
 #include <cstdint>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <vector>
 
 #include "../comm/symmetric_heap.h"
@@ -124,8 +125,12 @@ class AllreduceEngine {
   //  explicit_bucket: DDP bucket index if the caller knows it, else -1.
   //  overlapped: the call runs concurrently with compute (DDP hook) -> use at most
   //  cfg.overlap_lanes CTAs instead of the whole GPU.
+  //  codec: the wire format of the 8-bit layers, replacing CGX_COMPRESSION_FORMAT's when given.
+  // With an FP8 format (CompressionEnv::codec) every layer must have bits 8 or 32 and rounding is to
+  // nearest; every compressed stage (node-local, cross-node, the leaders' compressed broadcast) uses
+  // it. std::invalid_argument otherwise, before any stage runs.
   void allreduce_cuda(void* data, int dtype, int64_t numel, bool average, int explicit_bucket,
-                      cudaStream_t stream, bool overlapped = false);
+                      cudaStream_t stream, bool overlapped = false, std::optional<WireCodec> codec = std::nullopt);
   // Same, with an explicit layer list (offsets relative to `data`).
   void allreduce_cuda_layers(void* data, int dtype, const std::vector<LayerSpec>& layers, bool average,
                              const CompressionEnv& env, cudaStream_t stream, bool overlapped = false);
@@ -177,7 +182,7 @@ class AllreduceEngine {
   void run_layers(bool cuda, void* data, int dtype, std::vector<LayerSpec> layers, bool average,
                   const CompressionEnv& env, cudaStream_t stream);
   void intra_stage(bool cuda, void* data, int dtype, const std::vector<LayerSpec>& group, bool skip_incomplete,
-                   float prescale, RngParams rng, cudaStream_t stream);
+                   float prescale, RngParams rng, cudaStream_t stream, WireCodec codec);
   // the node-local stage of a sharded call over the local ranks: fused kernel or generic reducer
   void sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
                      const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale, const RngParams& rng,
@@ -201,7 +206,7 @@ class AllreduceEngine {
     uint64_t plan_generation = 0;
     int64_t numel = -1;
     int dtype = -1;
-    int env_bits = 0, env_bucket = 0;
+    int env_bits = 0, env_bucket = 0, env_codec = 0;
     bool skip_incomplete = false;
     bool overlapped = false;
     std::vector<Launch> launches;
@@ -209,7 +214,7 @@ class AllreduceEngine {
   std::vector<BucketFast> fast_;
   std::vector<Launch>* recording_ = nullptr;
   void launch_fused(const Launch& l, void* data, float prescale, RngParams rng, cudaStream_t stream,
-                    const std::vector<LayerSpec>* layers = nullptr);
+                    WireCodec codec, const std::vector<LayerSpec>* layers = nullptr);
   void observe(EngineStage::Kind kind, const std::vector<LayerSpec>* layers, const RngParams& rng, float scale) {
     if (observer_) observer_->stage(EngineStage{kind, layers, nullptr, rng, scale});
   }

@@ -412,7 +412,14 @@ cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint
 
 cudaError_t launch_quantize_items_f32(const ItemKernelArgs& a, const float* src_f32, uint32_t base_elem,
                                       uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) {
-  if (a.codec != kMaxMin) return cudaErrorInvalidValue;
+  if (a.codec != kMaxMin) {
+    // the FP8 kernels of an fp32 tensor, on the scratch seen from the tensor's element 0 (items
+    // address src + elem_off), then out = decode(wire)
+    if (rng.enabled) return cudaErrorInvalidValue;
+    cudaError_t e = quantize_fp8_t<float>(a, src_f32 - base_elem, wire, 1.0f, stream);
+    if (e != cudaSuccess || out == nullptr) return e;
+    return launch_dequantize_items(a, wire, out, stream);
+  }
   CGX_BY_DTYPE(a.dtype, (quantize_t<float, float>(a, src_f32, base_elem, wire, 1.0f, rng, (float*)out, stream)),
                (quantize_t<float, __half>(a, src_f32, base_elem, wire, 1.0f, rng, (__half*)out, stream)),
                (quantize_t<float, __nv_bfloat16>(a, src_f32, base_elem, wire, 1.0f, rng, (__nv_bfloat16*)out, stream)))

@@ -1073,5 +1073,91 @@ __device__ __noinline__ void bucket_rs_fp8(const T* src, const WarpItem it, floa
   }
 }
 
+// ======================================================================================
+// FP8 in the allreduce (sra_kernel phase B, oneshot_kernel phase 2). Phase B sums as the
+// reduce-scatter does -- my values * prescale, then fl(float(code) * unit) of every source in slot
+// order, each add rounded on its own -- encodes the fp32 sum once, publishes meta + codes and writes
+// the values decoded from its own codes to `blk`, so every rank ends with the same bytes. The
+// one-shot receiver sums the decoded values of every source, its own included, from +0.
+// ======================================================================================
+template <typename T, int CODEC, int GPL, bool VEC, typename DST>
+__device__ __forceinline__ void full_reduce_fp8_x(float (&x)[GPL][8], T* __restrict__ blk, const WarpItem& it,
+                                                  float prescale, const SrcSet& ss, const DST& ds) {
+  slice_scale<GPL>(x, prescale);
+  slice_accumulate_fp8<CODEC, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), x);
+  full_publish_fp8_x<T, CODEC, GPL, VEC>(x, it, ds, blk);
+}
+template <typename T, int CODEC, int GPL, typename DST>
+__device__ __noinline__ void full_reduce_fp8_unaligned(T* __restrict__ blk, const WarpItem it, float prescale,
+                                                       const SrcSet ss, const DST ds) {
+  float x[GPL][8];
+  slice_load_scalar<T, GPL>(blk, x);
+  full_reduce_fp8_x<T, CODEC, GPL, false>(x, blk, it, prescale, ss, ds);
+}
+
+// generic bucket item: two passes (min/max of the sums, then encode), as bucket_quantize; every
+// lane reads a group of `blk` before it writes the same group
+template <typename T, int CODEC, typename DST>
+__device__ __noinline__ void bucket_reduce_fp8(T* __restrict__ blk, const WarpItem it, float prescale,
+                                               const SrcSet ss, const DST ds) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  float mn = CGX_INF_POS, mx = CGX_INF_NEG;
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<T>(blk, g, n, prescale, x, nv);
+    bucket_add_sources_fp8<CODEC>(ss, it, g, x);
+    minmax8_pred(x, nv, mn, mx);
+  }
+  warp_minmax(mn, mx);
+  const BucketMeta m = fp8_meta(mn, mx, CODEC);
+  const float inv = fp8_inv_unit(m.unit);
+  const DST du = unicast_of(ds);
+  if (lane_id() == 0) dst_st_v2(du, it.meta_off, __float_as_uint(m.unit), __float_as_uint(m.min));
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+    int nv;
+    bucket_load_group<T>(blk, g, n, prescale, x, nv);
+    bucket_add_sources_fp8<CODEC>(ss, it, g, x);
+    uint32_t lo, hi;
+    fp8_encode8<CODEC>(x, inv, lo, hi);
+    const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
+    const uint32_t o = it.pay_off + g * 8u;
+    for (int t = 0; t < 8; ++t) dst_st_u8(du, o + t, (uint32_t)(w >> (8 * t)) & 0xFFu);
+    float dec[8];
+    fp8_decode8<CODEC>(lo, hi, m.unit, dec);
+    store8_scalar<T>(blk + g * 8u, nv, dec);
+  }
+}
+
+// out = sum of the decoded values of all sources, slot order, from +0 (one-shot phase 2)
+template <typename TO, int CODEC, int GPL, bool VEC>
+__device__ __forceinline__ void full_recv_sum_fp8(const SrcSet& ss, const WarpItem& it, TO* __restrict__ out) {
+  float x[GPL][8];
+#pragma unroll
+  for (int k = 0; k < GPL; ++k)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) x[k][j] = 0.f;
+  slice_accumulate_fp8<CODEC, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), x);
+  slice_store<TO, GPL, VEC>(out, x);
+}
+template <typename TO, int CODEC, int GPL>
+__device__ __noinline__ void full_recv_sum_fp8_unaligned(const SrcSet ss, const WarpItem it, TO* __restrict__ out) {
+  full_recv_sum_fp8<TO, CODEC, GPL, false>(ss, it, out);
+}
+template <typename TO, int CODEC>
+__device__ __noinline__ void bucket_recv_sum_fp8(const SrcSet ss, const WarpItem it, TO* __restrict__ out) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    float x[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) x[j] = 0.f;
+    bucket_add_sources_fp8<CODEC>(ss, it, g, x);
+    store8_scalar<TO>(out + g * 8u, (int)min(8u, n - g * 8u), x);
+  }
+}
+
 }  // namespace dev
 }  // namespace cgx

@@ -55,8 +55,8 @@ struct SraParams {
   uint64_t out_shift;            // reduce-scatter: element of `data` that lands on out[0];
                                  // all-gather: element of `out` that data[0] lands on (rank * shard stride)
   int gather;                    // with `out`: 1 = all-gather, 0 = reduce-scatter
-  int codec;                     // WireCodec of the reduce-scatter / all-gather (common/quant_math.h); an FP8
-                                 // codec needs uniform_bits 8
+  int codec;                     // WireCodec of the compressed items (common/quant_math.h); an FP8 codec
+                                 // needs uniform_bits 8
 };
 
 constexpr int kSraThreads = 256;
@@ -129,7 +129,7 @@ struct ItemKernelArgs {
   int slice_elems;
   int uniform_bits;
   int codec = 0;  // WireCodec: an FP8 codec needs an 8-bit plan whose items [first, first+count) are all
-                  // compressed, and deterministic rounding; launch_quantize_items_f32 does not take one
+                  // compressed, and deterministic rounding
 };
 // wire = quantize(src[T] * prescale)
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,

@@ -33,6 +33,14 @@ cudaError_t launch_sra_fused(const SraParams& p, cudaStream_t stream) {
       default: return cudaErrorInvalidValue;
     }
   }
+  if (p.codec != kMaxMin) {
+    switch (p.dtype) {
+      case kF32: return launch_sra_fp8_f32(p, stream);
+      case kF16: return launch_sra_fp8_f16(p, stream);
+      case kBF16: return launch_sra_fp8_bf16(p, stream);
+      default: return cudaErrorInvalidValue;
+    }
+  }
   switch (p.dtype) {
     case kF32: return launch_sra_f32(p, stream);
     case kF16: return launch_sra_f16(p, stream);

@@ -311,7 +311,9 @@ __device__ __forceinline__ void sra_phase_a(const SraParams& p, const LaneItems&
 
 // ---- phase B: reduce my chunk. The registers of this phase belong to the sources' words (four
 // sources in flight); the NEXT item's own values are only pulled towards L2.
-template <typename T, int KB, int GPL>
+// CODEC: the wire codec of the compressed items; an FP8 codec sums the decoded sources, encodes the
+// fp32 sum once and keeps the values decoded from its own codes (item_ops.cuh).
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems& li, uint32_t epoch, int stage) {
   const int r = p.rank, W = p.world;
   const int seg0 = stage * W;
@@ -332,6 +334,19 @@ __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems&
     if (i + kSraWarps < own_end) {
       const WarpItem itn = lane_item(li, p, i + kSraWarps, seg0);
       if (!(p.mc_reduce && item_kind(itn) == kItemRaw)) slice_prefetch_l2<T, GPL>(data + itn.elem_off);
+    }
+    if constexpr (CODEC != kMaxMin) {
+      if (kind == kItemFull) {
+        if (al)
+          full_reduce_fp8_x<T, CODEC, GPL, true>(x, blk, it, p.prescale, ss, ds);
+        else
+          full_reduce_fp8_unaligned<T, CODEC, GPL>(blk, it, p.prescale, ss, ds);
+        continue;
+      }
+      if (kind == kItemBucket) {
+        bucket_reduce_fp8<T, CODEC>(blk, it, p.prescale, ss, ds);
+        continue;
+      }
     }
     if (kind == kItemFull) {
       if (al)
@@ -477,8 +492,11 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
   }
 }
 
-template <typename T, int KB, int GPL>
+// CODEC: the wire codec of the compressed items; the FP8 ones exist with KB 8 only, in translation
+// units of their own (sra_fp8_*.cu)
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) sra_kernel(const __grid_constant__ SraParams p) {
+  static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   __shared__ LaneItems li;
   __shared__ int s_abort;
   const int lane = blockIdx.x;
@@ -489,7 +507,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) sra_kernel(const _
   trace_mark(p, lane, 0, true);
 
   _Pragma("unroll 1") for (int t = 0; t < stages; ++t) {
-    sra_phase_a<T, KB, GPL>(p, li, epoch, t);
+    sra_phase_a<T, KB, GPL, CODEC>(p, li, epoch, t);
     __syncthreads();
     trace_mark(p, lane, 1);
     if (threadIdx.x < 32) {
@@ -504,7 +522,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) sra_kernel(const _
     }
     __syncthreads();
     trace_mark(p, lane, 2);
-    if (!s_abort) sra_phase_b<T, KB, GPL>(p, li, epoch, t);
+    if (!s_abort) sra_phase_b<T, KB, GPL, CODEC>(p, li, epoch, t);
     __syncthreads();
     trace_mark(p, lane, 3);
     if (threadIdx.x < 32 && !s_abort) {
@@ -513,7 +531,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) sra_kernel(const _
     }
   }
 
-  if (!s_abort) sra_phase_c<T, KB, GPL>(p, li, epoch, stages);
+  if (!s_abort) sra_phase_c<T, KB, GPL, false, CODEC>(p, li, epoch, stages);
   trace_mark(p, lane, 5);
   sync_finish(p.sync, epoch, p.lanes);
 }
@@ -528,8 +546,11 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) sra_kernel(const _
 // the reference's tiny-tensor all-to-all, /root/reference/src/common/reducer.cc:35-94.)
 // Consecutive calls alternate between two regions (epoch parity): a peer can be one call ahead.
 // ===========================================================================
-template <typename T, int KB, int GPL>
+// CODEC as in sra_kernel: an FP8 image holds the codes of x * prescale, and phase 2 sums every
+// image's decoded values from +0 in rank order.
+template <typename T, int KB, int GPL, int CODEC = kMaxMin>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(const __grid_constant__ SraParams p) {
+  static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   __shared__ LaneItems li;
   __shared__ int s_abort;
   const int lane = blockIdx.x;
@@ -561,6 +582,21 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(con
       if (i + kSraWarps < total) slice_prefetch_l2<T, GPL>(data + lane_item(li, p, i + kSraWarps, 0).elem_off);
       const uint32_t kind = item_kind(it);
       T* blk = data + it.elem_off;
+      if constexpr (CODEC != kMaxMin) {
+        if (hot == 1) {
+          slice_scale<GPL>(x, p.prescale);
+          full_send_fp8_x<CODEC, GPL>(x, it, ds);
+          continue;
+        }
+        if (kind == kItemFull) {
+          full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, ds, (T*)nullptr);
+          continue;
+        }
+        if (kind == kItemBucket) {
+          bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, ds, (T*)nullptr);
+          continue;
+        }
+      }
       if (hot == 1)
         full_send_x<T, KB, GPL, false, true>(x, it, p.prescale, rng, ds, (T*)nullptr);
       else if (hot == 2)
@@ -592,6 +628,19 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(con
         const uint32_t kind = item_kind(it);
         T* blk = data + it.elem_off;
         const bool al = group_aligned<T>(blk);
+        if constexpr (CODEC != kMaxMin) {
+          if (kind == kItemFull) {
+            if (al)
+              full_recv_sum_fp8<T, CODEC, GPL, true>(ss, it, blk);
+            else
+              full_recv_sum_fp8_unaligned<T, CODEC, GPL>(ss, it, blk);
+            continue;
+          }
+          if (kind == kItemBucket) {
+            bucket_recv_sum_fp8<T, CODEC>(ss, it, blk);
+            continue;
+          }
+        }
         if (kind == kItemFull && al) {
           full_recv_sum<T, KB, GPL, true>(ss, it, blk);
         } else if (kind == kItemFull) {
@@ -792,7 +841,9 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __
 // OP: kOpAllreduce (SRA / one-shot by p.oneshot), kOpReduceScatter or kOpAllGather. The reduce-
 // scatter and all-gather kernels are instantiated in translation units of their own
 // (rs_* / ag_{f32,f16,bf16}.cu): out-of-line helpers are register-allocated per module, and sharing
-// them with another kernel would change the allreduce kernels' spill counts.
+// them with another kernel would change the allreduce kernels' spill counts. For the same reason the
+// FP8 allreduce (launch_sra_fp8_t: sra_kernel / oneshot_kernel with an FP8 codec) has its own
+// sra_fp8_{f32,f16,bf16}.cu.
 enum : int { kOpAllreduce = 0, kOpReduceScatter = 1, kOpAllGather = 2 };
 
 template <typename T, int KB, int GPL, int OP, int CODEC = kMaxMin>
@@ -802,15 +853,15 @@ cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
   else if constexpr (OP == kOpAllGather)
     dev::ag_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if (p.oneshot)
-    dev::oneshot_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    dev::oneshot_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else
-    dev::sra_kernel<T, KB, GPL><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    dev::sra_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
 template <typename T, int GPL, int OP>
 cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
-  if (p.codec != kMaxMin) {  // FP8: the reduce-scatter and all-gather of 8-bit plans only
+  if (p.codec != kMaxMin) {  // FP8: the reduce-scatter and all-gather of 8-bit plans (the allreduce: launch_sra_fp8_t)
     if constexpr (OP == kOpAllreduce) {
       return cudaErrorInvalidValue;
     } else {
@@ -831,6 +882,19 @@ cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
 template <typename T, int OP = kOpAllreduce>
 cudaError_t launch_sra_t(const SraParams& p, cudaStream_t stream) {
   return p.slice_elems == 1024 ? launch_sra_gpl<T, 4, OP>(p, stream) : launch_sra_gpl<T, 2, OP>(p, stream);
+}
+
+// The FP8 allreduce: sra_kernel / oneshot_kernel of an 8-bit plan with p.codec kE4M3 or kE5M2
+template <typename T, int GPL>
+cudaError_t launch_sra_fp8_gpl(const SraParams& p, cudaStream_t stream) {
+  if (p.uniform_bits != 8) return cudaErrorInvalidValue;
+  if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, kOpAllreduce, kE4M3>(p, stream);
+  if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, kOpAllreduce, kE5M2>(p, stream);
+  return cudaErrorInvalidValue;
+}
+template <typename T>
+cudaError_t launch_sra_fp8_t(const SraParams& p, cudaStream_t stream) {
+  return p.slice_elems == 1024 ? launch_sra_fp8_gpl<T, 4>(p, stream) : launch_sra_fp8_gpl<T, 2>(p, stream);
 }
 
 template <typename T>
@@ -857,5 +921,9 @@ cudaError_t launch_rs_bf16(const SraParams& p, cudaStream_t stream);
 cudaError_t launch_ag_f32(const SraParams& p, cudaStream_t stream);
 cudaError_t launch_ag_f16(const SraParams& p, cudaStream_t stream);
 cudaError_t launch_ag_bf16(const SraParams& p, cudaStream_t stream);
+// defined once per dtype in sra_fp8_{f32,f16,bf16}.cu
+cudaError_t launch_sra_fp8_f32(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_sra_fp8_f16(const SraParams& p, cudaStream_t stream);
+cudaError_t launch_sra_fp8_bf16(const SraParams& p, cudaStream_t stream);
 
 }  // namespace cgx

@@ -53,7 +53,7 @@ c10::intrusive_ptr<c10::ivalue::Future> CgxCommHook::runHook(c10d::GradBucket& b
   const bool registered = step >= s.register_step;
   if (bucket.isLast()) s.step.fetch_add(1, std::memory_order_relaxed);
   // average == true: the 1/world scale is applied inside the kernel, before quantization
-  auto work = s.pg->allreduce_bucket(bucket.getBufferRef(), registered ? (int64_t)idx : -1, true);
+  auto work = s.pg->allreduce_bucket(bucket.getBufferRef(), registered ? (int64_t)idx : -1, true, s.codec);
   return work->getFuture();
 }
 
@@ -140,8 +140,14 @@ std::shared_ptr<HookState> register_native_hook(const std::shared_ptr<c10d::Redu
                                                 c10::intrusive_ptr<ProcessGroupCGX> pg, int64_t layer_min_size,
                                                 int bits, int bucket_size, int register_step,
                                                 std::vector<int64_t> candidates, int64_t period,
-                                                std::map<std::pair<int64_t, int64_t>, int> loaded) {
+                                                std::map<std::pair<int64_t, int64_t>, int> loaded,
+                                                std::optional<WireCodec> codec) {
   TORCH_CHECK(period >= 1, "register_native_hook: period must be >= 1, got ", period);
+  if (codec && *codec != kMaxMin) {
+    if (!candidates.empty())
+      throw std::invalid_argument("register_native_hook: adaptive widths have no FP8 formats");
+    if (bits != 8) throw std::invalid_argument("register_native_hook: an FP8 format uses bits 8");
+  }
   for (int64_t c : candidates)
     TORCH_CHECK(c >= 1 && c <= 8, "register_native_hook: candidate width ", c, " is outside 1..8");
   auto st = std::make_shared<HookState>();
@@ -153,6 +159,7 @@ std::shared_ptr<HookState> register_native_hook(const std::shared_ptr<c10d::Redu
   st->candidates = std::move(candidates);
   st->period = period;
   st->loaded = std::move(loaded);
+  st->codec = codec;
   reducer->register_comm_hook(std::make_unique<CgxCommHook>(st));
   return st;
 }

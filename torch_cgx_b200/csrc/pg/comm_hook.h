@@ -18,6 +18,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <utility>
 #include <vector>
 
@@ -34,6 +35,7 @@ struct HookState {
   int64_t layer_min_size = 1024;
   int bits = 32;
   int bucket_size = 1024;
+  std::optional<WireCodec> codec;  // wire format of the 8-bit layers; none: CGX_COMPRESSION_FORMAT's
   int register_step = 2;  // DDP rebuilds its buckets after the first iteration
   std::atomic<int64_t> step{0};
 
@@ -71,11 +73,13 @@ class CgxCommHook : public c10d::CommHookInterface {
 };
 
 // registers the hook on `reducer` (a torch.distributed.Reducer) and returns the shared state.
-// Non-empty `candidates` turns on adaptive widths; `loaded` is applied at registration.
+// Non-empty `candidates` turns on adaptive widths; `loaded` is applied at registration. An FP8
+// `codec` (bits 8, fixed widths) sends the compressed layers as FP8 codes.
 std::shared_ptr<HookState> register_native_hook(const std::shared_ptr<c10d::Reducer>& reducer,
                                                 c10::intrusive_ptr<ProcessGroupCGX> pg, int64_t layer_min_size,
                                                 int bits, int bucket_size, int register_step,
                                                 std::vector<int64_t> candidates = {}, int64_t period = 1,
-                                                std::map<std::pair<int64_t, int64_t>, int> loaded = {});
+                                                std::map<std::pair<int64_t, int64_t>, int> loaded = {},
+                                                std::optional<WireCodec> codec = std::nullopt);
 
 }  // namespace cgx

@@ -383,10 +383,11 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::enqueue_cuda(c10d::OpType op, co
   return work;
 }
 
-c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, bool average, int bucket_idx) {
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce(at::Tensor& t, bool average, int bucket_idx,
+                                                                 std::optional<WireCodec> codec) {
   return enqueue_cuda(c10d::OpType::ALLREDUCE, "cgx:all_reduce", t, nullptr, [&](cudaStream_t s) {
     engine_->allreduce_cuda(t.data_ptr(), to_cgx_dtype(t.scalar_type()), t.numel(), average, bucket_idx, s,
-                            /*overlapped=*/bucket_idx >= 0);
+                            /*overlapped=*/bucket_idx >= 0, codec);
   });
 }
 
@@ -544,7 +545,8 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   });
 }
 
-c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx) {
+c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx,
+                                                                     std::optional<WireCodec> codec) {
   // host tensors: queued to the worker thread in call order (reference: enqueue/runLoop,
   // ProcessGroupCGX.cc:300-339); the returned Work's future completes when the job is done, errors
   // are delivered through it
@@ -559,6 +561,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor&
   // environment + layer table are captured NOW, on the caller's thread (functional.compression()
   // restores os.environ as soon as this returns)
   auto call = std::make_shared<AllreduceEngine::CpuCall>(engine_->prepare_cpu(tensor.numel(), bucket_idx));
+  if (codec) call->env.codec = *codec;
   worker_->submit([this, fut, tensor, dtype, average, call]() mutable {
     try {
       engine_->allreduce_cpu_prepared(tensor.data_ptr(), dtype, *call, average);
@@ -582,11 +585,11 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::allreduce(std::vector<at::Tensor
 }
 
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::allreduce_bucket(at::Tensor& tensor, int64_t bucket_idx,
-                                                                 bool average) {
+                                                                 bool average, std::optional<WireCodec> codec) {
   c10d::ReduceOp op = average ? c10d::ReduceOp::AVG : c10d::ReduceOp::SUM;
   if (eligible_for_engine(tensor, op))
-    return tensor.is_cuda() ? engine_allreduce(tensor, average, (int)bucket_idx)
-                            : engine_allreduce_cpu(tensor, average, (int)bucket_idx);
+    return tensor.is_cuda() ? engine_allreduce(tensor, average, (int)bucket_idx, codec)
+                            : engine_allreduce_cpu(tensor, average, (int)bucket_idx, codec);
   std::vector<at::Tensor> ts{tensor};
   c10d::AllreduceOptions o;
   if (average && !tensor.is_cuda()) {

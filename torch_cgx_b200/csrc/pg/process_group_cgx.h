@@ -175,8 +175,10 @@ class ProcessGroupCGX : public c10d::Backend {
 
   // ---- cgx-specific API (bound to Python) ----------------------------------
   // allreduce of one DDP bucket whose index is known (no cursor guessing);
-  // average == true fuses the 1/world scale into the kernel.
-  c10::intrusive_ptr<c10d::Work> allreduce_bucket(at::Tensor& tensor, int64_t bucket_idx, bool average);
+  // average == true fuses the 1/world scale into the kernel. `codec`, when given, is the wire format
+  // of the 8-bit layers in place of CGX_COMPRESSION_FORMAT's (AllreduceEngine::allreduce_cuda).
+  c10::intrusive_ptr<c10d::Work> allreduce_bucket(at::Tensor& tensor, int64_t bucket_idx, bool average,
+                                                  std::optional<WireCodec> codec = std::nullopt);
   // Compressed reduce-scatter or all-gather through the fused P2P kernel; the c10d entry points of
   // both stay with the delegate.
   //  kReduceScatter (reduce_scatter_tensor semantics): `in` holds size() * out.numel() elements,
@@ -239,8 +241,10 @@ class ProcessGroupCGX : public c10d::Backend {
   template <class Run>
   c10::intrusive_ptr<c10d::Work> enqueue_cuda(c10d::OpType op, const char* title, at::Tensor& out,
                                               const at::Tensor* in, Run&& run);
-  c10::intrusive_ptr<c10d::Work> engine_allreduce(at::Tensor& t, bool average, int bucket_idx);
-  c10::intrusive_ptr<c10d::Work> engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx);
+  c10::intrusive_ptr<c10d::Work> engine_allreduce(at::Tensor& t, bool average, int bucket_idx,
+                                                  std::optional<WireCodec> codec = std::nullopt);
+  c10::intrusive_ptr<c10d::Work> engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx,
+                                                      std::optional<WireCodec> codec = std::nullopt);
   void ensure_cuda(c10::DeviceIndex dev);
 
   c10::intrusive_ptr<c10d::Store> store_;

@@ -60,10 +60,16 @@ class CpuBackend : public BlockBackend {
     }
   }
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
-                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t) override {
+                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t, WireCodec codec) override {
     const Plan& p = dp.plan;
+    if (codec != kMaxMin) check_fp8(p, first, count, rng);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
+      if (codec != kMaxMin) {
+        cpu::quantize_block_fp8(acc_f32 + (d.elem_off - base_elem), d, wire + d.wire_off, codec);
+        if (out) cpu::decode_block_fp8_store(wire + d.wire_off, p.dtype, d, out, codec);
+        continue;
+      }
       cpu::quantize_block(acc_f32 + (d.elem_off - base_elem), p.dtype, d, wire + d.wire_off, rng, b);
       if (out) cpu::decode_block_store(wire + d.wire_off, p.dtype, d, out);
     }
@@ -111,8 +117,9 @@ class CudaBackend : public BlockBackend {
                "accumulate_items");
   }
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
-                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) override {
-    cuda_check(launch_quantize_items_f32(args(dp, first, count), acc_f32, base_elem, wire, rng, out, stream),
+                    uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream, WireCodec codec) override {
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng);
+    cuda_check(launch_quantize_items_f32(args(dp, first, count, codec), acc_f32, base_elem, wire, rng, out, stream),
                "quantize_items_f32");
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,

@@ -34,9 +34,10 @@ class BlockBackend {
   virtual void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
                           uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream,
                           WireCodec codec = kMaxMin) = 0;
-  // wire = quantize(acc_f32); out[T] = decode(wire) when out != nullptr
+  // wire = quantize(acc_f32); out[T] = decode(wire) when out != nullptr (an FP8 codec as in quantize)
   virtual void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first,
-                            uint32_t count, uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream) = 0;
+                            uint32_t count, uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream,
+                            WireCodec codec = kMaxMin) = 0;
   // dst[T] = decode(wire)
   virtual void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                           cudaStream_t stream, WireCodec codec = kMaxMin) = 0;

@@ -68,11 +68,18 @@ const DevicePlan* FusedSra::prepare_impl(const std::vector<LayerSpec>& layers, i
   return &dp;
 }
 
-void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream) {
-  launch(dp, data, prescale, rng, stream, false);
-}
-
 namespace {
+
+// an FP8 allreduce: a known codec, compressed blocks of 8 bits only, round to nearest
+void check_allreduce_codec(const Plan& plan, WireCodec codec, const RngParams& rng) {
+  if (codec == kMaxMin) return;
+  if (codec != kE4M3 && codec != kE5M2) throw std::invalid_argument("cgx allreduce: unknown wire codec");
+  if (rng.stochastic) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
+  for (const BlockDesc& d : plan.blocks)
+    if (block_bits(d) != 8 && block_bits(d) < kRawBits)
+      throw std::invalid_argument("cgx allreduce: an FP8 format needs layers of bits 8 or 32, got " +
+                                  std::to_string(block_bits(d)));
+}
 
 // split_for_fusion cuts a layer at multiples of its bucket size. A bucket above kMaxBlockElems is
 // quantized as kMaxBlockElems-element buckets counted from the layer start, while skip_incomplete
@@ -102,6 +109,12 @@ std::vector<std::vector<LayerSpec>> split_shard(const std::vector<LayerSpec>& la
 }
 
 }  // namespace
+
+void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
+                   WireCodec codec) {
+  check_allreduce_codec(dp.plan, codec, rng);
+  launch(dp, data, prescale, rng, stream, false, nullptr, 0, false, codec);
+}
 
 void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
                            const void* out, uint64_t S, int rank, int world, WireCodec codec) {
@@ -202,8 +215,9 @@ FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>&
 }
 
 void FusedSra::run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng,
-                           cudaStream_t stream) {
-  launch(dp, data, prescale, rng, stream, true);
+                           cudaStream_t stream, WireCodec codec) {
+  check_allreduce_codec(dp.plan, codec, rng);
+  launch(dp, data, prescale, rng, stream, true, nullptr, 0, false, codec);
 }
 
 // Pipeline depth of the fused kernel: every chunk's item list can be cut into S pieces, each with

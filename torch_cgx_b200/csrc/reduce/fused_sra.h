@@ -103,14 +103,20 @@ class FusedSra {
 
   // In-place allreduce of `data` over the layers of `dp`. Stream-ordered, no
   // host synchronisation. Every rank must call this the same number of times
-  // in the same order (epoch counter).
-  void run(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream);
+  // in the same order (epoch counter). An FP8 `codec` (common/quant_math.h; a plan of bits 8 or 32,
+  // round to nearest, else std::invalid_argument before anything is launched) gives the 8-bit
+  // records FP8 codes: the sender encodes prescale * x, the owner adds each decoded value
+  // fl(float(code) * unit) with its own rounding, encodes the fp32 sum once and keeps its decoded codes.
+  void run(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
+           WireCodec codec = kMaxMin);
 
   // One-shot variant (single signalling hop, for latency-bound messages): plan over the WHOLE
   // buffer (one chunk); nullptr if its packed image does not fit the heap's one-shot slots.
   const DevicePlan* prepare_oneshot(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                                     cudaStream_t stream, int max_lanes = 0);
-  void run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream);
+  // An FP8 `codec` as in run(): every rank sums the decoded images from +0.
+  void run_oneshot(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
+                   WireCodec codec = kMaxMin);
 
   // A sharded collective over S-element shards; `shard_layers` is the quantization table of ONE
   // shard (offsets from the shard start, tiling [0, S)); every shard uses it, so buckets are counted

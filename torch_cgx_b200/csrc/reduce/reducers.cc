@@ -86,7 +86,7 @@ void Reducer::broadcast(void* data, size_t bytes, int root, cudaStream_t stream)
 }
 
 void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                                   int root, const RngParams& rng, cudaStream_t stream) {
+                                   int root, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
   const int W = comm_->size(), r = comm_->rank();
   if (W == 1) return;
   const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream, 1);  // the whole buffer is one chunk
@@ -97,8 +97,11 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
   uint8_t* wire = scratch(4, row_bytes(plan));
   std::vector<P2POp> x;
   if (r == root) {
-    ops_->quantize(dp, data, 0, nb, wire, 1.0f, make_rng_key(rng, root, 2), stream);
-    ops_->dequantize(dp, wire, 0, nb, data, stream);  // the root keeps what the receivers will decode
+    // the root keeps what the receivers will decode
+    codec_runs(plan, 0, nb, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->quantize(dp, data, b, n, wire, 1.0f, make_rng_key(rng, root, 2), stream, c);
+      ops_->dequantize(dp, wire, b, n, data, stream, c);
+    });
     for (int p = 0; p < W; ++p)
       if (p != root) x.push_back({true, wire, bytes, p});
     bytes_sent_ += bytes * (uint64_t)(W - 1);
@@ -106,7 +109,8 @@ void Reducer::broadcast_compressed(void* data, int dtype, const std::vector<Laye
   } else {
     x.push_back({false, wire, bytes, root});
     comm_->exchange(x, stream);
-    ops_->dequantize(dp, wire, 0, nb, data, stream);
+    codec_runs(plan, 0, nb, codec,
+               [&](uint32_t b, uint32_t n, WireCodec c) { ops_->dequantize(dp, wire, b, n, data, stream, c); });
   }
 }
 
@@ -253,7 +257,7 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
 
 // ---------------------------------------------------------------------- SRA --
 void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                           float prescale, const RngParams& rng, cudaStream_t stream) {
+                           float prescale, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
   const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
   const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
@@ -272,7 +276,10 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->quantize(dp, data, pb, pn, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream);
+    if (pn)
+      codec_runs(plan, pb, pn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->quantize(dp, data, b, n, sendb + row * p, prescale, make_rng_key(rng, r, 0), stream, c);
+      });
     if (plan.chunk_wire_bytes[p]) x.push_back({true, sendb + row * p, plan.chunk_wire_bytes[p], p});
     if (plan.chunk_wire_bytes[r]) x.push_back({false, recvb + row * p, plan.chunk_wire_bytes[r], p});
     bytes_sent_ += plan.chunk_wire_bytes[p];
@@ -282,9 +289,14 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   if (cn) {
     ops_->accumulate(dp, nullptr, cb, cn, acc, lo, data, prescale, stream);
     for (int q = 0; q < W; ++q)
-      if (q != r) ops_->accumulate(dp, recvb + row * q, cb, cn, acc, lo, nullptr, 1.0f, stream);
+      if (q != r)
+        codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+          ops_->accumulate(dp, recvb + row * q, b, n, acc, lo, nullptr, 1.0f, stream, c);
+        });
     // requantize + self-decode so that every rank ends with identical values
-    ops_->quantize_f32(dp, acc, lo, cb, cn, mine, make_rng_key(rng, r, 1), data, stream);
+    codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->quantize_f32(dp, acc, lo, b, n, mine, make_rng_key(rng, r, 1), data, stream, c);
+    });
   }
   // phase 2: all-gather of the reduced chunks
   x.clear();
@@ -298,13 +310,16 @@ void SraReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& 
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
-    if (pn) ops_->dequantize(dp, recvb + row * p, pb, pn, data, stream);
+    if (pn)
+      codec_runs(plan, pb, pn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->dequantize(dp, recvb + row * p, b, n, data, stream, c);
+      });
   }
 }
 
 // --------------------------------------------------------------------- Ring --
 void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                            float prescale, const RngParams& rng, cudaStream_t stream) {
+                            float prescale, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
   const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
   const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;
@@ -326,13 +341,18 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
     RngParams hop = rng;
     hop.seq = rng.seq * 16u + (uint32_t)s;
     if (cn(sseg))
-      ops_->quantize_f32(dp, acc, lo, cb(sseg), cn(sseg), bufa, make_rng_key(hop, r, 0), nullptr, stream);
+      codec_runs(plan, cb(sseg), cn(sseg), codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->quantize_f32(dp, acc, lo, b, n, bufa, make_rng_key(hop, r, 0), nullptr, stream, c);
+      });
     std::vector<P2POp> x;
     if (plan.chunk_wire_bytes[sseg]) x.push_back({true, bufa, plan.chunk_wire_bytes[sseg], right});
     if (plan.chunk_wire_bytes[rseg]) x.push_back({false, bufb, plan.chunk_wire_bytes[rseg], left});
     bytes_sent_ += plan.chunk_wire_bytes[sseg];
     comm_->exchange(x, stream);
-    if (cn(rseg)) ops_->accumulate(dp, bufb, cb(rseg), cn(rseg), acc, lo, nullptr, 1.0f, stream);
+    if (cn(rseg))
+      codec_runs(plan, cb(rseg), cn(rseg), codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->accumulate(dp, bufb, b, n, acc, lo, nullptr, 1.0f, stream, c);
+      });
   }
   // the fully reduced segment of this rank: requantize once more and self-decode
   int cur = (r + 1) % W;
@@ -341,7 +361,10 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
   fin.seq = rng.seq * 16u + 15u;
   uint8_t* have = bufa;
   uint8_t* next = bufb;
-  if (cn(cur)) ops_->quantize_f32(dp, acc, lo, cb(cur), cn(cur), have, make_rng_key(fin, r, 1), data, stream);
+  if (cn(cur))
+    codec_runs(plan, cb(cur), cn(cur), codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->quantize_f32(dp, acc, lo, b, n, have, make_rng_key(fin, r, 1), data, stream, c);
+    });
   // all-gather: forward the already-compressed bytes around the ring, decode locally
   for (int s = 0; s + 1 < W; ++s) {
     const int rseg = (cur + W - 1) % W;
@@ -350,7 +373,10 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
     if (plan.chunk_wire_bytes[rseg]) x.push_back({false, next, plan.chunk_wire_bytes[rseg], left});
     bytes_sent_ += plan.chunk_wire_bytes[cur];
     comm_->exchange(x, stream);
-    if (cn(rseg)) ops_->dequantize(dp, next, cb(rseg), cn(rseg), data, stream);
+    if (cn(rseg))
+      codec_runs(plan, cb(rseg), cn(rseg), codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+        ops_->dequantize(dp, next, b, n, data, stream, c);
+      });
     std::swap(have, next);
     cur = rseg;
   }
@@ -358,7 +384,8 @@ void RingReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>&
 
 // ----------------------------------------------------------------- AllToAll --
 void AllToAllReducer::allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                                float prescale, const RngParams& rng, cudaStream_t stream) {
+                                float prescale, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
+  if (codec != kMaxMin) throw std::invalid_argument(kAllToAllNoFp8);
   const DevicePlan& dp = plan_for(layers, dtype, skip_incomplete, stream);
   const Plan& plan = dp.plan;
   if (plan.blocks.empty()) return;

@@ -30,17 +30,21 @@ class Reducer {
   Reducer(Communicator* comm, BlockBackend* ops);
   virtual ~Reducer();
   virtual const char* name() const = 0;
-  // in-place allreduce of data[T] restricted to `layers`
+  // in-place allreduce of data[T] restricted to `layers`. An FP8 `codec` (layers of bits 8 or 32,
+  // round to nearest) sends the compressed layers' 8-bit records as FP8 codes and adds each decoded
+  // value with its own rounding; raw layers are unchanged. The debug all-to-all reduction has no FP8
+  // form and throws std::invalid_argument (kAllToAllNoFp8) before anything is sent.
   virtual void allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                         float prescale, const RngParams& rng, cudaStream_t stream) = 0;
+                         float prescale, const RngParams& rng, cudaStream_t stream, WireCodec codec = kMaxMin) = 0;
   // raw broadcast of `bytes` from group rank `root`
   void broadcast(void* data, size_t bytes, int root, cudaStream_t stream);
   // Compressed broadcast of `layers` (reference: Reducer::Broadcast with do_compression,
   // /root/reference/src/common/reducer.cc:96-160): the root quantizes, decodes its own bytes back
   // into `data` (so it holds exactly what every receiver will decode) and sends the SAME packed
-  // bytes to every peer; receivers decode. Raw layers travel as T inside the same record.
+  // bytes to every peer; receivers decode. Raw layers travel as T inside the same record. An FP8
+  // `codec` as in allreduce.
   void broadcast_compressed(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete,
-                            int root, const RngParams& rng, cudaStream_t stream);
+                            int root, const RngParams& rng, cudaStream_t stream, WireCodec codec = kMaxMin);
   // Compressed reduce-scatter over the communicator's W ranks, the scatter phase of the SRA alone.
   // `shard_layers` is ONE shard's table (offsets from the shard start, tiling [0, S)); the plan is
   // that table replicated W times at stride S, so chunk c is copy c and buckets are counted from each
@@ -107,7 +111,7 @@ class SraReducer : public Reducer {
   using Reducer::Reducer;
   const char* name() const override { return "SRA"; }
   void allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete, float prescale,
-                 const RngParams& rng, cudaStream_t stream) override;
+                 const RngParams& rng, cudaStream_t stream, WireCodec codec) override;
 };
 
 class RingReducer : public Reducer {
@@ -115,7 +119,7 @@ class RingReducer : public Reducer {
   using Reducer::Reducer;
   const char* name() const override { return "RING"; }
   void allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete, float prescale,
-                 const RngParams& rng, cudaStream_t stream) override;
+                 const RngParams& rng, cudaStream_t stream, WireCodec codec) override;
 };
 
 // Debug variant (CGX_DEBUG_ALL_TO_ALL_REDUCTION): every rank quantizes the whole
@@ -126,8 +130,11 @@ class AllToAllReducer : public Reducer {
   using Reducer::Reducer;
   const char* name() const override { return "ALLTOALL"; }
   void allreduce(void* data, int dtype, const std::vector<LayerSpec>& layers, bool skip_incomplete, float prescale,
-                 const RngParams& rng, cudaStream_t stream) override;
+                 const RngParams& rng, cudaStream_t stream, WireCodec codec) override;
 };
+
+constexpr const char* kAllToAllNoFp8 =
+    "cgx: the debug all-to-all reduction (CGX_DEBUG_ALL_TO_ALL_REDUCTION) has no FP8 formats";
 
 std::unique_ptr<Reducer> make_reducer(ReductionType type, Communicator* comm, BlockBackend* ops);
 

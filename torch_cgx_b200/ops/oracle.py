@@ -267,7 +267,8 @@ def _check_fp8_table(layers: Sequence[Layer], fmt: str | None) -> None:
 
 def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, world: int | None = None,
                   lanes: int = 1, min_lane_elems: int = 2048, average: bool = False,
-                  skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
+                  skip_incomplete: bool = False, prescale: float | None = None,
+                  fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's result of the deterministic compressed SRA allreduce (DESIGN §2.3).
 
     For each bucket, the owner c (the rank whose chunk holds it) forms in fp32
@@ -276,7 +277,10 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
     is Q(acc), the owner's self-decoded copy, stored in the input dtype on every rank.
     Raw runs (uncompressed layers, skip_incomplete tails) replace Q by a rounding to the
     dtype, per peer contribution and once at the end. Elements outside every layer are kept.
+    ``fmt`` ("e4m3" / "e5m2"): Q is the FP8 round trip of ``fp8_quantize_dequantize``, for the
+    peers' contributions and for the fp32 sum alike; the table may hold bits 8 and 32 only.
     """
+    _check_fp8_table(layers, fmt)
     W = len(inputs)
     assert world is None or world == W
     dtype = inputs[0].dtype
@@ -286,17 +290,20 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
     outs = [t.detach().reshape(-1).float().cpu().numpy().copy() for t in inputs]
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
         sl = slice(off, off + m)
-        res = _contribution(_sra_acc(xs, sl, owner[sl], bits, bucket, dtype), bits, bucket, dtype)
+        res = _contribution(_sra_acc(xs, sl, owner[sl], bits, bucket, dtype, fmt), bits, bucket, dtype, fmt)
         for o in outs:
             o[sl] = res
     return _to_tensors(outs, dtype)
 
 
 def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
-                      skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
+                      skip_incomplete: bool = False, prescale: float | None = None,
+                      fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's result of the one-shot allreduce: each contribution, the own one included,
     is quantized once (raw runs: rounded to the dtype) and the decoded values are summed in
-    fp32 in rank order starting from +0; no second quantization, one rounding to the dtype."""
+    fp32 in rank order starting from +0; no second quantization, one rounding to the dtype.
+    ``fmt``: the contributions take the FP8 round trip instead (as in ``sra_reference``)."""
+    _check_fp8_table(layers, fmt)
     W = len(inputs)
     dtype = inputs[0].dtype
     xs = _scaled_inputs(inputs, _prescale(W, average, prescale))
@@ -306,7 +313,7 @@ def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *
         acc = np.zeros(m, _F32)
         with np.errstate(all="ignore"):
             for q in range(W):
-                acc = acc + _contribution(xs[q][sl], bits, bucket, dtype)
+                acc = acc + _contribution(xs[q][sl], bits, bucket, dtype, fmt)
         res = round_to_dtype(acc, dtype)
         for o in outs:
             o[sl] = res
@@ -317,12 +324,12 @@ def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *
 GENERIC_MIN_LANE_ELEMS = 2048  # Reducer::plan_for: one lane per rank chunk, default min_lane_elems
 
 
-def _quantized(v: np.ndarray, segs, dtype: torch.dtype) -> np.ndarray:
+def _quantized(v: np.ndarray, segs, dtype: torch.dtype, fmt: str | None = None) -> np.ndarray:
     """``_contribution`` of every layer run of a whole-buffer fp32 array, buckets counted from
     each run's start; elements outside every run are returned unchanged."""
     out = v.copy()
     for off, m, bits, bucket in segs:
-        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, dtype)
+        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, dtype, fmt)
     return out
 
 
@@ -331,7 +338,8 @@ def _own_values(inputs: Sequence[torch.Tensor]) -> List[np.ndarray]:
 
 
 def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
-                   skip_incomplete: bool = False, prescale: float | None = None) -> List[torch.Tensor]:
+                   skip_incomplete: bool = False, prescale: float | None = None,
+                   fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's result of the compressed Ring allreduce (``RingReducer``, deterministic rounding).
 
     Chunk c is rank c's chunk of the lanes = 1 plan. Rank r starts with acc_r = prescale*x_r in fp32.
@@ -340,7 +348,9 @@ def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, a
     (c - 1) mod W; every rank ends with Q(acc_{(c-1) mod W}) on chunk c, stored in the dtype (at
     W = 1: Q(prescale*x)). Q is one quantization round with buckets counted from the layer start;
     raw runs replace it by a rounding to the dtype. Elements outside every layer are kept.
+    ``fmt``: Q is the FP8 round trip (as in ``sra_reference``).
     """
+    _check_fp8_table(layers, fmt)
     W = len(inputs)
     dtype = inputs[0].dtype
     n = inputs[0].numel()
@@ -349,7 +359,7 @@ def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, a
     acc = _scaled_inputs(inputs, _prescale(W, average, prescale))
     with np.errstate(all="ignore"):
         for s in range(W - 1):
-            sent = [_quantized(a, segs, dtype) for a in acc]  # every rank sends before it adds
+            sent = [_quantized(a, segs, dtype, fmt) for a in acc]  # every rank sends before it adds
             for r in range(W):
                 sel = chunk == (r - s) % W
                 dst = acc[(r + 1) % W]
@@ -357,7 +367,7 @@ def ring_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, a
     outs = _own_values(inputs)
     for c in range(W):
         sel = chunk == c
-        final = _quantized(acc[(c - 1) % W], segs, dtype)
+        final = _quantized(acc[(c - 1) % W], segs, dtype, fmt)
         for o in outs:
             o[sel] = final[sel]
     return _to_tensors(outs, dtype)
@@ -387,17 +397,19 @@ def alltoall_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], 
 
 
 def broadcast_compressed_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, root: int,
-                                   skip_incomplete: bool = False) -> List[torch.Tensor]:
+                                   skip_incomplete: bool = False, fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's result of ``Reducer::broadcast_compressed``: one quantization round of the
     root's values (prescale 1, one chunk, buckets from the layer start; a ``skip_incomplete`` tail
     stays raw), the root included so that all ranks agree. Elements outside every layer keep each
-    rank's own values. With one rank nothing is sent and the values are unchanged."""
+    rank's own values. With one rank nothing is sent and the values are unchanged. ``fmt``: the
+    FP8 round trip instead of max-min's."""
+    _check_fp8_table(layers, fmt)
     W = len(inputs)
     dtype = inputs[0].dtype
     outs = _own_values(inputs)
     if W > 1:
         segs = layer_segments(layers, skip_incomplete)
-        q = _quantized(_own_values([inputs[root]])[0], segs, dtype)
+        q = _quantized(_own_values([inputs[root]])[0], segs, dtype, fmt)
         for o in outs:
             for off, m, _, _ in segs:
                 o[off:off + m] = q[off:off + m]
@@ -414,7 +426,7 @@ _ELSIZE = {torch.float32: 4, torch.float16: 2, torch.bfloat16: 2}
 ENGINE_PERTURBATIONS = ("prescale_local", "raw_broadcast", "cross_seq_unmarked", "oneshot_shifted")
 
 
-def _generic_allreduce(kind, ins, layers, *, prescale, skip_incomplete, stochastic, seed, seq):
+def _generic_allreduce(kind, ins, layers, *, prescale, skip_incomplete, stochastic, seed, seq, fmt=None):
     """One generic reducer's allreduce over ``ins`` (one tensor per rank of its group)."""
     if stochastic:
         from .. import _C
@@ -424,6 +436,10 @@ def _generic_allreduce(kind, ins, layers, *, prescale, skip_incomplete, stochast
                                                                prescale=float(prescale))
         return out
     kw = dict(skip_incomplete=skip_incomplete, prescale=prescale)
+    if fmt is not None:
+        if kind == "ALLTOALL":
+            raise ValueError("the debug all-to-all reduction has no FP8 formats")
+        kw["fmt"] = fmt
     if kind == "SRA":
         return sra_reference(ins, layers, lanes=1, min_lane_elems=GENERIC_MIN_LANE_ELEMS, **kw)
     if kind == "RING":
@@ -434,7 +450,7 @@ def _generic_allreduce(kind, ins, layers, *, prescale, skip_incomplete, stochast
 def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, local_size: int, config: dict,
                      lanes: int, slot_bytes: Tuple[int, int] = (0, 0), average: bool = False, call_seq: int = 1,
                      cuda: bool = True, overlapped: bool = False, skip_incomplete: bool = False,
-                     stochastic: bool = False, seed: int = 0, perturb: str | None = None):
+                     stochastic: bool = False, seed: int = 0, perturb: str | None = None, fmt: str | None = None):
     """Every rank's result of one ``AllreduceEngine`` allreduce over ``layers`` and the stages each
     rank issues, ``(outputs, stages)``; ``stages[r]`` is a list of dicts (kind, layers, lanes, numel,
     seed, seq, stochastic, scale) in the order rank r issues them.
@@ -460,8 +476,13 @@ def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *,
     ``C.LocalReducerGroup``) with these sequence numbers instead of the deterministic references.
     ``perturb`` (one of ``ENGINE_PERTURBATIONS``) switches on a wrong semantics, for the tests that
     show the reference tells it apart.
+    ``fmt`` ("e4m3" / "e5m2"): every compressed stage uses that FP8 format (deterministic only).
     """
     from .. import _C
+
+    _check_fp8_table(layers, fmt)
+    if fmt is not None and stochastic:
+        raise ValueError("the FP8 formats round to nearest only")
 
     cfg = dict(ENGINE_DEFAULTS, **config)
     W, L = len(inputs), local_size
@@ -544,16 +565,16 @@ def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *,
                             sim(outs, gl, plan_lanes, False, skip_incomplete, True, seed, s3, cfg["min_lane_elems"],
                                 prescale=float(ps1))
                         elif kind == "oneshot":
-                            outs = oneshot_reference(ins, gl, skip_incomplete=skip_incomplete, prescale=ps1)
+                            outs = oneshot_reference(ins, gl, skip_incomplete=skip_incomplete, prescale=ps1, fmt=fmt)
                         else:
                             outs = sra_reference(ins, gl, lanes=plan_lanes, min_lane_elems=cfg["min_lane_elems"],
-                                                 skip_incomplete=skip_incomplete, prescale=ps1)
+                                                 skip_incomplete=skip_incomplete, prescale=ps1, fmt=fmt)
                         ins = [o.reshape(-1) for o in outs]
                 else:
                     log(rk, "generic_intra", intra, seq, ps1)
                     ins = _generic_allreduce(cfg["inner_reduction"], ins, intra, prescale=ps1,
                                              skip_incomplete=skip_incomplete, stochastic=stochastic, seed=seed,
-                                             seq=seq)
+                                             seq=seq, fmt=fmt)
                 setvals(rk, ins)
         if not multi:
             continue
@@ -565,7 +586,7 @@ def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *,
             log(rk, "cross", group, cseq, cscale)
             setvals(rk, _generic_allreduce(cfg["cross_reduction"], [state[r] for r in rk], group, prescale=cscale,
                                            skip_incomplete=skip_incomplete, stochastic=stochastic, seed=seed,
-                                           seq=cseq))
+                                           seq=cseq, fmt=fmt))
         if not leaders_only:
             continue
         compressed = (cfg["intra_compress"] and any(l[2] < RAW_BITS for l in group)
@@ -581,7 +602,8 @@ def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *,
                     _C.LocalReducerGroup(L, "SRA", 20_000).broadcast_compressed(outs, group, 0, skip_incomplete,
                                                                                 True, seed, bseq)
                 else:
-                    outs = broadcast_compressed_reference(ins, group, root=0, skip_incomplete=skip_incomplete)
+                    outs = broadcast_compressed_reference(ins, group, root=0, skip_incomplete=skip_incomplete,
+                                                          fmt=fmt)
                 setvals(rk, outs)
             else:
                 log(rk, "bcast_raw", group, seq, 1.0)

@@ -89,6 +89,9 @@ class AdaptiveCGXState(CGXState):
         period: int = 1000,
     ):
         super().__init__(process_group, layer_min_size, compression_params)
+        if self.quantization_format is not None:
+            raise ValueError("AdaptiveCGXState: adaptive widths do not take FP8 formats, got "
+                             f"bits={self.quantization_format!r}")
         self.candidate_bits = tuple(int(b) for b in candidate_bits)
         if not self.candidate_bits or any(b < 1 or b > 8 for b in self.candidate_bits):
             raise ValueError(f"candidate_bits must be widths in 1..8, got {candidate_bits}")

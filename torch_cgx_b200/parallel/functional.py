@@ -43,11 +43,29 @@ _VARS = {
 }
 
 
+_FORMAT_VAR = "CGX_COMPRESSION_FORMAT"
+
+
 @contextlib.contextmanager
-def compression(bits: Optional[int] = None, bucket_size: Optional[int] = None,
+def compression(bits: Optional[A2aBits] = None, bucket_size: Optional[int] = None,
                 skip_incomplete: Optional[bool] = None, stochastic: Optional[bool] = None,
                 seed: Optional[int] = None) -> Iterator[None]:
-    """Temporarily override the env-level compression config (None = leave as is; bits=32 disables)."""
+    """Temporarily override the env-level compression config (None = leave as is; bits=32 disables).
+
+    ``bits="e4m3"`` or ``"e5m2"`` compresses at 8 bits and sends the allreduce's 8-bit layers as
+    FP8 codes with one fp32 scale per bucket (``CGX_COMPRESSION_FORMAT``); an integer ``bits``
+    selects max-min. FP8 rounds to nearest: an unknown name, or a name with ``stochastic=True`` or
+    ``CGX_STOCHASTIC_ROUNDING=1``, raises ValueError before anything is changed.
+    """
+    fmt = None
+    if bits is not None:
+        if isinstance(bits, str):
+            from .. import _C
+
+            _C.a2a_bits(bits, bool(stochastic), "allreduce")  # CGX_STOCHASTIC_ROUNDING=1: the call raises
+            fmt, bits = bits, 8
+        else:
+            fmt = "maxmin"
     new = {"bits": bits, "bucket_size": bucket_size, "skip_incomplete": skip_incomplete,
            "stochastic": stochastic, "seed": seed}
     saved = {}
@@ -58,6 +76,9 @@ def compression(bits: Optional[int] = None, bucket_size: Optional[int] = None,
             var = _VARS[k]
             saved[var] = os.environ.get(var)
             os.environ[var] = str(int(v))
+        if fmt is not None:
+            saved[_FORMAT_VAR] = os.environ.get(_FORMAT_VAR)
+            os.environ[_FORMAT_VAR] = fmt
         yield
     finally:
         for var, old in saved.items():
@@ -67,9 +88,10 @@ def compression(bits: Optional[int] = None, bucket_size: Optional[int] = None,
                 os.environ[var] = old
 
 
-def all_reduce(tensor: torch.Tensor, bits: Optional[int] = None, bucket_size: Optional[int] = None,
+def all_reduce(tensor: torch.Tensor, bits: Optional[A2aBits] = None, bucket_size: Optional[int] = None,
                average: bool = False, group=None, async_op: bool = False, **kw):
-    """``dist.all_reduce`` (SUM or AVG) with the given quantization for this call.
+    """``dist.all_reduce`` (SUM or AVG) with the given quantization for this call; ``bits`` may be an
+    FP8 format, ``"e4m3"`` or ``"e5m2"`` (see :func:`compression`).
 
     Note: with ``async_op=True`` the parameters are captured when the call is *issued*.
     """

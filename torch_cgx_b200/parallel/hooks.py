@@ -17,7 +17,7 @@ H100-first differences:
 """
 
 import os
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple, Union
 
 import torch
 import torch.distributed as dist
@@ -30,8 +30,25 @@ COMPRESSION_MINIMAL_SIZE = "CGX_COMPRESSION_MINIMAL_SIZE"
 VALUE_NO_COMPRESS = 32
 
 
+def _width_and_format(bits: Union[int, str]) -> Tuple[int, Optional[str]]:
+    """``bits`` of the compressed allreduce: a max-min width, or an FP8 format name ("e4m3" /
+    "e5m2"), whose layers are compressed at 8 bits. ValueError for any other name."""
+    if not isinstance(bits, str):
+        return int(bits), None
+    from .. import _C
+
+    _C.a2a_bits(bits, False, "allreduce")
+    return 8, bits
+
+
 class CGXState(object):
-    """State of :func:`cgx_hook` (argument-compatible with the reference)."""
+    """State of :func:`cgx_hook` (argument-compatible with the reference).
+
+    ``compression_params["bits"]`` is a max-min width or an FP8 format, ``"e4m3"`` or ``"e5m2"``
+    (the usual choice for gradients): the compressed layers are then registered at 8 bits and sent
+    as FP8 codes with one fp32 scale per bucket. ``quantization_bits`` holds the width and
+    ``quantization_format`` the format name (None: max-min, or ``CGX_COMPRESSION_FORMAT``'s).
+    """
 
     def __init__(
         self,
@@ -44,12 +61,14 @@ class CGXState(object):
         self.layer_min_size = max(layer_min_size, min_size_to_compress)
         self.quantization_bits = int(os.getenv(COMPRESSION_QUANTIZATION_BITS, str(VALUE_NO_COMPRESS)))
         self.quantization_bucket_size = int(os.getenv(COMPRESSION_BUCKET_SIZE, "1024"))
+        self.quantization_format: Optional[str] = None
         self.step = 0
         self.layer_idx = 0
         # step at which layers are registered (DDP rebuilds buckets after the 1st iteration)
         self.register_step = 2
         if compression_params is not None:
-            self.quantization_bits = compression_params.get("bits", self.quantization_bits)
+            self.quantization_bits, self.quantization_format = _width_and_format(
+                compression_params.get("bits", self.quantization_bits))
             self.quantization_bucket_size = compression_params.get("bucket_size", self.quantization_bucket_size)
 
     def should_compress_(self, tensor: torch.Tensor) -> bool:
@@ -63,13 +82,14 @@ class CGXState(object):
         return {
             "step": self.step,
             "layer_min_size": self.layer_min_size,
-            "quantization_bits": self.quantization_bits,
+            "quantization_bits": self.quantization_format or self.quantization_bits,
             "quantization_bucket_size": self.quantization_bucket_size,
         }
 
     def load_state_dict(self, sd: Dict[str, int]) -> None:
         self.layer_min_size = int(sd.get("layer_min_size", self.layer_min_size))
-        self.quantization_bits = int(sd.get("quantization_bits", self.quantization_bits))
+        self.quantization_bits, self.quantization_format = _width_and_format(
+            sd.get("quantization_bits", self.quantization_format or self.quantization_bits))
         self.quantization_bucket_size = int(sd.get("quantization_bucket_size", self.quantization_bucket_size))
         # layers must be re-registered with the (new) process: restart the warm-up
         self.step = 0
@@ -88,14 +108,16 @@ def _native_backend(group, tensor: torch.Tensor):
     return hit[1]
 
 
-def _allreduce_fut(process_group, tensor: torch.Tensor, bucket_idx: int = -1) -> torch.futures.Future[torch.Tensor]:
-    """Average ``tensor`` across the group, return a future of the tensor."""
+def _allreduce_fut(process_group, tensor: torch.Tensor, bucket_idx: int = -1,
+                   fmt: Optional[str] = None) -> torch.futures.Future[torch.Tensor]:
+    """Average ``tensor`` across the group, return a future of the tensor. ``fmt``: the FP8 format
+    of the 8-bit layers (None: ``CGX_COMPRESSION_FORMAT``'s)."""
     group_to_use = process_group if process_group is not None else dist.group.WORLD
     native = _native_backend(group_to_use, tensor)
     if native is not None:
         # 1/world is applied inside the kernel, before quantization (same
         # numerics as the reference's div-then-allreduce, without the extra pass)
-        work = native.allreduce_bucket(tensor, bucket_idx, True)
+        work = native.allreduce_bucket(tensor, bucket_idx, True, fmt)
         return work.get_future().then(lambda fut: fut.value()[0])
     # any other backend (nccl / gloo): the reference's recipe verbatim
     tensor.div_(group_to_use.size())
@@ -118,7 +140,8 @@ def cgx_hook(state: CGXState, bucket: dist.GradBucket) -> torch.futures.Future[t
     if bucket.is_last():
         state.step += 1
         state.layer_idx = 0
-    return _allreduce_fut(state.process_group, bucket.buffer(), bucket.index() if registered else -1)
+    return _allreduce_fut(state.process_group, bucket.buffer(), bucket.index() if registered else -1,
+                          state.quantization_format)
 
 
 def register_cgx_hook(ddp_model, state: CGXState, native: Optional[bool] = None):
@@ -150,7 +173,8 @@ def register_cgx_hook(ddp_model, state: CGXState, native: Optional[bool] = None)
     if adaptive:
         extra = dict(candidates=list(state.candidate_bits), period=int(state.period), assignment=dict(state._loaded))
     handle = _C.register_native_hook(ddp_model.reducer, backend, int(state.layer_min_size),
-                                     int(state.quantization_bits), int(state.quantization_bucket_size),
+                                     state.quantization_format or int(state.quantization_bits),
+                                     int(state.quantization_bucket_size),
                                      int(state.register_step), **extra)
     try:
         ddp_model.logger._set_comm_hook_name("cgx_native_hook")
