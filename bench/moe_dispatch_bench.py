@@ -12,12 +12,21 @@ returns them into T k slots (token * k + choice), slot output_index[j] for recei
   combine  (a): all_to_all(back, recv); out.index_copy_(0, output_index, back)
   combine  (b): all_to_all(out, recv, output_index)
 
+With --codes, an FP8 expert GEMM's input instead (e4m3, routed dispatch, bucket 128 and bucket = H):
+
+  dispatch (c): all_to_all(recv, x, input_index, bits="e4m3"), then the per-group FP8 quantize a
+                caller writes in torch (amax, scale, cast) to get codes and scales for the GEMM
+  dispatch (d): all_to_all(codes, x, input_index, bits="e4m3", output_scales=scales)
+
 Arms alternate in one run, CUDA events around each, medians over --iters after --warmup. The HBM
 bytes of an arm are computed from shapes, all ranks together: the kernel reads the sent rows and
 writes the received rows (2 N H es), writes and reads its wire image once (2 N H bits / 8, plus
 8 bytes per 512-element bucket; raw at 32 bits, and own chunks are copied, not counted as wire);
 arm (a) adds the permutation's read and write of N rows (2 N H es). Virtual ranks share one GPU's
 HBM and exchange through it, so NVLink is not part of these numbers.
+For (c) and (d) the wire is 1 byte per element plus 8 per bucket; (c) writes the received rows in
+the dtype and its quantize reads them and writes 1 byte per element plus 4 per bucket, (d) writes
+those codes and scales directly.
 """
 import argparse
 import json
@@ -130,6 +139,73 @@ def run_config(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bflo
     return res
 
 
+def run_codes(W, T, H, k, bucket, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
+    """routed e4m3 dispatch: decode + torch quantize (c) against the codes output (d)"""
+    dev = torch.device("cuda", 0)
+    es = torch.tensor([], dtype=dtype).element_size()
+    route = routing(W, T, k, seed=T * 31 + H * 7 + k, device=dev)
+    send_rows = [route[q][2] for q in range(W)]
+    recv_n = [sum(send_rows[q][r] for q in range(W)) for r in range(W)]
+    counts = [[send_rows[q][r] * H for r in range(W)] for q in range(W)]
+    g = C.LocalSraGroup(W, lanes, slot_mb << 20, 20000, 256)
+    xs = [torch.randn(T, H, device=dev, dtype=dtype) for _ in range(W)]
+    ii = [route[q][0] for q in range(W)]
+    recv = [torch.empty(recv_n[r], H, device=dev, dtype=dtype) for r in range(W)]
+    codes = [torch.empty(recv_n[r], H, device=dev, dtype=torch.float8_e4m3fn) for r in range(W)]
+    scales = [torch.empty(recv_n[r], H // bucket, device=dev, dtype=torch.float32) for r in range(W)]
+    tq = [None] * W
+    flat = lambda ts: [t.reshape(-1) for t in ts]  # noqa: E731
+
+    def disp_c():
+        g.all_to_all(flat(xs), flat(recv), counts, bits="e4m3", bucket_size=bucket, input_index=ii, row=H)
+        for r in range(W):
+            v = recv[r].reshape(-1, bucket).float()
+            unit = v.abs().amax(dim=1, keepdim=True) * (1.0 / 448.0)
+            inv = torch.where(unit > 0, 1.0 / unit, torch.zeros_like(unit))
+            tq[r] = ((v * inv).clamp(-448.0, 448.0).to(torch.float8_e4m3fn), unit)
+
+    def disp_d():
+        g.all_to_all(flat(xs), flat(codes), counts, bits="e4m3", bucket_size=bucket, input_index=ii, row=H,
+                     output_scales=flat(scales))
+
+    arms = {"dispatch_c": disp_c, "dispatch_d": disp_d}
+    ts = {name: [] for name in arms}
+    for it in range(warmup + iters):
+        for name, fn in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            if it >= warmup:
+                ts[name].append(e0.elapsed_time(e1) * 1000.0)
+    g.check()
+    # (d) decodes to what (c) received, before its rounding to the dtype
+    for r in range(W):
+        dec = (codes[r].float().reshape(-1, bucket) * scales[r].reshape(-1, 1)).reshape(recv[r].shape).to(dtype)
+        own = sum(send_rows[q][r] for q in range(r))  # the own chunk: encoded by (d), copied by (c)
+        mine = slice(own, own + send_rows[r][r])
+        keep = torch.ones(recv_n[r], dtype=torch.bool, device=dev)
+        keep[mine] = False
+        assert torch.equal(dec[keep], recv[r][keep]), "codes arm differs from the decoded arm"
+
+    N = T * k * W
+    own = sum(send_rows[q][q] for q in range(W))
+    elems_wire = (N - own) * H
+    wire = elems_wire + (elems_wire // bucket) * 8
+    codes_out = N * H + N * H // bucket * 4
+    d_bytes = N * H * es + 2 * wire + codes_out
+    c_bytes = N * H * es + 2 * wire + N * H * es + N * H * es + codes_out
+    res = {"W": W, "T": T, "H": H, "topk": k, "bits": "e4m3", "bucket": bucket, "dtype": str(dtype).replace("torch.", "")}
+    for name in arms:
+        res[name + "_us"] = round(median(ts[name]), 1)
+    res["bytes_c_GB"] = round(c_bytes / 1e9, 3)
+    res["bytes_d_GB"] = round(d_bytes / 1e9, 3)
+    del g, xs, recv, codes, scales, tq
+    torch.cuda.empty_cache()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--world", type=int, default=8)
@@ -145,10 +221,29 @@ def main():
     ap.add_argument("--slot-mb", type=int, default=4)
     ap.add_argument("--max-gb", type=float, default=60.0, help="skip configurations whose buffers exceed this")
     ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
+    ap.add_argument("--codes", action="store_true",
+                    help="time the FP8 codes output, arms (c) and (d) at bucket 128 and bucket = H, instead")
     args = ap.parse_args()
     name, power = gpu_info()
     print(json.dumps({"gpu": name, "power_limit": power}), flush=True)
     rows = []
+    if args.codes:
+        for H in args.hidden:
+            for T in args.tokens:
+                for k in args.topk:
+                    need = args.world * (2 * T * k + T) * H * 2 / 1e9
+                    if need > args.max_gb:
+                        print(json.dumps({"H": H, "T": T, "topk": k, "skipped": f"needs {need:.1f} GB"}), flush=True)
+                        continue
+                    for bucket in (128, H):
+                        r = run_codes(args.world, T, H, k, bucket, args.iters, args.warmup, args.lanes, args.slot_mb)
+                        r.update(gpu=name, power_limit=power)
+                        rows.append(r)
+                        print(json.dumps(r), flush=True)
+        if args.out:
+            Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in rows))
+        return
     for H in args.hidden:
         for T in args.tokens:
             for k in args.topk:

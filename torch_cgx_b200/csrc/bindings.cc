@@ -309,9 +309,39 @@ std::vector<std::vector<uint64_t>> check_counts(const CountMatrix& counts, size_
   return out;
 }
 
+// the dtype of an all-to-all output: the inputs', or with codes (output_scales) one byte per element,
+// uint8 or the codec's float8
+bool a2a_output_dtype_ok(const at::Tensor& t, int dt, WireCodec codes_codec) {
+  if (codes_codec == kMaxMin) return cgx_dtype(t) == dt;
+  const at::ScalarType s = t.scalar_type();
+  return s == at::kByte || s == (codes_codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2);
+}
+
+// The codes output of the all-to-all bindings: `output_scales` holds one contiguous float32 tensor
+// per rank, on the side of the outputs, with one element per bucket of the rank's output; the
+// outputs then hold codes (a2a_output_dtype_ok). Returns the pointers (empty: decoded output).
+std::vector<float*> a2a_scales(const std::optional<std::vector<at::Tensor>>& scales,
+                               const std::vector<at::Tensor>& outputs, const A2aBits& wb, int64_t bucket) {
+  std::vector<float*> ptrs;
+  if (!scales) return ptrs;
+  if (wb.codec == kMaxMin) throw py::value_error("cgx all_to_all: output_scales needs bits \"e4m3\" or \"e5m2\"");
+  if (bucket < 1 || bucket > (int64_t)kMaxBlockElems)
+    throw py::value_error("cgx all_to_all: output_scales needs 1 <= bucket_size <= " + std::to_string(kMaxBlockElems));
+  TORCH_CHECK(scales->size() == outputs.size(), "all_to_all: one output_scales tensor per rank");
+  for (size_t r = 0; r < outputs.size(); ++r) {
+    const at::Tensor& s = (*scales)[r];
+    TORCH_CHECK(s.scalar_type() == at::kFloat && s.is_contiguous() && s.is_cuda() == outputs[r].is_cuda() &&
+                    s.numel() * bucket == outputs[r].numel(),
+                "all_to_all: rank ", r, "'s output_scales must be a contiguous float32 tensor of one element per ",
+                "bucket of its output, on the outputs' device");
+    ptrs.push_back(s.data_ptr<float>());
+  }
+  return ptrs;
+}
+
 // rank r's input holds row r of the matrix, its output column r
 void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<at::Tensor>& outputs,
-                       const std::vector<std::vector<uint64_t>>& counts, bool cuda) {
+                       const std::vector<std::vector<uint64_t>>& counts, bool cuda, WireCodec codes_codec = kMaxMin) {
   const size_t W = counts.size();
   TORCH_CHECK(inputs.size() == W && outputs.size() == W, "all_to_all: one input and one output per rank");
   const int dt = cgx_dtype(inputs[0]);
@@ -322,7 +352,8 @@ void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<
       nout += counts[q][r];
     }
     for (const at::Tensor* t : {&inputs[r], &outputs[r]})
-      TORCH_CHECK(t->is_cuda() == cuda && t->is_contiguous() && cgx_dtype(*t) == dt,
+      TORCH_CHECK(t->is_cuda() == cuda && t->is_contiguous() &&
+                      (t == &inputs[r] ? cgx_dtype(*t) == dt : a2a_output_dtype_ok(*t, dt, codes_codec)),
                   "all_to_all: contiguous tensors of one dtype, all on ", cuda ? "the GPU" : "the CPU");
     TORCH_CHECK((uint64_t)inputs[r].numel() == nin && (uint64_t)outputs[r].numel() == nout,
                 "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
@@ -331,10 +362,11 @@ void check_a2a_tensors(const std::vector<at::Tensor>& inputs, const std::vector<
 
 void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                             const CountMatrix& counts_in, const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic,
-                            uint64_t seed, uint32_t seq) {
+                            uint64_t seed, uint32_t seq, const std::optional<std::vector<at::Tensor>>& output_scales) {
   const A2aBits wb = a2a_bits(bits_arg, stochastic);
   const auto counts = check_counts(counts_in, inputs.size());
-  check_a2a_tensors(inputs, outputs, counts, false);
+  const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
+  check_a2a_tensors(inputs, outputs, counts, false, output_scales ? wb.codec : kMaxMin);
   std::vector<const void*> in;
   std::vector<void*> out;
   for (size_t r = 0; r < inputs.size(); ++r) {
@@ -342,7 +374,7 @@ void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
     out.push_back(outputs[r].data_ptr());
   }
   all_to_all_simulate(cgx_dtype(inputs[0]), in, out, counts, wb.bits, wb.codec, (uint32_t)bucket,
-                      make_rng(stochastic, seed, seq));
+                      make_rng(stochastic, seed, seq), output_scales ? &scales : nullptr);
 }
 
 // the items of one chunk from common/a2a.h, rows as in plan_to_dict, offsets in the contiguous image
@@ -611,9 +643,13 @@ class LocalSraGroup {
   // outputs[r], rows of `row` elements; the counts then describe the logical buffers of whole rows.
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
                   const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
-                  const IndexList& input_index, const IndexList& output_index, int64_t row) {
+                  const IndexList& input_index, const IndexList& output_index, int64_t row,
+                  const std::optional<std::vector<at::Tensor>>& output_scales) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)world_);
+    TORCH_CHECK((int)outputs.size() == world_, "all_to_all: one input and one output per rank");
+    const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
+    const WireCodec codes_codec = output_scales ? wb.codec : kMaxMin;
     const bool routed = !input_index.empty() || !output_index.empty();
     TORCH_CHECK(input_index.empty() || (int)input_index.size() == world_, "all_to_all: one input_index per rank");
     TORCH_CHECK(output_index.empty() || (int)output_index.size() == world_, "all_to_all: one output_index per rank");
@@ -650,7 +686,9 @@ class LocalSraGroup {
         nout += counts[q][r];
       }
       for (const at::Tensor* t : {&inputs[r], &outputs[r]})
-        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == cgx_dtype(inputs[0]),
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() &&
+                        (t == &inputs[r] ? cgx_dtype(*t) == cgx_dtype(inputs[0])
+                                         : a2a_output_dtype_ok(*t, cgx_dtype(inputs[0]), codes_codec)),
                     "all_to_all: contiguous tensors of one dtype, all on the GPU");
       TORCH_CHECK((in_ix || (uint64_t)inputs[r].numel() == nin) && (out_ix || (uint64_t)outputs[r].numel() == nout),
                   "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
@@ -662,7 +700,8 @@ class LocalSraGroup {
                 std::vector<uint64_t> out_counts(world_);
                 for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
                 fused_[r]->all_to_all(inputs[r].data_ptr(), outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits,
-                                      wb.codec, (uint32_t)bucket, rng, streams_[r].stream(), routed ? &routes[r] : nullptr);
+                                      wb.codec, (uint32_t)bucket, rng, streams_[r].stream(), routed ? &routes[r] : nullptr,
+                                      scales.empty() ? nullptr : scales[r]);
               });
   }
   void check() {
@@ -812,16 +851,18 @@ class LocalReducerGroup {
   }
   // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
-                  const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq) {
+                  const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
+                  const std::optional<std::vector<at::Tensor>>& output_scales) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)hub_.world());
-    check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda());
+    const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
+    check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda(), output_scales ? wb.codec : kMaxMin);
     const RngParams rng = make_rng(stochastic, seed, seq);
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
       std::vector<uint64_t> out_counts(counts.size());
       for (size_t q = 0; q < counts.size(); ++q) out_counts[q] = counts[q][r];
       red.all_to_all(in, outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits, wb.codec, (uint32_t)bucket, rng,
-                     s);
+                     s, scales.empty() ? nullptr : scales[r]);
     }, false);
   }
   // bytes each rank's reducer counted as sent during the last call
@@ -1557,16 +1598,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("all_to_all_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
               const std::vector<int64_t>& in_splits, const A2aBitsArg& bits, int bucket_size, bool stochastic,
-              int64_t seed, const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index) {
+              int64_t seed, const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index,
+              const std::optional<at::Tensor>& out_scales) {
              const A2aBits wb = a2a_bits(bits, stochastic);
              return pg.all_to_all_compressed(out, in, out_splits, in_splits, wb.bits, wb.codec, bucket_size,
-                                             stochastic, seed,
-                                             in_index.value_or(at::Tensor()), out_index.value_or(at::Tensor()));
+                                             stochastic, seed, in_index.value_or(at::Tensor()),
+                                             out_index.value_or(at::Tensor()), out_scales.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
            py::arg("input_split_sizes") = std::vector<int64_t>{}, py::arg("bits") = 8, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("input_index") = py::none(),
-           py::arg("output_index") = py::none(), py::call_guard<py::gil_scoped_release>())
+           py::arg("output_index") = py::none(), py::arg("output_scales") = py::none(),
+           py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -1745,7 +1788,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("prescale") = py::none(), py::arg("bits") = py::none());
   m.def("all_to_all_simulate", &py_all_to_all_simulate, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
         py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
-        py::arg("seq") = 0);
+        py::arg("seq") = 0, py::arg("output_scales") = py::none());
   m.def(
       "a2a_bits",
       [](const A2aBitsArg& bits, bool stochastic, const std::string& op) {
@@ -1863,7 +1906,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
-           py::arg("row") = 1)
+           py::arg("row") = 1, py::arg("output_scales") = py::none())
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))
@@ -1886,7 +1929,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("bits") = py::none())
       .def("all_to_all", &LocalReducerGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
-           py::arg("seq") = 0)
+           py::arg("seq") = 0, py::arg("output_scales") = py::none())
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())

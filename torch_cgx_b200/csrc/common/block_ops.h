@@ -238,6 +238,22 @@ inline void decode_block_fp8_store(const uint8_t* rec, int dtype, const BlockDes
   }
 }
 
+// An FP8 record undecoded (the all-to-all's codes output): codes[elem_off + i] = element i's code,
+// scales[(elem_off + i) / B] = its bucket's unit; elem_off is a multiple of B
+inline void unpack_block_fp8(const uint8_t* rec, const BlockDesc& d, uint8_t* codes, float* scales) {
+  const uint32_t n = block_n(d);
+  const uint32_t B = d.bucket;
+  const uint32_t nb = block_num_buckets(n, B);
+  const uint32_t gpb = bucket_groups(B);
+  const BucketMeta* meta = reinterpret_cast<const BucketMeta*>(rec);
+  const uint8_t* pay = rec + block_meta_bytes(n, B);
+  for (uint32_t b = 0; b < nb; ++b) {
+    const uint32_t lo = b * B, hi = lo + B < n ? lo + B : n;
+    scales[d.elem_off / B + b] = meta[b].unit;
+    std::memcpy(codes + (size_t)d.elem_off + lo, pay + (size_t)b * gpb * 8u, hi - lo);
+  }
+}
+
 // acc[i] = fl(acc[i] + fl(float(code) * unit)): the reduce-scatter's accumulation of an FP8 record
 inline void decode_block_fp8_add(const uint8_t* rec, const BlockDesc& d, float* acc, int codec) {
   const uint32_t n = block_n(d);

@@ -98,12 +98,21 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
 
 void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, const std::vector<void*>& out_bufs,
                          const std::vector<std::vector<uint64_t>>& counts, int bits, WireCodec codec,
-                         uint32_t bucket, const RngParams& rng) {
+                         uint32_t bucket, const RngParams& rng, const std::vector<float*>* out_scales) {
   const int W = (int)in_bufs.size();
   if ((int)out_bufs.size() != W || (int)counts.size() != W)
     throw std::invalid_argument("all_to_all_simulate: need one input, output and count row per rank");
   for (const auto& row : counts)
     if ((int)row.size() != W) throw std::invalid_argument("all_to_all_simulate: counts must be W x W");
+  const bool codes = out_scales != nullptr;
+  if (codes) {
+    if ((int)out_scales->size() != W) throw std::invalid_argument("all_to_all_simulate: need one scales buffer per rank");
+    if (codec == kMaxMin || bits != 8) throw std::invalid_argument("all_to_all_simulate: codes need an FP8 codec");
+    if (bucket < 1 || bucket > kMaxBlockElems) throw std::invalid_argument("all_to_all_simulate: bad bucket for codes");
+    for (const auto& row : counts)
+      for (uint64_t n : row)
+        if (n % bucket) throw std::invalid_argument("all_to_all_simulate: with codes every count holds whole buckets");
+  }
   const int es = dtype_size(dtype);
   std::vector<float> acc(kMaxBlockElems);
   std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
@@ -114,10 +123,10 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
       for (int s = 0; s < q; ++s) out_off += counts[s][r];
       const uint64_t n = counts[q][r];
       const uint8_t* src = static_cast<const uint8_t*>(in_bufs[q]) + in_off * es;
-      uint8_t* dst = static_cast<uint8_t*>(out_bufs[r]) + out_off * es;
+      uint8_t* dst = static_cast<uint8_t*>(out_bufs[r]) + out_off * (codes ? 1 : es);
       in_off += n;
       if (n == 0) continue;
-      if (q == r || bits >= kRawBits) {
+      if (!codes && (q == r || bits >= kRawBits)) {
         std::memcpy(dst, src, n * es);
         continue;
       }
@@ -132,6 +141,11 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
         d.n_bits = (a2a_block_n(g, b) & 0xFFFFFFu) | ((uint32_t)g.bits << 24);
         d.bucket = g.bucket;
         cpu::load_block(src, dtype, d, 1.0f, acc.data());
+        if (codes) {
+          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+          cpu::unpack_block_fp8(rec.data(), d, dst, (*out_scales)[r] + out_off / bucket);
+          continue;
+        }
         if (codec != kMaxMin) {
           cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
           cpu::decode_block_fp8_store(rec.data(), dtype, d, dst, codec);

@@ -56,10 +56,12 @@ void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& i
 // chunk is copied, and so is every chunk when bits >= kRawBits (raw). Every other chunk is decode(Q(x))
 // with buckets counted from the chunk's first element (common/a2a.h) and the pair's random stream
 // a2a_rng_stream(q, r). With an FP8 codec (bits 8) the chunks use its records instead of max-min's
-// and round to nearest.
+// and round to nearest. With `out_scales` (one per rank; an FP8 codec, bucket <= kMaxBlockElems
+// dividing every count) out_bufs[r] receives one code byte per element and out_scales[r] the unit of
+// every bucket, undecoded, the own chunk encoded too (the fused kernel's codes output).
 void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, const std::vector<void*>& out_bufs,
                          const std::vector<std::vector<uint64_t>>& counts, int bits, WireCodec codec,
-                         uint32_t bucket, const RngParams& rng);
+                         uint32_t bucket, const RngParams& rng, const std::vector<float*>* out_scales = nullptr);
 
 // Quantize->dequantize round trip of one rank's buffer through the plan's
 // blocks (what a single compression step does to the data); used by the Python

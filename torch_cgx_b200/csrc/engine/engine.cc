@@ -44,12 +44,32 @@ std::vector<std::vector<LayerSpec>> split_for_fusion(const std::vector<LayerSpec
   return groups;
 }
 
+namespace {
+// the communicator of a one-rank group: there is no one to exchange with
+class SelfCommunicator : public Communicator {
+ public:
+  explicit SelfCommunicator(bool cuda) : cuda_(cuda) {}
+  int rank() const override { return 0; }
+  int size() const override { return 1; }
+  bool is_cuda() const override { return cuda_; }
+  void exchange(const std::vector<P2POp>& ops, cudaStream_t) override {
+    if (!ops.empty()) throw std::logic_error("cgx: a one-rank group has no peer to exchange with");
+  }
+  void barrier() override {}
+
+ private:
+  bool cuda_;
+};
+}  // namespace
+
 AllreduceEngine::AllreduceEngine(int rank, int world, const EngineConfig& cfg)
     : rank_(rank), world_(world), local_size_(world), cfg_(cfg) {}
 
 AllreduceEngine::~AllreduceEngine() {
   // reducers release their scratch through the block backend: they must go first
   for (GenericPath* g : {&gen_cuda_, &gen_cpu_}) {
+    g->self.reset();
+    g->self_comm.reset();
     g->cross.reset();
     g->intra.reset();
     g->cross_comm.reset();
@@ -68,6 +88,8 @@ void AllreduceEngine::set_topology(int local_size) {
 void AllreduceEngine::attach_generic(bool cuda, std::unique_ptr<Communicator> intra,
                                      std::unique_ptr<Communicator> cross) {
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  g.self.reset();
+  g.self_comm.reset();
   g.intra.reset();
   g.cross.reset();
   g.ops = cuda ? make_cuda_block_backend() : make_cpu_block_backend();
@@ -329,14 +351,14 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
 void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                  const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
                                  uint32_t bucket, const RngParams& rng_in, cudaStream_t stream,
-                                 const A2aRoute* route) {
+                                 const A2aRoute* route, float* out_scales) {
   if (nodes() > 1)
     throw std::runtime_error("cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE " +
                              std::to_string(local_size_) + " < world size " + std::to_string(world_) + ")");
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route, out_scales);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
   if (routed && !routes_in_kernel(cuda, dtype, bits, bucket, route->row))
     throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
@@ -351,10 +373,19 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
   stats_.elements += total;
   if (fused) {
     const FusedSra::A2aCounts n =
-        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, route);
+        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, route, out_scales);
     stats_.kernel_launches += n.launches;
     stats_.wire_bytes += n.wire_bytes;
     stats_.raw_bytes += n.raw_bytes;
+    return;
+  }
+  if (world_ == 1 && out_scales != nullptr) {
+    if (!g.ops) throw std::runtime_error("cgx: the compressed all_to_all has no block backend");
+    if (!g.self) {
+      g.self_comm = std::make_unique<SelfCommunicator>(cuda);
+      g.self = make_reducer(ReductionType::kSRA, g.self_comm.get(), g.ops.get());
+    }
+    g.self->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, out_scales);
     return;
   }
   if (world_ == 1) {
@@ -367,7 +398,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
     return;
   }
   const uint64_t before = g.intra->bytes_sent();
-  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream);
+  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, out_scales);
   stats_.wire_bytes += g.intra->bytes_sent() - before;
   for (int q = 0; q < world_; ++q)
     if (q != rank_) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);

@@ -74,6 +74,10 @@ struct GenericPath {
   std::unique_ptr<Communicator> cross_comm;  // ranks with my local rank on the other nodes (null if one node)
   std::unique_ptr<Reducer> intra;
   std::unique_ptr<Reducer> cross;
+  // world 1: a reducer over a one-rank communicator, made on first use, that encodes the all-to-all's
+  // codes output (nothing is exchanged)
+  std::unique_ptr<Communicator> self_comm;
+  std::unique_ptr<Reducer> self;
 };
 
 class AllreduceEngine {
@@ -165,10 +169,12 @@ class AllreduceEngine {
   // the arguments): the fused kernel on the P2P transport, else the generic intra-node reducer. One
   // node only: with several nodes every rank throws the same std::runtime_error before anything runs.
   // A `route` with an index needs routes_in_kernel(); callers compose index_select / index_copy_
-  // around a plain call otherwise.
+  // around a plain call otherwise. `out_scales` selects the codes output (FusedSra::all_to_all); at
+  // world 1 without a heap the chunk is then encoded by the generic reducer's path, not copied.
   void all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
-                  const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route = nullptr);
+                  const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route = nullptr,
+                  float* out_scales = nullptr);
   // whether a routed all-to-all of rows of `row` elements runs inside the fused kernel: the P2P
   // transport with a heap, and rows that hold whole quantization items (a2a_rows_fit)
   bool routes_in_kernel(bool cuda, int dtype, int bits, uint32_t bucket, uint64_t row) const;

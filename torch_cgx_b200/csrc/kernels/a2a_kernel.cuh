@@ -168,9 +168,10 @@ __device__ __forceinline__ bool a2a_window_item(const A2aGeom& g, const A2aWindo
   return true;
 }
 
-// one item of a chunk for a peer in an FP8 codec (KB 8 records, round to nearest)
-template <typename T, int CODEC, int GPL>
-__device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& it, const OneDst& push) {
+// one item of a chunk in an FP8 codec (KB 8 records, round to nearest): to a peer's slot (OneDst),
+// or to the codes output (CodesDst)
+template <typename T, int CODEC, int GPL, typename DST>
+__device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& it, const DST& push) {
   if (item_kind(it) == kItemFull) {
     if (group_aligned<T>(src)) {
       float x[GPL][8];
@@ -221,7 +222,7 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
       src = chunk + it.elem_off;
     }
     if constexpr (CODEC != kMaxMin) {
-      a2a_send_item_fp8<T, CODEC, GPL>(src, it, push);
+      a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, push);
       continue;
     }
     const uint32_t kind = item_kind(it);
@@ -241,7 +242,42 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
   }
 }
 
-template <typename T, int KB, int GPL, bool IDX, int CODEC>
+// codes output: where element e of the logical receive buffer goes (p.out holds one code byte per
+// element; nullptr: a bad index), and the scale of the bucket that starts there
+__device__ __forceinline__ uint8_t* a2a_codes_addr(const A2aParams& p, bool idx, uint32_t e) {
+  uint8_t* codes = reinterpret_cast<uint8_t*>(p.out);
+  return idx ? a2a_row_addr(p, codes, p.out_index, p.out_rows, e, 1u) : codes + e;
+}
+__device__ __forceinline__ float* a2a_scales_addr(const A2aParams& p, const uint8_t* codes) {
+  return p.out_scales + (uint64_t)(codes - reinterpret_cast<const uint8_t*>(p.out)) / p.bucket;
+}
+
+// codes output, my own chunk: every item through the peers' FP8 encoder, straight into (codes,
+// scales), one warp per item over the whole grid
+template <typename T, int GPL, bool IDX, int CODEC>
+__device__ __forceinline__ void a2a_encode_own(const A2aParams& p) {
+  const int r = p.rank;
+  const A2aGeom g = a2a_geom(p.in_cnt[r], p.bits, p.bucket, (int)sizeof(T));
+  const uint32_t nb = a2a_num_blocks(g), total = nb * g.block_items, nwarps = gridDim.x * kSraWarps;
+  for (uint32_t t = blockIdx.x * kSraWarps + (threadIdx.x >> 5); t < total; t += nwarps) {
+    const uint32_t b = t / g.block_items, j = t - b * g.block_items;
+    if (b + 1u == nb && j >= a2a_block_num_items(g, a2a_block_n(g, b))) continue;
+    const WarpItem it = a2a_block_item(g, b, j);
+    const T* src;
+    if constexpr (IDX) {
+      src = a2a_row_addr(p, reinterpret_cast<const T*>(p.in), p.in_index, p.in_rows, p.in_off[r] + it.elem_off, 0u);
+      if (src == nullptr) continue;
+    } else {
+      src = reinterpret_cast<const T*>(p.in) + p.in_off[r] + it.elem_off;
+    }
+    uint8_t* codes = a2a_codes_addr(p, IDX, p.out_off[r] + it.elem_off);
+    if (codes == nullptr) continue;
+    const CodesDst ds{codes, a2a_scales_addr(p, codes), it.meta_off, it.pay_off, item_n(it)};
+    a2a_send_item_fp8<T, CODEC, GPL, CodesDst>(src, it, ds);
+  }
+}
+
+template <typename T, int KB, int GPL, bool IDX, int CODEC, bool CODES>
 __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k) {
   const int r = p.rank;
   const A2aGeom g = a2a_geom(p.out_cnt[q], p.bits, p.bucket, (int)sizeof(T));
@@ -253,6 +289,11 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
     uint32_t wire;
     if (!a2a_window_item(g, w, t, it, wire)) continue;
     const SrcSet ss{share + wire, 0u, 1, -1};
+    if constexpr (CODES) {
+      uint8_t* codes = a2a_codes_addr(p, IDX, p.out_off[q] + it.elem_off);
+      if (codes != nullptr) fp8_unpack_item<GPL>(ss.base, it, codes, a2a_scales_addr(p, codes));
+      continue;
+    }
     T* dst;
     if constexpr (IDX) {
       dst = a2a_row_addr(p, reinterpret_cast<T*>(p.out), p.out_index, p.out_rows, p.out_off[q] + it.elem_off, 1u);
@@ -284,9 +325,12 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
 // IDX: the routed form (A2aParams::in_index / out_index); only the item addresses and the own-chunk
 // copy differ, and the plain instantiations compile as before.
 // CODEC: the wire codec of the peers' chunks (quant_math.h); the FP8 ones exist with KB 8 only.
-template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin>
+// CODES (FP8 codecs only, A2aParams::out_scales set): the output receives the codes and units of
+// every chunk undecoded, the own chunk encoded like a peer's.
+template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin, bool CODES = false>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const __grid_constant__ A2aParams p) {
   static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
+  static_assert(!CODES || CODEC != kMaxMin, "codes are delivered for the FP8 codecs only");
   __shared__ int s_abort;
   __shared__ uint32_t s_send[kMaxPeers], s_recv[kMaxPeers];  // this lane's windows per destination / source
   const int lane = blockIdx.x, r = p.rank, W = p.world;
@@ -331,7 +375,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if (s_abort) break;
     for (int s = 1; s < W; ++s) {
       const int q = (r + W - s) % W;
-      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX, CODEC>(p, q, bpw, k);
+      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX, CODEC, CODES>(p, q, bpw, k);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_recv)
@@ -340,7 +384,9 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 
   // my own chunk last: the pushes to the peers are on the critical path, the copy is not
   if (!s_abort) {
-    if constexpr (IDX)
+    if constexpr (CODES)
+      a2a_encode_own<T, GPL, IDX, CODEC>(p);
+    else if constexpr (IDX)
       a2a_copy_own_rows<T>(p);
     else
       a2a_copy_own<T>(p);
@@ -366,14 +412,20 @@ template <typename T, int GPL, bool IDX>
 cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
   if (p.codec != kMaxMin) {
     if (p.bits != 8) return cudaErrorInvalidValue;
-    if (p.codec == kE4M3)
+    const bool codes = p.out_scales != nullptr;
+    if (p.codec == kE4M3 && codes)
+      dev::a2a_kernel<T, 8, GPL, IDX, kE4M3, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    else if (p.codec == kE4M3)
       dev::a2a_kernel<T, 8, GPL, IDX, kE4M3><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    else if (p.codec == kE5M2 && codes)
+      dev::a2a_kernel<T, 8, GPL, IDX, kE5M2, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
     else if (p.codec == kE5M2)
       dev::a2a_kernel<T, 8, GPL, IDX, kE5M2><<<p.lanes, kSraThreads, 0, stream>>>(p);
     else
       return cudaErrorInvalidValue;
     return cudaGetLastError();
   }
+  if (p.out_scales != nullptr) return cudaErrorInvalidValue;
   const int kb = (p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0;
   switch (kb) {
     case 2: dev::a2a_kernel<T, 2, GPL, IDX><<<p.lanes, kSraThreads, 0, stream>>>(p); break;

@@ -207,6 +207,14 @@ dequantize_items_fp8_kernel(const uint8_t* __restrict__ wire, const WarpItem* __
   }
 }
 
+// codes / scales = the records' FP8 codes and units, undecoded (the generic all-to-all's codes output)
+template <int GPL>
+__global__ void __launch_bounds__(kThreads, 3)
+unpack_items_fp8_kernel(const uint8_t* __restrict__ wire, const WarpItem* __restrict__ items, uint32_t first,
+                        uint32_t count, uint8_t* __restrict__ codes, float* __restrict__ scales, uint32_t bucket) {
+  CGX_ITEM_LOOP(it) { fp8_unpack_item<GPL>(wire, it, codes + it.elem_off, scales + it.elem_off / bucket); }
+}
+
 // acc (fp32 scratch) = float(init_src) * prescale   (init_src != nullptr)
 // acc = fl(acc + fl(float(code) * unit))            (wire != nullptr)
 template <typename T, int CODEC, int GPL>
@@ -433,6 +441,18 @@ cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire
   CGX_BY_DTYPE(a.dtype, (dequantize_t<float>(a, wire, (float*)dst, stream)),
                (dequantize_t<__half>(a, wire, (__half*)dst, stream)),
                (dequantize_t<__nv_bfloat16>(a, wire, (__nv_bfloat16*)dst, stream)))
+}
+
+cudaError_t launch_unpack_items_fp8(const ItemKernelArgs& a, const uint8_t* wire, uint8_t* codes, float* scales,
+                                    uint32_t bucket, cudaStream_t stream) {
+  if (a.count == 0) return cudaSuccess;
+  if (a.uniform_bits != 8 || bucket == 0) return cudaErrorInvalidValue;
+  const int grid = grid_for(a.count);
+  if (a.slice_elems == 1024)
+    unpack_items_fp8_kernel<4><<<grid, kThreads, 0, stream>>>(wire, a.items, a.first, a.count, codes, scales, bucket);
+  else
+    unpack_items_fp8_kernel<2><<<grid, kThreads, 0, stream>>>(wire, a.items, a.first, a.count, codes, scales, bucket);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* wire, float* acc_f32,

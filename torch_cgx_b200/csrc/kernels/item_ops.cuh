@@ -960,6 +960,82 @@ __device__ __noinline__ void bucket_recv_fp8(const uint8_t* rec, const WarpItem 
   }
 }
 
+// ---- FP8 codes handed to the caller undecoded (the all-to-all's codes output) ----------------------
+// Inside an item the codes of an FP8 record are in element order (full items: group g at pay_off +
+// 8g; bucket items: one bucket, byte i at pay_off + i), so element e of the item is codes[e] and the
+// unit of its bucket b is scales[b]: unpacking is a copy.
+//
+// The destination that lets the FP8 encoders write an item straight to (codes, scales): a meta store
+// (dst_st_v2: only metas use it in the FP8 encoders) keeps the unit, payload stores land at
+// codes + (off - pay_off), and the bytes past the item's n elements (a bucket's padding) are dropped.
+struct CodesDst {
+  uint8_t* codes;
+  float* scales;
+  uint32_t meta_off, pay_off, n;
+};
+__device__ __forceinline__ CodesDst unicast_of(const CodesDst& ds) { return ds; }
+__device__ __forceinline__ void dst_st_v2(const CodesDst& ds, uint32_t off, uint32_t a, uint32_t) {
+  ds.scales[(off - ds.meta_off) >> 3] = __uint_as_float(a);
+}
+__device__ __forceinline__ void dst_st_u8(const CodesDst& ds, uint32_t off, uint32_t v) {
+  const uint32_t o = off - ds.pay_off;
+  if (o < ds.n) st_u8(ds.codes + o, v);
+}
+// 16 payload bytes of a full item (never past n: full items are whole slices)
+__device__ __forceinline__ void dst_st_v4(const CodesDst& ds, uint32_t off, const uint4& v) {
+  uint8_t* d = ds.codes + (off - ds.pay_off);
+  if ((reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
+    st_v4(d, v);
+    return;
+  }
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int t = 0; t < 16; ++t) st_u8(d + t, (w[t >> 2] >> (8 * (t & 3))) & 0xFFu);
+}
+
+// one item of an FP8 record -> its codes and the units of its buckets, with the loads of slice_fetch
+template <int GPL>
+__device__ __forceinline__ void full_unpack_fp8(const uint8_t* rec, const WarpItem& it, uint8_t* codes, float* scales) {
+  uint32_t lo[GPL], hi[GPL];
+  load_words<8, GPL>(rec + it.pay_off, 8, lo, hi);
+  uint8_t* d = codes + lane_id() * (GPL * 8u);
+  if ((reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
+#pragma unroll
+    for (int k = 0; k < GPL; k += 2) st_v4(d + k * 8, make_uint4(lo[k], hi[k], lo[k + 1], hi[k + 1]));
+  } else {
+#pragma unroll
+    for (int k = 0; k < GPL; ++k)
+#pragma unroll
+      for (int t = 0; t < 8; ++t) st_u8(d + k * 8 + t, ((t < 4 ? lo[k] : hi[k]) >> (8 * (t & 3))) & 0xFFu);
+  }
+  const uint32_t nb = item_n(it) >> (item_lpb_log2(it) + 3u);  // buckets of 8 << lg elements
+  for (uint32_t b = lane_id(); b < nb; b += 32) scales[b] = __uint_as_float(ld_sys_u32(rec + it.meta_off + b * 8u));
+}
+// (inline: one definition across the translation units that include this header)
+inline __device__ __noinline__ void bucket_unpack_fp8(const uint8_t* rec, const WarpItem it, uint8_t* codes, float* scales) {
+  const uint32_t n = item_n(it);
+  const uint32_t ng = div_up(n, 8u);
+  if (lane_id() == 0) *scales = __uint_as_float(ld_sys_u32(rec + it.meta_off));
+  for (uint32_t g = lane_id(); g < ng; g += 32) {
+    uint32_t lo, hi;
+    load_word<8>(rec + it.pay_off, g, 8, lo, hi);
+    uint8_t* d = codes + g * 8u;
+    const uint32_t nv = min(8u, n - g * 8u);
+    if (nv == 8u && (reinterpret_cast<uintptr_t>(d) & 7u) == 0) {
+      st_v2(d, lo, hi);
+    } else {
+      for (uint32_t t = 0; t < nv; ++t) st_u8(d + t, ((t < 4 ? lo : hi) >> (8 * (t & 3))) & 0xFFu);
+    }
+  }
+}
+template <int GPL>
+__device__ __forceinline__ void fp8_unpack_item(const uint8_t* rec, const WarpItem& it, uint8_t* codes, float* scales) {
+  if (item_kind(it) == kItemFull)
+    full_unpack_fp8<GPL>(rec, it, codes, scales);
+  else
+    bucket_unpack_fp8(rec, it, codes, scales);
+}
+
 // ======================================================================================
 // FP8 in the sharded collectives (rs_kernel, ag_kernel and the generic reducers' item kernels).
 // The sender prescales, then encodes as above; the all-gather's owner writes what every receiver

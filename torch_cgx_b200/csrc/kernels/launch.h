@@ -111,6 +111,10 @@ struct A2aParams {
   uint64_t in_rows;
   uint64_t out_rows;
   int codec;                       // WireCodec (common/quant_math.h); FP8 codecs need bits 8, round to nearest
+  // nullptr: `out` receives the decoded values (T). Otherwise (FP8 codecs only) `out` receives one
+  // FP8 code byte per element and out_scales[e / bucket] the unit of the bucket starting at output
+  // element e, every chunk -- the own one included -- encoded; counts and rows hold whole buckets.
+  float* out_scales;
 };
 // defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
 // p.out_index is set
@@ -140,6 +144,10 @@ cudaError_t launch_quantize_items_f32(const ItemKernelArgs& a, const float* src_
                                       uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream);
 // dst[T] = decode(wire)
 cudaError_t launch_dequantize_items(const ItemKernelArgs& a, const uint8_t* wire, void* dst, cudaStream_t stream);
+// an FP8 plan's records undecoded (any dtype, a.codec ignored): codes[elem_off + i] = the code of
+// element i of an item, scales[elem_off / bucket + b] = the unit of its bucket b
+cudaError_t launch_unpack_items_fp8(const ItemKernelArgs& a, const uint8_t* wire, uint8_t* codes, float* scales,
+                                    uint32_t bucket, cudaStream_t stream);
 // acc_f32[elem_off - base_elem + i] = float(init_src[elem_off + i]) * prescale   (init_src != nullptr)
 // acc_f32[...] += decode(wire)                                                   (wire != nullptr)
 // (an FP8 codec adds fl(float(code) * unit), a separate rounding)

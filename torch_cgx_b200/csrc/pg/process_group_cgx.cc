@@ -482,13 +482,23 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
                                                                       WireCodec codec, int bucket_size, bool stochastic,
                                                                       int64_t seed,
                                                                       const at::Tensor& in_index,
-                                                                      const at::Tensor& out_index) {
+                                                                      const at::Tensor& out_index,
+                                                                      const at::Tensor& out_scales) {
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
   TORCH_CHECK(in.device() == out.device(), "cgx: all_to_all: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
-  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
-              "cgx: all_to_all needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(),
-              " and ", out.scalar_type());
+  const bool codes = out_scales.defined();
+  if (codes) {
+    TORCH_CHECK(codec != kMaxMin, "cgx: all_to_all: output_scales needs bits=\"e4m3\" or \"e5m2\"");
+    const at::ScalarType want = codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
+    TORCH_CHECK(dtype >= 0 && out.scalar_type() == want, "cgx: all_to_all: with output_scales the input must be ",
+                "float32, float16 or bfloat16 and the output ", want, ", got ", in.scalar_type(), " and ",
+                out.scalar_type());
+  } else {
+    TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(),
+                "cgx: all_to_all needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(),
+                " and ", out.scalar_type());
+  }
   TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: all_to_all needs contiguous tensors");
   TORCH_CHECK(in.dim() >= 1 && out.dim() >= 1, "cgx: all_to_all needs tensors with at least one dimension");
   TORCH_CHECK(in.sizes().slice(1) == out.sizes().slice(1), "cgx: all_to_all: the input rows ", in.sizes().slice(1),
@@ -507,6 +517,16 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   const bool ii = in_index.defined(), oi = out_index.defined();
   int64_t row = 1;
   for (int64_t d : in.sizes().slice(1)) row *= d;
+  if (codes) {
+    TORCH_CHECK(bucket_size <= (int)kMaxBlockElems && row % bucket_size == 0, "cgx: all_to_all: output_scales needs ",
+                "bucket_size <= ", kMaxBlockElems, " dividing the row length ", row, ", got ", bucket_size);
+    TORCH_CHECK(out_scales.is_cuda() && out_scales.device() == out.device() && out_scales.scalar_type() == at::kFloat &&
+                    out_scales.is_contiguous() && out_scales.dim() == 2 && out_scales.size(0) == out.size(0) &&
+                    out_scales.size(1) == row / bucket_size,
+                "cgx: all_to_all: output_scales must be a contiguous float32 tensor of shape [", out.size(0), ", ",
+                row / bucket_size, "] on ", out.device(), ", got ", out_scales.scalar_type(), " ", out_scales.sizes(),
+                " on ", out_scales.device());
+  }
   const std::vector<uint64_t> in_counts = a2a_counts(ii ? in_index.size(0) : in.size(0), in_splits, W, row, "input", ii);
   const std::vector<uint64_t> out_counts =
       a2a_counts(oi ? out_index.size(0) : out.size(0), out_splits, W, row, "output", oi);
@@ -520,17 +540,18 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   route.in_rows = (uint64_t)in.size(0);
   route.out_rows = (uint64_t)out.size(0);
   const bool routed = ii || oi;
+  float* scales = codes ? out_scales.data_ptr<float>() : nullptr;
   check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec, (uint32_t)bucket_size,
-                   getRank(), W, routed ? &route : nullptr);
+                   getRank(), W, routed ? &route : nullptr, scales);
   // the one place that decides where the rows are routed: inside the fused kernel when it can
   // address them, else around a plain call, which computes the same by definition
   const bool in_kernel = routed && engine_->routes_in_kernel(true, dtype, bits, (uint32_t)bucket_size, (uint64_t)row);
   return enqueue_cuda(c10d::OpType::ALLTOALL_BASE, "cgx:all_to_all", out, &in, [&](cudaStream_t s) {
-    for (const at::Tensor* t : {&in_index, &out_index})
+    for (const at::Tensor* t : {&in_index, &out_index, &out_scales})
       if (t->defined()) c10::cuda::CUDACachingAllocator::recordStream(t->storage().data_ptr(), *comm_stream_);
     if (!routed || in_kernel) {
       engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec,
-                          (uint32_t)bucket_size, rng, s, routed ? &route : nullptr);
+                          (uint32_t)bucket_size, rng, s, routed ? &route : nullptr, scales);
       return;
     }
     // the temporaries live on the comm stream only
@@ -539,9 +560,16 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     std::vector<int64_t> recv_shape = out.sizes().vec();
     recv_shape[0] = oi ? out_index.size(0) : out.size(0);
     at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;
+    at::Tensor recv_scales = codes && oi ? at::empty({recv_shape[0], out_scales.size(1)}, out_scales.options()) : out_scales;
     engine_->all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits, codec,
-                        (uint32_t)bucket_size, rng, s);
-    if (oi) out.index_copy_(0, out_index, recv);
+                        (uint32_t)bucket_size, rng, s, nullptr, codes ? recv_scales.data_ptr<float>() : nullptr);
+    if (oi && codes) {
+      // the codes move as their bytes
+      out.view(at::kByte).index_copy_(0, out_index, recv.view(at::kByte));
+      out_scales.index_copy_(0, out_index, recv_scales);
+    } else if (oi) {
+      out.index_copy_(0, out_index, recv);
+    }
   });
 }
 

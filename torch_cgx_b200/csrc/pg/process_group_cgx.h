@@ -205,12 +205,17 @@ class ProcessGroupCGX : public c10d::Backend {
   // of the received rows goes to out[out_index[j]] (undefined tensors: no index). The splits then
   // count index entries. Bitwise in.index_select -> plain call -> out.index_copy_, which is what
   // runs when AllreduceEngine::routes_in_kernel says the fused kernel cannot route the rows.
+  // Codes output: with `out_scales` defined (an FP8 codec) `out` is a float8 tensor of the codec's
+  // type that receives the codes of every row, the own chunk encoded too, and out_scales (fp32,
+  // [out rows, H / bucket_size], H % bucket_size == 0) the unit of every bucket; the routed
+  // composition then index_copy_s both.
   c10::intrusive_ptr<c10d::Work> all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                        const std::vector<int64_t>& out_splits,
                                                        const std::vector<int64_t>& in_splits, int bits,
                                                        WireCodec codec, int bucket_size, bool stochastic,
                                                        int64_t seed, const at::Tensor& in_index = at::Tensor(),
-                                                       const at::Tensor& out_index = at::Tensor());
+                                                       const at::Tensor& out_index = at::Tensor(),
+                                                       const at::Tensor& out_scales = at::Tensor());
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

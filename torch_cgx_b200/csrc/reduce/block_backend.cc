@@ -85,6 +85,14 @@ class CpuBackend : public BlockBackend {
         cpu::decode_block_store(wire + d.wire_off, dp.plan.dtype, d, dst);
     }
   }
+  void unpack_fp8(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, uint8_t* codes,
+                  float* scales, cudaStream_t) override {
+    check_fp8(dp.plan, first, count, RngKey{});
+    for (uint32_t b = first; b < first + count; ++b) {
+      const BlockDesc& d = dp.plan.blocks[b];
+      cpu::unpack_block_fp8(wire + d.wire_off, d, codes, scales);
+    }
+  }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t) override { std::memcpy(dst, src, bytes); }
 };
 
@@ -126,6 +134,13 @@ class CudaBackend : public BlockBackend {
                   cudaStream_t stream, WireCodec codec) override {
     if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
     cuda_check(launch_dequantize_items(args(dp, first, count, codec), wire, dst, stream), "dequantize_items");
+  }
+  void unpack_fp8(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, uint8_t* codes,
+                  float* scales, cudaStream_t stream) override {
+    check_fp8(dp.plan, first, count, RngKey{});
+    if (count == 0) return;
+    cuda_check(launch_unpack_items_fp8(args(dp, first, count), wire, codes, scales, dp.plan.blocks[first].bucket, stream),
+               "unpack_items_fp8");
   }
   void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) override {
     cuda_check(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, stream), "cudaMemcpyAsync");

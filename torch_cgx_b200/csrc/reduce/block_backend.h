@@ -41,6 +41,10 @@ class BlockBackend {
   // dst[T] = decode(wire)
   virtual void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                           cudaStream_t stream, WireCodec codec = kMaxMin) = 0;
+  // codes[elem_off + i] / scales[elem_off / bucket + b] = the undecoded FP8 codes and units of the
+  // records (compressed blocks of an 8-bit plan whose bucket divides every block's offset)
+  virtual void unpack_fp8(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, uint8_t* codes,
+                          float* scales, cudaStream_t stream) = 0;
   virtual void copy(void* dst, const void* src, size_t bytes, cudaStream_t stream) = 0;
 };
 

@@ -298,7 +298,7 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
 
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
-                      int rank, int world, const A2aRoute* route) {
+                      int rank, int world, const A2aRoute* route, const float* out_scales) {
   if ((int)in_counts.size() != world || (int)out_counts.size() != world)
     throw std::invalid_argument("cgx all_to_all: need one input and one output count per rank");
   if (bits < 1 || (bits > 8 && bits < kRawBits))
@@ -328,17 +328,34 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
   }
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const uintptr_t a = reinterpret_cast<uintptr_t>(in), b = reinterpret_cast<uintptr_t>(out);
-  if (nin > 0 && nout > 0 && a < b + nout * es && b < a + nin * es)
-    throw std::invalid_argument("cgx all_to_all: the output overlaps the input");
+  auto overlap = [](uintptr_t x, uint64_t nx, uintptr_t y, uint64_t ny) { return nx > 0 && ny > 0 && x < y + ny && y < x + nx; };
+  if (out_scales == nullptr) {
+    if (overlap(a, nin * es, b, nout * es)) throw std::invalid_argument("cgx all_to_all: the output overlaps the input");
+    return;
+  }
+  // codes output: one byte per output element, one fp32 unit per bucket
+  if (codec == kMaxMin) throw std::invalid_argument("cgx all_to_all: output_scales needs an FP8 format (e4m3 or e5m2)");
+  if (bucket > kMaxBlockElems)
+    throw std::invalid_argument("cgx all_to_all: output_scales needs bucket_size <= " + std::to_string(kMaxBlockElems));
+  for (int q = 0; q < world; ++q)
+    if (in_counts[q] % bucket || out_counts[q] % bucket)
+      throw std::invalid_argument("cgx all_to_all: with output_scales, every chunk must hold whole buckets");
+  if (route != nullptr && route->row % bucket)
+    throw std::invalid_argument("cgx all_to_all: with output_scales, the row length must be a multiple of bucket_size");
+  const uintptr_t s = reinterpret_cast<uintptr_t>(out_scales);
+  const uint64_t ns = nout / bucket * sizeof(float);
+  if (overlap(a, nin * es, b, nout)) throw std::invalid_argument("cgx all_to_all: the codes overlap the input");
+  if (overlap(a, nin * es, s, ns)) throw std::invalid_argument("cgx all_to_all: output_scales overlaps the input");
+  if (overlap(b, nout, s, ns)) throw std::invalid_argument("cgx all_to_all: output_scales overlaps the codes");
 }
 
 FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                          const std::vector<uint64_t>& out_counts, int dtype, int bits,
                                          WireCodec codec, uint32_t bucket, const RngParams& rng,
-                                         cudaStream_t stream, const A2aRoute* route) {
+                                         cudaStream_t stream, const A2aRoute* route, float* out_scales) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   const int W = world(), r = rank();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, route);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, route, out_scales);
   if (codec != kMaxMin && rng.stochastic)
     throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
   const uint64_t es = (uint64_t)dtype_size(dtype);
@@ -377,6 +394,7 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
   p.bits = bits >= kRawBits ? kRawBits : bits;
   p.bucket = bucket;
   p.codec = codec;
+  p.out_scales = out_scales;
   p.epoch_hint = epoch_;
   p.rng = make_rng_key(rng, r, 0);
   p.slot_bytes = heap_->layout().slot_bytes;

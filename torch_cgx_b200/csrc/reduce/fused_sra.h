@@ -81,9 +81,12 @@ struct A2aRoute {
 // rank on both sides, bits 1..8 or >= 32 (8 with an FP8 codec), a bucket >= 1, the own chunk the same size on both sides,
 // tensors below 2^32 elements and an output that does not overlap the input; with a route, counts
 // of whole rows and no overlap of the tensors the indices address; std::invalid_argument otherwise.
+// With `out_scales` (the codes output) `out` holds one byte per element and out_scales one float per
+// bucket: an FP8 codec, a bucket of at most kMaxBlockElems that divides every count (and the row),
+// and codes, scales and input pairwise disjoint.
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
-                      int rank, int world, const A2aRoute* route = nullptr);
+                      int rank, int world, const A2aRoute* route = nullptr, const float* out_scales = nullptr);
 
 class FusedSra {
  public:
@@ -161,12 +164,15 @@ class FusedSra {
   // With a `route` that has an index, the routed kernel gathers the sent rows and scatters the
   // received ones by index; that needs a2a_rows_fit(route->row, bits, bucket, dtype) (else
   // std::invalid_argument: the caller composes index_select / index_copy_ around a plain call).
+  // With `out_scales` (an FP8 codec) `out` receives the codes and out_scales the units of every chunk,
+  // undecoded, the own chunk encoded by the same encoder (A2aParams::out_scales).
   struct A2aCounts {
     uint64_t launches = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's sends
   };
   A2aCounts all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                        const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
-                       uint32_t bucket, const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr);
+                       uint32_t bucket, const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr,
+                       float* out_scales = nullptr);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

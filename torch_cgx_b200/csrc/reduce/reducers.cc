@@ -201,9 +201,13 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
 
 void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                          const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
-                         uint32_t bucket, const RngParams& rng, cudaStream_t stream) {
+                         uint32_t bucket, const RngParams& rng, cudaStream_t stream, float* out_scales) {
   const int W = comm_->size(), r = comm_->rank();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W);
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, nullptr, out_scales);
+  if (out_scales != nullptr) {
+    all_to_all_codes(in, static_cast<uint8_t*>(out), out_scales, in_counts, out_counts, dtype, codec, bucket, stream);
+    return;
+  }
   const size_t es = (size_t)dtype_size(dtype);
   const bool raw = bits >= kRawBits;
   const uint8_t* src = static_cast<const uint8_t*>(in);
@@ -252,6 +256,48 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
     if (!rw[q]) continue;
     const DevicePlan& dp = plan_for({LayerSpec{0, out_counts[q], bits, bucket}}, dtype, false, stream, 1);
     ops_->dequantize(dp, recvb + ro[q], 0, (uint32_t)dp.plan.blocks.size(), dst + oo[q], stream, codec);
+  }
+}
+
+void Reducer::all_to_all_codes(const void* in, uint8_t* codes, float* scales, const std::vector<uint64_t>& in_counts,
+                               const std::vector<uint64_t>& out_counts, int dtype, WireCodec codec, uint32_t bucket,
+                               cudaStream_t stream) {
+  const int W = comm_->size(), r = comm_->rank();
+  const size_t es = (size_t)dtype_size(dtype);
+  const uint8_t* src = static_cast<const uint8_t*>(in);
+  // every chunk has a record here, the own one included; element offsets of the outputs
+  std::vector<size_t> io(W), oo(W), sw(W), rw(W), so(W + 1, 0), ro(W + 1, 0);
+  uint64_t i = 0, o = 0;
+  for (int q = 0; q < W; ++q) {
+    io[q] = (size_t)i * es;
+    oo[q] = (size_t)o;
+    i += in_counts[q];
+    o += out_counts[q];
+    sw[q] = a2a_chunk_wire(a2a_geom((uint32_t)in_counts[q], 8, bucket, (int)es));
+    rw[q] = q == r ? 0 : a2a_chunk_wire(a2a_geom((uint32_t)out_counts[q], 8, bucket, (int)es));
+    so[q + 1] = so[q] + (sw[q] + 255) / 256 * 256;
+    ro[q + 1] = ro[q] + (rw[q] + 255) / 256 * 256;
+  }
+  uint8_t* sendb = scratch(0, so[W] + 16);
+  uint8_t* recvb = scratch(1, ro[W] + 16);
+  for (int q = 0; q < W; ++q) {
+    if (!sw[q]) continue;
+    const DevicePlan& dp = plan_for({LayerSpec{0, in_counts[q], 8, bucket}}, dtype, false, stream, 1);
+    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, RngKey{}, stream, codec);
+    if (q == r) ops_->unpack_fp8(dp, sendb + so[q], 0, (uint32_t)dp.plan.blocks.size(), codes + oo[r], scales + oo[r] / bucket, stream);
+  }
+  std::vector<P2POp> x;
+  for (int q = 0; q < W; ++q) {
+    if (q == r) continue;
+    if (sw[q]) x.push_back({true, sendb + so[q], sw[q], q});
+    if (rw[q]) x.push_back({false, recvb + ro[q], rw[q], q});
+    bytes_sent_ += sw[q];
+  }
+  comm_->exchange(x, stream);
+  for (int q = 0; q < W; ++q) {
+    if (!rw[q]) continue;
+    const DevicePlan& dp = plan_for({LayerSpec{0, out_counts[q], 8, bucket}}, dtype, false, stream, 1);
+    ops_->unpack_fp8(dp, recvb + ro[q], 0, (uint32_t)dp.plan.blocks.size(), codes + oo[q], scales + oo[q] / bucket, stream);
   }
 }
 

@@ -68,10 +68,13 @@ class Reducer {
   // arguments and checks): each chunk for a peer is quantized by the standalone item kernels through
   // a one-layer plan of the chunk, the records are exchanged and every peer's chunk is decoded into
   // its rows; the own chunk is copied, and with bits >= 32 every chunk travels as its bytes. An FP8
-  // `codec` quantizes and decodes the 8-bit records with the block backend's FP8 primitives.
+  // `codec` quantizes and decodes the 8-bit records with the block backend's FP8 primitives. With
+  // `out_scales` (an FP8 codec) the records are unpacked instead of decoded (BlockBackend::unpack_fp8)
+  // into the codes `out` and the units out_scales, and the own chunk is quantized into a record and
+  // unpacked too: bitwise the fused kernel's codes output.
   void all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
-                  const RngParams& rng, cudaStream_t stream);
+                  const RngParams& rng, cudaStream_t stream, float* out_scales = nullptr);
   uint64_t bytes_sent() const { return bytes_sent_; }
   size_t num_plans() const { return plans_.size(); }
   uint64_t plan_uploads() const { return plans_.uploads(); }
@@ -84,6 +87,9 @@ class Reducer {
   const DevicePlan& plan_for(const std::vector<LayerSpec>& layers, int dtype, bool skip_incomplete,
                              cudaStream_t stream, int world = 0);
   uint8_t* scratch(int slot, size_t bytes);  // grow-only scratch buffers of the backend's memory kind
+  void all_to_all_codes(const void* in, uint8_t* codes, float* scales, const std::vector<uint64_t>& in_counts,
+                        const std::vector<uint64_t>& out_counts, int dtype, WireCodec codec, uint32_t bucket,
+                        cudaStream_t stream);
   static size_t row_bytes(const Plan& p) { return ((size_t)p.max_chunk_wire + 255) / 256 * 256; }
   // [first element, one past last element) spanned by the blocks of a chunk / of the whole plan
   static void chunk_span(const Plan& p, int chunk, uint32_t* lo, uint32_t* hi);

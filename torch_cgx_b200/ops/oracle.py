@@ -670,15 +670,14 @@ FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2,
 _FP8_MIN_UNIT = _F32(2.0 ** -126)
 
 
-def _fp8_qdq_buckets(v: np.ndarray, fmt: str, bucket: int) -> np.ndarray:
-    """FP8 round trip of a flat fp32 array whose buckets start at index 0, in numpy fp32 arithmetic
-    and torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126),
-    code = float8(clamp(x * inv, ±FMAX)), decoded as float(code) * unit. The clamp stands for the
-    hardware's saturation: torch's casts give NaN / Inf past the largest finite value."""
+def _fp8_code_buckets(v: np.ndarray, fmt: str, bucket: int) -> Tuple[torch.Tensor, np.ndarray]:
+    """FP8 codes of a flat fp32 array whose buckets start at index 0, in numpy fp32 arithmetic and
+    torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126),
+    code = float8(clamp(x * inv, ±FMAX)). The clamp stands for the hardware's saturation: torch's
+    casts give NaN / Inf past the largest finite value. Returns the codes as a [buckets, bucket]
+    float8 tensor (the last bucket padded with its last value) and the units, fp32 [buckets]."""
     tdt, fmax = FP8_FORMATS[fmt]
     n = v.size
-    if n == 0:
-        return np.zeros(0, _F32)
     nb = -(-n // bucket)
     pad = nb * bucket - n
     vp = np.concatenate([v, np.repeat(v[-1:], pad)]) if pad else v
@@ -690,9 +689,34 @@ def _fp8_qdq_buckets(v: np.ndarray, fmt: str, bucket: int) -> np.ndarray:
         unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
         inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
         t = np.clip((b * inv).astype(_F32), _F32(-fmax), _F32(fmax))
-        code = torch.from_numpy(np.ascontiguousarray(t)).to(tdt).float().numpy()
-        dec = (code * unit).astype(_F32)
+    return torch.from_numpy(np.ascontiguousarray(t)).to(tdt), unit.reshape(-1).astype(_F32)
+
+
+def _fp8_qdq_buckets(v: np.ndarray, fmt: str, bucket: int) -> np.ndarray:
+    """FP8 round trip of a flat fp32 array whose buckets start at index 0: the codes of
+    ``_fp8_code_buckets`` decoded as float(code) * unit."""
+    n = v.size
+    if n == 0:
+        return np.zeros(0, _F32)
+    code, unit = _fp8_code_buckets(v, fmt, bucket)
+    with np.errstate(all="ignore"):
+        dec = (code.float().numpy() * unit[:, None]).astype(_F32)  # one fp32 multiply
     return dec.reshape(-1)[:n]
+
+
+def fp8_quantize(x: torch.Tensor, fmt: str, bucket_size: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """FP8 (``fmt`` "e4m3" / "e5m2") codes and per-bucket units of a flat tensor, buckets of
+    ``bucket_size`` (clamped as every bucket) from its first element: ``(codes, units)``, the codes
+    a float8 tensor of ``x.numel()`` elements, the units fp32, one per bucket. ``codes.float() *
+    units`` (bucket-wise, one fp32 multiply) is ``fp8_quantize_dequantize`` before its rounding to
+    ``x.dtype``."""
+    if fmt not in FP8_FORMATS:
+        raise ValueError(f"unknown FP8 format {fmt!r}")
+    v = x.detach().reshape(-1).float().cpu().numpy()
+    if v.size == 0:
+        return torch.empty(0, dtype=FP8_FORMATS[fmt][0]), torch.empty(0, dtype=torch.float32)
+    code, unit = _fp8_code_buckets(v, fmt, effective_bucket(bucket_size))
+    return code.reshape(-1)[:v.size].clone(), torch.from_numpy(unit)
 
 
 def fp8_quantize_dequantize(x: torch.Tensor, fmt: str, bucket_size: int) -> torch.Tensor:
@@ -732,6 +756,60 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
             parts.append(chunk)
         outs.append(torch.cat(parts) if parts else flat[r].new_empty(0))
     return outs
+
+
+def all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, fmt: str,
+                               bucket_size: int) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """Every rank's codes output of the FP8 all-to-all (``output_scales``): rank r's codes are, in
+    source order, ``fp8_quantize`` of every chunk it receives, its own chunk included, and its scales
+    the units of those chunks' buckets, concatenated (flat; every count a multiple of
+    ``bucket_size``, so the scales of a row-major ``[rows, H / bucket_size]`` matrix)."""
+    W = len(inputs)
+    flat = [t.detach().reshape(-1).cpu() for t in inputs]
+    codes, scales = [], []
+    for r in range(W):
+        cs, us = [], []
+        for q in range(W):
+            a = sum(int(c) for c in counts[q][:r])
+            c, u = fp8_quantize(flat[q][a:a + int(counts[q][r])], fmt, bucket_size)
+            cs.append(c)
+            us.append(u)
+        codes.append(torch.cat(cs))
+        scales.append(torch.cat(us))
+    return codes, scales
+
+
+def routed_all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
+                                      input_index: Sequence[torch.Tensor | None],
+                                      output_index: Sequence[torch.Tensor | None], row: int, *, fmt: str,
+                                      bucket_size: int, outputs: Sequence[torch.Tensor] | None = None,
+                                      output_scales: Sequence[torch.Tensor] | None = None
+                                      ) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """The routed codes output as the composition that defines it: ``index_select`` of the sent rows,
+    ``all_to_all_codes_reference``, then ``index_copy_`` of the received rows' codes (as bytes) and
+    scales into copies of ``outputs[r]`` / ``output_scales[r]`` (``None``: the received rows are the
+    output). Outputs are flat: codes as float8, scales fp32."""
+    W = len(inputs)
+    send = []
+    for q in range(W):
+        x = inputs[q].detach().cpu().reshape(-1, row)
+        ix = input_index[q]
+        send.append((x if ix is None else x.index_select(0, ix.cpu())).reshape(-1))
+    codes, scales = all_to_all_codes_reference(send, counts, fmt=fmt, bucket_size=bucket_size)
+    nsr = row // bucket_size
+    out_c, out_s = [], []
+    for r in range(W):
+        ix = output_index[r]
+        if ix is None:
+            out_c.append(codes[r])
+            out_s.append(scales[r])
+            continue
+        base = outputs[r].detach().cpu().reshape(-1, row).view(torch.uint8).clone()
+        base.index_copy_(0, ix.cpu(), codes[r].view(torch.uint8).reshape(-1, row))
+        out_c.append(base.reshape(-1).view(codes[r].dtype))
+        sb = output_scales[r].detach().cpu().reshape(-1, nsr).clone()
+        out_s.append(sb.index_copy_(0, ix.cpu(), scales[r].reshape(-1, nsr)).reshape(-1))
+    return out_c, out_s
 
 
 def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],

@@ -238,7 +238,8 @@ def _a2a_bits(bits: A2aBits, stochastic: bool) -> A2aBits:
 def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[Sequence[int]] = None,
                       input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8, bucket_size: int = 512,
                       group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
-                      input_index: Optional[torch.Tensor] = None, output_index: Optional[torch.Tensor] = None):
+                      input_index: Optional[torch.Tensor] = None, output_index: Optional[torch.Tensor] = None,
+                      output_scales: Optional[torch.Tensor] = None):
     """Compressed ``dist.all_to_all_single`` on a ``cgx`` group.
 
     Splits count dim-0 rows (``None``: equal splits). Rows ``input_split_sizes[q]`` of ``input`` go
@@ -268,6 +269,16 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     range is not checked on the host: the kernel skips that row and the call fails (``work.wait()``
     raises, naming the index), after which the group refuses further collectives.
 
+    FP8 codes for an FP8 expert GEMM: with ``output_scales`` (and ``bits="e4m3"`` / ``"e5m2"``)
+    ``output`` is a ``torch.float8_e4m3fn`` / ``torch.float8_e5m2`` tensor of the input's shape per
+    row that receives the wire's codes undecoded, and ``output_scales`` (CUDA float32, contiguous,
+    ``[output.shape[0], H // bucket_size]`` with ``H`` the elements of a row) the fp32 unit of every
+    bucket. ``H % bucket_size == 0`` and ``bucket_size <= 8192``, so every bucket lies inside one row;
+    ``bucket_size == H`` gives one scale per row, the row-wise scaling ``torch._scaled_mm`` takes.
+    ``codes[j, bB:(b+1)B].float() * output_scales[j, b]`` is the value the decoded call gives before
+    its rounding to the input dtype. The own chunk is encoded too, with the peers' encoder. The index
+    keywords route codes and scales rows alike. Not differentiable.
+
     As with NCCL, the splits are the caller's contract: rank q's ``input_split_sizes[r]`` must equal
     rank r's ``output_split_sizes[q]``. Malformed splits on one rank (wrong length, sum or sign, or
     rows of another size than the output's) raise ``RuntimeError`` before anything is launched.
@@ -277,16 +288,43 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     from .hooks import _native_backend
 
     bits = _a2a_bits(bits, stochastic)
+    if output_scales is not None:
+        _check_codes_output(output, input, output_scales, bits, int(bucket_size))
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
     if native is None:
         raise RuntimeError("cgx.all_to_all_single needs a process group with the cgx backend")
     work = native.all_to_all_compressed(output, input, _splits(output_split_sizes), _splits(input_split_sizes),
                                         bits, int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
-                                        input_index, output_index)
+                                        input_index, output_index, output_scales)
     if async_op:
         return work
     work.wait()  # the current stream waits for the kernel; the host does not
     return None
+
+
+def _check_codes_output(output: torch.Tensor, input: torch.Tensor, scales: torch.Tensor, bits: A2aBits,
+                        bucket_size: int) -> None:
+    """ValueError unless (output, scales) can receive the codes output of ``all_to_all_single``."""
+    from ..ops.oracle import FP8_FORMATS
+
+    if not isinstance(bits, str):
+        raise ValueError(f"cgx.all_to_all_single: output_scales needs bits='e4m3' or 'e5m2', got bits={bits}")
+    want = FP8_FORMATS[bits][0]
+    if output.dtype != want:
+        raise ValueError(f"cgx.all_to_all_single: with bits={bits!r} and output_scales the output must be {want}, "
+                         f"got {output.dtype}")
+    H = 1
+    for d in input.shape[1:]:
+        H *= int(d)
+    if bucket_size < 1 or bucket_size > 8192 or H % bucket_size != 0:
+        raise ValueError(f"cgx.all_to_all_single: output_scales needs a bucket_size <= 8192 that divides the row "
+                         f"length {H}, got {bucket_size}")
+    shape = (output.shape[0], H // bucket_size)
+    if (scales.dtype != torch.float32 or not scales.is_cuda or scales.device != output.device
+            or not scales.is_contiguous() or tuple(scales.shape) != shape):
+        raise ValueError(f"cgx.all_to_all_single: output_scales must be a contiguous float32 tensor of shape "
+                         f"{list(shape)} on {output.device}, got {scales.dtype} {list(scales.shape)} on "
+                         f"{scales.device}{'' if scales.is_contiguous() else ' (not contiguous)'}")
 
 
 def _a2a_output(input: torch.Tensor, output_split_sizes: Optional[Sequence[int]],
