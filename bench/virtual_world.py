@@ -16,6 +16,17 @@ bucket. Both move the same packed bytes; the reduce-scatter also accumulates. It
 the FP8 wire formats, e4m3 and e5m2, which move the bytes of bits 8 (the reduce-scatter row next to
 them runs at bits 8).
 
+--op ag_codes times the FP8 all-gather's codes output (e4m3, bf16, H in --hiddens, buckets of 128
+and of H, --rows rows of H per virtual rank) two ways, the arms alternating in one run:
+  (c) the decoded call, all_gather_into_tensor(out, x, bits="e4m3"), then the FP8 quantize a caller
+      writes in torch (amax, scale, cast) to the same scale layout;
+  (d) the codes call, all_gather_into_tensor(codes, x, bits="e4m3", output_scales=scales).
+Each arm's median over --iters is taken --repeats times (min, median and max reported). HBM bytes
+are computed from shapes, all virtual ranks together: every rank reads its shard (S es), writes its
+record to W - 1 peers and they read it (2 (W - 1) (S + 8 S / B)); (d) writes W S codes and W S / B
+fp32 scales; (c) writes the W S decoded values, and its quantize reads them once and writes the same
+codes and scales. The row asserts that (d) decoded, T(code * scale), equals (c)'s decoded output.
+
 --op sra --bits may name them too: every row then runs at bits 8 with that format, the allreduce's
 included. The allreduce also gets a one-shot row ("kernel": "oneshot") at --oneshot-kbs KB per
 virtual rank, the sizes the engine sends through the one-shot kernel. Every row is timed for each of
@@ -57,8 +68,13 @@ def main():
     ap.add_argument("--bucket", type=int, default=512)
     ap.add_argument("--mbs", default="8,32")
     ap.add_argument("--out", default="gpurun_out/virtual_world.json")
-    ap.add_argument("--op", default="sra", choices=["sra", "all_to_all"],
-                    help="sra: allreduce, reduce-scatter and all-gather rows; all_to_all: a2a next to rs_kernel")
+    ap.add_argument("--op", default="sra", choices=["sra", "all_to_all", "ag_codes"],
+                    help="sra: allreduce, reduce-scatter and all-gather rows; all_to_all: a2a next to rs_kernel; "
+                         "ag_codes: the all-gather's FP8 codes output against decode + torch quantize")
+    ap.add_argument("--hiddens", default="4096,7168", help="ag_codes: row lengths H")
+    ap.add_argument("--rows", type=int, default=1024, help="ag_codes: rows of H per virtual rank's shard")
+    ap.add_argument("--repeats", type=int, default=3, help="ag_codes: medians taken per arm")
+    ap.add_argument("--iters", type=int, default=10, help="ag_codes: timed calls per arm and repeat")
     ap.add_argument("--dtypes", default="float32", help="comma-separated dtypes")
     ap.add_argument("--oneshot-kbs", default="256,1024", help="one-shot allreduce sizes, KB per virtual rank")
     args = ap.parse_args()
@@ -67,8 +83,8 @@ def main():
     lanes = 264 // W
     rows = []
     sampler = ClockSampler(0).start()
-    if args.op == "all_to_all":
-        rows = all_to_all_rows(args, dev, W, lanes)
+    if args.op in ("all_to_all", "ag_codes"):
+        rows = (all_to_all_rows if args.op == "all_to_all" else ag_codes_rows)(args, dev, W, lanes)
         clocks = sampler.stop()
         Path(args.out).parent.mkdir(parents=True, exist_ok=True)
         Path(args.out).write_text(json.dumps({"clocks": clocks, "rows": rows}, indent=1))
@@ -213,6 +229,68 @@ def all_to_all_rows(args, dev, W, lanes):
                 torch.cuda.empty_cache()
                 rows.append(row)
                 print(json.dumps(row), flush=True)
+    return rows
+
+
+def ag_codes_rows(args, dev, W, lanes):
+    rows = []
+    name = torch.cuda.get_device_name(0)
+    dtype, es = torch.bfloat16, 2
+    for H in [int(h) for h in args.hiddens.split(",")]:
+        S = args.rows * H
+        g = C.LocalSraGroup(W, lanes, S + S // 8 + (1 << 20), 20000, 4096)
+        xs = [torch.randn(S, device=dev).to(dtype) for _ in range(W)]
+        for B in (128, H):
+            shard = [(0, S, 8, B)]
+            dec = [torch.empty(W * S, device=dev, dtype=dtype) for _ in range(W)]
+            codes = [torch.empty(W * S, device=dev, dtype=torch.float8_e4m3fn) for _ in range(W)]
+            scales = [torch.empty(W * S // B, device=dev) for _ in range(W)]
+            tq = [None] * W
+
+            def arm_c():
+                g.all_gather(xs, dec, shard, bits="e4m3")
+                for r in range(W):
+                    v = dec[r].view(-1, B).float()
+                    unit = v.abs().amax(dim=1, keepdim=True) * (1.0 / 448.0)
+                    inv = torch.where(unit > 0, 1.0 / unit, torch.zeros_like(unit))
+                    tq[r] = ((v * inv).clamp(-448.0, 448.0).to(torch.float8_e4m3fn), unit)
+
+            def arm_d():
+                g.all_gather(xs, codes, shard, bits="e4m3", output_scales=scales)
+
+            arms = {"c": arm_c, "d": arm_d}
+            meds = {k: [] for k in arms}
+            for _ in range(args.repeats):
+                ts = {k: [] for k in arms}
+                for it in range(3 + args.iters):
+                    for k, fn in arms.items():
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record()
+                        fn()
+                        e1.record()
+                        torch.cuda.synchronize()
+                        if it >= 3:
+                            ts[k].append(e0.elapsed_time(e1) * 1e3)
+                for k in arms:
+                    meds[k].append(sorted(ts[k])[len(ts[k]) // 2])
+            g.check()
+            for r in range(W):
+                got = (codes[r].float() * scales[r].repeat_interleave(B)).to(dtype)
+                assert torch.equal(got.view(torch.int16), dec[r].view(torch.int16)), "codes arm differs from decoded arm"
+            wire = S + S // B * 8
+            common = W * (S * es + 2 * (W - 1) * wire + W * S + W * S // B * 4)
+            row = {"op": "ag_codes", "gpu": name, "world": W, "dtype": "bfloat16", "bits": "e4m3", "H": H, "bucket": B,
+                   "rows_per_rank": args.rows, "lanes_per_rank": lanes,
+                   "hbm_c_GB": round((common + 2 * W * W * S * es) / 1e9, 3), "hbm_d_GB": round(common / 1e9, 3)}
+            for k in arms:
+                v = sorted(meds[k])
+                row[f"{k}_us"] = {"min": round(v[0], 1), "median": round(v[len(v) // 2], 1), "max": round(v[-1], 1)}
+            row["c_over_d"] = round(row["c_us"]["median"] / row["d_us"]["median"], 2)
+            rows.append(row)
+            print(json.dumps(row), flush=True)
+            del dec, codes, scales, tq
+        del g, xs
+        torch.cuda.empty_cache()
     return rows
 
 

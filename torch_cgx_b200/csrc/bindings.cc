@@ -266,15 +266,77 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
                           codec);
 }
 
+// the dtype of an all-to-all output: the inputs', or with codes (output_scales) one byte per element,
+// uint8 or the codec's float8
+bool a2a_output_dtype_ok(const at::Tensor& t, int dt, WireCodec codes_codec) {
+  if (codes_codec == kMaxMin) return cgx_dtype(t) == dt;
+  const at::ScalarType s = t.scalar_type();
+  return s == at::kByte || s == (codes_codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2);
+}
+
+// The codes output of the all-gather bindings: outputs[r] holds W * S code bytes (uint8 or the
+// codec's float8) and output_scales[r] one contiguous float32 per bucket of it, on the inputs'
+// device. ValueError for a codec or table without codes (codes_bucket). Returns the scale pointers.
+std::vector<float*> ag_scales(const std::vector<at::Tensor>& inputs, const std::vector<at::Tensor>& outputs,
+                              const std::vector<LayerSpec>& shard, WireCodec codec,
+                              const std::vector<at::Tensor>& scales) {
+  const uint64_t B = codes_bucket(ShardedOp::kAllGather, shard, codec);
+  const uint64_t W = inputs.size(), S = shard_elems(shard);
+  TORCH_CHECK(W >= 1 && outputs.size() == W && scales.size() == W,
+              "all_gather: one input, one output and one output_scales tensor per rank");
+  const int dt = cgx_dtype(inputs[0]);
+  std::vector<float*> ptrs;
+  for (size_t r = 0; r < W; ++r) {
+    const at::Tensor &i = inputs[r], &o = outputs[r], &sc = scales[r];
+    TORCH_CHECK(i.is_contiguous() && cgx_dtype(i) == dt && i.device() == inputs[0].device() && (uint64_t)i.numel() == S,
+                "all_gather: contiguous inputs of S elements, of one dtype and device");
+    TORCH_CHECK(o.is_contiguous() && o.device() == i.device() && a2a_output_dtype_ok(o, dt, codec) &&
+                    (uint64_t)o.numel() == W * S,
+                "all_gather: rank ", r, "'s codes output must be a contiguous uint8 or ",
+                codec == kE4M3 ? "float8_e4m3fn" : "float8_e5m2", " tensor of W * S elements on the inputs' device");
+    TORCH_CHECK(sc.is_contiguous() && sc.device() == i.device() && sc.scalar_type() == at::kFloat &&
+                    (uint64_t)sc.numel() * B == W * S,
+                "all_gather: rank ", r, "'s output_scales must be a contiguous float32 tensor of one element per ",
+                "bucket of its output, on the inputs' device");
+    ptrs.push_back(sc.data_ptr<float>());
+  }
+  return ptrs;
+}
+
 // All-gather oracle (ag_kernel): shard q is one quantization round trip (roundtrip_simulate) of
 // in_q placed at q * S, through copy q of the replicated table and rank q's publish stream (phase
 // 1, the SRA's requantization), so the RNG counters are the kernel's element indices. Every output
 // gets the same bytes.
+// With `output_scales` (an FP8 `bits`): the codes output, shard q's records of that round trip
+// undecoded (codes_simulate) at q * S of every output and q * S / B of every scales tensor.
 void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<at::Tensor> outputs,
                             const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed,
-                            uint32_t seq, const std::optional<A2aBitsArg>& bits) {
+                            uint32_t seq, const std::optional<A2aBitsArg>& bits,
+                            const std::optional<std::vector<at::Tensor>>& output_scales) {
   const auto shard = to_layers(shard_layers);
   const WireCodec codec = sharded_codec(bits, shard, stochastic, "all_gather");
+  if (output_scales) {
+    const std::vector<float*> scales = ag_scales(inputs, outputs, shard, codec, *output_scales);
+    TORCH_CHECK(inputs[0].device().is_cpu(), "all_gather_simulate: CPU tensors");
+    const int W = (int)inputs.size();
+    const uint64_t S = shard_elems(shard);
+    const size_t es = (size_t)dtype_size(cgx_dtype(inputs[0])), per_copy = shard.size();
+    const auto layers = replicate(shard, W, S);
+    std::vector<uint8_t> full((size_t)W * S * es);  // the shards where the plan addresses them
+    for (int q = 0; q < W; ++q) std::memcpy(full.data() + (size_t)q * S * es, inputs[q].data_ptr(), S * es);
+    uint8_t* codes0 = static_cast<uint8_t*>(outputs[0].data_ptr());
+    for (int q = 0; q < W; ++q) {
+      const std::vector<LayerSpec> copy(layers.begin() + (ptrdiff_t)(q * per_copy),
+                                        layers.begin() + (ptrdiff_t)((q + 1) * per_copy));
+      codes_simulate(build_plan(copy, make_opts(1, 1, cgx_dtype(inputs[0]), false, 1 << 30)), full.data(), codes0,
+                     scales[0], codec);
+    }
+    for (int r = 1; r < W; ++r) {
+      std::memcpy(outputs[r].data_ptr(), codes0, (size_t)W * S);
+      std::memcpy(scales[r], scales[0], (size_t)output_scales->at(0).numel() * sizeof(float));
+    }
+    return;
+  }
   const uint64_t S = check_sharded_simulate(ShardedOp::kAllGather, inputs, outputs, shard);
   const int W = (int)inputs.size();
   const int dt = cgx_dtype(inputs[0]);
@@ -307,14 +369,6 @@ std::vector<std::vector<uint64_t>> check_counts(const CountMatrix& counts, size_
     }
   }
   return out;
-}
-
-// the dtype of an all-to-all output: the inputs', or with codes (output_scales) one byte per element,
-// uint8 or the codec's float8
-bool a2a_output_dtype_ok(const at::Tensor& t, int dt, WireCodec codes_codec) {
-  if (codes_codec == kMaxMin) return cgx_dtype(t) == dt;
-  const at::ScalarType s = t.scalar_type();
-  return s == at::kByte || s == (codes_codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2);
 }
 
 // The codes output of the all-to-all bindings: `output_scales` holds one contiguous float32 tensor
@@ -631,10 +685,12 @@ class LocalSraGroup {
             bits);
   }
   // all-gather: inputs[r] holds virtual rank r's shard of S elements, outputs[r] receives W * S
+  // (output_scales: the codes output, outputs[r] then one code byte per element, ag_scales)
   void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                   const std::vector<LayerTuple>& shard_layers, bool stochastic, uint64_t seed, uint32_t seq,
-                  const std::optional<A2aBitsArg>& bits) {
-    sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq, bits);
+                  const std::optional<A2aBitsArg>& bits, const std::optional<std::vector<at::Tensor>>& output_scales) {
+    sharded(ShardedOp::kAllGather, inputs, outputs, shard_layers, false, false, stochastic, seed, seq, bits,
+            output_scales);
   }
   // all-to-all: counts[q][r] elements go from virtual rank q to r; inputs[r] holds row r of the
   // matrix in destination order, outputs[r] receives column r in source order.
@@ -741,15 +797,19 @@ class LocalSraGroup {
 
   void sharded(ShardedOp op, std::vector<at::Tensor>& inputs, std::vector<at::Tensor>& outputs,
                const std::vector<LayerTuple>& shard_layers, bool average, bool skip_incomplete, bool stochastic,
-               uint64_t seed, uint32_t seq, const std::optional<A2aBitsArg>& bits) {
+               uint64_t seed, uint32_t seq, const std::optional<A2aBitsArg>& bits,
+               const std::optional<std::vector<at::Tensor>>& output_scales = std::nullopt) {
     const bool rs = op == ShardedOp::kReduceScatter;
     const WireCodec codec = sharded_codec(bits, to_layers(shard_layers), stochastic, op_name(op));
     TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_,
                 "need one input and one output per virtual rank");
+    const std::vector<float*> scales =
+        output_scales ? ag_scales(inputs, outputs, to_layers(shard_layers), codec, *output_scales) : std::vector<float*>{};
     const int dt = cgx_dtype(inputs[0]);
     for (int r = 0; r < world_; ++r) {
       for (const at::Tensor* t : {&inputs[r], &outputs[r]})
-        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && cgx_dtype(*t) == dt, "bad tensor");
+        TORCH_CHECK(t->is_cuda() && t->is_contiguous() && ((t == &outputs[r] && output_scales) || cgx_dtype(*t) == dt),
+                    "bad tensor");
       const at::Tensor &full = rs ? inputs[r] : outputs[r], &shard = rs ? outputs[r] : inputs[r];
       TORCH_CHECK(full.numel() == shard.numel() * world_,
                   rs ? "inputs must hold W x the output elements" : "outputs must hold W x the input elements");
@@ -765,7 +825,7 @@ class LocalSraGroup {
               [&](int r) {
                 fused_[r]->sharded(op, specs, dt, skip_incomplete, inputs[r].data_ptr(), outputs[r].data_ptr(),
                                    (uint64_t)(rs ? outputs[r] : inputs[r]).numel(), ps, rng, streams_[r].stream(), 0,
-                                   nullptr, codec);
+                                   nullptr, codec, scales.empty() ? nullptr : scales[r]);
               });
   }
 
@@ -840,13 +900,19 @@ class LocalReducerGroup {
   // Reducer::all_gather: inputs[r] holds rank r's shard of S elements, outputs[r] receives W * S
   void all_gather(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs,
                   const std::vector<LayerTuple>& shard_layers, bool skip_incomplete, bool stochastic, uint64_t seed,
-                  uint32_t seq, const std::optional<A2aBitsArg>& bits) {
+                  uint32_t seq, const std::optional<A2aBitsArg>& bits,
+                  const std::optional<std::vector<at::Tensor>>& output_scales) {
     const auto specs = to_layers(shard_layers);
     const WireCodec codec = sharded_codec(bits, specs, stochastic, "all_gather");
     const RngParams rng = make_rng(stochastic, seed, seq);
-    check_outputs(inputs, outputs, false);
+    std::vector<float*> scales;
+    if (output_scales)
+      scales = ag_scales(inputs, outputs, specs, codec, *output_scales);
+    else
+      check_outputs(inputs, outputs, false);
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
-      red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s, codec);
+      red.all_gather(in, outputs[r].data_ptr(), dt, specs, skip_incomplete, rng, s, codec,
+                     scales.empty() ? nullptr : scales[r]);
     });
   }
   // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
@@ -1126,8 +1192,11 @@ class LocalEngineGroup {
   // all-gather runs without skip_incomplete, as the process group's does. `bits`, when given,
   // replaces the environment's width: an integer, or an FP8 format name (a2a_bits; the table's
   // layers then need bits 8 or 32).
+  // With output_scales (all-gather, an FP8 `bits`): the codes output (ag_scales), the table by
+  // default one 8-bit layer with the environment's bucket size.
   void sharded(bool reduce_scatter, std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, bool average,
-               const std::optional<std::vector<LayerTuple>>& shard_layers, const std::optional<A2aBitsArg>& bits) {
+               const std::optional<std::vector<LayerTuple>>& shard_layers, const std::optional<A2aBitsArg>& bits,
+               const std::optional<std::vector<at::Tensor>>& output_scales = std::nullopt) {
     const ShardedOp op = reduce_scatter ? ShardedOp::kReduceScatter : ShardedOp::kAllGather;
     TORCH_CHECK((int)outputs.size() == world_, "LocalEngineGroup: one output per virtual rank");
     CompressionEnv env = CompressionEnv::read();
@@ -1141,14 +1210,23 @@ class LocalEngineGroup {
     const bool skip = reduce_scatter && env.skip_incomplete;
     RngParams rng = make_rng(env.stochastic, env.seed, 0);
     const std::vector<LayerSpec> given = shard_layers ? to_layers(*shard_layers) : std::vector<LayerSpec>{};
+    std::vector<float*> scales;
+    if (output_scales) {
+      const int64_t S = inputs.empty() ? 0 : inputs[0].numel();
+      scales = ag_scales(inputs, outputs,
+                         shard_layers ? given : std::vector<LayerSpec>{LayerSpec{0, (uint64_t)S, 8, (uint32_t)env.bucket_size}},
+                         codec, *output_scales);
+    }
     run(inputs, [&](AllreduceEngine& e, int r, void* in, int dt, int64_t n, bool cuda, cudaStream_t s) {
-      TORCH_CHECK(outputs[r].is_contiguous() && cgx_dtype(outputs[r]) == dt &&
+      TORCH_CHECK(outputs[r].is_contiguous() && (!scales.empty() || cgx_dtype(outputs[r]) == dt) &&
                       outputs[r].device() == inputs[r].device(),
                   "LocalEngineGroup: contiguous outputs of the inputs' dtype and device");
       TORCH_CHECK(cuda || !e.fused(), "LocalEngineGroup: host tensors need a group without heaps (p2p=False)");
       const int64_t S = reduce_scatter ? outputs[r].numel() : n;
       TORCH_CHECK((reduce_scatter ? n : outputs[r].numel()) == S * world_, "LocalEngineGroup: the full buffer holds W x S");
-      const std::vector<LayerSpec> table = e.sharded_table(S, given, env.bits, env.bucket_size);
+      const std::vector<LayerSpec> table =
+          scales.empty() || shard_layers ? e.sharded_table(S, given, env.bits, env.bucket_size)
+                                         : std::vector<LayerSpec>{LayerSpec{0, (uint64_t)S, 8, (uint32_t)env.bucket_size}};
       at::Tensor staging;
       if (const int64_t sn = e.sharded_staging_numel(S)) staging = at::empty({sn}, inputs[r].options());
       // upload every window's plan and wait for it before any rank launches (see the class comment)
@@ -1158,7 +1236,7 @@ class LocalEngineGroup {
         intra_hub(r)->barrier(e.local_rank());
       }
       e.sharded(cuda, op, in, outputs[r].data_ptr(), staging.defined() ? staging.data_ptr() : nullptr, dt, S, table,
-                average, skip, rng, s, false, codec);
+                average, skip, rng, s, false, codec, scales.empty() ? nullptr : scales[r]);
       // the staging buffer is freed on the caller's stream when this returns: let its work finish first
       if (staging.defined() && cuda) cuda_check(cudaStreamSynchronize(s), "LocalEngineGroup: sharded call");
     });
@@ -1585,16 +1663,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::call_guard<py::gil_scoped_release>())
       .def("all_gather_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const A2aBitsArg& bits, int bucket_size,
-              bool stochastic, int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers) {
+              bool stochastic, int64_t seed, bool overlapped, const std::vector<LayerTuple>& layers,
+              const std::optional<at::Tensor>& out_scales) {
              const auto table = to_layers(layers);
              const A2aBits wb = a2a_bits(bits, stochastic, "all_gather");
              sharded_codec(bits, table, stochastic, "all_gather");
              return pg.sharded_compressed(ShardedOp::kAllGather, out, in, false, wb.bits, wb.codec, bucket_size, false,
-                                          stochastic, seed, overlapped, table);
+                                          stochastic, seed, overlapped, table, out_scales.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("bits") = 4, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("overlapped") = false,
-           py::arg("layers") = std::vector<LayerTuple>{}, py::call_guard<py::gil_scoped_release>())
+           py::arg("layers") = std::vector<LayerTuple>{}, py::arg("output_scales") = py::none(),
+           py::call_guard<py::gil_scoped_release>())
       .def("all_to_all_compressed",
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
               const std::vector<int64_t>& in_splits, const A2aBitsArg& bits, int bucket_size, bool stochastic,
@@ -1807,7 +1887,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("slot_bytes"), py::arg("lanes"));
   m.def("all_gather_simulate", &py_all_gather_simulate, py::arg("inputs"), py::arg("outputs"),
         py::arg("shard_layers"), py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0,
-        py::arg("bits") = py::none());
+        py::arg("bits") = py::none(), py::arg("output_scales") = py::none());
   m.def("oneshot_simulate", &py_oneshot_simulate, py::arg("tensors"), py::arg("layers"), py::arg("lanes") = 1,
         py::arg("average") = false, py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
         py::arg("seed") = 0, py::arg("seq") = 0, py::arg("min_lane_elems") = 2048, py::arg("prescale") = py::none(),
@@ -1902,7 +1982,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("shard_layers"), py::arg("average") = false, py::arg("skip_incomplete") = false,
            py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
       .def("all_gather", &LocalSraGroup::all_gather, py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers"),
-           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
+           py::arg("stochastic") = false, py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none(),
+           py::arg("output_scales") = py::none())
       .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
@@ -1932,7 +2013,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("seq") = 0, py::arg("output_scales") = py::none())
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
-           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none())
+           py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none(), py::arg("output_scales") = py::none())
       .def("bytes_sent", &LocalReducerGroup::bytes_sent)
       .def("num_plans", &LocalReducerGroup::num_plans, py::arg("rank"))
       .def("plan_uploads", &LocalReducerGroup::plan_uploads, py::arg("rank"))
@@ -1954,10 +2035,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("bits") = py::none())
       .def("all_gather",
            [](LocalEngineGroup& g, std::vector<at::Tensor> in, std::vector<at::Tensor> out,
-              std::optional<std::vector<LayerTuple>> shard_layers, std::optional<A2aBitsArg> bits) {
-             g.sharded(false, std::move(in), std::move(out), false, shard_layers, bits);
+              std::optional<std::vector<LayerTuple>> shard_layers, std::optional<A2aBitsArg> bits,
+              std::optional<std::vector<at::Tensor>> output_scales) {
+             g.sharded(false, std::move(in), std::move(out), false, shard_layers, bits, output_scales);
            },
-           py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none(), py::arg("bits") = py::none())
+           py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none(), py::arg("bits") = py::none(),
+           py::arg("output_scales") = py::none())
       .def("stats", &LocalEngineGroup::stats, py::arg("rank"))
       .def("check", &LocalEngineGroup::check)
       .def("log", &LocalEngineGroup::log, py::arg("rank"))

@@ -175,4 +175,17 @@ void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngPa
   }
 }
 
+void codes_simulate(const Plan& plan, const void* src, uint8_t* codes, float* scales, WireCodec codec) {
+  if (codec == kMaxMin) throw std::invalid_argument("codes_simulate: needs an FP8 codec");
+  std::vector<float> acc(kMaxBlockElems);
+  std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
+  for (const BlockDesc& d : plan.blocks) {
+    if (block_bits(d) != 8 || d.elem_off % d.bucket)
+      throw std::invalid_argument("codes_simulate: needs 8-bit blocks that start on a bucket boundary");
+    cpu::load_block(src, plan.dtype, d, 1.0f, acc.data());
+    cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+    cpu::unpack_block_fp8(rec.data(), d, codes, scales);
+  }
+}
+
 }  // namespace cgx

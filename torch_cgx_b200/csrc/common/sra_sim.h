@@ -71,4 +71,9 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
 void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngParams& rng, int rank, int phase,
                         WireCodec codec = kMaxMin);
 
+// The FP8 records of `plan`'s blocks (every one compressed at 8 bits, buckets dividing the block
+// offsets) of the values in `src`, left undecoded: codes[elem_off + i] = element i's code and
+// scales[elem_off / bucket + b] the unit of its bucket b (the all-gather's codes output).
+void codes_simulate(const Plan& plan, const void* src, uint8_t* codes, float* scales, WireCodec codec);
+
 }  // namespace cgx

@@ -243,7 +243,8 @@ void AllreduceEngine::prepare_sharded(ShardedOp op, const std::vector<LayerSpec>
 
 void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
                                     const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale,
-                                    const RngParams& rng, cudaStream_t stream, bool overlapped, WireCodec codec) {
+                                    const RngParams& rng, cudaStream_t stream, bool overlapped, WireCodec codec,
+                                    float* out_scales) {
   const bool rs = op == ShardedOp::kReduceScatter;
   if (fused_sharded(cuda)) {
     FusedSra::WindowHook hook;
@@ -253,7 +254,8 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
         observer_->before_fused_launch(dp, stream);
       };
     const FusedSra::RsCounts n = fused_->sharded(op, table, dtype, skip_incomplete, in, out, S, prescale, rng,
-                                                 stream, overlapped ? cfg_.overlap_lanes : 0, hook, codec);
+                                                 stream, overlapped ? cfg_.overlap_lanes : 0, hook, codec,
+                                                 out_scales);
     stats_.kernel_launches += n.launches;
     stats_.elements += n.elements;
     stats_.wire_bytes += n.wire_bytes;
@@ -266,7 +268,7 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
   if (rs)
     g.intra->reduce_scatter(in, out, dtype, table, skip_incomplete, prescale, rng, stream, codec);
   else
-    g.intra->all_gather(in, out, dtype, table, skip_incomplete, rng, stream, codec);
+    g.intra->all_gather(in, out, dtype, table, skip_incomplete, rng, stream, codec, out_scales);
   // the fused kernel's conventions: the elements of the window, the raw bytes a raw exchange would move
   const uint64_t L = (uint64_t)local_size_, es = (uint64_t)dtype_size(dtype);
   stats_.wire_bytes += g.intra->bytes_sent() - before;
@@ -287,14 +289,18 @@ void AllreduceEngine::sharded_intra(bool cuda, ShardedOp op, const void* in, voi
 void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out, void* staging, int dtype,
                               int64_t shard_numel, const std::vector<LayerSpec>& shard_layers, bool average,
                               bool skip_incomplete, const RngParams& rng_in, cudaStream_t stream, bool overlapped,
-                              WireCodec codec) {
+                              WireCodec codec, float* out_scales) {
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const int N = nodes(), L = local_size_;
   const std::string title = std::string("cgx: the compressed ") + op_title(op);
+  // every rank evaluates the same condition, so every rank refuses and none is left waiting
+  if (out_scales != nullptr && N > 1)
+    throw std::runtime_error(title + " with output_scales runs on one node only (CGX_LOCAL_SIZE " +
+                             std::to_string(L) + " < world size " + std::to_string(world_) + ")");
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
   if (shard_numel <= 0) return;
-  check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_, codec);
+  check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_, codec, out_scales);
   if (codec != kMaxMin && rng_in.stochastic)
     throw std::invalid_argument(title + ": the FP8 formats round to nearest only");
   if (!fused && (L > 1 || N == 1) && !g.intra)
@@ -344,7 +350,7 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
     NvtxRange r1("cgx:intra_node", (uint64_t)n);
     sharded_intra(cuda, op, N > 1 ? at(gathered, (size_t)n * shard_bytes) : in,
                   at(out, (size_t)n * L * shard_bytes), dtype, S, intra_table, skip_incomplete, 1.0f, rng, stream,
-                  overlapped, codec);
+                  overlapped, codec, out_scales);
   }
 }
 

@@ -150,9 +150,13 @@ class AllreduceEngine {
   // dtype for the node partials / the gathered shards. Host memory runs the generic reducers only.
   // Adds to the same counters as the allreduce. An FP8 `codec` (layers of bits 8 or 32) is the wire
   // format of every compressed stage, node-local and cross-node (FusedSra::sharded).
+  // `out_scales` selects the all-gather's codes output (check_sharded_buffers, FusedSra::sharded); it
+  // runs on one node only: with several nodes every rank throws the same std::runtime_error before
+  // anything runs.
   void sharded(bool cuda, ShardedOp op, const void* in, void* out, void* staging, int dtype, int64_t shard_numel,
                const std::vector<LayerSpec>& shard_layers, bool average, bool skip_incomplete,
-               const RngParams& rng_in, cudaStream_t stream, bool overlapped, WireCodec codec = kMaxMin);
+               const RngParams& rng_in, cudaStream_t stream, bool overlapped, WireCodec codec = kMaxMin,
+               float* out_scales = nullptr);
   // The table of one S-element shard: `layers` when given, else one layer of S elements with `bits`
   // / `bucket`, raw unless S exceeds CGX_COMPRESSION_MINIMAL_SIZE.
   std::vector<LayerSpec> sharded_table(int64_t shard_numel, std::vector<LayerSpec> layers, int bits,
@@ -192,7 +196,7 @@ class AllreduceEngine {
   // the node-local stage of a sharded call over the local ranks: fused kernel or generic reducer
   void sharded_intra(bool cuda, ShardedOp op, const void* in, void* out, int dtype, uint64_t S,
                      const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale, const RngParams& rng,
-                     cudaStream_t stream, bool overlapped, WireCodec codec);
+                     cudaStream_t stream, bool overlapped, WireCodec codec, float* out_scales = nullptr);
   bool fused_sharded(bool cuda) const { return cuda && fused_ && cfg_.inner_comm == CommType::kP2P; }
   // the node-local stage's table: raw in a multi-node all-gather, and in a multi-node
   // reduce-scatter without CGX_INTRA_COMPRESS

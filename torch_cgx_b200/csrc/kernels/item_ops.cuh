@@ -960,7 +960,7 @@ __device__ __noinline__ void bucket_recv_fp8(const uint8_t* rec, const WarpItem 
   }
 }
 
-// ---- FP8 codes handed to the caller undecoded (the all-to-all's codes output) ----------------------
+// ---- FP8 codes handed to the caller undecoded (the all-to-all's and all-gather's codes output) -----
 // Inside an item the codes of an FP8 record are in element order (full items: group g at pay_off +
 // 8g; bucket items: one bucket, byte i at pay_off + i), so element e of the item is codes[e] and the
 // unit of its bucket b is scales[b]: unpacking is a copy.
@@ -991,6 +991,33 @@ __device__ __forceinline__ void dst_st_v4(const CodesDst& ds, uint32_t off, cons
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
   for (int t = 0; t < 16; ++t) st_u8(d + t, (w[t >> 2] >> (8 * (t & 3))) & 0xFFu);
+}
+
+// The all-gather owner's codes output: every store of the FP8 encoder goes to the peers' slots and
+// to the owner's (codes, scales), so the owner keeps exactly the bytes it published.
+template <typename D>
+struct TeeDst {
+  D peers;
+  CodesDst own;
+};
+template <typename D>
+__device__ __forceinline__ TeeDst<D> unicast_of(const TeeDst<D>& ds) {
+  return TeeDst<D>{unicast_of(ds.peers), ds.own};
+}
+template <typename D>
+__device__ __forceinline__ void dst_st_v2(const TeeDst<D>& ds, uint32_t off, uint32_t a, uint32_t b) {
+  dst_st_v2(ds.peers, off, a, b);
+  dst_st_v2(ds.own, off, a, b);
+}
+template <typename D>
+__device__ __forceinline__ void dst_st_u8(const TeeDst<D>& ds, uint32_t off, uint32_t v) {
+  dst_st_u8(ds.peers, off, v);
+  dst_st_u8(ds.own, off, v);
+}
+template <typename D>
+__device__ __forceinline__ void dst_st_v4(const TeeDst<D>& ds, uint32_t off, const uint4& v) {
+  dst_st_v4(ds.peers, off, v);
+  dst_st_v4(ds.own, off, v);
 }
 
 // one item of an FP8 record -> its codes and the units of its buckets, with the loads of slice_fetch

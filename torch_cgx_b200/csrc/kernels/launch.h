@@ -57,6 +57,12 @@ struct SraParams {
   int gather;                    // with `out`: 1 = all-gather, 0 = reduce-scatter
   int codec;                     // WireCodec of the compressed items (common/quant_math.h); an FP8 codec
                                  // needs uniform_bits 8
+  // all-gather only. nullptr: `out` receives the decoded values (T). Otherwise (an FP8 codec, every
+  // item compressed) `out` receives one FP8 code byte per element and out_scales[e / out_bucket] the
+  // unit of the bucket starting at output element e, for every chunk; the own chunk holds the bytes
+  // its owner published.
+  float* out_scales;
+  uint32_t out_bucket;
 };
 
 constexpr int kSraThreads = 256;

@@ -372,7 +372,9 @@ __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems&
 // AG (the all-gather's decode): the chunks arrive in recv1 under flags1 and are decoded into p.out;
 // a timed-out wait also sets *abort_out. AG is a compile-time switch so that the allreduce's
 // instantiation is the same code as before it existed. CODEC: the all-gather's wire codec.
-template <typename T, int KB, int GPL, bool AG = false, int CODEC = kMaxMin>
+// CODES (all-gather, FP8 codec): every item is unpacked into p.out (codes) and p.out_scales instead
+// of decoded; the scale index is the item's element in the whole output over p.out_bucket.
+template <typename T, int KB, int GPL, bool AG = false, int CODEC = kMaxMin, bool CODES = false>
 __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems& li, uint32_t epoch, int stages,
                                             int* abort_out = nullptr) {
   const int lane = blockIdx.x;
@@ -428,11 +430,16 @@ __device__ __forceinline__ void sra_phase_c(const SraParams& p, const LaneItems&
       auto fetch = [&](uint32_t i, WarpItem& it, SliceWords<GPL>& w) -> bool {
         if (i >= end) return false;
         it = lane_item(li, p, i, s);
-        const bool h = item_kind(it) == kItemFull && group_aligned<T>(data + it.elem_off);
+        const bool h = !CODES && item_kind(it) == kItemFull && group_aligned<T>(data + it.elem_off);
         if (h) slice_fetch<KB, GPL>(slot, it.meta_off, it.pay_off, item_lpb_log2(it), KB ? KB : item_bits(it), w);
         return h;
       };
       auto one = [&](const WarpItem& it, const SliceWords<GPL>& w, bool hot) {
+        if constexpr (CODES) {
+          fp8_unpack_item<GPL>(slot, it, reinterpret_cast<uint8_t*>(p.out) + it.elem_off,
+                               p.out_scales + it.elem_off / p.out_bucket);
+          return;
+        }
         const uint32_t kind = item_kind(it);
         T* blk = data + it.elem_off;
         if constexpr (CODEC != kMaxMin) {
@@ -757,8 +764,11 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) rs_kernel(const __
 // of my chunk at element e reads in[e - rank * S] (p.out_shift) and writes out[e].
 // Like rs_kernel it ends with a handshake on flags2: a peer's next call can only overwrite my
 // recv1 slots after every lane of this call has decoded them (docs/MEMORY_MODEL.md).
+// CODES (an FP8 codec, p.out_scales set; every item compressed): `out` holds one code byte per
+// element and every chunk's records are handed over undecoded; the owner's encoder stores each byte
+// it publishes to its own codes and scales too (TeeDst), phase C unpacks the peers' records.
 // ===========================================================================
-template <typename T, int KB, int GPL, int CODEC = kMaxMin>
+template <typename T, int KB, int GPL, int CODEC = kMaxMin, bool CODES = false>
 __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& li, uint32_t epoch) {
   const int r = p.rank, W = p.world;
   const uint32_t warp = threadIdx.x >> 5;
@@ -776,12 +786,26 @@ __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& 
     const uint32_t kind = item_kind(it);
     const T* src = in + ((uint64_t)it.elem_off - p.out_shift);
     T* dst = out + it.elem_off;
-    const bool al = group_aligned<T>(src) && group_aligned<T>(dst);
+    const bool al = group_aligned<T>(src) && (CODES || group_aligned<T>(dst));
     float x[GPL][8];
     if (al && kind == kItemFull) slice_load_vec<T, GPL>(src, x);
     if (al && kind == kItemRaw) raw_load_vec<T, GPL>(src, x);
     if (i + kSraWarps < end)
       slice_prefetch_l2<T, GPL>(in + ((uint64_t)lane_item(li, p, i + kSraWarps, 0).elem_off - p.out_shift));
+    if constexpr (CODES) {
+      const TeeDst<MultiDst> td{ds, CodesDst{reinterpret_cast<uint8_t*>(p.out) + it.elem_off,
+                                             p.out_scales + it.elem_off / p.out_bucket, it.meta_off, it.pay_off,
+                                             item_n(it)}};
+      if (kind == kItemFull && al) {
+        slice_scale<GPL>(x, p.prescale);
+        full_send_fp8_x<CODEC, GPL>(x, it, td);
+      } else if (kind == kItemFull) {
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(src, it, p.prescale, td, (T*)nullptr);
+      } else {
+        bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, td, (T*)nullptr);
+      }
+      continue;
+    }
     if (CODEC != kMaxMin && kind == kItemFull) {
       if (al) {
         slice_scale<GPL>(x, p.prescale);
@@ -807,9 +831,10 @@ __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& 
   }
 }
 
-template <typename T, int KB, int GPL, int CODEC = kMaxMin>
+template <typename T, int KB, int GPL, int CODEC = kMaxMin, bool CODES = false>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __grid_constant__ SraParams p) {
   static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
+  static_assert(!CODES || CODEC != kMaxMin, "codes are delivered for the FP8 codecs only");
   __shared__ LaneItems li;
   __shared__ int s_abort;
   const int lane = blockIdx.x;
@@ -819,11 +844,11 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __
   lane_items_load(li, p, p.world, 1);
   trace_mark(p, lane, 0, true);
 
-  ag_publish<T, KB, GPL, CODEC>(p, li, epoch);
+  ag_publish<T, KB, GPL, CODEC, CODES>(p, li, epoch);
   __syncthreads();
   trace_mark(p, lane, 3);
   if (threadIdx.x < 32) signal_peers(p.flags1, p.world, p.rank, p.flag_stride, lane, flag);
-  sra_phase_c<T, KB, GPL, true, CODEC>(p, li, epoch, 1, &s_abort);
+  sra_phase_c<T, KB, GPL, true, CODEC, CODES>(p, li, epoch, 1, &s_abort);
   __syncthreads();
 
   // slot handshake, as in rs_kernel: every lane, whether or not it had items
@@ -846,12 +871,12 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) ag_kernel(const __
 // sra_fp8_{f32,f16,bf16}.cu.
 enum : int { kOpAllreduce = 0, kOpReduceScatter = 1, kOpAllGather = 2 };
 
-template <typename T, int KB, int GPL, int OP, int CODEC = kMaxMin>
+template <typename T, int KB, int GPL, int OP, int CODEC = kMaxMin, bool CODES = false>
 cudaError_t launch_sra_inst(const SraParams& p, cudaStream_t stream) {
   if constexpr (OP == kOpReduceScatter)
     dev::rs_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if constexpr (OP == kOpAllGather)
-    dev::ag_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    dev::ag_kernel<T, KB, GPL, CODEC, CODES><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else if (p.oneshot)
     dev::oneshot_kernel<T, KB, GPL, CODEC><<<p.lanes, kSraThreads, 0, stream>>>(p);
   else
@@ -866,11 +891,21 @@ cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
       return cudaErrorInvalidValue;
     } else {
       if (p.uniform_bits != 8) return cudaErrorInvalidValue;
+      if constexpr (OP == kOpAllGather) {
+        if (p.out_scales != nullptr) {  // the codes output
+          if (p.out_bucket == 0) return cudaErrorInvalidValue;
+          if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, OP, kE4M3, true>(p, stream);
+          if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, OP, kE5M2, true>(p, stream);
+          return cudaErrorInvalidValue;
+        }
+      }
+      if (p.out_scales != nullptr) return cudaErrorInvalidValue;
       if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, OP, kE4M3>(p, stream);
       if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, OP, kE5M2>(p, stream);
       return cudaErrorInvalidValue;
     }
   }
+  if (p.out_scales != nullptr) return cudaErrorInvalidValue;
   switch (p.uniform_bits) {
     case 2: return launch_sra_inst<T, 2, GPL, OP>(p, stream);
     case 4: return launch_sra_inst<T, 4, GPL, OP>(p, stream);

@@ -396,15 +396,27 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
                                                                    int bucket_size, bool skip_incomplete,
                                                                    bool stochastic,
                                                                    int64_t seed, bool overlapped,
-                                                                   const std::vector<LayerSpec>& layers) {
+                                                                   const std::vector<LayerSpec>& layers,
+                                                                   const at::Tensor& out_scales) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
+  const bool codes = out_scales.defined();
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: ", name, "_compressed needs CUDA tensors");
   TORCH_CHECK(in.device() == out.device(), "cgx: ", name, "_compressed: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
-  TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(), "cgx: ", name,
-              "_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(), " and ",
-              out.scalar_type());
+  if (codes) {
+    TORCH_CHECK(!rs, "cgx: output_scales is an all_gather output");
+    TORCH_CHECK(codec != kMaxMin, "cgx: all_gather: output_scales needs bits=\"e4m3\" or \"e5m2\"");
+    const at::ScalarType want = codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
+    TORCH_CHECK(dtype >= 0 && out.scalar_type() == want, "cgx: all_gather: with output_scales the input must be ",
+                "float32, float16 or bfloat16 and the output ", want, ", got ", in.scalar_type(), " and ",
+                out.scalar_type());
+    TORCH_CHECK(layers.empty(), "cgx: all_gather: output_scales takes no layer table (raw layers have no codes)");
+  } else {
+    TORCH_CHECK(dtype >= 0 && out.scalar_type() == in.scalar_type(), "cgx: ", name,
+                "_compressed needs float32, float16 or bfloat16 tensors of one dtype, got ", in.scalar_type(), " and ",
+                out.scalar_type());
+  }
   TORCH_CHECK(in.is_contiguous() && out.is_contiguous(), "cgx: ", name, "_compressed needs contiguous tensors");
   const at::Tensor& full = rs ? in : out;
   const at::Tensor& shard = rs ? out : in;
@@ -417,13 +429,35 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
-  const std::vector<LayerSpec> table = engine_->sharded_table(shard.numel(), layers, bits, bucket_size);
+  // the codes output: one 8-bit layer whatever CGX_COMPRESSION_MINIMAL_SIZE says (a raw one has no codes)
+  const std::vector<LayerSpec> table =
+      codes ? std::vector<LayerSpec>{LayerSpec{0, (uint64_t)shard.numel(), 8, (uint32_t)std::max(1, bucket_size)}}
+            : engine_->sharded_table(shard.numel(), layers, bits, bucket_size);
   if (codec != kMaxMin)
     for (const LayerSpec& l : table)
       TORCH_CHECK(l.bits == 8 || l.bits >= kRawBits, "cgx: ", name,
                   "_compressed: an FP8 format needs layers of bits 8 or 32, got ", l.bits);
+  float* scales = nullptr;
+  if (codes) {
+    const int W = getSize();
+    // every rank evaluates the same condition, so every rank refuses and none is left waiting
+    TORCH_CHECK(local_size() >= W, "cgx: the compressed all_gather with output_scales runs on one node only ",
+                "(CGX_LOCAL_SIZE ", local_size(), " < world size ", W, ")");
+    const int64_t S = in.numel();
+    TORCH_CHECK(bucket_size >= 1 && bucket_size <= (int)kMaxBlockElems && S % bucket_size == 0,
+                "cgx: all_gather: output_scales needs 1 <= bucket_size <= ", kMaxBlockElems,
+                " dividing the input's ", S, " elements, got ", bucket_size);
+    TORCH_CHECK(out_scales.is_cuda() && out_scales.device() == out.device() && out_scales.scalar_type() == at::kFloat &&
+                    out_scales.is_contiguous() && out_scales.numel() * bucket_size == out.numel(),
+                "cgx: all_gather: output_scales must be a contiguous float32 tensor of ", out.numel() / bucket_size,
+                " elements on ", out.device(), ", got ", out_scales.scalar_type(), " ", out_scales.sizes(), " on ",
+                out_scales.device());
+    scales = out_scales.data_ptr<float>();
+    check_sharded_buffers(op, table, dtype, in.data_ptr(), out.data_ptr(), (uint64_t)S, getRank(), W, codec, scales);
+  }
   return enqueue_cuda(rs ? c10d::OpType::_REDUCE_SCATTER_BASE : c10d::OpType::_ALLGATHER_BASE,
                       rs ? "cgx:reduce_scatter" : "cgx:all_gather", out, &in, [&](cudaStream_t s) {
+                        if (codes) c10::cuda::CUDACachingAllocator::recordStream(out_scales.storage().data_ptr(), *comm_stream_);
                         // several nodes: the node partials / gathered shards, N x S elements
                         at::Tensor staging;
                         if (const int64_t n = engine_->sharded_staging_numel(shard.numel())) {
@@ -433,7 +467,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
                         }
                         engine_->sharded(true, op, in.data_ptr(), out.data_ptr(),
                                          staging.defined() ? staging.data_ptr() : nullptr, dtype, shard.numel(), table,
-                                         average, skip_incomplete, rng, s, overlapped, codec);
+                                         average, skip_incomplete, rng, s, overlapped, codec, scales);
                       });
 }
 

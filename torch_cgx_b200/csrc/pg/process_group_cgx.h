@@ -191,11 +191,15 @@ class ProcessGroupCGX : public c10d::Backend {
   // `bits` / `bucket_size`. seed < 0: CGX_SEED. overlapped: at most CGX_OVERLAP_LANES CTAs (runs
   // beside compute).
   // An FP8 `codec` (bits 8, round to nearest; `layers` of bits 8 or 32) gives the 8-bit records FP8 codes.
+  // `out_scales` (all-gather, FP8 codec, no `layers`): `out` is a float8 tensor of the codec's type
+  // that receives every shard's codes undecoded and out_scales (contiguous float32, one element per
+  // bucket of `out`; bucket_size <= kMaxBlockElems dividing the shard) their units. One node only.
   c10::intrusive_ptr<c10d::Work> sharded_compressed(ShardedOp op, at::Tensor& out, at::Tensor& in, bool average,
                                                     int bits, WireCodec codec, int bucket_size, bool skip_incomplete,
                                                     bool stochastic,
                                                     int64_t seed, bool overlapped,
-                                                    const std::vector<LayerSpec>& layers);
+                                                    const std::vector<LayerSpec>& layers,
+                                                    const at::Tensor& out_scales = at::Tensor());
   // Compressed all_to_all_single: dim-0 rows of `in` go to the ranks by `in_splits`, rows of `out`
   // come from the ranks by `out_splits` (empty: equal splits). The own chunk is copied, every other
   // chunk quantized once with `bits` (1..8; 32: raw) and buckets of `bucket_size` counted from the

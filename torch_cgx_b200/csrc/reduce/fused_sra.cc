@@ -116,8 +116,28 @@ void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngPa
   launch(dp, data, prescale, rng, stream, false, nullptr, 0, false, codec);
 }
 
+uint32_t codes_bucket(ShardedOp op, const std::vector<LayerSpec>& shard_layers, WireCodec codec) {
+  if (op != ShardedOp::kAllGather)
+    throw std::invalid_argument("cgx reduce_scatter: output_scales is an all_gather output");
+  if (codec != kE4M3 && codec != kE5M2)
+    throw std::invalid_argument("cgx all_gather: output_scales needs an FP8 format (e4m3 or e5m2)");
+  const uint32_t B = shard_layers.empty() ? 1u : shard_layers[0].bucket;
+  if (B < 1 || B > kMaxBlockElems)
+    throw std::invalid_argument("cgx all_gather: output_scales needs 1 <= bucket_size <= " +
+                                std::to_string(kMaxBlockElems) + ", got " + std::to_string(B));
+  for (const LayerSpec& l : shard_layers) {
+    if (l.bits != 8)
+      throw std::invalid_argument("cgx all_gather: output_scales needs every layer at bits 8 (raw layers have no codes)");
+    if (l.bucket != B || l.numel % B)
+      throw std::invalid_argument("cgx all_gather: output_scales needs one bucket_size that divides every layer, got "
+                                  "a layer of " + std::to_string(l.numel) + " elements and bucket " +
+                                  std::to_string(l.bucket));
+  }
+  return B;
+}
+
 void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
-                           const void* out, uint64_t S, int rank, int world, WireCodec codec) {
+                           const void* out, uint64_t S, int rank, int world, WireCodec codec, const float* out_scales) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
   if (codec != kMaxMin && codec != kE4M3 && codec != kE5M2)
@@ -127,12 +147,25 @@ void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_lay
       if (l.bits != 8 && l.bits < kRawBits)
         throw std::invalid_argument(std::string("cgx ") + name + ": an FP8 format needs layers of bits 8 or 32, got " +
                                     std::to_string(l.bits));
+  const uint64_t bucket = out_scales != nullptr ? codes_bucket(op, shard_layers, codec) : 0;
   const uint64_t table = shard_elems(shard_layers);
   if (table != S)
     throw std::invalid_argument(std::string("cgx ") + name + ": the shard layers tile [0, " + std::to_string(table) +
                                 ") but the " + (rs ? "output" : "input") + " has " + std::to_string(S) + " elements");
   if (S == 0) return;
   const uint64_t es = (uint64_t)dtype_size(dtype);
+  if (out_scales != nullptr) {
+    // codes output: S * es input bytes, W * S code bytes, W * S / B fp32 units; the input cannot be
+    // a chunk of the codes (the dtypes differ)
+    const uintptr_t a = reinterpret_cast<uintptr_t>(in), b = reinterpret_cast<uintptr_t>(out),
+                    s = reinterpret_cast<uintptr_t>(out_scales);
+    const uint64_t nin = S * es, ncodes = (uint64_t)world * S, nscales = ncodes / bucket * sizeof(float);
+    auto overlap = [](uintptr_t x, uint64_t nx, uintptr_t y, uint64_t ny) { return x < y + ny && y < x + nx; };
+    if (overlap(a, nin, b, ncodes)) throw std::invalid_argument("cgx all_gather: the codes overlap the input");
+    if (overlap(a, nin, s, nscales)) throw std::invalid_argument("cgx all_gather: output_scales overlaps the input");
+    if (overlap(b, ncodes, s, nscales)) throw std::invalid_argument("cgx all_gather: output_scales overlaps the codes");
+    return;
+  }
   const uintptr_t full = reinterpret_cast<uintptr_t>(rs ? in : out);
   const uintptr_t shard = reinterpret_cast<uintptr_t>(rs ? out : in);
   const bool own_chunk = shard == full + (uint64_t)rank * S * es;
@@ -188,11 +221,12 @@ void FusedSra::prepare_sharded(const std::vector<LayerSpec>& shard_layers, int d
 FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype,
                                      bool skip_incomplete, const void* in, void* out, uint64_t S, float prescale,
                                      const RngParams& rng, cudaStream_t stream, int max_lanes,
-                                     const WindowHook& before_launch, WireCodec codec) {
+                                     const WindowHook& before_launch, WireCodec codec, float* out_scales) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
   RsCounts n;
-  check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world(), codec);
+  check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world(), codec, out_scales);
+  const uint32_t out_bucket = out_scales != nullptr ? codes_bucket(op, shard_layers, codec) : 0;
   if (codec != kMaxMin && rng.stochastic)
     throw std::invalid_argument(std::string("cgx ") + name + ": the FP8 formats round to nearest only");
   if (S == 0) return n;
@@ -202,7 +236,8 @@ FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>&
     if (dp == nullptr)
       throw std::runtime_error(std::string("cgx ") + name + ": window plan does not fit the heap slots");
     if (before_launch) before_launch(w, *dp);
-    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs, codec);
+    launch(*dp, const_cast<void*>(in), prescale, rng, stream, false, out, (uint64_t)rank() * S, !rs, codec, out_scales,
+           out_bucket);
     const Plan& pl = dp->plan;
     const uint64_t mine = pl.chunk_wire_bytes[rank()], my_elems = pl.chunk_elems[rank()];
     ++n.launches;
@@ -234,7 +269,8 @@ int FusedSra::pick_stages(const DevicePlan&) const {
 }
 
 void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
-                      bool oneshot, void* out, uint64_t out_shift, bool gather, WireCodec codec) {
+                      bool oneshot, void* out, uint64_t out_shift, bool gather, WireCodec codec, float* out_scales,
+                      uint32_t out_bucket) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   if (dp.plan.items.empty()) return;
   ++epoch_;
@@ -292,6 +328,8 @@ void FusedSra::launch(const DevicePlan& dp, void* data, float prescale, const Rn
   p.gather = gather ? 1 : 0;
   // a window of raw layers only has no compressed item: the max-min kernel moves it the same way
   p.codec = dp.plan.uniform_bits == 0 ? kMaxMin : codec;
+  p.out_scales = out_scales;
+  p.out_bucket = out_bucket;
   cuda_check(launch_sra_fused(p, stream), "launch_sra_fused");
   ++launches_;
 }

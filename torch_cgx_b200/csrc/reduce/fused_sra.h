@@ -54,8 +54,17 @@ inline std::vector<LayerSpec> replicate(const std::vector<LayerSpec>& shard, int
 // (the reduce-scatter's `out`, the all-gather's `in`) is disjoint from the full one or exactly its
 // chunk `rank` of `world`; with an FP8 `codec` every layer has bits 8 or 32 (raw);
 // std::invalid_argument otherwise.
+// With `out_scales` (the all-gather's codes output) `out` holds one byte per element and out_scales
+// one float per bucket: an FP8 codec, every layer of bits 8 with one bucket B <= kMaxBlockElems
+// dividing its size (so every bucket lies inside one shard), and input, codes and scales pairwise
+// disjoint.
 void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, const void* in,
-                           const void* out, uint64_t S, int rank, int world, WireCodec codec = kMaxMin);
+                           const void* out, uint64_t S, int rank, int world, WireCodec codec = kMaxMin,
+                           const float* out_scales = nullptr);
+// The bucket B of the all-gather's codes output: the scale of the bucket starting at output element
+// e is out_scales[e / B]. std::invalid_argument unless `op` is the all-gather, `codec` an FP8 codec
+// and the table as check_sharded_buffers requires.
+uint32_t codes_bucket(ShardedOp op, const std::vector<LayerSpec>& shard_layers, WireCodec codec);
 
 // The windows of a reduce-scatter: the shard's layer table (offsets from the shard start, tiling
 // [0, S) in order; std::invalid_argument otherwise) cut by split_for_fusion into shard-relative
@@ -138,13 +147,17 @@ class FusedSra {
   // An FP8 `codec` (common/quant_math.h; layers of bits 8 or 32, round to nearest) gives the 8-bit
   // records FP8 codes: the sender encodes prescale * x, the reduce-scatter adds each decoded value
   // fl(float(code) * unit) with its own rounding, and the all-gather's owner keeps the decoded codes.
+  // With `out_scales` (all-gather, FP8 codec; check_sharded_buffers) `out` receives the codes and
+  // out_scales the units of every shard undecoded, the own shard's being the bytes it published
+  // (SraParams::out_scales); the wire and the counts are the decoded call's.
   struct RsCounts {
     uint64_t launches = 0, elements = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's share
   };
   using WindowHook = std::function<void(const std::vector<LayerSpec>& window, const DevicePlan& dp)>;
   RsCounts sharded(ShardedOp op, const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                    const void* in, void* out, uint64_t S, float prescale, const RngParams& rng, cudaStream_t stream,
-                   int max_lanes = 0, const WindowHook& before_launch = nullptr, WireCodec codec = kMaxMin);
+                   int max_lanes = 0, const WindowHook& before_launch = nullptr, WireCodec codec = kMaxMin,
+                   float* out_scales = nullptr);
   // builds and uploads the plans of every window without launching anything
   void prepare_sharded(const std::vector<LayerSpec>& shard_layers, int dtype, bool skip_incomplete,
                        cudaStream_t stream, int max_lanes = 0);
@@ -213,7 +226,7 @@ class FusedSra {
                                  cudaStream_t stream, int plan_world, uint32_t capacity, int max_lanes);
   void launch(const DevicePlan& dp, void* data, float prescale, const RngParams& rng, cudaStream_t stream,
               bool oneshot, void* out = nullptr, uint64_t out_shift = 0, bool gather = false,
-              WireCodec codec = kMaxMin);
+              WireCodec codec = kMaxMin, float* out_scales = nullptr, uint32_t out_bucket = 0);
   std::unordered_map<uint64_t, std::vector<std::vector<LayerSpec>>> rs_windows_;
 };
 

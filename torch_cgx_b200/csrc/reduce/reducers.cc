@@ -162,9 +162,12 @@ void Reducer::reduce_scatter(const void* in, void* out, int dtype, const std::ve
 }
 
 void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                         bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec) {
+                         bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec,
+                         float* out_scales) {
   const int W = comm_->size(), r = comm_->rank();
   const uint64_t S = shard_elems(shard_layers);
+  if (out_scales != nullptr) check_sharded_buffers(ShardedOp::kAllGather, shard_layers, dtype, in, out, S, r, W, codec,
+                                                   out_scales);
   if (S == 0) return;
   if (S * (uint64_t)W >= (1ull << 32))
     throw std::invalid_argument("cgx all_gather: the output exceeds 2^32 elements");
@@ -174,14 +177,23 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   uint8_t* recvb = scratch(1, row * W);
   uint8_t* mine = scratch(2, row);
   const size_t shard_bytes = (size_t)S * dtype_size(dtype);
-  uint8_t* own = static_cast<uint8_t*>(out) + (size_t)r * shard_bytes;
-  if (in != own) ops_->copy(own, in, shard_bytes, stream);
-  // the root's part of the compressed broadcast: quantize once, keep what the peers will decode
+  uint8_t* codes = static_cast<uint8_t*>(out);
   const uint32_t cb = plan.chunk_begin(r), cn = plan.chunk_end(r) - cb;
-  codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
-    ops_->quantize(dp, out, b, n, mine, 1.0f, make_rng_key(rng, r, 1), stream, c);
-    ops_->dequantize(dp, mine, b, n, out, stream, c);
-  });
+  if (out_scales != nullptr) {
+    // the plan addresses my shard at element r * S of the output: read it from `in` through a base
+    // shifted by that much, quantize it once and hand over the record the peers receive
+    const uint8_t* base = static_cast<const uint8_t*>(in) - (size_t)r * shard_bytes;
+    ops_->quantize(dp, base, cb, cn, mine, 1.0f, make_rng_key(rng, r, 1), stream, codec);
+    ops_->unpack_fp8(dp, mine, cb, cn, codes, out_scales, stream);
+  } else {
+    uint8_t* own = static_cast<uint8_t*>(out) + (size_t)r * shard_bytes;
+    if (in != own) ops_->copy(own, in, shard_bytes, stream);
+    // the root's part of the compressed broadcast: quantize once, keep what the peers will decode
+    codec_runs(plan, cb, cn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
+      ops_->quantize(dp, out, b, n, mine, 1.0f, make_rng_key(rng, r, 1), stream, c);
+      ops_->dequantize(dp, mine, b, n, out, stream, c);
+    });
+  }
   std::vector<P2POp> x;
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
@@ -193,6 +205,10 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
   for (int p = 0; p < W; ++p) {
     if (p == r) continue;
     const uint32_t pb = plan.chunk_begin(p), pn = plan.chunk_end(p) - pb;
+    if (out_scales != nullptr) {
+      ops_->unpack_fp8(dp, recvb + row * p, pb, pn, codes, out_scales, stream);
+      continue;
+    }
     codec_runs(plan, pb, pn, codec, [&](uint32_t b, uint32_t n, WireCodec c) {
       ops_->dequantize(dp, recvb + row * p, b, n, out, stream, c);
     });

@@ -62,8 +62,13 @@ class Reducer {
   // its phase-1 stream), decodes it into its own chunk and sends the same bytes to every peer, which
   // decode them. Every rank's `out` is the same bytes, bitwise the fused ag_kernel's; raw layers
   // (bits 32) are copied unchanged. `in` may be `out`'s chunk rank(), or disjoint from it.
+  // With `out_scales` (the codes output, check_sharded_buffers) every chunk's records are unpacked
+  // instead of decoded (BlockBackend::unpack_fp8) into the codes `out` and the units out_scales, the
+  // own one from the record this rank sends: bitwise the fused ag_kernel's codes output, with the
+  // decoded call's wire.
   void all_gather(const void* in, void* out, int dtype, const std::vector<LayerSpec>& shard_layers,
-                  bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec = kMaxMin);
+                  bool skip_incomplete, const RngParams& rng, cudaStream_t stream, WireCodec codec = kMaxMin,
+                  float* out_scales = nullptr);
   // Compressed all-to-all over the communicator's W ranks, bitwise FusedSra::all_to_all (same
   // arguments and checks): each chunk for a peer is quantized by the standalone item kernels through
   // a one-layer plan of the chunk, the records are exchanged and every peer's chunk is decoded into

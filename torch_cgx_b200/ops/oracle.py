@@ -779,6 +779,15 @@ def all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[
     return codes, scales
 
 
+def all_gather_codes_reference(inputs: Sequence[torch.Tensor], fmt: str,
+                               bucket_size: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The codes output of the FP8 all-gather (``output_scales``), the same on every rank: codes
+    ``fp8_quantize`` of every rank's shard concatenated in rank order (float8, flat), and the units
+    of their buckets likewise (fp32, flat; every shard a multiple of ``bucket_size``)."""
+    parts = [fp8_quantize(t.detach().reshape(-1).cpu(), fmt, bucket_size) for t in inputs]
+    return torch.cat([c for c, _ in parts]), torch.cat([u for _, u in parts])
+
+
 def routed_all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
                                       input_index: Sequence[torch.Tensor | None],
                                       output_index: Sequence[torch.Tensor | None], row: int, *, fmt: str,

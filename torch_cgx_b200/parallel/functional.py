@@ -102,15 +102,17 @@ def all_reduce(tensor: torch.Tensor, bits: Optional[A2aBits] = None, bucket_size
 
 def _sharded(method: str, api: str, output: torch.Tensor, input: torch.Tensor, head: tuple, *, group,
              async_op: bool, stochastic: bool, seed: Optional[int],
-             layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool):
-    """``native.<method>(output, input, *head, stochastic, seed, overlapped, layers)`` on the group's cgx backend."""
+             layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool, **native_kw):
+    """``native.<method>(output, input, *head, stochastic, seed, overlapped, layers, **native_kw)`` on the
+    group's cgx backend."""
     from .hooks import _native_backend
 
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
     if native is None:
         raise RuntimeError(f"cgx.{api} needs a process group with the cgx backend")
     work = getattr(native, method)(output, input, *head, bool(stochastic), -1 if seed is None else int(seed),
-                                   bool(overlapped), [tuple(int(v) for v in l) for l in (layers or [])])
+                                   bool(overlapped), [tuple(int(v) for v in l) for l in (layers or [])],
+                                   **native_kw)
     if async_op:
         return work
     work.wait()  # the current stream waits for the kernel; the host does not
@@ -183,16 +185,22 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBi
 
 def _all_gather(output: torch.Tensor, input: torch.Tensor, *, bits: A2aBits, bucket_size: int, group,
                 async_op: bool, stochastic: bool, seed: Optional[int],
-                layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool):
+                layers: Optional[Sequence[Tuple[int, int, int, int]]], overlapped: bool,
+                output_scales: Optional[torch.Tensor] = None):
     bits = _sharded_bits(bits, stochastic, layers, "all_gather")
+    kw = {}
+    if output_scales is not None:
+        _check_ag_codes_output(output, input, output_scales, bits, int(bucket_size), layers)
+        kw["output_scales"] = output_scales
     return _sharded("all_gather_compressed", "all_gather_into_tensor", output, input, (bits, int(bucket_size)),
                     group=group, async_op=async_op, stochastic=stochastic, seed=seed, layers=layers,
-                    overlapped=overlapped)
+                    overlapped=overlapped, **kw)
 
 
 def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBits = 4, bucket_size: int = 512,
                            group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
-                           layers: Optional[Sequence[Tuple[int, int, int, int]]] = None):
+                           layers: Optional[Sequence[Tuple[int, int, int, int]]] = None,
+                           output_scales: Optional[torch.Tensor] = None):
     """Compressed ``dist.all_gather_into_tensor`` on a ``cgx`` group.
 
     ``output`` holds ``world * input.numel()`` elements; chunk q receives rank q's ``input``
@@ -214,9 +222,23 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aB
     the other nodes, which decode them; each node then shares the decoded shards among its ranks
     uncompressed. Every shard is still quantized exactly once, so with round-to-nearest every
     rank's ``output`` is the same as on one node.
+
+    FP8 codes for an FP8 GEMM on the gathered tensor: with ``output_scales`` (and ``bits="e4m3"`` /
+    ``"e5m2"``) ``output`` is a ``torch.float8_e4m3fn`` / ``torch.float8_e5m2`` tensor of ``world *
+    input.numel()`` elements that receives the wire's codes undecoded, and ``output_scales`` (CUDA
+    float32, contiguous, ``output.numel() // bucket_size`` elements, any shape) the fp32 unit of
+    every bucket: the bucket starting at element ``e`` of ``output`` has the scale
+    ``output_scales.view(-1)[e // bucket_size]``. ``input.numel() % bucket_size == 0`` and
+    ``bucket_size <= 8192``, so every bucket lies inside one shard. Each owner's chunk holds the
+    bytes it sent, and ``(codes.float() * scales.view(-1).repeat_interleave(bucket_size))``, one
+    fp32 multiply, rounded to the input dtype is the decoded call's output bit for bit. With
+    ``bucket_size`` equal to a row of ``H`` elements there is one scale per row, the row-wise scaling
+    ``torch._scaled_mm`` takes (``scale_a`` ``[M, 1]`` for gathered activations, ``scale_b`` ``[1, N]``
+    for a gathered weight ``[N, K]`` used as ``codes.view(N, K).t()``). No ``layers`` table, round to
+    nearest, one node only (several nodes raise on every rank); not differentiable.
     """
     return _all_gather(output, input, bits=bits, bucket_size=bucket_size, group=group, async_op=async_op,
-                       stochastic=stochastic, seed=seed, layers=layers, overlapped=False)
+                       stochastic=stochastic, seed=seed, layers=layers, overlapped=False, output_scales=output_scales)
 
 
 def _splits(s: Optional[Sequence[int]]) -> List[int]:
@@ -302,17 +324,42 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     return None
 
 
-def _check_codes_output(output: torch.Tensor, input: torch.Tensor, scales: torch.Tensor, bits: A2aBits,
-                        bucket_size: int) -> None:
-    """ValueError unless (output, scales) can receive the codes output of ``all_to_all_single``."""
+def _check_codes_format(api: str, output: torch.Tensor, bits: A2aBits) -> None:
+    """ValueError unless ``bits`` is an FP8 format and ``output`` a tensor of its float8 dtype (the
+    codes output of ``api``)."""
     from ..ops.oracle import FP8_FORMATS
 
     if not isinstance(bits, str):
-        raise ValueError(f"cgx.all_to_all_single: output_scales needs bits='e4m3' or 'e5m2', got bits={bits}")
+        raise ValueError(f"cgx.{api}: output_scales needs bits='e4m3' or 'e5m2', got bits={bits}")
     want = FP8_FORMATS[bits][0]
     if output.dtype != want:
-        raise ValueError(f"cgx.all_to_all_single: with bits={bits!r} and output_scales the output must be {want}, "
+        raise ValueError(f"cgx.{api}: with bits={bits!r} and output_scales the output must be {want}, "
                          f"got {output.dtype}")
+
+
+def _check_ag_codes_output(output: torch.Tensor, input: torch.Tensor, scales: torch.Tensor, bits: A2aBits,
+                           bucket_size: int, layers) -> None:
+    """ValueError unless (output, scales) can receive the codes output of ``all_gather_into_tensor``."""
+    api = "all_gather_into_tensor"
+    _check_codes_format(api, output, bits)
+    if layers:
+        raise ValueError(f"cgx.{api}: output_scales takes no layers table (one FP8 layer per shard)")
+    S = input.numel()
+    if bucket_size < 1 or bucket_size > 8192 or S % bucket_size != 0:
+        raise ValueError(f"cgx.{api}: output_scales needs a bucket_size <= 8192 that divides the input's {S} "
+                         f"elements, got {bucket_size}")
+    n = output.numel() // bucket_size
+    if (scales.dtype != torch.float32 or not scales.is_cuda or scales.device != output.device
+            or not scales.is_contiguous() or scales.numel() != n):
+        raise ValueError(f"cgx.{api}: output_scales must be a contiguous float32 tensor of {n} elements on "
+                         f"{output.device}, got {scales.dtype} {list(scales.shape)} on {scales.device}"
+                         f"{'' if scales.is_contiguous() else ' (not contiguous)'}")
+
+
+def _check_codes_output(output: torch.Tensor, input: torch.Tensor, scales: torch.Tensor, bits: A2aBits,
+                        bucket_size: int) -> None:
+    """ValueError unless (output, scales) can receive the codes output of ``all_to_all_single``."""
+    _check_codes_format("all_to_all_single", output, bits)
     H = 1
     for d in input.shape[1:]:
         H *= int(d)
