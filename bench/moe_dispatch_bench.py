@@ -18,6 +18,17 @@ With --codes, an FP8 expert GEMM's input instead (e4m3, routed dispatch, bucket 
                 caller writes in torch (amax, scale, cast) to get codes and scales for the GEMM
   dispatch (d): all_to_all(codes, x, input_index, bits="e4m3", output_scales=scales)
 
+With --combine, the weighted top-k combine that follows (fp32 gates [T, k], seeded):
+
+  combine (b)+sum: all_to_all(slots, recv, output_index), then the torch weighted sum of the README's
+                   earlier recipe, (slots.view(T, k, H) * gate.unsqueeze(-1)).sum(1) (fp32 result)
+  combine (e):     all_to_all(slots, recv, output_index, gate=gate, combine_out=out), the fused combine
+
+Arm (e)'s output is checked bit for bit against the composition it is defined as: its slots equal
+arm (b)'s, and rank 0's first 64 tokens equal the oracle's fma chain over those slots. Bytes: both
+run arm (b)'s kernel; (e) then reads the T k slot rows back and writes T rows in the dtype; the
+torch sum reads the slots, writes and reads an fp32 [T, k, H] product and writes T fp32 rows.
+
 Arms alternate in one run, CUDA events around each, medians over --iters after --warmup. The HBM
 bytes of an arm are computed from shapes, all ranks together: the kernel reads the sent rows and
 writes the received rows (2 N H es), writes and reads its wire image once (2 N H bits / 8, plus
@@ -139,6 +150,72 @@ def run_config(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bflo
     return res
 
 
+def run_combine(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
+    from torch_cgx_b200.ops import oracle as O
+
+    dev = torch.device("cuda", 0)
+    es = torch.tensor([], dtype=dtype).element_size()
+    route = routing(W, T, k, seed=T * 31 + H * 7 + k, device=dev)
+    send_rows = [route[q][2] for q in range(W)]
+    recv_n = [sum(send_rows[q][r] for q in range(W)) for r in range(W)]
+    comb_counts = [[send_rows[r][q] * H for r in range(W)] for q in range(W)]
+    g = C.LocalSraGroup(W, lanes, slot_mb << 20, 20000, 256)
+    gen = torch.Generator(device=dev).manual_seed(T + H + k)
+    recv = [torch.randn(recv_n[r], H, device=dev, generator=gen).to(dtype) for r in range(W)]
+    gate = [torch.rand(T, k, device=dev, generator=gen) for _ in range(W)]
+    slots_b = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    slots_e = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    out_e = [torch.empty(T, H, device=dev, dtype=dtype) for _ in range(W)]
+    out_b = [None] * W
+    oi = [route[q][1] for q in range(W)]
+    flat = lambda ts: [t.reshape(-1) for t in ts]  # noqa: E731
+
+    def comb_b_sum():
+        g.all_to_all(flat(recv), flat(slots_b), comb_counts, bits=bits, bucket_size=512, output_index=oi, row=H)
+        for q in range(W):
+            out_b[q] = (slots_b[q].view(T, k, H) * gate[q].unsqueeze(-1)).sum(1)
+
+    def comb_e():
+        g.all_to_all(flat(recv), flat(slots_e), comb_counts, bits=bits, bucket_size=512, output_index=oi, row=H,
+                     gate=gate, combine_out=flat(out_e))
+
+    arms = {"combine_b_sum": comb_b_sum, "combine_fused": comb_e}
+    ts = {name: [] for name in arms}
+    for it in range(warmup + iters):
+        for name, fn in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            if it >= warmup:
+                ts[name].append(e0.elapsed_time(e1) * 1000.0)
+    g.check()
+    for q in range(W):
+        assert torch.equal(slots_b[q], slots_e[q]), "the fused combine's slots differ from the routed call's"
+    n = min(T, 64)
+    want = O.combine_rows_reference(slots_b[0][:n * k].cpu(), gate[0][:n].cpu())
+    assert torch.equal(want.view(torch.int16), out_e[0][:n].cpu().view(torch.int16)), "fused combine != composition"
+
+    N = T * k * W
+    own = sum(send_rows[q][q] for q in range(W))
+    elems_wire = (N - own) * H
+    wbits = 8 if isinstance(bits, str) else bits
+    wire = elems_wire * es if wbits >= 32 else elems_wire * wbits // 8 + (elems_wire // 512) * 8
+    kernel_bytes = 2 * N * H * es + 2 * wire
+    fused_bytes = kernel_bytes + N * H * es + W * T * H * es
+    torch_bytes = kernel_bytes + N * H * es + 2 * N * H * 4 + W * T * H * 4
+    res = {"W": W, "T": T, "H": H, "topk": k, "bits": bits, "dtype": str(dtype).replace("torch.", "")}
+    for name in arms:
+        res[name + "_us"] = round(median(ts[name]), 1)
+        res[name + "_spread_us"] = [round(min(ts[name]), 1), round(max(ts[name]), 1)]
+    res["bytes_fused_GB"] = round(fused_bytes / 1e9, 3)
+    res["bytes_b_sum_GB"] = round(torch_bytes / 1e9, 3)
+    del g, recv, slots_b, slots_e, out_e, out_b
+    torch.cuda.empty_cache()
+    return res
+
+
 def run_codes(W, T, H, k, bucket, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
     """routed e4m3 dispatch: decode + torch quantize (c) against the codes output (d)"""
     dev = torch.device("cuda", 0)
@@ -223,10 +300,29 @@ def main():
     ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
     ap.add_argument("--codes", action="store_true",
                     help="time the FP8 codes output, arms (c) and (d) at bucket 128 and bucket = H, instead")
+    ap.add_argument("--combine", action="store_true",
+                    help="time the weighted top-k combine, arm (e) against arm (b) and the torch sum, instead")
     args = ap.parse_args()
     name, power = gpu_info()
     print(json.dumps({"gpu": name, "power_limit": power}), flush=True)
     rows = []
+    if args.combine:
+        for H in args.hidden:
+            for T in args.tokens:
+                for k in args.topk:
+                    need = args.world * (2 * T * k * 2 + T * (2 + 4 * k)) * H / 1e9
+                    if need > args.max_gb:
+                        print(json.dumps({"H": H, "T": T, "topk": k, "skipped": f"needs {need:.1f} GB"}), flush=True)
+                        continue
+                    for bits in args.bits:
+                        r = run_combine(args.world, T, H, k, bits, args.iters, args.warmup, args.lanes, args.slot_mb)
+                        r.update(gpu=name, power_limit=power)
+                        rows.append(r)
+                        print(json.dumps(r), flush=True)
+        if args.out:
+            Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in rows))
+        return
     if args.codes:
         for H in args.hidden:
             for T in args.tokens:

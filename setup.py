@@ -49,6 +49,7 @@ SOURCES = [
     "kernels/a2a_bf16.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
+    "kernels/combine_rows.cu",
     "kernels/residual_relu.cu",
     "kernels/batchnorm_cl.cu",
     "kernels/quant_error.cu",

@@ -30,8 +30,10 @@ from .backend import (  # noqa: E402
 from .parallel.functional import (  # noqa: E402
     all_gather_into_tensor,
     all_reduce,
+    all_to_all_combine,
     all_to_all_single,
     compression,
+    differentiable_all_to_all_combine,
     differentiable_all_to_all_single,
     reduce_scatter_tensor,
 )
@@ -68,7 +70,9 @@ __all__ = [
     "register_cgx_hook",
     "reduce_scatter_tensor",
     "all_to_all_single",
+    "all_to_all_combine",
     "differentiable_all_to_all_single",
+    "differentiable_all_to_all_combine",
     "register_layer",
     "reset_layers",
     "set_quantization_bits",

@@ -608,6 +608,43 @@ class PreparedCodec {
 };
 
 // ---- single-process multi-rank harness --------------------------------------
+// The combine arguments of the virtual-rank all-to-all bindings: gate[r] (CUDA float32 [T, k],
+// k <= 32) and combine_out[r] (T * row elements of the inputs' dtype) for every rank r that
+// combines; ValueError on malformed ones. Fills routes[r]'s combine fields (topk 0: no combine)
+// and returns the zeroed arrival masks of the fused kernel, to be kept until the call returns.
+std::vector<at::Tensor> combine_routes(std::vector<A2aRoute>& routes, const std::vector<at::Tensor>& inputs,
+                                       const IndexList& gate, const IndexList& combine_out, const A2aBits& wb,
+                                       int64_t bucket, int64_t row, bool codes) {
+  std::vector<at::Tensor> masks;
+  if (gate.empty() && combine_out.empty()) return masks;
+  TORCH_CHECK_VALUE(gate.size() == routes.size() && combine_out.size() == routes.size(),
+                    "all_to_all: one gate and one combine_out per rank");
+  TORCH_CHECK_VALUE(!codes, "cgx all_to_all: a codes output (output_scales) has no combine");
+  for (size_t r = 0; r < routes.size(); ++r) {
+    TORCH_CHECK_VALUE(gate[r].has_value() == combine_out[r].has_value(),
+                      "all_to_all: rank ", r, " needs both a gate and a combine_out, or neither");
+    if (!gate[r]) continue;
+    const at::Tensor &g = *gate[r], &o = *combine_out[r];
+    TORCH_CHECK_VALUE(g.is_cuda() && g.scalar_type() == at::kFloat && g.is_contiguous() && g.dim() == 2,
+                      "all_to_all: rank ", r, "'s gate must be a contiguous CUDA float32 tensor [T, k]");
+    const int64_t T = g.size(0), k = g.size(1);
+    TORCH_CHECK_VALUE(k >= 1 && k <= 32, "all_to_all: rank ", r, "'s gate has k = ", k, ", not in 1..32");
+    A2aRoute& rt = routes[r];
+    TORCH_CHECK_VALUE(rt.out_index != nullptr && rt.out_rows == (uint64_t)(T * k), "all_to_all: rank ", r,
+                      " combines through an output_index into T * k = ", T * k, " slots");
+    TORCH_CHECK_VALUE(o.is_cuda() && o.is_contiguous() && o.scalar_type() == inputs[r].scalar_type() &&
+                          o.numel() == T * row,
+                      "all_to_all: rank ", r, "'s combine_out must be T * row contiguous elements of the inputs' dtype");
+    rt.combine_out = o.data_ptr();
+    rt.gate = g.data_ptr<float>();
+    rt.topk = (uint32_t)k;
+    const int64_t span = a2a_row_span(wb.bits, (uint32_t)bucket, dtype_size(cgx_dtype(inputs[r])));
+    masks.push_back(at::zeros({T * (row / span)}, g.options().dtype(at::kInt)));
+    rt.masks = reinterpret_cast<uint32_t*>(masks.back().data_ptr<int32_t>());
+  }
+  return masks;
+}
+
 class LocalSraGroup {
  public:
   LocalSraGroup(int world, int lanes, int64_t slot_bytes, int64_t timeout_ms, int64_t min_lane_elems)
@@ -697,10 +734,14 @@ class LocalSraGroup {
   // Routed form (the fused kernel's, so a2a_rows_fit(row, ...) must hold): input_index[r] /
   // output_index[r], when given and not None, are rank r's int64 row indices into inputs[r] /
   // outputs[r], rows of `row` elements; the counts then describe the logical buffers of whole rows.
+  // Combine (A2aRoute::combine_out): with gate[r] (CUDA float32 [T, k]) and combine_out[r] ([T, row]
+  // elements of the inputs' dtype) outputs[r] is rank r's slots buffer of T * k rows, named by its
+  // output_index, and the kernel writes the weighted combine of the slots into combine_out[r].
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
                   const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
                   const IndexList& input_index, const IndexList& output_index, int64_t row,
-                  const std::optional<std::vector<at::Tensor>>& output_scales) {
+                  const std::optional<std::vector<at::Tensor>>& output_scales, const IndexList& gate,
+                  const IndexList& combine_out) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)world_);
     TORCH_CHECK((int)outputs.size() == world_, "all_to_all: one input and one output per rank");
@@ -734,6 +775,8 @@ class LocalSraGroup {
         }
       }
     }
+    const std::vector<at::Tensor> masks =
+        combine_routes(routes, inputs, gate, combine_out, wb, bucket, row, output_scales.has_value());
     for (int r = 0; r < world_; ++r) {
       const bool in_ix = routes[r].in_index != nullptr, out_ix = routes[r].out_index != nullptr;
       uint64_t nin = 0, nout = 0;
@@ -916,20 +959,53 @@ class LocalReducerGroup {
     });
   }
   // Reducer::all_to_all: counts[q][r] elements go from rank q to r (as LocalSraGroup.all_to_all)
+  // Combine, the composed path of the process group (CUDA only): with gate[r], combine_out[r] and
+  // output_index[r] (as LocalSraGroup.all_to_all) the received rows land in a scratch buffer, are
+  // index_copy_'d into the slots outputs[r] by output_index[r], and combine_rows_kernel writes
+  // combine_out[r] from the slots.
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
                   const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
-                  const std::optional<std::vector<at::Tensor>>& output_scales) {
+                  const std::optional<std::vector<at::Tensor>>& output_scales, const IndexList& output_index,
+                  int64_t row, const IndexList& gate, const IndexList& combine_out) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)hub_.world());
     const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
     check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda(), output_scales ? wb.codec : kMaxMin);
     const RngParams rng = make_rng(stochastic, seed, seq);
+    const bool combine = !gate.empty() || !combine_out.empty();
+    std::vector<A2aRoute> routes((size_t)hub_.world());
+    std::vector<at::Tensor> recv;
+    if (combine) {
+      TORCH_CHECK_VALUE(inputs[0].is_cuda(), "all_to_all: the combine runs on CUDA tensors");
+      TORCH_CHECK_VALUE(row >= 1 && output_index.size() == routes.size(), "all_to_all: the combine needs row >= 1 ",
+                        "and one output_index per rank");
+      for (size_t r = 0; r < routes.size(); ++r) {
+        const std::optional<at::Tensor>& ix = output_index[r];
+        TORCH_CHECK_VALUE(ix && ix->is_cuda() && ix->scalar_type() == at::kLong && ix->dim() == 1 &&
+                              ix->is_contiguous() && ix->numel() * row == outputs[r].numel(),
+                          "all_to_all: rank ", r, "'s output_index must be a contiguous CUDA int64 vector of one ",
+                          "entry per row of its output");
+        routes[r].out_index = ix->data_ptr<int64_t>();
+        routes[r].row = (uint64_t)row;
+        routes[r].out_rows = (uint64_t)ix->numel();
+        recv.push_back(at::empty_like(outputs[r]));
+      }
+      combine_routes(routes, inputs, gate, combine_out, wb, bucket, row, output_scales.has_value());
+    }
     run(inputs, [&](Reducer& red, int r, void* in, int dt, cudaStream_t s) {
       std::vector<uint64_t> out_counts(counts.size());
       for (size_t q = 0; q < counts.size(); ++q) out_counts[q] = counts[q][r];
-      red.all_to_all(in, outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits, wb.codec, (uint32_t)bucket, rng,
-                     s, scales.empty() ? nullptr : scales[r]);
+      red.all_to_all(in, combine ? recv[r].data_ptr() : outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits,
+                     wb.codec, (uint32_t)bucket, rng, s, scales.empty() ? nullptr : scales[r]);
     }, false);
+    for (size_t r = 0; combine && r < routes.size(); ++r) {
+      outputs[r].view({-1, row}).index_copy_(0, *output_index[r], recv[r].view({-1, row}));
+      if (routes[r].topk == 0) continue;
+      cuda_check(launch_combine_rows(outputs[r].data_ptr(), routes[r].gate, routes[r].combine_out,
+                                     cgx_dtype(inputs[r]), routes[r].out_rows / routes[r].topk, routes[r].topk,
+                                     (uint32_t)row, c10::cuda::getCurrentCUDAStream().stream()),
+                 "launch_combine_rows");
+    }
   }
   // bytes each rank's reducer counted as sent during the last call
   std::vector<int64_t> bytes_sent() const { return last_sent_; }
@@ -1679,17 +1755,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            [](ProcessGroupCGX& pg, at::Tensor out, at::Tensor in, const std::vector<int64_t>& out_splits,
               const std::vector<int64_t>& in_splits, const A2aBitsArg& bits, int bucket_size, bool stochastic,
               int64_t seed, const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index,
-              const std::optional<at::Tensor>& out_scales) {
+              const std::optional<at::Tensor>& out_scales, const std::optional<at::Tensor>& gate,
+              const std::optional<at::Tensor>& combine_out) {
              const A2aBits wb = a2a_bits(bits, stochastic);
              return pg.all_to_all_compressed(out, in, out_splits, in_splits, wb.bits, wb.codec, bucket_size,
                                              stochastic, seed, in_index.value_or(at::Tensor()),
-                                             out_index.value_or(at::Tensor()), out_scales.value_or(at::Tensor()));
+                                             out_index.value_or(at::Tensor()), out_scales.value_or(at::Tensor()),
+                                             gate.value_or(at::Tensor()), combine_out.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
            py::arg("input_split_sizes") = std::vector<int64_t>{}, py::arg("bits") = 8, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("input_index") = py::none(),
            py::arg("output_index") = py::none(), py::arg("output_scales") = py::none(),
-           py::call_guard<py::gil_scoped_release>())
+           py::arg("gate") = py::none(), py::arg("combine_out") = py::none(), py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -1987,7 +2065,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("all_to_all", &LocalSraGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
-           py::arg("row") = 1, py::arg("output_scales") = py::none())
+           py::arg("row") = 1, py::arg("output_scales") = py::none(), py::arg("gate") = IndexList{},
+           py::arg("combine_out") = IndexList{})
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))
@@ -2010,7 +2089,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("bits") = py::none())
       .def("all_to_all", &LocalReducerGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
-           py::arg("seq") = 0, py::arg("output_scales") = py::none())
+           py::arg("seq") = 0, py::arg("output_scales") = py::none(), py::arg("output_index") = IndexList{},
+           py::arg("row") = 1, py::arg("gate") = IndexList{}, py::arg("combine_out") = IndexList{})
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none(), py::arg("output_scales") = py::none())

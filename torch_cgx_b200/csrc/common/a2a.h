@@ -113,22 +113,22 @@ CGX_HD WarpItem a2a_block_item(const A2aGeom& g, uint32_t b, uint32_t j) {
 }
 
 // ---- routed rows --------------------------------------------------------------------------------
-// True iff every item a2a_block_item can produce for a chunk of whole rows of H elements lies
-// inside one row, so that the routed kernel can address an item as one span of one indexed row.
-// Items start at multiples of their span within a block, blocks at multiples of every span, and a
-// chunk of rows ends on a row boundary; so this holds iff H is a multiple of the span: 512 raw
-// elements, the slice for power-of-two buckets up to the slice (a chunk of whole slices has no
-// bucket tail), otherwise the clamped bucket. The element size does not enter.
-CGX_HD bool a2a_rows_fit(uint32_t H, int bits, uint32_t bucket, int elsize) {
+// The span of a routed item: every item a2a_block_item can produce for a chunk of whole rows of a
+// multiple of this many elements lies inside one row and covers exactly this many elements. Items
+// start at multiples of their span within a block, blocks at multiples of every span, and a chunk
+// of rows ends on a row boundary; the span is 512 raw elements, the slice for power-of-two buckets
+// up to the slice (a chunk of whole slices has no bucket tail), otherwise the clamped bucket. The
+// element size does not enter.
+CGX_HD uint32_t a2a_row_span(int bits, uint32_t bucket, int elsize) {
   const A2aGeom g = a2a_geom(0, bits, bucket, elsize);
-  uint32_t span;
-  if (g.bits >= kRawBits)
-    span = kRawItemElems;
-  else if (g.bucket >= 8u && (g.bucket & (g.bucket - 1u)) == 0u && g.bucket <= g.slice)
-    span = g.slice;
-  else
-    span = g.bucket;
-  return H >= 1u && H % span == 0u;
+  if (g.bits >= kRawBits) return kRawItemElems;
+  if (g.bucket >= 8u && (g.bucket & (g.bucket - 1u)) == 0u && g.bucket <= g.slice) return g.slice;
+  return g.bucket;
+}
+// True iff the routed kernel can address every item of a chunk of whole rows of H elements as one
+// span of one indexed row: H is a multiple of the span.
+CGX_HD bool a2a_rows_fit(uint32_t H, int bits, uint32_t bucket, int elsize) {
+  return H >= 1u && H % a2a_row_span(bits, bucket, elsize) == 0u;
 }
 
 // ---- windows ----------------------------------------------------------------------------------

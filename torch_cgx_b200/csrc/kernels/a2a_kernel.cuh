@@ -21,6 +21,7 @@
 // slots (docs/MEMORY_MODEL.md).
 #pragma once
 #include "../common/a2a.h"
+#include "combine.cuh"
 #include "sra_kernels.cuh"
 
 namespace cgx {
@@ -104,8 +105,39 @@ __device__ __forceinline__ T* a2a_row_addr(const A2aParams& p, T* base, const in
   return base + (uint64_t)i * p.row + (e - row * p.row);
 }
 
-// my own chunk, routed: one warp per row, through both indices
+// Combine: the warp has stored slot row s, columns [col, col + p.span) (docs/MEMORY_MODEL.md). Lane
+// 0 sets bit s % topk of the segment's mask with acquire-release semantics; __syncwarp orders the
+// lanes' stores before it and its acquire before their loads. A bit already set is a repeated slot
+// (recorded; the segment then never fills). The warp that fills the mask writes the segment.
+__device__ __forceinline__ uint32_t atom_or_acq_rel_gpu(uint32_t* p, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.gpu.global.or.b32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+  return old;
+}
 template <typename T>
+__device__ __forceinline__ void a2a_combine_arrive(const A2aParams& p, const T* dst) {
+  const T* slots = reinterpret_cast<const T*>(p.out);
+  const uint64_t e = (uint64_t)(dst - slots), H = p.row;
+  const uint64_t s = e / H, t = s / p.topk;
+  const uint32_t c = (uint32_t)(s - t * p.topk), seg = (uint32_t)(e - s * H) / p.span;
+  __syncwarp();
+  uint32_t old = 0;
+  if (lane_id() == 0) old = atom_or_acq_rel_gpu(p.masks + t * (H / p.span) + seg, 1u << c);
+  old = __shfl_sync(kAll, old, 0);
+  if (old & (1u << c)) {
+    if (lane_id() == 0) *p.status = (uint32_t)kSraBadIndex | ((uint32_t)p.rank << 8) | (2u << 16);
+    return;
+  }
+  const uint32_t full = p.topk == 32u ? ~0u : (1u << p.topk) - 1u;
+  if ((old | (1u << c)) != full) return;
+  const uint64_t col = (uint64_t)seg * p.span;
+  combine_segment<T>(slots + t * p.topk * H + col, H, p.gate + t * p.topk, p.topk,
+                     reinterpret_cast<T*>(p.combine_out) + t * H + col, p.span);
+}
+
+// my own chunk, routed: one warp per row, through both indices (COMBINE: then arrives at every
+// segment of the slot row)
+template <typename T, bool COMBINE>
 __device__ __forceinline__ void a2a_copy_own_rows(const A2aParams& p) {
   const uint32_t H = p.row, rows = p.in_cnt[p.rank] / H;
   const uint32_t nwarps = gridDim.x * kSraWarps;
@@ -121,6 +153,8 @@ __device__ __forceinline__ void a2a_copy_own_rows(const A2aParams& p) {
       done = vecs * 16u / (uint32_t)sizeof(T);
     }
     for (uint32_t i = done + lane_id(); i < H; i += 32) dst[i] = src[i];
+    if constexpr (COMBINE)
+      for (uint32_t col = 0; col < H; col += p.span) a2a_combine_arrive<T>(p, dst + col);
   }
 }
 
@@ -277,7 +311,7 @@ __device__ __forceinline__ void a2a_encode_own(const A2aParams& p) {
   }
 }
 
-template <typename T, int KB, int GPL, bool IDX, int CODEC, bool CODES>
+template <typename T, int KB, int GPL, bool IDX, int CODEC, bool CODES, bool COMBINE>
 __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k) {
   const int r = p.rank;
   const A2aGeom g = a2a_geom(p.out_cnt[q], p.bits, p.bucket, (int)sizeof(T));
@@ -301,8 +335,10 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
     } else {
       dst = chunk + it.elem_off;
     }
+    // COMBINE: the item is one span of one slot row (a2a_rows_fit)
     if constexpr (CODEC != kMaxMin) {
       a2a_recv_item_fp8<T, CODEC, GPL>(ss.base, it, dst);
+      if constexpr (COMBINE) a2a_combine_arrive<T>(p, dst);
       continue;
     }
     const uint32_t kind = item_kind(it);
@@ -319,6 +355,7 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
     } else {
       raw_ag_recv<T>(ss, it, dst);
     }
+    if constexpr (COMBINE) a2a_combine_arrive<T>(p, dst);
   }
 }
 
@@ -327,10 +364,13 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
 // CODEC: the wire codec of the peers' chunks (quant_math.h); the FP8 ones exist with KB 8 only.
 // CODES (FP8 codecs only, A2aParams::out_scales set): the output receives the codes and units of
 // every chunk undecoded, the own chunk encoded like a peer's.
-template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin, bool CODES = false>
+// COMBINE (routed, decoded output; A2aParams::combine_out set): the weighted top-k combine of the
+// slots, finalized per segment by the last warp to store into it.
+template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin, bool CODES = false, bool COMBINE = false>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const __grid_constant__ A2aParams p) {
   static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   static_assert(!CODES || CODEC != kMaxMin, "codes are delivered for the FP8 codecs only");
+  static_assert(!COMBINE || (IDX && !CODES), "the combine needs the routed, decoded output");
   __shared__ int s_abort;
   __shared__ uint32_t s_send[kMaxPeers], s_recv[kMaxPeers];  // this lane's windows per destination / source
   const int lane = blockIdx.x, r = p.rank, W = p.world;
@@ -375,7 +415,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if (s_abort) break;
     for (int s = 1; s < W; ++s) {
       const int q = (r + W - s) % W;
-      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX, CODEC, CODES>(p, q, bpw, k);
+      if (s_recv[q] > k) a2a_recv_window<T, KB, GPL, IDX, CODEC, CODES, COMBINE>(p, q, bpw, k);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_recv)
@@ -387,7 +427,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if constexpr (CODES)
       a2a_encode_own<T, GPL, IDX, CODEC>(p);
     else if constexpr (IDX)
-      a2a_copy_own_rows<T>(p);
+      a2a_copy_own_rows<T, COMBINE>(p);
     else
       a2a_copy_own<T>(p);
   }
@@ -408,8 +448,33 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 
 }  // namespace dev
 
+// the combine instantiations: routed, decoded output, every codec and KB
+template <typename T, int GPL>
+cudaError_t launch_a2a_combine(const A2aParams& p, cudaStream_t stream) {
+  if (p.out_scales != nullptr || (p.codec != kMaxMin && p.bits != 8)) return cudaErrorInvalidValue;
+  if (p.codec == kE4M3) {
+    dev::a2a_kernel<T, 8, GPL, true, kE4M3, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    return cudaGetLastError();
+  }
+  if (p.codec == kE5M2) {
+    dev::a2a_kernel<T, 8, GPL, true, kE5M2, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    return cudaGetLastError();
+  }
+  if (p.codec != kMaxMin) return cudaErrorInvalidValue;
+  switch ((p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0) {
+    case 2: dev::a2a_kernel<T, 2, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 4: dev::a2a_kernel<T, 4, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 8: dev::a2a_kernel<T, 8, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    default: dev::a2a_kernel<T, 0, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+  }
+  return cudaGetLastError();
+}
+
 template <typename T, int GPL, bool IDX>
 cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
+  if constexpr (IDX) {
+    if (p.combine_out != nullptr) return launch_a2a_combine<T, GPL>(p, stream);
+  }
   if (p.codec != kMaxMin) {
     if (p.bits != 8) return cudaErrorInvalidValue;
     const bool codes = p.out_scales != nullptr;

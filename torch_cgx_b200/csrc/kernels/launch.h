@@ -68,8 +68,9 @@ struct SraParams {
 constexpr int kSraThreads = 256;
 constexpr int kSraWarps = kSraThreads / 32;
 constexpr int kSraCtasPerSm = 2;
-// kSraBadIndex: the routed all-to-all met an index naming a row outside its tensor; the status word
-// then holds (rank << 8) | (0 input_index, 1 output_index) << 16 instead of the peer and the lane
+// kSraBadIndex: the routed all-to-all met an index naming a row outside its tensor, or (the combine)
+// an output_index naming one slot twice; the status word then holds (rank << 8) | which << 16
+// instead of the peer and the lane, which = 0 input_index, 1 output_index, 2 a repeated slot
 enum SraStatus : uint32_t { kSraOk = 0, kSraTimeoutPhase1 = 1, kSraTimeoutPhase2 = 2, kSraAborted = 3, kSraBadIndex = 4 };
 
 // max CTAs of the fused kernel that can be co-resident on the current device
@@ -121,6 +122,16 @@ struct A2aParams {
   // FP8 code byte per element and out_scales[e / bucket] the unit of the bucket starting at output
   // element e, every chunk -- the own one included -- encoded; counts and rows hold whole buckets.
   float* out_scales;
+  // Weighted top-k combine (routed, decoded output only; nullptr: none). `out` holds the slots:
+  // row s = t * topk + c is choice c of token t. Once every slot row of token t has landed in the
+  // columns [seg * span, (seg + 1) * span), the last warp to arrive writes those columns of
+  // combine_out[t] = T(fma chain of gate[t, c] * slot row c, c = 0 .. topk - 1) (combine_segment).
+  // masks[t * (row / span) + seg] collects the arrived choices, one bit each; zero before the launch.
+  void* combine_out;               // T*: [out_rows / topk, row]
+  const float* gate;               // [out_rows / topk, topk]
+  uint32_t* masks;
+  uint32_t topk;                   // 1..32
+  uint32_t span;                   // a2a_row_span(bits, bucket, dtype)
 };
 // defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
 // p.out_index is set
@@ -160,6 +171,12 @@ cudaError_t launch_unpack_items_fp8(const ItemKernelArgs& a, const uint8_t* wire
 cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* wire, float* acc_f32,
                                         uint32_t base_elem, const void* init_src, float prescale,
                                         cudaStream_t stream);
+
+// ---- weighted top-k combine of slot rows (combine_rows_kernel, the combine's composed path) ----
+// out[t, h] = T(acc) with acc = g_0 * x_0, then acc = fma(g_c, x_c, acc) for c = 1 .. k - 1, where
+// x_c = float(slots[t * k + c, h]) and g_c = gate[t, c]; slots [T * k, H], gate [T, k] fp32, out [T, H]
+cudaError_t launch_combine_rows(const void* slots, const float* gate, void* out, int dtype, uint64_t T, uint32_t k,
+                                uint32_t H, cudaStream_t stream);
 
 // ---- elementwise helpers (K4/K7 of the reference) ---------------------------
 cudaError_t launch_scale_inplace(void* data, int dtype, uint64_t n, float scale, cudaStream_t stream);

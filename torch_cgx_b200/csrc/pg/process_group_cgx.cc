@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstring>
 
+#include "../common/a2a.h"
 #include "../kernels/launch.h"
 #include "c10d_communicator.h"
 
@@ -517,7 +518,9 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
                                                                       int64_t seed,
                                                                       const at::Tensor& in_index,
                                                                       const at::Tensor& out_index,
-                                                                      const at::Tensor& out_scales) {
+                                                                      const at::Tensor& out_scales,
+                                                                      const at::Tensor& gate,
+                                                                      const at::Tensor& combine_out) {
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
   TORCH_CHECK(in.device() == out.device(), "cgx: all_to_all: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
@@ -551,6 +554,29 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   const bool ii = in_index.defined(), oi = out_index.defined();
   int64_t row = 1;
   for (int64_t d : in.sizes().slice(1)) row *= d;
+  const bool combine = combine_out.defined();
+  int64_t topk = 0;
+  if (combine) {
+    // the checks of cgx.all_to_all_combine, repeated for callers of the binding
+    TORCH_CHECK_VALUE(!codes, "cgx: all_to_all_combine: a codes output (output_scales) has no combine");
+    TORCH_CHECK_VALUE(oi, "cgx: all_to_all_combine needs an output_index");
+    TORCH_CHECK_VALUE(gate.defined() && gate.scalar_type() == at::kFloat && gate.is_cuda() &&
+                          gate.device() == out.device() && gate.is_contiguous() && gate.dim() == 2,
+                      "cgx: all_to_all_combine: the gate must be a contiguous CUDA float32 tensor [T, k] on ",
+                      out.device());
+    topk = gate.size(1);
+    TORCH_CHECK_VALUE(topk >= 1 && topk <= 32, "cgx: all_to_all_combine: k = ", topk, " is not in 1..32");
+    const int64_t T = gate.size(0);
+    TORCH_CHECK_VALUE(out_index.size(0) == T * topk && out.size(0) == T * topk,
+                      "cgx: all_to_all_combine: output_index and the slots need T * k = ", T * topk,
+                      " entries and rows, got ", out_index.size(0), " and ", out.size(0));
+    TORCH_CHECK_VALUE(combine_out.scalar_type() == in.scalar_type() && combine_out.is_cuda() &&
+                          combine_out.device() == out.device() && combine_out.is_contiguous() &&
+                          combine_out.dim() >= 1 && combine_out.size(0) == T &&
+                          combine_out.sizes().slice(1) == in.sizes().slice(1),
+                      "cgx: all_to_all_combine: the output must be a contiguous ", in.scalar_type(), " tensor of ", T,
+                      " rows like the input's on ", out.device());
+  }
   if (codes) {
     TORCH_CHECK(bucket_size <= (int)kMaxBlockElems && row % bucket_size == 0, "cgx: all_to_all: output_scales needs ",
                 "bucket_size <= ", kMaxBlockElems, " dividing the row length ", row, ", got ", bucket_size);
@@ -573,6 +599,11 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   route.row = (uint64_t)row;
   route.in_rows = (uint64_t)in.size(0);
   route.out_rows = (uint64_t)out.size(0);
+  if (combine) {
+    route.combine_out = combine_out.data_ptr();
+    route.gate = gate.data_ptr<float>();
+    route.topk = (uint32_t)topk;
+  }
   const bool routed = ii || oi;
   float* scales = codes ? out_scales.data_ptr<float>() : nullptr;
   check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec, (uint32_t)bucket_size,
@@ -581,8 +612,17 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   // address them, else around a plain call, which computes the same by definition
   const bool in_kernel = routed && engine_->routes_in_kernel(true, dtype, bits, (uint32_t)bucket_size, (uint64_t)row);
   return enqueue_cuda(c10d::OpType::ALLTOALL_BASE, "cgx:all_to_all", out, &in, [&](cudaStream_t s) {
-    for (const at::Tensor* t : {&in_index, &out_index, &out_scales})
+    for (const at::Tensor* t : {&in_index, &out_index, &out_scales, &gate, &combine_out})
       if (t->defined()) c10::cuda::CUDACachingAllocator::recordStream(t->storage().data_ptr(), *comm_stream_);
+    at::Tensor masks;
+    if (combine && in_kernel) {
+      // the arrival masks, zeroed on the comm stream inside the call, so a captured graph zeroes
+      // them on every replay
+      c10::cuda::CUDAStreamGuard sg(*comm_stream_);
+      const int64_t segs = row / (int64_t)a2a_row_span(bits, (uint32_t)bucket_size, (int)dtype_size(dtype));
+      masks = at::zeros({gate.size(0) * segs}, in.options().dtype(at::kInt));
+      route.masks = reinterpret_cast<uint32_t*>(masks.data_ptr<int32_t>());
+    }
     if (!routed || in_kernel) {
       engine_->all_to_all(true, in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec,
                           (uint32_t)bucket_size, rng, s, routed ? &route : nullptr, scales);
@@ -604,6 +644,11 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     } else if (oi) {
       out.index_copy_(0, out_index, recv);
     }
+    // the combine of the slots now in `out`, by the same arithmetic as the fused kernel's
+    if (combine)
+      cuda_check(launch_combine_rows(out.data_ptr(), gate.data_ptr<float>(), combine_out.data_ptr(), dtype,
+                                     (uint64_t)gate.size(0), (uint32_t)topk, (uint32_t)row, s),
+                 "launch_combine_rows");
   });
 }
 

@@ -213,13 +213,20 @@ class ProcessGroupCGX : public c10d::Backend {
   // type that receives the codes of every row, the own chunk encoded too, and out_scales (fp32,
   // [out rows, H / bucket_size], H % bucket_size == 0) the unit of every bucket; the routed
   // composition then index_copy_s both.
+  // Weighted top-k combine (DESIGN §2.13d): with `combine_out` ([T, ...] like the input's rows) and
+  // `gate` (CUDA float32 [T, k], k <= 32) `out` is the slots buffer of T * k rows, filled through
+  // `out_index` exactly as the routed call fills it, and combine_out[t] = T(fma chain over the slots
+  // t * k + c with the gates, c = 0 .. k - 1): inside the fused kernel when routes_in_kernel, else
+  // combine_rows_kernel after the composition. Malformed combine arguments raise ValueError.
   c10::intrusive_ptr<c10d::Work> all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                        const std::vector<int64_t>& out_splits,
                                                        const std::vector<int64_t>& in_splits, int bits,
                                                        WireCodec codec, int bucket_size, bool stochastic,
                                                        int64_t seed, const at::Tensor& in_index = at::Tensor(),
                                                        const at::Tensor& out_index = at::Tensor(),
-                                                       const at::Tensor& out_scales = at::Tensor());
+                                                       const at::Tensor& out_scales = at::Tensor(),
+                                                       const at::Tensor& gate = at::Tensor(),
+                                                       const at::Tensor& combine_out = at::Tensor());
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

@@ -367,6 +367,23 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const uintptr_t a = reinterpret_cast<uintptr_t>(in), b = reinterpret_cast<uintptr_t>(out);
   auto overlap = [](uintptr_t x, uint64_t nx, uintptr_t y, uint64_t ny) { return nx > 0 && ny > 0 && x < y + ny && y < x + nx; };
+  if (route != nullptr && route->combine_out != nullptr) {
+    const uint64_t k = route->topk;
+    if (k < 1 || k > 32) throw std::invalid_argument("cgx all_to_all_combine: top-k must be 1..32");
+    if (route->out_index == nullptr) throw std::invalid_argument("cgx all_to_all_combine: needs an output_index");
+    if (out_scales != nullptr) throw std::invalid_argument("cgx all_to_all_combine: a codes output (output_scales) has no combine");
+    uint64_t entries = 0;
+    for (int q = 0; q < world; ++q) entries += out_counts[q] / route->row;
+    if (route->out_rows % k || entries != route->out_rows)
+      throw std::invalid_argument("cgx all_to_all_combine: output_index must have one entry per slot, T * k = " +
+                                  std::to_string(route->out_rows) + " with k = " + std::to_string(k) + ", got " +
+                                  std::to_string(entries));
+    const uintptr_t c = reinterpret_cast<uintptr_t>(route->combine_out), g = reinterpret_cast<uintptr_t>(route->gate);
+    const uint64_t nc = route->out_rows / k * route->row * es, ng = route->out_rows * sizeof(float);
+    if (overlap(a, nin * es, c, nc)) throw std::invalid_argument("cgx all_to_all_combine: the output overlaps the input");
+    if (overlap(a, nin * es, g, ng)) throw std::invalid_argument("cgx all_to_all_combine: the gate overlaps the input");
+    if (overlap(b, nout * es, c, nc)) throw std::invalid_argument("cgx all_to_all_combine: the output overlaps the slots");
+  }
   if (out_scales == nullptr) {
     if (overlap(a, nin * es, b, nout * es)) throw std::invalid_argument("cgx all_to_all: the output overlaps the input");
     return;
@@ -398,6 +415,8 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
     throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
+  if (routed && route->combine_out != nullptr && route->masks == nullptr)
+    throw std::invalid_argument("cgx all_to_all_combine: the fused combine needs its arrival masks");
   if (routed && !a2a_rows_fit((uint32_t)route->row, bits, bucket, (int)es))
     throw std::invalid_argument("cgx all_to_all: rows of " + std::to_string(route->row) +
                                 " elements do not hold whole quantization items at this bucket size");
@@ -454,6 +473,13 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
     p.row = (uint32_t)route->row;
     p.in_rows = route->in_rows;
     p.out_rows = route->out_rows;
+    if (route->combine_out != nullptr) {
+      p.combine_out = route->combine_out;
+      p.gate = route->gate;
+      p.masks = route->masks;
+      p.topk = route->topk;
+      p.span = a2a_row_span(bits, bucket, (int)es);
+    }
   }
   last_lanes_ = G;
   cudaError_t e = cudaErrorInvalidValue;
@@ -473,6 +499,10 @@ std::string FusedSra::status_message() const {
   const uint32_t s = heap_->status_host();
   if (s == 0) return std::string();
   const uint32_t code = s & 0xFF, peer = (s >> 8) & 0xFF, lane = s >> 16;
+  if (code == kSraBadIndex && lane == 2)
+    return "cgx: all_to_all on rank " + std::to_string(peer) +
+           ": output_index repeats a slot (the combine of its token was skipped; the group refuses further "
+           "collectives)";
   if (code == kSraBadIndex)
     return "cgx: all_to_all on rank " + std::to_string(peer) + ": " + (lane ? "output_index" : "input_index") +
            " holds a row outside the " + (lane ? "output" : "input") +

@@ -79,11 +79,20 @@ std::vector<std::vector<LayerSpec>> reduce_scatter_windows(const std::vector<Lay
 // of the logical receive buffer is written to row out_index[j] of `out` (out_rows rows). A nullptr
 // index means that side is the logical buffer itself. The index values live on the device and are
 // checked by the kernel (kSraBadIndex), not here.
+// Weighted top-k combine (DESIGN §2.13d; combine_out != nullptr, with out_index): `out` is the slots
+// buffer of out_rows = T * topk rows, slot t * topk + c is choice c of token t, and combine_out
+// ([T, row], the input's dtype) receives T(acc), acc = gate[t, 0] * slot 0, then
+// fma(gate[t, c], slot c, acc) for c = 1 .. topk - 1. `masks` is zeroed scratch of
+// T * (row / a2a_row_span) words for the fused kernel's arrivals.
 struct A2aRoute {
   const int64_t* in_index = nullptr;
   const int64_t* out_index = nullptr;
   uint64_t row = 1;
   uint64_t in_rows = 0, out_rows = 0;
+  void* combine_out = nullptr;
+  const float* gate = nullptr;  // [T, topk] fp32
+  uint32_t topk = 0;            // 1..32
+  uint32_t* masks = nullptr;
 };
 
 // The arguments of one rank's all-to-all (FusedSra::all_to_all, Reducer::all_to_all): a count per
@@ -92,7 +101,9 @@ struct A2aRoute {
 // of whole rows and no overlap of the tensors the indices address; std::invalid_argument otherwise.
 // With `out_scales` (the codes output) `out` holds one byte per element and out_scales one float per
 // bucket: an FP8 codec, a bucket of at most kMaxBlockElems that divides every count (and the row),
-// and codes, scales and input pairwise disjoint.
+// and codes, scales and input pairwise disjoint. A combine (route->combine_out) needs an out_index
+// whose entries are the out_rows = T * topk slots, topk in 1..32, no codes output, and neither
+// combine_out nor the gate overlapping the input, or combine_out the slots.
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
                       int rank, int world, const A2aRoute* route = nullptr, const float* out_scales = nullptr);

@@ -848,6 +848,36 @@ def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence
     return outs
 
 
+def combine_rows_reference(slots: torch.Tensor, gate: torch.Tensor) -> torch.Tensor:
+    """The weighted top-k combine of slot rows: ``slots`` ``[T*k, H]`` (any float dtype), ``gate``
+    ``[T, k]`` fp32. For every ``t, h``, with ``x_c = float(slots[t*k + c, h])`` and ``g_c = gate[t, c]``:
+    ``acc = fp32(g_0 * x_0)``, then ``acc = fma(g_c, x_c, acc)`` for ``c = 1 .. k-1`` in that order,
+    rounded once each (``_fma32_np``); the result is ``acc`` rounded to nearest in the slots' dtype."""
+    T, k = gate.shape
+    x = slots.detach().cpu().float().reshape(T, k, -1).numpy()
+    g = gate.detach().cpu().float().numpy()
+    with np.errstate(all="ignore"):
+        acc = (g[:, 0, None].astype(np.float64) * x[:, 0].astype(np.float64)).astype(_F32)
+    for c in range(1, k):
+        acc = _fma32_np(g[:, c, None], x[:, c], acc)
+    return torch.from_numpy(np.ascontiguousarray(acc, dtype=_F32)).to(slots.dtype)
+
+
+def routed_all_to_all_combine_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
+                                        output_index: Sequence[torch.Tensor], gates: Sequence[torch.Tensor],
+                                        row: int, *, bits: int | str,
+                                        bucket_size: int) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """Every rank's weighted top-k combine as the composition that defines it: ``routed_all_to_all_reference``
+    into slots (rank r's ``output_index[r]`` a permutation of ``[0, T_r * k_r)``), then
+    ``combine_rows_reference`` with ``gates[r]`` (``[T_r, k_r]``). Returns (slots, outputs), flat."""
+    W = len(inputs)
+    bases = [inputs[r].new_zeros(output_index[r].numel() * row) for r in range(W)]
+    slots = routed_all_to_all_reference(inputs, counts, [None] * W, output_index, row, bits=bits,
+                                        bucket_size=bucket_size, outputs=bases)
+    outs = [combine_rows_reference(slots[r].reshape(-1, row), gates[r]).reshape(-1) for r in range(W)]
+    return slots, outs
+
+
 # ---- the sharded collectives over several nodes (AllreduceEngine::sharded, DESIGN §2.9b) -----------
 SHARDED_PERTURBATIONS = ("prescale_local", "requantized_gather", "quantized_own_partial", "transposed_ranks")
 _CROSS_SEQ = 0x40000000  # the allreduce's cross-node marker

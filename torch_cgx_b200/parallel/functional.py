@@ -450,3 +450,148 @@ def differentiable_all_to_all_single(input: torch.Tensor, output_split_sizes: Op
     return _AllToAll.apply(input, None if output_split_sizes is None else _splits(output_split_sizes),
                            None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
                            int(bucket_size), group, bool(stochastic), input_index, output_index, output_rows)
+
+
+def _overlaps(a: torch.Tensor, b: torch.Tensor) -> bool:
+    """whether the bytes of two dense tensors overlap (same device)"""
+    if a.device != b.device or a.numel() == 0 or b.numel() == 0:
+        return False
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
+
+
+def _check_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Tensor, output_index: torch.Tensor,
+                   slots: Optional[torch.Tensor]) -> None:
+    """ValueError unless the arguments of ``all_to_all_combine`` are well formed. The checks that need
+    no GPU come first, the device checks last."""
+    api = "cgx.all_to_all_combine"
+    if output.dtype != input.dtype:
+        raise ValueError(f"{api}: the output must have the input's dtype {input.dtype}, got {output.dtype} "
+                         "(a codes output has no combine)")
+    if gate.dtype != torch.float32 or gate.dim() != 2 or not gate.is_contiguous():
+        raise ValueError(f"{api}: the gate must be a contiguous float32 tensor [T, k], got {gate.dtype} "
+                         f"{list(gate.shape)}{'' if gate.is_contiguous() else ' (not contiguous)'}")
+    T, k = int(gate.shape[0]), int(gate.shape[1])
+    if not 1 <= k <= 32:
+        raise ValueError(f"{api}: k = {k} choices per token, at most 32 are supported")
+    rows = tuple(input.shape[1:])
+    if tuple(output.shape) != (T,) + rows or not output.is_contiguous():
+        raise ValueError(f"{api}: the output must be a contiguous tensor of shape {[T, *rows]}, got "
+                         f"{list(output.shape)}")
+    if output_index.dtype != torch.int64 or output_index.dim() != 1 or output_index.numel() != T * k:
+        raise ValueError(f"{api}: output_index must be an int64 vector of T * k = {T * k} entries, got "
+                         f"{output_index.dtype} {list(output_index.shape)}")
+    if slots is not None and (slots.dtype != input.dtype or tuple(slots.shape) != (T * k,) + rows
+                              or not slots.is_contiguous()):
+        raise ValueError(f"{api}: slots must be a contiguous {input.dtype} tensor of shape {[T * k, *rows]}, got "
+                         f"{slots.dtype} {list(slots.shape)}")
+    for name, t in (("the output", output), ("slots", slots), ("the gate", gate)):
+        if t is not None and _overlaps(t, input):
+            raise ValueError(f"{api}: {name} overlaps the input")
+    if slots is not None and _overlaps(slots, output):
+        raise ValueError(f"{api}: slots overlap the output")
+    for name, t in (("input", input), ("output", output), ("gate", gate), ("output_index", output_index),
+                    ("slots", slots)):
+        if t is not None and (not t.is_cuda or t.device != input.device):
+            raise ValueError(f"{api}: {name} must be on the input's CUDA device, got {t.device}")
+
+
+def all_to_all_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Tensor, output_index: torch.Tensor,
+                       output_split_sizes: Optional[Sequence[int]] = None,
+                       input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8, bucket_size: int = 512,
+                       group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
+                       slots: Optional[torch.Tensor] = None):
+    """The routed compressed all-to-all of an MoE combine followed by the weighted top-k sum, in one call.
+
+    ``gate`` is a contiguous CUDA float32 ``[T, k]`` (``1 <= k <= 32``), ``output`` ``[T, ...]`` in the
+    input's dtype and row shape, ``output_index`` a CUDA int64 permutation of ``[0, T*k)`` with
+    ``sum(output_split_sizes)`` entries. Slot ``s = t*k + c`` is choice ``c`` of token ``t``.
+    The call is defined as the composition
+      1. ``slots = all_to_all_single(slots, input, ..., output_index=output_index)`` (any ``bits``,
+         stochastic rounding included, the own chunk copied bit for bit), into a ``[T*k, ...]`` buffer;
+      2. for every ``t`` and element ``h``, with ``x_c = float(slots[t*k + c, h])`` and
+         ``g_c = gate[t, c]``: ``acc = fp32(g_0 * x_0)``, then ``acc = fma(g_c, x_c, acc)`` for
+         ``c = 1 .. k-1`` in that order, and ``output[t, h] = acc`` rounded to nearest in the dtype.
+    NaN and signed zeros follow from that arithmetic. With ``slots`` given, it receives exactly the
+    routed call's rows; otherwise the buffer is scratch.
+
+    On the P2P transport, when every quantization item lies inside one row, the sum happens inside
+    the all-to-all kernel: the last warp to store a token's slot segment sums it, so the slots are
+    read back while they are likely still in L2, with no extra launch. Elsewhere (NCCL transport,
+    rows the kernel cannot route, world 1 without a heap) the routed composition runs, then one
+    standalone combine kernel with the same arithmetic; both give the same bits.
+
+    Raises ``ValueError`` before anything runs for a gate of the wrong dtype, device, layout or
+    shape, ``k > 32``, an index length other than ``T*k``, an output, slots or gate that overlap the
+    input, and a float8 output (a codes output has no combine). A repeated slot, like an index out
+    of range, is found by the kernel: the call fails (``work.wait()`` raises, naming
+    ``output_index``) and the group refuses further collectives. Dropped tokens (an index that is
+    not a permutation) are not supported: call ``all_to_all_single`` and sum the rows yourself.
+    """
+    from .hooks import _native_backend
+
+    bits = _a2a_bits(bits, stochastic)
+    _check_combine(output, input, gate, output_index, slots)
+    if slots is None:
+        slots = input.new_empty((gate.shape[0] * gate.shape[1],) + tuple(input.shape[1:]))
+    native = _native_backend(group if group is not None else dist.group.WORLD, input)
+    if native is None:
+        raise RuntimeError("cgx.all_to_all_combine needs a process group with the cgx backend")
+    work = native.all_to_all_compressed(slots, input, _splits(output_split_sizes), _splits(input_split_sizes),
+                                        bits, int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
+                                        None, output_index, None, gate, output)
+    if async_op:
+        return work
+    work.wait()
+    return None
+
+
+class _AllToAllCombine(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, input, gate, output_index, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size,
+                group, stochastic):
+        input, gate = input.contiguous(), gate.contiguous()
+        T, k = gate.shape
+        slots = input.new_empty((T * k,) + tuple(input.shape[1:]))
+        out = input.new_empty((T,) + tuple(input.shape[1:]))
+        all_to_all_combine(out, input, gate, output_index, output_split_sizes, input_split_sizes, bits=bits,
+                           bucket_size=bucket_size, group=group, stochastic=stochastic, slots=slots)
+        ctx.save_for_backward(gate, slots, output_index)
+        ctx.splits = (output_split_sizes, input_split_sizes)
+        ctx.grad_bits, ctx.bucket_size, ctx.group, ctx.stochastic = grad_bits, bucket_size, group, stochastic
+        ctx.in_shape = input.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        gate, slots, output_index = ctx.saved_tensors
+        out_splits, in_splits = ctx.splits
+        T, k = gate.shape
+        grad = grad.contiguous()
+        g2 = grad.reshape(T, 1, -1)
+        grad_slots = (g2 * gate.unsqueeze(-1)).to(grad.dtype).reshape((T * k,) + tuple(grad.shape[1:]))
+        gin = grad.new_empty(ctx.in_shape)
+        all_to_all_single(gin, grad_slots, in_splits, out_splits, bits=ctx.grad_bits, bucket_size=ctx.bucket_size,
+                          group=ctx.group, stochastic=ctx.stochastic, input_index=output_index)
+        grad_gate = (g2.float() * slots.reshape(T, k, -1).float()).sum(-1)
+        return gin, grad_gate, None, None, None, None, None, None, None, None
+
+
+def differentiable_all_to_all_combine(input: torch.Tensor, gate: torch.Tensor, output_index: torch.Tensor,
+                                      output_split_sizes: Optional[Sequence[int]] = None,
+                                      input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8,
+                                      grad_bits: Optional[A2aBits] = None, bucket_size: int = 512, group=None,
+                                      stochastic: bool = False) -> torch.Tensor:
+    """``all_to_all_combine`` that returns its ``[T, ...]`` output and has a backward pass, for the
+    combine of an MoE layer. The gradients, from the slots the forward received:
+      - input: ``grad_out[t] * gate[t, c]`` (in the dtype) for every slot ``t*k + c``, sent back by the
+        routed ``all_to_all_single`` (``input_index=output_index``, splits swapped) at ``grad_bits``
+        (``None``: ``bits``);
+      - gate: ``sum_h grad_out[t, h] * slots[t*k + c, h]`` in fp32.
+    """
+    bits = _a2a_bits(bits, stochastic)
+    gb = _a2a_bits(bits if grad_bits is None else grad_bits, stochastic)
+    return _AllToAllCombine.apply(input, gate, output_index,
+                                  None if output_split_sizes is None else _splits(output_split_sizes),
+                                  None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
+                                  int(bucket_size), group, bool(stochastic))
