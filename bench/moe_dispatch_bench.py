@@ -29,6 +29,21 @@ arm (b)'s, and rank 0's first 64 tokens equal the oracle's fma chain over those 
 run arm (b)'s kernel; (e) then reads the T k slot rows back and writes T rows in the dtype; the
 torch sum reads the slots, writes and reads an fp32 [T, k, H] product and writes T fp32 rows.
 
+With --combine-backward, the backward of differentiable_all_to_all_combine (grad_out [T, H] in the
+dtype, the forward's slots [T k, H] and fp32 gates [T, k], seeded):
+
+  backward torch: grad_slots = (grad_out * gate) in the dtype, all_to_all(gin, grad_slots,
+                  input_index=output_index), and the torch gate gradient (grad_out.float() *
+                  slots.float()).sum(-1)
+  backward fused: all_to_all(gin, grad_out, input_index=output_index // k,
+                  input_scale=gate.view(-1)[output_index]) and combine_gate_grad(grad_out, slots, k)
+
+The input gradients of the two arms are checked bit for bit, and rank 0's first 64 fused gate
+gradients against the oracle. Bytes: both run the same exchange; the torch arm adds grad_slots
+(read grad_out, write and read an fp32 [T, k, H] product, write the dtype) and its gate gradient
+(fp32 copies of grad_out and the slots, the fp32 product written and read); the fused arm reads
+grad_out and the slots once.
+
 Arms alternate in one run, CUDA events around each, medians over --iters after --warmup. The HBM
 bytes of an arm are computed from shapes, all ranks together: the kernel reads the sent rows and
 writes the received rows (2 N H es), writes and reads its wire image once (2 N H bits / 8, plus
@@ -216,6 +231,78 @@ def run_combine(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bfl
     return res
 
 
+def run_combine_backward(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
+    from torch_cgx_b200.ops import oracle as O
+
+    dev = torch.device("cuda", 0)
+    es = torch.tensor([], dtype=dtype).element_size()
+    route = routing(W, T, k, seed=T * 31 + H * 7 + k, device=dev)
+    send_rows = [route[q][2] for q in range(W)]
+    recv_n = [sum(send_rows[q][r] for q in range(W)) for r in range(W)]
+    back_counts = [[send_rows[q][r] * H for r in range(W)] for q in range(W)]  # the combine's, swapped
+    g = C.LocalSraGroup(W, lanes, slot_mb << 20, 20000, 256)
+    gen = torch.Generator(device=dev).manual_seed(T + H + k)
+    grad = [torch.randn(T, H, device=dev, generator=gen).to(dtype) for _ in range(W)]
+    slots = [torch.randn(T * k, H, device=dev, generator=gen).to(dtype) for _ in range(W)]
+    gate = [torch.rand(T, k, device=dev, generator=gen) for _ in range(W)]
+    oi = [route[q][1] for q in range(W)]
+    gin_t = [torch.empty(recv_n[r], H, device=dev, dtype=dtype) for r in range(W)]
+    gin_f = [torch.empty(recv_n[r], H, device=dev, dtype=dtype) for r in range(W)]
+    gg_t, gg_f = [None] * W, [None] * W
+    flat = lambda ts: [t.reshape(-1) for t in ts]  # noqa: E731
+
+    def bwd_torch():
+        gs = [(grad[q].reshape(T, 1, H) * gate[q].unsqueeze(-1)).to(dtype).reshape(T * k, H) for q in range(W)]
+        g.all_to_all(flat(gs), flat(gin_t), back_counts, bits=bits, bucket_size=512, input_index=oi, row=H)
+        for q in range(W):
+            gg_t[q] = (grad[q].reshape(T, 1, H).float() * slots[q].reshape(T, k, H).float()).sum(-1)
+
+    def bwd_fused():
+        ii = [torch.div(ix, k, rounding_mode="floor") for ix in oi]
+        sc = [gate[q].reshape(-1)[oi[q]] for q in range(W)]
+        g.all_to_all(flat(grad), flat(gin_f), back_counts, bits=bits, bucket_size=512, input_index=ii, row=H,
+                     input_scale=sc)
+        for q in range(W):
+            gg_f[q] = C.combine_gate_grad(grad[q], slots[q], k)
+
+    arms = {"backward_torch": bwd_torch, "backward_fused": bwd_fused}
+    ts = {name: [] for name in arms}
+    for it in range(warmup + iters):
+        for name, fn in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            if it >= warmup:
+                ts[name].append(e0.elapsed_time(e1) * 1000.0)
+    g.check()
+    for r in range(W):
+        assert torch.equal(gin_t[r].view(torch.int16), gin_f[r].view(torch.int16)), "input gradients differ"
+    n = min(T, 64)
+    want = O.combine_gate_grad_reference(grad[0][:n].cpu(), slots[0][:n * k].cpu())
+    assert torch.equal(want, gg_f[0][:n].cpu()), "fused gate gradient != oracle"
+
+    N = T * k * W
+    own = sum(send_rows[q][q] for q in range(W))
+    elems_wire = (N - own) * H
+    wbits = 8 if isinstance(bits, str) else bits
+    wire = elems_wire * es if wbits >= 32 else elems_wire * wbits // 8 + (elems_wire // 512) * 8
+    kernel_bytes = 2 * N * H * es + 2 * wire
+    TH, TkH = W * T * H, N * H
+    torch_bytes = kernel_bytes + (TH * es + 8 * TkH + TkH * es) + (TH * (es + 8) + TkH * (es + 16))
+    fused_bytes = kernel_bytes + TH * es + TkH * es
+    res = {"W": W, "T": T, "H": H, "topk": k, "bits": bits, "dtype": str(dtype).replace("torch.", "")}
+    for name in arms:
+        res[name + "_us"] = round(median(ts[name]), 1)
+        res[name + "_spread_us"] = [round(min(ts[name]), 1), round(max(ts[name]), 1)]
+    res["bytes_fused_GB"] = round(fused_bytes / 1e9, 3)
+    res["bytes_torch_GB"] = round(torch_bytes / 1e9, 3)
+    del g, grad, slots, gin_t, gin_f
+    torch.cuda.empty_cache()
+    return res
+
+
 def run_codes(W, T, H, k, bucket, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
     """routed e4m3 dispatch: decode + torch quantize (c) against the codes output (d)"""
     dev = torch.device("cuda", 0)
@@ -302,10 +389,31 @@ def main():
                     help="time the FP8 codes output, arms (c) and (d) at bucket 128 and bucket = H, instead")
     ap.add_argument("--combine", action="store_true",
                     help="time the weighted top-k combine, arm (e) against arm (b) and the torch sum, instead")
+    ap.add_argument("--combine-backward", action="store_true",
+                    help="time the combine's backward, the scaled send and the gate-gradient kernel against "
+                         "grad_slots, the routed call and the torch gate gradient, instead")
     args = ap.parse_args()
     name, power = gpu_info()
     print(json.dumps({"gpu": name, "power_limit": power}), flush=True)
     rows = []
+    if args.combine_backward:
+        for H in args.hidden:
+            for T in args.tokens:
+                for k in args.topk:
+                    need = args.world * (T * k * (2 + 2 + 8) + T * 6) * H / 1e9
+                    if need > args.max_gb:
+                        print(json.dumps({"H": H, "T": T, "topk": k, "skipped": f"needs {need:.1f} GB"}), flush=True)
+                        continue
+                    for bits in args.bits:
+                        r = run_combine_backward(args.world, T, H, k, bits, args.iters, args.warmup, args.lanes,
+                                                 args.slot_mb)
+                        r.update(gpu=name, power_limit=power)
+                        rows.append(r)
+                        print(json.dumps(r), flush=True)
+        if args.out:
+            Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in rows))
+        return
     if args.combine:
         for H in args.hidden:
             for T in args.tokens:

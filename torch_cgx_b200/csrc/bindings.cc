@@ -737,11 +737,13 @@ class LocalSraGroup {
   // Combine (A2aRoute::combine_out): with gate[r] (CUDA float32 [T, k]) and combine_out[r] ([T, row]
   // elements of the inputs' dtype) outputs[r] is rank r's slots buffer of T * k rows, named by its
   // output_index, and the kernel writes the weighted combine of the slots into combine_out[r].
+  // Scaled send (A2aRoute::in_scale): input_scale[r], when given and not None, is a contiguous CUDA
+  // float32 vector of one entry per input_index[r] entry; sent row i is T(x * input_scale[r][i]).
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
                   const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
                   const IndexList& input_index, const IndexList& output_index, int64_t row,
                   const std::optional<std::vector<at::Tensor>>& output_scales, const IndexList& gate,
-                  const IndexList& combine_out) {
+                  const IndexList& combine_out, const IndexList& input_scale) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)world_);
     TORCH_CHECK((int)outputs.size() == world_, "all_to_all: one input and one output per rank");
@@ -774,6 +776,17 @@ class LocalSraGroup {
           (side ? rt.out_index : rt.in_index) = ix.data_ptr<int64_t>();
         }
       }
+    }
+    TORCH_CHECK_VALUE(input_scale.empty() || (int)input_scale.size() == world_, "all_to_all: one input_scale per rank");
+    for (int r = 0; r < (int)input_scale.size(); ++r) {
+      if (!input_scale[r]) continue;
+      const at::Tensor& sc = *input_scale[r];
+      TORCH_CHECK_VALUE(routes[r].in_index != nullptr, "all_to_all: rank ", r, "'s input_scale needs an input_index");
+      TORCH_CHECK_VALUE(sc.is_cuda() && sc.scalar_type() == at::kFloat && sc.dim() == 1 && sc.is_contiguous() &&
+                            sc.numel() == input_index[r]->numel(),
+                        "all_to_all: rank ", r, "'s input_scale must be a contiguous CUDA float32 vector of one ",
+                        "entry per input_index entry");
+      routes[r].in_scale = sc.data_ptr<float>();
     }
     const std::vector<at::Tensor> masks =
         combine_routes(routes, inputs, gate, combine_out, wb, bucket, row, output_scales.has_value());
@@ -1756,18 +1769,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
               const std::vector<int64_t>& in_splits, const A2aBitsArg& bits, int bucket_size, bool stochastic,
               int64_t seed, const std::optional<at::Tensor>& in_index, const std::optional<at::Tensor>& out_index,
               const std::optional<at::Tensor>& out_scales, const std::optional<at::Tensor>& gate,
-              const std::optional<at::Tensor>& combine_out) {
+              const std::optional<at::Tensor>& combine_out, const std::optional<at::Tensor>& in_scale) {
              const A2aBits wb = a2a_bits(bits, stochastic);
              return pg.all_to_all_compressed(out, in, out_splits, in_splits, wb.bits, wb.codec, bucket_size,
                                              stochastic, seed, in_index.value_or(at::Tensor()),
                                              out_index.value_or(at::Tensor()), out_scales.value_or(at::Tensor()),
-                                             gate.value_or(at::Tensor()), combine_out.value_or(at::Tensor()));
+                                             gate.value_or(at::Tensor()), combine_out.value_or(at::Tensor()),
+                                             in_scale.value_or(at::Tensor()));
            },
            py::arg("output"), py::arg("input"), py::arg("output_split_sizes") = std::vector<int64_t>{},
            py::arg("input_split_sizes") = std::vector<int64_t>{}, py::arg("bits") = 8, py::arg("bucket_size") = 512,
            py::arg("stochastic") = false, py::arg("seed") = -1, py::arg("input_index") = py::none(),
            py::arg("output_index") = py::none(), py::arg("output_scales") = py::none(),
-           py::arg("gate") = py::none(), py::arg("combine_out") = py::none(), py::call_guard<py::gil_scoped_release>())
+           py::arg("gate") = py::none(), py::arg("combine_out") = py::none(), py::arg("input_scale") = py::none(),
+           py::call_guard<py::gil_scoped_release>())
       .def("init_cuda", &ProcessGroupCGX::init_cuda, py::call_guard<py::gil_scoped_release>())
       .def("p2p_ready", &ProcessGroupCGX::p2p_ready)
       .def("lanes", &ProcessGroupCGX::lanes)
@@ -1977,6 +1992,30 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dequantize", &py_dequantize, py::arg("wire"), py::arg("like"), py::arg("layers"), py::arg("world") = 1,
         py::arg("lanes") = 1, py::arg("skip_incomplete") = false, py::arg("min_lane_elems") = 2048);
 
+  // The gate gradient of the weighted top-k combine (combine_gate_grad_kernel, DESIGN §2.13e) on the
+  // current stream: grad_out [T, ...] and slots [T * k, ...] contiguous, of one dtype, any alignment;
+  // returns grad_gate [T, k] float32.
+  m.def(
+      "combine_gate_grad",
+      [](const at::Tensor& grad_out, const at::Tensor& slots, int64_t k) {
+        TORCH_CHECK_VALUE(k >= 1 && k <= 32, "combine_gate_grad: k = ", k, " is not in 1..32");
+        TORCH_CHECK_VALUE(grad_out.is_cuda() && slots.is_cuda() && grad_out.device() == slots.device() &&
+                              grad_out.is_contiguous() && slots.is_contiguous() && grad_out.dim() >= 1 &&
+                              slots.scalar_type() == grad_out.scalar_type(),
+                          "combine_gate_grad: contiguous CUDA float32, float16 or bfloat16 tensors of one dtype");
+        const int64_t T = grad_out.size(0), H = T > 0 ? grad_out.numel() / T : 0;
+        TORCH_CHECK_VALUE(slots.numel() == T * k * H && H < (1ll << 32), "combine_gate_grad: slots must hold T * k = ",
+                          T * k, " rows of the ", H, " elements of a grad_out row");
+        c10::cuda::CUDAGuard g(grad_out.device());
+        at::Tensor out = at::empty({T, k}, grad_out.options().dtype(at::kFloat));
+        cuda_check(launch_combine_gate_grad(grad_out.data_ptr(), slots.data_ptr(), out.data_ptr<float>(),
+                                            cgx_dtype(grad_out), (uint64_t)T, (uint32_t)k, (uint32_t)H,
+                                            c10::cuda::getCurrentCUDAStream()),
+                   "launch_combine_gate_grad");
+        return out;
+      },
+      py::arg("grad_out"), py::arg("slots"), py::arg("k"));
+
   m.def("scale_", [](at::Tensor t, double s) {
     TORCH_CHECK(t.is_cuda() && t.is_contiguous(), "scale_: contiguous CUDA tensor");
     c10::cuda::CUDAGuard g(t.device());
@@ -2066,7 +2105,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("input_index") = IndexList{}, py::arg("output_index") = IndexList{},
            py::arg("row") = 1, py::arg("output_scales") = py::none(), py::arg("gate") = IndexList{},
-           py::arg("combine_out") = IndexList{})
+           py::arg("combine_out") = IndexList{}, py::arg("input_scale") = IndexList{})
       .def("check", &LocalSraGroup::check)
       .def("allreduce_with_absent_rank", &LocalSraGroup::allreduce_with_absent_rank, py::arg("tensors"),
            py::arg("layers"), py::arg("absent"))

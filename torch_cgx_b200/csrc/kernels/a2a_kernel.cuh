@@ -69,6 +69,26 @@ __device__ __forceinline__ bool a2a_wait(const A2aParams& p, const uint64_t* my_
   return __all_sync(kAll, rc == 0);
 }
 
+// The scaled send (SCALE): the values T(x * s) of one row, 16 bytes or one element at a time
+template <typename T>
+__device__ __forceinline__ uint4 scale_round16(const uint4& raw, float s) {
+  float x[DT<T>::kVec];
+  unpack16<T>(raw, x);
+#pragma unroll
+  for (int i = 0; i < DT<T>::kVec; ++i) x[i] = scale_round<T>(x[i], s);
+  return pack16<T>(x);
+}
+__device__ __forceinline__ uint32_t elem_bits(float v) { return __float_as_uint(v); }
+__device__ __forceinline__ uint32_t elem_bits(__half v) { return __half_as_ushort(v); }
+__device__ __forceinline__ uint32_t elem_bits(__nv_bfloat16 v) { return __bfloat16_as_ushort(v); }
+template <int GPL, typename T>
+__device__ __forceinline__ void slice_scale_round(float (&x)[GPL][8], float s) {
+#pragma unroll
+  for (int k = 0; k < GPL; ++k)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) x[k][j] = scale_round<T>(x[k][j], s);
+}
+
 // raw items travel as the T bits, unchanged (a NaN keeps its payload, -0 stays -0)
 template <typename T>
 __device__ __forceinline__ void a2a_raw_send(const T* src, const WarpItem& it, uint8_t* slot) {
@@ -85,6 +105,26 @@ __device__ __forceinline__ void a2a_raw_send(const T* src, const WarpItem& it, u
       st_u32(dst + i * 4u, reinterpret_cast<const uint32_t*>(src)[i]);
     else
       st_u16(dst + i * 2u, reinterpret_cast<const uint16_t*>(src)[i]);
+  }
+}
+// the same for the bits of T(x * s) (SCALE)
+template <typename T>
+__device__ __forceinline__ void a2a_raw_send_scaled(const T* src, const WarpItem& it, uint8_t* slot, float s) {
+  const uint32_t n = item_n(it);
+  uint8_t* dst = slot + it.meta_off;
+  uint32_t done = 0;
+  if ((reinterpret_cast<uintptr_t>(src) & 15u) == 0) {
+    const uint32_t vecs = n * (uint32_t)sizeof(T) / 16u;
+    for (uint32_t v = lane_id(); v < vecs; v += 32)
+      st_v4(dst + v * 16u, scale_round16<T>(reinterpret_cast<const uint4*>(src)[v], s));
+    done = vecs * 16u / (uint32_t)sizeof(T);
+  }
+  for (uint32_t i = done + lane_id(); i < n; i += 32) {
+    const uint32_t b = elem_bits(scale_round_to<T>(DT<T>::to_float(src[i]), s));
+    if (sizeof(T) == 4)
+      st_u32(dst + i * 4u, b);
+    else
+      st_u16(dst + i * 2u, (uint16_t)b);
   }
 }
 
@@ -136,8 +176,8 @@ __device__ __forceinline__ void a2a_combine_arrive(const A2aParams& p, const T* 
 }
 
 // my own chunk, routed: one warp per row, through both indices (COMBINE: then arrives at every
-// segment of the slot row)
-template <typename T, bool COMBINE>
+// segment of the slot row; SCALE: the row's T(x * s), as sent to the peers)
+template <typename T, bool COMBINE, bool SCALE = false>
 __device__ __forceinline__ void a2a_copy_own_rows(const A2aParams& p) {
   const uint32_t H = p.row, rows = p.in_cnt[p.rank] / H;
   const uint32_t nwarps = gridDim.x * kSraWarps;
@@ -146,13 +186,24 @@ __device__ __forceinline__ void a2a_copy_own_rows(const A2aParams& p) {
     T* dst = a2a_row_addr(p, reinterpret_cast<T*>(p.out), p.out_index, p.out_rows, p.out_off[p.rank] + j * H, 1u);
     if (src == nullptr || dst == nullptr) continue;
     uint32_t done = 0;
-    if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
-      const uint32_t vecs = H * (uint32_t)sizeof(T) / 16u;
-      for (uint32_t v = lane_id(); v < vecs; v += 32)
-        reinterpret_cast<uint4*>(dst)[v] = reinterpret_cast<const uint4*>(src)[v];
-      done = vecs * 16u / (uint32_t)sizeof(T);
+    if constexpr (SCALE) {
+      const float s = p.in_scale[p.in_off[p.rank] / H + j];
+      if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
+        const uint32_t vecs = H * (uint32_t)sizeof(T) / 16u;
+        for (uint32_t v = lane_id(); v < vecs; v += 32)
+          reinterpret_cast<uint4*>(dst)[v] = scale_round16<T>(reinterpret_cast<const uint4*>(src)[v], s);
+        done = vecs * 16u / (uint32_t)sizeof(T);
+      }
+      for (uint32_t i = done + lane_id(); i < H; i += 32) dst[i] = scale_round_to<T>(DT<T>::to_float(src[i]), s);
+    } else {
+      if (((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15u) == 0) {
+        const uint32_t vecs = H * (uint32_t)sizeof(T) / 16u;
+        for (uint32_t v = lane_id(); v < vecs; v += 32)
+          reinterpret_cast<uint4*>(dst)[v] = reinterpret_cast<const uint4*>(src)[v];
+        done = vecs * 16u / (uint32_t)sizeof(T);
+      }
+      for (uint32_t i = done + lane_id(); i < H; i += 32) dst[i] = src[i];
     }
-    for (uint32_t i = done + lane_id(); i < H; i += 32) dst[i] = src[i];
     if constexpr (COMBINE)
       for (uint32_t col = 0; col < H; col += p.span) a2a_combine_arrive<T>(p, dst + col);
   }
@@ -202,6 +253,19 @@ __device__ __forceinline__ bool a2a_window_item(const A2aGeom& g, const A2aWindo
   return true;
 }
 
+// A full item of T(x * s) that is not vector aligned (SCALE): out of line, as full_send_unaligned
+template <typename T, int KB, int GPL, int CODEC, typename DST>
+__device__ __noinline__ void a2a_send_scaled_unaligned(const T* __restrict__ src, const WarpItem it, float s,
+                                                       const RngKey rng, const DST ds) {
+  float x[GPL][8];
+  slice_load_scalar<T, GPL>(src, x);
+  slice_scale_round<GPL, T>(x, s);
+  if constexpr (CODEC != kMaxMin)
+    full_send_fp8_x<CODEC, GPL>(x, it, ds);
+  else
+    full_send_x<T, KB, GPL, false, false>(x, it, 1.0f, rng, ds, (T*)nullptr);
+}
+
 // one item of a chunk in an FP8 codec (KB 8 records, round to nearest): to a peer's slot (OneDst),
 // or to the codes output (CodesDst)
 template <typename T, int CODEC, int GPL, typename DST>
@@ -216,6 +280,22 @@ __device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& 
     }
   } else {
     bucket_quantize_fp8<T, CODEC>(src, it, push);
+  }
+}
+// the same for the values T(x * s) (SCALE)
+template <typename T, int CODEC, int GPL, typename DST>
+__device__ __forceinline__ void a2a_send_item_fp8_scaled(const T* src, const WarpItem& it, const DST& push, float s) {
+  if (item_kind(it) == kItemFull) {
+    if (group_aligned<T>(src)) {
+      float x[GPL][8];
+      slice_load_vec<T, GPL>(src, x);
+      slice_scale_round<GPL, T>(x, s);
+      full_send_fp8_x<CODEC, GPL>(x, it, push);
+    } else {
+      a2a_send_scaled_unaligned<T, 8, GPL, CODEC, DST>(src, it, s, RngKey{}, push);
+    }
+  } else {
+    bucket_quantize_fp8_rounded<T, CODEC>(src, it, s, push);
   }
 }
 template <typename T, int CODEC, int GPL>
@@ -233,7 +313,32 @@ __device__ __forceinline__ void a2a_recv_item_fp8(const uint8_t* rec, const Warp
   }
 }
 
-template <typename T, int KB, int GPL, bool IDX, int CODEC>
+// one item of the values T(x * s) to a peer's slot (SCALE), every codec
+template <typename T, int KB, int GPL, int CODEC>
+__device__ __forceinline__ void a2a_send_item_scaled(const T* src, const WarpItem& it, float s, const RngKey& rng,
+                                                     const OneDst& push) {
+  if constexpr (CODEC != kMaxMin) {
+    a2a_send_item_fp8_scaled<T, CODEC, GPL, OneDst>(src, it, push, s);
+    return;
+  }
+  const uint32_t kind = item_kind(it);
+  if (kind == kItemFull) {
+    if (group_aligned<T>(src)) {
+      float x[GPL][8];
+      slice_load_vec<T, GPL>(src, x);
+      slice_scale_round<GPL, T>(x, s);
+      full_send_x<T, KB, GPL, false, true>(x, it, 1.0f, rng, push, (T*)nullptr);
+    } else {
+      a2a_send_scaled_unaligned<T, KB, GPL, kMaxMin, OneDst>(src, it, s, rng, push);
+    }
+  } else if (kind == kItemBucket) {
+    bucket_quantize_rounded<T, OneDst>(src, it, s, rng, push);
+  } else {
+    a2a_raw_send_scaled<T>(src, it, push.p, s);
+  }
+}
+
+template <typename T, int KB, int GPL, bool IDX, int CODEC, bool SCALE>
 __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint32_t bpw, uint32_t k,
                                                 const RngKey& rng) {
   const int r = p.rank;
@@ -254,6 +359,11 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
       if (src == nullptr) continue;
     } else {
       src = chunk + it.elem_off;
+    }
+    if constexpr (SCALE) {
+      // and one scale load
+      a2a_send_item_scaled<T, KB, GPL, CODEC>(src, it, p.in_scale[(p.in_off[q] + it.elem_off) / p.row], rng, push);
+      continue;
     }
     if constexpr (CODEC != kMaxMin) {
       a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, push);
@@ -366,11 +476,15 @@ __device__ __forceinline__ void a2a_recv_window(const A2aParams& p, int q, uint3
 // every chunk undecoded, the own chunk encoded like a peer's.
 // COMBINE (routed, decoded output; A2aParams::combine_out set): the weighted top-k combine of the
 // slots, finalized per segment by the last warp to store into it.
-template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin, bool CODES = false, bool COMBINE = false>
+// SCALE (routed, decoded output, no combine; A2aParams::in_scale set): sent row i is T(x * in_scale[i]),
+// the own rows included.
+template <typename T, int KB, int GPL, bool IDX = false, int CODEC = kMaxMin, bool CODES = false, bool COMBINE = false,
+          bool SCALE = false>
 __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const __grid_constant__ A2aParams p) {
   static_assert(CODEC == kMaxMin || KB == 8, "the FP8 codecs use 8-bit records");
   static_assert(!CODES || CODEC != kMaxMin, "codes are delivered for the FP8 codecs only");
   static_assert(!COMBINE || (IDX && !CODES), "the combine needs the routed, decoded output");
+  static_assert(!SCALE || (IDX && !CODES && !COMBINE), "the scaled send needs the routed, decoded output");
   __shared__ int s_abort;
   __shared__ uint32_t s_send[kMaxPeers], s_recv[kMaxPeers];  // this lane's windows per destination / source
   const int lane = blockIdx.x, r = p.rank, W = p.world;
@@ -404,7 +518,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
       const int q = (r + s) % W;
       if (s_send[q] <= k) continue;
       rng.stream = a2a_rng_stream(r, q);
-      a2a_send_window<T, KB, GPL, IDX, CODEC>(p, q, bpw, k, rng);
+      a2a_send_window<T, KB, GPL, IDX, CODEC, SCALE>(p, q, bpw, k, rng);
     }
     __syncthreads();
     if (threadIdx.x < 32 && has_send)
@@ -427,7 +541,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     if constexpr (CODES)
       a2a_encode_own<T, GPL, IDX, CODEC>(p);
     else if constexpr (IDX)
-      a2a_copy_own_rows<T, COMBINE>(p);
+      a2a_copy_own_rows<T, COMBINE, SCALE>(p);
     else
       a2a_copy_own<T>(p);
   }
@@ -470,9 +584,34 @@ cudaError_t launch_a2a_combine(const A2aParams& p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// the scaled-send instantiations: routed, decoded output, no combine, every codec and KB
+template <typename T, int GPL>
+cudaError_t launch_a2a_scaled(const A2aParams& p, cudaStream_t stream) {
+  if (p.out_scales != nullptr || p.combine_out != nullptr || p.in_index == nullptr ||
+      (p.codec != kMaxMin && p.bits != 8))
+    return cudaErrorInvalidValue;
+  if (p.codec == kE4M3) {
+    dev::a2a_kernel<T, 8, GPL, true, kE4M3, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    return cudaGetLastError();
+  }
+  if (p.codec == kE5M2) {
+    dev::a2a_kernel<T, 8, GPL, true, kE5M2, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+    return cudaGetLastError();
+  }
+  if (p.codec != kMaxMin) return cudaErrorInvalidValue;
+  switch ((p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0) {
+    case 2: dev::a2a_kernel<T, 2, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 4: dev::a2a_kernel<T, 4, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    case 8: dev::a2a_kernel<T, 8, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+    default: dev::a2a_kernel<T, 0, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
+  }
+  return cudaGetLastError();
+}
+
 template <typename T, int GPL, bool IDX>
 cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
   if constexpr (IDX) {
+    if (p.in_scale != nullptr) return launch_a2a_scaled<T, GPL>(p, stream);
     if (p.combine_out != nullptr) return launch_a2a_combine<T, GPL>(p, stream);
   }
   if (p.codec != kMaxMin) {

@@ -31,6 +31,17 @@ struct DT<__nv_bfloat16> {
   __device__ __forceinline__ static __nv_bfloat16 from_float(float v) { return __float2bfloat16_rn(v); }
 };
 
+// T(x * s): one fp32 multiply, rounded to nearest even in T (fp32: no second rounding); scale_round
+// gives it back in fp32. The scaled send of the routed all-to-all (DESIGN §2.13e) sends these values.
+template <typename T>
+__device__ __forceinline__ T scale_round_to(float x, float s) {
+  return DT<T>::from_float(__fmul_rn(x, s));
+}
+template <typename T>
+__device__ __forceinline__ float scale_round(float x, float s) {
+  return DT<T>::to_float(scale_round_to<T>(x, s));
+}
+
 // 16 B of T <-> fp32 registers
 template <typename T>
 __device__ __forceinline__ void unpack16(const uint4& raw, float* out);

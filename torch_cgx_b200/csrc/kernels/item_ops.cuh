@@ -470,13 +470,14 @@ __device__ __noinline__ void full_recv_unaligned(const SrcSet ss, const WarpItem
 // generic bucket items (cold): ONE bucket of n <= kMaxBlockElems elements, any alignment,
 // any bit width. Two passes (min/max, then encode); lane l handles groups l, l+32, ...
 // ======================================================================================
-template <typename TS>
+// ROUND: the products are rounded to TS as well, x = TS(x * prescale) (scale_round)
+template <typename TS, bool ROUND = false>
 __device__ __forceinline__ void bucket_load_group(const TS* __restrict__ src, uint32_t g, uint32_t n, float prescale,
                                                   float (&x)[8], int& nv) {
   nv = (int)min(8u, n - g * 8u);
   load8_scalar<TS>(src + g * 8u, nv, x);
 #pragma unroll
-  for (int j = 0; j < 8; ++j) x[j] = __fmul_rn(x[j], prescale);
+  for (int j = 0; j < 8; ++j) x[j] = ROUND ? scale_round<TS>(x[j], prescale) : __fmul_rn(x[j], prescale);
 }
 
 __device__ __forceinline__ void bucket_add_sources(const SrcSet& ss, const WarpItem& it, uint32_t g, int bits,
@@ -496,11 +497,11 @@ __device__ __forceinline__ void bucket_add_sources(const SrcSet& ss, const WarpI
 }
 
 // phase A / phase B / quantize of a generic bucket. `ss.n == 0`: nothing to add (send);
-// self_out != nullptr: write the self-decoded values there
-template <typename TS, typename TO, typename DST>
-__device__ __noinline__ void bucket_quantize(const TS* __restrict__ src, const WarpItem it, float prescale,
-                                             const RngKey rng, const SrcSet ss, const DST ds,
-                                             TO* __restrict__ self_out) {
+// self_out != nullptr: write the self-decoded values there; ROUND: as bucket_load_group
+template <typename TS, typename TO, typename DST, bool ROUND>
+__device__ __forceinline__ void bucket_quantize_body(const TS* __restrict__ src, const WarpItem& it, float prescale,
+                                                     const RngKey& rng, const SrcSet& ss, const DST& ds,
+                                                     TO* __restrict__ self_out) {
   const uint32_t n = item_n(it);
   const int bits = item_bits(it);
   const uint32_t ng = div_up(n, 8u);
@@ -508,7 +509,7 @@ __device__ __noinline__ void bucket_quantize(const TS* __restrict__ src, const W
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, prescale, x, nv);
+    bucket_load_group<TS, ROUND>(src, g, n, prescale, x, nv);
     if (ss.n > 0) bucket_add_sources(ss, it, g, bits, x);
     minmax8_pred(x, nv, mn, mx);
   }
@@ -522,7 +523,7 @@ __device__ __noinline__ void bucket_quantize(const TS* __restrict__ src, const W
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, prescale, x, nv);
+    bucket_load_group<TS, ROUND>(src, g, n, prescale, x, nv);
     if (ss.n > 0) bucket_add_sources(ss, it, g, bits, x);
     float r[8];
     if (rng.enabled) {
@@ -549,6 +550,18 @@ __device__ __noinline__ void bucket_quantize(const TS* __restrict__ src, const W
       store8_scalar<TO>(self_out + g * 8u, nv, dec);
     }
   }
+}
+template <typename TS, typename TO, typename DST>
+__device__ __noinline__ void bucket_quantize(const TS* __restrict__ src, const WarpItem it, float prescale,
+                                             const RngKey rng, const SrcSet ss, const DST ds,
+                                             TO* __restrict__ self_out) {
+  bucket_quantize_body<TS, TO, DST, false>(src, it, prescale, rng, ss, ds, self_out);
+}
+// send of the generic bucket of TS(src * scale) (scale_round)
+template <typename TS, typename DST>
+__device__ __noinline__ void bucket_quantize_rounded(const TS* __restrict__ src, const WarpItem it, float scale,
+                                                     const RngKey rng, const DST ds) {
+  bucket_quantize_body<TS, TS, DST, true>(src, it, scale, rng, SrcSet{nullptr, 0u, 0, -1}, ds, (TS*)nullptr);
 }
 
 // decode one source (ss.n == 1) or the sum of all sources into `out`
@@ -907,8 +920,9 @@ __device__ __noinline__ void full_recv_fp8_unaligned(const uint8_t* rec, const W
 
 // generic bucket item (cold): ONE bucket of n <= kMaxBlockElems elements, any alignment; the codes
 // of the last group's missing elements are 0, as on the host
-// of the values src * prescale; self_out != nullptr: also the values decoded from the codes there
-template <typename TS, typename TO, int CODEC, typename DST>
+// of the values src * prescale; self_out != nullptr: also the values decoded from the codes there;
+// ROUND: as bucket_load_group
+template <typename TS, typename TO, int CODEC, typename DST, bool ROUND = false>
 __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, const WarpItem& it, float prescale,
                                                 const DST& ds, TO* __restrict__ self_out) {
   const uint32_t n = item_n(it);
@@ -917,7 +931,7 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, prescale, x, nv);
+    bucket_load_group<TS, ROUND>(src, g, n, prescale, x, nv);
     minmax8_pred(x, nv, mn, mx);
   }
   warp_minmax(mn, mx);
@@ -928,7 +942,7 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
   for (uint32_t g = lane_id(); g < ng; g += 32) {
     float x[8];
     int nv;
-    bucket_load_group<TS>(src, g, n, prescale, x, nv);
+    bucket_load_group<TS, ROUND>(src, g, n, prescale, x, nv);
     uint32_t lo, hi;
     fp8_encode8<CODEC>(x, inv, lo, hi);
     const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
@@ -944,6 +958,12 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
 template <typename TS, int CODEC, typename DST>
 __device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const DST ds) {
   bucket_fp8_body<TS, float, CODEC>(src, it, 1.0f, ds, (float*)nullptr);
+}
+// the same for the bucket of TS(src * scale) (scale_round)
+template <typename TS, int CODEC, typename DST>
+__device__ __noinline__ void bucket_quantize_fp8_rounded(const TS* __restrict__ src, const WarpItem it, float scale,
+                                                         const DST ds) {
+  bucket_fp8_body<TS, float, CODEC, DST, true>(src, it, scale, ds, (float*)nullptr);
 }
 
 template <typename TO, int CODEC>

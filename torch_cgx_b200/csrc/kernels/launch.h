@@ -132,6 +132,9 @@ struct A2aParams {
   uint32_t* masks;
   uint32_t topk;                   // 1..32
   uint32_t span;                   // a2a_row_span(bits, bucket, dtype)
+  // Scaled send (with in_index, decoded output, no combine; nullptr: none): row i of the logical send
+  // buffer is T(x * in_scale[i]), one fp32 multiply rounded to nearest in T, the own rows included.
+  const float* in_scale;
 };
 // defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
 // p.out_index is set
@@ -177,6 +180,17 @@ cudaError_t launch_accumulate_items_f32(const ItemKernelArgs& a, const uint8_t* 
 // x_c = float(slots[t * k + c, h]) and g_c = gate[t, c]; slots [T * k, H], gate [T, k] fp32, out [T, H]
 cudaError_t launch_combine_rows(const void* slots, const float* gate, void* out, int dtype, uint64_t T, uint32_t k,
                                 uint32_t H, cudaStream_t stream);
+// The gradient of that combine with respect to the gate (combine_gate_grad_kernel, DESIGN §2.13e):
+// grad_gate[t, c] = sum over h of float(grad_out[t, h]) * float(slots[t * k + c, h]) in fp32, in a
+// fixed order: lane l = (h / V) % 32 (V = 16 / sizeof(T)) runs acc = fma(go_h, x_h, acc) from +0
+// over its elements in increasing h, then acc += shfl_xor(acc, m) for m = 16, 8, 4, 2, 1.
+// grad_out [T, H], slots [T * k, H] and grad_gate [T, k] (fp32) contiguous, k 1..32; grad_out and
+// slots at any element alignment.
+cudaError_t launch_combine_gate_grad(const void* grad_out, const void* slots, float* grad_gate, int dtype, uint64_t T,
+                                     uint32_t k, uint32_t H, cudaStream_t stream);
+// rows[i, h] = T(float(rows[i, h]) * scale[i]) in place, rows [R, H] contiguous: the scaled send of
+// the routed all-to-all's composed path, with the fused kernel's rounding
+cudaError_t launch_scale_rows(void* rows, const float* scale, int dtype, uint64_t R, uint64_t H, cudaStream_t stream);
 
 // ---- elementwise helpers (K4/K7 of the reference) ---------------------------
 cudaError_t launch_scale_inplace(void* data, int dtype, uint64_t n, float scale, cudaStream_t stream);

@@ -520,7 +520,8 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
                                                                       const at::Tensor& out_index,
                                                                       const at::Tensor& out_scales,
                                                                       const at::Tensor& gate,
-                                                                      const at::Tensor& combine_out) {
+                                                                      const at::Tensor& combine_out,
+                                                                      const at::Tensor& in_scale) {
   TORCH_CHECK(in.is_cuda() && out.is_cuda(), "cgx: all_to_all needs CUDA tensors");
   TORCH_CHECK(in.device() == out.device(), "cgx: all_to_all: input and output on different devices");
   const int dtype = to_cgx_dtype(in.scalar_type());
@@ -577,6 +578,18 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
                       "cgx: all_to_all_combine: the output must be a contiguous ", in.scalar_type(), " tensor of ", T,
                       " rows like the input's on ", out.device());
   }
+  const bool scaled = in_scale.defined();
+  if (scaled) {
+    // the checks of cgx.all_to_all_single's input_scale, repeated for callers of the binding
+    TORCH_CHECK_VALUE(ii, "cgx: all_to_all: input_scale needs an input_index");
+    TORCH_CHECK_VALUE(!codes, "cgx: all_to_all: input_scale has no codes output (output_scales)");
+    TORCH_CHECK_VALUE(!combine, "cgx: all_to_all: input_scale has no combine (gate)");
+    TORCH_CHECK_VALUE(in_scale.scalar_type() == at::kFloat && in_scale.is_cuda() && in_scale.device() == in.device() &&
+                          in_scale.is_contiguous() && in_scale.dim() == 1 && in_scale.size(0) == in_index.size(0),
+                      "cgx: all_to_all: input_scale must be a contiguous CUDA float32 vector of ", in_index.size(0),
+                      " entries (one per input_index entry) on ", in.device(), ", got ", in_scale.scalar_type(), " ",
+                      in_scale.sizes(), " on ", in_scale.device());
+  }
   if (codes) {
     TORCH_CHECK(bucket_size <= (int)kMaxBlockElems && row % bucket_size == 0, "cgx: all_to_all: output_scales needs ",
                 "bucket_size <= ", kMaxBlockElems, " dividing the row length ", row, ", got ", bucket_size);
@@ -604,6 +617,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     route.gate = gate.data_ptr<float>();
     route.topk = (uint32_t)topk;
   }
+  if (scaled) route.in_scale = in_scale.data_ptr<float>();
   const bool routed = ii || oi;
   float* scales = codes ? out_scales.data_ptr<float>() : nullptr;
   check_all_to_all(in.data_ptr(), out.data_ptr(), in_counts, out_counts, dtype, bits, codec, (uint32_t)bucket_size,
@@ -612,7 +626,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   // address them, else around a plain call, which computes the same by definition
   const bool in_kernel = routed && engine_->routes_in_kernel(true, dtype, bits, (uint32_t)bucket_size, (uint64_t)row);
   return enqueue_cuda(c10d::OpType::ALLTOALL_BASE, "cgx:all_to_all", out, &in, [&](cudaStream_t s) {
-    for (const at::Tensor* t : {&in_index, &out_index, &out_scales, &gate, &combine_out})
+    for (const at::Tensor* t : {&in_index, &out_index, &out_scales, &gate, &combine_out, &in_scale})
       if (t->defined()) c10::cuda::CUDACachingAllocator::recordStream(t->storage().data_ptr(), *comm_stream_);
     at::Tensor masks;
     if (combine && in_kernel) {
@@ -631,6 +645,11 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     // the temporaries live on the comm stream only
     c10::cuda::CUDAStreamGuard sg(*comm_stream_);
     const at::Tensor send = ii ? in.index_select(0, in_index) : in;
+    // the scaled send: the selected rows times their scales, rounded as the fused kernel rounds them
+    if (scaled)
+      cuda_check(launch_scale_rows(send.data_ptr(), in_scale.data_ptr<float>(), dtype, (uint64_t)send.size(0),
+                                   (uint64_t)row, s),
+                 "launch_scale_rows");
     std::vector<int64_t> recv_shape = out.sizes().vec();
     recv_shape[0] = oi ? out_index.size(0) : out.size(0);
     at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;

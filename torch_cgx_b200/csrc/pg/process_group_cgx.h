@@ -218,6 +218,11 @@ class ProcessGroupCGX : public c10d::Backend {
   // `out_index` exactly as the routed call fills it, and combine_out[t] = T(fma chain over the slots
   // t * k + c with the gates, c = 0 .. k - 1): inside the fused kernel when routes_in_kernel, else
   // combine_rows_kernel after the composition. Malformed combine arguments raise ValueError.
+  // Scaled send (DESIGN §2.13e): with `in_scale` (contiguous CUDA float32, one entry per in_index
+  // entry) sent row i is T(float(in[in_index[i]]) * in_scale[i]), one fp32 multiply rounded to
+  // nearest in the dtype, and the call is the routed call on those rows: inside the fused kernel
+  // when routes_in_kernel, else index_select, scale_rows_kernel and the plain call. It needs
+  // in_index and refuses a codes output, a combine and a scale overlapping `out` with ValueError.
   c10::intrusive_ptr<c10d::Work> all_to_all_compressed(at::Tensor& out, at::Tensor& in,
                                                        const std::vector<int64_t>& out_splits,
                                                        const std::vector<int64_t>& in_splits, int bits,
@@ -226,7 +231,8 @@ class ProcessGroupCGX : public c10d::Backend {
                                                        const at::Tensor& out_index = at::Tensor(),
                                                        const at::Tensor& out_scales = at::Tensor(),
                                                        const at::Tensor& gate = at::Tensor(),
-                                                       const at::Tensor& combine_out = at::Tensor());
+                                                       const at::Tensor& combine_out = at::Tensor(),
+                                                       const at::Tensor& in_scale = at::Tensor());
   // force the lazy CUDA-side initialisation (heap allocation + IPC exchange)
   void init_cuda(int64_t device_index);
   bool p2p_ready() const { return engine_ && engine_->has_p2p(); }

@@ -384,6 +384,16 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
     if (overlap(a, nin * es, g, ng)) throw std::invalid_argument("cgx all_to_all_combine: the gate overlaps the input");
     if (overlap(b, nout * es, c, nc)) throw std::invalid_argument("cgx all_to_all_combine: the output overlaps the slots");
   }
+  if (route != nullptr && route->in_scale != nullptr) {
+    if (route->in_index == nullptr) throw std::invalid_argument("cgx all_to_all: input_scale needs an input_index");
+    if (out_scales != nullptr)
+      throw std::invalid_argument("cgx all_to_all: input_scale has no codes output (output_scales)");
+    if (route->combine_out != nullptr) throw std::invalid_argument("cgx all_to_all: input_scale has no combine (gate)");
+    uint64_t sent = 0;
+    for (int q = 0; q < world; ++q) sent += in_counts[q] / route->row;
+    if (overlap(b, nout * es, reinterpret_cast<uintptr_t>(route->in_scale), sent * sizeof(float)))
+      throw std::invalid_argument("cgx all_to_all: input_scale overlaps the output");
+  }
   if (out_scales == nullptr) {
     if (overlap(a, nin * es, b, nout * es)) throw std::invalid_argument("cgx all_to_all: the output overlaps the input");
     return;
@@ -480,6 +490,7 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
       p.topk = route->topk;
       p.span = a2a_row_span(bits, bucket, (int)es);
     }
+    p.in_scale = route->in_scale;
   }
   last_lanes_ = G;
   cudaError_t e = cudaErrorInvalidValue;

@@ -93,6 +93,7 @@ struct A2aRoute {
   const float* gate = nullptr;  // [T, topk] fp32
   uint32_t topk = 0;            // 1..32
   uint32_t* masks = nullptr;
+  const float* in_scale = nullptr;  // scaled send: one fp32 per in_index entry (A2aParams::in_scale)
 };
 
 // The arguments of one rank's all-to-all (FusedSra::all_to_all, Reducer::all_to_all): a count per
@@ -103,7 +104,8 @@ struct A2aRoute {
 // bucket: an FP8 codec, a bucket of at most kMaxBlockElems that divides every count (and the row),
 // and codes, scales and input pairwise disjoint. A combine (route->combine_out) needs an out_index
 // whose entries are the out_rows = T * topk slots, topk in 1..32, no codes output, and neither
-// combine_out nor the gate overlapping the input, or combine_out the slots.
+// combine_out nor the gate overlapping the input, or combine_out the slots. A scaled send
+// (route->in_scale) needs an in_index, no codes output and no combine, and a scale not overlapping `out`.
 void check_all_to_all(const void* in, const void* out, const std::vector<uint64_t>& in_counts,
                       const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
                       int rank, int world, const A2aRoute* route = nullptr, const float* out_scales = nullptr);

@@ -824,18 +824,26 @@ def routed_all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Se
 def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
                                 input_index: Sequence[torch.Tensor | None],
                                 output_index: Sequence[torch.Tensor | None], row: int, *, bits: int | str,
-                                bucket_size: int, outputs: Sequence[torch.Tensor] | None = None) -> List[torch.Tensor]:
+                                bucket_size: int, outputs: Sequence[torch.Tensor] | None = None,
+                                input_scale: Sequence[torch.Tensor | None] | None = None) -> List[torch.Tensor]:
     """Every rank's output of the routed all-to-all, as the composition that defines it: rank q sends
     ``inputs[q].index_select(0, input_index[q])`` (rows of ``row`` elements; ``None``: the input
     itself), ``all_to_all_reference`` exchanges the rows (``counts[q][r]`` elements, whole rows), and
     rank r writes what it receives with ``index_copy_(0, output_index[r], ...)`` into a copy of
-    ``outputs[r]`` (``None``: the received rows are the output). Outputs are flat."""
+    ``outputs[r]`` (``None``: the received rows are the output). Outputs are flat.
+    ``input_scale[q]`` (fp32, one entry per ``input_index[q]`` entry; ``None``: unscaled) scales the
+    selected rows first: ``(selected.float() * input_scale[q][:, None]).to(dtype)``, one fp32 multiply
+    rounded to nearest even in the dtype."""
     W = len(inputs)
     send = []
     for q in range(W):
         x = inputs[q].detach().cpu().reshape(-1, row)
         ix = input_index[q]
-        send.append((x if ix is None else x.index_select(0, ix.cpu())).reshape(-1))
+        sel = x if ix is None else x.index_select(0, ix.cpu())
+        sc = None if input_scale is None else input_scale[q]
+        if sc is not None:
+            sel = (sel.float() * sc.detach().cpu().float()[:, None]).to(x.dtype)
+        send.append(sel.reshape(-1))
     recv = all_to_all_reference(send, counts, bits=bits, bucket_size=bucket_size)
     outs = []
     for r in range(W):
@@ -861,6 +869,34 @@ def combine_rows_reference(slots: torch.Tensor, gate: torch.Tensor) -> torch.Ten
     for c in range(1, k):
         acc = _fma32_np(g[:, c, None], x[:, c], acc)
     return torch.from_numpy(np.ascontiguousarray(acc, dtype=_F32)).to(slots.dtype)
+
+
+def combine_gate_grad_reference(grad_out: torch.Tensor, slots: torch.Tensor) -> torch.Tensor:
+    """The gate gradient of the weighted top-k combine in the order of ``combine_gate_grad_kernel``:
+    ``grad_out`` ``[T, H]``, ``slots`` ``[T*k, H]`` of one float dtype; returns fp32 ``[T, k]`` with
+    ``out[t, c] = sum_h float(grad_out[t, h]) * float(slots[t*k + c, h])``, summed as follows. With
+    ``V = 16 // element_size``, element ``h`` belongs to lane ``l = (h // V) % 32``; every lane starts
+    at ``+0`` and runs ``acc = fma(go_h, x_h, acc)`` (``_fma32_np``, one rounding) over its elements
+    in increasing ``h``; then ``acc += acc[lane ^ m]`` in fp32 for ``m = 16, 8, 4, 2, 1``, which leaves
+    the same value in every lane."""
+    T = grad_out.shape[0]
+    V = 16 // grad_out.element_size()
+    go = grad_out.detach().cpu().float().reshape(T, 1, -1).numpy()
+    H = go.shape[-1]
+    x = slots.detach().cpu().float().reshape(T, -1, H).numpy()
+    k = x.shape[1]
+    acc = np.zeros((T, k, 32), dtype=_F32)
+    lanes = np.arange(32)
+    # step j of every lane: its (j // V)-th group of V elements, element j % V of it
+    for j in range((H + 32 * V - 1) // (32 * V) * V):
+        h = ((j // V) * 32 + lanes) * V + j % V
+        ok = h < H
+        hc = np.where(ok, h, 0)
+        acc = np.where(ok, _fma32_np(go[:, :, hc], x[:, :, hc], acc), acc).astype(_F32)
+    with np.errstate(all="ignore"):
+        for m in (16, 8, 4, 2, 1):
+            acc = (acc + acc[:, :, lanes ^ m]).astype(_F32)
+    return torch.from_numpy(np.ascontiguousarray(acc[:, :, 0]))
 
 
 def routed_all_to_all_combine_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],

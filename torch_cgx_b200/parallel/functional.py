@@ -261,7 +261,7 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
                       input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8, bucket_size: int = 512,
                       group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
                       input_index: Optional[torch.Tensor] = None, output_index: Optional[torch.Tensor] = None,
-                      output_scales: Optional[torch.Tensor] = None):
+                      output_scales: Optional[torch.Tensor] = None, input_scale: Optional[torch.Tensor] = None):
     """Compressed ``dist.all_to_all_single`` on a ``cgx`` group.
 
     Splits count dim-0 rows (``None``: equal splits). Rows ``input_split_sizes[q]`` of ``input`` go
@@ -301,6 +301,16 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     its rounding to the input dtype. The own chunk is encoded too, with the peers' encoder. The index
     keywords route codes and scales rows alike. Not differentiable.
 
+    Scaled rows on send, for the backward of an MoE combine: with ``input_index``, ``input_scale``
+    (a contiguous CUDA float32 vector, one entry per ``input_index`` entry) makes sent row i
+    ``(input[input_index[i]].float() * input_scale[i]).to(input.dtype)``: one fp32 multiply, rounded
+    to nearest even (fp32 input: no second rounding). The call then behaves exactly like the routed
+    call on those rows (quantization, stochastic rounding, every ``bits``, ``output_index``, the own
+    chunk copied bit for bit as scaled). NaN, Inf, zero and negative scales follow from that
+    arithmetic. ``ValueError`` before anything is sent without ``input_index``, for a scale of the
+    wrong dtype, device, layout or length, with ``output_scales``, or for a scale overlapping
+    ``output``.
+
     As with NCCL, the splits are the caller's contract: rank q's ``input_split_sizes[r]`` must equal
     rank r's ``output_split_sizes[q]``. Malformed splits on one rank (wrong length, sum or sign, or
     rows of another size than the output's) raise ``RuntimeError`` before anything is launched.
@@ -310,6 +320,8 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     from .hooks import _native_backend
 
     bits = _a2a_bits(bits, stochastic)
+    if input_scale is not None:
+        _check_input_scale(output, input, input_index, input_scale, output_scales)
     if output_scales is not None:
         _check_codes_output(output, input, output_scales, bits, int(bucket_size))
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
@@ -317,11 +329,31 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
         raise RuntimeError("cgx.all_to_all_single needs a process group with the cgx backend")
     work = native.all_to_all_compressed(output, input, _splits(output_split_sizes), _splits(input_split_sizes),
                                         bits, int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
-                                        input_index, output_index, output_scales)
+                                        input_index, output_index, output_scales, None, None, input_scale)
     if async_op:
         return work
     work.wait()  # the current stream waits for the kernel; the host does not
     return None
+
+
+def _check_input_scale(output: torch.Tensor, input: torch.Tensor, input_index: Optional[torch.Tensor],
+                       scale: torch.Tensor, output_scales: Optional[torch.Tensor]) -> None:
+    """ValueError unless ``scale`` can be the ``input_scale`` of ``all_to_all_single``; the checks that
+    need no GPU come first, the device check last."""
+    api = "cgx.all_to_all_single"
+    if input_index is None:
+        raise ValueError(f"{api}: input_scale needs an input_index (one scale per sent row)")
+    if output_scales is not None:
+        raise ValueError(f"{api}: input_scale has no codes output (output_scales)")
+    n = int(input_index.shape[0]) if input_index.dim() == 1 else -1
+    if scale.dtype != torch.float32 or scale.dim() != 1 or not scale.is_contiguous() or scale.shape[0] != n:
+        raise ValueError(f"{api}: input_scale must be a contiguous float32 vector of one entry per input_index "
+                         f"entry ({n}), got {scale.dtype} {list(scale.shape)}"
+                         f"{'' if scale.is_contiguous() else ' (not contiguous)'}")
+    if _overlaps(scale, output):
+        raise ValueError(f"{api}: input_scale overlaps the output")
+    if not scale.is_cuda or scale.device != input.device:
+        raise ValueError(f"{api}: input_scale must be on the input's CUDA device, got {scale.device}")
 
 
 def _check_codes_format(api: str, output: torch.Tensor, bits: A2aBits) -> None:
@@ -549,7 +581,7 @@ def all_to_all_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Te
 class _AllToAllCombine(torch.autograd.Function):
     @staticmethod
     def forward(ctx, input, gate, output_index, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size,
-                group, stochastic):
+                group, stochastic, gate_grad):
         input, gate = input.contiguous(), gate.contiguous()
         T, k = gate.shape
         slots = input.new_empty((T * k,) + tuple(input.shape[1:]))
@@ -560,6 +592,7 @@ class _AllToAllCombine(torch.autograd.Function):
         ctx.splits = (output_split_sizes, input_split_sizes)
         ctx.grad_bits, ctx.bucket_size, ctx.group, ctx.stochastic = grad_bits, bucket_size, group, stochastic
         ctx.in_shape = input.shape
+        ctx.gate_grad = gate_grad
         return out
 
     @staticmethod
@@ -568,30 +601,49 @@ class _AllToAllCombine(torch.autograd.Function):
         out_splits, in_splits = ctx.splits
         T, k = gate.shape
         grad = grad.contiguous()
-        g2 = grad.reshape(T, 1, -1)
-        grad_slots = (g2 * gate.unsqueeze(-1)).to(grad.dtype).reshape((T * k,) + tuple(grad.shape[1:]))
         gin = grad.new_empty(ctx.in_shape)
-        all_to_all_single(gin, grad_slots, in_splits, out_splits, bits=ctx.grad_bits, bucket_size=ctx.bucket_size,
-                          group=ctx.group, stochastic=ctx.stochastic, input_index=output_index)
-        grad_gate = (g2.float() * slots.reshape(T, k, -1).float()).sum(-1)
-        return gin, grad_gate, None, None, None, None, None, None, None, None
+        # slot t*k + c goes back as grad[t] * gate[t, c], rounded to the dtype: scaled rows on send
+        work = all_to_all_single(gin, grad, in_splits, out_splits, bits=ctx.grad_bits, bucket_size=ctx.bucket_size,
+                                 group=ctx.group, async_op=True, stochastic=ctx.stochastic,
+                                 input_index=torch.div(output_index, k, rounding_mode="floor"),
+                                 input_scale=gate.reshape(-1)[output_index])
+        # on the caller's stream, while the exchange runs on the group's
+        if ctx.gate_grad == "fused":
+            from .. import _C
+
+            grad_gate = _C.combine_gate_grad(grad, slots, k)
+        else:
+            grad_gate = (grad.reshape(T, 1, -1).float() * slots.reshape(T, k, -1).float()).sum(-1)
+        work.wait()
+        return gin, grad_gate, None, None, None, None, None, None, None, None, None
 
 
 def differentiable_all_to_all_combine(input: torch.Tensor, gate: torch.Tensor, output_index: torch.Tensor,
                                       output_split_sizes: Optional[Sequence[int]] = None,
                                       input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8,
                                       grad_bits: Optional[A2aBits] = None, bucket_size: int = 512, group=None,
-                                      stochastic: bool = False) -> torch.Tensor:
+                                      stochastic: bool = False, gate_grad: str = "torch") -> torch.Tensor:
     """``all_to_all_combine`` that returns its ``[T, ...]`` output and has a backward pass, for the
     combine of an MoE layer. The gradients, from the slots the forward received:
-      - input: ``grad_out[t] * gate[t, c]`` (in the dtype) for every slot ``t*k + c``, sent back by the
-        routed ``all_to_all_single`` (``input_index=output_index``, splits swapped) at ``grad_bits``
-        (``None``: ``bits``);
-      - gate: ``sum_h grad_out[t, h] * slots[t*k + c, h]`` in fp32.
+      - input: ``grad_out[t] * gate[t, c]`` (one fp32 multiply, rounded to the dtype) for every slot
+        ``t*k + c``, sent back by the routed ``all_to_all_single`` with ``input_index=output_index // k``
+        and ``input_scale=gate.view(-1)[output_index]`` (splits swapped) at ``grad_bits`` (``None``:
+        ``bits``), so no ``[T*k, ...]`` gradient is materialized;
+      - gate: ``sum_h grad_out[t, h] * slots[t*k + c, h]`` in fp32. ``gate_grad="torch"`` computes it
+        with torch's reduction, in torch's order. ``gate_grad="fused"`` reads ``grad_out`` and the slots
+        once in one kernel, in a fixed order (DESIGN §2.13e): lane ``l = (h // V) % 32`` of a warp
+        (``V`` = 16 bytes of the dtype) runs ``acc = fma(grad_out[t, h], slots[t*k + c, h], acc)`` from
+        ``+0`` over its ``h`` in increasing order, then the 32 partial sums are added by an xor
+        butterfly (16, 8, 4, 2, 1). The two differ in the last bits; any other value raises
+        ``ValueError`` before the forward sends.
+    The gate gradient runs on the caller's stream while the input gradient's exchange runs.
     """
+    if gate_grad not in ("torch", "fused"):
+        raise ValueError(f"cgx.differentiable_all_to_all_combine: gate_grad must be 'torch' or 'fused', got "
+                         f"{gate_grad!r}")
     bits = _a2a_bits(bits, stochastic)
     gb = _a2a_bits(bits if grad_bits is None else grad_bits, stochastic)
     return _AllToAllCombine.apply(input, gate, output_index,
                                   None if output_split_sizes is None else _splits(output_split_sizes),
                                   None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
-                                  int(bucket_size), group, bool(stochastic))
+                                  int(bucket_size), group, bool(stochastic), gate_grad)
