@@ -47,6 +47,7 @@ SOURCES = [
     "kernels/a2a_f32.cu",
     "kernels/a2a_f16.cu",
     "kernels/a2a_bf16.cu",
+    "kernels/a2a_remote.cu",
     "kernels/sra_dispatch.cu",
     "kernels/item_kernels.cu",
     "kernels/combine_rows.cu",

@@ -431,6 +431,88 @@ void py_all_to_all_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
                       make_rng(stochastic, seed, seq), output_scales ? &scales : nullptr);
 }
 
+// The cross-node all-to-all's buffers for world rank `rank` with nodes of `local_size` ranks
+// (a2a_remote_params): counts[q] elements for or from rank q; returns (record bytes per rank,
+// region offset per rank, buffer bytes).
+// a2a_remote_params after checking its arguments; returns the buffer's bytes
+int64_t remote_params(A2aRemoteParams& p, const std::vector<int64_t>& counts, int rank, int local_size,
+                      const A2aBits& wb, int64_t bucket, int dtype, const char* what,
+                      std::vector<uint64_t>* wire = nullptr, std::vector<uint64_t>* region = nullptr) {
+  TORCH_CHECK(local_size >= 1 && !counts.empty() && (int64_t)counts.size() <= kA2aMaxWorld &&
+                  counts.size() % (size_t)local_size == 0 && rank >= 0 && rank < (int)counts.size(),
+              what, ": 1..", kA2aMaxWorld, " counts, a multiple of local_size, and a rank among them");
+  TORCH_CHECK(bucket >= 1, what, ": bucket_size must be >= 1");
+  for (int64_t n : counts) TORCH_CHECK(n >= 0 && n < (1ll << 32), what, ": counts must be in [0, 2^32)");
+  std::vector<uint64_t> c(counts.begin(), counts.end()), w, r;
+  return (int64_t)a2a_remote_params(p, c, rank, local_size, dtype, wb.bits, wb.codec, (uint32_t)bucket,
+                                    wire ? wire : &w, region ? region : &r);
+}
+
+std::tuple<std::vector<int64_t>, std::vector<int64_t>, int64_t> py_a2a_remote_wire(const std::vector<int64_t>& counts,
+                                                                                   int rank, int local_size,
+                                                                                   const A2aBitsArg& bits, int64_t bucket,
+                                                                                   int dtype) {
+  auto p = std::make_unique<A2aRemoteParams>();
+  std::vector<uint64_t> wire, region;
+  const int64_t total =
+      remote_params(*p, counts, rank, local_size, a2a_bits(bits, false), bucket, dtype, "a2a_remote_wire", &wire, &region);
+  return {std::vector<int64_t>(wire.begin(), wire.end()), std::vector<int64_t>(region.begin(), region.end()), total};
+}
+
+// One launch of the pack (a2a_pack) or unpack kernel on the current stream, as the engine launches
+// it for world rank `rank` (a2a_remote_params): pack quantizes every chunk of `input` for a rank of
+// another node into the returned buffer (or `out`); unpack decodes `records` (such a buffer) into
+// those chunks' rows of `output`, or with output_scales unpacks their codes and units.
+at::Tensor py_a2a_pack(const at::Tensor& input, const std::vector<int64_t>& counts, int rank, int local_size,
+                       const A2aBitsArg& bits, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
+                       const std::optional<at::Tensor>& out) {
+  const A2aBits wb = a2a_bits(bits, stochastic);
+  TORCH_CHECK(input.is_cuda() && input.is_contiguous(), "a2a_pack: a contiguous CUDA input");
+  TORCH_CHECK(wb.bits < kRawBits, "a2a_pack: raw chunks travel as their bytes, nothing is packed");
+  const int dt = cgx_dtype(input);
+  int64_t n = 0;
+  for (int64_t c : counts) n += c;
+  TORCH_CHECK(input.numel() == n, "a2a_pack: the input holds ", input.numel(), " elements, the counts ", n);
+  auto p = std::make_unique<A2aRemoteParams>();
+  const int64_t total = remote_params(*p, counts, rank, local_size, wb, bucket, dt, "a2a_pack");
+  at::Tensor buf = out ? *out : at::zeros({total + 16}, input.options().dtype(at::kByte));
+  TORCH_CHECK(buf.is_cuda() && buf.is_contiguous() && buf.scalar_type() == at::kByte && buf.numel() >= total,
+              "a2a_pack: out must be a contiguous CUDA uint8 tensor of at least ", total, " bytes");
+  c10::cuda::CUDAGuard g(input.device());
+  p->in = input.data_ptr();
+  p->out = buf.data_ptr();
+  p->rng = make_rng_key(make_rng(stochastic, seed, seq), rank, 0);
+  cuda_check(launch_a2a_pack(*p, c10::cuda::getCurrentCUDAStream().stream()), "launch_a2a_pack");
+  return buf;
+}
+
+void py_a2a_unpack(const at::Tensor& records, at::Tensor output, const std::vector<int64_t>& counts, int rank,
+                   int local_size, const A2aBitsArg& bits, int64_t bucket, const std::optional<at::Tensor>& output_scales) {
+  const A2aBits wb = a2a_bits(bits, false);
+  TORCH_CHECK(wb.bits < kRawBits, "a2a_unpack: raw chunks travel as their bytes, nothing is unpacked");
+  TORCH_CHECK(records.is_cuda() && records.is_contiguous() && records.scalar_type() == at::kByte,
+              "a2a_unpack: records must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(output.is_cuda() && output.is_contiguous(), "a2a_unpack: a contiguous CUDA output");
+  const bool codes = output_scales.has_value();
+  TORCH_CHECK(!codes || (wb.codec != kMaxMin && output_scales->is_cuda() && output_scales->is_contiguous() &&
+                         output_scales->scalar_type() == at::kFloat),
+              "a2a_unpack: output_scales needs an FP8 bits and a contiguous CUDA float32 tensor");
+  // a codes output has no element type of the sender's: any dtype gives the same records, since the
+  // record bytes of compressed (8-bit) blocks do not depend on the element size (block_wire_bytes)
+  const int dt = codes ? kF32 : cgx_dtype(output);
+  auto p = std::make_unique<A2aRemoteParams>();
+  const int64_t total = remote_params(*p, counts, rank, local_size, wb, bucket, dt, "a2a_unpack");
+  int64_t n = 0;
+  for (int64_t x : counts) n += x;
+  TORCH_CHECK(output.numel() == n, "a2a_unpack: the output holds ", output.numel(), " elements, the counts ", n);
+  TORCH_CHECK(records.numel() >= total, "a2a_unpack: records hold ", records.numel(), " bytes, need ", total);
+  c10::cuda::CUDAGuard g(output.device());
+  p->in = records.data_ptr();
+  p->out = output.data_ptr();
+  p->out_scales = codes ? output_scales->data_ptr<float>() : nullptr;
+  cuda_check(launch_a2a_unpack(*p, c10::cuda::getCurrentCUDAStream().stream()), "launch_a2a_unpack");
+}
+
 // the items of one chunk from common/a2a.h, rows as in plan_to_dict, offsets in the contiguous image
 at::Tensor py_a2a_items(int64_t n, int bits, int64_t bucket, int dtype) {
   const A2aGeom g = a2a_geom((uint32_t)n, bits, (uint32_t)bucket, dtype_size(dtype));
@@ -1168,7 +1250,7 @@ class LocalEngineGroup {
   LocalEngineGroup(int world, int local_size, const py::dict& config, int lanes, int64_t slot_bytes,
                    int64_t timeout_ms)
       : world_(world), local_size_(local_size), nodes_(local_size >= 1 ? world / local_size : 1) {
-    TORCH_CHECK(world >= 1 && world <= kMaxPeers, "LocalEngineGroup: world must be 1..", kMaxPeers, ", got ", world);
+    TORCH_CHECK(world >= 1 && world <= kA2aMaxWorld, "LocalEngineGroup: world must be 1..", kA2aMaxWorld, ", got ", world);
     TORCH_CHECK(local_size >= 1 && world % local_size == 0, "LocalEngineGroup: local_size ", local_size,
                 " does not divide the world ", world);
     // streams r and r + 8 share a hardware queue: a rank's kernel could wait behind a peer's that spins for it
@@ -1211,6 +1293,7 @@ class LocalEngineGroup {
     for (int n = 0; n < nodes; ++n) intra_hubs_.push_back(std::make_unique<LoopbackHub>(local_size, timeout_ms));
     for (int l = 0; l < local_size; ++l) cross_hubs_.push_back(std::make_unique<LoopbackHub>(nodes, timeout_ms));
     world_hub_ = std::make_unique<LoopbackHub>(world, timeout_ms);
+    a2a_hub_ = std::make_unique<LoopbackHub>(world, timeout_ms);
     for (int r = 0; r < world; ++r) {
       auto e = std::make_unique<AllreduceEngine>(r, world, cfg);
       e->set_topology(local_size);
@@ -1220,6 +1303,8 @@ class LocalEngineGroup {
         if (nodes > 1) cross = std::make_unique<LoopbackCommunicator>(cross_hub(r), e->node(), cuda);
         e->attach_generic(cuda, std::move(intra), std::move(cross));
       }
+      // the all-to-all's cross-node exchange, as the process group's CUDA delegate carries it
+      if (nodes > 1) e->attach_world(true, std::make_unique<LoopbackCommunicator>(a2a_hub_.get(), r, true));
       engines_.push_back(std::move(e));
       observers_.push_back(std::make_unique<Observer>(this, r));
       engines_[r]->set_observer(observers_[r].get());
@@ -1331,6 +1416,70 @@ class LocalEngineGroup {
     });
   }
 
+  // inputs[r] / outputs[r]: rank r's compressed all-to-all (AllreduceEngine::all_to_all), counts[q][r]
+  // elements from rank q to rank r; with output_scales (an FP8 `bits`) the codes output. A call's
+  // stochastic streams use the sequence number the engine gives it, which log(r) reports on several
+  // nodes. Routed forms (any of input_index, output_index, input_scale, gate with combine_out given
+  // for some rank; tensors of rows of `row` elements, the counts those of the logical buffers) run
+  // as the process group runs them when the fused kernel does not route the rows: a2a_compose.
+  void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
+                  const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed,
+                  const std::optional<std::vector<at::Tensor>>& output_scales, const IndexList& input_index,
+                  const IndexList& output_index, const IndexList& input_scale, const IndexList& gate,
+                  const IndexList& combine_out, int64_t row) {
+    const A2aBits wb = a2a_bits(bits_arg, stochastic);
+    const auto counts = check_counts(counts_in, (size_t)world_);
+    TORCH_CHECK((int)inputs.size() == world_ && (int)outputs.size() == world_,
+                "LocalEngineGroup: one input and one output per virtual rank");
+    const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
+    const RngParams rng = make_rng(stochastic, seed, 0);
+    auto opt = [&](const IndexList& l, int r) {
+      TORCH_CHECK(l.empty() || (int)l.size() == world_, "LocalEngineGroup: one entry per virtual rank or none");
+      return l.empty() || !l[r] ? at::Tensor() : *l[r];
+    };
+    bool routed = false;
+    for (const IndexList* l : {&input_index, &output_index, &input_scale, &gate, &combine_out})
+      for (const auto& t : *l) routed |= t.has_value();
+    if (!routed) {
+      check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda(), output_scales ? wb.codec : kMaxMin);
+      run(inputs,
+          [&](AllreduceEngine& e, int r, void* in, int dt, int64_t, bool cuda, cudaStream_t s) {
+            std::vector<uint64_t> out_counts(world_);
+            for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
+            e.all_to_all(cuda, in, outputs[r].data_ptr(), counts[r], out_counts, dt, wb.bits, wb.codec,
+                         (uint32_t)bucket, rng, s, nullptr, scales.empty() ? nullptr : scales[r]);
+          },
+          false);
+      return;
+    }
+    TORCH_CHECK(row >= 1, "LocalEngineGroup: row must be >= 1");
+    for (int r = 0; r < world_; ++r) {
+      uint64_t nin = 0, nout = 0;
+      for (int q = 0; q < world_; ++q) {
+        nin += counts[r][q];
+        nout += counts[q][r];
+      }
+      const at::Tensor ii = opt(input_index, r), oi = opt(output_index, r);
+      TORCH_CHECK(inputs[r].is_cuda() && outputs[r].is_cuda() && inputs[r].dim() == 2 && outputs[r].dim() == 2 &&
+                      inputs[r].size(1) == row && outputs[r].size(1) == row,
+                  "LocalEngineGroup: routed calls take CUDA tensors [rows, row]");
+      TORCH_CHECK((uint64_t)(ii.defined() ? ii.numel() : inputs[r].size(0)) * (uint64_t)row == nin &&
+                      (uint64_t)(oi.defined() ? oi.numel() : outputs[r].size(0)) * (uint64_t)row == nout,
+                  "all_to_all: rank ", r, "'s tensors do not match its row and column of the counts");
+    }
+    run(inputs,
+        [&](AllreduceEngine& e, int r, void*, int dt, int64_t, bool, cudaStream_t s) {
+          std::vector<uint64_t> out_counts(world_);
+          for (int q = 0; q < world_; ++q) out_counts[q] = counts[q][r];
+          c10::cuda::CUDAStreamGuard sg(streams_[r]);
+          const at::Tensor sc = scales.empty() ? at::Tensor() : (*output_scales)[r].view({outputs[r].size(0), -1});
+          a2a_compose(e, inputs[r], outputs[r], counts[r], out_counts, dt, wb.bits, wb.codec, (uint32_t)bucket, rng,
+                      opt(input_index, r), opt(output_index, r), opt(input_scale, r), sc, opt(gate, r),
+                      opt(combine_out, r), s);
+        },
+        false);
+  }
+
   py::dict stats(int r) const {
     TORCH_CHECK(r >= 0 && r < world_, "LocalEngineGroup: bad rank ", r);
     const EngineStats& s = engines_[r]->stats();
@@ -1395,12 +1544,25 @@ class LocalEngineGroup {
     }
     void stage(const EngineStage& s) override {
       static const char* kNames[] = {"oneshot", "sra",     "generic_intra", "cross",      "bcast_compressed", "bcast_raw",
-                                     "rs",      "ag",      "generic_rs",    "generic_ag", "cross_rs",         "cross_ag"};
+                                     "rs",      "ag",      "generic_rs",    "generic_ag", "cross_rs",         "cross_ag",
+                                     "a2a_cross", "a2a_intra"};
       // A sharded call over several nodes runs fused launches next to generic stages, whose
       // cudaMalloc / cudaFree can wait for a fused kernel of another node that spins for a peer the
       // same driver call holds up. Every rank issues the same sharded stages, so before each of them
       // all ranks drain their streams and meet: no fused kernel runs while a generic stage does.
-      if (s.sharded() && group->nodes_ > 1) {
+      if (s.a2a() && group->nodes_ > 1) {
+        // The all-to-all's node-local stages run one node at a time, in node order: with more than
+        // eight ranks two nodes' spinning kernels can share hardware queues, each behind the other.
+        // Node n meets n + 1 times before its stage (round 0 drains the pack) and N - n times after it,
+        // once its stream has drained; round t lets node t start after node t - 1 has finished.
+        const int n = rank / group->local_size_, N = group->nodes_;
+        const int rounds = s.kind == EngineStage::kA2aIntra ? n + 1 : N - n;
+        for (int t = 0; t < rounds; ++t) {
+          if (group->call_cuda_ && (t == 0 || s.kind == EngineStage::kA2aIntra))
+            cuda_check(cudaStreamSynchronize(group->streams_[rank].stream()), "LocalEngineGroup: quiesce");
+          group->world_hub_->barrier(rank);
+        }
+      } else if (s.sharded() && group->nodes_ > 1) {
         if (group->call_cuda_)
           cuda_check(cudaStreamSynchronize(group->streams_[rank].stream()), "LocalEngineGroup: quiesce");
         group->world_hub_->barrier(rank);
@@ -1446,19 +1608,21 @@ class LocalEngineGroup {
     for (auto& h : intra_hubs_) h->fail(msg);
     for (auto& h : cross_hubs_) h->fail(msg);
     world_hub_->fail(msg);
+    a2a_hub_->fail(msg);
   }
 
   // op(engine, rank, data, dtype, numel, cuda, stream) on every rank's thread; every rank's stream is
   // synchronised before this returns, and the first failure of any rank is raised
+  // (same_size false: the tensors may differ in size)
   template <class F>
-  void run(const std::vector<at::Tensor>& tensors, F&& op) {
+  void run(const std::vector<at::Tensor>& tensors, F&& op, bool same_size = true) {
     const int W = world_;
     TORCH_CHECK((int)tensors.size() == W, "LocalEngineGroup: need one tensor per virtual rank (", W, "), got ",
                 tensors.size());
     const int dt = cgx_dtype(tensors[0]);
     const bool cuda = tensors[0].is_cuda();
     for (const at::Tensor& t : tensors)
-      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && t.numel() == tensors[0].numel() &&
+      TORCH_CHECK(t.is_contiguous() && cgx_dtype(t) == dt && (!same_size || t.numel() == tensors[0].numel()) &&
                       t.device() == tensors[0].device(),
                   "LocalEngineGroup: contiguous tensors of one dtype, size and device");
     TORCH_CHECK(cuda || tensors[0].device().is_cpu(), "LocalEngineGroup: CPU or CUDA tensors");
@@ -1477,6 +1641,7 @@ class LocalEngineGroup {
     for (auto& h : intra_hubs_) h->reset(false);
     for (auto& h : cross_hubs_) h->reset(false);
     world_hub_->reset(false);
+    a2a_hub_->reset(false);
     call_cuda_ = cuda;
     for (auto& o : observers_) o->log.clear();
     const int64_t n = tensors[0].numel();
@@ -1502,6 +1667,7 @@ class LocalEngineGroup {
           intra_hub(r)->finish(engines_[r]->local_rank());
           cross_hub(r)->finish(engines_[r]->node());
           world_hub_->finish(r);
+          a2a_hub_->finish(r);
         });
       for (auto& t : threads) t.join();
       // a rank that threw skipped its own synchronise: nothing it queued may run on after this returns
@@ -1515,6 +1681,7 @@ class LocalEngineGroup {
     for (auto& h : intra_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
     for (auto& h : cross_hubs_) TORCH_CHECK(!h->failed(), "LocalEngineGroup: ", h->failure());
     TORCH_CHECK(!world_hub_->failed(), "LocalEngineGroup: ", world_hub_->failure());
+    TORCH_CHECK(!a2a_hub_->failed(), "LocalEngineGroup: ", a2a_hub_->failure());
     if (cuda) check();
   }
 
@@ -1524,6 +1691,7 @@ class LocalEngineGroup {
   HeapLayout layout_{};
   std::vector<std::unique_ptr<LoopbackHub>> intra_hubs_, cross_hubs_;
   std::unique_ptr<LoopbackHub> world_hub_;  // barriers of every rank (Observer::stage)
+  std::unique_ptr<LoopbackHub> a2a_hub_;    // the all-to-all's cross-node exchange
   std::vector<std::unique_ptr<AllreduceEngine>> engines_;  // after the hubs: released first
   std::vector<std::unique_ptr<Observer>> observers_;
   std::vector<c10::cuda::CUDAStream> streams_;
@@ -1969,6 +2137,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         return std::make_tuple(wb.bits, (int)wb.codec);
       },
       py::arg("bits"), py::arg("stochastic") = false, py::arg("op") = "all_to_all");
+  m.def("a2a_rng_stream", [](int src, int dst) { return (int64_t)a2a_rng_stream(src, dst); }, py::arg("src"),
+        py::arg("dst"));
+  m.attr("A2A_MAX_WORLD") = (int64_t)kA2aMaxWorld;
+  m.def("a2a_remote_wire", &py_a2a_remote_wire, py::arg("counts"), py::arg("rank"), py::arg("local_size"),
+        py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
+  m.def("a2a_pack", &py_a2a_pack, py::arg("input"), py::arg("counts"), py::arg("rank"), py::arg("local_size"),
+        py::arg("bits"), py::arg("bucket_size"), py::arg("stochastic") = false, py::arg("seed") = 0,
+        py::arg("seq") = 0, py::arg("out") = py::none());
+  m.def("a2a_unpack", &py_a2a_unpack, py::arg("records"), py::arg("output"), py::arg("counts"), py::arg("rank"),
+        py::arg("local_size"), py::arg("bits"), py::arg("bucket_size"), py::arg("output_scales") = py::none());
   m.def("a2a_items", &py_a2a_items, py::arg("numel"), py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);
   m.def(
       "a2a_rows_fit",
@@ -2160,6 +2338,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            },
            py::arg("inputs"), py::arg("outputs"), py::arg("shard_layers") = py::none(), py::arg("bits") = py::none(),
            py::arg("output_scales") = py::none())
+      .def("all_to_all", &LocalEngineGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
+           py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
+           py::arg("output_scales") = py::none(), py::arg("input_index") = IndexList{},
+           py::arg("output_index") = IndexList{}, py::arg("input_scale") = IndexList{}, py::arg("gate") = IndexList{},
+           py::arg("combine_out") = IndexList{}, py::arg("row") = 1)
       .def("stats", &LocalEngineGroup::stats, py::arg("rank"))
       .def("check", &LocalEngineGroup::check)
       .def("log", &LocalEngineGroup::log, py::arg("rank"))

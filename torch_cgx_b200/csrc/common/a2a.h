@@ -75,6 +75,12 @@ CGX_HD uint64_t a2a_chunk_wire(const A2aGeom& g) {
   return (uint64_t)(nb - 1u) * g.block_wire + block_wire_bytes(a2a_block_n(g, nb - 1u), g.bits, g.bucket, g.elsize);
 }
 
+// warp items of the whole chunk
+CGX_HD uint32_t a2a_chunk_items(const A2aGeom& g) {
+  const uint32_t nb = a2a_num_blocks(g);
+  return nb == 0 ? 0u : (nb - 1u) * g.block_items + a2a_block_num_items(g, a2a_block_n(g, nb - 1u));
+}
+
 // Item j of block b. elem_off counts from the chunk's first element; meta_off / pay_off count from
 // the block's record, which starts at b * block_wire in the chunk's contiguous wire image.
 CGX_HD WarpItem a2a_block_item(const A2aGeom& g, uint32_t b, uint32_t j) {
@@ -146,8 +152,21 @@ CGX_HD uint32_t a2a_lane_windows(const A2aGeom& g, int lane, int lanes, uint32_t
   return div_up(a2a_lane_blocks(a2a_num_blocks(g), lane, lanes), bpw);
 }
 
-// Random stream of the chunk rank `src` sends to rank `dst`: every pair has its own, and the
-// counters are the chunk's element indices.
-CGX_HD uint32_t a2a_rng_stream(int src, int dst) { return 2u * (uint32_t)(src * kMaxPeers + dst); }
+// Largest world of an all-to-all: a2a_rng_stream keeps every pair of ranks below it apart.
+constexpr int kA2aMaxWorld = 256;
+
+// Random stream of the chunk world rank `src` sends to world rank `dst`: every pair has its own,
+// and the counters are the chunk's element indices. The low parts of the ranks (mod 16) give the
+// stream word's bits 0..8, exactly 2 * (src * 16 + dst) below 16 ranks; the high parts (src / 16,
+// dst / 16, four bits each) go to bits 9..16. rounding_bits multiplies the word by an odd constant
+// into the Philox key, a bijection, so distinct words are distinct keys.
+CGX_HD uint32_t a2a_rng_stream(int src, int dst) {
+  const uint32_t s = (uint32_t)src, d = (uint32_t)dst, P = (uint32_t)kMaxPeers;
+  return 2u * ((s % P) * P + d % P) | (((s / P) | (d / P) << 4) << 9);
+}
+
+// Bytes of a chunk's region in the send or receive buffer of the cross-node all-to-all (and of
+// Reducer::all_to_all): its records, rounded up to 256 so every region starts 256-byte aligned.
+CGX_HD uint64_t a2a_region_bytes(uint64_t wire) { return (wire + 255u) / 256u * 256u; }
 
 }  // namespace cgx

@@ -68,6 +68,9 @@ AllreduceEngine::AllreduceEngine(int rank, int world, const EngineConfig& cfg)
 AllreduceEngine::~AllreduceEngine() {
   // reducers release their scratch through the block backend: they must go first
   for (GenericPath* g : {&gen_cuda_, &gen_cpu_}) {
+    for (GenericPath::Buf* b : {&g->a2a_send, &g->a2a_recv})
+      if (b->p) g->ops->release(b->p);
+    g->world_comm.reset();
     g->self.reset();
     g->self_comm.reset();
     g->cross.reset();
@@ -97,6 +100,14 @@ void AllreduceEngine::attach_generic(bool cuda, std::unique_ptr<Communicator> in
   g.cross_comm = std::move(cross);
   if (g.intra_comm) g.intra = make_reducer(cfg_.inner_reduction, g.intra_comm.get(), g.ops.get());
   if (g.cross_comm) g.cross = make_reducer(cfg_.cross_reduction, g.cross_comm.get(), g.ops.get());
+}
+
+void AllreduceEngine::attach_world(bool cuda, std::unique_ptr<Communicator> world) {
+  GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  if (!g.ops) throw std::logic_error("cgx: attach_world needs attach_generic first");
+  if (world && (world->size() != world_ || world->rank() != rank_))
+    throw std::invalid_argument("cgx: the world communicator must span the world, with this rank's world rank");
+  g.world_comm = std::move(world);
 }
 
 size_t AllreduceEngine::required_oneshot_slot_bytes(const EngineConfig& cfg) {
@@ -358,14 +369,27 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
                                  const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
                                  uint32_t bucket, const RngParams& rng_in, cudaStream_t stream,
                                  const A2aRoute* route, float* out_scales) {
-  if (nodes() > 1)
-    throw std::runtime_error("cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE " +
-                             std::to_string(local_size_) + " < world size " + std::to_string(world_) + ")");
   GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
   const bool fused = fused_sharded(cuda);
   if (fused) fused_->check_status();
-  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route, out_scales);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);
+  if (nodes() > 1) {
+    // every rank evaluates the same conditions, so every rank refuses and none is left waiting
+    if (world_ > kA2aMaxWorld)
+      throw std::runtime_error("cgx: the compressed all_to_all supports at most " + std::to_string(kA2aMaxWorld) +
+                               " ranks, got " + std::to_string(world_));
+    if (!cuda) throw std::runtime_error("cgx: the compressed all_to_all over several nodes needs device memory");
+    check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route, out_scales);
+    if (routed) throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
+    if (codec != kMaxMin && rng_in.stochastic)
+      throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
+    if (!g.world_comm) throw std::runtime_error("cgx: the compressed all_to_all over several nodes has no world communicator");
+    if (!fused && local_size_ > 1 && !g.intra)
+      throw std::runtime_error("cgx: the compressed all_to_all has no intra-node reducer");
+    a2a_nodes(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng_in, stream, route, out_scales);
+    return;
+  }
+  check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route, out_scales);
   if (routed && !routes_in_kernel(cuda, dtype, bits, bucket, route->row))
     throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
   if (!fused && world_ > 1 && !g.intra) throw std::runtime_error("cgx: the compressed all_to_all has no intra-node reducer");
@@ -377,15 +401,24 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
   RngParams rng = rng_in;
   rng.seq = call_seq_ << 4;
   stats_.elements += total;
-  if (fused) {
-    const FusedSra::A2aCounts n =
-        fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, route, out_scales);
+  a2a_node(cuda, in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, route, out_scales, 0);
+}
+
+void AllreduceEngine::a2a_node(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                               const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
+                               uint32_t bucket, const RngParams& rng, cudaStream_t stream, const A2aRoute* route,
+                               float* out_scales, int rank_base) {
+  GenericPath& g = cuda ? gen_cuda_ : gen_cpu_;
+  const int L = local_size_, lr = local_rank();
+  if (fused_sharded(cuda)) {
+    const FusedSra::A2aCounts n = fused_->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng,
+                                                     stream, route, out_scales, rank_base);
     stats_.kernel_launches += n.launches;
     stats_.wire_bytes += n.wire_bytes;
     stats_.raw_bytes += n.raw_bytes;
     return;
   }
-  if (world_ == 1 && out_scales != nullptr) {
+  if (L == 1 && out_scales != nullptr) {
     if (!g.ops) throw std::runtime_error("cgx: the compressed all_to_all has no block backend");
     if (!g.self) {
       g.self_comm = std::make_unique<SelfCommunicator>(cuda);
@@ -394,7 +427,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
     g.self->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, out_scales);
     return;
   }
-  if (world_ == 1) {
+  if (L == 1) {
     const size_t bytes = (size_t)in_counts[0] * (size_t)dtype_size(dtype);
     if (bytes == 0) return;
     if (cuda)
@@ -404,14 +437,129 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
     return;
   }
   const uint64_t before = g.intra->bytes_sent();
-  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, out_scales);
+  g.intra->all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rng, stream, out_scales, rank_base);
   stats_.wire_bytes += g.intra->bytes_sent() - before;
-  for (int q = 0; q < world_; ++q)
-    if (q != rank_) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);
+  for (int q = 0; q < L; ++q)
+    if (q != lr) stats_.raw_bytes += in_counts[q] * (uint64_t)dtype_size(dtype);
+}
+
+uint64_t a2a_remote_params(A2aRemoteParams& p, const std::vector<uint64_t>& counts, int rank, int L, int dtype,
+                           int bits, WireCodec codec, uint32_t bucket, std::vector<uint64_t>* wire,
+                           std::vector<uint64_t>* region) {
+  const int W = (int)counts.size();
+  const int es = dtype_size(dtype);
+  const bool raw = bits >= kRawBits;
+  std::memset(&p, 0, sizeof(p));
+  p.dtype = dtype;
+  p.bits = bits;
+  p.codec = codec;
+  p.bucket = bucket;
+  p.rank = rank;
+  wire->assign(W, 0);
+  region->assign(W, 0);
+  uint64_t off = 0, at = 0;
+  for (int q = 0; q < W; off += counts[q], ++q) {
+    if (q / L == rank / L || counts[q] == 0) continue;
+    const A2aGeom g = a2a_geom((uint32_t)counts[q], bits, bucket, es);
+    (*wire)[q] = raw ? counts[q] * (uint64_t)es : a2a_chunk_wire(g);
+    if (raw) continue;
+    (*region)[q] = at;
+    const int i = p.nchunks++;
+    p.peer[i] = q;
+    p.cnt[i] = (uint32_t)counts[q];
+    p.elem_off[i] = off;
+    p.wire_off[i] = at;
+    p.item_first[i + 1] = p.item_first[i] + a2a_chunk_items(g);
+    at += a2a_region_bytes((*wire)[q]);
+  }
+  return at;
+}
+
+// Several nodes (DESIGN §2.13f). The chunks for and from the ranks of my node are contiguous in
+// `in` and `out`: that sub-range is a one-node all-to-all among my node's ranks. Every other chunk
+// is packed into one send buffer (one 256-byte aligned region per destination, its records exactly
+// Reducer::all_to_all's), exchanged over the world communicator after the node-local stage and unpacked; at bits >= 32 the
+// chunks travel as their bytes, straight from `in` into `out`. Streams and the sequence number are
+// those of a one-node call of W ranks.
+void AllreduceEngine::a2a_nodes(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                                const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
+                                uint32_t bucket, const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route,
+                                float* out_scales) {
+  GenericPath& g = gen_cuda_;
+  const int W = world_, L = local_size_, n0 = node() * L;
+  const size_t es = (size_t)dtype_size(dtype), oes = out_scales != nullptr ? 1 : es;
+  const bool raw = bits >= kRawBits;
+  uint64_t total = 0;
+  for (uint64_t n : in_counts) total += n;
+  NvtxRange range("cgx:all_to_all_cuda", total);
+  ++call_seq_;
+  ++stats_.calls;
+  RngParams rng = rng_in;
+  rng.seq = call_seq_ << 4;
+  stats_.elements += total;
+  std::vector<uint64_t> io(W + 1, 0), oo(W + 1, 0);
+  for (int q = 0; q < W; ++q) {
+    io[q + 1] = io[q] + in_counts[q];
+    oo[q + 1] = oo[q] + out_counts[q];
+  }
+  // the remote chunks' records and their regions
+  auto pk = std::make_unique<A2aRemoteParams>();
+  auto up = std::make_unique<A2aRemoteParams>();
+  std::vector<uint64_t> sw, rw, so, ro;
+  const uint64_t send_bytes = a2a_remote_params(*pk, in_counts, rank_, L, dtype, bits, codec, bucket, &sw, &so);
+  const uint64_t recv_bytes = a2a_remote_params(*up, out_counts, rank_, L, dtype, bits, codec, bucket, &rw, &ro);
+  pk->rng = make_rng_key(rng, rank_, 0);
+  up->out_scales = out_scales;
+  auto buffer = [&](GenericPath::Buf& b, uint64_t bytes) -> uint8_t* {
+    if (b.cap < bytes) {
+      if (b.p) {
+        cuda_check(cudaStreamSynchronize(stream), "all_to_all scratch");  // an earlier call may still use it
+        g.ops->release(b.p);
+      }
+      b.cap = std::max<size_t>(bytes, b.cap * 2);
+      b.p = g.ops->alloc(b.cap);
+    }
+    return static_cast<uint8_t*>(b.p);
+  };
+  uint8_t* sendb = raw ? nullptr : buffer(g.a2a_send, send_bytes + 16);
+  uint8_t* recvb = raw ? nullptr : buffer(g.a2a_recv, recv_bytes + 16);
+  const uint8_t* src = static_cast<const uint8_t*>(in);
+  uint8_t* dst = static_cast<uint8_t*>(out);
+  if (pk->nchunks > 0) {
+    pk->in = in;
+    pk->out = sendb;
+    cuda_check(launch_a2a_pack(*pk, stream), "launch_a2a_pack");
+  }
+  static const std::vector<LayerSpec> kNoLayers;
+  std::vector<P2POp> x;
+  for (int q = 0; q < W; ++q) {
+    if (sw[q]) x.push_back({true, raw ? const_cast<uint8_t*>(src + io[q] * es) : sendb + so[q], sw[q], q});
+    if (rw[q]) x.push_back({false, raw ? dst + oo[q] * es : recvb + ro[q], rw[q], q});
+    stats_.wire_bytes += sw[q];
+    stats_.raw_bytes += in_counts[q] * es * (sw[q] != 0);
+  }
+  observe(EngineStage::kA2aIntra, &kNoLayers, rng, 1.0f);
+  {
+    NvtxRange r1("cgx:intra_node", (uint64_t)node());
+    const std::vector<uint64_t> ic(in_counts.begin() + n0, in_counts.begin() + n0 + L);
+    const std::vector<uint64_t> oc(out_counts.begin() + n0, out_counts.begin() + n0 + L);
+    a2a_node(true, src + io[n0] * es, dst + oo[n0] * oes, ic, oc, dtype, bits, codec, bucket, rng, stream, route,
+             out_scales != nullptr ? out_scales + oo[n0] / bucket : nullptr, n0);
+  }
+  observe(EngineStage::kA2aCross, &kNoLayers, rng, 1.0f);
+  {
+    NvtxRange r2("cgx:cross_node", (uint64_t)nodes());
+    g.world_comm->exchange(x, stream);
+  }
+  if (up->nchunks > 0) {
+    up->in = recvb;
+    up->out = out;
+    cuda_check(launch_a2a_unpack(*up, stream), "launch_a2a_unpack");
+  }
 }
 
 bool AllreduceEngine::routes_in_kernel(bool cuda, int dtype, int bits, uint32_t bucket, uint64_t row) const {
-  return fused_sharded(cuda) && row < (1ull << 32) && a2a_rows_fit((uint32_t)row, bits, bucket, dtype_size(dtype));
+  return nodes() == 1 && fused_sharded(cuda) && row < (1ull << 32) && a2a_rows_fit((uint32_t)row, bits, bucket, dtype_size(dtype));
 }
 
 void AllreduceEngine::allreduce_cpu(void* data, int dtype, int64_t numel, bool average, int explicit_bucket) {

@@ -17,6 +17,7 @@
 #include "../common/config.h"
 #include "../common/layers.h"
 #include "../comm/communicator.h"
+#include "../kernels/launch.h"
 #include "../reduce/block_backend.h"
 #include "../reduce/fused_sra.h"
 #include "../reduce/reducers.h"
@@ -41,11 +42,13 @@ std::vector<std::vector<LayerSpec>> split_for_fusion(const std::vector<LayerSpec
 
 // One stage of an allreduce or of a sharded collective as the engine issues it (EngineObserver::stage).
 // kRs / kAg are fused launches (one per window), kGenericRs / kGenericAg the generic intra-node
-// reducer, kCrossRs / kCrossAg the cross-node stage of a sharded call.
+// reducer, kCrossRs / kCrossAg the cross-node stage of a sharded call. An all-to-all over several
+// nodes issues kA2aIntra (the node's own chunks) and then kA2aCross (the exchange of the packed
+// remote chunks); one node issues none.
 struct EngineStage {
   enum Kind {
     kOneshot, kSra, kGenericIntra, kCross, kBcastCompressed, kBcastRaw,
-    kRs, kAg, kGenericRs, kGenericAg, kCrossRs, kCrossAg
+    kRs, kAg, kGenericRs, kGenericAg, kCrossRs, kCrossAg, kA2aCross, kA2aIntra
   };
   Kind kind;
   // the stage's layer table (a sharded stage: one shard's, or a fused launch's window of it); null
@@ -54,7 +57,8 @@ struct EngineStage {
   const DevicePlan* dp;                  // the plan of a fused launch (kOneshot / kSra / kRs / kAg), else null
   RngParams rng;                         // the sequence number the stage runs with
   float scale;                           // prescale of a reduction stage, 1 for a broadcast or an all-gather
-  bool sharded() const { return kind >= kRs; }
+  bool sharded() const { return kind >= kRs && kind <= kCrossAg; }
+  bool a2a() const { return kind >= kA2aCross; }
 };
 
 // Test seam: sees every stage an engine issues. Production engines have none (one branch per stage).
@@ -78,7 +82,24 @@ struct GenericPath {
   // codes output (nothing is exchanged)
   std::unique_ptr<Communicator> self_comm;
   std::unique_ptr<Reducer> self;
+  // all the world's ranks: the exchange of the all-to-all's cross-node chunks (null on one node)
+  std::unique_ptr<Communicator> world_comm;
+  // grow-only send and receive buffers of that exchange
+  struct Buf {
+    void* p = nullptr;
+    size_t cap = 0;
+  };
+  Buf a2a_send, a2a_recv;
 };
+
+// The parameters of the cross-node all-to-all's pack (counts: this rank's input counts) or unpack
+// (its output counts) launch for world rank `rank` with nodes of L ranks: every chunk for or from a
+// rank of another node, in rank order, its records in a 256-byte aligned region of one buffer.
+// wire[q] receives chunk q's record bytes (its bytes at bits >= 32, which launch nothing), 0 for my
+// node's ranks; region[q] its region's offset. Returns the buffer's bytes.
+uint64_t a2a_remote_params(A2aRemoteParams& p, const std::vector<uint64_t>& counts, int rank, int L, int dtype,
+                           int bits, WireCodec codec, uint32_t bucket, std::vector<uint64_t>* wire,
+                           std::vector<uint64_t>* region);
 
 class AllreduceEngine {
  public:
@@ -98,6 +119,9 @@ class AllreduceEngine {
   // Communicators may be null where the corresponding group has a single rank.
   void attach_generic(bool cuda, std::unique_ptr<Communicator> intra, std::unique_ptr<Communicator> cross);
   bool has_generic(bool cuda) const { return (cuda ? gen_cuda_ : gen_cpu_).ops != nullptr; }
+  // The communicator of all the world's ranks (rank() the world rank) that carries the cross-node
+  // chunks of a compressed all-to-all over several nodes; needs attach_generic(cuda) first.
+  void attach_world(bool cuda, std::unique_ptr<Communicator> world);
 
   // In-place SUM/AVG allreduce of a host buffer through the generic reducers.
   void allreduce_cpu(void* data, int dtype, int64_t numel, bool average, int explicit_bucket);
@@ -170,11 +194,16 @@ class AllreduceEngine {
                        cudaStream_t stream);
 
   // Compressed all-to-all of device (cuda) or host buffers on `stream` (FusedSra::all_to_all for
-  // the arguments): the fused kernel on the P2P transport, else the generic intra-node reducer. One
-  // node only: with several nodes every rank throws the same std::runtime_error before anything runs.
+  // the arguments): the fused kernel on the P2P transport, else the generic intra-node reducer.
   // A `route` with an index needs routes_in_kernel(); callers compose index_select / index_copy_
   // around a plain call otherwise. `out_scales` selects the codes output (FusedSra::all_to_all); at
   // world 1 without a heap the chunk is then encoded by the generic reducer's path, not copied.
+  // Several nodes (DESIGN §2.13f; device memory, at most kA2aMaxWorld ranks, no route): one launch
+  // packs every chunk for another node (launch_a2a_pack), the node's own chunks run the one-node path
+  // above on the node's sub-range with world-rank streams, one grouped exchange over the world
+  // communicator moves the records, and one launch unpacks the received records. Every chunk is
+  // quantized once by its sender and decoded once by its receiver: the result is the one-node
+  // all-to-all of W ranks, bit for bit.
   void all_to_all(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
                   const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route = nullptr,
@@ -198,6 +227,14 @@ class AllreduceEngine {
                      const std::vector<LayerSpec>& table, bool skip_incomplete, float prescale, const RngParams& rng,
                      cudaStream_t stream, bool overlapped, WireCodec codec, float* out_scales = nullptr);
   bool fused_sharded(bool cuda) const { return cuda && fused_ && cfg_.inner_comm == CommType::kP2P; }
+  // the all-to-all among the ranks of my node: counts and buffers of the node's sub-range, the
+  // streams of world ranks rank_base + local rank
+  void a2a_node(bool cuda, const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
+                const RngParams& rng, cudaStream_t stream, const A2aRoute* route, float* out_scales, int rank_base);
+  void a2a_nodes(const void* in, void* out, const std::vector<uint64_t>& in_counts,
+                 const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
+                 const RngParams& rng_in, cudaStream_t stream, const A2aRoute* route, float* out_scales);
   // the node-local stage's table: raw in a multi-node all-gather, and in a multi-node
   // reduce-scatter without CGX_INTRA_COMPRESS
   std::vector<LayerSpec> sharded_intra_table(ShardedOp op, std::vector<LayerSpec> table) const;

@@ -517,7 +517,7 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
     for (int s = 1; s < W; ++s) {
       const int q = (r + s) % W;
       if (s_send[q] <= k) continue;
-      rng.stream = a2a_rng_stream(r, q);
+      rng.stream = a2a_rng_stream(p.rank_base + r, p.rank_base + q);
       a2a_send_window<T, KB, GPL, IDX, CODEC, SCALE>(p, q, bpw, k, rng);
     }
     __syncthreads();

@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "../common/a2a.h"
 #include "../common/philox.h"
 #include "../common/wire.h"
 
@@ -135,12 +136,41 @@ struct A2aParams {
   // Scaled send (with in_index, decoded output, no combine; nullptr: none): row i of the logical send
   // buffer is T(x * in_scale[i]), one fp32 multiply rounded to nearest in T, the own rows included.
   const float* in_scale;
+  // world rank of local rank 0: the random streams are keyed by world ranks (a2a_rng_stream), so
+  // a node's chunks on several nodes use the streams they would use on one node of W ranks
+  int rank_base;
 };
 // defined once per dtype in a2a_{f32,f16,bf16}.cu; launches the routed kernel when p.in_index or
 // p.out_index is set
 cudaError_t launch_a2a_f32(const A2aParams& p, cudaStream_t stream);
 cudaError_t launch_a2a_f16(const A2aParams& p, cudaStream_t stream);
 cudaError_t launch_a2a_bf16(const A2aParams& p, cudaStream_t stream);
+
+// ---- cross-node all-to-all (a2a_remote.cu, DESIGN §2.13f) ---------------------------------------
+// The chunks one rank sends to (pack) or receives from (unpack) the ranks of other nodes, in one
+// launch each. Chunk i has cnt[i] elements at element elem_off[i] of the tensor (pack: `in`,
+// unpack: `out`) and its records at byte wire_off[i] of the buffer (pack: `out`, unpack: `in`),
+// a2a_chunk_wire bytes of them; item_first is the prefix sum of a2a_chunk_items over the chunks.
+// Compressed bits only (1..8; an FP8 codec with 8): raw chunks travel as their bytes.
+struct A2aRemoteParams {
+  const void* in;
+  void* out;
+  float* out_scales;               // unpack, FP8 codecs: codes output as A2aParams::out_scales; else nullptr
+  int dtype;
+  int bits;
+  int codec;
+  uint32_t bucket;                 // as requested (a2a_geom clamps it)
+  RngKey rng;                      // pack: .stream is filled in per chunk (a2a_rng_stream(rank, peer[i]))
+  int rank;                        // world rank of this rank
+  int nchunks;                     // <= kA2aMaxWorld
+  int peer[kA2aMaxWorld];          // world rank of chunk i's destination (pack) or source (unpack)
+  uint32_t cnt[kA2aMaxWorld];
+  uint64_t elem_off[kA2aMaxWorld];
+  uint64_t wire_off[kA2aMaxWorld];
+  uint32_t item_first[kA2aMaxWorld + 1];
+};
+cudaError_t launch_a2a_pack(const A2aRemoteParams& p, cudaStream_t stream);
+cudaError_t launch_a2a_unpack(const A2aRemoteParams& p, cudaStream_t stream);
 
 // ---- standalone item kernels (generic reducers, Python ops, tests, cross-node path) ----
 // All operate on items [first, first+count) of a device item table; `wire` is the base of the

@@ -239,6 +239,9 @@ void ProcessGroupCGX::ensure_cuda(c10::DeviceIndex dev) {
       intra = std::make_unique<C10dCommunicator>(cuda_delegate_, true, dev);
     }
     engine_->attach_generic(true, std::move(intra), std::move(cross));
+    // the compressed all-to-all's cross-node chunks travel between any two ranks of the world
+    if (engine_->nodes() > 1 && cuda_delegate_)
+      engine_->attach_world(true, std::make_unique<C10dCommunicator>(cuda_delegate_, true, dev));
   }
 
   if (cfg_.inner_comm == CommType::kP2P) {
@@ -546,10 +549,9 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   TORCH_CHECK(codec == kMaxMin || (bits == 8 && !stochastic),
               "cgx: all_to_all: the FP8 codecs use bits 8 and round to nearest");
   const int W = getSize();
-  TORCH_CHECK(W <= kMaxPeers, "cgx: all_to_all supports at most ", kMaxPeers, " ranks");
-  // every rank evaluates the same condition, so every rank refuses and none is left waiting
-  TORCH_CHECK(local_size() >= W, "cgx: the compressed all_to_all runs on one node only (CGX_LOCAL_SIZE ",
-              local_size(), " < world size ", W, ")");
+  // one node: the fused kernel's peers; several nodes: the cross-node stage's stream keys (a2a_rng_stream)
+  const int max_world = local_size() >= W ? kMaxPeers : kA2aMaxWorld;
+  TORCH_CHECK(W <= max_world, "cgx: all_to_all supports at most ", max_world, " ranks", local_size() >= W ? " on one node" : "");
   check_a2a_index(in_index, in, "input_index");
   check_a2a_index(out_index, out, "output_index");
   const bool ii = in_index.defined(), oi = out_index.defined();
@@ -644,31 +646,43 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
     }
     // the temporaries live on the comm stream only
     c10::cuda::CUDAStreamGuard sg(*comm_stream_);
-    const at::Tensor send = ii ? in.index_select(0, in_index) : in;
-    // the scaled send: the selected rows times their scales, rounded as the fused kernel rounds them
-    if (scaled)
-      cuda_check(launch_scale_rows(send.data_ptr(), in_scale.data_ptr<float>(), dtype, (uint64_t)send.size(0),
-                                   (uint64_t)row, s),
-                 "launch_scale_rows");
-    std::vector<int64_t> recv_shape = out.sizes().vec();
-    recv_shape[0] = oi ? out_index.size(0) : out.size(0);
-    at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;
-    at::Tensor recv_scales = codes && oi ? at::empty({recv_shape[0], out_scales.size(1)}, out_scales.options()) : out_scales;
-    engine_->all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits, codec,
-                        (uint32_t)bucket_size, rng, s, nullptr, codes ? recv_scales.data_ptr<float>() : nullptr);
-    if (oi && codes) {
-      // the codes move as their bytes
-      out.view(at::kByte).index_copy_(0, out_index, recv.view(at::kByte));
-      out_scales.index_copy_(0, out_index, recv_scales);
-    } else if (oi) {
-      out.index_copy_(0, out_index, recv);
-    }
-    // the combine of the slots now in `out`, by the same arithmetic as the fused kernel's
-    if (combine)
-      cuda_check(launch_combine_rows(out.data_ptr(), gate.data_ptr<float>(), combine_out.data_ptr(), dtype,
-                                     (uint64_t)gate.size(0), (uint32_t)topk, (uint32_t)row, s),
-                 "launch_combine_rows");
+    a2a_compose(*engine_, in, out, in_counts, out_counts, dtype, bits, codec, (uint32_t)bucket_size, rng, in_index,
+                out_index, in_scale, out_scales, gate, combine_out, s);
   });
+}
+
+void a2a_compose(AllreduceEngine& engine, const at::Tensor& in, const at::Tensor& out,
+                 const std::vector<uint64_t>& in_counts, const std::vector<uint64_t>& out_counts, int dtype, int bits,
+                 WireCodec codec, uint32_t bucket, const RngParams& rng, const at::Tensor& in_index,
+                 const at::Tensor& out_index, const at::Tensor& in_scale, const at::Tensor& out_scales,
+                 const at::Tensor& gate, const at::Tensor& combine_out, cudaStream_t s) {
+  const bool ii = in_index.defined(), oi = out_index.defined(), codes = out_scales.defined();
+  int64_t row = 1;
+  for (int64_t d : in.sizes().slice(1)) row *= d;
+  const at::Tensor send = ii ? in.index_select(0, in_index) : in;
+  // the scaled send: the selected rows times their scales, rounded as the fused kernel rounds them
+  if (in_scale.defined())
+    cuda_check(launch_scale_rows(send.data_ptr(), in_scale.data_ptr<float>(), dtype, (uint64_t)send.size(0),
+                                 (uint64_t)row, s),
+               "launch_scale_rows");
+  std::vector<int64_t> recv_shape = out.sizes().vec();
+  recv_shape[0] = oi ? out_index.size(0) : out.size(0);
+  at::Tensor recv = oi ? at::empty(recv_shape, out.options()) : out;
+  at::Tensor recv_scales = codes && oi ? at::empty({recv_shape[0], out_scales.size(1)}, out_scales.options()) : out_scales;
+  engine.all_to_all(true, send.data_ptr(), recv.data_ptr(), in_counts, out_counts, dtype, bits, codec, bucket, rng, s,
+                    nullptr, codes ? recv_scales.data_ptr<float>() : nullptr);
+  if (oi && codes) {
+    // the codes move as their bytes
+    out.view(at::kByte).index_copy_(0, out_index, recv.view(at::kByte));
+    out_scales.index_copy_(0, out_index, recv_scales);
+  } else if (oi) {
+    out.index_copy_(0, out_index, recv);
+  }
+  // the combine of the slots now in `out`, by the same arithmetic as the fused kernel's
+  if (combine_out.defined())
+    cuda_check(launch_combine_rows(out.data_ptr(), gate.data_ptr<float>(), combine_out.data_ptr(), dtype,
+                                   (uint64_t)gate.size(0), (uint32_t)gate.size(1), (uint32_t)row, s),
+               "launch_combine_rows");
 }
 
 c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::engine_allreduce_cpu(at::Tensor& t, bool average, int bucket_idx,

@@ -41,6 +41,19 @@ namespace cgx {
 
 class ProcessGroupCGX;
 
+// The routed, scaled, combine and indexed-codes forms of the compressed all-to-all composed around
+// engine.all_to_all's plain call, for rows the fused kernel does not route (routes_in_kernel false,
+// which includes every call over several nodes): index_select of the sent rows, scale_rows_kernel,
+// the plain call, index_copy_ of the received rows (codes as their bytes) and combine_rows_kernel,
+// on stream `s`, which must be the current torch stream (the temporaries live on it). Undefined
+// tensors are absent forms; the counts are those of the logical buffers. The same result as the
+// fused kernel's routed call by definition.
+void a2a_compose(AllreduceEngine& engine, const at::Tensor& in, const at::Tensor& out,
+                 const std::vector<uint64_t>& in_counts, const std::vector<uint64_t>& out_counts, int dtype, int bits,
+                 WireCodec codec, uint32_t bucket, const RngParams& rng, const at::Tensor& in_index,
+                 const at::Tensor& out_index, const at::Tensor& in_scale, const at::Tensor& out_scales,
+                 const at::Tensor& gate, const at::Tensor& combine_out, cudaStream_t s);
+
 // Work of one engine allreduce. Like ProcessGroupNCCL it is "complete" for stream-ordering purposes
 // as soon as the kernel is enqueued (wait() makes the caller's stream wait on the end event, the
 // CUDA-aware Future carries the same event). Failures are asynchronous: when a fused kernel
@@ -204,7 +217,8 @@ class ProcessGroupCGX : public c10d::Backend {
   // come from the ranks by `out_splits` (empty: equal splits). The own chunk is copied, every other
   // chunk quantized once with `bits` (1..8; 32: raw) and buckets of `bucket_size` counted from the
   // chunk's start; an FP8 `codec` (bits 8, round to nearest) gives the 8-bit records FP8 codes. seed < 0: CGX_SEED. Malformed splits throw before anything is enqueued; the
-  // splits of a pair must agree on both ranks (the caller's contract). One node only.
+  // splits of a pair must agree on both ranks (the caller's contract). At most 16 ranks on one node;
+  // over several nodes at most 256, the same result (AllreduceEngine::all_to_all, DESIGN §2.13f).
   // Routed form: with `in_index` row i of the sent rows is in[in_index[i]], with `out_index` row j
   // of the received rows goes to out[out_index[j]] (undefined tensors: no index). The splits then
   // count index entries. Bitwise in.index_select -> plain call -> out.index_copy_, which is what

@@ -417,7 +417,8 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
 FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                                          const std::vector<uint64_t>& out_counts, int dtype, int bits,
                                          WireCodec codec, uint32_t bucket, const RngParams& rng,
-                                         cudaStream_t stream, const A2aRoute* route, float* out_scales) {
+                                         cudaStream_t stream, const A2aRoute* route, float* out_scales,
+                                         int rank_base) {
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   const int W = world(), r = rank();
   check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, route, out_scales);
@@ -464,6 +465,7 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
   p.out_scales = out_scales;
   p.epoch_hint = epoch_;
   p.rng = make_rng_key(rng, r, 0);
+  p.rank_base = rank_base;
   p.slot_bytes = heap_->layout().slot_bytes;
   p.lane_slot = lane_slot;
   p.flag_stride = heap_->layout().flag_stride;

@@ -192,13 +192,14 @@ class FusedSra {
   // std::invalid_argument: the caller composes index_select / index_copy_ around a plain call).
   // With `out_scales` (an FP8 codec) `out` receives the codes and out_scales the units of every chunk,
   // undecoded, the own chunk encoded by the same encoder (A2aParams::out_scales).
+  // `rank_base`: the world rank of the heap's rank 0 (A2aParams::rank_base), 0 on one node.
   struct A2aCounts {
     uint64_t launches = 0, wire_bytes = 0, raw_bytes = 0;  // this rank's sends
   };
   A2aCounts all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                        const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
                        uint32_t bucket, const RngParams& rng, cudaStream_t stream, const A2aRoute* route = nullptr,
-                       float* out_scales = nullptr);
+                       float* out_scales = nullptr, int rank_base = 0);
 
   // throws std::runtime_error if a kernel reported a timeout / abort (sticky)
   void check_status();

@@ -217,7 +217,8 @@ void Reducer::all_gather(const void* in, void* out, int dtype, const std::vector
 
 void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                          const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec,
-                         uint32_t bucket, const RngParams& rng, cudaStream_t stream, float* out_scales) {
+                         uint32_t bucket, const RngParams& rng, cudaStream_t stream, float* out_scales,
+                         int rank_base) {
   const int W = comm_->size(), r = comm_->rank();
   check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, nullptr, out_scales);
   if (out_scales != nullptr) {
@@ -241,8 +242,8 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
       sw[q] = a2a_chunk_wire(a2a_geom((uint32_t)in_counts[q], bits, bucket, (int)es));
       rw[q] = a2a_chunk_wire(a2a_geom((uint32_t)out_counts[q], bits, bucket, (int)es));
     }
-    so[q + 1] = so[q] + (sw[q] + 255) / 256 * 256;
-    ro[q + 1] = ro[q] + (rw[q] + 255) / 256 * 256;
+    so[q + 1] = so[q] + a2a_region_bytes(sw[q]);
+    ro[q + 1] = ro[q] + a2a_region_bytes(rw[q]);
   }
   if (in_counts[r]) ops_->copy(dst + oo[r], src + io[r], in_counts[r] * es, stream);
   uint8_t* sendb = raw ? nullptr : scratch(0, so[W] + 16);
@@ -250,7 +251,7 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
   for (int q = 0; q < W; ++q) {
     if (!sw[q]) continue;
     RngKey key = make_rng_key(rng, r, 0);
-    key.stream = a2a_rng_stream(r, q);
+    key.stream = a2a_rng_stream(rank_base + r, rank_base + q);
     const DevicePlan& dp = plan_for({LayerSpec{0, in_counts[q], bits, bucket}}, dtype, false, stream, 1);
     ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, key, stream, codec);
   }

@@ -76,10 +76,12 @@ class Reducer {
   // `codec` quantizes and decodes the 8-bit records with the block backend's FP8 primitives. With
   // `out_scales` (an FP8 codec) the records are unpacked instead of decoded (BlockBackend::unpack_fp8)
   // into the codes `out` and the units out_scales, and the own chunk is quantized into a record and
-  // unpacked too: bitwise the fused kernel's codes output.
+  // unpacked too: bitwise the fused kernel's codes output. `rank_base` is the world rank of the
+  // communicator's rank 0: the chunk from rank q to rank p uses a2a_rng_stream(rank_base + q,
+  // rank_base + p), the stream it has in an all-to-all of all the world's ranks.
   void all_to_all(const void* in, void* out, const std::vector<uint64_t>& in_counts,
                   const std::vector<uint64_t>& out_counts, int dtype, int bits, WireCodec codec, uint32_t bucket,
-                  const RngParams& rng, cudaStream_t stream, float* out_scales = nullptr);
+                  const RngParams& rng, cudaStream_t stream, float* out_scales = nullptr, int rank_base = 0);
   uint64_t bytes_sent() const { return bytes_sent_; }
   size_t num_plans() const { return plans_.size(); }
   uint64_t plan_uploads() const { return plans_.uploads(); }

@@ -315,7 +315,8 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     rank r's ``output_split_sizes[q]``. Malformed splits on one rank (wrong length, sum or sign, or
     rows of another size than the output's) raise ``RuntimeError`` before anything is launched.
     CUDA float32 / float16 / bfloat16, contiguous, ``output`` not overlapping ``input``, at most 16
-    ranks, all on one node (several nodes raise on every rank).
+    ranks on one node, at most 256 over several nodes (each of at most 16 ranks), where the result is
+    the same as on one node, bit for bit.
     """
     from .hooks import _native_backend
 
