@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Error of the all-to-all wire codecs, computed on the CPU with the simulator (C.all_to_all_simulate,
 bit for bit what a2a_kernel delivers) from seeded inputs: max-min 8-bit against the FP8 formats
-e4m3 and e5m2, at buckets of 128 and 512 elements.
+e4m3 and e5m2 and their power-of-two-scale twins e4m3_pow2 and e5m2_pow2, at buckets of 128 and 512
+elements.
 
 Inputs, rows of H = 7168 fp32 elements (one MoE hidden state per row):
   gaussian   N(0, 1)
@@ -10,8 +11,10 @@ Inputs, rows of H = 7168 fp32 elements (one MoE hidden state per row):
   student_t  Student-t with 3 degrees of freedom (heavy tails everywhere)
 
 Reported per (input, bucket, codec): the relative L2 error ||dec - x|| / ||x|| and the largest
-per-element relative error |dec - x| / |x| over elements with |x| >= 1e-3 * rms(x). This says
-nothing about training accuracy.
+per-element relative error |dec - x| / |x| over elements with |x| >= 1e-3 * rms(x). For
+--op all_to_all also the share of elements whose value changes when the decoded rows go through the
+same codec a second time (requant_changed_pct): 0 for a codec whose decode of its encode is a
+projection. This says nothing about training accuracy.
 
 --op reduce_scatter / all_gather report the same for the compressed reduce-scatter and all-gather
 of --world ranks (C.reduce_scatter_simulate / C.all_gather_simulate, bit for bit what rs_kernel and
@@ -106,14 +109,18 @@ def main():
     for i, kind in enumerate(("gaussian", "outliers", "student_t")):
         x, mask = make_rows(kind, args.rows, args.seed + i)
         for bucket in args.buckets:
-            for bits in (8, "e4m3", "e5m2"):
+            for bits in (8, "e4m3", "e5m2", "e4m3_pow2", "e5m2_pow2"):
+                extra = {}
                 if args.op == "all_to_all":
-                    rel_l2, max_rel = errors(x, decode(x, bits, bucket), ~mask)
+                    dec = decode(x, bits, bucket)
+                    rel_l2, max_rel = errors(x, dec, ~mask)
+                    again = decode(dec, bits, bucket)
+                    extra["requant_changed_pct"] = round(100 * float((again != dec).double().mean()), 3)
                 else:
                     exact, got, m = sharded(args.op, kind, args.rows, args.seed + i, args.world, bits, bucket)
                     rel_l2, max_rel = errors(exact, got, ~m)
                 r = {"op": args.op, "input": kind, "bucket": bucket, "codec": "maxmin8" if bits == 8 else bits,
-                     "rel_l2_pct": round(100 * rel_l2, 3), "max_rel_pct": round(100 * max_rel, 2)}
+                     "rel_l2_pct": round(100 * rel_l2, 3), "max_rel_pct": round(100 * max_rel, 2), **extra}
                 res.append(r)
                 print(json.dumps(r), flush=True)
     if args.out:

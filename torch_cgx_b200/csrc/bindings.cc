@@ -195,8 +195,13 @@ A2aBits a2a_bits(const A2aBitsArg& arg, bool stochastic, const char* op = "all_t
     codec = kE4M3;
   else if (*name == "e5m2")
     codec = kE5M2;
+  else if (*name == "e4m3_pow2")
+    codec = kE4M3Pow2;
+  else if (*name == "e5m2_pow2")
+    codec = kE5M2Pow2;
   else
-    throw py::value_error(std::string("cgx ") + op + ": bits must be 1..8, 32, \"e4m3\" or \"e5m2\", got \"" +
+    throw py::value_error(std::string("cgx ") + op +
+                          ": bits must be 1..8, 32, \"e4m3\", \"e5m2\", \"e4m3_pow2\" or \"e5m2_pow2\", got \"" +
                           *name + "\"");
   if (stochastic)
     throw py::value_error(std::string("cgx ") + op + ": bits=\"" + *name +
@@ -271,7 +276,7 @@ void py_reduce_scatter_simulate(const std::vector<at::Tensor>& inputs, std::vect
 bool a2a_output_dtype_ok(const at::Tensor& t, int dt, WireCodec codes_codec) {
   if (codes_codec == kMaxMin) return cgx_dtype(t) == dt;
   const at::ScalarType s = t.scalar_type();
-  return s == at::kByte || s == (codes_codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2);
+  return s == at::kByte || s == (fp8_base(codes_codec) == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2);
 }
 
 // The codes output of the all-gather bindings: outputs[r] holds W * S code bytes (uint8 or the
@@ -293,7 +298,7 @@ std::vector<float*> ag_scales(const std::vector<at::Tensor>& inputs, const std::
     TORCH_CHECK(o.is_contiguous() && o.device() == i.device() && a2a_output_dtype_ok(o, dt, codec) &&
                     (uint64_t)o.numel() == W * S,
                 "all_gather: rank ", r, "'s codes output must be a contiguous uint8 or ",
-                codec == kE4M3 ? "float8_e4m3fn" : "float8_e5m2", " tensor of W * S elements on the inputs' device");
+                fp8_base(codec) == kE4M3 ? "float8_e4m3fn" : "float8_e5m2", " tensor of W * S elements on the inputs' device");
     TORCH_CHECK(sc.is_contiguous() && sc.device() == i.device() && sc.scalar_type() == at::kFloat &&
                     (uint64_t)sc.numel() * B == W * S,
                 "all_gather: rank ", r, "'s output_scales must be a contiguous float32 tensor of one element per ",

@@ -208,7 +208,7 @@ inline void quantize_block_fp8(const float* acc, const BlockDesc& d, uint8_t* re
       mx = nan_max(mx, acc[i]);
     }
     meta[b] = fp8_meta(mn, mx, codec);
-    const float inv = fp8_inv_unit(meta[b].unit);
+    const float inv = fp8_inv_unit(meta[b].unit, codec);
     uint8_t* dst = pay + (size_t)b * gpb * 8u;
     for (uint32_t i = lo; i < lo + div_up(hi - lo, 8u) * 8u; ++i)
       dst[i - lo] = i < hi ? (uint8_t)fp8_encode(acc[i], inv, codec) : 0u;

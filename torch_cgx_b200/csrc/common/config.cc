@@ -98,7 +98,10 @@ int parse_wire_format(const std::string& name, const char* what) {
   if (name.empty() || name == "maxmin") return kMaxMin;
   if (name == "e4m3") return kE4M3;
   if (name == "e5m2") return kE5M2;
-  throw std::invalid_argument(std::string("cgx: ") + what + " must be \"maxmin\", \"e4m3\" or \"e5m2\", got \"" +
+  if (name == "e4m3_pow2") return kE4M3Pow2;
+  if (name == "e5m2_pow2") return kE5M2Pow2;
+  throw std::invalid_argument(std::string("cgx: ") + what +
+                              " must be \"maxmin\", \"e4m3\", \"e5m2\", \"e4m3_pow2\" or \"e5m2_pow2\", got \"" +
                               name + "\"");
 }
 

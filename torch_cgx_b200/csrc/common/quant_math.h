@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <type_traits>
 
 #if defined(__CUDACC__)
 #define CGX_HD __host__ __device__ __forceinline__
@@ -152,32 +153,97 @@ CGX_HD uint32_t unpack1(uint64_t w, int j, int bits) {
 // 8-bit layout: meta {unit, +0.0f} where max-min stores {unit, min}, then one byte per element.
 // A NaN or an Inf in a bucket makes unit NaN or Inf and every element decodes to NaN (0 * Inf is
 // NaN); a bucket whose unit is below 2^-126 has 1 / unit = 0 and decodes to signed zeros.
-enum WireCodec : int { kMaxMin = 0, kE4M3 = 1, kE5M2 = 2 };
+// kE4M3Pow2 / kE5M2Pow2: the element format of kE4M3 / kE5M2 with a power-of-two unit 2^k, k the
+// smallest integer >= -126 with max|x| <= FMAX * 2^k (DESIGN §2.13g). x * 2^-k and code * 2^k are
+// exact, so decode(encode(.)) is a projection, and every finite unit is an E8M0 value. A NaN or Inf
+// bucket keeps unit = max|x| and decodes to NaN; a zero bucket has unit 2^-126.
+enum WireCodec : int { kMaxMin = 0, kE4M3 = 1, kE5M2 = 2, kE4M3Pow2 = 3, kE5M2Pow2 = 4 };
+
+// the element format of an FP8 codec (kE4M3 or kE5M2), and whether its units are powers of two;
+// constant-folded where the codec is a template argument
+CGX_HD constexpr int fp8_base(int codec) {
+  return codec == kE4M3Pow2 ? kE4M3 : codec == kE5M2Pow2 ? kE5M2 : codec;
+}
+CGX_HD constexpr bool fp8_pow2(int codec) { return codec == kE4M3Pow2 || codec == kE5M2Pow2; }
+CGX_HD constexpr bool is_fp8_codec(int codec) { return codec >= kE4M3 && codec <= kE5M2Pow2; }
+
+// f(std::integral_constant<int, C>()) for the FP8 codec C equal to `codec`, `otherwise` for any other
+// value: how the launchers turn the runtime codec into the kernels' compile-time one
+template <typename R, typename F>
+R dispatch_fp8(int codec, R otherwise, F&& f) {
+  switch (codec) {
+    case kE4M3: return f(std::integral_constant<int, kE4M3>());
+    case kE5M2: return f(std::integral_constant<int, kE5M2>());
+    case kE4M3Pow2: return f(std::integral_constant<int, kE4M3Pow2>());
+    case kE5M2Pow2: return f(std::integral_constant<int, kE5M2Pow2>());
+    default: return otherwise;
+  }
+}
 
 constexpr float kFp8MinUnit = 1.17549435e-38f;  // 2^-126: a smaller unit decodes its bucket to zeros
 constexpr uint32_t kFp8NaNCode = 0x7Fu;         // the code cvt.rn.satfinite writes for any NaN
 
+CGX_HD uint32_t fp32_bits(float f) {
+#if defined(__CUDA_ARCH__)
+  return __float_as_uint(f);
+#else
+  uint32_t u;
+  std::memcpy(&u, &f, 4);
+  return u;
+#endif
+}
+CGX_HD float fp32_from_bits(uint32_t u) {
+#if defined(__CUDA_ARCH__)
+  return __uint_as_float(u);
+#else
+  float f;
+  std::memcpy(&f, &u, 4);
+  return f;
+#endif
+}
+
 // largest finite value of the format, and its reciprocal correctly rounded to fp32 (a literal per
 // format, as rcp_levels)
-CGX_HD float fp8_max(int codec) { return codec == kE5M2 ? 57344.0f : 448.0f; }
-CGX_HD float fp8_rcp_max(int codec) { return codec == kE5M2 ? 1.0f / 57344.0f : 1.0f / 448.0f; }
+CGX_HD float fp8_max(int codec) { return fp8_base(codec) == kE5M2 ? 57344.0f : 448.0f; }
+CGX_HD float fp8_rcp_max(int codec) { return fp8_base(codec) == kE5M2 ? 1.0f / 57344.0f : 1.0f / 448.0f; }
 
-// steps 1-2: unit = nan_max(-min, max) * fp32(1 / FMAX), one rounding; the meta's second word is +0
+// the power-of-two unit of a bucket whose nan_max(-min, max) is a (a >= +0 or NaN). FMAX is
+// 1.75 * 2^E (E = 8 for e4m3, 15 for e5m2), so for a = 1.f * 2^e, a <= FMAX * 2^k holds from
+// k = e - E on when 1.f <= 1.75 (f <= 0x600000) and from e - E + 1 otherwise. Zeros and fp32
+// subnormals give k < -126 and take the clamp. Integer operations only: no log2 / exp2 rounding.
+CGX_HD float fp8_pow2_unit(float a, int codec) {
+  const uint32_t ax = fp32_bits(a) & 0x7FFFFFFFu;
+  if (ax >= 0x7F800000u) return a;  // NaN or +Inf: the bucket decodes to NaN, as with an fp32 unit
+  const int E = fp8_base(codec) == kE5M2 ? 15 : 8;
+  int k = (int)(ax >> 23) - 127 - E + ((ax & 0x7FFFFFu) > 0x600000u ? 1 : 0);
+  k = k < -126 ? -126 : k;  // k <= 127 - 8 + 1 = 120: FLT_MAX <= 448 * 2^120
+  return fp32_from_bits((uint32_t)(k + 127) << 23);
+}
+
+// steps 1-2: unit = nan_max(-min, max) * fp32(1 / FMAX), one rounding (the pow2 codecs: the unit of
+// fp8_pow2_unit); the meta's second word is +0
 CGX_HD BucketMeta fp8_meta(float mn, float mx, int codec) {
   BucketMeta m;
   const float a = nan_max(-mn, mx);
+  if (fp8_pow2(codec)) {
+    m.unit = fp8_pow2_unit(a, codec);
+  } else {
 #if defined(__CUDA_ARCH__)
-  m.unit = __fmul_rn(a, fp8_rcp_max(codec));
+    m.unit = __fmul_rn(a, fp8_rcp_max(codec));
 #else
-  m.unit = a * fp8_rcp_max(codec);
-  if (m.unit != m.unit) m.unit = canonical_nan();
+    m.unit = a * fp8_rcp_max(codec);
+    if (m.unit != m.unit) m.unit = canonical_nan();
 #endif
+  }
   m.min = 0.f;
   return m;
 }
 
-// step 3: 1 / unit, or 0 below 2^-126 (NaN stays NaN: NaN < x is false)
-CGX_HD float fp8_inv_unit(float unit) {
+// step 3: 1 / unit, or 0 below 2^-126 (NaN stays NaN: NaN < x is false). A finite pow2 unit 2^k
+// (k in [-126, 120]) has the exact inverse 2^-k, exponent field 254 - (k + 127); NaN and Inf take
+// the fp32-scale rule, so a poisoned bucket has the same codes in both formats.
+CGX_HD float fp8_inv_unit(float unit, int codec) {
+  if (fp8_pow2(codec) && fp32_bits(unit) < 0x7F800000u) return fp32_from_bits((254u - (fp32_bits(unit) >> 23)) << 23);
 #if defined(__CUDA_ARCH__)
   return unit < kFp8MinUnit ? 0.f : __frcp_rn(unit);
 #else
@@ -189,6 +255,7 @@ CGX_HD float fp8_inv_unit(float unit) {
 // (subnormals included), anything beyond the largest finite value -- infinities too -- saturates to
 // it, and a NaN of any sign or payload becomes kFp8NaNCode.
 inline uint32_t fp8_from_float_host(float v, int codec) {
+  codec = fp8_base(codec);
   const int mb = codec == kE5M2 ? 2 : 3, bias = codec == kE5M2 ? 15 : 7;
   const uint32_t maxcode = codec == kE5M2 ? 0x7Bu : 0x7Eu;
   uint32_t u;
@@ -212,6 +279,7 @@ inline uint32_t fp8_from_float_host(float v, int codec) {
 
 // exact value of an FP8 code
 inline float fp8_to_float_host(uint32_t code, int codec) {
+  codec = fp8_base(codec);
   const int mb = codec == kE5M2 ? 2 : 3, bias = codec == kE5M2 ? 15 : 7;
   const uint32_t mag = code & 0x7Fu, ef = mag >> mb, mf = mag & ((1u << mb) - 1u);
   float v;
@@ -230,7 +298,7 @@ CGX_HD uint32_t fp8x2_encode(float x0, float x1, float inv, int codec) {
 #if defined(__CUDA_ARCH__)
   const float a = __fmul_rn(x0, inv), b = __fmul_rn(x1, inv);
   unsigned short h;
-  if (codec == kE5M2)
+  if (fp8_base(codec) == kE5M2)
     asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
   else
     asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
@@ -243,7 +311,7 @@ CGX_HD void fp8x2_decode(uint32_t pair, float unit, int codec, float& d0, float&
 #if defined(__CUDA_ARCH__)
   const unsigned short in = (unsigned short)pair;
   uint32_t h2;
-  if (codec == kE5M2)
+  if (fp8_base(codec) == kE5M2)
     asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(h2) : "h"(in));
   else
     asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(in));

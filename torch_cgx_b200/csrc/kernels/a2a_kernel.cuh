@@ -566,15 +566,11 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 template <typename T, int GPL>
 cudaError_t launch_a2a_combine(const A2aParams& p, cudaStream_t stream) {
   if (p.out_scales != nullptr || (p.codec != kMaxMin && p.bits != 8)) return cudaErrorInvalidValue;
-  if (p.codec == kE4M3) {
-    dev::a2a_kernel<T, 8, GPL, true, kE4M3, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    return cudaGetLastError();
-  }
-  if (p.codec == kE5M2) {
-    dev::a2a_kernel<T, 8, GPL, true, kE5M2, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    return cudaGetLastError();
-  }
-  if (p.codec != kMaxMin) return cudaErrorInvalidValue;
+  if (p.codec != kMaxMin)
+    return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+      dev::a2a_kernel<T, 8, GPL, true, decltype(c)::value, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+      return cudaGetLastError();
+    });
   switch ((p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0) {
     case 2: dev::a2a_kernel<T, 2, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
     case 4: dev::a2a_kernel<T, 4, GPL, true, kMaxMin, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
@@ -590,15 +586,11 @@ cudaError_t launch_a2a_scaled(const A2aParams& p, cudaStream_t stream) {
   if (p.out_scales != nullptr || p.combine_out != nullptr || p.in_index == nullptr ||
       (p.codec != kMaxMin && p.bits != 8))
     return cudaErrorInvalidValue;
-  if (p.codec == kE4M3) {
-    dev::a2a_kernel<T, 8, GPL, true, kE4M3, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    return cudaGetLastError();
-  }
-  if (p.codec == kE5M2) {
-    dev::a2a_kernel<T, 8, GPL, true, kE5M2, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    return cudaGetLastError();
-  }
-  if (p.codec != kMaxMin) return cudaErrorInvalidValue;
+  if (p.codec != kMaxMin)
+    return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+      dev::a2a_kernel<T, 8, GPL, true, decltype(c)::value, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+      return cudaGetLastError();
+    });
   switch ((p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0) {
     case 2: dev::a2a_kernel<T, 2, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
     case 4: dev::a2a_kernel<T, 4, GPL, true, kMaxMin, false, false, true><<<p.lanes, kSraThreads, 0, stream>>>(p); break;
@@ -617,17 +609,13 @@ cudaError_t launch_a2a_gpl(const A2aParams& p, cudaStream_t stream) {
   if (p.codec != kMaxMin) {
     if (p.bits != 8) return cudaErrorInvalidValue;
     const bool codes = p.out_scales != nullptr;
-    if (p.codec == kE4M3 && codes)
-      dev::a2a_kernel<T, 8, GPL, IDX, kE4M3, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    else if (p.codec == kE4M3)
-      dev::a2a_kernel<T, 8, GPL, IDX, kE4M3><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    else if (p.codec == kE5M2 && codes)
-      dev::a2a_kernel<T, 8, GPL, IDX, kE5M2, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    else if (p.codec == kE5M2)
-      dev::a2a_kernel<T, 8, GPL, IDX, kE5M2><<<p.lanes, kSraThreads, 0, stream>>>(p);
-    else
-      return cudaErrorInvalidValue;
-    return cudaGetLastError();
+    return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+      if (codes)
+        dev::a2a_kernel<T, 8, GPL, IDX, decltype(c)::value, true><<<p.lanes, kSraThreads, 0, stream>>>(p);
+      else
+        dev::a2a_kernel<T, 8, GPL, IDX, decltype(c)::value><<<p.lanes, kSraThreads, 0, stream>>>(p);
+      return cudaGetLastError();
+    });
   }
   if (p.out_scales != nullptr) return cudaErrorInvalidValue;
   const int kb = (p.bits == 2 || p.bits == 4 || p.bits == 8) ? p.bits : 0;

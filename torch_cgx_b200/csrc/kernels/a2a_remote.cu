@@ -112,10 +112,11 @@ int a2a_remote_grid(uint32_t items) {
 
 template <typename T, int GPL>
 cudaError_t launch_pack_gpl(const A2aRemoteParams& p, int grid, cudaStream_t s) {
-  if (p.codec == kE4M3) {
-    dev::a2a_pack_kernel<T, 8, GPL, kE4M3><<<grid, kSraThreads, 0, s>>>(p);
-  } else if (p.codec == kE5M2) {
-    dev::a2a_pack_kernel<T, 8, GPL, kE5M2><<<grid, kSraThreads, 0, s>>>(p);
+  if (p.codec != kMaxMin) {
+    return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+      dev::a2a_pack_kernel<T, 8, GPL, decltype(c)::value><<<grid, kSraThreads, 0, s>>>(p);
+      return cudaGetLastError();
+    });
   } else {
     switch (p.bits) {
       case 2: dev::a2a_pack_kernel<T, 2, GPL, kMaxMin><<<grid, kSraThreads, 0, s>>>(p); break;
@@ -130,14 +131,14 @@ cudaError_t launch_pack_gpl(const A2aRemoteParams& p, int grid, cudaStream_t s) 
 template <typename T, int GPL>
 cudaError_t launch_unpack_gpl(const A2aRemoteParams& p, int grid, cudaStream_t s) {
   const bool codes = p.out_scales != nullptr;
-  if (p.codec == kE4M3 && codes) {
-    dev::a2a_unpack_kernel<T, 8, GPL, kE4M3, true><<<grid, kSraThreads, 0, s>>>(p);
-  } else if (p.codec == kE5M2 && codes) {
-    dev::a2a_unpack_kernel<T, 8, GPL, kE5M2, true><<<grid, kSraThreads, 0, s>>>(p);
-  } else if (p.codec == kE4M3) {
-    dev::a2a_unpack_kernel<T, 8, GPL, kE4M3, false><<<grid, kSraThreads, 0, s>>>(p);
-  } else if (p.codec == kE5M2) {
-    dev::a2a_unpack_kernel<T, 8, GPL, kE5M2, false><<<grid, kSraThreads, 0, s>>>(p);
+  if (p.codec != kMaxMin) {
+    return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+      if (codes)
+        dev::a2a_unpack_kernel<T, 8, GPL, decltype(c)::value, true><<<grid, kSraThreads, 0, s>>>(p);
+      else
+        dev::a2a_unpack_kernel<T, 8, GPL, decltype(c)::value, false><<<grid, kSraThreads, 0, s>>>(p);
+      return cudaGetLastError();
+    });
   } else {
     switch (p.bits) {
       case 2: dev::a2a_unpack_kernel<T, 2, GPL, kMaxMin, false><<<grid, kSraThreads, 0, s>>>(p); break;

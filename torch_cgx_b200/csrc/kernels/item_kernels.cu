@@ -339,6 +339,10 @@ cudaError_t dequantize_t(const ItemKernelArgs& a, const uint8_t* wire, T* dst, c
       if (g4_) { CALL(kE4M3, 4); } else { CALL(kE4M3, 2); }       \
     } else if ((a).codec == kE5M2) {                               \
       if (g4_) { CALL(kE5M2, 4); } else { CALL(kE5M2, 2); }       \
+    } else if ((a).codec == kE4M3Pow2) {                           \
+      if (g4_) { CALL(kE4M3Pow2, 4); } else { CALL(kE4M3Pow2, 2); } \
+    } else if ((a).codec == kE5M2Pow2) {                           \
+      if (g4_) { CALL(kE5M2Pow2, 4); } else { CALL(kE5M2Pow2, 2); } \
     } else {                                                       \
       return cudaErrorInvalidValue;                                \
     }                                                              \

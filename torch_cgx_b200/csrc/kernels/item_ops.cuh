@@ -823,7 +823,7 @@ __device__ __noinline__ void raw_ag_recv(const SrcSet ss, const WarpItem it, T* 
 }
 
 // ======================================================================================
-// FP8 codecs of the compressed all-to-all (quant_math.h, CODEC = kE4M3 / kE5M2): 8-bit records
+// FP8 codecs of the compressed all-to-all (quant_math.h, CODEC = kE4M3 / kE5M2 and the Pow2 twins): 8-bit records
 // whose meta is {unit, +0} and whose byte j of a group is element j's FP8 code. Same slices, same
 // min/max reductions and the same 8-bit word loads and stores as max-min; only the element
 // arithmetic differs: one FMUL + half a cvt.satfinite per element to encode, half a cvt.f16x2 +
@@ -885,7 +885,7 @@ __device__ __forceinline__ void full_send_fp8_codes(const float (&x)[GPL][8], co
 #pragma unroll
   for (int k = 0; k < GPL; ++k) {
     m[k] = fp8_meta(mn[k], mx[k], CODEC);
-    fp8_encode8<CODEC>(x[k], fp8_inv_unit(m[k].unit), lo[k], hi[k]);
+    fp8_encode8<CODEC>(x[k], fp8_inv_unit(m[k].unit, CODEC), lo[k], hi[k]);
   }
   slice_store_meta<GPL>(m, lg, ds, it.meta_off);
   store_words<8, GPL>(ds, it.pay_off, 8, lo, hi);
@@ -936,7 +936,7 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
   }
   warp_minmax(mn, mx);
   const BucketMeta m = fp8_meta(mn, mx, CODEC);
-  const float inv = fp8_inv_unit(m.unit);
+  const float inv = fp8_inv_unit(m.unit, CODEC);
   const DST du = unicast_of(ds);
   if (lane_id() == 0) dst_st_v2(du, it.meta_off, __float_as_uint(m.unit), __float_as_uint(m.min));
   for (uint32_t g = lane_id(); g < ng; g += 32) {
@@ -1235,7 +1235,7 @@ __device__ __noinline__ void bucket_reduce_fp8(T* __restrict__ blk, const WarpIt
   }
   warp_minmax(mn, mx);
   const BucketMeta m = fp8_meta(mn, mx, CODEC);
-  const float inv = fp8_inv_unit(m.unit);
+  const float inv = fp8_inv_unit(m.unit, CODEC);
   const DST du = unicast_of(ds);
   if (lane_id() == 0) dst_st_v2(du, it.meta_off, __float_as_uint(m.unit), __float_as_uint(m.min));
   for (uint32_t g = lane_id(); g < ng; g += 32) {

@@ -894,15 +894,14 @@ cudaError_t launch_sra_gpl(const SraParams& p, cudaStream_t stream) {
       if constexpr (OP == kOpAllGather) {
         if (p.out_scales != nullptr) {  // the codes output
           if (p.out_bucket == 0) return cudaErrorInvalidValue;
-          if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, OP, kE4M3, true>(p, stream);
-          if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, OP, kE5M2, true>(p, stream);
-          return cudaErrorInvalidValue;
+          return dispatch_fp8(p.codec, cudaErrorInvalidValue, [&](auto c) {
+            return launch_sra_inst<T, 8, GPL, OP, decltype(c)::value, true>(p, stream);
+          });
         }
       }
       if (p.out_scales != nullptr) return cudaErrorInvalidValue;
-      if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, OP, kE4M3>(p, stream);
-      if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, OP, kE5M2>(p, stream);
-      return cudaErrorInvalidValue;
+      return dispatch_fp8(p.codec, cudaErrorInvalidValue,
+                          [&](auto c) { return launch_sra_inst<T, 8, GPL, OP, decltype(c)::value>(p, stream); });
     }
   }
   if (p.out_scales != nullptr) return cudaErrorInvalidValue;
@@ -919,13 +918,12 @@ cudaError_t launch_sra_t(const SraParams& p, cudaStream_t stream) {
   return p.slice_elems == 1024 ? launch_sra_gpl<T, 4, OP>(p, stream) : launch_sra_gpl<T, 2, OP>(p, stream);
 }
 
-// The FP8 allreduce: sra_kernel / oneshot_kernel of an 8-bit plan with p.codec kE4M3 or kE5M2
+// The FP8 allreduce: sra_kernel / oneshot_kernel of an 8-bit plan with an FP8 p.codec
 template <typename T, int GPL>
 cudaError_t launch_sra_fp8_gpl(const SraParams& p, cudaStream_t stream) {
   if (p.uniform_bits != 8) return cudaErrorInvalidValue;
-  if (p.codec == kE4M3) return launch_sra_inst<T, 8, GPL, kOpAllreduce, kE4M3>(p, stream);
-  if (p.codec == kE5M2) return launch_sra_inst<T, 8, GPL, kOpAllreduce, kE5M2>(p, stream);
-  return cudaErrorInvalidValue;
+  return dispatch_fp8(p.codec, cudaErrorInvalidValue,
+                      [&](auto c) { return launch_sra_inst<T, 8, GPL, kOpAllreduce, decltype(c)::value>(p, stream); });
 }
 template <typename T>
 cudaError_t launch_sra_fp8_t(const SraParams& p, cudaStream_t stream) {

@@ -411,7 +411,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
   if (codes) {
     TORCH_CHECK(!rs, "cgx: output_scales is an all_gather output");
     TORCH_CHECK(codec != kMaxMin, "cgx: all_gather: output_scales needs bits=\"e4m3\" or \"e5m2\"");
-    const at::ScalarType want = codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
+    const at::ScalarType want = fp8_base(codec) == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
     TORCH_CHECK(dtype >= 0 && out.scalar_type() == want, "cgx: all_gather: with output_scales the input must be ",
                 "float32, float16 or bfloat16 and the output ", want, ", got ", in.scalar_type(), " and ",
                 out.scalar_type());
@@ -531,7 +531,7 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
   const bool codes = out_scales.defined();
   if (codes) {
     TORCH_CHECK(codec != kMaxMin, "cgx: all_to_all: output_scales needs bits=\"e4m3\" or \"e5m2\"");
-    const at::ScalarType want = codec == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
+    const at::ScalarType want = fp8_base(codec) == kE4M3 ? at::kFloat8_e4m3fn : at::kFloat8_e5m2;
     TORCH_CHECK(dtype >= 0 && out.scalar_type() == want, "cgx: all_to_all: with output_scales the input must be ",
                 "float32, float16 or bfloat16 and the output ", want, ", got ", in.scalar_type(), " and ",
                 out.scalar_type());

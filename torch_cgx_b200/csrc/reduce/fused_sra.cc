@@ -73,7 +73,7 @@ namespace {
 // an FP8 allreduce: a known codec, compressed blocks of 8 bits only, round to nearest
 void check_allreduce_codec(const Plan& plan, WireCodec codec, const RngParams& rng) {
   if (codec == kMaxMin) return;
-  if (codec != kE4M3 && codec != kE5M2) throw std::invalid_argument("cgx allreduce: unknown wire codec");
+  if (!is_fp8_codec(codec)) throw std::invalid_argument("cgx allreduce: unknown wire codec");
   if (rng.stochastic) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
   for (const BlockDesc& d : plan.blocks)
     if (block_bits(d) != 8 && block_bits(d) < kRawBits)
@@ -119,8 +119,8 @@ void FusedSra::run(const DevicePlan& dp, void* data, float prescale, const RngPa
 uint32_t codes_bucket(ShardedOp op, const std::vector<LayerSpec>& shard_layers, WireCodec codec) {
   if (op != ShardedOp::kAllGather)
     throw std::invalid_argument("cgx reduce_scatter: output_scales is an all_gather output");
-  if (codec != kE4M3 && codec != kE5M2)
-    throw std::invalid_argument("cgx all_gather: output_scales needs an FP8 format (e4m3 or e5m2)");
+  if (!is_fp8_codec(codec))
+    throw std::invalid_argument("cgx all_gather: output_scales needs an FP8 format (e4m3, e5m2, e4m3_pow2 or e5m2_pow2)");
   const uint32_t B = shard_layers.empty() ? 1u : shard_layers[0].bucket;
   if (B < 1 || B > kMaxBlockElems)
     throw std::invalid_argument("cgx all_gather: output_scales needs 1 <= bucket_size <= " +
@@ -140,7 +140,7 @@ void check_sharded_buffers(ShardedOp op, const std::vector<LayerSpec>& shard_lay
                            const void* out, uint64_t S, int rank, int world, WireCodec codec, const float* out_scales) {
   const bool rs = op == ShardedOp::kReduceScatter;
   const char* name = op_name(op);
-  if (codec != kMaxMin && codec != kE4M3 && codec != kE5M2)
+  if (codec != kMaxMin && !is_fp8_codec(codec))
     throw std::invalid_argument(std::string("cgx ") + name + ": unknown wire codec");
   if (codec != kMaxMin)
     for (const LayerSpec& l : shard_layers)
@@ -341,7 +341,7 @@ void check_all_to_all(const void* in, const void* out, const std::vector<uint64_
     throw std::invalid_argument("cgx all_to_all: need one input and one output count per rank");
   if (bits < 1 || (bits > 8 && bits < kRawBits))
     throw std::invalid_argument("cgx all_to_all: bits must be in 1..8, or 32 for none");
-  if (codec != kMaxMin && codec != kE4M3 && codec != kE5M2)
+  if (codec != kMaxMin && !is_fp8_codec(codec))
     throw std::invalid_argument("cgx all_to_all: unknown wire codec");
   if (codec != kMaxMin && bits != 8) throw std::invalid_argument("cgx all_to_all: the FP8 codecs use bits 8");
   if (bucket < 1) throw std::invalid_argument("cgx all_to_all: bucket_size must be >= 1");

@@ -230,7 +230,7 @@ def quantize_dequantize_layers(x: torch.Tensor, layers: Sequence[Layer], *, skip
                                prescale: float = 1.0, fmt: str | None = None) -> torch.Tensor:
     """One quantize -> dequantize round trip of ``prescale * x`` through a layer table, in
     ``x.dtype`` (raw runs: the value rounded to the dtype). Elements outside every layer are 0,
-    as in a freshly dequantized tensor. ``fmt`` ("e4m3" / "e5m2"): the compressed layers (bits 8)
+    as in a freshly dequantized tensor. ``fmt`` (a name of ``FP8_FORMATS``): the compressed layers (bits 8)
     take the FP8 round trip of ``fp8_quantize_dequantize`` instead of max-min's."""
     _check_fp8_table(layers, fmt)
     v = _scaled_inputs([x], _F32(prescale))[0]
@@ -277,7 +277,7 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
     is Q(acc), the owner's self-decoded copy, stored in the input dtype on every rank.
     Raw runs (uncompressed layers, skip_incomplete tails) replace Q by a rounding to the
     dtype, per peer contribution and once at the end. Elements outside every layer are kept.
-    ``fmt`` ("e4m3" / "e5m2"): Q is the FP8 round trip of ``fp8_quantize_dequantize``, for the
+    ``fmt`` (a name of ``FP8_FORMATS``): Q is the FP8 round trip of ``fp8_quantize_dequantize``, for the
     peers' contributions and for the fp32 sum alike; the table may hold bits 8 and 32 only.
     """
     _check_fp8_table(layers, fmt)
@@ -476,7 +476,7 @@ def engine_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *,
     ``C.LocalReducerGroup``) with these sequence numbers instead of the deterministic references.
     ``perturb`` (one of ``ENGINE_PERTURBATIONS``) switches on a wrong semantics, for the tests that
     show the reference tells it apart.
-    ``fmt`` ("e4m3" / "e5m2"): every compressed stage uses that FP8 format (deterministic only).
+    ``fmt`` (a name of ``FP8_FORMATS``): every compressed stage uses that FP8 format (deterministic only).
     """
     from .. import _C
 
@@ -634,7 +634,7 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
         prescale*x_r  (kept unquantized)  +  sum over q != r, in rank order, of Q(prescale*x_q)
     rounded once to the dtype: the SRA's phase-B accumulator without the requantization. Raw runs
     round each peer contribution to the dtype. Elements outside every layer are 0. The prescale is
-    ``prescale`` when given, else 1/W when averaging, else 1. ``fmt`` ("e4m3" / "e5m2"): Q is
+    ``prescale`` when given, else 1/W when averaging, else 1. ``fmt`` (a name of ``FP8_FORMATS``): Q is
     the FP8 round trip (``fp8_quantize_dequantize`` of the prescaled values), and the table's
     compressed layers have bits 8.
     """
@@ -665,15 +665,33 @@ def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[
 
 
 # ---- FP8 wire formats of the all-to-all (common/quant_math.h, DESIGN §2.13b) ------------------------
-# name -> (torch dtype, largest finite value)
-FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0)}
+# name -> (torch dtype, largest finite value). The "_pow2" formats have their base format's codes
+# with a power-of-two unit per bucket (DESIGN §2.13g).
+FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0),
+               "e4m3_pow2": (torch.float8_e4m3fn, 448.0), "e5m2_pow2": (torch.float8_e5m2, 57344.0)}
 _FP8_MIN_UNIT = _F32(2.0 ** -126)
+
+
+def _fp8_pow2_units(a: np.ndarray, fmax: float) -> Tuple[np.ndarray, np.ndarray]:
+    """The power-of-two unit 2^k of buckets whose max |x| is ``a`` (fp32, >= +0 or NaN), k the smallest
+    integer >= -126 with a <= fmax * 2^k, and its inverse 2^-k. With a = m * 2^e and fmax = fm * 2^fe
+    (frexp, m and fm in [0.5, 1)), a <= fmax * 2^k holds from k = e - fe on when m <= fm, from
+    e - fe + 1 otherwise. A NaN or Inf ``a`` is its own unit, with the fp32-scale formats' inverse."""
+    finite = np.isfinite(a)
+    m, e = np.frexp(np.where(finite, a, 0).astype(np.float64))
+    fm, fe = np.frexp(fmax)
+    k = e.astype(np.int64) - fe + (m > fm)
+    k = np.where(a == 0, -126, np.maximum(k, -126))
+    with np.errstate(all="ignore"):
+        unit = np.where(finite, np.ldexp(1.0, k), a).astype(_F32)
+        inv = np.where(finite, np.ldexp(1.0, -k), _F32(1.0) / unit).astype(_F32)
+    return unit, inv
 
 
 def _fp8_code_buckets(v: np.ndarray, fmt: str, bucket: int) -> Tuple[torch.Tensor, np.ndarray]:
     """FP8 codes of a flat fp32 array whose buckets start at index 0, in numpy fp32 arithmetic and
-    torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126),
-    code = float8(clamp(x * inv, ±FMAX)). The clamp stands for the hardware's saturation: torch's
+    torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126), or for the
+    "_pow2" formats the unit of ``_fp8_pow2_units``; code = float8(clamp(x * inv, ±FMAX)). The clamp stands for the hardware's saturation: torch's
     casts give NaN / Inf past the largest finite value. Returns the codes as a [buckets, bucket]
     float8 tensor (the last bucket padded with its last value) and the units, fp32 [buckets]."""
     tdt, fmax = FP8_FORMATS[fmt]
@@ -686,8 +704,11 @@ def _fp8_code_buckets(v: np.ndarray, fmt: str, bucket: int) -> Tuple[torch.Tenso
         mn, mx = _nan_minmax(b)
         a = np.maximum(-mn, mx)  # NaN propagates
         a = np.where(a == 0, _F32(0.0), a)  # +0, as max.NaN gives for a zero bucket
-        unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
-        inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
+        if fmt.endswith("_pow2"):
+            unit, inv = _fp8_pow2_units(a, fmax)
+        else:
+            unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
+            inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
         t = np.clip((b * inv).astype(_F32), _F32(-fmax), _F32(fmax))
     return torch.from_numpy(np.ascontiguousarray(t)).to(tdt), unit.reshape(-1).astype(_F32)
 
@@ -705,7 +726,7 @@ def _fp8_qdq_buckets(v: np.ndarray, fmt: str, bucket: int) -> np.ndarray:
 
 
 def fp8_quantize(x: torch.Tensor, fmt: str, bucket_size: int) -> Tuple[torch.Tensor, torch.Tensor]:
-    """FP8 (``fmt`` "e4m3" / "e5m2") codes and per-bucket units of a flat tensor, buckets of
+    """FP8 (``fmt`` a name of ``FP8_FORMATS``) codes and per-bucket units of a flat tensor, buckets of
     ``bucket_size`` (clamped as every bucket) from its first element: ``(codes, units)``, the codes
     a float8 tensor of ``x.numel()`` elements, the units fp32, one per bucket. ``codes.float() *
     units`` (bucket-wise, one fp32 multiply) is ``fp8_quantize_dequantize`` before its rounding to
@@ -720,7 +741,7 @@ def fp8_quantize(x: torch.Tensor, fmt: str, bucket_size: int) -> Tuple[torch.Ten
 
 
 def fp8_quantize_dequantize(x: torch.Tensor, fmt: str, bucket_size: int) -> torch.Tensor:
-    """FP8 (``fmt`` "e4m3" / "e5m2") round trip of a flat tensor, buckets of ``bucket_size``
+    """FP8 (``fmt`` a name of ``FP8_FORMATS``) round trip of a flat tensor, buckets of ``bucket_size``
     (clamped as every bucket) from its first element, rounded to ``x.dtype``."""
     if fmt not in FP8_FORMATS:
         raise ValueError(f"unknown FP8 format {fmt!r}")
@@ -735,7 +756,7 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
     go from rank q to rank r; rank q's input holds its chunks in destination order and rank r's
     output the chunks it receives in source order. The own chunk, and every chunk when ``bits`` is
     32, is the input unchanged; every other chunk is ``quantize_dequantize_layers`` of one layer, so
-    buckets are counted from the chunk's first element. ``bits`` "e4m3" / "e5m2": every other chunk
+    buckets are counted from the chunk's first element. ``bits`` an FP8 format: every other chunk
     is ``fp8_quantize_dequantize`` instead."""
     if isinstance(bits, str) and bits not in FP8_FORMATS:
         raise ValueError(f"unknown FP8 format {bits!r}")
@@ -984,7 +1005,8 @@ def _rs_hier(inputs, shard_layers, local_size, *, average, intra_compress, pertu
 
 def reduce_scatter_hier_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer], *,
                                   local_size: int, average: bool = False, skip_incomplete: bool = False,
-                                  intra_compress: bool = True, perturb: str | None = None) -> List[torch.Tensor]:
+                                  intra_compress: bool = True, perturb: str | None = None,
+                                  fmt: str | None = None) -> List[torch.Tensor]:
     """Every rank's output of the compressed reduce-scatter over N = W / L nodes of L = ``local_size``
     consecutive ranks (deterministic rounding); rank r = n*L + l, ``inputs[r]`` holds W shards of S.
 
@@ -997,10 +1019,12 @@ def reduce_scatter_hier_reference(inputs: Sequence[torch.Tensor], shard_layers: 
        rank (n, l) gets P[n] unquantized plus Q of every other node's P[n], in node order.
     With N = 1 this is ``reduce_scatter_reference``, and with L = 1 bitwise the same over W ranks.
     ``perturb`` (one of ``SHARDED_PERTURBATIONS``) switches on a wrong semantics for the tests.
+    ``fmt`` (a name of ``FP8_FORMATS``): both stages use that FP8 format (``reduce_scatter_reference``).
     """
     def stage(ins, table, prescale, _seq, cross):
-        fn = _rs_quantized_own if (cross and perturb == "quantized_own_partial") else reduce_scatter_reference
-        return fn(ins, table, prescale=prescale, skip_incomplete=skip_incomplete)
+        if cross and perturb == "quantized_own_partial":
+            return _rs_quantized_own(ins, table, prescale=prescale, skip_incomplete=skip_incomplete)
+        return reduce_scatter_reference(ins, table, prescale=prescale, skip_incomplete=skip_incomplete, fmt=fmt)
 
     return _rs_hier(inputs, shard_layers, local_size, average=average, intra_compress=intra_compress,
                     perturb=perturb, stage=stage)

@@ -9,7 +9,8 @@ FSDP2 takes a custom reduce-scatter and all-gather per module (``FSDPModule.set_
     cgx.set_cgx_all_gather(model, bits=8)            # one comm per FSDPModule, per-parameter table
 
 ``bits`` may also be an FP8 wire format: ``"e4m3"`` for the parameter all-gather and ``"e5m2"`` for
-the gradient reduce-scatter are the usual choice.
+the gradient reduce-scatter are the usual choice, and ``"e4m3_pow2"`` / ``"e5m2_pow2"`` give the
+same codes with power-of-two scales.
 
 Both work over any number of nodes: across nodes they run in two stages, the semantics of
 ``reduce_scatter_tensor`` and ``all_gather_into_tensor`` (functional.py).

@@ -17,7 +17,8 @@ and so is the compressed all-gather (``dist.all_gather_into_tensor`` stays uncom
 
     cgx.all_gather_into_tensor(flat_params, shard, bits=8)
 
-Both also take an FP8 wire format, ``bits="e4m3"`` or ``"e5m2"``, in place of max-min 8-bit.
+Both also take an FP8 wire format, ``bits="e4m3"`` or ``"e5m2"`` (or ``"e4m3_pow2"`` / ``"e5m2_pow2"``,
+with power-of-two scales), in place of max-min 8-bit.
 
 and the compressed all-to-all of expert-parallel MoE layers (``dist.all_to_all_single`` stays
 uncompressed)::
@@ -52,8 +53,9 @@ def compression(bits: Optional[A2aBits] = None, bucket_size: Optional[int] = Non
                 seed: Optional[int] = None) -> Iterator[None]:
     """Temporarily override the env-level compression config (None = leave as is; bits=32 disables).
 
-    ``bits="e4m3"`` or ``"e5m2"`` compresses at 8 bits and sends the allreduce's 8-bit layers as
-    FP8 codes with one fp32 scale per bucket (``CGX_COMPRESSION_FORMAT``); an integer ``bits``
+    ``bits="e4m3"``, ``"e5m2"``, ``"e4m3_pow2"`` or ``"e5m2_pow2"`` compresses at 8 bits and sends
+    the allreduce's 8-bit layers as FP8 codes with one fp32 scale per bucket (``CGX_COMPRESSION_FORMAT``;
+    the ``_pow2`` formats' scales are powers of two, see ``all_to_all_single``); an integer ``bits``
     selects max-min. FP8 rounds to nearest: an unknown name, or a name with ``stochastic=True`` or
     ``CGX_STOCHASTIC_ROUNDING=1``, raises ValueError before anything is changed.
     """
@@ -119,7 +121,7 @@ def _sharded(method: str, api: str, output: torch.Tensor, input: torch.Tensor, h
     return None
 
 
-A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2"
+A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2" / "e4m3_pow2" / "e5m2_pow2"
 
 
 def _sharded_bits(bits: A2aBits, stochastic: bool, layers: Optional[Sequence[Tuple[int, int, int, int]]],
@@ -168,7 +170,7 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBi
     in rank order. ``e5m2``'s wider exponent range suits gradients. A ``layers`` table may then hold
     bits 8 (FP8) and 32 (raw) only. A NaN or an Inf in a peer's bucket makes that bucket of the sum
     NaN. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as does any other
-    string.
+    string. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales (see ``all_to_all_single``).
 
     Over several nodes (``local_size`` consecutive ranks each) the reduction has two stages: inside
     each node, for every node's block of shards, the reduce-scatter above over the local ranks
@@ -216,15 +218,15 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aB
     the usual choice for weights being ``e4m3``. Every rank, the owner included, writes the values
     decoded from the same codes, so at world 1 the output is ``ops.oracle.fp8_quantize_dequantize``
     of the input. A ``layers`` table may then hold bits 8 (FP8) and 32 (raw) only; FP8 rounds to
-    nearest only.
+    nearest only. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales (see ``all_to_all_single``).
 
     Over several nodes the owner's quantized bytes first go to the ranks of the same local rank on
     the other nodes, which decode them; each node then shares the decoded shards among its ranks
     uncompressed. Every shard is still quantized exactly once, so with round-to-nearest every
     rank's ``output`` is the same as on one node.
 
-    FP8 codes for an FP8 GEMM on the gathered tensor: with ``output_scales`` (and ``bits="e4m3"`` /
-    ``"e5m2"``) ``output`` is a ``torch.float8_e4m3fn`` / ``torch.float8_e5m2`` tensor of ``world *
+    FP8 codes for an FP8 GEMM on the gathered tensor: with ``output_scales`` (and an FP8 ``bits``)
+    ``output`` is a ``torch.float8_e4m3fn`` / ``torch.float8_e5m2`` tensor (the format's) of ``world *
     input.numel()`` elements that receives the wire's codes undecoded, and ``output_scales`` (CUDA
     float32, contiguous, ``output.numel() // bucket_size`` elements, any shape) the fp32 unit of
     every bucket: the bucket starting at element ``e`` of ``output`` has the scale
@@ -279,6 +281,12 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     NaN in every element. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as
     does any other string.
 
+    ``bits="e4m3_pow2"`` or ``"e5m2_pow2"`` sends the same bytes with the codes of e4m3 / e5m2 and a
+    power-of-two scale per bucket, ``unit = 2^k`` with k the smallest integer >= -126 such that
+    ``max|x| <= FMAX * 2^k``. Encoding and decoding are then exact multiplications, so quantizing
+    the decoded values again at the same buckets gives them back unchanged, and every unit is
+    exactly representable as ``torch.float8_e8m0fnu``. A zero bucket has unit 2^-126.
+
     Routed form, for MoE token dispatch and combine without a permutation copy: ``input_index``
     (CUDA int64, ``sum(input_split_sizes)`` entries in ``[0, input.shape[0])``, repeats allowed)
     makes row i of the sent buffer ``input[input_index[i]]``; ``output_index`` (``sum(output_split_sizes)``
@@ -291,8 +299,8 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     range is not checked on the host: the kernel skips that row and the call fails (``work.wait()``
     raises, naming the index), after which the group refuses further collectives.
 
-    FP8 codes for an FP8 expert GEMM: with ``output_scales`` (and ``bits="e4m3"`` / ``"e5m2"``)
-    ``output`` is a ``torch.float8_e4m3fn`` / ``torch.float8_e5m2`` tensor of the input's shape per
+    FP8 codes for an FP8 expert GEMM: with ``output_scales`` (and an FP8 ``bits``) ``output`` is a
+    ``torch.float8_e4m3fn`` (e4m3, e4m3_pow2) / ``torch.float8_e5m2`` (e5m2, e5m2_pow2) tensor of the input's shape per
     row that receives the wire's codes undecoded, and ``output_scales`` (CUDA float32, contiguous,
     ``[output.shape[0], H // bucket_size]`` with ``H`` the elements of a row) the fp32 unit of every
     bucket. ``H % bucket_size == 0`` and ``bucket_size <= 8192``, so every bucket lies inside one row;
@@ -363,7 +371,8 @@ def _check_codes_format(api: str, output: torch.Tensor, bits: A2aBits) -> None:
     from ..ops.oracle import FP8_FORMATS
 
     if not isinstance(bits, str):
-        raise ValueError(f"cgx.{api}: output_scales needs bits='e4m3' or 'e5m2', got bits={bits}")
+        raise ValueError(f"cgx.{api}: output_scales needs bits='e4m3', 'e5m2', 'e4m3_pow2' or 'e5m2_pow2', "
+                         f"got bits={bits}")
     want = FP8_FORMATS[bits][0]
     if output.dtype != want:
         raise ValueError(f"cgx.{api}: with bits={bits!r} and output_scales the output must be {want}, "
