@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Error of the all-to-all wire codecs, computed on the CPU with the simulator (C.all_to_all_simulate,
 bit for bit what a2a_kernel delivers) from seeded inputs: max-min 8-bit against the FP8 formats
-e4m3 and e5m2 and their power-of-two-scale twins e4m3_pow2 and e5m2_pow2, at buckets of 128 and 512
-elements.
+e4m3 and e5m2, their power-of-two-scale twins e4m3_pow2 and e5m2_pow2 and their stochastic twins
+e4m3_sr and e5m2_sr, at buckets of 128 and 512 elements.
 
 Inputs, rows of H = 7168 fp32 elements (one MoE hidden state per row):
   gaussian   N(0, 1)
@@ -14,7 +14,9 @@ Reported per (input, bucket, codec): the relative L2 error ||dec - x|| / ||x|| a
 per-element relative error |dec - x| / |x| over elements with |x| >= 1e-3 * rms(x). For
 --op all_to_all also the share of elements whose value changes when the decoded rows go through the
 same codec a second time (requant_changed_pct): 0 for a codec whose decode of its encode is a
-projection. This says nothing about training accuracy.
+projection, and the bias: the relative L2 norm ||mean(dec) - x|| / ||x|| of the mean decoded value
+over --seeds seeds of the random stream (only the _sr codecs depend on the seed; for the others
+this is their deterministic error). This says nothing about training accuracy.
 
 --op reduce_scatter / all_gather report the same for the compressed reduce-scatter and all-gather
 of --world ranks (C.reduce_scatter_simulate / C.all_gather_simulate, bit for bit what rs_kernel and
@@ -58,11 +60,12 @@ def _student_t(rows, g, dof=3.0):
     return z / torch.sqrt(chi2 / dof)
 
 
-def decode(x, bits, bucket):
+def decode(x, bits, bucket, seed=0):
     """x's rows sent from rank 0 to rank 1 through the codec: what rank 1 receives"""
     n = x.numel()
     out = [torch.empty(0), torch.empty(n)]
-    C.all_to_all_simulate([x.reshape(-1), torch.empty(0)], out, [[0, n], [0, 0]], bits=bits, bucket_size=bucket)
+    C.all_to_all_simulate([x.reshape(-1), torch.empty(0)], out, [[0, n], [0, 0]], bits=bits, bucket_size=bucket,
+                          seed=seed)
     return out[1].reshape(x.shape)
 
 
@@ -102,6 +105,7 @@ def main():
     ap.add_argument("--out", type=str, default=None, help="also write the JSON lines here")
     ap.add_argument("--op", default="all_to_all", choices=["all_to_all", "reduce_scatter", "all_gather"])
     ap.add_argument("--world", type=int, default=8, help="--op reduce_scatter / all_gather: ranks")
+    ap.add_argument("--seeds", type=int, default=16, help="--op all_to_all: seeds of the bias column")
     args = ap.parse_args()
     if args.op != "all_to_all" and args.rows % args.world:
         ap.error("--rows must be divisible by --world")
@@ -109,13 +113,16 @@ def main():
     for i, kind in enumerate(("gaussian", "outliers", "student_t")):
         x, mask = make_rows(kind, args.rows, args.seed + i)
         for bucket in args.buckets:
-            for bits in (8, "e4m3", "e5m2", "e4m3_pow2", "e5m2_pow2"):
+            for bits in (8, "e4m3", "e5m2", "e4m3_pow2", "e5m2_pow2", "e4m3_sr", "e5m2_sr"):
                 extra = {}
                 if args.op == "all_to_all":
                     dec = decode(x, bits, bucket)
                     rel_l2, max_rel = errors(x, dec, ~mask)
                     again = decode(dec, bits, bucket)
                     extra["requant_changed_pct"] = round(100 * float((again != dec).double().mean()), 3)
+                    mean = torch.stack([decode(x, bits, bucket, s).double() for s in range(args.seeds)]).mean(0)
+                    xd = x[:, ~mask].double()
+                    extra["bias_rel_l2_pct"] = round(100 * float((mean[:, ~mask] - xd).norm() / xd.norm()), 4)
                 else:
                     exact, got, m = sharded(args.op, kind, args.rows, args.seed + i, args.world, bits, bucket)
                     rel_l2, max_rel = errors(exact, got, ~m)

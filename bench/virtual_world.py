@@ -13,7 +13,8 @@ rank in W chunks, with equal splits and with skewed ones (chunk q -> r gets a sh
 1 + (r - q) mod W, so every rank still sends and receives `mb` MB but pairs differ up to W : 1),
 next to the reduce-scatter (rs_kernel) of the same `mb` MB input per rank, same dtype, bits and
 bucket. Both move the same packed bytes; the reduce-scatter also accumulates. Its --bits may name
-the FP8 wire formats, e4m3 and e5m2 (and e4m3_pow2 / e5m2_pow2, their power-of-two-scale twins),
+the FP8 wire formats, e4m3 and e5m2 (and e4m3_pow2 / e5m2_pow2, their power-of-two-scale twins, and
+e4m3_sr / e5m2_sr, which round stochastically),
 which move the bytes of bits 8 (the reduce-scatter row next to them runs at bits 8).
 
 --op ag_codes times the FP8 all-gather's codes output (e4m3, bf16, H in --hiddens, buckets of 128
@@ -193,7 +194,7 @@ def skewed_counts(W, n):
 
 def a2a_bits(b):
     """an all-to-all --bits entry: an integer width, or an FP8 format name"""
-    return b if b in ("e4m3", "e5m2", "e4m3_pow2", "e5m2_pow2") else int(b)
+    return b if b in ("e4m3", "e5m2", "e4m3_pow2", "e5m2_pow2", "e4m3_sr", "e5m2_sr") else int(b)
 
 
 def all_to_all_rows(args, dev, W, lanes):

@@ -179,9 +179,10 @@ void py_oneshot_simulate(std::vector<at::Tensor> tensors, const std::vector<Laye
 }
 
 // The `bits` of every all-to-all, reduce-scatter and all-gather binding: 1..8 or 32 (max-min levels,
-// or raw), or the name of an FP8 wire codec, which travels in 8-bit records and rounds to nearest
-// only. Integers are checked where they are used, as before; an unknown name, or an FP8 codec with
-// stochastic rounding, raises ValueError naming `op` before anything runs.
+// or raw), or the name of an FP8 wire codec, which travels in 8-bit records. The `_sr` codecs round
+// stochastically whatever `stochastic` says; the others round to nearest only. Integers are checked
+// where they are used, as before; an unknown name, or a round-to-nearest FP8 codec with stochastic
+// rounding, raises ValueError naming `op` before anything runs.
 using A2aBitsArg = std::variant<int64_t, std::string>;
 struct A2aBits {
   int bits;
@@ -199,13 +200,18 @@ A2aBits a2a_bits(const A2aBitsArg& arg, bool stochastic, const char* op = "all_t
     codec = kE4M3Pow2;
   else if (*name == "e5m2_pow2")
     codec = kE5M2Pow2;
+  else if (*name == "e4m3_sr")
+    codec = kE4M3SR;
+  else if (*name == "e5m2_sr")
+    codec = kE5M2SR;
   else
     throw py::value_error(std::string("cgx ") + op +
-                          ": bits must be 1..8, 32, \"e4m3\", \"e5m2\", \"e4m3_pow2\" or \"e5m2_pow2\", got \"" +
+                          ": bits must be 1..8, 32, \"e4m3\", \"e5m2\", \"e4m3_pow2\", \"e5m2_pow2\", \"e4m3_sr\" or "
+                          "\"e5m2_sr\", got \"" +
                           *name + "\"");
-  if (stochastic)
+  if (stochastic && !fp8_sr(codec))
     throw py::value_error(std::string("cgx ") + op + ": bits=\"" + *name +
-                          "\" rounds to nearest only; stochastic rounding needs integer bits");
+                          "\" rounds to nearest only; stochastic rounding needs integer bits or an _sr format");
   return {8, codec};
 }
 
@@ -334,7 +340,7 @@ void py_all_gather_simulate(const std::vector<at::Tensor>& inputs, std::vector<a
       const std::vector<LayerSpec> copy(layers.begin() + (ptrdiff_t)(q * per_copy),
                                         layers.begin() + (ptrdiff_t)((q + 1) * per_copy));
       codes_simulate(build_plan(copy, make_opts(1, 1, cgx_dtype(inputs[0]), false, 1 << 30)), full.data(), codes0,
-                     scales[0], codec);
+                     scales[0], codec, make_rng_key(make_rng(stochastic, seed, seq), q, 1));
     }
     for (int r = 1; r < W; ++r) {
       std::memcpy(outputs[r].data_ptr(), codes0, (size_t)W * S);
@@ -2144,6 +2150,23 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       py::arg("bits"), py::arg("stochastic") = false, py::arg("op") = "all_to_all");
   m.def("a2a_rng_stream", [](int src, int dst) { return (int64_t)a2a_rng_stream(src, dst); }, py::arg("src"),
         py::arg("dst"));
+  // The 16 random bits of n consecutive elements from first_elem on, as the stochastic encoders draw
+  // them: element i takes half i % 8 of rounding_bits of the group at first_elem + 8 * (i / 8). The
+  // stream is the raw word (rank * 2 + phase, or a2a_rng_stream). For the references of the SR codecs.
+  m.def(
+      "philox_u16",
+      [](uint64_t seed, uint32_t seq, uint32_t stream, uint32_t first_elem, int64_t n) {
+        TORCH_CHECK(n >= 0, "philox_u16: n must be >= 0");
+        RngKey k{(uint32_t)seed, (uint32_t)(seed >> 32), seq, stream, 1u};
+        at::Tensor out = at::empty({n}, at::kInt);
+        int32_t* o = out.data_ptr<int32_t>();
+        for (int64_t g = 0; g < n; g += 8) {
+          const Philox4 a = rounding_bits(k, first_elem + (uint32_t)g);
+          for (int64_t j = 0; j < 8 && g + j < n; ++j) o[g + j] = (int32_t)((a.v[j >> 1] >> ((j & 1) * 16)) & 0xFFFFu);
+        }
+        return out;
+      },
+      py::arg("seed"), py::arg("seq"), py::arg("stream"), py::arg("first_elem"), py::arg("n"));
   m.attr("A2A_MAX_WORLD") = (int64_t)kA2aMaxWorld;
   m.def("a2a_remote_wire", &py_a2a_remote_wire, py::arg("counts"), py::arg("rank"), py::arg("local_size"),
         py::arg("bits"), py::arg("bucket_size"), py::arg("dtype") = 0);

@@ -192,8 +192,10 @@ inline void decode_block_foreach(const uint8_t* rec, int dtype, const BlockDesc&
 }
 
 // FP8 codecs (quant_math.h) of an 8-bit block: the record layout of quantize_block at bits 8,
-// meta {unit, +0} per bucket and element i's code at byte i of its bucket's payload
-inline void quantize_block_fp8(const float* acc, const BlockDesc& d, uint8_t* rec, int codec) {
+// meta {unit, +0} per bucket and element i's code at byte i of its bucket's payload. The SR codecs
+// draw element j of the pack group at block element i0 from half j of rounding_bits(rng, elem_off + i0),
+// the bits the max-min encoder would use for it; the others ignore rng.
+inline void quantize_block_fp8(const float* acc, const BlockDesc& d, uint8_t* rec, int codec, const RngKey& rng) {
   const uint32_t n = block_n(d);
   const uint32_t B = d.bucket;
   const uint32_t nb = block_num_buckets(n, B);
@@ -210,6 +212,14 @@ inline void quantize_block_fp8(const float* acc, const BlockDesc& d, uint8_t* re
     meta[b] = fp8_meta(mn, mx, codec);
     const float inv = fp8_inv_unit(meta[b].unit, codec);
     uint8_t* dst = pay + (size_t)b * gpb * 8u;
+    if (fp8_sr(codec)) {
+      for (uint32_t i0 = lo; i0 < hi; i0 += 8u) {
+        const Philox4 a = rounding_bits(rng, d.elem_off + i0);
+        for (uint32_t j = 0; j < 8u; ++j)
+          dst[i0 - lo + j] = i0 + j < hi ? (uint8_t)fp8_encode_sr(acc[i0 + j], inv, codec, a.v[j >> 1] >> ((j & 1u) * 16u)) : 0u;
+      }
+      continue;
+    }
     for (uint32_t i = lo; i < lo + div_up(hi - lo, 8u) * 8u; ++i)
       dst[i - lo] = i < hi ? (uint8_t)fp8_encode(acc[i], inv, codec) : 0u;
   }

@@ -100,8 +100,11 @@ int parse_wire_format(const std::string& name, const char* what) {
   if (name == "e5m2") return kE5M2;
   if (name == "e4m3_pow2") return kE4M3Pow2;
   if (name == "e5m2_pow2") return kE5M2Pow2;
+  if (name == "e4m3_sr") return kE4M3SR;
+  if (name == "e5m2_sr") return kE5M2SR;
   throw std::invalid_argument(std::string("cgx: ") + what +
-                              " must be \"maxmin\", \"e4m3\", \"e5m2\", \"e4m3_pow2\" or \"e5m2_pow2\", got \"" +
+                              " must be \"maxmin\", \"e4m3\", \"e5m2\", \"e4m3_pow2\", \"e5m2_pow2\", \"e4m3_sr\" or "
+                              "\"e5m2_sr\", got \"" +
                               name + "\"");
 }
 

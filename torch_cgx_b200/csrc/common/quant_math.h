@@ -157,15 +157,18 @@ CGX_HD uint32_t unpack1(uint64_t w, int j, int bits) {
 // smallest integer >= -126 with max|x| <= FMAX * 2^k (DESIGN §2.13g). x * 2^-k and code * 2^k are
 // exact, so decode(encode(.)) is a projection, and every finite unit is an E8M0 value. A NaN or Inf
 // bucket keeps unit = max|x| and decodes to NaN; a zero bucket has unit 2^-126.
-enum WireCodec : int { kMaxMin = 0, kE4M3 = 1, kE5M2 = 2, kE4M3Pow2 = 3, kE5M2Pow2 = 4 };
+// kE4M3SR / kE5M2SR: the records, units and decoder of kE4M3 / kE5M2; only the encoder differs, it
+// rounds stochastically (fp8_sr_snap, DESIGN §2.13h) with the max-min encoder's random bits.
+enum WireCodec : int { kMaxMin = 0, kE4M3 = 1, kE5M2 = 2, kE4M3Pow2 = 3, kE5M2Pow2 = 4, kE4M3SR = 5, kE5M2SR = 6 };
 
-// the element format of an FP8 codec (kE4M3 or kE5M2), and whether its units are powers of two;
-// constant-folded where the codec is a template argument
+// the element format of an FP8 codec (kE4M3 or kE5M2), whether its units are powers of two, and
+// whether it rounds stochastically; constant-folded where the codec is a template argument
 CGX_HD constexpr int fp8_base(int codec) {
-  return codec == kE4M3Pow2 ? kE4M3 : codec == kE5M2Pow2 ? kE5M2 : codec;
+  return (codec == kE4M3Pow2 || codec == kE4M3SR) ? kE4M3 : (codec == kE5M2Pow2 || codec == kE5M2SR) ? kE5M2 : codec;
 }
 CGX_HD constexpr bool fp8_pow2(int codec) { return codec == kE4M3Pow2 || codec == kE5M2Pow2; }
-CGX_HD constexpr bool is_fp8_codec(int codec) { return codec >= kE4M3 && codec <= kE5M2Pow2; }
+CGX_HD constexpr bool fp8_sr(int codec) { return codec == kE4M3SR || codec == kE5M2SR; }
+CGX_HD constexpr bool is_fp8_codec(int codec) { return codec >= kE4M3 && codec <= kE5M2SR; }
 
 // f(std::integral_constant<int, C>()) for the FP8 codec C equal to `codec`, `otherwise` for any other
 // value: how the launchers turn the runtime codec into the kernels' compile-time one
@@ -176,6 +179,8 @@ R dispatch_fp8(int codec, R otherwise, F&& f) {
     case kE5M2: return f(std::integral_constant<int, kE5M2>());
     case kE4M3Pow2: return f(std::integral_constant<int, kE4M3Pow2>());
     case kE5M2Pow2: return f(std::integral_constant<int, kE5M2Pow2>());
+    case kE4M3SR: return f(std::integral_constant<int, kE4M3SR>());
+    case kE5M2SR: return f(std::integral_constant<int, kE5M2SR>());
     default: return otherwise;
   }
 }
@@ -292,11 +297,10 @@ inline float fp8_to_float_host(uint32_t code, int codec) {
   return (code & 0x80u) ? -v : v;
 }
 
-// steps 4-5 for two elements, the unit the device converts: the code of x0 in bits 0..7, of x1 in
-// bits 8..15 (the order of the 8-bit record). cvt's first source goes to the upper byte.
-CGX_HD uint32_t fp8x2_encode(float x0, float x1, float inv, int codec) {
+// cvt.rn.satfinite of two values already in the format's units: the code of a in bits 0..7, of b
+// in bits 8..15 (the order of the 8-bit record). cvt's first source goes to the upper byte.
+CGX_HD uint32_t fp8x2_cvt(float a, float b, int codec) {
 #if defined(__CUDA_ARCH__)
-  const float a = __fmul_rn(x0, inv), b = __fmul_rn(x1, inv);
   unsigned short h;
   if (fp8_base(codec) == kE5M2)
     asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
@@ -304,8 +308,53 @@ CGX_HD uint32_t fp8x2_encode(float x0, float x1, float inv, int codec) {
     asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(b), "f"(a));
   return h;
 #else
-  return fp8_from_float_host(x0 * inv, codec) | (fp8_from_float_host(x1 * inv, codec) << 8);
+  return fp8_from_float_host(a, codec) | (fp8_from_float_host(b, codec) << 8);
 #endif
+}
+
+// steps 4-5 for two elements, the unit the device converts
+CGX_HD uint32_t fp8x2_encode(float x0, float x1, float inv, int codec) {
+#if defined(__CUDA_ARCH__)
+  return fp8x2_cvt(__fmul_rn(x0, inv), __fmul_rn(x1, inv), codec);
+#else
+  return fp8x2_cvt(x0 * inv, x1 * inv, codec);
+#endif
+}
+
+// Stochastic rounding of y = fp32(x * inv) onto the format's grid (kE4M3SR / kE5M2SR, DESIGN §2.13h),
+// with h the element's 16 random bits: the grid spacing at |y| is s = 2^(max(e, emin) - mb), t = |y| / s
+// = n + f, and |y| becomes (n + 1) * s iff h + floor(2^16 * f) >= 2^16, else n * s: floor(t + h * 2^-16),
+// the rule encode_level applies to max-min levels. The result is y's sign times that grid value, which
+// cvt.rn.satfinite then converts exactly (or saturates); NaN and Inf pass unchanged (-> the NaN code,
+// FMAX), and fp32 subnormals become +-0. Integer operations on the bits of y only, the same on host and
+// device. t's discarded bits are those below bit `shift` of the mantissa with its implicit bit.
+CGX_HD float fp8_sr_snap(float y, uint32_t h, int codec) {
+  const int mb = fp8_base(codec) == kE5M2 ? 2 : 3, emin_b = fp8_base(codec) == kE5M2 ? 127 - 14 : 127 - 6;
+  const uint32_t u = fp32_bits(y), ay = u & 0x7FFFFFFFu, eb = ay >> 23;
+  if (ay >= 0x7F800000u) return y;
+  const uint32_t shift = 23u - (uint32_t)mb + ((int)eb < emin_b ? (uint32_t)(emin_b - (int)eb) : 0u);
+  const uint32_t man = (ay & 0x7FFFFFu) | 0x800000u;
+  // d >= 4, and floor(2^16 f) = (man mod 2^shift) >> d; man < 2^24, so it is 0 once d >= 24: zeros
+  // and fp32 subnormals (shift > 100) round to 0
+  const uint32_t d = shift - 16u;
+  const uint32_t f16 = (man >> (d < 31u ? d : 31u)) & 0xFFFFu;
+  const uint32_t up = ((h & 0xFFFFu) + f16) >> 16;
+  uint32_t r;
+  if (shift <= 23u)
+    r = (ay & ~((1u << shift) - 1u)) + (up << shift);  // n * s, plus s: a carry into the exponent is exact
+  else
+    r = up ? (uint32_t)(emin_b - mb) << 23 : 0u;  // n = 0: 0 or s, the format's smallest subnormal
+  return fp32_from_bits((u & 0x80000000u) | r);
+}
+
+// two elements of an SR codec, with the random bits of each
+CGX_HD uint32_t fp8x2_encode_sr(float x0, float x1, float inv, int codec, uint32_t h0, uint32_t h1) {
+#if defined(__CUDA_ARCH__)
+  const float a = __fmul_rn(x0, inv), b = __fmul_rn(x1, inv);
+#else
+  const float a = x0 * inv, b = x1 * inv;
+#endif
+  return fp8x2_cvt(fp8_sr_snap(a, h0, codec), fp8_sr_snap(b, h1, codec), codec);
 }
 CGX_HD void fp8x2_decode(uint32_t pair, float unit, int codec, float& d0, float& d1) {
 #if defined(__CUDA_ARCH__)
@@ -331,6 +380,9 @@ CGX_HD void fp8x2_decode(uint32_t pair, float unit, int codec, float& d0, float&
 
 // one element (the host codec and the generic paths)
 CGX_HD uint32_t fp8_encode(float x, float inv, int codec) { return fp8x2_encode(x, 0.f, inv, codec) & 0xFFu; }
+CGX_HD uint32_t fp8_encode_sr(float x, float inv, int codec, uint32_t h) {
+  return fp8x2_encode_sr(x, 0.f, inv, codec, h, 0u) & 0xFFu;
+}
 CGX_HD float fp8_decode(uint32_t code, float unit, int codec) {
   float d0, d1;
   fp8x2_decode(code & 0xFFu, unit, codec, d0, d1);

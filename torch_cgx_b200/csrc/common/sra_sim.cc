@@ -23,10 +23,10 @@ void sra_simulate(const Plan& plan, const std::vector<void*>& bufs, float presca
         for (int q = 0; q < W; ++q) {
           if (q == c) continue;
           cpu::load_block(bufs[q], plan.dtype, d, prescale, tmp.data());
-          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec, make_rng_key(rng, q, 0));
           cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
         }
-        cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+        cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec, make_rng_key(rng, c, 1));
         for (int p = 0; p < W; ++p) cpu::decode_block_fp8_store(rec.data(), plan.dtype, d, bufs[p], codec);
         continue;
       }
@@ -58,7 +58,7 @@ void reduce_scatter_simulate(const Plan& plan, const std::vector<const void*>& i
         if (q == c) continue;
         cpu::load_block(in_bufs[q], plan.dtype, d, prescale, tmp.data());
         if (codec != kMaxMin && block_bits(d) < kRawBits) {
-          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+          cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec, make_rng_key(rng, q, 0));
           cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
           continue;
         }
@@ -84,7 +84,7 @@ void oneshot_simulate(const Plan& plan, const std::vector<void*>& bufs, float pr
     for (int q = 0; q < W; ++q) {
       cpu::load_block(bufs[q], plan.dtype, d, prescale, tmp.data());
       if (codec != kMaxMin && block_bits(d) < kRawBits) {
-        cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec);
+        cpu::quantize_block_fp8(tmp.data(), d, rec.data(), codec, make_rng_key(rng, q, 0));
         cpu::decode_block_fp8_add(rec.data(), d, acc.data(), codec);
         continue;
       }
@@ -142,12 +142,12 @@ void all_to_all_simulate(int dtype, const std::vector<const void*>& in_bufs, con
         d.bucket = g.bucket;
         cpu::load_block(src, dtype, d, 1.0f, acc.data());
         if (codes) {
-          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec, key);
           cpu::unpack_block_fp8(rec.data(), d, dst, (*out_scales)[r] + out_off / bucket);
           continue;
         }
         if (codec != kMaxMin) {
-          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+          cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec, key);
           cpu::decode_block_fp8_store(rec.data(), dtype, d, dst, codec);
           continue;
         }
@@ -166,7 +166,7 @@ void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngPa
     const BlockDesc& d = plan.blocks[b];
     cpu::load_block(buf, plan.dtype, d, prescale, acc.data());
     if (codec != kMaxMin && block_bits(d) < kRawBits) {
-      cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+      cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec, make_rng_key(rng, rank, phase));
       cpu::decode_block_fp8_store(rec.data(), plan.dtype, d, buf, codec);
       continue;
     }
@@ -175,7 +175,8 @@ void roundtrip_simulate(const Plan& plan, void* buf, float prescale, const RngPa
   }
 }
 
-void codes_simulate(const Plan& plan, const void* src, uint8_t* codes, float* scales, WireCodec codec) {
+void codes_simulate(const Plan& plan, const void* src, uint8_t* codes, float* scales, WireCodec codec,
+                    const RngKey& rng) {
   if (codec == kMaxMin) throw std::invalid_argument("codes_simulate: needs an FP8 codec");
   std::vector<float> acc(kMaxBlockElems);
   std::vector<uint8_t> rec(kMaxBlockElems * 4 + 64 + kMaxBlockBuckets * 8 + 64);
@@ -183,7 +184,7 @@ void codes_simulate(const Plan& plan, const void* src, uint8_t* codes, float* sc
     if (block_bits(d) != 8 || d.elem_off % d.bucket)
       throw std::invalid_argument("codes_simulate: needs 8-bit blocks that start on a bucket boundary");
     cpu::load_block(src, plan.dtype, d, 1.0f, acc.data());
-    cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec);
+    cpu::quantize_block_fp8(acc.data(), d, rec.data(), codec, rng);
     cpu::unpack_block_fp8(rec.data(), d, codes, scales);
   }
 }

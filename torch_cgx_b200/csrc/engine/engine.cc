@@ -312,7 +312,7 @@ void AllreduceEngine::sharded(bool cuda, ShardedOp op, const void* in, void* out
   if (fused) fused_->check_status();
   if (shard_numel <= 0) return;
   check_sharded_buffers(op, shard_layers, dtype, in, out, (uint64_t)shard_numel, rank_, world_, codec, out_scales);
-  if (codec != kMaxMin && rng_in.stochastic)
+  if (codec != kMaxMin && !fp8_sr(codec) && rng_in.stochastic)
     throw std::invalid_argument(title + ": the FP8 formats round to nearest only");
   if (!fused && (L > 1 || N == 1) && !g.intra)
     throw std::runtime_error(title + (L > 1 ? " has no intra-node reducer" : " of one rank needs the P2P transport"));
@@ -381,7 +381,7 @@ void AllreduceEngine::all_to_all(bool cuda, const void* in, void* out, const std
     if (!cuda) throw std::runtime_error("cgx: the compressed all_to_all over several nodes needs device memory");
     check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, rank_, world_, route, out_scales);
     if (routed) throw std::logic_error("cgx: a routed all_to_all reached a path that does not route rows");
-    if (codec != kMaxMin && rng_in.stochastic)
+    if (codec != kMaxMin && !fp8_sr(codec) && rng_in.stochastic)
       throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
     if (!g.world_comm) throw std::runtime_error("cgx: the compressed all_to_all over several nodes has no world communicator");
     if (!fused && local_size_ > 1 && !g.intra)
@@ -680,7 +680,8 @@ void AllreduceEngine::run_layers(bool cuda, void* data, int dtype, std::vector<L
   const bool multi_node = nodes() > 1;
   const WireCodec codec = (WireCodec)env.codec;
   if (codec != kMaxMin) {  // checked before anything is counted or sent
-    if (env.stochastic) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
+    if (env.stochastic && !fp8_sr(codec))
+      throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
     for (const LayerSpec& l : layers)
       if (l.bits != 8 && l.bits < kRawBits)
         throw std::invalid_argument("cgx allreduce: an FP8 format needs layers of bits 8 or 32, got " +

@@ -261,41 +261,43 @@ __device__ __noinline__ void a2a_send_scaled_unaligned(const T* __restrict__ src
   slice_load_scalar<T, GPL>(src, x);
   slice_scale_round<GPL, T>(x, s);
   if constexpr (CODEC != kMaxMin)
-    full_send_fp8_x<CODEC, GPL>(x, it, ds);
+    full_send_fp8_x<CODEC, GPL>(x, it, rng, ds);
   else
     full_send_x<T, KB, GPL, false, false>(x, it, 1.0f, rng, ds, (T*)nullptr);
 }
 
-// one item of a chunk in an FP8 codec (KB 8 records, round to nearest): to a peer's slot (OneDst),
-// or to the codes output (CodesDst)
+// one item of a chunk in an FP8 codec (KB 8 records; the SR codecs draw from the pair's key `rng`):
+// to a peer's slot (OneDst), or to the codes output (CodesDst)
 template <typename T, int CODEC, int GPL, typename DST>
-__device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& it, const DST& push) {
+__device__ __forceinline__ void a2a_send_item_fp8(const T* src, const WarpItem& it, const RngKey& rng,
+                                                  const DST& push) {
   if (item_kind(it) == kItemFull) {
     if (group_aligned<T>(src)) {
       float x[GPL][8];
       slice_load_vec<T, GPL>(src, x);
-      full_send_fp8_x<CODEC, GPL>(x, it, push);
+      full_send_fp8_x<CODEC, GPL>(x, it, rng, push);
     } else {
-      full_send_fp8_unaligned<T, CODEC, GPL>(src, it, push);
+      full_send_fp8_unaligned<T, CODEC, GPL>(src, it, rng, push);
     }
   } else {
-    bucket_quantize_fp8<T, CODEC>(src, it, push);
+    bucket_quantize_fp8<T, CODEC>(src, it, rng, push);
   }
 }
 // the same for the values T(x * s) (SCALE)
 template <typename T, int CODEC, int GPL, typename DST>
-__device__ __forceinline__ void a2a_send_item_fp8_scaled(const T* src, const WarpItem& it, const DST& push, float s) {
+__device__ __forceinline__ void a2a_send_item_fp8_scaled(const T* src, const WarpItem& it, const RngKey& rng,
+                                                         const DST& push, float s) {
   if (item_kind(it) == kItemFull) {
     if (group_aligned<T>(src)) {
       float x[GPL][8];
       slice_load_vec<T, GPL>(src, x);
       slice_scale_round<GPL, T>(x, s);
-      full_send_fp8_x<CODEC, GPL>(x, it, push);
+      full_send_fp8_x<CODEC, GPL>(x, it, rng, push);
     } else {
-      a2a_send_scaled_unaligned<T, 8, GPL, CODEC, DST>(src, it, s, RngKey{}, push);
+      a2a_send_scaled_unaligned<T, 8, GPL, CODEC, DST>(src, it, s, rng, push);
     }
   } else {
-    bucket_quantize_fp8_rounded<T, CODEC>(src, it, s, push);
+    bucket_quantize_fp8_rounded<T, CODEC>(src, it, s, rng, push);
   }
 }
 template <typename T, int CODEC, int GPL>
@@ -318,7 +320,7 @@ template <typename T, int KB, int GPL, int CODEC>
 __device__ __forceinline__ void a2a_send_item_scaled(const T* src, const WarpItem& it, float s, const RngKey& rng,
                                                      const OneDst& push) {
   if constexpr (CODEC != kMaxMin) {
-    a2a_send_item_fp8_scaled<T, CODEC, GPL, OneDst>(src, it, push, s);
+    a2a_send_item_fp8_scaled<T, CODEC, GPL, OneDst>(src, it, rng, push, s);
     return;
   }
   const uint32_t kind = item_kind(it);
@@ -366,7 +368,7 @@ __device__ __forceinline__ void a2a_send_window(const A2aParams& p, int q, uint3
       continue;
     }
     if constexpr (CODEC != kMaxMin) {
-      a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, push);
+      a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, rng, push);
       continue;
     }
     const uint32_t kind = item_kind(it);
@@ -397,9 +399,9 @@ __device__ __forceinline__ float* a2a_scales_addr(const A2aParams& p, const uint
 }
 
 // codes output, my own chunk: every item through the peers' FP8 encoder, straight into (codes,
-// scales), one warp per item over the whole grid
+// scales), one warp per item over the whole grid; `rng` is the key of the pair (r, r)
 template <typename T, int GPL, bool IDX, int CODEC>
-__device__ __forceinline__ void a2a_encode_own(const A2aParams& p) {
+__device__ __forceinline__ void a2a_encode_own(const A2aParams& p, const RngKey& rng) {
   const int r = p.rank;
   const A2aGeom g = a2a_geom(p.in_cnt[r], p.bits, p.bucket, (int)sizeof(T));
   const uint32_t nb = a2a_num_blocks(g), total = nb * g.block_items, nwarps = gridDim.x * kSraWarps;
@@ -417,7 +419,7 @@ __device__ __forceinline__ void a2a_encode_own(const A2aParams& p) {
     uint8_t* codes = a2a_codes_addr(p, IDX, p.out_off[r] + it.elem_off);
     if (codes == nullptr) continue;
     const CodesDst ds{codes, a2a_scales_addr(p, codes), it.meta_off, it.pay_off, item_n(it)};
-    a2a_send_item_fp8<T, CODEC, GPL, CodesDst>(src, it, ds);
+    a2a_send_item_fp8<T, CODEC, GPL, CodesDst>(src, it, rng, ds);
   }
 }
 
@@ -538,12 +540,16 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) a2a_kernel(const _
 
   // my own chunk last: the pushes to the peers are on the critical path, the copy is not
   if (!s_abort) {
-    if constexpr (CODES)
-      a2a_encode_own<T, GPL, IDX, CODEC>(p);
-    else if constexpr (IDX)
+    if constexpr (CODES) {
+      RngKey rng = p.rng;
+      rng.seq += epoch - p.epoch_hint;
+      rng.stream = a2a_rng_stream(p.rank_base + r, p.rank_base + r);
+      a2a_encode_own<T, GPL, IDX, CODEC>(p, rng);
+    } else if constexpr (IDX) {
       a2a_copy_own_rows<T, COMBINE, SCALE>(p);
-    else
+    } else {
       a2a_copy_own<T>(p);
+    }
   }
 
   // slot handshake, as in rs_kernel: every lane, whether or not it had windows

@@ -38,12 +38,12 @@ __global__ void __launch_bounds__(kSraThreads) a2a_pack_kernel(const __grid_cons
     const int i = a2a_remote_item<T>(p, t, it, rec);
     const T* src = reinterpret_cast<const T*>(p.in) + p.elem_off[i] + it.elem_off;
     const OneDst push{reinterpret_cast<uint8_t*>(p.out) + rec};
-    if constexpr (CODEC != kMaxMin) {
-      a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, push);
-      continue;
-    }
     RngKey rng = p.rng;
     rng.stream = a2a_rng_stream(p.rank, p.peer[i]);
+    if constexpr (CODEC != kMaxMin) {
+      a2a_send_item_fp8<T, CODEC, GPL, OneDst>(src, it, rng, push);
+      continue;
+    }
     if (item_kind(it) == kItemFull) {
       if (group_aligned<T>(src)) {
         float x[GPL][8];

@@ -164,11 +164,12 @@ accumulate_items_kernel(const uint8_t* __restrict__ wire, const WarpItem* __rest
 
 // The FP8 codecs of an 8-bit plan (the generic all-to-all, reduce-scatter and all-gather):
 // wire = quantize(src * prescale), dst = decode(wire), acc (+)= decode(wire). Plain T tensors, round
-// to nearest; the items are all compressed (the reducers pass raw layers to the max-min kernels).
+// to nearest (the SR codecs: stochastically, with `rng`); the items are all compressed (the reducers
+// pass raw layers to the max-min kernels). The SR codecs decode with their base format's kernels.
 template <typename T, int CODEC, int GPL>
 __global__ void __launch_bounds__(kThreads, 3)
 quantize_items_fp8_kernel(const T* __restrict__ src, const WarpItem* __restrict__ items, uint32_t first,
-                          uint32_t count, uint8_t* wire, float prescale) {
+                          uint32_t count, uint8_t* wire, float prescale, const RngKey rng) {
   const OneDst ds{wire};
   CGX_ITEM_LOOP(it) {
     const T* s = src + it.elem_off;
@@ -177,12 +178,12 @@ quantize_items_fp8_kernel(const T* __restrict__ src, const WarpItem* __restrict_
         float x[GPL][8];
         slice_load_vec<T, GPL>(s, x);
         slice_scale<GPL>(x, prescale);
-        full_send_fp8_x<CODEC, GPL>(x, it, ds);
+        full_send_fp8_x<CODEC, GPL>(x, it, rng, ds);
       } else {
-        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(s, it, prescale, ds, (T*)nullptr);
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(s, it, prescale, rng, ds, (T*)nullptr);
       }
     } else {
-      bucket_send_fp8<T, T, CODEC>(s, it, prescale, ds, (T*)nullptr);
+      bucket_send_fp8<T, T, CODEC>(s, it, prescale, rng, ds, (T*)nullptr);
     }
   }
 }
@@ -330,32 +331,40 @@ cudaError_t dequantize_t(const ItemKernelArgs& a, const uint8_t* wire, T* dst, c
   return cudaGetLastError();
 }
 
-// CODEC x GPL dispatch of the FP8 kernels (8-bit plans only)
-#define CGX_DISPATCH_FP8(a, CALL)                                  \
+// CODEC x GPL dispatch of the FP8 kernels (8-bit plans only); the SR codecs only where the kernel
+// encodes (SR: true)
+#define CGX_DISPATCH_FP8_SR(a, SR, CALL)                           \
   do {                                                             \
     if ((a).uniform_bits != 8) return cudaErrorInvalidValue;       \
     const bool g4_ = (a).slice_elems == 1024;                      \
-    if ((a).codec == kE4M3) {                                      \
+    const int c_ = (SR) ? (a).codec : fp8_base((a).codec);         \
+    if (c_ == kE4M3) {                                             \
       if (g4_) { CALL(kE4M3, 4); } else { CALL(kE4M3, 2); }       \
-    } else if ((a).codec == kE5M2) {                               \
+    } else if (c_ == kE5M2) {                                      \
       if (g4_) { CALL(kE5M2, 4); } else { CALL(kE5M2, 2); }       \
-    } else if ((a).codec == kE4M3Pow2) {                           \
+    } else if (c_ == kE4M3Pow2) {                                  \
       if (g4_) { CALL(kE4M3Pow2, 4); } else { CALL(kE4M3Pow2, 2); } \
-    } else if ((a).codec == kE5M2Pow2) {                           \
+    } else if (c_ == kE5M2Pow2) {                                  \
       if (g4_) { CALL(kE5M2Pow2, 4); } else { CALL(kE5M2Pow2, 2); } \
+    } else if ((SR) && c_ == kE4M3SR) {                            \
+      if (g4_) { CALL(kE4M3SR, 4); } else { CALL(kE4M3SR, 2); }   \
+    } else if ((SR) && c_ == kE5M2SR) {                            \
+      if (g4_) { CALL(kE5M2SR, 4); } else { CALL(kE5M2SR, 2); }   \
     } else {                                                       \
       return cudaErrorInvalidValue;                                \
     }                                                              \
   } while (0)
+#define CGX_DISPATCH_FP8(a, CALL) CGX_DISPATCH_FP8_SR(a, false, CALL)
 
 template <typename T>
-cudaError_t quantize_fp8_t(const ItemKernelArgs& a, const T* src, uint8_t* wire, float prescale,
+cudaError_t quantize_fp8_t(const ItemKernelArgs& a, const T* src, uint8_t* wire, float prescale, const RngKey& rng,
                            cudaStream_t stream) {
   if (a.count == 0) return cudaSuccess;
   const int grid = grid_for(a.count);
-#define CGX_CALL(C_, GPL_) \
-  quantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(src, a.items, a.first, a.count, wire, prescale)
-  CGX_DISPATCH_FP8(a, CGX_CALL);
+#define CGX_CALL(C_, GPL_)                                                                                      \
+  quantize_items_fp8_kernel<T, C_, GPL_><<<grid, kThreads, 0, stream>>>(src, a.items, a.first, a.count, wire, prescale, \
+                                                                        rng)
+  CGX_DISPATCH_FP8_SR(a, true, CGX_CALL);
 #undef CGX_CALL
   return cudaGetLastError();
 }
@@ -410,10 +419,10 @@ cudaError_t accumulate_t(const ItemKernelArgs& a, const uint8_t* wire, float* ac
 cudaError_t launch_quantize_items(const ItemKernelArgs& a, const void* src, uint8_t* wire, float prescale,
                                   const RngKey& rng, cudaStream_t stream) {
   if (a.codec != kMaxMin) {
-    if (rng.enabled) return cudaErrorInvalidValue;
-    CGX_BY_DTYPE(a.dtype, (quantize_fp8_t<float>(a, (const float*)src, wire, prescale, stream)),
-                 (quantize_fp8_t<__half>(a, (const __half*)src, wire, prescale, stream)),
-                 (quantize_fp8_t<__nv_bfloat16>(a, (const __nv_bfloat16*)src, wire, prescale, stream)))
+    if (rng.enabled && !fp8_sr(a.codec)) return cudaErrorInvalidValue;
+    CGX_BY_DTYPE(a.dtype, (quantize_fp8_t<float>(a, (const float*)src, wire, prescale, rng, stream)),
+                 (quantize_fp8_t<__half>(a, (const __half*)src, wire, prescale, rng, stream)),
+                 (quantize_fp8_t<__nv_bfloat16>(a, (const __nv_bfloat16*)src, wire, prescale, rng, stream)))
   }
   CGX_BY_DTYPE(a.dtype,
                (quantize_t<float, float>(a, (const float*)src, 0, wire, prescale, rng, nullptr, stream)),
@@ -427,8 +436,8 @@ cudaError_t launch_quantize_items_f32(const ItemKernelArgs& a, const float* src_
   if (a.codec != kMaxMin) {
     // the FP8 kernels of an fp32 tensor, on the scratch seen from the tensor's element 0 (items
     // address src + elem_off), then out = decode(wire)
-    if (rng.enabled) return cudaErrorInvalidValue;
-    cudaError_t e = quantize_fp8_t<float>(a, src_f32 - base_elem, wire, 1.0f, stream);
+    if (rng.enabled && !fp8_sr(a.codec)) return cudaErrorInvalidValue;
+    cudaError_t e = quantize_fp8_t<float>(a, src_f32 - base_elem, wire, 1.0f, rng, stream);
     if (e != cudaSuccess || out == nullptr) return e;
     return launch_dequantize_items(a, wire, out, stream);
   }

@@ -827,7 +827,9 @@ __device__ __noinline__ void raw_ag_recv(const SrcSet ss, const WarpItem it, T* 
 // whose meta is {unit, +0} and whose byte j of a group is element j's FP8 code. Same slices, same
 // min/max reductions and the same 8-bit word loads and stores as max-min; only the element
 // arithmetic differs: one FMUL + half a cvt.satfinite per element to encode, half a cvt.f16x2 +
-// one F2F + one FMUL to decode. Round to nearest only.
+// one F2F + one FMUL to decode. The SR codecs (fp8_sr) add one Philox call per group of 8 and a few
+// integer operations per element (fp8_sr_snap); every encoder takes the key and the item's element
+// index, which the round-to-nearest codecs ignore.
 // ======================================================================================
 // per-row NaN-propagating min / max of the bucket each row of the slice belongs to (slice_meta's
 // reductions)
@@ -858,11 +860,22 @@ __device__ __forceinline__ void slice_minmax(const float (&x)[GPL][8], uint32_t 
   }
 }
 
-// 8 values of one group -> their codes, element j in byte j of (lo, hi)
+// 8 values of one group -> their codes, element j in byte j of (lo, hi). An SR codec rounds element j
+// with half j of the Philox word of the group's first element `first` (quantize_block_fp8's bits).
 template <int CODEC>
-__device__ __forceinline__ void fp8_encode8(const float (&x)[8], float inv, uint32_t& lo, uint32_t& hi) {
-  const uint32_t p0 = fp8x2_encode(x[0], x[1], inv, CODEC), p1 = fp8x2_encode(x[2], x[3], inv, CODEC);
-  const uint32_t p2 = fp8x2_encode(x[4], x[5], inv, CODEC), p3 = fp8x2_encode(x[6], x[7], inv, CODEC);
+__device__ __forceinline__ void fp8_encode8(const float (&x)[8], float inv, const RngKey& rng, uint32_t first,
+                                            uint32_t& lo, uint32_t& hi) {
+  uint32_t p0, p1, p2, p3;
+  if constexpr (fp8_sr(CODEC)) {
+    const Philox4 a = rounding_word(rng, first);
+    p0 = fp8x2_encode_sr(x[0], x[1], inv, CODEC, a.v[0], a.v[0] >> 16);
+    p1 = fp8x2_encode_sr(x[2], x[3], inv, CODEC, a.v[1], a.v[1] >> 16);
+    p2 = fp8x2_encode_sr(x[4], x[5], inv, CODEC, a.v[2], a.v[2] >> 16);
+    p3 = fp8x2_encode_sr(x[6], x[7], inv, CODEC, a.v[3], a.v[3] >> 16);
+  } else {
+    p0 = fp8x2_encode(x[0], x[1], inv, CODEC), p1 = fp8x2_encode(x[2], x[3], inv, CODEC);
+    p2 = fp8x2_encode(x[4], x[5], inv, CODEC), p3 = fp8x2_encode(x[6], x[7], inv, CODEC);
+  }
   lo = __byte_perm(p0, p1, 0x5410);
   hi = __byte_perm(p2, p3, 0x5410);
 }
@@ -877,30 +890,33 @@ __device__ __forceinline__ void fp8_decode8(uint32_t lo, uint32_t hi, float unit
 // full item, values already in registers: meta + codes to the destination; the codes stay in
 // (lo, hi) and the units in m for a caller that decodes them itself
 template <int CODEC, int GPL, typename DST>
-__device__ __forceinline__ void full_send_fp8_codes(const float (&x)[GPL][8], const WarpItem& it, const DST& ds,
-                                                    BucketMeta (&m)[GPL], uint32_t (&lo)[GPL], uint32_t (&hi)[GPL]) {
+__device__ __forceinline__ void full_send_fp8_codes(const float (&x)[GPL][8], const WarpItem& it, const RngKey& rng,
+                                                    const DST& ds, BucketMeta (&m)[GPL], uint32_t (&lo)[GPL],
+                                                    uint32_t (&hi)[GPL]) {
   const uint32_t lg = item_lpb_log2(it);
   float mn[GPL], mx[GPL];
   slice_minmax<GPL>(x, lg, mn, mx);
 #pragma unroll
   for (int k = 0; k < GPL; ++k) {
     m[k] = fp8_meta(mn[k], mx[k], CODEC);
-    fp8_encode8<CODEC>(x[k], fp8_inv_unit(m[k].unit, CODEC), lo[k], hi[k]);
+    fp8_encode8<CODEC>(x[k], fp8_inv_unit(m[k].unit, CODEC), rng, it.elem_off + lane_group<GPL>(k) * 8u, lo[k], hi[k]);
   }
   slice_store_meta<GPL>(m, lg, ds, it.meta_off);
   store_words<8, GPL>(ds, it.pay_off, 8, lo, hi);
 }
 template <int CODEC, int GPL, typename DST>
-__device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds) {
+__device__ __forceinline__ void full_send_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const RngKey& rng,
+                                                const DST& ds) {
   BucketMeta m[GPL];
   uint32_t lo[GPL], hi[GPL];
-  full_send_fp8_codes<CODEC, GPL>(x, it, ds, m, lo, hi);
+  full_send_fp8_codes<CODEC, GPL>(x, it, rng, ds, m, lo, hi);
 }
 template <typename TS, int CODEC, int GPL, typename DST>
-__device__ __noinline__ void full_send_fp8_unaligned(const TS* __restrict__ src, const WarpItem it, const DST ds) {
+__device__ __noinline__ void full_send_fp8_unaligned(const TS* __restrict__ src, const WarpItem it, const RngKey rng,
+                                                     const DST ds) {
   float x[GPL][8];
   slice_load_scalar<TS, GPL>(src, x);
-  full_send_fp8_x<CODEC, GPL>(x, it, ds);
+  full_send_fp8_x<CODEC, GPL>(x, it, rng, ds);
 }
 
 // out = decode(already fetched words of ONE source)
@@ -924,7 +940,7 @@ __device__ __noinline__ void full_recv_fp8_unaligned(const uint8_t* rec, const W
 // ROUND: as bucket_load_group
 template <typename TS, typename TO, int CODEC, typename DST, bool ROUND = false>
 __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, const WarpItem& it, float prescale,
-                                                const DST& ds, TO* __restrict__ self_out) {
+                                                const RngKey& rng, const DST& ds, TO* __restrict__ self_out) {
   const uint32_t n = item_n(it);
   const uint32_t ng = div_up(n, 8u);
   float mn = CGX_INF_POS, mx = CGX_INF_NEG;
@@ -944,7 +960,7 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
     int nv;
     bucket_load_group<TS, ROUND>(src, g, n, prescale, x, nv);
     uint32_t lo, hi;
-    fp8_encode8<CODEC>(x, inv, lo, hi);
+    fp8_encode8<CODEC>(x, inv, rng, it.elem_off + g * 8u, lo, hi);
     const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
     const uint32_t o = it.pay_off + g * 8u;
     for (int t = 0; t < 8; ++t) dst_st_u8(du, o + t, (uint32_t)(w >> (8 * t)) & 0xFFu);
@@ -956,14 +972,15 @@ __device__ __forceinline__ void bucket_fp8_body(const TS* __restrict__ src, cons
   }
 }
 template <typename TS, int CODEC, typename DST>
-__device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const DST ds) {
-  bucket_fp8_body<TS, float, CODEC>(src, it, 1.0f, ds, (float*)nullptr);
+__device__ __noinline__ void bucket_quantize_fp8(const TS* __restrict__ src, const WarpItem it, const RngKey rng,
+                                                 const DST ds) {
+  bucket_fp8_body<TS, float, CODEC>(src, it, 1.0f, rng, ds, (float*)nullptr);
 }
 // the same for the bucket of TS(src * scale) (scale_round)
 template <typename TS, int CODEC, typename DST>
 __device__ __noinline__ void bucket_quantize_fp8_rounded(const TS* __restrict__ src, const WarpItem it, float scale,
-                                                         const DST ds) {
-  bucket_fp8_body<TS, float, CODEC, DST, true>(src, it, scale, ds, (float*)nullptr);
+                                                         const RngKey rng, const DST ds) {
+  bucket_fp8_body<TS, float, CODEC, DST, true>(src, it, scale, rng, ds, (float*)nullptr);
 }
 
 template <typename TO, int CODEC>
@@ -1092,11 +1109,11 @@ __device__ __forceinline__ void fp8_unpack_item(const uint8_t* rec, const WarpIt
 // full item, values in registers and already prescaled: publish meta + codes, and the decoded
 // values to `out` (VEC: group aligned)
 template <typename TO, int CODEC, int GPL, bool VEC, typename DST>
-__device__ __forceinline__ void full_publish_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const DST& ds,
-                                                   TO* __restrict__ out) {
+__device__ __forceinline__ void full_publish_fp8_x(const float (&x)[GPL][8], const WarpItem& it, const RngKey& rng,
+                                                   const DST& ds, TO* __restrict__ out) {
   BucketMeta m[GPL];
   uint32_t lo[GPL], hi[GPL];
-  full_send_fp8_codes<CODEC, GPL>(x, it, ds, m, lo, hi);
+  full_send_fp8_codes<CODEC, GPL>(x, it, rng, ds, m, lo, hi);
   float d[GPL][8];
 #pragma unroll
   for (int k = 0; k < GPL; ++k) fp8_decode8<CODEC>(lo[k], hi[k], m[k].unit, d[k]);
@@ -1105,20 +1122,21 @@ __device__ __forceinline__ void full_publish_fp8_x(const float (&x)[GPL][8], con
 // unaligned full item of src * prescale; SELF: also the decoded values to `self_out`
 template <typename TS, typename TO, int CODEC, int GPL, bool SELF, typename DST>
 __device__ __noinline__ void full_send_fp8_scaled_unaligned(const TS* __restrict__ src, const WarpItem it,
-                                                            float prescale, const DST ds, TO* __restrict__ self_out) {
+                                                            float prescale, const RngKey rng, const DST ds,
+                                                            TO* __restrict__ self_out) {
   float x[GPL][8];
   slice_load_scalar<TS, GPL>(src, x);
   slice_scale<GPL>(x, prescale);
   if (SELF)
-    full_publish_fp8_x<TO, CODEC, GPL, false>(x, it, ds, self_out);
+    full_publish_fp8_x<TO, CODEC, GPL, false>(x, it, rng, ds, self_out);
   else
-    full_send_fp8_x<CODEC, GPL>(x, it, ds);
+    full_send_fp8_x<CODEC, GPL>(x, it, rng, ds);
 }
 // generic bucket item of src * prescale; self_out != nullptr: also the decoded values there
 template <typename TS, typename TO, int CODEC, typename DST>
 __device__ __noinline__ void bucket_send_fp8(const TS* __restrict__ src, const WarpItem it, float prescale,
-                                             const DST ds, TO* __restrict__ self_out) {
-  bucket_fp8_body<TS, TO, CODEC>(src, it, prescale, ds, self_out);
+                                             const RngKey rng, const DST ds, TO* __restrict__ self_out) {
+  bucket_fp8_body<TS, TO, CODEC>(src, it, prescale, rng, ds, self_out);
 }
 
 // x = fl(x + fl(float(code) * unit)) for every source of the set, in slot order; the words of
@@ -1205,24 +1223,24 @@ __device__ __noinline__ void bucket_rs_fp8(const T* src, const WarpItem it, floa
 // ======================================================================================
 template <typename T, int CODEC, int GPL, bool VEC, typename DST>
 __device__ __forceinline__ void full_reduce_fp8_x(float (&x)[GPL][8], T* __restrict__ blk, const WarpItem& it,
-                                                  float prescale, const SrcSet& ss, const DST& ds) {
+                                                  float prescale, const RngKey& rng, const SrcSet& ss, const DST& ds) {
   slice_scale<GPL>(x, prescale);
   slice_accumulate_fp8<CODEC, GPL>(ss, it.meta_off, it.pay_off, item_lpb_log2(it), x);
-  full_publish_fp8_x<T, CODEC, GPL, VEC>(x, it, ds, blk);
+  full_publish_fp8_x<T, CODEC, GPL, VEC>(x, it, rng, ds, blk);
 }
 template <typename T, int CODEC, int GPL, typename DST>
 __device__ __noinline__ void full_reduce_fp8_unaligned(T* __restrict__ blk, const WarpItem it, float prescale,
-                                                       const SrcSet ss, const DST ds) {
+                                                       const RngKey rng, const SrcSet ss, const DST ds) {
   float x[GPL][8];
   slice_load_scalar<T, GPL>(blk, x);
-  full_reduce_fp8_x<T, CODEC, GPL, false>(x, blk, it, prescale, ss, ds);
+  full_reduce_fp8_x<T, CODEC, GPL, false>(x, blk, it, prescale, rng, ss, ds);
 }
 
 // generic bucket item: two passes (min/max of the sums, then encode), as bucket_quantize; every
 // lane reads a group of `blk` before it writes the same group
 template <typename T, int CODEC, typename DST>
 __device__ __noinline__ void bucket_reduce_fp8(T* __restrict__ blk, const WarpItem it, float prescale,
-                                               const SrcSet ss, const DST ds) {
+                                               const RngKey rng, const SrcSet ss, const DST ds) {
   const uint32_t n = item_n(it);
   const uint32_t ng = div_up(n, 8u);
   float mn = CGX_INF_POS, mx = CGX_INF_NEG;
@@ -1244,7 +1262,7 @@ __device__ __noinline__ void bucket_reduce_fp8(T* __restrict__ blk, const WarpIt
     bucket_load_group<T>(blk, g, n, prescale, x, nv);
     bucket_add_sources_fp8<CODEC>(ss, it, g, x);
     uint32_t lo, hi;
-    fp8_encode8<CODEC>(x, inv, lo, hi);
+    fp8_encode8<CODEC>(x, inv, rng, it.elem_off + g * 8u, lo, hi);
     const uint64_t w = ((uint64_t)hi << 32 | lo) & (nv >= 8 ? ~0ull : (1ull << (8 * nv)) - 1ull);
     const uint32_t o = it.pay_off + g * 8u;
     for (int t = 0; t < 8; ++t) dst_st_u8(du, o + t, (uint32_t)(w >> (8 * t)) & 0xFFu);

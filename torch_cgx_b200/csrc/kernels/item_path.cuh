@@ -434,13 +434,17 @@ __device__ __forceinline__ void store_words(const DST& ds, uint32_t pay_off, int
   }
 }
 
-// stochastic rounding offsets of one group from its Philox word (host twin: rounding_from_bits).
-// The keys are made opaque per call: otherwise the ten round keys become loop invariants that the
-// compiler hoists out of the item loops -- 18 registers the deterministic path needs.
-__device__ __forceinline__ void rounding8(const RngKey& rng, uint32_t first_elem, float (&r)[8]) {
+// the Philox word of one group (host twin: rounding_bits). The keys are made opaque per call:
+// otherwise the ten round keys become loop invariants that the compiler hoists out of the item
+// loops -- 18 registers the deterministic path needs.
+__device__ __forceinline__ Philox4 rounding_word(const RngKey& rng, uint32_t first_elem) {
   uint32_t k0 = rng.seed_lo ^ (rng.stream * 0x9E3779B9u), k1 = rng.seed_hi;
   asm volatile("" : "+r"(k0), "+r"(k1));
-  const Philox4 a = philox4x32_10(first_elem, 0u, 0u, rng.seq, k0, k1);
+  return philox4x32_10(first_elem, 0u, 0u, rng.seq, k0, k1);
+}
+// stochastic rounding offsets of one group from its Philox word (host twin: rounding_from_bits)
+__device__ __forceinline__ void rounding8(const RngKey& rng, uint32_t first_elem, float (&r)[8]) {
+  const Philox4 a = rounding_word(rng, first_elem);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const uint32_t h = (a.v[j >> 1] >> ((j & 1) * 16)) & 0xFFFFu;

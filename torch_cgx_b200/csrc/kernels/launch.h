@@ -118,7 +118,7 @@ struct A2aParams {
   uint32_t row;
   uint64_t in_rows;
   uint64_t out_rows;
-  int codec;                       // WireCodec (common/quant_math.h); FP8 codecs need bits 8, round to nearest
+  int codec;                       // WireCodec (common/quant_math.h); FP8 codecs need bits 8 (SR codecs: rng)
   // nullptr: `out` receives the decoded values (T). Otherwise (FP8 codecs only) `out` receives one
   // FP8 code byte per element and out_scales[e / bucket] the unit of the bucket starting at output
   // element e, every chunk -- the own one included -- encoded; counts and rows hold whole buckets.

@@ -252,15 +252,15 @@ __device__ __forceinline__ void sra_phase_a(const SraParams& p, const LaneItems&
     if constexpr (CODEC != kMaxMin) {
       if (hot == 1) {
         slice_scale<GPL>(x, p.prescale);
-        full_send_fp8_x<CODEC, GPL>(x, it, push);
+        full_send_fp8_x<CODEC, GPL>(x, it, rng, push);
         return;
       }
       if (kind == kItemFull) {
-        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, push, (T*)nullptr);
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, rng, push, (T*)nullptr);
         return;
       }
       if (kind == kItemBucket) {
-        bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, push, (T*)nullptr);
+        bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, rng, push, (T*)nullptr);
         return;
       }
     }
@@ -338,13 +338,13 @@ __device__ __forceinline__ void sra_phase_b(const SraParams& p, const LaneItems&
     if constexpr (CODEC != kMaxMin) {
       if (kind == kItemFull) {
         if (al)
-          full_reduce_fp8_x<T, CODEC, GPL, true>(x, blk, it, p.prescale, ss, ds);
+          full_reduce_fp8_x<T, CODEC, GPL, true>(x, blk, it, p.prescale, rng, ss, ds);
         else
-          full_reduce_fp8_unaligned<T, CODEC, GPL>(blk, it, p.prescale, ss, ds);
+          full_reduce_fp8_unaligned<T, CODEC, GPL>(blk, it, p.prescale, rng, ss, ds);
         continue;
       }
       if (kind == kItemBucket) {
-        bucket_reduce_fp8<T, CODEC>(blk, it, p.prescale, ss, ds);
+        bucket_reduce_fp8<T, CODEC>(blk, it, p.prescale, rng, ss, ds);
         continue;
       }
     }
@@ -592,15 +592,15 @@ __global__ void __launch_bounds__(kSraThreads, kSraCtasPerSm) oneshot_kernel(con
       if constexpr (CODEC != kMaxMin) {
         if (hot == 1) {
           slice_scale<GPL>(x, p.prescale);
-          full_send_fp8_x<CODEC, GPL>(x, it, ds);
+          full_send_fp8_x<CODEC, GPL>(x, it, rng, ds);
           continue;
         }
         if (kind == kItemFull) {
-          full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, ds, (T*)nullptr);
+          full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(blk, it, p.prescale, rng, ds, (T*)nullptr);
           continue;
         }
         if (kind == kItemBucket) {
-          bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, ds, (T*)nullptr);
+          bucket_send_fp8<T, T, CODEC>(blk, it, p.prescale, rng, ds, (T*)nullptr);
           continue;
         }
       }
@@ -798,23 +798,23 @@ __device__ __forceinline__ void ag_publish(const SraParams& p, const LaneItems& 
                                              item_n(it)}};
       if (kind == kItemFull && al) {
         slice_scale<GPL>(x, p.prescale);
-        full_send_fp8_x<CODEC, GPL>(x, it, td);
+        full_send_fp8_x<CODEC, GPL>(x, it, rng, td);
       } else if (kind == kItemFull) {
-        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(src, it, p.prescale, td, (T*)nullptr);
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, false>(src, it, p.prescale, rng, td, (T*)nullptr);
       } else {
-        bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, td, (T*)nullptr);
+        bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, rng, td, (T*)nullptr);
       }
       continue;
     }
     if (CODEC != kMaxMin && kind == kItemFull) {
       if (al) {
         slice_scale<GPL>(x, p.prescale);
-        full_publish_fp8_x<T, CODEC, GPL, true>(x, it, ds, dst);
+        full_publish_fp8_x<T, CODEC, GPL, true>(x, it, rng, ds, dst);
       } else {
-        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, true>(src, it, p.prescale, ds, dst);
+        full_send_fp8_scaled_unaligned<T, T, CODEC, GPL, true>(src, it, p.prescale, rng, ds, dst);
       }
     } else if (CODEC != kMaxMin && kind == kItemBucket) {
-      bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, ds, dst);
+      bucket_send_fp8<T, T, CODEC>(src, it, p.prescale, rng, ds, dst);
     } else if (kind == kItemFull) {
       if (al)
         full_send_x<T, KB, GPL, true, true>(x, it, p.prescale, rng, ds, dst);

@@ -428,8 +428,8 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::sharded_compressed(ShardedOp op,
               " has ", full.numel(), " elements, expected world size (", getSize(), ") x ", rs ? "output" : "input",
               " (", shard.numel(), ")");
   TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: ", name, "_compressed: bits must be 1..8 or 32");
-  TORCH_CHECK(codec == kMaxMin || (bits == 8 && !stochastic), "cgx: ", name,
-              "_compressed: the FP8 formats use bits 8 and round to nearest");
+  TORCH_CHECK(codec == kMaxMin || (bits == 8 && (!stochastic || fp8_sr(codec))), "cgx: ", name,
+              "_compressed: the FP8 formats use bits 8 and round to nearest (stochastically: the _sr formats)");
   RngParams rng;
   rng.stochastic = stochastic;
   rng.seed = seed >= 0 ? (uint64_t)seed : CompressionEnv::read().seed;
@@ -546,8 +546,8 @@ c10::intrusive_ptr<c10d::Work> ProcessGroupCGX::all_to_all_compressed(at::Tensor
               " and the output rows ", out.sizes().slice(1), " differ");
   TORCH_CHECK(bits >= 1 && (bits <= 8 || bits == kRawBits), "cgx: all_to_all: bits must be 1..8 or 32");
   TORCH_CHECK(bucket_size >= 1, "cgx: all_to_all: bucket_size must be >= 1");
-  TORCH_CHECK(codec == kMaxMin || (bits == 8 && !stochastic),
-              "cgx: all_to_all: the FP8 codecs use bits 8 and round to nearest");
+  TORCH_CHECK(codec == kMaxMin || (bits == 8 && (!stochastic || fp8_sr(codec))),
+              "cgx: all_to_all: the FP8 codecs use bits 8 and round to nearest (stochastically: the _sr codecs)");
   const int W = getSize();
   // one node: the fused kernel's peers; several nodes: the cross-node stage's stream keys (a2a_rng_stream)
   const int max_world = local_size() >= W ? kMaxPeers : kA2aMaxWorld;

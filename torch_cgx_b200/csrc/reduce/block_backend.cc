@@ -13,9 +13,9 @@ namespace cgx {
 namespace {
 
 // what the FP8 codecs of the block primitives support: compressed blocks of 8-bit plans, rounded to
-// nearest (the reducers pass raw blocks with kMaxMin)
-void check_fp8(const Plan& p, uint32_t first, uint32_t count, const RngKey& rng) {
-  bool ok = p.uniform_bits == 8 && !rng.enabled;
+// nearest unless the codec rounds stochastically (the reducers pass raw blocks with kMaxMin)
+void check_fp8(const Plan& p, uint32_t first, uint32_t count, const RngKey& rng, WireCodec codec) {
+  bool ok = p.uniform_bits == 8 && (!rng.enabled || fp8_sr(codec));
   for (uint32_t b = first; ok && b < first + count; ++b) ok = block_bits(p.blocks[b]) < kRawBits;
   if (!ok)
     throw std::invalid_argument("cgx: an FP8 codec needs compressed blocks of an 8-bit plan and round to nearest");
@@ -33,13 +33,13 @@ class CpuBackend : public BlockBackend {
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
                 const RngKey& rng, cudaStream_t, WireCodec codec) override {
     const Plan& p = dp.plan;
-    if (codec != kMaxMin) check_fp8(p, first, count, rng);
+    if (codec != kMaxMin) check_fp8(p, first, count, rng, codec);
     std::vector<float> acc(kMaxBlockElems);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
       cpu::load_block(src, p.dtype, d, prescale, acc.data());
       if (codec != kMaxMin)
-        cpu::quantize_block_fp8(acc.data(), d, wire + d.wire_off, codec);
+        cpu::quantize_block_fp8(acc.data(), d, wire + d.wire_off, codec, rng);
       else
         cpu::quantize_block(acc.data(), p.dtype, d, wire + d.wire_off, rng, b);
     }
@@ -48,7 +48,7 @@ class CpuBackend : public BlockBackend {
                   uint32_t base_elem, const void* init_src, float prescale, cudaStream_t,
                   WireCodec codec) override {
     const Plan& p = dp.plan;
-    if (codec != kMaxMin) check_fp8(p, first, count, RngKey{});
+    if (codec != kMaxMin) check_fp8(p, first, count, RngKey{}, codec);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
       float* a = acc_f32 + (d.elem_off - base_elem);
@@ -62,11 +62,11 @@ class CpuBackend : public BlockBackend {
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
                     uint8_t* wire, const RngKey& rng, void* out, cudaStream_t, WireCodec codec) override {
     const Plan& p = dp.plan;
-    if (codec != kMaxMin) check_fp8(p, first, count, rng);
+    if (codec != kMaxMin) check_fp8(p, first, count, rng, codec);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = p.blocks[b];
       if (codec != kMaxMin) {
-        cpu::quantize_block_fp8(acc_f32 + (d.elem_off - base_elem), d, wire + d.wire_off, codec);
+        cpu::quantize_block_fp8(acc_f32 + (d.elem_off - base_elem), d, wire + d.wire_off, codec, rng);
         if (out) cpu::decode_block_fp8_store(wire + d.wire_off, p.dtype, d, out, codec);
         continue;
       }
@@ -76,7 +76,7 @@ class CpuBackend : public BlockBackend {
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                   cudaStream_t, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{}, codec);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = dp.plan.blocks[b];
       if (codec != kMaxMin)
@@ -87,7 +87,7 @@ class CpuBackend : public BlockBackend {
   }
   void unpack_fp8(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, uint8_t* codes,
                   float* scales, cudaStream_t) override {
-    check_fp8(dp.plan, first, count, RngKey{});
+    check_fp8(dp.plan, first, count, RngKey{}, kE4M3);
     for (uint32_t b = first; b < first + count; ++b) {
       const BlockDesc& d = dp.plan.blocks[b];
       cpu::unpack_block_fp8(wire + d.wire_off, d, codes, scales);
@@ -112,32 +112,32 @@ class CudaBackend : public BlockBackend {
   void release(void* p) override { cudaFree(p); }
   void quantize(const DevicePlan& dp, const void* src, uint32_t first, uint32_t count, uint8_t* wire, float prescale,
                 const RngKey& rng, cudaStream_t stream, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng);
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng, codec);
     cuda_check(launch_quantize_items(args(dp, first, count, codec), src, wire, prescale, rng, stream),
                "quantize_items");
   }
   void accumulate(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, float* acc_f32,
                   uint32_t base_elem, const void* init_src, float prescale, cudaStream_t stream,
                   WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{}, codec);
     cuda_check(launch_accumulate_items_f32(args(dp, first, count, codec), wire, acc_f32, base_elem, init_src, prescale,
                                            stream),
                "accumulate_items");
   }
   void quantize_f32(const DevicePlan& dp, const float* acc_f32, uint32_t base_elem, uint32_t first, uint32_t count,
                     uint8_t* wire, const RngKey& rng, void* out, cudaStream_t stream, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng);
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, rng, codec);
     cuda_check(launch_quantize_items_f32(args(dp, first, count, codec), acc_f32, base_elem, wire, rng, out, stream),
                "quantize_items_f32");
   }
   void dequantize(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, void* dst,
                   cudaStream_t stream, WireCodec codec) override {
-    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{});
+    if (codec != kMaxMin) check_fp8(dp.plan, first, count, RngKey{}, codec);
     cuda_check(launch_dequantize_items(args(dp, first, count, codec), wire, dst, stream), "dequantize_items");
   }
   void unpack_fp8(const DevicePlan& dp, const uint8_t* wire, uint32_t first, uint32_t count, uint8_t* codes,
                   float* scales, cudaStream_t stream) override {
-    check_fp8(dp.plan, first, count, RngKey{});
+    check_fp8(dp.plan, first, count, RngKey{}, kE4M3);
     if (count == 0) return;
     cuda_check(launch_unpack_items_fp8(args(dp, first, count), wire, codes, scales, dp.plan.blocks[first].bucket, stream),
                "unpack_items_fp8");

@@ -70,11 +70,12 @@ const DevicePlan* FusedSra::prepare_impl(const std::vector<LayerSpec>& layers, i
 
 namespace {
 
-// an FP8 allreduce: a known codec, compressed blocks of 8 bits only, round to nearest
+// an FP8 allreduce: a known codec, compressed blocks of 8 bits only, round to nearest unless the codec
+// rounds stochastically
 void check_allreduce_codec(const Plan& plan, WireCodec codec, const RngParams& rng) {
   if (codec == kMaxMin) return;
   if (!is_fp8_codec(codec)) throw std::invalid_argument("cgx allreduce: unknown wire codec");
-  if (rng.stochastic) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
+  if (rng.stochastic && !fp8_sr(codec)) throw std::invalid_argument("cgx allreduce: the FP8 formats round to nearest only");
   for (const BlockDesc& d : plan.blocks)
     if (block_bits(d) != 8 && block_bits(d) < kRawBits)
       throw std::invalid_argument("cgx allreduce: an FP8 format needs layers of bits 8 or 32, got " +
@@ -227,7 +228,7 @@ FusedSra::RsCounts FusedSra::sharded(ShardedOp op, const std::vector<LayerSpec>&
   RsCounts n;
   check_sharded_buffers(op, shard_layers, dtype, in, out, S, rank(), world(), codec, out_scales);
   const uint32_t out_bucket = out_scales != nullptr ? codes_bucket(op, shard_layers, codec) : 0;
-  if (codec != kMaxMin && rng.stochastic)
+  if (codec != kMaxMin && !fp8_sr(codec) && rng.stochastic)
     throw std::invalid_argument(std::string("cgx ") + name + ": the FP8 formats round to nearest only");
   if (S == 0) return n;
   // plans are launched as soon as they are prepared: a plan-cache trim frees the plans before it
@@ -422,7 +423,7 @@ FusedSra::A2aCounts FusedSra::all_to_all(const void* in, void* out, const std::v
   if (!heap_->connected()) throw std::runtime_error("cgx: symmetric heap is not connected");
   const int W = world(), r = rank();
   check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, route, out_scales);
-  if (codec != kMaxMin && rng.stochastic)
+  if (codec != kMaxMin && !fp8_sr(codec) && rng.stochastic)
     throw std::invalid_argument("cgx all_to_all: the FP8 codecs round to nearest only");
   const uint64_t es = (uint64_t)dtype_size(dtype);
   const bool routed = route != nullptr && (route->in_index != nullptr || route->out_index != nullptr);

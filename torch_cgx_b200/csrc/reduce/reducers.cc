@@ -222,7 +222,8 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
   const int W = comm_->size(), r = comm_->rank();
   check_all_to_all(in, out, in_counts, out_counts, dtype, bits, codec, bucket, r, W, nullptr, out_scales);
   if (out_scales != nullptr) {
-    all_to_all_codes(in, static_cast<uint8_t*>(out), out_scales, in_counts, out_counts, dtype, codec, bucket, stream);
+    all_to_all_codes(in, static_cast<uint8_t*>(out), out_scales, in_counts, out_counts, dtype, codec, bucket, rng, stream,
+                     rank_base);
     return;
   }
   const size_t es = (size_t)dtype_size(dtype);
@@ -278,7 +279,7 @@ void Reducer::all_to_all(const void* in, void* out, const std::vector<uint64_t>&
 
 void Reducer::all_to_all_codes(const void* in, uint8_t* codes, float* scales, const std::vector<uint64_t>& in_counts,
                                const std::vector<uint64_t>& out_counts, int dtype, WireCodec codec, uint32_t bucket,
-                               cudaStream_t stream) {
+                               const RngParams& rng, cudaStream_t stream, int rank_base) {
   const int W = comm_->size(), r = comm_->rank();
   const size_t es = (size_t)dtype_size(dtype);
   const uint8_t* src = static_cast<const uint8_t*>(in);
@@ -299,8 +300,10 @@ void Reducer::all_to_all_codes(const void* in, uint8_t* codes, float* scales, co
   uint8_t* recvb = scratch(1, ro[W] + 16);
   for (int q = 0; q < W; ++q) {
     if (!sw[q]) continue;
+    RngKey key = make_rng_key(rng, r, 0);
+    key.stream = a2a_rng_stream(rank_base + r, rank_base + q);
     const DevicePlan& dp = plan_for({LayerSpec{0, in_counts[q], 8, bucket}}, dtype, false, stream, 1);
-    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, RngKey{}, stream, codec);
+    ops_->quantize(dp, src + io[q], 0, (uint32_t)dp.plan.blocks.size(), sendb + so[q], 1.0f, key, stream, codec);
     if (q == r) ops_->unpack_fp8(dp, sendb + so[q], 0, (uint32_t)dp.plan.blocks.size(), codes + oo[r], scales + oo[r] / bucket, stream);
   }
   std::vector<P2POp> x;

@@ -96,7 +96,7 @@ class Reducer {
   uint8_t* scratch(int slot, size_t bytes);  // grow-only scratch buffers of the backend's memory kind
   void all_to_all_codes(const void* in, uint8_t* codes, float* scales, const std::vector<uint64_t>& in_counts,
                         const std::vector<uint64_t>& out_counts, int dtype, WireCodec codec, uint32_t bucket,
-                        cudaStream_t stream);
+                        const RngParams& rng, cudaStream_t stream, int rank_base);
   static size_t row_bytes(const Plan& p) { return ((size_t)p.max_chunk_wire + 255) / 256 * 256; }
   // [first element, one past last element) spanned by the blocks of a chunk / of the whole plan
   static void chunk_span(const Plan& p, int chunk, uint32_t* lo, uint32_t* hi);

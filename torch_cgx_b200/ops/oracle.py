@@ -216,27 +216,36 @@ def _scaled_inputs(inputs: Sequence[torch.Tensor], ps: _F32) -> List[np.ndarray]
         return [t.detach().reshape(-1).float().cpu().numpy() * ps for t in inputs]
 
 
-def _contribution(v: np.ndarray, bits: int, bucket: int, dtype: torch.dtype, fmt: str | None = None) -> np.ndarray:
+def _contribution(v: np.ndarray, bits: int, bucket: int, dtype: torch.dtype, fmt: str | None = None,
+                  sr_key: Tuple[int, int, int, int] | None = None) -> np.ndarray:
     """What a receiver decodes of one sent contribution: one quantization round (in the FP8 format
-    ``fmt`` when given), or the value rounded to the dtype for raw runs."""
+    ``fmt`` when given), or the value rounded to the dtype for raw runs. An ``_sr`` format needs
+    ``sr_key = (seed, seq, stream, first_elem)``: the key and the element index of ``v[0]``."""
     if bits >= RAW_BITS:
         return round_to_dtype(v, dtype)
+    if fmt in FP8_SR_FORMATS:
+        if sr_key is None:
+            raise ValueError(f"the FP8 format {fmt!r} rounds stochastically: this reference has no random stream")
+        return _fp8_sr_qdq_buckets(v, fmt, bucket, _sr_words(*sr_key, v.size, bucket))
     if fmt is not None:
         return _fp8_qdq_buckets(v, fmt, bucket)
     return _qdq_buckets(v, bits, bucket)[0]
 
 
 def quantize_dequantize_layers(x: torch.Tensor, layers: Sequence[Layer], *, skip_incomplete: bool = False,
-                               prescale: float = 1.0, fmt: str | None = None) -> torch.Tensor:
+                               prescale: float = 1.0, fmt: str | None = None,
+                               sr_stream: Tuple[int, int, int, int] | None = None) -> torch.Tensor:
     """One quantize -> dequantize round trip of ``prescale * x`` through a layer table, in
     ``x.dtype`` (raw runs: the value rounded to the dtype). Elements outside every layer are 0,
     as in a freshly dequantized tensor. ``fmt`` (a name of ``FP8_FORMATS``): the compressed layers (bits 8)
-    take the FP8 round trip of ``fp8_quantize_dequantize`` instead of max-min's."""
+    take the FP8 round trip of ``fp8_quantize_dequantize`` instead of max-min's. An ``_sr`` format
+    needs ``sr_stream = (seed, seq, stream, base)``: element i of ``x`` has element index base + i."""
     _check_fp8_table(layers, fmt)
     v = _scaled_inputs([x], _F32(prescale))[0]
     out = np.zeros(v.size, _F32)
     for off, m, bits, bucket in layer_segments(layers, skip_incomplete):
-        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, x.dtype, fmt)
+        key = None if sr_stream is None else (*sr_stream[:3], sr_stream[3] + off)
+        out[off:off + m] = _contribution(v[off:off + m], bits, bucket, x.dtype, fmt, key)
     return _to_tensors([out], x.dtype)[0].view_as(x)
 
 
@@ -258,7 +267,7 @@ def _sra_acc(xs: Sequence[np.ndarray], sl: slice, own: np.ndarray, bits: int, bu
 def _check_fp8_table(layers: Sequence[Layer], fmt: str | None) -> None:
     if fmt is None:
         return
-    if fmt not in FP8_FORMATS:
+    if fmt not in FP8_FORMATS and fmt not in FP8_SR_FORMATS:
         raise ValueError(f"unknown FP8 format {fmt!r}")
     for l in layers:
         if int(l[2]) != 8 and int(l[2]) < RAW_BITS:
@@ -298,11 +307,12 @@ def sra_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, wo
 
 def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *, average: bool = False,
                       skip_incomplete: bool = False, prescale: float | None = None,
-                      fmt: str | None = None) -> List[torch.Tensor]:
+                      fmt: str | None = None, seed: int = 0, seq: int = 0) -> List[torch.Tensor]:
     """Every rank's result of the one-shot allreduce: each contribution, the own one included,
     is quantized once (raw runs: rounded to the dtype) and the decoded values are summed in
     fp32 in rank order starting from +0; no second quantization, one rounding to the dtype.
-    ``fmt``: the contributions take the FP8 round trip instead (as in ``sra_reference``)."""
+    ``fmt``: the contributions take the FP8 round trip instead (as in ``sra_reference``); an ``_sr``
+    format rounds rank q's with stream q * 2 of (``seed``, ``seq``), elements indexed from the buffer start."""
     _check_fp8_table(layers, fmt)
     W = len(inputs)
     dtype = inputs[0].dtype
@@ -313,7 +323,7 @@ def oneshot_reference(inputs: Sequence[torch.Tensor], layers: Sequence[Layer], *
         acc = np.zeros(m, _F32)
         with np.errstate(all="ignore"):
             for q in range(W):
-                acc = acc + _contribution(xs[q][sl], bits, bucket, dtype, fmt)
+                acc = acc + _contribution(xs[q][sl], bits, bucket, dtype, fmt, (seed, seq, 2 * q, off))
         res = round_to_dtype(acc, dtype)
         for o in outs:
             o[sl] = res
@@ -655,13 +665,16 @@ def reduce_scatter_reference(inputs: Sequence[torch.Tensor], shard_layers: Seque
 
 
 def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[Layer],
-                         fmt: str | None = None) -> torch.Tensor:
+                         fmt: str | None = None, seed: int = 0, seq: int = 0) -> torch.Tensor:
     """Every rank's output of the compressed all-gather (deterministic rounding): the concatenation
     over q of ``quantize_dequantize_layers(inputs[q], shard_layers, fmt=fmt)``. ``shard_layers`` is
     one shard's table (offsets from the shard start), so buckets are counted from each shard's
-    start; the owner's shard is quantized like every other. Raw runs are the value in the dtype."""
-    return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers, fmt=fmt)
-                      for t in inputs])
+    start; the owner's shard is quantized like every other. Raw runs are the value in the dtype. An
+    ``_sr`` format rounds shard q with stream q * 2 + 1 of (``seed``, ``seq``), its element i having
+    index q * S + i (S the shard's size), as the all-gather publishes it."""
+    return torch.cat([quantize_dequantize_layers(t.detach().reshape(-1).cpu(), shard_layers, fmt=fmt,
+                                                 sr_stream=(seed, seq, 2 * q + 1, q * t.numel()))
+                      for q, t in enumerate(inputs)])
 
 
 # ---- FP8 wire formats of the all-to-all (common/quant_math.h, DESIGN §2.13b) ------------------------
@@ -669,6 +682,9 @@ def all_gather_reference(inputs: Sequence[torch.Tensor], shard_layers: Sequence[
 # with a power-of-two unit per bucket (DESIGN §2.13g).
 FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0),
                "e4m3_pow2": (torch.float8_e4m3fn, 448.0), "e5m2_pow2": (torch.float8_e5m2, 57344.0)}
+# The "_sr" formats: the records, units and decoder of their base format, rounded stochastically
+# (DESIGN §2.13h) with 16 random bits per element.
+FP8_SR_FORMATS = {"e4m3_sr": "e4m3", "e5m2_sr": "e5m2"}
 _FP8_MIN_UNIT = _F32(2.0 ** -126)
 
 
@@ -688,6 +704,20 @@ def _fp8_pow2_units(a: np.ndarray, fmax: float) -> Tuple[np.ndarray, np.ndarray]
     return unit, inv
 
 
+def _fp8_units(b: np.ndarray, fmt: str) -> Tuple[np.ndarray, np.ndarray]:
+    """unit and inverse of every row of ``b`` (buckets, fp32) in the FP8 format ``fmt``"""
+    fmax = FP8_FORMATS[fmt][1]
+    with np.errstate(all="ignore"):
+        mn, mx = _nan_minmax(b)
+        a = np.maximum(-mn, mx)  # NaN propagates
+        a = np.where(a == 0, _F32(0.0), a)  # +0, as max.NaN gives for a zero bucket
+        if fmt.endswith("_pow2"):
+            return _fp8_pow2_units(a, fmax)
+        unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
+        inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
+    return unit, inv
+
+
 def _fp8_code_buckets(v: np.ndarray, fmt: str, bucket: int) -> Tuple[torch.Tensor, np.ndarray]:
     """FP8 codes of a flat fp32 array whose buckets start at index 0, in numpy fp32 arithmetic and
     torch's float8 casts: unit = max|x| * fp32(1/FMAX), inv = 1/unit (0 below 2^-126), or for the
@@ -700,15 +730,8 @@ def _fp8_code_buckets(v: np.ndarray, fmt: str, bucket: int) -> Tuple[torch.Tenso
     pad = nb * bucket - n
     vp = np.concatenate([v, np.repeat(v[-1:], pad)]) if pad else v
     b = vp.reshape(nb, bucket)
+    unit, inv = _fp8_units(b, fmt)
     with np.errstate(all="ignore"):
-        mn, mx = _nan_minmax(b)
-        a = np.maximum(-mn, mx)  # NaN propagates
-        a = np.where(a == 0, _F32(0.0), a)  # +0, as max.NaN gives for a zero bucket
-        if fmt.endswith("_pow2"):
-            unit, inv = _fp8_pow2_units(a, fmax)
-        else:
-            unit = (a * (_F32(1.0) / _F32(fmax))).astype(_F32)
-            inv = np.where(unit < _FP8_MIN_UNIT, _F32(0.0), _F32(1.0) / unit).astype(_F32)
         t = np.clip((b * inv).astype(_F32), _F32(-fmax), _F32(fmax))
     return torch.from_numpy(np.ascontiguousarray(t)).to(tdt), unit.reshape(-1).astype(_F32)
 
@@ -750,15 +773,113 @@ def fp8_quantize_dequantize(x: torch.Tensor, fmt: str, bucket_size: int) -> torc
     return _to_tensors([dec], x.dtype)[0].view_as(x)
 
 
+def _sr_words(seed: int, seq: int, stream: int, first: int, n: int, bucket: int) -> np.ndarray:
+    """The 16 random bits of n elements from element index ``first`` on, whose buckets of ``bucket``
+    start at ``first``: every bucket's pack groups start at its first element (``_C.philox_u16``)."""
+    from .. import _C
+
+    parts = [_C.philox_u16(int(seed), int(seq), int(stream), int(first) + b, min(bucket, n - b)).numpy()
+             for b in range(0, n, bucket)]
+    return np.concatenate(parts).astype(np.int64) if parts else np.zeros(0, np.int64)
+
+
+def _fp8_sr_round(y: np.ndarray, base: str, h: np.ndarray) -> np.ndarray:
+    """The SR rule on y = fp32(x * inv) (DESIGN §2.13h), in float64 and frexp: with s = 2^(max(floor(log2
+    |y|), emin) - mb) the grid spacing at |y|, t = |y| / s = n + f, |y| becomes (n + 1) * s when h +
+    floor(2^16 f) >= 2^16 and n * s otherwise, saturated to FMAX; y's sign is kept, NaN stays NaN and
+    Inf saturates."""
+    emin, mb = (-6, 3) if base == "e4m3" else (-14, 2)
+    fmax = FP8_FORMATS[base][1]
+    ay = np.abs(y.astype(np.float64))
+    finite = np.isfinite(ay)
+    m, e = np.frexp(np.where(finite, ay, 1.0))
+    se = np.maximum(e.astype(np.int64) - 1, emin) - mb
+    t = np.ldexp(np.where(finite, ay, 0.0), -se)  # exact: a power-of-two scaling of a 24-bit value
+    n = np.floor(t)
+    up = (h + np.floor((t - n) * 65536.0)) >= 65536.0
+    mag = np.where(finite, np.minimum(np.ldexp(n + up, se), fmax), fmax)
+    return np.where(np.isnan(y), np.nan, np.copysign(mag, y)).astype(_F32)
+
+
+def _fp8_sr_code_buckets(v: np.ndarray, fmt: str, bucket: int, words: np.ndarray) -> Tuple[torch.Tensor, np.ndarray]:
+    """``_fp8_code_buckets`` of an ``_sr`` format: the units of its base format, and the codes of the SR
+    rule with element i's random bits ``words[i]``."""
+    base = FP8_SR_FORMATS[fmt]
+    n = v.size
+    nb = -(-n // bucket)
+    pad = nb * bucket - n
+    vp = np.concatenate([v, np.repeat(v[-1:], pad)]) if pad else v
+    hp = np.concatenate([words, np.zeros(pad, np.int64)]) if pad else words
+    b = vp.reshape(nb, bucket)
+    unit, inv = _fp8_units(b, base)
+    with np.errstate(all="ignore"):
+        y = (b * inv).astype(_F32)
+    g = _fp8_sr_round(y, base, hp.reshape(nb, bucket))
+    return torch.from_numpy(np.ascontiguousarray(g)).to(FP8_FORMATS[base][0]), unit.reshape(-1).astype(_F32)
+
+
+def _fp8_sr_qdq_buckets(v: np.ndarray, fmt: str, bucket: int, words: np.ndarray) -> np.ndarray:
+    n = v.size
+    if n == 0:
+        return np.zeros(0, _F32)
+    code, unit = _fp8_sr_code_buckets(v, fmt, bucket, words)
+    with np.errstate(all="ignore"):
+        dec = (code.float().numpy() * unit[:, None]).astype(_F32)
+    return dec.reshape(-1)[:n]
+
+
+def _sr_input(x: torch.Tensor, fmt: str, words) -> Tuple[np.ndarray, np.ndarray]:
+    if fmt not in FP8_SR_FORMATS:
+        raise ValueError(f"unknown stochastic FP8 format {fmt!r}")
+    v = x.detach().reshape(-1).float().cpu().numpy()
+    h = np.asarray(words.numpy() if isinstance(words, torch.Tensor) else words, dtype=np.int64).reshape(-1)
+    if h.size != v.size:
+        raise ValueError(f"need one random word per element: {h.size} words for {v.size} elements")
+    return v, h & 0xFFFF
+
+
+def fp8_sr_quantize(x: torch.Tensor, fmt: str, bucket: int, words) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Codes and units of ``x`` (flat, buckets of ``bucket`` from its first element) in the stochastic
+    FP8 format ``fmt`` ("e4m3_sr" / "e5m2_sr"), element i rounded with the 16-bit word ``words[i]``:
+    ``(codes, units)`` as ``fp8_quantize`` gives them. Computed from the rule of DESIGN §2.13h, not
+    by the encoder; the words of a collective come from ``_C.philox_u16``."""
+    v, h = _sr_input(x, fmt, words)
+    if v.size == 0:
+        return torch.empty(0, dtype=FP8_FORMATS[FP8_SR_FORMATS[fmt]][0]), torch.empty(0, dtype=torch.float32)
+    code, unit = _fp8_sr_code_buckets(v, fmt, effective_bucket(bucket), h)
+    return code.reshape(-1)[:v.size].clone(), torch.from_numpy(unit)
+
+
+def fp8_sr_quantize_dequantize(x: torch.Tensor, fmt: str, bucket: int, words) -> torch.Tensor:
+    """The round trip of ``fp8_sr_quantize``: float(code) * unit, rounded to ``x.dtype``."""
+    v, h = _sr_input(x, fmt, words)
+    dec = _fp8_sr_qdq_buckets(v, fmt, effective_bucket(bucket), h)
+    return _to_tensors([dec], x.dtype)[0].view_as(x)
+
+
+def _a2a_chunk_fp8(chunk: torch.Tensor, fmt: str, bucket_size: int, seed: int, seq: int, q: int, r: int,
+                   codes: bool):
+    """The FP8 record of the chunk rank q sends rank r: decoded, or (codes, units) with ``codes``"""
+    if fmt in FP8_SR_FORMATS:
+        from .. import _C
+
+        n = chunk.numel()
+        w = _sr_words(seed, seq, _C.a2a_rng_stream(q, r), 0, n, effective_bucket(bucket_size))
+        return fp8_sr_quantize(chunk, fmt, bucket_size, w) if codes else fp8_sr_quantize_dequantize(
+            chunk, fmt, bucket_size, w)
+    return fp8_quantize(chunk, fmt, bucket_size) if codes else fp8_quantize_dequantize(chunk, fmt, bucket_size)
+
+
 def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, bits: int | str,
-                         bucket_size: int) -> List[torch.Tensor]:
+                         bucket_size: int, seed: int = 0, seq: int = 0) -> List[torch.Tensor]:
     """Every rank's output of the compressed all-to-all (round to nearest). ``counts[q][r]`` elements
     go from rank q to rank r; rank q's input holds its chunks in destination order and rank r's
     output the chunks it receives in source order. The own chunk, and every chunk when ``bits`` is
     32, is the input unchanged; every other chunk is ``quantize_dequantize_layers`` of one layer, so
     buckets are counted from the chunk's first element. ``bits`` an FP8 format: every other chunk
-    is ``fp8_quantize_dequantize`` instead."""
-    if isinstance(bits, str) and bits not in FP8_FORMATS:
+    is ``fp8_quantize_dequantize`` instead; an ``_sr`` format rounds the chunk from q to r with the
+    stream ``a2a_rng_stream(q, r)`` of (``seed``, ``seq``), elements indexed from the chunk's start."""
+    if isinstance(bits, str) and bits not in FP8_FORMATS and bits not in FP8_SR_FORMATS:
         raise ValueError(f"unknown FP8 format {bits!r}")
     fp8 = isinstance(bits, str)
     W = len(inputs)
@@ -771,7 +892,7 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
             n = int(counts[q][r])
             chunk = flat[q][a:a + n].clone()
             if q != r and n > 0 and fp8:
-                chunk = fp8_quantize_dequantize(chunk, bits, bucket_size)
+                chunk = _a2a_chunk_fp8(chunk, bits, bucket_size, seed, seq, q, r, False)
             elif q != r and n > 0 and bits < RAW_BITS:
                 chunk = quantize_dequantize_layers(chunk, [(0, n, int(bits), int(bucket_size))])
             parts.append(chunk)
@@ -780,11 +901,13 @@ def all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequen
 
 
 def all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]], *, fmt: str,
-                               bucket_size: int) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+                               bucket_size: int, seed: int = 0,
+                               seq: int = 0) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
     """Every rank's codes output of the FP8 all-to-all (``output_scales``): rank r's codes are, in
     source order, ``fp8_quantize`` of every chunk it receives, its own chunk included, and its scales
     the units of those chunks' buckets, concatenated (flat; every count a multiple of
-    ``bucket_size``, so the scales of a row-major ``[rows, H / bucket_size]`` matrix)."""
+    ``bucket_size``, so the scales of a row-major ``[rows, H / bucket_size]`` matrix). An ``_sr``
+    format rounds as in ``all_to_all_reference``, the own chunk with the stream ``a2a_rng_stream(r, r)``."""
     W = len(inputs)
     flat = [t.detach().reshape(-1).cpu() for t in inputs]
     codes, scales = [], []
@@ -792,7 +915,7 @@ def all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[
         cs, us = [], []
         for q in range(W):
             a = sum(int(c) for c in counts[q][:r])
-            c, u = fp8_quantize(flat[q][a:a + int(counts[q][r])], fmt, bucket_size)
+            c, u = _a2a_chunk_fp8(flat[q][a:a + int(counts[q][r])], fmt, bucket_size, seed, seq, q, r, True)
             cs.append(c)
             us.append(u)
         codes.append(torch.cat(cs))
@@ -800,12 +923,19 @@ def all_to_all_codes_reference(inputs: Sequence[torch.Tensor], counts: Sequence[
     return codes, scales
 
 
-def all_gather_codes_reference(inputs: Sequence[torch.Tensor], fmt: str,
-                               bucket_size: int) -> Tuple[torch.Tensor, torch.Tensor]:
+def all_gather_codes_reference(inputs: Sequence[torch.Tensor], fmt: str, bucket_size: int, seed: int = 0,
+                               seq: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
     """The codes output of the FP8 all-gather (``output_scales``), the same on every rank: codes
     ``fp8_quantize`` of every rank's shard concatenated in rank order (float8, flat), and the units
-    of their buckets likewise (fp32, flat; every shard a multiple of ``bucket_size``)."""
-    parts = [fp8_quantize(t.detach().reshape(-1).cpu(), fmt, bucket_size) for t in inputs]
+    of their buckets likewise (fp32, flat; every shard a multiple of ``bucket_size``). An ``_sr``
+    format rounds shard q as ``all_gather_reference`` does."""
+    if fmt in FP8_SR_FORMATS:
+        B = effective_bucket(bucket_size)
+        parts = [fp8_sr_quantize(t.detach().reshape(-1).cpu(), fmt, bucket_size,
+                                 _sr_words(seed, seq, 2 * q + 1, q * t.numel(), t.numel(), B))
+                 for q, t in enumerate(inputs)]
+    else:
+        parts = [fp8_quantize(t.detach().reshape(-1).cpu(), fmt, bucket_size) for t in inputs]
     return torch.cat([c for c, _ in parts]), torch.cat([u for _, u in parts])
 
 

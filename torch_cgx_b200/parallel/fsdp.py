@@ -10,7 +10,8 @@ FSDP2 takes a custom reduce-scatter and all-gather per module (``FSDPModule.set_
 
 ``bits`` may also be an FP8 wire format: ``"e4m3"`` for the parameter all-gather and ``"e5m2"`` for
 the gradient reduce-scatter are the usual choice, and ``"e4m3_pow2"`` / ``"e5m2_pow2"`` give the
-same codes with power-of-two scales.
+same codes with power-of-two scales. The reduce-scatter also takes ``"e5m2_sr"`` / ``"e4m3_sr"``,
+rounded stochastically; the all-gather does not.
 
 Both work over any number of nodes: across nodes they run in two stages, the semantics of
 ``reduce_scatter_tensor`` and ``all_gather_into_tensor`` (functional.py).
@@ -44,6 +45,14 @@ def _bits(bits: A2aBits, adaptive) -> A2aBits:
     return int(bits)
 
 
+def _check_gather_bits(bits: A2aBits) -> None:
+    """ValueError for a stochastic FP8 format: the FSDP2 all-gather rounds to nearest, so that the
+    backward re-gather sees the weights the forward saw"""
+    if isinstance(bits, str) and bits.endswith("_sr"):
+        raise ValueError(f"cgx: the FSDP2 all-gather rounds to nearest, so that the backward re-gather sees "
+                         f"the forward's weights; bits={bits!r} rounds stochastically")
+
+
 def _table_bits(bits: A2aBits) -> int:
     """the width of a table entry for ``bits``: an FP8 format travels in 8-bit records"""
     return 8 if isinstance(bits, str) else int(bits)
@@ -56,7 +65,8 @@ class CGXReduceScatter(ReduceScatter):
     shard's table as ``(elem_off, numel, bits, bucket_size)`` tuples (None = one layer of ``bits`` /
     ``bucket_size`` per shard). ``adaptive`` is an :class:`~torch_cgx_b200.AdaptiveFSDPState` that
     rewrites ``layers``; ``set_cgx_adaptive`` sets it. ``bits`` may be an FP8 format, ``"e5m2"`` or
-    ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``stochastic``, no ``adaptive``)."""
+    ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``stochastic``, no ``adaptive``), or ``"e5m2_sr"``
+    / ``"e4m3_sr"``, which round stochastically whatever ``stochastic`` says."""
 
     def __init__(self, bits: A2aBits = 4, bucket_size: int = 512, stochastic: bool = False,
                  layers: Optional[Sequence[Layer]] = None, name: str = "", adaptive=None):
@@ -126,10 +136,12 @@ class CGXAllGather(AllGather):
     see the weights the forward saw. A ``uint8`` buffer (FSDP2's all-gather of mixed-dtype inputs)
     goes to ``dist.all_gather_into_tensor`` unchanged. ``adaptive`` is an
     :class:`~torch_cgx_b200.AdaptiveFSDPState` that rewrites ``layers``; ``set_cgx_adaptive`` sets it.
-    ``bits`` may be an FP8 format, usually ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``adaptive``)."""
+    ``bits`` may be an FP8 format, usually ``"e4m3"`` (``layers`` then of bits 8 or 32, no ``adaptive``),
+    but not a stochastic one (``"e4m3_sr"`` / ``"e5m2_sr"``: ValueError), for the same reason."""
 
     def __init__(self, bits: A2aBits = 4, bucket_size: int = 512, layers: Optional[Sequence[Layer]] = None,
                  name: str = "", adaptive=None):
+        _check_gather_bits(bits)
         self.bits = _bits(bits, adaptive)
         self.bucket_size = int(bucket_size)
         self.layers = _table(layers)
@@ -161,6 +173,7 @@ def set_cgx_all_gather(model: torch.nn.Module, bits: A2aBits = 4,
     the comms. Call it after ``fully_shard`` and before the first forward."""
     from torch.distributed.fsdp import FSDPModule
 
+    _check_gather_bits(bits)
     comms = []
     for name, m in model.named_modules():
         if not isinstance(m, FSDPModule):

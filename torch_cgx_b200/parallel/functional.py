@@ -18,7 +18,8 @@ and so is the compressed all-gather (``dist.all_gather_into_tensor`` stays uncom
     cgx.all_gather_into_tensor(flat_params, shard, bits=8)
 
 Both also take an FP8 wire format, ``bits="e4m3"`` or ``"e5m2"`` (or ``"e4m3_pow2"`` / ``"e5m2_pow2"``,
-with power-of-two scales), in place of max-min 8-bit.
+with power-of-two scales, or ``"e4m3_sr"`` / ``"e5m2_sr"``, rounded stochastically), in place of
+max-min 8-bit.
 
 and the compressed all-to-all of expert-parallel MoE layers (``dist.all_to_all_single`` stays
 uncompressed)::
@@ -53,11 +54,12 @@ def compression(bits: Optional[A2aBits] = None, bucket_size: Optional[int] = Non
                 seed: Optional[int] = None) -> Iterator[None]:
     """Temporarily override the env-level compression config (None = leave as is; bits=32 disables).
 
-    ``bits="e4m3"``, ``"e5m2"``, ``"e4m3_pow2"`` or ``"e5m2_pow2"`` compresses at 8 bits and sends
-    the allreduce's 8-bit layers as FP8 codes with one fp32 scale per bucket (``CGX_COMPRESSION_FORMAT``;
-    the ``_pow2`` formats' scales are powers of two, see ``all_to_all_single``); an integer ``bits``
-    selects max-min. FP8 rounds to nearest: an unknown name, or a name with ``stochastic=True`` or
-    ``CGX_STOCHASTIC_ROUNDING=1``, raises ValueError before anything is changed.
+    ``bits="e4m3"``, ``"e5m2"``, ``"e4m3_pow2"``, ``"e5m2_pow2"``, ``"e4m3_sr"`` or ``"e5m2_sr"``
+    compresses at 8 bits and sends the allreduce's 8-bit layers as FP8 codes with one fp32 scale per
+    bucket (``CGX_COMPRESSION_FORMAT``; the ``_pow2`` formats' scales are powers of two, the ``_sr``
+    formats round stochastically, see ``all_to_all_single``); an integer ``bits`` selects max-min.
+    The other FP8 formats round to nearest: an unknown name, or one of them with ``stochastic=True``
+    or ``CGX_STOCHASTIC_ROUNDING=1``, raises ValueError before anything is changed.
     """
     fmt = None
     if bits is not None:
@@ -121,7 +123,8 @@ def _sharded(method: str, api: str, output: torch.Tensor, input: torch.Tensor, h
     return None
 
 
-A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2" / "e4m3_pow2" / "e5m2_pow2"
+A2aBits = Union[int, str]  # 1..8, 32, or an FP8 wire format: "e4m3" / "e5m2" / "e4m3_pow2" / "e5m2_pow2" /
+# "e4m3_sr" / "e5m2_sr"
 
 
 def _sharded_bits(bits: A2aBits, stochastic: bool, layers: Optional[Sequence[Tuple[int, int, int, int]]],
@@ -170,7 +173,8 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aBi
     in rank order. ``e5m2``'s wider exponent range suits gradients. A ``layers`` table may then hold
     bits 8 (FP8) and 32 (raw) only. A NaN or an Inf in a peer's bucket makes that bucket of the sum
     NaN. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as does any other
-    string. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales (see ``all_to_all_single``).
+    string. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales, and ``"e4m3_sr"`` /
+    ``"e5m2_sr"`` round stochastically whatever ``stochastic`` says (see ``all_to_all_single``).
 
     Over several nodes (``local_size`` consecutive ranks each) the reduction has two stages: inside
     each node, for every node's block of shards, the reduce-scatter above over the local ranks
@@ -218,7 +222,8 @@ def all_gather_into_tensor(output: torch.Tensor, input: torch.Tensor, bits: A2aB
     the usual choice for weights being ``e4m3``. Every rank, the owner included, writes the values
     decoded from the same codes, so at world 1 the output is ``ops.oracle.fp8_quantize_dequantize``
     of the input. A ``layers`` table may then hold bits 8 (FP8) and 32 (raw) only; FP8 rounds to
-    nearest only. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales (see ``all_to_all_single``).
+    nearest only. ``"e4m3_pow2"`` / ``"e5m2_pow2"`` use power-of-two scales, and ``"e4m3_sr"`` /
+    ``"e5m2_sr"`` round stochastically whatever ``stochastic`` says (see ``all_to_all_single``).
 
     Over several nodes the owner's quantized bytes first go to the ranks of the same local rank on
     the other nodes, which decode them; each node then shares the decoded shards among its ranks
@@ -249,8 +254,8 @@ def _splits(s: Optional[Sequence[int]]) -> List[int]:
 
 def _a2a_bits(bits: A2aBits, stochastic: bool) -> A2aBits:
     """``bits`` as the native all-to-all takes it: an int, or an FP8 format name. An unknown name, or
-    an FP8 format with ``stochastic``, raises ValueError (the native parser's check, run here so that
-    it fires before anything is sent)."""
+    a round-to-nearest FP8 format with ``stochastic``, raises ValueError (the native parser's check,
+    run here so that it fires before anything is sent)."""
     if not isinstance(bits, str):
         return int(bits)
     from .. import _C
@@ -278,8 +283,17 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     converted by Hopper's FP8 instructions. Its relative error per element is at most 2^-4 (e4m3)
     or 2^-3 (e5m2) whatever else the bucket holds, so it suits rows with a few outlier channels;
     max-min 8-bit is more accurate on well-behaved data. A bucket holding a NaN or an Inf decodes to
-    NaN in every element. FP8 rounds to nearest only: ``stochastic=True`` raises ``ValueError``, as
-    does any other string.
+    NaN in every element. These formats round to nearest only: ``stochastic=True`` raises
+    ``ValueError``, as does any other string.
+
+    ``bits="e4m3_sr"`` or ``"e5m2_sr"`` sends the records, scales and decoder of e4m3 / e5m2, but
+    rounds every code stochastically, whatever ``stochastic`` says (both values give the same bytes):
+    ``y = x / unit`` becomes one of its two neighbours on the format's grid, the one away from zero
+    with probability equal to its distance from the other (in steps of 2^-16). The decoded value is
+    then unbiased up to 2^-16 of a grid step, and values far below the bucket's maximum survive in
+    expectation instead of flushing to zero. The random bits are those integer stochastic rounding
+    uses for the same elements: ``seed`` (``None``: ``CGX_SEED``), the call sequence and the pair of
+    ranks. They suit gradients, whose rounding errors then cancel across steps and ranks.
 
     ``bits="e4m3_pow2"`` or ``"e5m2_pow2"`` sends the same bytes with the codes of e4m3 / e5m2 and a
     power-of-two scale per bucket, ``unit = 2^k`` with k the smallest integer >= -126 such that
@@ -300,7 +314,7 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     raises, naming the index), after which the group refuses further collectives.
 
     FP8 codes for an FP8 expert GEMM: with ``output_scales`` (and an FP8 ``bits``) ``output`` is a
-    ``torch.float8_e4m3fn`` (e4m3, e4m3_pow2) / ``torch.float8_e5m2`` (e5m2, e5m2_pow2) tensor of the input's shape per
+    ``torch.float8_e4m3fn`` (e4m3, e4m3_pow2, e4m3_sr) / ``torch.float8_e5m2`` (e5m2, e5m2_pow2, e5m2_sr) tensor of the input's shape per
     row that receives the wire's codes undecoded, and ``output_scales`` (CUDA float32, contiguous,
     ``[output.shape[0], H // bucket_size]`` with ``H`` the elements of a row) the fp32 unit of every
     bucket. ``H % bucket_size == 0`` and ``bucket_size <= 8192``, so every bucket lies inside one row;
@@ -368,12 +382,12 @@ def _check_input_scale(output: torch.Tensor, input: torch.Tensor, input_index: O
 def _check_codes_format(api: str, output: torch.Tensor, bits: A2aBits) -> None:
     """ValueError unless ``bits`` is an FP8 format and ``output`` a tensor of its float8 dtype (the
     codes output of ``api``)."""
-    from ..ops.oracle import FP8_FORMATS
+    from ..ops.oracle import FP8_FORMATS, FP8_SR_FORMATS
 
     if not isinstance(bits, str):
-        raise ValueError(f"cgx.{api}: output_scales needs bits='e4m3', 'e5m2', 'e4m3_pow2' or 'e5m2_pow2', "
-                         f"got bits={bits}")
-    want = FP8_FORMATS[bits][0]
+        raise ValueError(f"cgx.{api}: output_scales needs bits='e4m3', 'e5m2', 'e4m3_pow2', 'e5m2_pow2', "
+                         f"'e4m3_sr' or 'e5m2_sr', got bits={bits}")
+    want = FP8_FORMATS[FP8_SR_FORMATS.get(bits, bits)][0]
     if output.dtype != want:
         raise ValueError(f"cgx.{api}: with bits={bits!r} and output_scales the output must be {want}, "
                          f"got {output.dtype}")

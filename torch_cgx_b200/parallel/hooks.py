@@ -32,8 +32,8 @@ VALUE_NO_COMPRESS = 32
 
 def _width_and_format(bits: Union[int, str]) -> Tuple[int, Optional[str]]:
     """``bits`` of the compressed allreduce: a max-min width, or an FP8 format name ("e4m3",
-    "e5m2", "e4m3_pow2" or "e5m2_pow2"), whose layers are compressed at 8 bits. ValueError for any
-    other name."""
+    "e5m2", "e4m3_pow2", "e5m2_pow2", "e4m3_sr" or "e5m2_sr"), whose layers are compressed at 8 bits.
+    ValueError for any other name."""
     if not isinstance(bits, str):
         return int(bits), None
     from .. import _C
@@ -46,7 +46,8 @@ class CGXState(object):
     """State of :func:`cgx_hook` (argument-compatible with the reference).
 
     ``compression_params["bits"]`` is a max-min width or an FP8 format, ``"e4m3"`` or ``"e5m2"``
-    (the usual choice for gradients), or ``"e4m3_pow2"`` / ``"e5m2_pow2"`` with power-of-two scales:
+    (the usual choice for gradients), ``"e4m3_pow2"`` / ``"e5m2_pow2"`` with power-of-two scales, or
+    ``"e4m3_sr"`` / ``"e5m2_sr"``, rounded stochastically with each rank's own random stream:
     the compressed layers are then registered at 8 bits and sent as FP8 codes with one fp32 scale
     per bucket. ``quantization_bits`` holds the width and
     ``quantization_format`` the format name (None: max-min, or ``CGX_COMPRESSION_FORMAT``'s).
