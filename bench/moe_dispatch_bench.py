@@ -44,6 +44,22 @@ gradients against the oracle. Bytes: both run the same exchange; the torch arm a
 (fp32 copies of grad_out and the slots, the fp32 product written and read); the fused arm reads
 grad_out and the slots once.
 
+With --dispatch-backward, the backward of the dispatch (the gradient of the received rows [T k, H]
+in the dtype, seeded), which returns every slot's gradient to its token's rank and sums each
+token's k rows:
+
+  backward index_add_: all_to_all(gin, grad), then zeros(T, H).index_add_(0, order // k, gin), the
+                       backward of differentiable_all_to_all_single with input_index
+  backward fused:      all_to_all(slots, grad, output_index=order, gate=ones(T, k), combine_out=out),
+                       the unit-gate combine of differentiable_all_to_all_dispatch
+
+Both arms exchange the same rows. Each row also reports whether every timed run of an arm gave the
+bits of its first run (index_add_ adds with atomics in whatever order they land), the largest
+absolute difference of each arm from the float64 sum of the same slots, and checks rank 0's first
+64 fused tokens against the oracle. Bytes: the index_add_ arm adds the zero fill of [T, H], the read
+of gin and a read-modify-write of a [T, H] row per slot (2 T k H es); the fused arm reads the slots
+back, writes [T, H] and reads the T k fp32 unit gates.
+
 Arms alternate in one run, CUDA events around each, medians over --iters after --warmup. The HBM
 bytes of an arm are computed from shapes, all ranks together: the kernel reads the sent rows and
 writes the received rows (2 N H es), writes and reads its wire image once (2 N H bits / 8, plus
@@ -303,6 +319,87 @@ def run_combine_backward(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=
     return res
 
 
+def run_dispatch_backward(W, T, H, k, bits, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
+    from torch_cgx_b200.ops import oracle as O
+
+    dev = torch.device("cuda", 0)
+    es = torch.tensor([], dtype=dtype).element_size()
+    route = routing(W, T, k, seed=T * 31 + H * 7 + k, device=dev)
+    send_rows = [route[q][2] for q in range(W)]
+    recv_n = [sum(send_rows[q][r] for q in range(W)) for r in range(W)]
+    back_counts = [[send_rows[r][q] * H for r in range(W)] for q in range(W)]  # the dispatch's, swapped
+    g = C.LocalSraGroup(W, lanes, slot_mb << 20, 20000, 256)
+    gen = torch.Generator(device=dev).manual_seed(T + H + k)
+    grad = [torch.randn(recv_n[r], H, device=dev, generator=gen).to(dtype) for r in range(W)]
+    ii = [route[q][0] for q in range(W)]
+    oi = [route[q][1] for q in range(W)]
+    unit = [torch.ones(T, k, device=dev) for _ in range(W)]
+    gin = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    slots = [torch.empty(T * k, H, device=dev, dtype=dtype) for _ in range(W)]
+    out_a = [torch.empty(T, H, device=dev, dtype=dtype) for _ in range(W)]
+    out_f = [torch.empty(T, H, device=dev, dtype=dtype) for _ in range(W)]
+    flat = lambda ts: [t.reshape(-1) for t in ts]  # noqa: E731
+
+    def bwd_index_add():
+        g.all_to_all(flat(grad), flat(gin), back_counts, bits=bits, bucket_size=512)
+        for q in range(W):
+            out_a[q].zero_().index_add_(0, ii[q], gin[q])
+
+    def bwd_fused():
+        g.all_to_all(flat(grad), flat(slots), back_counts, bits=bits, bucket_size=512, output_index=oi, row=H,
+                     gate=unit, combine_out=flat(out_f))
+
+    arms = {"backward_index_add": (bwd_index_add, out_a), "backward_fused": (bwd_fused, out_f)}
+    ts = {name: [] for name in arms}
+    first = {}
+    stable = {name: True for name in arms}
+    for it in range(warmup + iters):
+        for name, (fn, outs) in arms.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            if it >= warmup:
+                ts[name].append(e0.elapsed_time(e1) * 1000.0)
+            if name not in first:
+                first[name] = [o.clone() for o in outs]
+            else:
+                stable[name] &= all(torch.equal(a.view(torch.uint8), b.view(torch.uint8))
+                                    for a, b in zip(first[name], outs))
+    g.check()
+    n = min(T, 64)
+    want = O.dispatch_sum_reference(slots[0][:n * k].cpu(), k)
+    assert torch.equal(want.view(torch.int16), out_f[0][:n].cpu().view(torch.int16)), "fused backward != oracle"
+    err = {name: 0.0 for name in arms}
+    for q in range(W):
+        exact = slots[q].view(T, k, H).double().sum(1)
+        for name, (_, outs) in arms.items():
+            err[name] = max(err[name], float((outs[q].double() - exact).abs().max()))
+        del exact
+
+    N = T * k * W
+    own = sum(send_rows[q][q] for q in range(W))
+    elems_wire = (N - own) * H
+    wbits = 8 if isinstance(bits, str) else bits
+    wire = elems_wire * es if wbits >= 32 else elems_wire * wbits // 8 + (elems_wire // 512) * 8
+    kernel_bytes = 2 * N * H * es + 2 * wire
+    TH, TkH = W * T * H, N * H
+    index_add_bytes = kernel_bytes + TH * es + TkH * es + 2 * TkH * es
+    fused_bytes = kernel_bytes + TkH * es + TH * es + N * 4
+    res = {"W": W, "T": T, "H": H, "topk": k, "bits": bits, "dtype": str(dtype).replace("torch.", "")}
+    for name in arms:
+        res[name + "_us"] = round(median(ts[name]), 1)
+        res[name + "_spread_us"] = [round(min(ts[name]), 1), round(max(ts[name]), 1)]
+        res[name + "_bitwise_stable"] = stable[name]
+        res[name + "_max_abs_err_vs_f64"] = err[name]
+    res["bytes_index_add_GB"] = round(index_add_bytes / 1e9, 3)
+    res["bytes_fused_GB"] = round(fused_bytes / 1e9, 3)
+    del g, grad, gin, slots, out_a, out_f, first
+    torch.cuda.empty_cache()
+    return res
+
+
 def run_codes(W, T, H, k, bucket, iters, warmup, lanes, slot_mb, dtype=torch.bfloat16):
     """routed e4m3 dispatch: decode + torch quantize (c) against the codes output (d)"""
     dev = torch.device("cuda", 0)
@@ -392,10 +489,31 @@ def main():
     ap.add_argument("--combine-backward", action="store_true",
                     help="time the combine's backward, the scaled send and the gate-gradient kernel against "
                          "grad_slots, the routed call and the torch gate gradient, instead")
+    ap.add_argument("--dispatch-backward", action="store_true",
+                    help="time the dispatch's backward, the unit-gate combine against the routed call and "
+                         "index_add_, instead")
     args = ap.parse_args()
     name, power = gpu_info()
     print(json.dumps({"gpu": name, "power_limit": power}), flush=True)
     rows = []
+    if args.dispatch_backward:
+        for H in args.hidden:
+            for T in args.tokens:
+                for k in args.topk:
+                    need = (args.world * (T * k * 3 * 2 + T * 4 * 2) + T * k * 8) * H / 1e9
+                    if need > args.max_gb:
+                        print(json.dumps({"H": H, "T": T, "topk": k, "skipped": f"needs {need:.1f} GB"}), flush=True)
+                        continue
+                    for bits in args.bits:
+                        r = run_dispatch_backward(args.world, T, H, k, bits, args.iters, args.warmup, args.lanes,
+                                                  args.slot_mb)
+                        r.update(gpu=name, power_limit=power)
+                        rows.append(r)
+                        print(json.dumps(r), flush=True)
+        if args.out:
+            Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(args.out).write_text("".join(json.dumps(r) + "\n" for r in rows))
+        return
     if args.combine_backward:
         for H in args.hidden:
             for T in args.tokens:

@@ -34,6 +34,7 @@ from .parallel.functional import (  # noqa: E402
     all_to_all_single,
     compression,
     differentiable_all_to_all_combine,
+    differentiable_all_to_all_dispatch,
     differentiable_all_to_all_single,
     reduce_scatter_tensor,
 )
@@ -73,6 +74,7 @@ __all__ = [
     "all_to_all_combine",
     "differentiable_all_to_all_single",
     "differentiable_all_to_all_combine",
+    "differentiable_all_to_all_dispatch",
     "register_layer",
     "reset_layers",
     "set_quantization_bits",

@@ -1068,13 +1068,25 @@ class LocalReducerGroup {
   // Combine, the composed path of the process group (CUDA only): with gate[r], combine_out[r] and
   // output_index[r] (as LocalSraGroup.all_to_all) the received rows land in a scratch buffer, are
   // index_copy_'d into the slots outputs[r] by output_index[r], and combine_rows_kernel writes
-  // combine_out[r] from the slots.
+  // combine_out[r] from the slots. input_index[r], when given and not None, selects rank r's sent
+  // rows of `row` elements from inputs[r] first (index_select, as the process group composes it).
   void all_to_all(std::vector<at::Tensor> inputs, std::vector<at::Tensor> outputs, const CountMatrix& counts_in,
                   const A2aBitsArg& bits_arg, int64_t bucket, bool stochastic, uint64_t seed, uint32_t seq,
                   const std::optional<std::vector<at::Tensor>>& output_scales, const IndexList& output_index,
-                  int64_t row, const IndexList& gate, const IndexList& combine_out) {
+                  int64_t row, const IndexList& gate, const IndexList& combine_out, const IndexList& input_index) {
     const A2aBits wb = a2a_bits(bits_arg, stochastic);
     const auto counts = check_counts(counts_in, (size_t)hub_.world());
+    TORCH_CHECK_VALUE(input_index.empty() || (row >= 1 && input_index.size() == inputs.size()),
+                      "all_to_all: input_index needs row >= 1 and one entry per rank");
+    for (size_t r = 0; r < input_index.size(); ++r) {
+      const std::optional<at::Tensor>& ix = input_index[r];
+      if (!ix) continue;
+      TORCH_CHECK_VALUE(ix->device() == inputs[r].device() && ix->scalar_type() == at::kLong && ix->dim() == 1 &&
+                            ix->is_contiguous() && inputs[r].is_contiguous() && inputs[r].numel() % row == 0,
+                        "all_to_all: rank ", r, "'s input_index must be a contiguous int64 vector on its input's ",
+                        "device, and the input whole rows");
+      inputs[r] = inputs[r].view({-1, row}).index_select(0, *ix).reshape(-1);
+    }
     const std::vector<float*> scales = a2a_scales(output_scales, outputs, wb, bucket);
     check_a2a_tensors(inputs, outputs, counts, inputs[0].is_cuda(), output_scales ? wb.codec : kMaxMin);
     const RngParams rng = make_rng(stochastic, seed, seq);
@@ -2335,7 +2347,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("all_to_all", &LocalReducerGroup::all_to_all, py::arg("inputs"), py::arg("outputs"), py::arg("counts"),
            py::arg("bits") = 8, py::arg("bucket_size") = 512, py::arg("stochastic") = false, py::arg("seed") = 0,
            py::arg("seq") = 0, py::arg("output_scales") = py::none(), py::arg("output_index") = IndexList{},
-           py::arg("row") = 1, py::arg("gate") = IndexList{}, py::arg("combine_out") = IndexList{})
+           py::arg("row") = 1, py::arg("gate") = IndexList{}, py::arg("combine_out") = IndexList{},
+           py::arg("input_index") = IndexList{})
       .def("all_gather", &LocalReducerGroup::all_gather, py::arg("inputs"), py::arg("outputs"),
            py::arg("shard_layers"), py::arg("skip_incomplete") = false, py::arg("stochastic") = false,
            py::arg("seed") = 0, py::arg("seq") = 0, py::arg("bits") = py::none(), py::arg("output_scales") = py::none())

@@ -976,7 +976,8 @@ def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence
                                 input_index: Sequence[torch.Tensor | None],
                                 output_index: Sequence[torch.Tensor | None], row: int, *, bits: int | str,
                                 bucket_size: int, outputs: Sequence[torch.Tensor] | None = None,
-                                input_scale: Sequence[torch.Tensor | None] | None = None) -> List[torch.Tensor]:
+                                input_scale: Sequence[torch.Tensor | None] | None = None, seed: int = 0,
+                                seq: int = 0) -> List[torch.Tensor]:
     """Every rank's output of the routed all-to-all, as the composition that defines it: rank q sends
     ``inputs[q].index_select(0, input_index[q])`` (rows of ``row`` elements; ``None``: the input
     itself), ``all_to_all_reference`` exchanges the rows (``counts[q][r]`` elements, whole rows), and
@@ -984,7 +985,8 @@ def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence
     ``outputs[r]`` (``None``: the received rows are the output). Outputs are flat.
     ``input_scale[q]`` (fp32, one entry per ``input_index[q]`` entry; ``None``: unscaled) scales the
     selected rows first: ``(selected.float() * input_scale[q][:, None]).to(dtype)``, one fp32 multiply
-    rounded to nearest even in the dtype."""
+    rounded to nearest even in the dtype. ``seed`` / ``seq``: the random bits of an ``_sr`` format, as
+    in ``all_to_all_reference``."""
     W = len(inputs)
     send = []
     for q in range(W):
@@ -995,7 +997,7 @@ def routed_all_to_all_reference(inputs: Sequence[torch.Tensor], counts: Sequence
         if sc is not None:
             sel = (sel.float() * sc.detach().cpu().float()[:, None]).to(x.dtype)
         send.append(sel.reshape(-1))
-    recv = all_to_all_reference(send, counts, bits=bits, bucket_size=bucket_size)
+    recv = all_to_all_reference(send, counts, bits=bits, bucket_size=bucket_size, seed=seed, seq=seq)
     outs = []
     for r in range(W):
         ix = output_index[r]
@@ -1052,16 +1054,49 @@ def combine_gate_grad_reference(grad_out: torch.Tensor, slots: torch.Tensor) -> 
 
 def routed_all_to_all_combine_reference(inputs: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
                                         output_index: Sequence[torch.Tensor], gates: Sequence[torch.Tensor],
-                                        row: int, *, bits: int | str,
-                                        bucket_size: int) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+                                        row: int, *, bits: int | str, bucket_size: int, seed: int = 0,
+                                        seq: int = 0) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
     """Every rank's weighted top-k combine as the composition that defines it: ``routed_all_to_all_reference``
     into slots (rank r's ``output_index[r]`` a permutation of ``[0, T_r * k_r)``), then
-    ``combine_rows_reference`` with ``gates[r]`` (``[T_r, k_r]``). Returns (slots, outputs), flat."""
+    ``combine_rows_reference`` with ``gates[r]`` (``[T_r, k_r]``). Returns (slots, outputs), flat.
+    ``seed`` / ``seq``: the random bits of an ``_sr`` format."""
     W = len(inputs)
     bases = [inputs[r].new_zeros(output_index[r].numel() * row) for r in range(W)]
     slots = routed_all_to_all_reference(inputs, counts, [None] * W, output_index, row, bits=bits,
-                                        bucket_size=bucket_size, outputs=bases)
+                                        bucket_size=bucket_size, outputs=bases, seed=seed, seq=seq)
     outs = [combine_rows_reference(slots[r].reshape(-1, row), gates[r]).reshape(-1) for r in range(W)]
+    return slots, outs
+
+
+def dispatch_sum_reference(slots: torch.Tensor, k: int) -> torch.Tensor:
+    """The sum of each token's k slot rows, as the backward of an MoE dispatch defines it: ``slots``
+    ``[T*k, H]`` (any float dtype); for every ``t, h``, with ``x_c = float(slots[t*k + c, h])``,
+    ``acc = x_0``, then ``acc = acc + x_c`` for ``c = 1 .. k-1`` in that order, each add an IEEE fp32
+    add (numpy float32); the result is ``acc`` rounded to nearest in the slots' dtype. NaN, Inf and
+    signed zeros follow from IEEE addition: k slots of -0 sum to -0."""
+    x = slots.detach().cpu().float().reshape(slots.shape[0] // k, k, -1).numpy()
+    acc = x[:, 0].copy()
+    with np.errstate(all="ignore"):
+        for c in range(1, k):
+            acc = np.add(acc, x[:, c], dtype=_F32)
+    return torch.from_numpy(np.ascontiguousarray(acc, dtype=_F32)).to(slots.dtype)
+
+
+def dispatch_backward_reference(grads: Sequence[torch.Tensor], counts: Sequence[Sequence[int]],
+                                slot_index: Sequence[torch.Tensor], k: int, row: int, *, bits: int | str,
+                                bucket_size: int, input_index: Sequence[torch.Tensor | None] | None = None,
+                                seed: int = 0, seq: int = 0) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """Every rank's input gradient of ``differentiable_all_to_all_dispatch``, as the composition that
+    defines it: ``routed_all_to_all_reference`` of the gradients ``grads`` (rank q's rows gathered by
+    ``input_index[q]``, the forward's output index; ``None``: in order; ``counts[q][r]`` elements go
+    back from rank q to rank r) into zeroed slots scattered by ``slot_index[r]`` (a permutation of
+    ``[0, T_r * k)``), then ``dispatch_sum_reference`` of each token's k slots. Returns (slots,
+    gradients), flat."""
+    W = len(grads)
+    bases = [grads[r].new_zeros(slot_index[r].numel() * row) for r in range(W)]
+    slots = routed_all_to_all_reference(grads, counts, input_index or [None] * W, slot_index, row, bits=bits,
+                                        bucket_size=bucket_size, outputs=bases, seed=seed, seq=seq)
+    outs = [dispatch_sum_reference(slots[r].reshape(-1, row), k).reshape(-1) for r in range(W)]
     return slots, outs
 
 

@@ -26,6 +26,7 @@ uncompressed)::
 
     cgx.all_to_all_single(recv, tokens, recv_splits, send_splits, bits=8)
     y = cgx.differentiable_all_to_all_single(tokens, recv_splits, send_splits, bits="e4m3", grad_bits="e5m2")
+    x = cgx.differentiable_all_to_all_dispatch(tokens, slot_order, recv_splits, send_splits, bits="e4m3")
 """
 from __future__ import annotations
 
@@ -517,7 +518,7 @@ def _overlaps(a: torch.Tensor, b: torch.Tensor) -> bool:
 
 
 def _check_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Tensor, output_index: torch.Tensor,
-                   slots: Optional[torch.Tensor]) -> None:
+                   slots: Optional[torch.Tensor], input_index: Optional[torch.Tensor] = None) -> None:
     """ValueError unless the arguments of ``all_to_all_combine`` are well formed. The checks that need
     no GPU come first, the device checks last."""
     api = "cgx.all_to_all_combine"
@@ -537,6 +538,10 @@ def _check_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Tensor
     if output_index.dtype != torch.int64 or output_index.dim() != 1 or output_index.numel() != T * k:
         raise ValueError(f"{api}: output_index must be an int64 vector of T * k = {T * k} entries, got "
                          f"{output_index.dtype} {list(output_index.shape)}")
+    if input_index is not None and (input_index.dtype != torch.int64 or input_index.dim() != 1
+                                    or not input_index.is_contiguous()):
+        raise ValueError(f"{api}: input_index must be a contiguous int64 vector, got {input_index.dtype} "
+                         f"{list(input_index.shape)}")
     if slots is not None and (slots.dtype != input.dtype or tuple(slots.shape) != (T * k,) + rows
                               or not slots.is_contiguous()):
         raise ValueError(f"{api}: slots must be a contiguous {input.dtype} tensor of shape {[T * k, *rows]}, got "
@@ -547,7 +552,7 @@ def _check_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Tensor
     if slots is not None and _overlaps(slots, output):
         raise ValueError(f"{api}: slots overlap the output")
     for name, t in (("input", input), ("output", output), ("gate", gate), ("output_index", output_index),
-                    ("slots", slots)):
+                    ("slots", slots), ("input_index", input_index)):
         if t is not None and (not t.is_cuda or t.device != input.device):
             raise ValueError(f"{api}: {name} must be on the input's CUDA device, got {t.device}")
 
@@ -556,15 +561,18 @@ def all_to_all_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Te
                        output_split_sizes: Optional[Sequence[int]] = None,
                        input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8, bucket_size: int = 512,
                        group=None, async_op: bool = False, stochastic: bool = False, seed: Optional[int] = None,
-                       slots: Optional[torch.Tensor] = None):
+                       slots: Optional[torch.Tensor] = None, input_index: Optional[torch.Tensor] = None):
     """The routed compressed all-to-all of an MoE combine followed by the weighted top-k sum, in one call.
 
     ``gate`` is a contiguous CUDA float32 ``[T, k]`` (``1 <= k <= 32``), ``output`` ``[T, ...]`` in the
     input's dtype and row shape, ``output_index`` a CUDA int64 permutation of ``[0, T*k)`` with
     ``sum(output_split_sizes)`` entries. Slot ``s = t*k + c`` is choice ``c`` of token ``t``.
-    The call is defined as the composition
-      1. ``slots = all_to_all_single(slots, input, ..., output_index=output_index)`` (any ``bits``,
-         stochastic rounding included, the own chunk copied bit for bit), into a ``[T*k, ...]`` buffer;
+    ``input_index`` (optional, CUDA int64, ``sum(input_split_sizes)`` entries) gathers the sent rows
+    from ``input`` as in ``all_to_all_single``, for an input whose rows are grouped otherwise (by
+    local expert, say). The call is defined as the composition
+      1. ``slots = all_to_all_single(slots, input, ..., input_index=input_index, output_index=output_index)``
+         (any ``bits``, stochastic rounding included, the own chunk copied bit for bit), into a
+         ``[T*k, ...]`` buffer;
       2. for every ``t`` and element ``h``, with ``x_c = float(slots[t*k + c, h])`` and
          ``g_c = gate[t, c]``: ``acc = fp32(g_0 * x_0)``, then ``acc = fma(g_c, x_c, acc)`` for
          ``c = 1 .. k-1`` in that order, and ``output[t, h] = acc`` rounded to nearest in the dtype.
@@ -587,7 +595,7 @@ def all_to_all_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Te
     from .hooks import _native_backend
 
     bits = _a2a_bits(bits, stochastic)
-    _check_combine(output, input, gate, output_index, slots)
+    _check_combine(output, input, gate, output_index, slots, input_index)
     if slots is None:
         slots = input.new_empty((gate.shape[0] * gate.shape[1],) + tuple(input.shape[1:]))
     native = _native_backend(group if group is not None else dist.group.WORLD, input)
@@ -595,7 +603,7 @@ def all_to_all_combine(output: torch.Tensor, input: torch.Tensor, gate: torch.Te
         raise RuntimeError("cgx.all_to_all_combine needs a process group with the cgx backend")
     work = native.all_to_all_compressed(slots, input, _splits(output_split_sizes), _splits(input_split_sizes),
                                         bits, int(bucket_size), bool(stochastic), -1 if seed is None else int(seed),
-                                        None, output_index, None, gate, output)
+                                        input_index, output_index, None, gate, output)
     if async_op:
         return work
     work.wait()
@@ -671,3 +679,84 @@ def differentiable_all_to_all_combine(input: torch.Tensor, gate: torch.Tensor, o
                                   None if output_split_sizes is None else _splits(output_split_sizes),
                                   None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
                                   int(bucket_size), group, bool(stochastic), gate_grad)
+
+
+def _check_slot_index(input: torch.Tensor, slot_index: torch.Tensor) -> int:
+    """``k``, the choices per token, if ``slot_index`` can be the slot index of
+    ``differentiable_all_to_all_dispatch``; ValueError otherwise. The device check comes last."""
+    api = "cgx.differentiable_all_to_all_dispatch"
+    if slot_index.dtype != torch.int64 or slot_index.dim() != 1 or not slot_index.is_contiguous():
+        raise ValueError(f"{api}: slot_index must be a contiguous int64 vector, got {slot_index.dtype} "
+                         f"{list(slot_index.shape)}{'' if slot_index.is_contiguous() else ' (not contiguous)'}")
+    T, n = int(input.shape[0]), int(slot_index.numel())
+    if T < 1 or n % T != 0 or not 1 <= n // T <= 32:
+        raise ValueError(f"{api}: slot_index must hold T * k entries with T = {T} tokens and k in 1..32, got {n}")
+    if not slot_index.is_cuda or slot_index.device != input.device:
+        raise ValueError(f"{api}: slot_index must be on the input's CUDA device, got {slot_index.device}")
+    return n // T
+
+
+class _AllToAllDispatch(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, input, slot_index, k, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size,
+                group, stochastic, output_index, output_rows):
+        ctx.slot_index, ctx.k = slot_index, k
+        return _AllToAll.forward(ctx, input, output_split_sizes, input_split_sizes, bits, grad_bits, bucket_size,
+                                 group, stochastic, torch.div(slot_index, k, rounding_mode="floor"), output_index,
+                                 output_rows)
+
+    @staticmethod
+    def backward(ctx, grad):
+        out_splits, in_splits = ctx.splits
+        _, output_index = ctx.index
+        grad = grad.contiguous()
+        gin = grad.new_empty(ctx.in_shape)
+        # the combine with unit gates: slot t*k + c comes back to row slot_index^-1, and each token's
+        # k slots are summed in fp32 in choice order, rounded once
+        unit = torch.ones(ctx.in_shape[0], ctx.k, dtype=torch.float32, device=grad.device)
+        all_to_all_combine(gin, grad, unit, ctx.slot_index, in_splits, out_splits, bits=ctx.grad_bits,
+                           bucket_size=ctx.bucket_size, group=ctx.group, stochastic=ctx.stochastic,
+                           input_index=output_index)
+        return gin, None, None, None, None, None, None, None, None, None, None, None
+
+
+def differentiable_all_to_all_dispatch(input: torch.Tensor, slot_index: torch.Tensor,
+                                       output_split_sizes: Optional[Sequence[int]] = None,
+                                       input_split_sizes: Optional[Sequence[int]] = None, bits: A2aBits = 8,
+                                       grad_bits: Optional[A2aBits] = None, bucket_size: int = 512, group=None,
+                                       stochastic: bool = False, output_index: Optional[torch.Tensor] = None,
+                                       output_rows: Optional[int] = None) -> torch.Tensor:
+    """The token dispatch of an MoE layer, with a backward that sums each token's k gradients inside
+    the exchange (DESIGN §2.13i).
+
+    ``input`` holds ``T`` tokens. ``slot_index`` is a contiguous CUDA int64 permutation of ``[0, T*k)``
+    (``1 <= k <= 32``), slot ``s = t*k + c`` being choice ``c`` of token ``t``, listed in the order the
+    rows are sent (``argsort`` of the flattened destinations, say): sent row ``i`` is token
+    ``slot_index[i] // k``. The forward is bit for bit ``differentiable_all_to_all_single(input, ...,
+    input_index=slot_index // k, output_index=output_index, output_rows=output_rows)``.
+
+    The backward is one ``all_to_all_combine`` with gates of one: the gradient travels back at
+    ``grad_bits`` (``None``: ``bits``) with the splits swapped, gathered by ``output_index`` if the
+    forward had one, returned row ``i`` lands in slot ``slot_index[i]``, and for every token ``t`` and
+    element ``h``, with ``x_c`` the fp32 value of slot ``t*k + c``, ``acc = x_0``, then ``acc = acc + x_c``
+    for ``c = 1 .. k-1`` in fp32, and ``grad_input[t, h] = acc`` rounded once to the dtype. A unit gate
+    is exact (``1 * x = x``, ``fma(1, x, acc) = x + acc``), so this is that sum bit for bit. Compared
+    with the ``index_add_`` backward of ``differentiable_all_to_all_single``, the order is fixed, so
+    two runs give the same bits; bf16 and fp16 are rounded once instead of once per choice; and a token
+    whose k gradients are all ``-0`` gets ``-0`` instead of ``+0`` (``index_add_`` starts from ``+0``).
+
+    ``ValueError`` before the forward sends anything for a ``slot_index`` of the wrong dtype, device,
+    layout or length, for ``output_index`` without ``output_rows``, and for an FP8 ``bits`` or
+    ``grad_bits`` with ``stochastic=True``. A repeated slot is found by the kernel in the backward: its
+    call fails with the combine's message, which names ``output_index`` (the combine's name for
+    ``slot_index``), and the group refuses further collectives.
+    """
+    if output_index is not None and output_rows is None:
+        raise ValueError("cgx.differentiable_all_to_all_dispatch: output_index needs output_rows")
+    bits = _a2a_bits(bits, stochastic)
+    gb = _a2a_bits(bits if grad_bits is None else grad_bits, stochastic)
+    k = _check_slot_index(input, slot_index)
+    return _AllToAllDispatch.apply(input, slot_index, k,
+                                   None if output_split_sizes is None else _splits(output_split_sizes),
+                                   None if input_split_sizes is None else _splits(input_split_sizes), bits, gb,
+                                   int(bucket_size), group, bool(stochastic), output_index, output_rows)
